@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — schedule prefixes/sec on the BASELINE.json north-star workload, plus the secondary configs.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--no-secondary]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--no-secondary] [--dump-outputs DIR]
 
 Headline (BASELINE.json configs[1]): 5-actor Raft model (seeded double-vote bug), RandomScheduler/FullyRandom fuzz,
 maxMessages=50, invariant every 5 deliveries, 10^7 prefixes per step per GPU (weak scaling: rank r, step s explores
@@ -9,7 +9,7 @@ its own seed range).  One "step" = one pass of the hot path over one batch of pr
 
   value : prefixes/s, results stay in HBM (demi_fuzz_batch_dev), CUDA-event timed
   e2e   : prefixes/s through the reference-facing C-ABI call demi_fuzz_batch with HOST buffers
-          (external program H2D + all result records D2H per step)
+          (external program H2D + all result records D2H per step), over the same number of steps
   roofline     : algorithmic HBM bytes of the fuzz kernel vs the measured copy peak; the profile-derived figures
                  (DRAM traffic, issue-slot utilisation) come from profiles/k1_profile.json and are dropped when that
                  capture was taken from another build of the kernels
@@ -17,6 +17,11 @@ its own seed range).  One "step" = one pass of the hot path over one batch of pr
   secondary    : configs[2] (one DPORwHeuristics search as a frontier, with the in-library NCCL steal round at N > 1),
                  configs[3] (DDMin / STSSched replays over a 2000-event trace), configs[4] (bcast32 + state-hash
                  dedup) — measured after, and outside, the headline's timed region (tools/secondary.py)
+
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step computed: every field of a fixed, seeded
+sample of its result records as DIR/<field>.npy (float64; the 64-bit hashes as exact 32-bit halves), the sampled
+prefix indices and the step's counters.  The seeds depend only on --steps, --warmup and --prefixes, so two builds run
+with the same arguments can be compared output for output.
 
 `--impl reference` times the CPU oracle alone on the SAME batch definition (the reference itself needs a JVM + sbt +
 Akka + the akka-raft application, none of which exist here).
@@ -40,6 +45,8 @@ RESULT_BYTES = 32          # sizeof(demi_fuzz_result): the algorithmic HBM bytes
 PREFIXES_PER_STEP = 10_000_000
 METRIC = "schedule prefixes/sec (5-actor Raft, depth 50)"
 K1_PROFILE = os.path.join(ROOT, "profiles", "k1_profile.json")
+HBM_PEAK_GBS = 3350.0      # H100 SXM data sheet (HBM3); used only when MEASURED_PEAKS.json is absent
+DUMP_SAMPLE = 1 << 18      # result records written by --dump-outputs (11 float64 arrays: 23 MB)
 
 
 def workload_config(n_per_step, n_gpus):
@@ -49,14 +56,14 @@ def workload_config(n_per_step, n_gpus):
         "scheduler": "RandomScheduler/FullyRandom(seed=base+i)",
         "max_messages": MAX_MESSAGES, "invariant_check_interval": INTERVAL,
         "prefixes_per_step_per_gpu": n_per_step, "sharding": "seed ranges per rank, no data-path collective",
-        "l2": "each step writes %d MB of fresh result records (> 126 MB L2); no input is re-read across steps"
+        "l2": "each step writes %d MB of fresh result records (> 50 MB L2); no input is re-read across steps"
               % (n_per_step * RESULT_BYTES // 1_000_000),
         "n_gpus": n_gpus,
     }
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         threading.Thread.__init__(self, daemon=True)
@@ -117,7 +124,7 @@ def measured_peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return HBM_PEAK_GBS, "fallback"
 
 
 def k1_profile(k1_id):
@@ -171,6 +178,27 @@ def run_reference(args):
     return 0
 
 
+def dump_outputs(out_dir, results_dev, n, n_violations, sum_steps, result_dtype):
+    """The last timed step's result records (a seeded sample of DUMP_SAMPLE of them) as float64 arrays."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    m = min(n, DUMP_SAMPLE)
+    idx = np.sort(np.random.default_rng(20240901).choice(n, size=m, replace=False))
+    rows = results_dev.view(n, RESULT_BYTES)[torch.from_numpy(idx).to(results_dev.device)]
+    rec = rows.cpu().numpy().reshape(-1).view(result_dtype)
+    arrays = {"prefix_index": idx, "step_counters": np.array([n_violations, sum_steps])}
+    for name in result_dtype.names:
+        v = rec[name]
+        if v.dtype.itemsize == 8:                        # exact in float64 as two 32-bit halves
+            arrays[name + "_lo"] = v & np.uint64(0xFFFFFFFF)
+            arrays[name + "_hi"] = v >> np.uint64(32)
+        else:
+            arrays[name] = v
+    for name, v in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(v).astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -180,6 +208,7 @@ def main():
     ap.add_argument("--prefixes", type=int, default=PREFIXES_PER_STEP)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -241,6 +270,8 @@ def main():
     total_ms = evs[0].elapsed_time(evs[K])
     kernel_ms = [evs[i].elapsed_time(evs[i + 1]) for i in range(K)]
     nv, ss = eng.fuzz_summary_dev(stream.cuda_stream)   # counters of the last step
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, results_dev, n, nv, ss, D._native.RESULT_DTYPE)
     t = torch.tensor([total_ms], dtype=torch.float64, device=dev)
     cnt = torch.tensor([float(nv), float(ss)], dtype=torch.float64, device=dev)
     if world > 1:
@@ -252,7 +283,7 @@ def main():
     # ------------------------------------------------ end-to-end through the host C ABI ("e2e")
     host_out = torch.empty(n * RESULT_BYTES, dtype=torch.uint8, pin_memory=True)
     host_np = host_out.numpy().view(D._native.RESULT_DTYPE)
-    e2e_steps = max(1, min(K, 3))
+    e2e_steps = K
     for s in range(1):
         eng.set_externals(ext)
         eng.fuzz_batch(seed_of(s), n, MAX_MESSAGES, INTERVAL, out=host_np)

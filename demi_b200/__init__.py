@@ -1,4 +1,4 @@
-"""demi_b200 — B200-native schedule-space exploration engine behind DEMi's
+"""demi_b200 — H100-native schedule-space exploration engine behind DEMi's
 Scheduler / TestOracle plugin surface.  See DESIGN.md."""
 from . import _native  # noqa: F401
 from .events import (Start, Kill, HardKill, Send, WaitQuiescence, Partition, UnPartition,  # noqa: F401

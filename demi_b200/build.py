@@ -1,9 +1,9 @@
 """Build the in-tree native libraries.
 
-  demi_b200/libdemi_b200.so  — the CUDA engine + C ABI (nvcc, sm_100a only)
+  demi_b200/libdemi_b200.so  — the CUDA engine + C ABI (nvcc, sm_90a only)
   oracle/liboracle.so        — the CPU oracle (gcc; test infrastructure only)
 
-Both are git-ignored and travel to the GPU box with the gpurun snapshot.
+Both are git-ignored build products.
 """
 import os
 import subprocess
@@ -16,7 +16,7 @@ ORACLE_DIR = os.path.join(ROOT, "oracle")
 ORACLE_LIB = os.path.join(ORACLE_DIR, "liboracle.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
 ]
@@ -76,8 +76,8 @@ def build_engine(force=False, verbose=False):
 
 
 def _cpu_stamp():
-    """The oracle is compiled -march=native, so a library built on another machine (it travels with the
-    gpurun snapshot) is rebuilt on the machine that runs it: model name + ISA flags identify the CPU."""
+    """The oracle is compiled -march=native, so a library built on another machine (a copied working tree)
+    is rebuilt on the machine that runs it: model name + ISA flags identify the CPU."""
     import hashlib
     model, flags = "", ""
     try:

@@ -75,7 +75,7 @@ static const LaneVariant* pick_lane_variant(const demi_handle* h);
 #ifndef DEMI_K1_ID
 #define DEMI_K1_ID "unknown"
 #endif
-extern "C" const char* demi_version(void) { return "demi_b200 0.2 (sm_100a) build " DEMI_BUILD_ID " k1 " DEMI_K1_ID; }
+extern "C" const char* demi_version(void) { return "demi_b200 0.2 (sm_90a) build " DEMI_BUILD_ID " k1 " DEMI_K1_ID; }
 
 extern "C" const char* demi_last_error(const demi_handle* h) {
   return h ? h->err.c_str() : g_create_error.c_str();

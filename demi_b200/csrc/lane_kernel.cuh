@@ -44,8 +44,8 @@ namespace demi {
 constexpr uint32_t LANE_DEFER = 0xFFFFu;      // internal status: hand over to the warp engine
 
 // The pending arrays are the only data this kernel re-reads from global memory; the result records are written once.
-// An L2 evict_last policy on the former (and evict-first stores for the latter) keeps the arrays cache-resident:
-// measured 533 -> 121 B of DRAM traffic per prefix (profiles/r2_k1_l2_policy.md).  Every access to the arrays goes
+// An L2 evict_last policy on the former (and evict-first stores for the latter) keeps the arrays cache-resident, so
+// that their stores are not written back to DRAM between a prefix's steps.  Every access to the arrays goes
 // through these two volatile asm statements (which keep their program order), and nothing else aliases the arrays,
 // so no "memory" clobber is needed.
 __device__ __forceinline__ uint64_t l2_evict_last_policy() {

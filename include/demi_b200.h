@@ -1,5 +1,5 @@
 /*
- * demi_b200.h — C ABI of the B200 schedule-space exploration engine.
+ * demi_b200.h — C ABI of the H100 schedule-space exploration engine.
  *
  * This is the drop-in boundary for the hot path of NetSys/demi (DEMi).  The
  * reference has no FFI: the path sits behind two Scala traits,

@@ -1,5 +1,5 @@
 """Secondary workloads of BASELINE.json (configs[2..4]) — one JSON line per config.
-Not the driver's bench.py; results are copied into profiles/."""
+Not bench.py; its JSON lines can be kept under profiles/."""
 import json
 import os
 import sys

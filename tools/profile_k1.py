@@ -1,10 +1,10 @@
 """Regenerate profiles/k1_profile.json: the profile-derived figures bench.py reports for the headline kernel.
 
-  (on the GPU box)  python tools/profile_k1.py            # runs ncu on tools/profile_k1.py --workload, parses the capture
+  (on an H100)  python tools/profile_k1.py            # runs ncu on tools/profile_k1.py --workload, parses the capture
 
 One `ncu --set full --clock-control none` capture of fuzz_lane_kernel over PREFIXES prefixes of the bench workload.
 The JSON records the hash of the kernel's sources (demi_b200.build.k1_source_id); bench.py refuses figures taken
-from other sources, and tests/test_bench_reference_arm.py fails when the committed profile is stale."""
+from other sources.  The ncu report itself (profiles/k1_profile.ncu-rep) is not kept in git."""
 import csv
 import io
 import json
@@ -16,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 PREFIXES = 4_000_000
 OUT = os.path.join(ROOT, "profiles", "k1_profile.json")
-REP = os.path.join(ROOT, "gpurun_out", "k1_profile")
+REP = os.path.join(ROOT, "profiles", "k1_profile")
 
 
 def workload():

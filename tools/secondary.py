@@ -31,7 +31,7 @@ def _peak():
         import json
         return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "fallback"                 # H100 SXM data sheet (HBM3)
 
 
 def _allmax(x, dev, world):
