@@ -103,38 +103,51 @@ struct LaneOutbox {
     base[(n * 3 + 2) * bd] = p1;
     n++;
   }
+  __device__ __forceinline__ bool reserve(uint32_t) { return true; }     // drain() reserves each staged send
   __device__ __forceinline__ void send(uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) { push(OP_SEND, dst, type, p0, p1); }
   __device__ __forceinline__ void schedule_once(uint32_t type, uint32_t p0, uint32_t p1) { push(OP_SCHED_ONCE, self, type, p0, p1); }
   __device__ __forceinline__ void schedule_repeating(uint32_t type, uint32_t p0, uint32_t p1) { push(OP_SCHED_REPEAT, self, type, p0, p1); }
   __device__ __forceinline__ void cancel_timer(uint32_t type, uint32_t p0, uint32_t p1) { push(OP_CANCEL, self, type, p0, p1); }
 };
 
-// small FIFO of bytes in two 64-bit registers
+// small FIFO of bytes in four 32-bit registers: entry i is byte (i & 3) of w[i >> 2], and the bytes at and above n
+// are zero.  Every operation is a few byte permutes (PRMT) or bitwise ops on the words; none loops over the entries.
 struct ByteQueue16 {
-  uint64_t lo, hi; uint32_t n;
-  __device__ __forceinline__ void clear() { lo = hi = 0; n = 0; }
+  uint32_t w[4]; uint32_t n;
+  __device__ __forceinline__ void clear() { w[0] = w[1] = w[2] = w[3] = 0; n = 0; }
   __device__ __forceinline__ uint32_t get(uint32_t i) const {
-    uint64_t v = i < 8 ? lo : hi;
-    return (uint32_t)(v >> ((i & 7) * 8)) & 0xFFu;
+    const uint32_t q = i >> 2;
+    const uint32_t x = q == 0 ? w[0] : q == 1 ? w[1] : q == 2 ? w[2] : w[3];
+    return __byte_perm(x, 0u, 0x4440u | (i & 3u));
   }
   __device__ __forceinline__ void push(uint32_t b) {      // caller checks n < 16
-    uint64_t v = (uint64_t)b << ((n & 7) * 8);
-    if (n < 8) lo |= v; else hi |= v;
+    const uint32_t v = b << ((n & 3u) * 8u);
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++) if ((n >> 2) == k) w[k] |= v;
     n++;
   }
-  __device__ __forceinline__ void remove_at(uint32_t i) { // order preserving
-    ByteQueue16 q; q.clear();
-    for (uint32_t k = 0; k < n; k++) if (k != i) q.push(get(k));
-    *this = q;
+  // Order preserving: every entry above i moves down one byte.  Word k is permuted with the word above it (byte 0 of
+  // w[k+1] is byte 4 of the pair); it keeps its `keep` bytes below i and takes the next byte for each one above:
+  // selector 0x3210 for keep = 4 (a word below i's), 0x4321 for keep = 0 (a word above it).
+  __device__ __forceinline__ void remove_at(uint32_t i) {
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+      const int keep = min(max((int)i - 4 * k, 0), 4);
+      const uint32_t sel = 0x4321u - (0x1111u >> (16 - 4 * keep));
+      w[k] = __byte_perm(w[k], k < 3 ? w[k + 1] : 0u, sel);
+    }
+    n--;
   }
 };
 
 // receive()'s view when its operations are applied as they are issued (`dst ! msg` is synchronous in the reference,
 // Instrumenter.scala:1098-1108): no staging in shared memory.  Only for models whose receive() cannot produce two equal
-// sends (MODEL::LANE_SENDS_DISTINCT), because the duplicate-send screen needs the whole outbox.
+// sends (MODEL::LANE_SENDS_DISTINCT), because the duplicate-send screen needs the whole outbox.  The model reserves
+// its sends before it issues them: reserve(k), then k sends.
 template <class M>
 struct LaneDirectOutbox {
   M* m; uint32_t self;
+  __device__ __forceinline__ bool reserve(uint32_t k) { return m->reserve_sends(self, k); }
   __device__ __forceinline__ void send(uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) { m->actor_send_produced(self, dst, type, p0, p1); }
   __device__ __forceinline__ void schedule_once(uint32_t type, uint32_t p0, uint32_t p1) { m->schedule_timer(OP_SCHED_ONCE, self, type, p0, p1); }
   __device__ __forceinline__ void schedule_repeating(uint32_t type, uint32_t p0, uint32_t p1) { m->schedule_timer(OP_SCHED_REPEAT, self, type, p0, p1); }
@@ -164,40 +177,56 @@ struct LaneMachine {
   uint64_t resend; uint32_t n_resend;
   uint32_t just, registry, cancelled;            // bit per timer slot
   uint32_t root_timers, window_timers;           // duplicate guards for the child-reuse rule
-  uint32_t n_nodes, parent_event, n_events, n_uniq;
+  // Every send takes the next Unique id and the next DepTracker node together (no child is reused in this engine), so
+  // the two are equal and one counter serves both: a send's word 3 is node | node << 16.
+  uint32_t n_nodes, parent_event, n_events;
   int32_t nsched, nmod;
   uint32_t ext_idx, ext_send_idx;
   uint32_t violation, status;
   uint32_t inaccessible, killed;
   uint64_t thash;
+  // the sends of one receive(), set up by reserve_sends: no partition or isolation in effect, and the linear part of
+  // the trace hash term of the next send with its dst, type, p0 and p1 words left out
+  bool sends_open;
+  uint64_t send_lin;
 
   __device__ __forceinline__ uint32_t& part_row(uint32_t a) { return smw[(N * SW + OBW + a) * BD]; }
   __device__ __forceinline__ LaneState actor(uint32_t a) { return LaneState{smw + a * SW * BD, BD}; }
 
   __device__ __forceinline__ void defer() { status = LANE_DEFER; }
 
-  // EventTrace.+= (EventTrace.scala:88-110)
+  // EventTrace.+= (EventTrace.scala:88-110); w3 = uniq | node << 16
   __device__ __forceinline__ void record_event(uint32_t kind, uint32_t src, uint32_t dst, uint32_t type,
-                                               uint32_t p0, uint32_t p1, uint32_t uniq, uint32_t node, uint32_t parent) {
+                                               uint32_t p0, uint32_t p1, uint32_t w3, uint32_t parent) {
     uint32_t w0 = kind | (src << 8) | (dst << 16) | (type << 24);
-    thash += demi_event_term(w0, p0, p1, uniq | (node << 16), n_events, parent);
+    thash += demi_event_term(w0, p0, p1, w3, n_events, parent);
+    record_rest(w0, p0, p1, w3, parent);
+  }
+  // the provenance copy of the element, and its position
+  __device__ __forceinline__ void record_rest(uint32_t w0, uint32_t p0, uint32_t p1, uint32_t w3, uint32_t parent) {
     if (REC) {
       if (n_events >= A->rec_cap) { defer(); return; }
-      rec_ev[n_events] = make_uint4(w0, p0, p1, uniq | (node << 16));
-      if (kind == DEMI_EV_MSG_SEND && node < A->rec_parent_cap) rec_par[node] = (uint16_t)parent;   // DepTracker edge
+      rec_ev[n_events] = make_uint4(w0, p0, p1, w3);
+      const uint32_t node = w3 >> 16;
+      if ((w0 & 0xFF) == DEMI_EV_MSG_SEND && node < A->rec_parent_cap) rec_par[node] = (uint16_t)parent;   // DepTracker edge
     }
     n_events++;
   }
 
-  // RandomizedHashSet.insert (schedulers/Util.scala:126-136)
-  __device__ __forceinline__ void pending_insert(uint4 e) {
-    if (n_pending >= A->pending_cap || n_pending >= LPCAP) { defer(); return; }
+  // RandomizedHashSet.insert (schedulers/Util.scala:126-136).  max_pending is brought up to date before each removal
+  // and at the end of the execution, the only points where the set can be at a maximum.
+  __device__ __forceinline__ bool pending_full(uint32_t k) const { return n_pending + k > A->pending_cap || n_pending + k > LPCAP; }
+  __device__ __forceinline__ void pending_push(uint4 e) {          // the caller has checked pending_full
     st_l2_hint(pend + n_pending * 32, e, pol);
     n_pending++;
-    if (n_pending > max_pending) max_pending = n_pending;
+  }
+  __device__ __forceinline__ void pending_insert(uint4 e) {
+    if (pending_full(1)) { defer(); return; }
+    pending_push(e);
   }
   // RandomizedHashSet.remove (schedulers/Util.scala:146-163)
   __device__ __forceinline__ uint4 pending_remove_at(uint32_t i) {
+    if (n_pending > max_pending) max_pending = n_pending;
     uint4 v = ld_l2_hint(pend + i * 32, pol);
     uint4 last = ld_l2_hint(pend + (n_pending - 1) * 32, pol);
     st_l2_hint(pend + i * 32, last, pol);
@@ -206,8 +235,11 @@ struct LaneMachine {
   }
 
   // EventOrchestrator.crosses_partition (EventOrchestrator.scala:345-351)
+  __device__ __forceinline__ bool network_open() { return !(inaccessible | killed) && !A->has_partitions; }   // everyone started, no one isolated
   __device__ __forceinline__ bool crosses_partition(uint32_t snd, uint32_t rcv) {
-    if (!(inaccessible | killed) && !A->has_partitions) return false;      // everyone started, no one isolated
+    return !network_open() && crosses_partition_closed(snd, rcv);
+  }
+  __device__ __forceinline__ bool crosses_partition_closed(uint32_t snd, uint32_t rcv) {
     bool snd_actor = snd < DEMI_MAX_ACTORS;
     if (snd == rcv && !((killed >> snd) & 1u)) return false;
     if (A->has_partitions && snd_actor) {
@@ -224,19 +256,36 @@ struct LaneMachine {
   // DepTracker.getMessage (DepTracker.scala:82-109): in the regime this engine
   // accepts no child is ever reused, so the Unique id is simply the next one.
   // The sends of receive() itself (sender an actor, no flags): the external / timer branches do not apply.
+  //
+  // reserve_sends(self, k) is called once before the next k of them: it checks the node and pending capacities for
+  // all k and defers if they do not fit, so that actor_send_produced applies each send with no further check.  With
+  // exactly k sends inserted this defers exactly when the per-send checks would have; a send that crosses a partition
+  // or hits a cancelled timer is not inserted, so there the reservation may be conservative (deferring is always
+  // exact: the general engine re-runs the prefix).  Only REC's trace capacity is still checked per event.
+  __device__ __forceinline__ bool reserve_sends(uint32_t self, uint32_t k) {
+    if (status) return false;
+    if (n_nodes + k > A->node_cap || pending_full(k)) { defer(); return false; }
+    sends_open = network_open();
+    // demi_event_term of the first send, dst / type / payload terms left out: word 0 = kind | self << 8, word 3 =
+    // node | node << 16 (node <= 0xFFFE, as n_nodes + k <= node_cap <= 0xFFFF), sequence n_events
+    send_lin = demi_hash6_lin(DEMI_EV_MSG_SEND | (self << 8), 0, 0, n_nodes * 0x10001u, n_events, parent_event);
+    return true;
+  }
   __device__ __forceinline__ void actor_send_produced(uint32_t self, uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) {
-    if (status) return;
+    if (REC && status) return;
     if (cancelled) {
       const int slot = MODEL::timer_slot(dst, type, p0, p1);
       if (slot >= 0 && ((cancelled >> slot) & 1u)) { cancelled &= ~(1u << slot); return; }
     }
-    if (n_nodes >= A->node_cap) { defer(); return; }
-    const uint32_t uniq = ++n_uniq, node = n_nodes++;
-    if (!crosses_partition(self, dst)) {
-      pending_insert(make_uint4(make_hdr(self, dst, type, 0), p0, p1, uniq | (node << 16)));
-      if (status) return;
-    }
-    record_event(DEMI_EV_MSG_SEND, self, dst, type, p0, p1, uniq, node, parent_event);
+    const uint32_t w3 = n_nodes++ * 0x10001u;
+    if (sends_open || !crosses_partition_closed(self, dst)) pending_push(make_uint4(make_hdr(self, dst, type, 0), p0, p1, w3));
+    // the hash term of this send: word 0 adds dst << 16 | type << 24 to the reserved kind | self << 8, and the next
+    // send's word 3 and sequence number are one node (0x10001) and one event further on
+    const uint32_t w0_tail = (dst << 16) | (type << 24);
+    thash += demi_hash6_fin(send_lin + (uint64_t)w0_tail * DEMI_HASH6_KA + (uint64_t)p0 * DEMI_HASH6_KB +
+                            (uint64_t)p1 * DEMI_HASH6_KC);
+    send_lin += 0x10001ull * DEMI_HASH6_KD + DEMI_HASH6_KE;
+    record_rest(DEMI_EV_MSG_SEND | (self << 8) | w0_tail, p0, p1, w3, parent_event);
   }
   // A timer message flushed from messagesToSend (sender deadLetters, recorded as "Timer"); `slot` is its key.
   __device__ __forceinline__ void timer_produced(uint32_t slot) {
@@ -246,14 +295,14 @@ struct LaneMachine {
     // two equal timer sends under one parent would share a Unique: defer those
     if (parent_event == 0) { if (root_timers & bit) { defer(); return; } root_timers |= bit; }
     else { if (window_timers & bit) { defer(); return; } window_timers |= bit; }
-    const uint32_t uniq = ++n_uniq, node = n_nodes++;
+    const uint32_t w3 = n_nodes++ * 0x10001u;
     uint32_t dst, type, p0, p1;
     MODEL::slot_msg(slot, dst, type, p0, p1);
     if (!crosses_partition(DEMI_DEADLETTERS, dst)) {
-      pending_insert(make_uint4(make_hdr(DEMI_DEADLETTERS, dst, type, DEMI_MF_TIMER), p0, p1, uniq | (node << 16)));
+      pending_insert(make_uint4(make_hdr(DEMI_DEADLETTERS, dst, type, DEMI_MF_TIMER), p0, p1, w3));
       if (status) return;
     }
-    record_event(DEMI_EV_MSG_SEND, DEMI_TIMER_SND, dst, type, p0, p1, uniq, node, parent_event);
+    record_event(DEMI_EV_MSG_SEND, DEMI_TIMER_SND, dst, type, p0, p1, w3, parent_event);
   }
   // An external Send flushed from messagesToSend (`hdr` carries DEMI_MF_EXTERNAL).
   __device__ __forceinline__ void external_produced(uint32_t hdr, uint32_t p0, uint32_t p1) {
@@ -264,12 +313,11 @@ struct LaneMachine {
       defer(); return;                          // an external that equals a timer key could share its Unique
     }
     if (n_nodes >= A->node_cap) { defer(); return; }
-    const uint32_t uniq = ++n_uniq;
     parent_event = 0;                           // reportNewlyEnabledExternal (DepTracker.scala:119-122)
-    const uint32_t node = n_nodes++;            // (identical external Sends are screened on the host)
-    pending_insert(make_uint4(hdr, p0, p1, uniq | (node << 16)));
+    const uint32_t w3 = n_nodes++ * 0x10001u;   // (identical external Sends are screened on the host)
+    pending_insert(make_uint4(hdr, p0, p1, w3));
     if (status) return;
-    record_event(DEMI_EV_MSG_SEND, hdr_src(hdr), dst, type, p0, p1, uniq, node, 0u);
+    record_event(DEMI_EV_MSG_SEND, hdr_src(hdr), dst, type, p0, p1, w3, 0u);
   }
 
   // ExternalEventInjector.handle_timer (ExternalEventInjector.scala:282-297)
@@ -310,7 +358,7 @@ struct LaneMachine {
       for (uint32_t i = 0; i < n_ops && !status; i++) {
         const uint32_t w0 = ob[(i * 3) * BD], p0 = ob[(i * 3 + 1) * BD], p1 = ob[(i * 3 + 2) * BD];
         const uint32_t kind = w0 & 0xFF, odst = (w0 >> 8) & 0xFF, otype = (w0 >> 16) & 0xFF;
-        if (kind == OP_SEND) { actor_send_produced(self, odst, otype, p0, p1); continue; }
+        if (kind == OP_SEND) { if (reserve_sends(self, 1)) actor_send_produced(self, odst, otype, p0, p1); continue; }
         if (kind == OP_CANCEL) { cancel_timer(odst, otype, p0, p1); continue; }
         schedule_timer(kind, odst, otype, p0, p1);
       }
@@ -396,7 +444,7 @@ struct LaneMachine {
           break;
         default: break;
       }
-      if (ek) record_event(ek, es, ed, 0, 0, 0, 0, 0, 0);
+      if (ek) record_event(ek, es, ed, 0, 0, 0, 0, 0);
       ext_idx++;
     }
   }
@@ -422,7 +470,7 @@ struct LaneMachine {
     if (nsched == 0x7FFFFFFF) nsched = 1;
     if (++nmod == A->interval) nmod = 0;
     uint32_t src = hdr_src(pick.x), dst = hdr_dst(pick.x), type = hdr_type(pick.x);
-    record_event(DEMI_EV_MSG_EVENT, src, dst, type, pick.y, pick.z, pick.w & 0xFFFF, pick.w >> 16, 0);
+    record_event(DEMI_EV_MSG_EVENT, src, dst, type, pick.y, pick.z, pick.w, 0);
     parent_event = pick.w >> 16;                                // reportNewlyDelivered (DepTracker.scala:132-135)
     window_timers = 0;
     // updateRepeatingTimer :405-421
@@ -483,7 +531,7 @@ struct LaneMachine {
     n_pending = max_pending = 0;
     tosend.clear(); resend = 0; n_resend = 0;
     just = registry = cancelled = root_timers = window_timers = 0;
-    n_nodes = 1; parent_event = 0; n_events = n_uniq = 0;
+    n_nodes = 1; parent_event = 0; n_events = 0;
     nsched = 0; nmod = 0; ext_idx = 0; ext_send_idx = 0;
     violation = status = 0;
     inaccessible = (N >= 32) ? 0xFFFFFFFFu : ((1u << N) - 1u);
@@ -507,12 +555,13 @@ struct LaneMachine {
       }
       if (status | violation) break;
       if (ext_idx < A->n_ext) {
-        record_event(DEMI_EV_QUIESCENCE, DEMI_DEADLETTERS, DEMI_DEADLETTERS, 0, 0, 0, 0, 0, 0);
+        record_event(DEMI_EV_QUIESCENCE, DEMI_DEADLETTERS, DEMI_DEADLETTERS, 0, 0, 0, 0, 0);
         continue;
       }
       break;
     }
     if (!status && nsched <= A->max_messages && !violation) violation = check_invariant();
+    if (n_pending > max_pending) max_pending = n_pending;
     out.status = (uint16_t)status;
     if (!status) {
       uint64_t sh = 0;
@@ -556,7 +605,8 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
   m.rec_ev = nullptr; m.rec_par = nullptr;
 
   const uint64_t count = (REC && args.index_list) ? (uint64_t)(*args.index_count) : args.n_prefixes;
-  unsigned long long my_steps = 0, my_viol = 0, my_defer = 0;
+  unsigned long long my_steps = 0;
+  uint32_t my_viol = 0, my_defer = 0;      // at most one per prefix of this thread
   for (uint64_t it = gthread; it < count; it += total) {
     const uint64_t idx = (REC && args.index_list) ? (uint64_t)args.index_list[it] : it;
     if (REC) {
@@ -602,8 +652,8 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
   }
   if ((tid & 31) == 0 && args.sum_steps && (my_steps | my_viol | my_defer)) {
     atomicAdd(args.sum_steps, my_steps);
-    atomicAdd(args.n_violations, my_viol);
-    if (my_defer) atomicAdd(args.sum_steps + 2, my_defer);      // [2]: prefixes handed to the general engine
+    atomicAdd(args.n_violations, (unsigned long long)my_viol);
+    if (my_defer) atomicAdd(args.sum_steps + 2, (unsigned long long)my_defer);      // [2]: prefixes handed to the general engine
   }
 }
 

@@ -52,6 +52,8 @@ struct Outbox {
     if (n >= OUTBOX_CAP) { overflow = true; return; }
     ops[n++] = make_uint4(op | (dst << 8) | (type << 16), p0, p1, 0u);
   }
+  // the next `k` operations are sends (models.cuh Raft5): nothing to prepare here
+  __device__ __forceinline__ bool reserve(uint32_t) { return true; }
   // `dst ! msg`
   __device__ __forceinline__ void send(uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) { push(OP_SEND, dst, type, p0, p1); }
   // context.system.scheduler.scheduleOnce(_, self, msg)

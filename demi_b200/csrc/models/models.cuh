@@ -255,10 +255,16 @@ struct Raft5 {
       default: break;
     }
     if (cancel_heartbeat) out.cancel_timer(HEARTBEAT_TICK, 0, 0);
+    // A broadcast goes to the four peers in ascending order: trip k sends to k + (k >= self), so no trip is spent on
+    // skipping `self`.  The outbox is told the number of sends first (out.reserve), so an engine that applies them as
+    // they are issued checks its capacities once per delivery; it returns false when they do not fit (the execution
+    // has stopped and the sends are not issued).
     if (plan != PLAN_NONE) {
+      const uint32_t n_sends = plan == PLAN_REPLY ? 1u : 4u;
+      if (!out.reserve(n_sends)) return;
 #pragma unroll 1
-      for (uint32_t j = (plan == PLAN_REPLY ? src : 0u), end = (plan == PLAN_REPLY ? src + 1u : 5u); j < end; j++) {
-        if (plan != PLAN_REPLY && j == self) continue;
+      for (uint32_t k = 0; k < n_sends; k++) {
+        const uint32_t j = plan == PLAN_REPLY ? src : k + (k >= self ? 1u : 0u);
         uint32_t q0 = plan_p0, q1 = 0, qt = plan == PLAN_REPLY ? plan_type : (uint32_t)REQUEST_VOTE;
         if (plan == PLAN_APPEND_ALL) {
           const uint32_t prev = s[NEXT + j];

@@ -56,6 +56,7 @@ struct ReplayArgs {
 template <class M>
 struct ReplayDirectOutbox {
   M* m; uint32_t self;
+  __device__ __forceinline__ bool reserve(uint32_t) { return true; }     // each send checks its own capacities
   __device__ __forceinline__ void send(uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) { m->event_produced(self, dst, type, p0, p1, false); }
   __device__ __forceinline__ void schedule_once(uint32_t type, uint32_t p0, uint32_t p1) { m->schedule_timer(OP_SCHED_ONCE, self, type, p0, p1); }
   __device__ __forceinline__ void schedule_repeating(uint32_t type, uint32_t p0, uint32_t p1) { m->schedule_timer(OP_SCHED_REPEAT, self, type, p0, p1); }

@@ -80,15 +80,29 @@ DEMI_HD uint32_t demi_fmix32(uint32_t h) {
   return h;
 }
 /* Multilinear hash of six 32-bit words into 64 bits: six 32x32->64 multiply-adds
- * (IMAD.WIDE on the GPU) and one 64-bit finaliser. */
-DEMI_HD uint64_t demi_hash6(uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e, uint32_t f) {
-  uint64_t acc = (uint64_t)a * 0x9E3779B1u + (uint64_t)b * 0x85EBCA77u + (uint64_t)c * 0xC2B2AE3Du +
-                 (uint64_t)d * 0x27D4EB2Fu + (uint64_t)e * 0x165667B1u + (uint64_t)f * 0xD3A2646Du +
-                 0x6A09E667BB67AE85ull;
+ * (IMAD.WIDE on the GPU) and one 64-bit finaliser.  The two halves are exposed:
+ * demi_hash6_lin is linear in each word mod 2^64, so a caller that hashes a run of
+ * items whose words differ by known amounts may advance the linear part by
+ * DEMI_HASH6_K* times the differences and apply demi_hash6_fin per item. */
+#define DEMI_HASH6_KA 0x9E3779B1u
+#define DEMI_HASH6_KB 0x85EBCA77u
+#define DEMI_HASH6_KC 0xC2B2AE3Du
+#define DEMI_HASH6_KD 0x27D4EB2Fu
+#define DEMI_HASH6_KE 0x165667B1u
+#define DEMI_HASH6_KF 0xD3A2646Du
+DEMI_HD uint64_t demi_hash6_lin(uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e, uint32_t f) {
+  return (uint64_t)a * DEMI_HASH6_KA + (uint64_t)b * DEMI_HASH6_KB + (uint64_t)c * DEMI_HASH6_KC +
+         (uint64_t)d * DEMI_HASH6_KD + (uint64_t)e * DEMI_HASH6_KE + (uint64_t)f * DEMI_HASH6_KF +
+         0x6A09E667BB67AE85ull;
+}
+DEMI_HD uint64_t demi_hash6_fin(uint64_t acc) {
   acc ^= acc >> 32;
   acc *= 0x9E3779B97F4A7C15ull;
   acc ^= acc >> 29;
   return acc;
+}
+DEMI_HD uint64_t demi_hash6(uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e, uint32_t f) {
+  return demi_hash6_fin(demi_hash6_lin(a, b, c, d, e, f));
 }
 /* One EventTrace element: words as laid out in demi_event (w0 = kind | src<<8 |
  * dst<<16 | type<<24, w3 = uniq | node<<16), seq = position in the trace,
