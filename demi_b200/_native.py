@@ -81,6 +81,20 @@ class IncDDMinOut(C.Structure):
 
 DF_ARVIND_ORDERING, DF_PRIORITIZE_PENDING = 1, 2
 IM_SRC_DST_FIFO = 0x100
+WC_LAST_ONLY = 0x200
+
+
+def clock_rule(type_, word, shift, bits):
+    """DEMI_CLOCK_RULE: messages of `type_` carry the logical clock (p[word] >> shift) & ((1 << bits) - 1)."""
+    return (type_ & 0xFF) | ((word & 0xFF) << 8) | ((shift & 0xFF) << 16) | ((bits & 0xFF) << 24)
+
+
+def type_set(types):
+    """A 256-bit message-type set as the 8 uint32 words demi_set_clock_rules takes."""
+    w = np.zeros(8, dtype=np.uint32)
+    for t in types:
+        w[t >> 5] |= np.uint32(1 << (t & 31))
+    return w
 
 DPOR_RESULT_DTYPE = np.dtype([("interleavings", "<u4"), ("violations", "<u4"), ("deliveries", "<u8"), ("races", "<u8"),
                               ("n_nodes", "<u4"), ("n_explored", "<u4"), ("heap_left", "<u4"), ("exhausted", "<u4"),
@@ -106,6 +120,7 @@ EXPORTS = [
     "demi_dpor_frontier", "demi_dpor_frontier_multi", "demi_comm_unique_id", "demi_comm_init", "demi_comm_rank",
     "demi_create_multi", "demi_conjoin_atoms", "demi_fuzzer_generate", "demi_experiment_save", "demi_experiment_load",
     "demi_load_model", "demi_actor_index", "demi_actor_name", "demi_set_user_filter",
+    "demi_set_clock_rules", "demi_wildcard_replay_batch", "demi_wildcard_replay_trace", "demi_wildcard_minimize",
 ]
 FILTER_RULE_DTYPE = np.dtype([("src_mask", "<u4"), ("dst_mask", "<u4"), ("type_mask", "<u4"), ("flags", "<u4")])
 FRULE_DEADLETTERS = 1
@@ -240,6 +255,15 @@ def lib():
     L.demi_experiment_load.argtypes = [C.c_char_p, C.POINTER(Experiment)]
     L.demi_conjoin_atoms.restype = C.c_int32
     L.demi_conjoin_atoms.argtypes = [vp, C.c_uint32, C.c_uint32]
+    L.demi_set_clock_rules.restype = C.c_int32
+    L.demi_set_clock_rules.argtypes = [vp, vp, C.c_uint32, vp]
+    L.demi_wildcard_replay_batch.restype = C.c_int32
+    L.demi_wildcard_replay_batch.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, vp]
+    L.demi_wildcard_replay_trace.restype = C.c_int32
+    L.demi_wildcard_replay_trace.argtypes = [vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, C.POINTER(C.c_uint32),
+                                             vp, C.c_uint32, C.POINTER(C.c_uint32), vp]
+    L.demi_wildcard_minimize.restype = C.c_int32
+    L.demi_wildcard_minimize.argtypes = [vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(IntMinOut)]
     L.demi_stats.restype = C.c_int32
     L.demi_stats.argtypes = [vp, C.POINTER(Perf)]
     _lib = L

@@ -2,8 +2,9 @@
 
   demi_b200/libdemi_b200.so  — the CUDA engine + C ABI (nvcc, sm_90a only)
   oracle/liboracle.so        — the CPU oracle (gcc; test infrastructure only)
+  oracle/liboracle_wildcard.so — the same oracle with the wildcard-minimization restatement (oracle/wildcard.mk)
 
-Both are git-ignored build products.
+All three are git-ignored build products.
 """
 import os
 import subprocess
@@ -14,6 +15,7 @@ CSRC = os.path.join(ROOT, "demi_b200", "csrc")
 LIB = os.path.join(ROOT, "demi_b200", "libdemi_b200.so")
 ORACLE_DIR = os.path.join(ROOT, "oracle")
 ORACLE_LIB = os.path.join(ORACLE_DIR, "liboracle.so")
+ORACLE_WILDCARD_LIB = os.path.join(ORACLE_DIR, "liboracle_wildcard.so")   # oracle/wildcard.mk
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -99,12 +101,14 @@ ORACLE_STAMP = os.path.join(ORACLE_DIR, ".build_cpu")
 def build_oracle(force=False):
     srcs = _sources(ORACLE_DIR, (".c", ".h")) + _sources(os.path.join(ROOT, "include"), (".h",))
     srcs.append(os.path.join(ORACLE_DIR, "Makefile"))
+    srcs.append(os.path.join(ORACLE_DIR, "wildcard.mk"))
     stamp = _cpu_stamp()
     same_cpu = os.path.exists(ORACLE_STAMP) and open(ORACLE_STAMP).read().strip() == stamp
-    if not force and same_cpu and _newer(ORACLE_LIB, srcs):
+    if not force and same_cpu and _newer(ORACLE_LIB, srcs) and _newer(ORACLE_WILDCARD_LIB, srcs):
         return ORACLE_LIB
     # make's chatter goes to stderr: bench.py prints exactly one JSON line on stdout
     subprocess.check_call(["make", "-B", "-C", ORACLE_DIR, "liboracle.so"], stdout=sys.stderr)
+    subprocess.check_call(["make", "-B", "-C", ORACLE_DIR, "-f", "wildcard.mk", "liboracle_wildcard.so"], stdout=sys.stderr)
     with open(ORACLE_STAMP, "w") as f:
         f.write(stamp + "\n")
     return ORACLE_LIB

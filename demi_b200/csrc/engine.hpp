@@ -76,6 +76,10 @@ struct demi_handle {
   // ---- FullyRandom's userDefinedFilter as rules (demi_set_user_filter); HardKill in the external program
   std::vector<demi_filter_rule> filter;
   bool has_hard_kill = false;
+  // ---- FingerprintFactory.getLogicalClock / causesClockIncrement as data (demi_set_clock_rules, capi_wildcard.cu):
+  // per type the packed rule (0 = no clock; a valid rule has bits >= 1, so it is never 0) and the incrementing set
+  uint32_t clock_rule[256] = {};
+  uint32_t clock_incr[8] = {};
   // ---- launch bookkeeping
   std::map<const void*, int> occupancy;          // kernel -> resident blocks per SM (asked once per handle)
   void* trace_rec = nullptr; size_t trace_rec_bytes = 0;   // demi_fuzz_trace's recording buffer

@@ -49,7 +49,14 @@ struct ReplayArgs {
   uint32_t* tosend;     // [warps][tosend_cap][32]
   uint32_t* pruned;     // [warps][n_uniq_words + N][32]  (only with DEMI_RF_FILTER_KNOWN_ABSENTS)
   unsigned long long* counters;   // [0] reproduced, [1] delivered
+  // wildcard replay (WILD instantiations only; the others ignore these): per trace event, for MsgEvents,
+  // mode << 16 | delivery ordinal; include masks over deliveries; the causesClockIncrement type set; the
+  // trace positions of ignored deliveries (single-test REC launches)
+  const uint32_t* wc_ev; const uint64_t* wc_include; uint32_t wc_words;
+  uint32_t wc_incr[8];
+  uint32_t* wc_ignored; uint32_t wc_ignored_cap; uint32_t* wc_ignored_count;
 };
+enum : uint32_t { WC_EXACT = 0, WC_CLASS = 1, WC_CLOCK = 2 };   // match mode of one delivery of the base trace
 
 // receive()'s view when its operations are applied as they are issued (program order is the reference's order:
 // `!`, scheduleOnce and cancel() act synchronously inside receive()); no staging in shared memory.
@@ -63,8 +70,11 @@ struct ReplayDirectOutbox {
   __device__ __forceinline__ void cancel_timer(uint32_t type, uint32_t p0, uint32_t p1) { m->cancel_timer(self, type, p0, p1); }
 };
 
-template <class MODEL, int BD, bool REC = false>
+// WILD: ClockClusterizer's wildcarded trace (capi_wildcard.cu).  The pending set is the insertion-ordered list of
+// the REC variant (Uniq order = list order), compacted in place when taken entries dominate it.
+template <class MODEL, int BD, bool REC = false, bool WILD = false>
 struct ReplayMachine {
+  static constexpr bool LIST = REC || WILD;
   static constexpr int N = MODEL::N_ACTORS;
   static constexpr int SW = MODEL::STATE_WORDS;
   static constexpr int OB = MODEL::REPLAY_OUTBOX;
@@ -123,9 +133,62 @@ struct ReplayMachine {
       s = (s + 1) & (A->table_slots - 1);
     }
   }
+  // ---- WILD: list entries before list_lo are all taken; list_compact squeezes the taken entries out, order kept
+  uint32_t list_lo;
+  __device__ __forceinline__ void list_compact() {
+    uint32_t j = 0;
+    for (uint32_t i = list_lo; i < n_list; i++) {
+      uint4 q = table[(size_t)i * 32];
+      if (q.w & 0x80000000u) table[(size_t)(j++) * 32] = q;
+    }
+    n_list = j; list_lo = 0;
+  }
+  __device__ __forceinline__ void list_take(uint32_t i, uint4 q) {
+    table[(size_t)i * 32] = make_uint4(q.x, q.y, q.z, q.w & 0x7FFFFFFFu);
+    n_pending--;
+    if (WILD && i == list_lo)
+      while (list_lo < n_list && !(table[(size_t)list_lo * 32].w & 0x80000000u)) list_lo++;
+  }
+  __device__ __forceinline__ bool wc_incr(uint32_t type) const { return (A->wc_incr[type >> 5] >> (type & 31)) & 1u; }
+  // The pending message a wildcard delivery from snd to rcv takes (STSScheduler.messagePending :381-403 and
+  // schedule_new_message :696-708): list position, or -1 when none matches.  The fingerprint queues of (snd, rcv)
+  // in the order of their head's Uniq id are the list's live entries of (snd, rcv) that no older live entry shares
+  // a fingerprint with.  The oldest matching message heads the first matching queue (BackTrackStrategy,
+  // ClockClusterizer.scala:107-112 for the clock-increment selector); LastOnlyStrategy takes the newest such head.
+  __device__ __forceinline__ int wild_pick(uint32_t snd, uint32_t rcv, uint32_t mode, uint32_t type, bool last) {
+    const uint32_t pair = snd | (rcv << 8);
+    int pick = -1;
+    // Last: the payloads of the queue heads met so far (a class selector matches one header, so the payload is the
+    // fingerprint); past HEADS of them an entry is checked against every older entry instead
+    constexpr uint32_t HEADS = 8;
+    uint32_t seen_p0[HEADS], seen_p1[HEADS], n_seen = 0;
+    for (uint32_t i = list_lo; i < n_list; i++) {
+      const uint4 q = table[(size_t)i * 32];
+      if (!(q.w & 0x80000000u) || (q.x & 0xFFFFu) != pair) continue;
+      const uint32_t t = (q.x >> 16) & 0xFF;
+      if (!(mode == WC_CLOCK ? wc_incr(t) : t == type)) continue;
+      if (mode == WC_CLOCK || !last) return (int)i;
+      bool head = true;
+      for (uint32_t k = 0; k < n_seen && k < HEADS && head; k++) head = !(seen_p0[k] == q.y && seen_p1[k] == q.z);
+      for (uint32_t j = list_lo; head && n_seen > HEADS && j < i; j++) {
+        const uint4 r = table[(size_t)j * 32];
+        head = !((r.w & 0x80000000u) && r.x == q.x && r.y == q.y && r.z == q.z);
+      }
+      if (head) {
+        pick = (int)i;
+        if (n_seen < HEADS) { seen_p0[n_seen] = q.y; seen_p1[n_seen] = q.z; }
+        n_seen++;
+      }
+    }
+    return pick;
+  }
+
   __device__ __forceinline__ void pending_add(uint32_t hdr, uint32_t p0, uint32_t p1, uint32_t uniq = 0) {
     if (n_pending >= A->pending_cap) { status = DEMI_PS_PENDING_OVF; return; }
-    if (REC) {
+    if (LIST) {
+      // n_pending < pending_cap <= table_slots, so compacting a full list frees a slot; compacting once dead entries
+      // outnumber live ones keeps every scan short (amortised O(1) per operation)
+      if (WILD && (n_list >= A->table_slots || n_list - list_lo >= 2 * n_pending + 32)) list_compact();
       if (n_list >= A->table_slots) { status = DEMI_RS_UNSUPPORTED; return; }
       table[(size_t)n_list * 32] = make_uint4(hdr, p0, p1, uniq | 0x80000000u);
       n_list++; n_pending++;
@@ -138,13 +201,12 @@ struct ReplayMachine {
     n_pending++;
   }
   __device__ __forceinline__ bool pending_take(uint32_t hdr, uint32_t p0, uint32_t p1, uint32_t* uniq_out = nullptr) {
-    if (REC) {
-      for (uint32_t i = 0; i < n_list; i++) {
+    if (LIST) {
+      for (uint32_t i = WILD ? list_lo : 0; i < n_list; i++) {
         uint4 q = table[(size_t)i * 32];
         if ((q.w & 0x80000000u) && q.x == hdr && q.y == p0 && q.z == p1) {
-          table[(size_t)i * 32] = make_uint4(q.x, q.y, q.z, q.w & 0x7FFFFFFFu);
           if (uniq_out) *uniq_out = q.w & 0xFFFFu;
-          n_pending--;
+          list_take(i, q);
           return true;
         }
       }
@@ -183,7 +245,7 @@ struct ReplayMachine {
     int slot = MODEL::timer_slot(dst, type, p0, p1);
     if (cancelled && slot >= 0 && ((cancelled >> slot) & 1u)) { cancelled &= ~(1u << slot); return; }
     uint32_t uniq = 0;
-    if (REC) {
+    if (LIST) {
       uniq = ++n_uniq;                                              // Uniq(...) :570; appendMsgSend :620-622
       rec_push(DEMI_EV_MSG_SEND, (!external && src == DEMI_DEADLETTERS) ? DEMI_TIMER_SND : src, dst, type, p0, p1, uniq);
     }
@@ -271,11 +333,21 @@ struct ReplayMachine {
     handle_timer((uint32_t)s2);
   }
 
+  // WILD + REC: the trace positions of ignored deliveries, from which WildcardMinimizer takes ignoredAbsentIds
+  // (WildcardMinimizer.scala:197-235)
+  const uint64_t* wc_inc; uint32_t n_ign;
+  __device__ __forceinline__ void note_ignored(uint32_t i) {
+    if (!(WILD && REC)) return;
+    if (A->wc_ignored && n_ign < A->wc_ignored_cap) A->wc_ignored[n_ign] = i;
+    n_ign++;
+  }
+
   __device__ __forceinline__ void run(uint32_t test_idx, uint32_t generation, demi_replay_result& out) {
     mask = A->masks ? A->masks + (size_t)test_idx * A->mask_words : nullptr;
     mword_idx = 0xFFFFFFFFu; mword = 0;
     const uint32_t skip = A->skips ? A->skips[test_idx] : 0xFFFFFFFFu;
     n_rec = n_uniq = n_list = 0;
+    if constexpr (WILD) { wc_inc = A->wc_include + (size_t)test_idx * A->wc_words; list_lo = 0; n_ign = 0; }
     gen = generation;
     for (uint32_t i = 0; i < N * SW; i++) smw[i * BD] = MODEL::init_word(i, A->model_flags);
     for (uint32_t a = 0; a < N; a++) part_row(a) = 0;
@@ -345,6 +417,14 @@ struct ReplayMachine {
         else if (kind == DEMI_EV_UNPARTITION) PF_ROW(src) |= 1u << dst;
       }
       if (!k || i == skip) continue;
+      uint32_t wmode = WC_EXACT;
+      if constexpr (WILD) {
+        if (kind == DEMI_EV_MSG_EVENT) {                             // ClockClusterizer.getNextTrace (:101-126)
+          const uint32_t w = __ldg(A->wc_ev + i), d = w & 0xFFFFu;
+          wmode = w >> 16;
+          if (wmode != WC_EXACT && !((__ldg(wc_inc + (d >> 6)) >> (d & 63)) & 1ull)) continue;
+        }
+      }
       // ---- STSSched: advanceReplay (:405-559)
       switch (kind) {
         case DEMI_EV_SPAWN: rec_push(kind, src, dst, 0, 0, 0, 0); inaccessible &= ~(1u << dst); killed &= ~(1u << dst); break;
@@ -358,12 +438,26 @@ struct ReplayMachine {
         case DEMI_EV_MSG_EVENT: {
           flush();                                                   // messagePending :381-403
           if (status) break;
+          if constexpr (WILD) {
+            if (wmode != WC_EXACT) {                                 // WildCardMatch: deliver the selected pending message
+              const int at = ((A->blocked_mask >> (dst & 31)) & 1u) ? -1
+                             : wild_pick(src, dst, wmode, type, (A->flags & DEMI_WC_LAST_ONLY) != 0);
+              if (at >= 0) {
+                const uint4 q = table[(size_t)at * 32];
+                const uint32_t qt = (q.x >> 16) & 0xFF;
+                list_take((uint32_t)at, q);
+                rec_push(DEMI_EV_MSG_EVENT, src, dst, qt, q.y, q.z, q.w & 0xFFFFu);
+                deliver(src, dst, qt, q.y, q.z);
+              } else { ignored++; note_ignored(i); }
+              break;
+            }
+          }
           uint32_t hdr = make_hdr(src, dst, type, 0);
           uint32_t duniq = 0;
           bool enabled = !((A->blocked_mask >> (dst & 31)) & 1u) && pending_take(hdr, e.y, e.z, &duniq);
           if (enabled) { rec_push(DEMI_EV_MSG_EVENT, src, dst, type, e.y, e.z, duniq); deliver(src, dst, type, e.y, e.z); }   // :696-772
           else if (strict) diverged = true;                          // ReplayScheduler: ReplayException
-          else ignored++;                                            // "Ignoring message" :528-529
+          else { ignored++; note_ignored(i); }                       // "Ignoring message" :528-529
           break;
         }
         default: break;
@@ -373,6 +467,7 @@ struct ReplayMachine {
     if (!status && !diverged) flush();                               // :682 before trace_finished
     out.violation = 0; out.delivered = 0; out.ignored = 0; out.state_hash = 0;
     if (REC && A->rec_count) *A->rec_count = n_rec;
+    if (WILD && REC && A->wc_ignored_count) *A->wc_ignored_count = n_ign;
     if (status) { out.status = (uint16_t)status; return; }
     if (diverged) { out.status = DEMI_RS_DIVERGED; out.delivered = (uint16_t)delivered; return; }
     uint32_t v = MODEL::invariant(LaneAll<SW>{smw, BD}, A->model_flags);      // :283-289
@@ -385,10 +480,10 @@ struct ReplayMachine {
   }
 };
 
-template <class MODEL, int BD, bool REC = false>
+template <class MODEL, int BD, bool REC = false, bool WILD = false>
 __global__ void __launch_bounds__(BD, (model_replay_direct<MODEL>::value && MODEL::N_ACTORS <= 8) ? 1024 / BD : 1)
 replay_lane_kernel(const __grid_constant__ ReplayArgs args) {
-  using M = ReplayMachine<MODEL, BD, REC>;
+  using M = ReplayMachine<MODEL, BD, REC, WILD>;
   extern __shared__ __align__(16) uint32_t lane_smem[];
   const uint32_t tid = threadIdx.x;
   const uint64_t gthread = (uint64_t)blockIdx.x * BD + tid;

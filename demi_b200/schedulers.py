@@ -192,6 +192,47 @@ class Engine(object):
                                                    sizes.ctypes.data, cap_events, C.byref(out)))
         return ev[:out.n_events].copy(), sizes[:out.n_internal_sizes].copy(), out
 
+    # ---- fungible clocks (wildcard_minimization/)
+    def set_clock_rules(self, rules, increment_types=()):
+        """FingerprintFactory.getLogicalClock / causesClockIncrement as data: rules = packed N.clock_rule words,
+        increment_types = the message types that causesClockIncrement.  ([], ()) is the reference's default."""
+        r = np.ascontiguousarray(list(rules), dtype=np.uint32)
+        inc = N.type_set(increment_types)
+        self._check(N.lib().demi_set_clock_rules(self._h, r.ctypes.data if len(r) else None, len(r), inc.ctypes.data))
+
+    def wildcard_words(self):
+        return max(1, (int((self._trace["kind"] == N.EV_MSG_EVENT).sum()) + 63) // 64)
+
+    def wildcard_replay_batch(self, include_masks, looking_for=0, flags=0):
+        """One STSScheduler.test per include mask (bits over the trace's deliveries, in trace order)."""
+        m = np.ascontiguousarray(include_masks, dtype=np.uint64).reshape(-1, self.wildcard_words())
+        out = np.empty(len(m), dtype=N.REPLAY_DTYPE)
+        self._check(N.lib().demi_wildcard_replay_batch(self._h, m.ctypes.data, len(m), looking_for or 0, flags,
+                                                       out.ctypes.data))
+        return out
+
+    def wildcard_replay_trace(self, include_mask, looking_for=0, flags=0, cap_events=65536):
+        """(result, recorded EventTrace, trace positions of the ignored deliveries)."""
+        m = np.ascontiguousarray(include_mask, dtype=np.uint64)
+        ev = np.zeros(cap_events, dtype=N.EVENT_DTYPE)
+        cap_ign = max(1, len(self._trace))
+        ign = np.zeros(cap_ign, dtype=np.uint32)
+        n, ni = C.c_uint32(), C.c_uint32()
+        res = np.zeros(1, dtype=N.REPLAY_DTYPE)
+        self._check(N.lib().demi_wildcard_replay_trace(self._h, m.ctypes.data, looking_for or 0, flags, ev.ctypes.data,
+                                                       cap_events, C.byref(n), ign.ctypes.data, cap_ign, C.byref(ni),
+                                                       res.ctypes.data))
+        return res[0], ev[:n.value].copy(), ign[:ni.value].copy()
+
+    def wildcard_minimize(self, looking_for, flags=0, cap_events=65536):
+        ev = np.zeros(cap_events, dtype=N.EVENT_DTYPE)
+        sizes = np.zeros(cap_events, dtype=np.uint32)
+        out = N.IntMinOut()
+        self._check(N.lib().demi_wildcard_minimize(self._h, looking_for or 0, flags, ev.ctypes.data, cap_events,
+                                                   sizes.ctypes.data, cap_events, C.byref(out)))
+        self._trace = ev[:out.n_events].copy()           # the handle's trace is now the minimized one
+        return self._trace.copy(), sizes[:out.n_internal_sizes].copy(), out
+
     def conjoin_atoms(self, e1, e2):
         """UnmodifiedEventDag.conjoinAtoms: externals e1, e2 (indices into the trace's externals) form one atom."""
         self._check(N.lib().demi_conjoin_atoms(self._h, e1, e2))
@@ -676,5 +717,79 @@ class STSSchedMinimizer(object):
         trace, sizes, out = self.engine.internal_minimize(self.violation, flags=self.flags)
         self._stats.record_series(sizes, internal=True)
         self._stats.total_replays += out.total_replays
+        self.last = out
+        return self._stats, trace
+
+
+# ---- fungible clocks: wildcard_minimization/ (WildcardMinimizer.scala, ClockClusterizer.scala,
+# AmbiguityResolutionStrategies.scala)
+RAFT5_REQUEST_VOTE, RAFT5_VOTE_REPLY, RAFT5_APPEND_ENTRIES, RAFT5_APPEND_REPLY, RAFT5_ELECTION_TICK = 4, 5, 7, 8, 3
+
+
+def raft5_clock_rules():
+    """raft5's FingerprintFactory: the term is p0 & 0xFF of RequestVote, VoteReply, AppendEntries and AppendReply,
+    and an ElectionTick increments the clock (the hint at ClockClusterizer.scala:24-27).  (rules, increment_types)
+    for Engine.set_clock_rules / WildcardMinimizer."""
+    rules = [N.clock_rule(t, 0, 0, 8) for t in (RAFT5_REQUEST_VOTE, RAFT5_VOTE_REPLY, RAFT5_APPEND_ENTRIES,
+                                                 RAFT5_APPEND_REPLY)]
+    return rules, (RAFT5_ELECTION_TICK,)
+
+
+class TestScheduler(object):
+    """WildcardMinimizer.scala:21-27."""
+    STSSched, DPORwHeuristics = "STSSched", "DPORwHeuristics"
+
+
+class ClusteringStrategy(object):
+    """WildcardMinimizer.scala:31-36."""
+    ClockClusterizer, SingletonClusterizer, ClockThenSingleton = "ClockClusterizer", "SingletonClusterizer", "ClockThenSingleton"
+
+
+class BackTrackStrategy(object):
+    """AmbiguityResolutionStrategies.scala:44-75: the first matching queue head (its backtrack points are a no-op
+    under STSSched)."""
+    flags = 0
+
+
+class LastOnlyStrategy(object):
+    """AmbiguityResolutionStrategies.scala:109-117: the last matching queue head."""
+    flags = N.WC_LAST_ONLY
+
+
+class WildcardMinimizer(object):
+    """WildcardMinimizer(schedulerConfig, mcs, trace, violation, ...) — wildcard_minimization/WildcardMinimizer.scala:
+    47-241 with testScheduler = STSSched and ClusteringStrategy.ClockClusterizer (runTheGamut's WildcardsNoBackTracks
+    and, with resolutionStrategy=LastOnlyStrategy(), WildcardsLastOnly, RunnerUtils.scala:413-440).  The message
+    fingerprinter's getLogicalClock / causesClockIncrement are `clock_rules` = (rules, increment_types), e.g.
+    raft5_clock_rules().  minimize() returns (MinimizationStats, minimized EventTrace)."""
+
+    def __init__(self, schedulerConfig, mcs, trace, violation, skipClockClusters=False, resolutionStrategy=None,
+                 testScheduler=TestScheduler.STSSched, stats=None, clusteringStrategy=ClusteringStrategy.ClockClusterizer,
+                 clock_rules=((), ()), filterKnownAbsents=False, engine=None):
+        if testScheduler != TestScheduler.STSSched:
+            raise NotImplementedError("WildcardMinimizer with DPORwHeuristics as the test scheduler is outside the accelerated path")
+        if clusteringStrategy != ClusteringStrategy.ClockClusterizer:
+            raise NotImplementedError("%s is outside the accelerated path" % clusteringStrategy)
+        if skipClockClusters:
+            raise NotImplementedError("skipClockClusters (the wildcard TestOracle) is outside the accelerated path")
+        if resolutionStrategy is not None and not isinstance(resolutionStrategy, (BackTrackStrategy, LastOnlyStrategy)):
+            raise NotImplementedError("BackTrackStrategy and LastOnlyStrategy are the accelerated resolution strategies")
+        self.resolutionStrategy = resolutionStrategy or BackTrackStrategy()     # :147-149
+        self.mcs, self.trace, self.violation = mcs, trace, violation
+        self.clock_rules = clock_rules
+        self.flags = self.resolutionStrategy.flags | (N.RF_FILTER_KNOWN_ABSENTS if filterKnownAbsents else 0)
+        self.engine = engine or Engine(schedulerConfig)
+        self._stats = stats or MinimizationStats()
+        self.last = None
+
+    def minimize(self):
+        self._stats.updateStrategy("FungibleClockMinimizer", "STSSched")        # :141
+        self._stats.record_prune_start()                                         # doMinimize :195
+        self.engine.set_trace(self.trace, self.mcs if isinstance(self.mcs, np.ndarray) else pack_externals(list(self.mcs)))
+        self.engine.set_clock_rules(*self.clock_rules)
+        trace, sizes, out = self.engine.wildcard_minimize(self.violation, flags=self.flags)
+        self._stats.record_series(sizes, internal=True)                         # :210-212 and the fencepost :184
+        self._stats.total_replays += out.total_replays
+        self._stats.record_prune_end()                                           # :182
         self.last = out
         return self._stats, trace

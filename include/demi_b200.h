@@ -292,6 +292,47 @@ int32_t demi_internal_minimize(demi_handle* h, uint32_t looking_for, uint32_t fl
                                demi_event* out_trace, uint32_t cap_events,
                                uint32_t* internal_sizes, uint32_t cap_sizes, demi_intmin_out* out);
 
+/* ---------------------------------------------- fungible clocks (wildcard minimization)
+ * FingerprintFactory.getLogicalClock / causesClockIncrement (MessageFingerprints.scala:26-31) as data.  A message's
+ * "class" (ClassTag(msg.getClass), ClockClusterizer.scala:115-118) is its `type` byte.
+ *   rules[i]  = type | word << 8 | shift << 16 | bits << 24: messages of `type` carry the logical clock
+ *               (p[word] >> shift) & ((1 << bits) - 1), word in {0,1} (p0, p1), shift <= 31, 1 <= bits <= 32.
+ *               A type without a rule has no clock (None).  At most one rule per type.
+ *   increment_types: 8 words, a 256-bit set of the types that causesClockIncrement; NULL = none.
+ * (NULL, 0, NULL) is the reference's default: no clocks, no clock-incrementing types (:28, :31).  Per handle, host
+ * data only; malformed rules return DEMI_ERR_INVALID and leave the previous rules in place. */
+#define DEMI_CLOCK_RULE(type, word, shift, bits) ((uint32_t)(type) | ((uint32_t)(word) << 8) | ((uint32_t)(shift) << 16) | ((uint32_t)(bits) << 24))
+int32_t demi_set_clock_rules(demi_handle* h, const uint32_t* rules, uint32_t n_rules, const uint32_t* increment_types);
+
+/* STSScheduler.test of one ClockClusterizer.getNextTrace (ClockClusterizer.scala:73-134) over the handle's trace,
+ * replaying its full external sequence.  A test is an include bitmask over the trace's deliveries (MsgEvents, in
+ * trace order; ceil(n_deliveries / 64) words per test).  Each delivery has a match mode fixed by the trace and the
+ * clock rules: an external delivery is replayed exactly whatever its bit says; an included clock-incrementing one
+ * becomes the "CausesClockIncrement" wildcard (oldest pending clock-incrementing message from its sender to its
+ * receiver); any other included one a class wildcard (a pending message of the same type, chosen among the
+ * fingerprint queues of (sender, receiver) ordered by the Uniq id of their head: the first matching head, or with
+ * DEMI_WC_LAST_ONLY the last one, AmbiguityResolutionStrategies.scala:44-75, :109-117).  A delivery whose bit is
+ * clear is left out.  A wildcard delivers the selected pending message; an absent one is ignored (:528-529).
+ * flags: DEMI_RF_FILTER_KNOWN_ABSENTS, DEMI_WC_LAST_ONLY; DEMI_RF_STRICT is rejected.  The trace's MsgEvent Uniq ids
+ * must be distinct.  The pending set is bounded by demi_wildcard_pending_cap, in demi_limits.h. */
+#define DEMI_WC_LAST_ONLY 0x200u
+int32_t demi_wildcard_replay_batch(demi_handle* h, const uint64_t* include_masks, uint32_t n_tests,
+                                   uint32_t looking_for, uint32_t flags, demi_replay_result* out);
+/* One such test in recording mode: the EventTrace STSScheduler.test returns (wildcards recorded as the message they
+ * delivered, with its Uniq id) and the trace positions of the deliveries it ignored (ignoreAbsentCallback). */
+int32_t demi_wildcard_replay_trace(demi_handle* h, const uint64_t* include_mask, uint32_t looking_for, uint32_t flags,
+                                   demi_event* events, uint32_t cap_events, uint32_t* n_events,
+                                   uint32_t* ignored_positions, uint32_t cap_ignored, uint32_t* n_ignored,
+                                   demi_replay_result* result);
+/* WildcardMinimizer.minimize (wildcard_minimization/WildcardMinimizer.scala:133-241) with testScheduler = STSSched,
+ * ClockClusterizer and Aggressiveness.ALL_TIMERS_FIRST_ITR over the handle's trace (a verified MCS trace) and clock
+ * rules.  Decisions, total_replays, the internal sizes (one per test, then the final fencepost) and the returned
+ * trace are the sequential ones; tests are evaluated speculatively in batches.  `out->unignorable` is 0 (the
+ * minimizer has no unignorable set).  On return the handle's trace is the minimized one. */
+int32_t demi_wildcard_minimize(demi_handle* h, uint32_t looking_for, uint32_t flags,
+                               demi_event* out_trace, uint32_t cap_events,
+                               uint32_t* internal_sizes, uint32_t cap_sizes, demi_intmin_out* out);
+
 /* DDMin.minimize over the trace's externals with STSSched as the TestOracle
  * (RunnerUtils.stsSchedDDMin, RunnerUtils.scala:642-707; DeltaDebugging.scala:27-109).
  * WaitQuiescence externals are dropped first (RunnerUtils.scala:678-684).  The

@@ -12,6 +12,7 @@
 //   ReplayScheduler      schedulers/ReplayScheduler.scala:71 (replay; ReplayException :128-130)
 //   DDMin                minification/DeltaDebugging.scala:7 (minimize :27, verify_mcs :64)
 //   STSSchedMinimizer    minification/internal_minimization/ScheduleCheckers.scala:19 (minimize :34)
+//   WildcardMinimizer    minification/wildcard_minimization/WildcardMinimizer.scala:47 (minimize :133)
 //   DPORwHeuristics      schedulers/DPORwHeuristics.scala:77 (test :1193, setMaxMessagesToSchedule :123,
 //                        setDepthBound :116)
 //   MinimizationStats    minification/Minimizer.scala:30-237 (the counters DDMin / the minimizers drive)
@@ -28,6 +29,7 @@
 #include <optional>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <vector>
 #include "demi_b200.h"
 
@@ -336,6 +338,63 @@ class STSSchedMinimizer {
   demi_intmin_out last{};
  private:
   std::shared_ptr<Engine> engine; ExternalEvents mcs; EventTrace verified_mcs; ViolationFingerprint violation; uint32_t flags;
+};
+
+// ---- fungible clocks (minification/wildcard_minimization/)
+// FingerprintFactory.getLogicalClock / causesClockIncrement as data (demi_set_clock_rules): packed rules + the
+// clock-incrementing message types.
+struct ClockRules { std::vector<uint32_t> rules; std::vector<uint32_t> increment_types; };
+// raft5: the term is p0 & 0xFF of RequestVote, VoteReply, AppendEntries and AppendReply; ElectionTick increments it
+// (the hint at ClockClusterizer.scala:24-27).
+inline ClockRules raft5_clock_rules() {
+  return ClockRules{{DEMI_CLOCK_RULE(4, 0, 0, 8), DEMI_CLOCK_RULE(5, 0, 0, 8), DEMI_CLOCK_RULE(7, 0, 0, 8),
+                     DEMI_CLOCK_RULE(8, 0, 0, 8)}, {3}};
+}
+struct BackTrackStrategy {};           // AmbiguityResolutionStrategy (AmbiguityResolutionStrategies.scala:44-75)
+struct LastOnlyStrategy {};            // (:109-117)
+enum class TestScheduler { STSSched, DPORwHeuristics };                                   // WildcardMinimizer.scala:21-27
+enum class ClusteringStrategy { ClockClusterizer, SingletonClusterizer, ClockThenSingleton };   // :31-36
+
+// WildcardMinimizer(schedulerConfig, mcs, trace, violation, ...) (WildcardMinimizer.scala:47-241) with
+// testScheduler = STSSched and ClockClusterizer: runTheGamut's WildcardsNoBackTracks / WildcardsLastOnly
+// (RunnerUtils.scala:413-440).  The other test schedulers and clusterizers, and skipClockClusters, are outside the
+// accelerated path and throw std::invalid_argument.
+class WildcardMinimizer {
+ public:
+  template <class Strategy = BackTrackStrategy>
+  WildcardMinimizer(const SchedulerConfig& cfg, const ExternalEvents& mcs, const EventTrace& trace, ViolationFingerprint violation,
+                    ClockRules rules, Strategy = Strategy(), TestScheduler ts = TestScheduler::STSSched,
+                    ClusteringStrategy cs = ClusteringStrategy::ClockClusterizer, bool skipClockClusters = false,
+                    std::shared_ptr<Engine> e = nullptr)
+      : mcs(mcs), trace(trace), violation(violation), rules(std::move(rules)),
+        flags((cfg.filterKnownAbsents ? DEMI_RF_FILTER_KNOWN_ABSENTS : 0) |
+              (std::is_same<Strategy, LastOnlyStrategy>::value ? DEMI_WC_LAST_ONLY : 0)) {
+    static_assert(std::is_same<Strategy, BackTrackStrategy>::value || std::is_same<Strategy, LastOnlyStrategy>::value,
+                  "BackTrackStrategy and LastOnlyStrategy are the accelerated resolution strategies");
+    if (ts != TestScheduler::STSSched) throw std::invalid_argument("DPORwHeuristics as the test scheduler is outside the accelerated path");
+    if (cs != ClusteringStrategy::ClockClusterizer) throw std::invalid_argument("only ClockClusterizer is on the accelerated path");
+    if (skipClockClusters) throw std::invalid_argument("skipClockClusters is outside the accelerated path");
+    engine = e ? e : std::make_shared<Engine>(cfg);
+  }
+  std::pair<MinimizationStats, EventTrace> minimize() {
+    engine->check(demi_set_trace(engine->handle(), trace.data(), (uint32_t)trace.size(), mcs.data(), (uint32_t)mcs.size()));
+    uint32_t incr[8] = {};
+    for (uint32_t t : rules.increment_types) incr[(t & 0xFF) >> 5] |= 1u << (t & 31);
+    engine->check(demi_set_clock_rules(engine->handle(), rules.rules.data(), (uint32_t)rules.rules.size(), incr));
+    EventTrace out(65536); std::vector<uint32_t> sizes(65536);
+    engine->check(demi_wildcard_minimize(engine->handle(), violation, flags, out.data(), (uint32_t)out.size(), sizes.data(),
+                                         (uint32_t)sizes.size(), &last));
+    out.resize(last.n_events);
+    MinimizationStats s;
+    s.updateStrategy("FungibleClockMinimizer", "STSSched");                   // WildcardMinimizer.scala:141
+    s.record_series(sizes.data(), last.n_internal_sizes, true);               // :210-212 and the fencepost :184
+    s.total_replays_ref() = last.total_replays;
+    return {s, out};
+  }
+  demi_intmin_out last{};
+ private:
+  std::shared_ptr<Engine> engine; ExternalEvents mcs; EventTrace trace; ViolationFingerprint violation; ClockRules rules;
+  uint32_t flags;
 };
 
 // ProvenanceTracker(trace, depGraph) (schedulers/Util.scala:267-376): `trace` is the recorded EventTrace of an

@@ -158,4 +158,12 @@ static inline uint32_t demi_fr_pool_entries(int model, int32_t max_messages, uin
   }
 }
 
+/* ---- wildcard replay (demi_wildcard_replay_*): a wildcard delivery may deliver another message than the trace
+ * did, so the base trace's own sends no longer bound the pending set.  Bound: what an execution of at most
+ * n_deliveries deliveries can create (the executor rule above), clamped like the other pending capacities.  A test
+ * whose pending set would exceed it reports DEMI_PS_PENDING_OVF, in the engine and in the oracle alike. */
+static inline uint32_t demi_wildcard_pending_cap(int model, uint32_t n_deliveries, uint32_t n_ext_sends) {
+  return demi_pow2_at_least(demi_fr_pool_entries(model, (int32_t)n_deliveries, n_ext_sends), 64u, 8192u);
+}
+
 #endif /* DEMI_LIMITS_H */

@@ -75,6 +75,17 @@ JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_internalMinimi
   return demi_internal_minimize(H(h), (uint32_t)lookingFor, (uint32_t)flags, (demi_event*)BUF(env, events), (uint32_t)capEvents,
                                 (uint32_t*)BUF(env, sizes), (uint32_t)capSizes, (demi_intmin_out*)BUF(env, out));
 }
+/* rules: nRules packed u32 (DEMI_CLOCK_RULE); incrementTypes: 8 u32 words, may be null */
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_setClockRules(JNIEnv* env, jclass c, jlong h, jobject rules,
+    jint nRules, jobject incrementTypes) {
+  return demi_set_clock_rules(H(h), rules ? (const uint32_t*)BUF(env, rules) : 0, (uint32_t)nRules,
+                              incrementTypes ? (const uint32_t*)BUF(env, incrementTypes) : 0);
+}
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_wildcardMinimize(JNIEnv* env, jclass c, jlong h, jint lookingFor,
+    jint flags, jobject events, jint capEvents, jobject sizes, jint capSizes, jobject out) {
+  return demi_wildcard_minimize(H(h), (uint32_t)lookingFor, (uint32_t)flags, (demi_event*)BUF(env, events), (uint32_t)capEvents,
+                                (uint32_t*)BUF(env, sizes), (uint32_t)capSizes, (demi_intmin_out*)BUF(env, out));
+}
 JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_dporBatch(JNIEnv* env, jclass c, jlong h, jobject ext, jobject extOffsets,
     jint nSearches, jobject params, jobject results, jobject viol, jint capViol) {
   return demi_dpor_batch(H(h), (const demi_ext_event*)BUF(env, ext), (const uint32_t*)BUF(env, extOffsets), (uint32_t)nSearches,

@@ -27,6 +27,9 @@ object DemiNative {
                           events: ByteBuffer, capEvents: Int, count: ByteBuffer, result: ByteBuffer): Int
   @native def internalMinimize(h: Long, lookingFor: Int, flags: Int, events: ByteBuffer, capEvents: Int, sizes: ByteBuffer,
                                capSizes: Int, out: ByteBuffer): Int
+  @native def setClockRules(h: Long, rules: ByteBuffer, nRules: Int, incrementTypes: ByteBuffer): Int
+  @native def wildcardMinimize(h: Long, lookingFor: Int, flags: Int, events: ByteBuffer, capEvents: Int, sizes: ByteBuffer,
+                               capSizes: Int, out: ByteBuffer): Int
   @native def dporBatch(h: Long, ext: ByteBuffer, extOffsets: ByteBuffer, nSearches: Int, params: ByteBuffer,
                         results: ByteBuffer, viol: ByteBuffer, capViol: Int): Int
   @native def dporBatchEx(h: Long, ext: ByteBuffer, extOffsets: ByteBuffer, nSearches: Int, params: ByteBuffer, flags: Int,

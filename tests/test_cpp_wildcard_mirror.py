@@ -1,0 +1,34 @@
+"""The C++ host mirror's WildcardMinimizer (include/demi_b200.hpp) compiles against the C ABI and runs the
+fungible-clock stage after DDMin and internal minimization."""
+import os
+import subprocess
+
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def build(native, out_dir):
+    """Compiles the test into `out_dir` (the repository tree may be read-only) and returns the executable's path."""
+    native.lib()
+    exe = os.path.join(str(out_dir), "wildcard_mirror_test")
+    subprocess.check_call(["g++", "-std=c++17", "-O1", "-I" + os.path.join(ROOT, "include"),
+                           os.path.join(ROOT, "tests", "cpp", "wildcard_mirror_test.cpp"), "-o", exe,
+                           "-L" + os.path.join(ROOT, "demi_b200"), "-ldemi_b200",
+                           "-Wl,-rpath," + os.path.join(ROOT, "demi_b200")])
+    return exe
+
+
+def test_cpp_wildcard_mirror_without_a_gpu(native, tmp_path):
+    exe = build(native, tmp_path)
+    if native.lib().demi_device_count() > 0:
+        pytest.skip("a CUDA device is present (covered by the gpu test)")
+    out = subprocess.run([exe], capture_output=True, text=True, timeout=120)
+    assert out.returncode == 0 and "no-fallback contract" in out.stdout, out.stdout + out.stderr
+
+
+@pytest.mark.gpu
+def test_cpp_wildcard_mirror_on_gpu(native, tmp_path):
+    exe = build(native, tmp_path)
+    out = subprocess.run([exe], capture_output=True, text=True, timeout=600)
+    assert out.returncode == 0 and out.stdout.strip().endswith("OK"), out.stdout + out.stderr
