@@ -121,6 +121,7 @@ EXPORTS = [
     "demi_create_multi", "demi_conjoin_atoms", "demi_fuzzer_generate", "demi_experiment_save", "demi_experiment_load",
     "demi_load_model", "demi_actor_index", "demi_actor_name", "demi_set_user_filter",
     "demi_set_clock_rules", "demi_wildcard_replay_batch", "demi_wildcard_replay_trace", "demi_wildcard_minimize",
+    "demi_set_fuzzer", "demi_fuzz_campaign", "demi_fuzz_campaign_dev",
 ]
 FILTER_RULE_DTYPE = np.dtype([("src_mask", "<u4"), ("dst_mask", "<u4"), ("type_mask", "<u4"), ("flags", "<u4")])
 FRULE_DEADLETTERS = 1
@@ -130,6 +131,22 @@ MODEL_IR = 100
 class FuzzerConfig(C.Structure):
     _fields_ = [("kill", C.c_double), ("send", C.c_double), ("wait_quiescence", C.c_double), ("partition", C.c_double),
                 ("unpartition", C.c_double), ("num_events", C.c_uint32), ("send_type", C.c_uint32)]
+
+
+FUZZER_MAX_EVENTS = 4096
+
+
+def fuzzer_generate(cfg, seed, prefix, postfix=None):
+    """demi_fuzzer_generate: the program a campaign's execution with program seed `seed` runs (EXT_DTYPE array)."""
+    pre = np.ascontiguousarray(prefix, dtype=EXT_DTYPE)
+    post = np.ascontiguousarray(postfix if postfix is not None else np.zeros(0, dtype=EXT_DTYPE), dtype=EXT_DTYPE)
+    out = np.zeros(len(pre) + cfg.num_events + len(post) + 1, dtype=EXT_DTYPE)
+    n = C.c_uint32()
+    rc = lib().demi_fuzzer_generate(C.byref(cfg), seed, pre.ctypes.data if len(pre) else None, len(pre),
+                                    post.ctypes.data if len(post) else None, len(post), out.ctypes.data, len(out), C.byref(n))
+    if rc != OK:
+        raise RuntimeError("demi_fuzzer_generate: %s" % lib().demi_last_error(None).decode())
+    return out[:n.value].copy()
 
 
 class Experiment(C.Structure):
@@ -264,6 +281,12 @@ def lib():
                                              vp, C.c_uint32, C.POINTER(C.c_uint32), vp]
     L.demi_wildcard_minimize.restype = C.c_int32
     L.demi_wildcard_minimize.argtypes = [vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(IntMinOut)]
+    L.demi_set_fuzzer.restype = C.c_int32
+    L.demi_set_fuzzer.argtypes = [vp, C.POINTER(FuzzerConfig), vp, C.c_uint32, vp, C.c_uint32]
+    L.demi_fuzz_campaign.restype = C.c_int32
+    L.demi_fuzz_campaign.argtypes = [vp, C.POINTER(FuzzParams), C.c_int64, vp]
+    L.demi_fuzz_campaign_dev.restype = C.c_int32
+    L.demi_fuzz_campaign_dev.argtypes = [vp, C.POINTER(FuzzParams), C.c_int64, vp, vp]
     L.demi_stats.restype = C.c_int32
     L.demi_stats.argtypes = [vp, C.POINTER(Perf)]
     _lib = L

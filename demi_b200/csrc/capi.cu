@@ -1,6 +1,7 @@
 // capi.cu — the C ABI (include/demi_b200.h) over the CUDA engine.
 // No CPU fallback: every compute entry point needs a CUDA device.
 #include <climits>
+#include <cmath>
 #include <cstdlib>
 #include <cstdio>
 #include <cstdarg>
@@ -13,6 +14,7 @@
 #include "provenance_kernel.cuh"
 #include "lane_kernel.cuh"
 #include "models/model_ir.cuh"
+#include "fuzzer_gen.cuh"
 
 using namespace demi;
 
@@ -26,12 +28,14 @@ typedef void (*kernel_fn)(const KernelArgs);
 struct Variant {
   int model; uint32_t pcap, tcap; bool pend_global, record;
   kernel_fn fn; size_t smem_per_warp;
+  kernel_fn fn_prog;             // the campaign instantiation (PROG); none for the recording variants
 };
 template <class MODEL, int PCAP, int TCAP, bool PG, bool REC>
 static Variant make_variant() {
   using M = Machine<MODEL, PCAP, TCAP, PG, REC>;
   return Variant{MODEL::ID, (uint32_t)PCAP, (uint32_t)TCAP, PG, REC,
-                 fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS>, sizeof(typename M::Smem)};
+                 fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS>, sizeof(typename M::Smem),
+                 REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC>};
 }
 static const std::vector<Variant>& variants() {
   static const std::vector<Variant> v = {
@@ -59,14 +63,14 @@ static const Variant* pick_variant(int model, uint32_t pcap, uint32_t tcap, bool
 }
 
 // lane-engine table
-struct LaneVariant { int model; int bd; uint32_t lpcap; kernel_fn fn; kernel_fn fn_rec; size_t smem_per_block; };
+struct LaneVariant { int model; int bd; uint32_t lpcap; kernel_fn fn; kernel_fn fn_rec; size_t smem_per_block; kernel_fn fn_prog; };
 template <class MODEL, int BD, int LPCAP>
 static LaneVariant make_lane_variant() {
   using M = LaneMachine<MODEL, BD, LPCAP>;
   return LaneVariant{MODEL::ID, BD, (uint32_t)LPCAP, fuzz_lane_kernel<MODEL, BD, LPCAP>, fuzz_lane_kernel<MODEL, BD, LPCAP, true>,
-                     (size_t)M::WORDS * BD * sizeof(uint32_t)};
+                     (size_t)M::WORDS * BD * sizeof(uint32_t), fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>};
 }
-static const LaneVariant* pick_lane_variant(const demi_handle* h);
+static const LaneVariant* pick_lane_variant(const demi_handle* h, bool campaign = false);
 
 // ---------------------------------------------------------------- lifecycle
 #ifndef DEMI_BUILD_ID
@@ -132,6 +136,7 @@ extern "C" void demi_destroy(demi_handle* h) {
   demi_frontier_free(h);
   demi_comm_free(h);
   cudaFree(h->ir_blob_dev); cudaFree(h->trace_rec);
+  cudaFree(h->fz_fixed_dev); cudaFree(h->fz_arena);
   cudaFree(h->dedup.keys); cudaFree(h->dedup.vals); cudaFree(h->dedup.keep); cudaFree(h->dedup.counts);
   if (h->pinned) cudaFreeHost(h->pinned);
   if (h->ev0) cudaEventDestroy(h->ev0);
@@ -252,7 +257,8 @@ extern "C" int32_t demi_set_user_filter(demi_handle* h, const demi_filter_rule* 
   return DEMI_OK;
 }
 
-static const LaneVariant* pick_lane_variant(const demi_handle* h) {
+// campaign: the same conditions, over the handle's Fuzzer (demi_set_fuzzer) instead of its program
+static const LaneVariant* pick_lane_variant(const demi_handle* h, bool campaign) {
   static const std::vector<LaneVariant> v = {
 #ifndef DEMI_K1_BD_RAFT5
 #define DEMI_K1_BD_RAFT5 256
@@ -261,8 +267,10 @@ static const LaneVariant* pick_lane_variant(const demi_handle* h) {
     make_lane_variant<PingPong3, 256, 128>(),
     make_lane_variant<Bcast32, 128, 8192>(),
   };
-  if (!h->use_lane_engine || h->cfg.blocked_mask || !h->ext_sends_distinct || h->cfg.strategy != DEMI_RS_FULLY_RANDOM ||
-      h->has_hard_kill || !h->filter.empty()) return nullptr;          // actor termination and user filters: the general engine
+  const bool distinct = campaign ? h->fz_sends_distinct : h->ext_sends_distinct;
+  const bool hard_kill = campaign ? h->fz_has_hard_kill : h->has_hard_kill;
+  if (!h->use_lane_engine || h->cfg.blocked_mask || !distinct || h->cfg.strategy != DEMI_RS_FULLY_RANDOM ||
+      hard_kill || !h->filter.empty()) return nullptr;          // actor termination and user filters: the general engine
   for (const LaneVariant& lv : v) if (lv.model == h->cfg.model) return &lv;
   return nullptr;
 }
@@ -278,25 +286,29 @@ static int32_t ensure(demi_handle* h, void** p, size_t* cap, size_t need) {
   return DEMI_OK;
 }
 
-static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool record, LaunchPlan* plan) {
+// campaign: sized for the Fuzzer's largest program (fz_max_sends Sends); ext / n_ext are bound per execution
+static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool record, LaunchPlan* plan, bool campaign = false) {
   if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
-  if (h->ext_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
+  if (campaign && !h->has_fuzzer) return fail(h, DEMI_ERR_STATE, "demi_set_fuzzer has not been called");
+  if (!campaign && h->ext_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
   if (p->n_prefixes > 0xFFFFFFFFull) return fail(h, DEMI_ERR_INVALID, "n_prefixes > 2^32-1 per call");
   { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
-  const uint32_t pcap = demi_pending_cap(demi_model_key(h), p->max_messages, h->n_ext_sends);
-  const uint32_t tcap = demi_tosend_cap(h->n_ext_sends);
+  const uint32_t n_sends = campaign ? h->fz_max_sends : h->n_ext_sends;
+  const uint32_t pcap = demi_pending_cap(demi_model_key(h), p->max_messages, n_sends);
+  const uint32_t tcap = demi_tosend_cap(n_sends);
   const bool fifo = h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;          // SrcDstFIFO lives in the HBM-pending variants
   const Variant* v = pick_variant(h->cfg.model, pcap, tcap, record, fifo);
   if (!v) return fail(h, DEMI_ERR_CAPACITY, "no kernel variant for pending_cap=%u tosend_cap=%u", pcap, tcap);
+  const kernel_fn fn = campaign ? v->fn_prog : v->fn;
   const size_t smem = v->smem_per_warp * WARPS;
   // the attribute and the occupancy of a variant are fixed per device: asked once, not on every launch
   int blocks_per_sm = 0;
   {
-    auto it = h->occupancy.find((const void*)v->fn);
+    auto it = h->occupancy.find((const void*)fn);
     if (it == h->occupancy.end()) {
-      CUDA_TRY(h, cudaFuncSetAttribute(v->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, v->fn, WARPS * 32, smem));
-      h->occupancy[(const void*)v->fn] = blocks_per_sm;
+      CUDA_TRY(h, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, fn, WARPS * 32, smem));
+      h->occupancy[(const void*)fn] = blocks_per_sm;
     } else blocks_per_sm = it->second;
   }
   if (blocks_per_sm < 1) return fail(h, DEMI_ERR_CAPACITY, "kernel variant does not fit on an SM (smem %zu)", smem);
@@ -329,12 +341,12 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool recor
                      total_warps * (uint64_t)(v->pcap / 2 + 3 * FIFO_PAIRS) * sizeof(uint16_t))) != DEMI_OK) return rc;
     a.fifo_scratch = h->fifo_scratch;
   }
-  if (fifo && (h->has_hard_kill || !h->filter.empty()))
+  if (fifo && ((campaign ? h->fz_has_hard_kill : h->has_hard_kill) || !h->filter.empty()))
     return fail(h, DEMI_ERR_INVALID, "HardKill and userDefinedFilter are offered for FullyRandom only");
   a.n_filter = (uint32_t)h->filter.size();
   for (uint32_t i = 0; i < a.n_filter; i++) a.filter[i] = make_uint4(h->filter[i].src_mask, h->filter[i].dst_mask, h->filter[i].type_mask, h->filter[i].flags);
-  a.ext = h->ext_dev;
-  a.n_ext = (uint32_t)h->ext_host.size();
+  a.ext = campaign ? nullptr : h->ext_dev;
+  a.n_ext = campaign ? 0u : (uint32_t)h->ext_host.size();
   a.node_cap = node_cap;
   a.pending_cap = pcap;
   a.tosend_cap = tcap;
@@ -353,7 +365,8 @@ extern "C" int32_t demi_fuzz_batch_dev(demi_handle* h, const demi_fuzz_params* p
 }
 
 // One launch of the lane engine over `n_items` work items; what it defers is appended to h->ovf_list / h->ovf_count.
-static int32_t launch_lane(demi_handle* h, const LaneVariant* lv, kernel_fn lfn, const KernelArgs& base, uint64_t n_items, cudaStream_t s) {
+static int32_t launch_lane(demi_handle* h, const LaneVariant* lv, kernel_fn lfn, const KernelArgs& base, uint64_t n_items, cudaStream_t s,
+                           bool campaign = false) {
   const size_t lsmem = lv->smem_per_block;
   int bps = 0;
   {
@@ -374,8 +387,9 @@ static int32_t launch_lane(demi_handle* h, const LaneVariant* lv, kernel_fn lfn,
   CUDA_TRY(h, cudaMemsetAsync(h->ovf_count, 0, sizeof(uint32_t), s));
   KernelArgs la = base;
   la.lane_pend = h->lane_pend;
-  la.ext_sends = h->ext_sends_dev;
-  la.has_partitions = h->has_partitions ? 1u : 0u;
+  la.ext_sends = campaign ? nullptr : h->ext_sends_dev;           // a campaign binds each program's table
+  la.has_partitions = (campaign ? h->fz_has_partitions : h->has_partitions) ? 1u : 0u;
+  la.prog_lane_pcap = h->lane_pending_cap;
   la.ovf_list = h->ovf_list; la.ovf_count = h->ovf_count;
   if (h->lane_pending_cap) la.pending_cap = std::min(la.pending_cap, h->lane_pending_cap);     // deferring is always exact
   lfn<<<lgrid, lv->bd, lsmem, s>>>(la);
@@ -415,28 +429,19 @@ static int32_t launch_fuzz(demi_handle* h, const demi_fuzz_params* p, void* out_
   return DEMI_OK;
 }
 
-extern "C" int32_t demi_fuzz_batch(demi_handle* h, const demi_fuzz_params* p, demi_fuzz_result* out_host) {
-  if (!h) return DEMI_ERR_INVALID;
-  if (!out_host) return fail(h, DEMI_ERR_INVALID, "demi_fuzz_batch: null output");
-  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
-  const size_t bytes = (size_t)p->n_prefixes * sizeof(demi_fuzz_result);
+// Runs n records in chunks of `per` through launch(off, m, dst, first_chunk) on h->stream; chunk i's records travel to
+// the host on the copy stream while chunk i+1 is being explored.  Fills demi_perf (kernel_ms spans every launch).
+template <class Launch>
+static int32_t run_pipelined(demi_handle* h, const char* who, uint64_t n, uint64_t per, demi_fuzz_result* out_host, Launch launch) {
+  const size_t bytes = (size_t)n * sizeof(demi_fuzz_result);
   int32_t rc = ensure(h, (void**)&h->results_dev, &h->results_cap, std::max<size_t>(bytes, 32));
   if (rc != DEMI_OK) return rc;
-  // Pipeline: the batch is cut into chunks; chunk i's records travel to the host on the copy
-  // stream while chunk i+1 is being explored.
-  const uint64_t CHUNK = 2u << 20;
-  const uint64_t n = p->n_prefixes;
-  const uint64_t n_chunks = n <= 2 * CHUNK ? 1 : (n + CHUNK - 1) / CHUNK;
-  const uint64_t per = n_chunks ? (n + n_chunks - 1) / n_chunks : 0;
   CUDA_TRY(h, cudaEventRecord(h->ev0, h->stream));
-  if (n == 0) { rc = launch_fuzz(h, p, h->results_dev, h->stream, true); if (rc != DEMI_OK) return rc; }
+  if (n == 0) { rc = launch(0, 0, h->results_dev, true); if (rc != DEMI_OK) return rc; }
   std::vector<cudaEvent_t> evs;
-  for (uint64_t c = 0, off = 0; off < n; c++, off += per) {
-    demi_fuzz_params q = *p;
-    q.seed_base = p->seed_base + (int64_t)off;
-    q.n_prefixes = std::min<uint64_t>(per, n - off);
-    rc = launch_fuzz(h, &q, h->results_dev + off, h->stream, c == 0);
+  for (uint64_t off = 0; off < n; off += per) {
+    const uint64_t m = std::min<uint64_t>(per, n - off);
+    rc = launch(off, m, h->results_dev + off, off == 0);
     if (rc != DEMI_OK) break;
     cudaEvent_t ev;
     cudaError_t ce = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
@@ -444,10 +449,10 @@ extern "C" int32_t demi_fuzz_batch(demi_handle* h, const demi_fuzz_params* p, de
       evs.push_back(ev);
       ce = cudaEventRecord(ev, h->stream);
       if (ce == cudaSuccess) ce = cudaStreamWaitEvent(h->copy_stream, ev, 0);
-      if (ce == cudaSuccess) ce = cudaMemcpyAsync(out_host + off, h->results_dev + off, q.n_prefixes * sizeof(demi_fuzz_result),
+      if (ce == cudaSuccess) ce = cudaMemcpyAsync(out_host + off, h->results_dev + off, m * sizeof(demi_fuzz_result),
                                                   cudaMemcpyDeviceToHost, h->copy_stream);
     }
-    if (ce != cudaSuccess) { rc = fail(h, DEMI_ERR_CUDA, "demi_fuzz_batch: %s", cudaGetErrorString(ce)); break; }   // events freed below
+    if (ce != cudaSuccess) { rc = fail(h, DEMI_ERR_CUDA, "%s: %s", who, cudaGetErrorString(ce)); break; }   // events freed below
   }
   cudaError_t e = cudaEventRecord(h->ev1, h->stream);
   unsigned long long cnt[3] = {0, 0, 0};
@@ -456,7 +461,7 @@ extern "C" int32_t demi_fuzz_batch(demi_handle* h, const demi_fuzz_params* p, de
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->copy_stream);
   for (cudaEvent_t ev : evs) cudaEventDestroy(ev);
   if (rc != DEMI_OK) return rc;
-  if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "demi_fuzz_batch: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "%s: %s", who, cudaGetErrorString(e));
   float ms = 0;
   CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
   h->perf.kernel_ms = ms;
@@ -466,6 +471,23 @@ extern "C" int32_t demi_fuzz_batch(demi_handle* h, const demi_fuzz_params* p, de
   h->perf.d2h_bytes = bytes + sizeof(cnt);
   h->perf.h2d_bytes = 0;
   return DEMI_OK;
+}
+
+extern "C" int32_t demi_fuzz_batch(demi_handle* h, const demi_fuzz_params* p, demi_fuzz_result* out_host) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!out_host) return fail(h, DEMI_ERR_INVALID, "demi_fuzz_batch: null output");
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
+  const uint64_t CHUNK = 2u << 20;
+  const uint64_t n = p->n_prefixes;
+  const uint64_t n_chunks = n <= 2 * CHUNK ? 1 : (n + CHUNK - 1) / CHUNK;
+  const uint64_t per = n_chunks ? (n + n_chunks - 1) / n_chunks : 0;
+  return run_pipelined(h, "demi_fuzz_batch", n, per, out_host, [&](uint64_t off, uint64_t m, demi_fuzz_result* dst, bool first) {
+    demi_fuzz_params q = *p;
+    q.seed_base = p->seed_base + (int64_t)off;
+    q.n_prefixes = m;
+    return launch_fuzz(h, &q, dst, h->stream, first);
+  });
 }
 
 // Counts from the last *_dev batch launched on `stream` (waits for it).
@@ -674,6 +696,213 @@ extern "C" int32_t demi_fuzz_provenance(demi_handle* h, const demi_fuzz_params* 
   if (rc != DEMI_OK) return rc;
   if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "demi_fuzz_provenance: %s", cudaGetErrorString(e));
   return DEMI_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Campaigns: RunnerUtils.fuzz's loop (RunnerUtils.scala:75-91) with a fresh Fuzzer program per execution.
+// Execution i runs program fuzzer_generate(program_seed_base + i) under FullyRandom(seed_base + i).
+
+// the message-type ids a model defines (send_type must be one of them)
+static uint32_t model_type_count(const demi_handle* h) {
+  switch (h->cfg.model) {
+    case DEMI_MODEL_PINGPONG3: return 3;
+    case DEMI_MODEL_RAFT5: return 9;
+    case DEMI_MODEL_BCAST32: return 3;
+    default: return h->ir_n_types;
+  }
+}
+
+// new Fuzzer(num_events, weights, message_gen, prefix, postfix) (Fuzzer.scala:61-82): checked once here for what
+// would make one of its programs fail demi_set_externals, so that every generated program is a valid one.
+extern "C" int32_t demi_set_fuzzer(demi_handle* h, const demi_fuzzer_config* cfg, const demi_ext_event* prefix, uint32_t n_prefix,
+                                   const demi_ext_event* postfix, uint32_t n_postfix) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!cfg || (!prefix && n_prefix) || (!postfix && n_postfix)) return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: null argument");
+  { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
+  const int na = demi_model_actors(h);
+  uint32_t starts = 0, sends = 0;
+  bool hard_kill = false, partitions = false, distinct = true;
+  std::vector<uint4> sv;
+  for (int part = 0; part < 2; part++) {
+    const demi_ext_event* ev = part ? postfix : prefix;
+    const uint32_t n = part ? n_postfix : n_prefix;
+    const char* where = part ? "postfix" : "prefix";
+    for (uint32_t i = 0; i < n; i++) {
+      const demi_ext_event& e = ev[i];
+      if (e.kind < DEMI_EXT_START || e.kind > DEMI_EXT_HARD_KILL)
+        return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: %s event %u has unknown kind %u", where, i, e.kind);
+      const bool needs_a = e.kind != DEMI_EXT_WAIT_QUIESCENCE;
+      const bool needs_b = e.kind == DEMI_EXT_PARTITION || e.kind == DEMI_EXT_UNPARTITION;
+      if ((needs_a && e.a >= na) || (needs_b && e.b >= na))
+        return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: %s event %u names an unknown actor", where, i);
+      if (e.kind == DEMI_EXT_WAIT_QUIESCENCE && i > 0 && ev[i - 1].kind == DEMI_EXT_WAIT_QUIESCENCE)
+        return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: consecutive WaitQuiescence at %s event %u", where, i);
+      if (!part && e.kind == DEMI_EXT_START) starts++;
+      if (e.kind == DEMI_EXT_HARD_KILL) hard_kill = true;
+      if (needs_b) partitions = true;
+      if (e.kind != DEMI_EXT_SEND) continue;
+      sends++;
+      // the lane engine's screen (demi_set_externals): no two Sends of a program may be equal.  A generated Send is
+      // (alive actor, send_type, p0 = counter in 1..num_events, p1 = 0); a fixed Send that could equal one screens
+      // the campaign out, whichever actor the generated one picks.
+      const uint4 m = make_uint4((uint32_t)e.a | ((uint32_t)e.type << 8), e.p0, e.p1, 0u);
+      for (const uint4& o : sv) if (o.x == m.x && o.y == m.y && o.z == m.z) distinct = false;
+      if (cfg->send > 0.0 && e.type == cfg->send_type && e.p1 == 0 && e.p0 >= 1 && e.p0 <= cfg->num_events) distinct = false;
+      sv.push_back(m);
+    }
+  }
+  if (!starts) return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: the prefix has no Start (the Fuzzer's actors are the prefix's Starts, Fuzzer.scala:60)");
+  if (starts > DEMI_MAX_ACTORS) return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: %u Starts in the prefix, at most %d", starts, DEMI_MAX_ACTORS);
+  if (n_postfix && postfix[0].kind == DEMI_EXT_WAIT_QUIESCENCE)
+    return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: the postfix begins with WaitQuiescence (it may follow a generated one)");
+  if (cfg->send_type >= model_type_count(h))
+    return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: send_type %u is not a message type of the model", cfg->send_type);
+  const double w[5] = {cfg->kill, cfg->send, cfg->wait_quiescence, cfg->partition, cfg->unpartition};
+  double total = 0.0;
+  for (double x : w) {
+    if (!std::isfinite(x) || x < 0.0) return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: weights must be finite and >= 0");
+    total += x;
+  }
+  if (!(total > 0.0)) return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: the weights add up to 0");
+  if (cfg->num_events > DEMI_FUZZER_MAX_EVENTS)
+    return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: num_events %u, at most %d", cfg->num_events, DEMI_FUZZER_MAX_EVENTS);
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  cudaFree(h->fz_fixed_dev); h->fz_fixed_dev = nullptr; h->has_fuzzer = false;
+  if (n_prefix + n_postfix) {
+    CUDA_TRY(h, cudaMalloc(&h->fz_fixed_dev, (size_t)(n_prefix + n_postfix) * sizeof(demi_ext_event)));
+    CUDA_TRY(h, cudaMemcpy(h->fz_fixed_dev, prefix, (size_t)n_prefix * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
+    if (n_postfix)
+      CUDA_TRY(h, cudaMemcpy(h->fz_fixed_dev + n_prefix, postfix, (size_t)n_postfix * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
+  }
+  h->fuzzer = *cfg; h->fz_n_prefix = n_prefix; h->fz_n_postfix = n_postfix;
+  h->fz_max_sends = sends + cfg->num_events;
+  h->fz_has_hard_kill = hard_kill;
+  h->fz_has_partitions = partitions || cfg->partition > 0.0;
+  h->fz_sends_distinct = distinct;
+  h->has_fuzzer = true;
+  return DEMI_OK;
+}
+
+// One thread per program: program i of the chunk goes to events[i * stride ..), its {length, Sends} to hdr[i] and its
+// Sends, in the lane engine's form, to sends[i * send_stride ..).  The three sets live in local memory.
+__global__ void __launch_bounds__(128)
+fuzzer_gen_kernel(const demi_fuzzer_config cfg, int64_t seed_base, uint64_t n, const demi_ext_event* fixed, uint32_t n_prefix,
+                  uint32_t n_postfix, demi_ext_event* events, uint32_t stride, uint2* hdr, uint4* sends, uint32_t send_stride) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint8_t alive[DEMI_MAX_ACTORS];
+  uint16_t pairs[2 * (DEMI_MAX_ACTORS * (DEMI_MAX_ACTORS - 1) / 2)];
+  demi_ext_event* out = events + i * stride;
+  uint32_t n_sends = 0;
+  const uint32_t len = demi::fuzzer_generate(cfg, seed_base + (int64_t)i, fixed, n_prefix, fixed + n_prefix, n_postfix, alive, pairs,
+                                             out, &n_sends);
+  hdr[i] = make_uint2(len, n_sends);
+  uint4* st = sends + i * send_stride;
+  for (uint32_t j = 0, k = 0; j < len; j++) {
+    const demi_ext_event e = out[j];
+    if (e.kind == DEMI_EXT_SEND)
+      st[k++] = make_uint4(DEMI_DEADLETTERS | ((uint32_t)e.a << 8) | ((uint32_t)e.type << 16) | ((uint32_t)DEMI_MF_EXTERNAL << 24), e.p0, e.p1, 0u);
+  }
+}
+
+// programs per launch: the arena of one chunk stays under 512 MB
+static uint64_t campaign_chunk(const demi_handle* h, uint32_t* stride, uint32_t* send_stride) {
+  *stride = (uint32_t)demi::fuzzer_program_room(h->fuzzer, h->fz_n_prefix, h->fz_n_postfix);
+  *send_stride = std::max(h->fz_max_sends, 1u);
+  const uint64_t per = (uint64_t)*stride * sizeof(demi_ext_event) + sizeof(uint2) + (uint64_t)*send_stride * sizeof(uint4);
+  return std::max<uint64_t>(1, std::min<uint64_t>(2u << 20, ((uint64_t)512 << 20) / per));
+}
+
+// One chunk (n_prefixes <= campaign_chunk): generate its programs, then the lane engine, then the warp engine on what
+// the lane engine deferred (or on all of them).
+static int32_t launch_campaign(demi_handle* h, const demi_fuzz_params* p, int64_t program_seed_base, void* out_dev, cudaStream_t s,
+                               bool reset_counters) {
+  LaunchPlan plan;
+  int32_t rc = plan_launch(h, p, false, &plan, true);
+  if (rc != DEMI_OK) return rc;
+  const uint64_t n = p->n_prefixes;
+  if (n == 0) return DEMI_OK;
+  uint32_t stride, send_stride;
+  campaign_chunk(h, &stride, &send_stride);
+  const size_t b_ev = (size_t)n * stride * sizeof(demi_ext_event), b_hdr = ((size_t)n * sizeof(uint2) + 15) & ~(size_t)15;
+  if ((rc = ensure(h, &h->fz_arena, &h->fz_arena_bytes, b_ev + b_hdr + (size_t)n * send_stride * sizeof(uint4))) != DEMI_OK) return rc;
+  demi_ext_event* ev = (demi_ext_event*)h->fz_arena;
+  uint2* hdr = (uint2*)((unsigned char*)h->fz_arena + b_ev);
+  uint4* sends = (uint4*)((unsigned char*)h->fz_arena + b_ev + b_hdr);
+  if (reset_counters) {
+    CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
+    h->perf.kernel_launches = 0;
+    h->perf.prefixes = 0;
+  }
+  fuzzer_gen_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(h->fuzzer, program_seed_base, n, h->fz_fixed_dev, h->fz_n_prefix,
+                                                                 h->fz_n_postfix, ev, stride, hdr, sends, send_stride);
+  CUDA_TRY(h, cudaGetLastError());
+  h->perf.kernel_launches++;
+  KernelArgs& a = plan.args;
+  a.results = (demi_fuzz_result*)out_dev;
+  a.prog_ext = ev; a.prog_hdr = hdr; a.prog_sends = sends;
+  a.prog_stride = stride; a.prog_send_stride = send_stride;
+  a.prog_model_key = demi_model_key(h);
+  a.prog_max_messages = p->max_messages;
+  if (const LaneVariant* lv = pick_lane_variant(h, true)) {
+    if ((rc = launch_lane(h, lv, lv->fn_prog, a, n, s, true)) != DEMI_OK) return rc;
+    a.index_list = h->ovf_list;
+    a.index_count = h->ovf_count;
+  }
+  if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
+  plan.v->fn_prog<<<plan.grid, WARPS * 32, plan.smem, s>>>(a);
+  CUDA_TRY(h, cudaGetLastError());
+  h->perf.kernel_launches++;
+  h->perf.prefixes += n;
+  return DEMI_OK;
+}
+
+// What the campaign entry points need before the first chunk: campaign_chunk reads the Fuzzer, and the call-wide
+// n_prefixes limit of demi_fuzz_batch_dev (plan_launch only sees one chunk here).
+static int32_t check_campaign(demi_handle* h, const demi_fuzz_params* p) {
+  if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
+  if (!h->has_fuzzer) return fail(h, DEMI_ERR_STATE, "demi_set_fuzzer has not been called");
+  if (p->n_prefixes > 0xFFFFFFFFull) return fail(h, DEMI_ERR_INVALID, "n_prefixes > 2^32-1 per call");
+  return DEMI_OK;
+}
+
+// RunnerUtils.fuzz's loop (RunnerUtils.scala:75-91): `fuzzer.generateFuzzTest()` then `RandomScheduler.explore`, once
+// per execution, with results left in HBM.  No sync; demi_fuzz_summary_dev reads the counts.
+extern "C" int32_t demi_fuzz_campaign_dev(demi_handle* h, const demi_fuzz_params* p, int64_t program_seed_base, void* out_dev,
+                                          void* stream) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!out_dev) return fail(h, DEMI_ERR_INVALID, "demi_fuzz_campaign_dev: null output");
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  int32_t rc = check_campaign(h, p);
+  if (rc != DEMI_OK) return rc;
+  uint32_t stride, send_stride;
+  const uint64_t chunk = campaign_chunk(h, &stride, &send_stride), n = p->n_prefixes;
+  if (n == 0) return launch_campaign(h, p, program_seed_base, out_dev, (cudaStream_t)stream, true);
+  for (uint64_t off = 0; off < n; off += chunk) {
+    demi_fuzz_params q = *p;
+    q.seed_base = p->seed_base + (int64_t)off;
+    q.n_prefixes = std::min(chunk, n - off);
+    rc = launch_campaign(h, &q, program_seed_base + (int64_t)off, (demi_fuzz_result*)out_dev + off, (cudaStream_t)stream, off == 0);
+    if (rc != DEMI_OK) return rc;
+  }
+  return DEMI_OK;
+}
+
+// Same, records to the host, pipelined as demi_fuzz_batch.
+extern "C" int32_t demi_fuzz_campaign(demi_handle* h, const demi_fuzz_params* p, int64_t program_seed_base, demi_fuzz_result* out_host) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!out_host) return fail(h, DEMI_ERR_INVALID, "demi_fuzz_campaign: null output");
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  int32_t rc = check_campaign(h, p);
+  if (rc != DEMI_OK) return rc;
+  uint32_t stride, send_stride;
+  const uint64_t chunk = campaign_chunk(h, &stride, &send_stride);
+  return run_pipelined(h, "demi_fuzz_campaign", p->n_prefixes, chunk, out_host, [&](uint64_t off, uint64_t m, demi_fuzz_result* dst, bool first) {
+    demi_fuzz_params q = *p;
+    q.seed_base = p->seed_base + (int64_t)off;
+    q.n_prefixes = m;
+    return launch_campaign(h, &q, program_seed_base + (int64_t)off, dst, h->stream, first);
+  });
 }
 
 extern "C" int32_t demi_stats(const demi_handle* h, demi_perf* out) {

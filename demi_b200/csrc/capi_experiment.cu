@@ -7,91 +7,26 @@
 #include <vector>
 #include <sys/stat.h>
 #include "engine.hpp"
+#include "fuzzer_gen.cuh"
 
-namespace {
-// java.util.Random (Java SE specification); scala.util.Random delegates to it (Fuzzer.scala:68)
-struct JavaRandom {
-  uint64_t s;
-  explicit JavaRandom(int64_t seed) : s(((uint64_t)seed ^ 0x5DEECE66Dull) & ((1ull << 48) - 1)) {}
-  int32_t next(int bits) { s = (s * 0x5DEECE66Dull + 0xBull) & ((1ull << 48) - 1); return (int32_t)(int64_t)(s >> (48 - bits)); }
-  int32_t nextInt(int32_t bound) {
-    int32_t r = next(31), m = bound - 1;
-    if ((bound & m) == 0) return (int32_t)(((int64_t)bound * (int64_t)r) >> 31);
-    for (int32_t u = r; u - (r = u % bound) + m < 0; u = next(31)) {}
-    return r;
-  }
-  double nextDouble() { return (double)(((int64_t)next(26) << 27) + next(27)) * (1.0 / (double)(1ll << 53)); }
-};
-// RandomizedHashSet (schedulers/Util.scala:110-185) over small integer payloads
-struct RandSet {
-  std::vector<uint32_t> arr; JavaRandom rand;
-  explicit RandSet(int64_t seed) : rand(seed) {}
-  void insert(uint32_t v) { arr.push_back(v); }
-  bool empty() const { return arr.empty(); }
-  uint32_t removeRandomElement() { const int32_t i = rand.nextInt((int32_t)arr.size()); const uint32_t v = arr[i]; arr[i] = arr.back(); arr.pop_back(); return v; }
-  uint32_t getRandomElement() { return arr[rand.nextInt((int32_t)arr.size())]; }
-};
-}  // namespace
-
-// Fuzzer.generateFuzzTest (Fuzzer.scala:123-174) with generateNextEvent (:84-121), FuzzerWeights (:24-58) and reset
-// (:176-193).  The reference seeds the fuzzer and its three sets from the wall clock; all four take `seed` here.
+// Fuzzer.generateFuzzTest (Fuzzer.scala:123-174): the body is fuzzer_gen.cuh, shared with the campaign's generator kernel.
 extern "C" int32_t demi_fuzzer_generate(const demi_fuzzer_config* cfg, int64_t seed,
                                         const demi_ext_event* prefix, uint32_t n_prefix,
                                         const demi_ext_event* postfix, uint32_t n_postfix,
                                         demi_ext_event* out, uint32_t cap, uint32_t* n_out) {
   if (!cfg || !out || !n_out || (!prefix && n_prefix) || (!postfix && n_postfix))
     return fail(nullptr, DEMI_ERR_INVALID, "demi_fuzzer_generate: null argument");
-  const double weights[4] = {cfg->kill, cfg->send, cfg->partition, cfg->unpartition};     // allWeights, in this order (:40)
-  const double total = cfg->kill + cfg->send + cfg->partition + cfg->unpartition + cfg->wait_quiescence;
-  std::vector<uint32_t> nodes;
-  uint32_t next_id = 0;
-  for (uint32_t i = 0; i < n_prefix; i++) { if (prefix[i].kind == DEMI_EXT_START) nodes.push_back(prefix[i].a); next_id = std::max(next_id, prefix[i].id); }
-  for (uint32_t i = 0; i < n_postfix; i++) next_id = std::max(next_id, postfix[i].id);
-  JavaRandom rand(seed);
-  RandSet alive(seed), partitioned(seed), unpartitioned(seed);
-  for (uint32_t n : nodes) alive.insert(n);
-  for (size_t i = 0; i < nodes.size(); i++) for (size_t j = i + 1; j < nodes.size(); j++) unpartitioned.insert(nodes[i] | (nodes[j] << 8));
-  std::vector<demi_ext_event> test(prefix, prefix + n_prefix);
-  uint32_t counter = 0;
-  auto mk = [&](uint8_t kind, uint32_t a, uint32_t b, uint32_t type, uint32_t p0) {
-    demi_ext_event e{}; e.kind = kind; e.a = (uint8_t)a; e.b = (uint8_t)b; e.type = (uint8_t)type; e.p0 = p0; e.id = ++next_id; return e;
-  };
-  // returns false for "no more events" (Kill with nobody alive, :92-95)
-  auto next_event = [&](demi_ext_event& ev) -> bool {
-    for (;;) {
-      const double scaled = rand.nextDouble() * total;
-      int t = -1; double cur = 0.0;
-      for (int k = 0; k < 4; k++) { cur += weights[k]; if (scaled < cur) { t = k; break; } }
-      if (t < 0) { ev = mk(DEMI_EXT_WAIT_QUIESCENCE, 0, 0, 0, 0); return true; }
-      if (t == 0) { if (alive.empty()) return false; ev = mk(DEMI_EXT_KILL, alive.removeRandomElement(), 0, 0, 0); return true; }
-      if (t == 1) { ++counter; ev = mk(DEMI_EXT_SEND, alive.getRandomElement(), 0, cfg->send_type, counter); return true; }
-      if (t == 2) {
-        if (unpartitioned.empty()) continue;                                                // "Try again..."
-        const uint32_t p = unpartitioned.removeRandomElement(); partitioned.insert(p);
-        ev = mk(DEMI_EXT_PARTITION, p & 0xFF, p >> 8, 0, 0); return true;
-      }
-      if (partitioned.empty()) continue;
-      const uint32_t p = partitioned.removeRandomElement(); unpartitioned.insert(p);
-      ev = mk(DEMI_EXT_UNPARTITION, p & 0xFF, p >> 8, 0, 0); return true;
-    }
-  };
-  bool just_wq = !test.empty() && test.back().kind == DEMI_EXT_WAIT_QUIESCENCE;
-  bool ran_out = false;
-  for (uint32_t i = 0; i < cfg->num_events && !ran_out; i++) {
-    demi_ext_event ev{};
-    bool ok = next_event(ev);
-    while (ok && ev.kind == DEMI_EXT_WAIT_QUIESCENCE && just_wq) ok = next_event(ev);       // no two WaitQuiescence in a row
-    if (!ok) { ran_out = true; break; }
-    just_wq = ev.kind == DEMI_EXT_WAIT_QUIESCENCE;
-    test.push_back(ev);
-  }
-  if (!ran_out) {
-    test.insert(test.end(), postfix, postfix + n_postfix);
-    if (!test.empty() && test.back().kind != DEMI_EXT_WAIT_QUIESCENCE) test.push_back(mk(DEMI_EXT_WAIT_QUIESCENCE, 0, 0, 0, 0));
-  }
-  *n_out = (uint32_t)test.size();
-  if (test.size() > cap) return fail(nullptr, DEMI_ERR_CAPACITY, "demi_fuzzer_generate: %zu events, room for %u", test.size(), cap);
-  std::copy(test.begin(), test.end(), out);
+  uint32_t starts = 0;
+  for (uint32_t i = 0; i < n_prefix; i++) starts += prefix[i].kind == DEMI_EXT_START;
+  std::vector<uint8_t> alive(std::max(starts, 1u));
+  std::vector<uint16_t> pairs(2 * (size_t)demi::fuzzer_pair_room(starts) + 1);
+  std::vector<demi_ext_event> test((size_t)demi::fuzzer_program_room(*cfg, n_prefix, n_postfix));
+  uint32_t sends = 0;
+  const uint32_t len = demi::fuzzer_generate(*cfg, seed, prefix, n_prefix, postfix, n_postfix, alive.data(), pairs.data(),
+                                             test.data(), &sends);
+  *n_out = len;
+  if (len > cap) return fail(nullptr, DEMI_ERR_CAPACITY, "demi_fuzzer_generate: %u events, room for %u", len, cap);
+  std::copy(test.begin(), test.begin() + len, out);
   return DEMI_OK;
 }
 

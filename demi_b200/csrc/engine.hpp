@@ -80,6 +80,14 @@ struct demi_handle {
   // per type the packed rule (0 = no clock; a valid rule has bits >= 1, so it is never 0) and the incrementing set
   uint32_t clock_rule[256] = {};
   uint32_t clock_incr[8] = {};
+  // ---- the Fuzzer of demi_fuzz_campaign (demi_set_fuzzer) and the arena its generator kernel writes
+  bool has_fuzzer = false;
+  demi_fuzzer_config fuzzer{};
+  uint32_t fz_n_prefix = 0, fz_n_postfix = 0;
+  demi_ext_event* fz_fixed_dev = nullptr;                 // prefix | postfix
+  uint32_t fz_max_sends = 0;                              // Sends of the largest program: prefix + postfix + num_events
+  bool fz_has_hard_kill = false, fz_has_partitions = false, fz_sends_distinct = true;
+  void* fz_arena = nullptr; size_t fz_arena_bytes = 0;
   // ---- launch bookkeeping
   std::map<const void*, int> occupancy;          // kernel -> resident blocks per SM (asked once per handle)
   void* trace_rec = nullptr; size_t trace_rec_bytes = 0;   // demi_fuzz_trace's recording buffer

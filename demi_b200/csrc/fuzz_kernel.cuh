@@ -1,15 +1,18 @@
 // fuzz_kernel.cuh — K1: the persistent random-fuzz kernel.  One warp owns one
 // schedule prefix (one RandomScheduler execution) at a time and loops over the
 // prefix indices assigned to it; a block is WARPS independent warps.
+// PROG (campaigns, demi_fuzz_campaign): prefix idx runs program idx of the arena in `args.prog_*`, with that
+// program's capacities; the launch's own ext / n_ext / caps are the campaign's largest and size the scratch.
 #pragma once
 #include "machine.cuh"
 #include "models/models.cuh"
 
 namespace demi {
 
-template <class MODEL, int PCAP, int TCAP, bool PEND_GLOBAL, bool RECORD, int WARPS>
+template <class MODEL, int PCAP, int TCAP, bool PEND_GLOBAL, bool RECORD, int WARPS, bool PROG = false>
 __global__ void __launch_bounds__(WARPS * 32)
 fuzz_kernel(const __grid_constant__ KernelArgs args) {
+  static_assert(!(PROG && RECORD), "a campaign execution is recorded through demi_fuzz_trace on its program");
   using M = Machine<MODEL, PCAP, TCAP, PEND_GLOBAL, RECORD>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const uint32_t warp = threadIdx.x >> 5;
@@ -19,7 +22,8 @@ fuzz_kernel(const __grid_constant__ KernelArgs args) {
 
   M m;
   m.sm = reinterpret_cast<typename M::Smem*>(smem_raw + (size_t)warp * sizeof(typename M::Smem));
-  m.A = &args;
+  KernelArgs la;
+  if constexpr (PROG) { la = args; m.A = &la; } else m.A = &args;
   m.lane = lane;
   m.nodes_g = args.node_scratch + gw * args.node_cap;
   m.pend_g = PEND_GLOBAL ? (args.pend_scratch + gw * (uint64_t)PCAP) : nullptr;
@@ -39,6 +43,7 @@ fuzz_kernel(const __grid_constant__ KernelArgs args) {
     const uint64_t idx = args.index_list ? (uint64_t)args.index_list[it] : it;
     demi_fuzz_result r;
     if (RECORD) m.rec_ev = args.rec_events + it * (uint64_t)args.rec_cap;
+    if constexpr (PROG) prog_bind(la, args, idx, false);
     m.run(args.seed_base + (int64_t)idx, r);
     const bool retry = args.ovf_list && (r.status == DEMI_PS_PENDING_OVF || r.status == DEMI_PS_NODE_OVF);
     if (retry) {

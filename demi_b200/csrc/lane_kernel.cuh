@@ -587,9 +587,13 @@ struct LaneMachine {
 #endif
 // REC launches walk a work list (`index_list`): slot `it` of the list owns rec_events[it*rec_cap ..), rec_parent[it*cap ..),
 // rec_counts[it*4 ..) and results[it]; a deferred slot is handed to the general engine by POSITION (ovf_list holds `it`).
-template <class MODEL, int BD, int LPCAP, bool REC = false>
+// PROG (campaigns): prefix idx runs program idx of the arena in `args.prog_*` (see fuzz_kernel); the 0x80 | k entries
+// of messagesToSend resolve through that program's Send table.  A deferred prefix keeps its index, so the PROG
+// instantiation of the warp engine re-runs it on the same program.
+template <class MODEL, int BD, int LPCAP, bool REC = false, bool PROG = false>
 __global__ void __launch_bounds__(BD, DEMI_K1_MIN_BLOCKS)
 fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
+  static_assert(!(PROG && REC), "a campaign execution is recorded through demi_fuzz_trace on its program");
   using M = LaneMachine<MODEL, BD, LPCAP, REC>;
   extern __shared__ __align__(16) uint32_t lane_smem[];
   const uint32_t tid = threadIdx.x;
@@ -600,7 +604,8 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
   M m;
   m.smw = lane_smem + tid;
   m.pend = args.lane_pend + gwarp * (uint64_t)LPCAP * 32 + (tid & 31);
-  m.A = &args;
+  KernelArgs la;
+  if constexpr (PROG) { la = args; m.A = &la; } else m.A = &args;
   m.pol = l2_evict_last_policy();
   m.rec_ev = nullptr; m.rec_par = nullptr;
 
@@ -614,6 +619,7 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
       m.rec_par = args.rec_parent + it * (uint64_t)args.rec_parent_cap;
       m.rec_par[0] = 0;
     }
+    if constexpr (PROG) prog_bind(la, args, idx, true);
     demi_fuzz_result r;
     m.run(args.seed_base + (int64_t)idx, r);
     if (r.status == LANE_DEFER) {

@@ -165,7 +165,28 @@ struct KernelArgs {
   uint32_t  has_partitions;   // program contains Partition/UnPartition events
   // FullyRandom's userDefinedFilter as rules (demi_set_user_filter): {src_mask, dst_mask, type_mask, flags}
   uint4     filter[DEMI_MAX_FILTER_RULES]; uint32_t n_filter;
+  // campaign launches (the PROG kernels): execution idx runs program idx of the arena, under that program's own
+  // capacities (demi_pending_cap / demi_tosend_cap / demi_node_cap of its Sends).  Appended last, so that the
+  // parameter offsets of the other kernels stay where they were.
+  const demi_ext_event* prog_ext;      // [n][prog_stride] events
+  const uint2* prog_hdr;               // [n] {length, number of Sends}
+  const uint4* prog_sends;             // [n][prog_send_stride] the Sends as in `ext_sends` (lane engine)
+  uint32_t prog_stride, prog_send_stride;
+  int32_t  prog_model_key;             // the `model` argument of the capacity rules
+  int32_t  prog_max_messages;          // max_messages as the caller gave it (the capacity rules read it unmapped)
+  uint32_t prog_lane_pcap;             // lane engine: defer beyond this many pending messages (0 = no extra limit)
 };
+// The program view of a campaign execution: `la` is the executing thread's copy of the launch arguments.
+__device__ __forceinline__ void prog_bind(KernelArgs& la, const KernelArgs& args, uint64_t idx, bool lane) {
+  const uint2 h = args.prog_hdr[idx];
+  la.ext = args.prog_ext + idx * (uint64_t)args.prog_stride;
+  la.n_ext = h.x;
+  la.pending_cap = demi_pending_cap(args.prog_model_key, args.prog_max_messages, h.y);
+  if (lane && args.prog_lane_pcap && args.prog_lane_pcap < la.pending_cap) la.pending_cap = args.prog_lane_pcap;
+  la.tosend_cap = demi_tosend_cap(h.y);
+  la.node_cap = demi_node_cap(demi_pending_cap(args.prog_model_key, args.prog_max_messages, h.y));
+  la.ext_sends = args.prog_sends + idx * (uint64_t)args.prog_send_stride;
+}
 
 // -----------------------------------------------------------------------------
 // The machine.  MODEL supplies: N_ACTORS, STATE_WORDS, init_state(), receive(),

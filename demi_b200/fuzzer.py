@@ -69,6 +69,7 @@ class FuzzerWeights(object):
 
     def __init__(self, kill=0.01, send=0.3, wait_quiescence=0.1, partition=0.1, unpartition=0.1):
         self.allWeights = [kill, send, partition, unpartition]
+        self.wait_quiescence = wait_quiescence
         self.totalMass = sum(self.allWeights) + wait_quiescence
         self.eventTypes = ["Kill", "Send", "Partition", "UnPartition"]
 
@@ -80,6 +81,16 @@ class FuzzerWeights(object):
             if scaled < current:
                 return t
         return None            # WaitQuiescence
+
+
+def fuzzer_config(fuzzer):
+    """The demi_fuzzer_config of a Fuzzer whose message_gen is a ClientCommandGenerator (what the C ABI generates)."""
+    from . import _native as N
+    if not isinstance(fuzzer.message_gen, ClientCommandGenerator):
+        raise ValueError("the C ABI's Fuzzer generates Send(random alive actor, send_type, counter) only")
+    w = fuzzer.weights
+    kill, send, partition, unpartition = w.allWeights
+    return N.FuzzerConfig(kill, send, w.wait_quiescence, partition, unpartition, fuzzer.num_events, fuzzer.message_gen.msg_type)
 
 
 class ClientCommandGenerator(object):

@@ -8,12 +8,13 @@ CPU path here: constructing an engine without a CUDA device raises.
   RandomScheduler   <- schedulers/RandomScheduler.scala:41 (explore :234, test :597,
                        setMaxMessages :55, setInvariant :521)
 """
+import collections
 import ctypes as C
 
 import numpy as np
 
 from . import _native as N
-from .events import pack_externals
+from .events import pack_externals, unpack_externals
 
 
 class DemiError(RuntimeError):
@@ -95,6 +96,35 @@ class Engine(object):
     def fuzz_batch_dev(self, seed_base, n, max_messages, interval, out_ptr, stream=0, looking_for=0, flags=0):
         p = N.FuzzParams(seed_base, n, max_messages, interval, looking_for or 0, flags)
         self._check(N.lib().demi_fuzz_batch_dev(self._h, C.byref(p), C.c_void_p(out_ptr), C.c_void_p(stream)))
+
+    # ---- campaigns: a fresh Fuzzer program per execution (RunnerUtils.fuzz's loop, RunnerUtils.scala:75-91)
+    def set_fuzzer(self, config, prefix, postfix=()):
+        """demi_set_fuzzer: `config` is a FuzzerConfig (fuzzer.fuzzer_config builds one from a Fuzzer)."""
+        pre = prefix if isinstance(prefix, np.ndarray) else pack_externals(prefix)
+        post = postfix if isinstance(postfix, np.ndarray) else pack_externals(list(postfix))
+        pre = np.ascontiguousarray(pre, dtype=N.EXT_DTYPE)
+        post = np.ascontiguousarray(post, dtype=N.EXT_DTYPE)
+        self._fuzzer = (config, pre, post)
+        self._check(N.lib().demi_set_fuzzer(self._h, C.byref(config), pre.ctypes.data if len(pre) else None, len(pre),
+                                            post.ctypes.data if len(post) else None, len(post)))
+
+    def fuzzer_program(self, program_seed):
+        """The program the campaign execution with this program seed runs (demi_fuzzer_generate on the host)."""
+        cfg, pre, post = self._fuzzer
+        return N.fuzzer_generate(cfg, program_seed, pre, post)
+
+    def fuzz_campaign(self, seed_base, n, max_messages, interval, program_seed_base, looking_for=0, out=None, flags=0):
+        p = N.FuzzParams(seed_base, n, max_messages, interval, looking_for or 0, flags)
+        if out is None:
+            out = np.empty(n, dtype=N.RESULT_DTYPE)
+        elif out.dtype != N.RESULT_DTYPE or len(out) < n or not out.flags["C_CONTIGUOUS"]:
+            raise ValueError("out must be a C-contiguous array of >= %d demi_fuzz_result records" % n)
+        self._check(N.lib().demi_fuzz_campaign(self._h, C.byref(p), program_seed_base, out.ctypes.data))
+        return out
+
+    def fuzz_campaign_dev(self, seed_base, n, max_messages, interval, program_seed_base, out_ptr, stream=0, looking_for=0, flags=0):
+        p = N.FuzzParams(seed_base, n, max_messages, interval, looking_for or 0, flags)
+        self._check(N.lib().demi_fuzz_campaign_dev(self._h, C.byref(p), program_seed_base, C.c_void_p(out_ptr), C.c_void_p(stream)))
 
     def fuzz_summary_dev(self, stream=0):
         nv, ss = C.c_uint64(), C.c_uint64()
@@ -439,6 +469,76 @@ class RandomScheduler(object):
         self.stats = stats
         r = self.explore(events, violation_fingerprint)
         return None if r is None else r[0]
+
+
+PROGRAM_SEED_OFFSET = 1 << 32          # fuzz(): program_seed_base defaults to seed_base + this
+FuzzFound = collections.namedtuple("FuzzFound", "trace violation dep_graph initialTrace filtered externals execution")
+
+
+def fuzz(fuzzer, schedulerConfig, validate_replay=False, invariant_check_interval=30, maxMessages=None,
+         randomizationStrategy=None, computeProvenance=False, violationWereLookingFor=None, max_executions=100000,
+         seed_base=0, program_seed_base=None, engine=None, chunk=1 << 16):
+    """RunnerUtils.fuzz (RunnerUtils.scala:62-147).  Execution i runs program fuzzer.generateFuzzTest() drawn with seed
+    program_seed_base + i under FullyRandom(seed_base + i); executions run in campaign launches of `chunk`.
+
+    Deviations, on purpose: the reference loops until it finds a violation, here the loop stops after `max_executions`
+    and returns None.  It seeds the Fuzzer and FullyRandom from the wall clock; here they take the two separate bases
+    (with one base the two java.util.Random streams would be the same stream); program_seed_base defaults to
+    seed_base + 2^32 for that reason.  An execution that overflows a capacity
+    of the engine (status != 0) has no result and is passed over.
+
+    As written: an execution stops at its first violation of any kind (explore(fuzzTest) has no lookingFor), and
+    `violationWereLookingFor` (a predicate on the violation code, or a code) then accepts or rejects it; a rejected one
+    moves the loop on to the next execution.  The first accepted one is re-generated and recorded (demi_fuzz_trace);
+    with `validate_replay` it is replayed strictly (ReplayScheduler) and skipped (`deterministic = false`) if the replay
+    diverges or ends without a violation (`replayer.violationAtEnd.isEmpty`, RunnerUtils.scala:106-109).  With `computeProvenance`, `filtered` is ProvenanceTracker.pruneConcurrentEvents's
+    deliveries.  Returns FuzzFound(trace, violation, dep graph, initialTrace, filtered, the program, its index)."""
+    from .fuzzer import fuzzer_config
+    if randomizationStrategy not in (None, schedulerConfig.strategy):
+        raise ValueError("the randomization strategy is the SchedulerConfig's")
+    if violationWereLookingFor is None:
+        accept = lambda v: True
+    elif callable(violationWereLookingFor):
+        accept = violationWereLookingFor
+    else:
+        accept = lambda v: v == violationWereLookingFor
+    if computeProvenance and maxMessages is None:
+        raise ValueError("computeProvenance needs maxMessages (the pruning mask covers maxMessages + 2 deliveries)")
+    eng = engine or Engine(schedulerConfig)
+    eng.set_fuzzer(fuzzer_config(fuzzer), fuzzer.prefix, fuzzer.postfix)
+    if program_seed_base is None:
+        program_seed_base = seed_base + PROGRAM_SEED_OFFSET
+    mm = -1 if maxMessages is None else maxMessages
+    done = 0
+    while done < max_executions:
+        n = min(chunk, max_executions - done)
+        res = eng.fuzz_campaign(seed_base + done, n, mm, invariant_check_interval, program_seed_base + done)
+        for i in np.nonzero((res["violation"] != 0) & (res["status"] == 0))[0]:
+            violation = int(res["violation"][i])
+            if not accept(violation):
+                continue
+            k = done + int(i)
+            program = eng.fuzzer_program(program_seed_base + k)
+            eng.set_externals(program)
+            trace, dep, r = eng.fuzz_trace(seed_base + k, mm, invariant_check_interval)
+            if validate_replay:
+                try:
+                    rr = ReplayScheduler(schedulerConfig, trace, unpack_externals(program), engine=eng).replay(0)
+                    deterministic = int(rr["violation"]) != 0
+                except ReplayScheduler.ReplayException:
+                    deterministic = False
+                if not deterministic:
+                    continue
+            deliveries = trace[trace["kind"] == N.EV_MSG_EVENT]
+            initial = np.concatenate([[0], deliveries["node"]]).astype(np.uint16)   # DepTracker.getInitialTrace: root first
+            filtered = None
+            if computeProvenance:
+                eng.set_externals(program)
+                _, out, _ = eng.fuzz_provenance(seed_base + k, [0], mm, invariant_check_interval)
+                filtered = trace[ProvenanceTracker(eng, trace, dep).prune_concurrent_events(int(out[0]["affected_mask"]))]
+            return FuzzFound(trace, violation, dep, initial, filtered, program, k)
+        done += n
+    return None
 
 
 def mask_of(externals, subseq):

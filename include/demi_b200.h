@@ -596,6 +596,25 @@ int32_t demi_fuzzer_generate(const demi_fuzzer_config* cfg, int64_t seed,
                              const demi_ext_event* prefix, uint32_t n_prefix,
                              const demi_ext_event* postfix, uint32_t n_postfix,
                              demi_ext_event* out, uint32_t cap, uint32_t* n_out);
+/* Fuzzing campaigns: RunnerUtils.fuzz's loop (RunnerUtils.scala:75-91) as written, a new Fuzzer program for every
+ * execution.  demi_set_fuzzer sets the handle's Fuzzer (Fuzzer.scala:61-82); it leaves the handle's externals alone.
+ * It rejects what would make a generated program fail demi_set_externals: unknown kinds or actors, a prefix without
+ * Start (the Fuzzer's actors are the prefix's Starts, :60) or with more than DEMI_MAX_ACTORS Start events (a restart
+ * after Kill or HardKill counts too: the generator's sets hold one entry per Start), consecutive
+ * WaitQuiescence in the prefix or postfix, a postfix that begins with WaitQuiescence, a send_type the model does not
+ * define, weights that are negative, not finite or add up to 0, and num_events above DEMI_FUZZER_MAX_EVENTS. */
+#define DEMI_FUZZER_MAX_EVENTS 4096
+int32_t demi_set_fuzzer(demi_handle* h, const demi_fuzzer_config* cfg, const demi_ext_event* prefix, uint32_t n_prefix,
+                        const demi_ext_event* postfix, uint32_t n_postfix);
+/* n_prefixes executions; execution i runs the program demi_fuzzer_generate(cfg, program_seed_base + i, prefix, postfix)
+ * under FullyRandom(seed = seed_base + i).  Record i equals demi_set_externals(that program) followed by demi_fuzz_batch
+ * with seed_base + i and n_prefixes = 1: each execution has its own program's capacities (demi_limits.h).  The reference
+ * seeds both from the wall clock; the two bases are separate so that the two java.util.Random streams differ.  No state
+ * passes between executions (Fuzzer.reset, :177-193), so any split of a campaign gives the same records.
+ * DEMI_ERR_STATE when no Fuzzer is set.  _dev: records stay in HBM (`out_dev`, n_prefixes records), no sync;
+ * demi_fuzz_summary_dev reads the counts afterwards.  demi_perf.kernel_ms includes the programs' generation. */
+int32_t demi_fuzz_campaign(demi_handle* h, const demi_fuzz_params* p, int64_t program_seed_base, demi_fuzz_result* out_host);
+int32_t demi_fuzz_campaign_dev(demi_handle* h, const demi_fuzz_params* p, int64_t program_seed_base, void* out_dev, void* stream);
 /* The flat experiment directory that replaces ExperimentSerializer's Java object streams (Serialization.scala:57-74,
  * :176-254): externals.bin (demi_ext_event[]), event_trace.bin (demi_event[]), dep_parent.bin (uint16[], optional),
  * mcs.bin (uint64[] mask over the externals, optional), meta.json {model, model_flags, violation}.  Load: the counts

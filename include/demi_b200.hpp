@@ -24,6 +24,7 @@
 #pragma once
 #include <algorithm>
 #include <cstdint>
+#include <functional>
 #include <map>
 #include <memory>
 #include <optional>
@@ -160,9 +161,36 @@ class Engine {
   // UnmodifiedEventDag.conjoinAtoms (minification/Util.scala:167-178): DDMin treats the two externals as one atom
   void conjoin_atoms(uint32_t i1, uint32_t i2) { check(demi_conjoin_atoms(h, i1, i2)); }      // indices into the trace's externals
   demi_perf stats() const { demi_perf p{}; demi_stats(h, &p); return p; }
+  // ---- campaigns: a new Fuzzer program per execution (RunnerUtils.fuzz's loop, RunnerUtils.scala:75-91)
+  // demi_set_fuzzer: new Fuzzer(num_events, weights, message_gen, prefix, postfix) (Fuzzer.scala:61-82)
+  void set_fuzzer(const demi_fuzzer_config& c, const ExternalEvents& prefix, const ExternalEvents& postfix = {}) {
+    check(demi_set_fuzzer(h, &c, prefix.data(), (uint32_t)prefix.size(), postfix.empty() ? nullptr : postfix.data(),
+                          (uint32_t)postfix.size()));
+    fz_cfg = c; fz_prefix = prefix; fz_postfix = postfix;
+  }
+  // the program the campaign execution with this program seed runs (demi_fuzzer_generate)
+  ExternalEvents fuzzer_program(int64_t program_seed) const {
+    ExternalEvents out(fz_prefix.size() + fz_cfg.num_events + fz_postfix.size() + 1);
+    uint32_t n = 0;
+    check(demi_fuzzer_generate(&fz_cfg, program_seed, fz_prefix.data(), (uint32_t)fz_prefix.size(),
+                               fz_postfix.empty() ? nullptr : fz_postfix.data(), (uint32_t)fz_postfix.size(), out.data(),
+                               (uint32_t)out.size(), &n));
+    out.resize(n);
+    return out;
+  }
+  // demi_fuzz_campaign: record i = program fuzzer_program(program_seed_base + i) under FullyRandom(seed_base + i)
+  std::vector<demi_fuzz_result> fuzz_campaign(int64_t seed_base, uint64_t n, int32_t max_messages, int32_t interval,
+                                              int64_t program_seed_base, uint32_t looking_for = 0) {
+    demi_fuzz_params p{seed_base, n, max_messages, interval, looking_for, 0};
+    std::vector<demi_fuzz_result> out(n);
+    check(demi_fuzz_campaign(h, &p, program_seed_base, out.data()));
+    return out;
+  }
   const SchedulerConfig cfg;
  private:
   demi_handle* h = nullptr;
+  demi_fuzzer_config fz_cfg{};
+  ExternalEvents fz_prefix, fz_postfix;
 };
 
 inline std::vector<uint64_t> mask_of(const ExternalEvents& all, const ExternalEvents& subseq) {
@@ -425,6 +453,82 @@ class ProvenanceTracker {
   EventTrace trace;
   std::vector<uint16_t> dep_parent;
 };
+
+// RunnerUtils.fuzz (RunnerUtils.scala:62-147), the mirror of demi_b200.fuzz (schedulers.py), with the same deviations:
+// it stops after max_executions (nullopt), execution i draws its program with seed program_seed_base + i (default
+// seed_base + 2^32, so that the Fuzzer's and FullyRandom's java.util.Random streams differ) and runs under
+// FullyRandom(seed_base + i), and an execution that overflows an engine capacity is passed over.  As written:
+// executions stop at their first violation of any kind, the predicate filters on the host, the first accepted
+// execution in index order is re-generated and recorded (demi_fuzz_trace); with validate_replay it must replay
+// strictly and end in a violation (replayer.violationAtEnd non-empty, :106-109), else the loop goes on; with
+// computeProvenance `filtered` holds the deliveries ProvenanceTracker keeps.
+struct FuzzFound {
+  EventTrace trace;
+  ViolationFingerprint violation = 0;
+  std::vector<uint16_t> depGraph;          // DepTracker tree as parent pointers
+  std::vector<uint16_t> initialTrace;      // DepTracker.getInitialTrace: the root, then each delivery's node
+  EventTrace filtered;                     // computeProvenance: the deliveries that stay
+  ExternalEvents externals;                // the program (fuzzTest)
+  uint64_t execution = 0;
+};
+constexpr int64_t PROGRAM_SEED_OFFSET = 1ll << 32;
+inline std::optional<FuzzFound> fuzz(const demi_fuzzer_config& fuzzer, const ExternalEvents& prefix, const ExternalEvents& postfix,
+                                     const SchedulerConfig& cfg, bool validate_replay = false, int32_t invariant_check_interval = 30,
+                                     std::optional<int32_t> maxMessages = std::nullopt, bool computeProvenance = false,
+                                     std::function<bool(ViolationFingerprint)> violationWereLookingFor = nullptr,
+                                     uint64_t max_executions = 100000, int64_t seed_base = 0,
+                                     std::optional<int64_t> program_seed_base = std::nullopt,
+                                     std::shared_ptr<Engine> e = nullptr, uint64_t chunk = 1u << 16) {
+  if (computeProvenance && !maxMessages)
+    throw std::invalid_argument("computeProvenance needs maxMessages (the pruning mask covers maxMessages + 2 deliveries)");
+  std::shared_ptr<Engine> eng = e ? e : std::make_shared<Engine>(cfg);
+  eng->set_fuzzer(fuzzer, prefix, postfix);
+  const int64_t pbase = program_seed_base ? *program_seed_base : seed_base + PROGRAM_SEED_OFFSET;
+  const int32_t mm = maxMessages ? *maxMessages : -1;
+  for (uint64_t done = 0; done < max_executions;) {
+    const uint64_t n = std::min(chunk, max_executions - done);
+    const std::vector<demi_fuzz_result> res =
+        eng->fuzz_campaign(seed_base + (int64_t)done, n, mm, invariant_check_interval, pbase + (int64_t)done);
+    for (uint64_t i = 0; i < n; i++) {
+      if (res[i].status || !res[i].violation) continue;
+      const ViolationFingerprint v = res[i].violation;
+      if (violationWereLookingFor && !violationWereLookingFor(v)) continue;
+      const uint64_t k = done + i;
+      FuzzFound f;
+      f.externals = eng->fuzzer_program(pbase + (int64_t)k);
+      f.execution = k; f.violation = v;
+      eng->check(demi_set_externals(eng->handle(), f.externals.data(), (uint32_t)f.externals.size()));
+      demi_fuzz_params p{seed_base + (int64_t)k, 1, mm, invariant_check_interval, 0, 0};
+      f.trace.resize(65536); f.depGraph.resize(65536);
+      uint32_t n_ev = 0, n_nodes = 0; demi_fuzz_result r{};
+      eng->check(demi_fuzz_trace(eng->handle(), &p, seed_base + (int64_t)k, f.trace.data(), (uint32_t)f.trace.size(), &n_ev,
+                                 f.depGraph.data(), (uint32_t)f.depGraph.size(), &n_nodes, &r));
+      f.trace.resize(n_ev); f.depGraph.resize(n_nodes);
+      if (validate_replay) {
+        bool deterministic = true;
+        try {
+          ReplayScheduler replayer(cfg, f.trace, f.externals, false, eng);
+          deterministic = replayer.replay(0).violation != 0;
+        } catch (const ReplayException&) { deterministic = false; }
+        if (!deterministic) continue;
+      }
+      f.initialTrace.push_back(0);
+      for (const demi_event& x : f.trace) if (x.kind == DEMI_EV_MSG_EVENT) f.initialTrace.push_back(x.node);
+      if (computeProvenance) {
+        eng->check(demi_set_externals(eng->handle(), f.externals.data(), (uint32_t)f.externals.size()));
+        const uint32_t words = (uint32_t)((mm + 2 + 63) / 64), which = 0;
+        std::vector<uint64_t> keep(words);
+        demi_provenance_out po{};
+        eng->check(demi_fuzz_provenance(eng->handle(), &p, &which, 1, keep.data(), words, &po, nullptr));
+        ProvenanceTracker pt(eng, f.trace, f.depGraph);
+        for (uint32_t idx : pt.pruneConcurrentEvents(po.affected_mask)) f.filtered.push_back(f.trace[idx]);
+      }
+      return f;
+    }
+    done += n;
+  }
+  return std::nullopt;
+}
 
 class DPORwHeuristics {
  public:

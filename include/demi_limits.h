@@ -13,9 +13,16 @@
  * timersCancelledThisStep capacities (entries). */
 #define DEMI_TIMERSET_CAP 16
 
+/* Shared by host and device code (the campaign kernels apply the capacity rules per program). */
+#if defined(__CUDACC__)
+#define DEMI_HD __host__ __device__ __forceinline__
+#else
+#define DEMI_HD static inline
+#endif
+
 /* Pending-set capacity class for a (model, max_messages) pair: smallest power
  * of two >= the model's worst-case bound, clamped to [64, 8192]. */
-static inline uint32_t demi_pow2_at_least(uint32_t x, uint32_t lo, uint32_t hi) {
+DEMI_HD uint32_t demi_pow2_at_least(uint32_t x, uint32_t lo, uint32_t hi) {
   uint32_t c = lo;
   while (c < x && c < hi) c <<= 1;
   return c;
@@ -26,7 +33,7 @@ static inline uint32_t demi_pow2_at_least(uint32_t x, uint32_t lo, uint32_t hi) 
  *  raft5:     10 timers + net +4 per delivery              -> 16 + 4*(max_messages+1)
  *  bcast32:   net +30 per delivery                         -> 8 + 31*(max_messages+1) */
 /* model IR (demi_model_ir.h): the bound comes from the blob's "max sends of one receive()", model = 100 + 256 * fanout */
-static inline uint32_t demi_pending_bound(int model, int32_t max_messages, uint32_t n_ext_sends) {
+DEMI_HD uint32_t demi_pending_bound(int model, int32_t max_messages, uint32_t n_ext_sends) {
   uint32_t d = (max_messages < 0) ? 0u : (uint32_t)max_messages;
   if (d > 100000u) d = 100000u;
   if ((model & 0xFF) == 100) return n_ext_sends + 8u + (uint32_t)(model >> 8) * (d + 1u);
@@ -37,15 +44,15 @@ static inline uint32_t demi_pending_bound(int model, int32_t max_messages, uint3
     default: return 64u;
   }
 }
-static inline uint32_t demi_pending_cap(int model, int32_t max_messages, uint32_t n_ext_sends) {
+DEMI_HD uint32_t demi_pending_cap(int model, int32_t max_messages, uint32_t n_ext_sends) {
   return demi_pow2_at_least(demi_pending_bound(model, max_messages, n_ext_sends), 64u, 8192u);
 }
 /* messagesToSend capacity: externals of one segment + timers. */
-static inline uint32_t demi_tosend_cap(uint32_t n_ext_sends) {
+DEMI_HD uint32_t demi_tosend_cap(uint32_t n_ext_sends) {
   return demi_pow2_at_least(n_ext_sends + DEMI_TIMERSET_CAP, 32u, 1024u);
 }
 /* DepTracker node capacity: one node per enabled message + root. u16 ids. */
-static inline uint32_t demi_node_cap(uint32_t pending_cap) {
+DEMI_HD uint32_t demi_node_cap(uint32_t pending_cap) {
   uint32_t c = 2u * pending_cap + 64u;
   return c > 65535u ? 65535u : c;
 }
@@ -63,11 +70,6 @@ static inline uint32_t demi_external_type_mask(int model) {      /* model IR: ta
 /* ---- hashes ---------------------------------------------------------------
  * Order-sensitive and cheap on a GPU: a 64-bit SUM of per-item terms; each
  * term hashes the item's words together with its sequence number. */
-#if defined(__CUDACC__)
-#define DEMI_HD __host__ __device__ __forceinline__
-#else
-#define DEMI_HD static inline
-#endif
 
 /* EventTypes.isExternal by message type: the filter is a 32-bit mask, so a type >= 32 (possible in a loaded model)
  * is never external; it must not alias onto bit (type & 31). */

@@ -180,6 +180,16 @@ JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_fuzzerGenerate
                               postfix ? (const demi_ext_event*)BUF(env, postfix) : 0, (uint32_t)nPostfix, (demi_ext_event*)BUF(env, out),
                               (uint32_t)cap, (uint32_t*)BUF(env, nOut));
 }
+/* demi_set_fuzzer / demi_fuzz_campaign: RunnerUtils.fuzz's loop with a new Fuzzer program per execution */
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_setFuzzer(JNIEnv* env, jclass c, jlong h, jobject cfg,
+    jobject prefix, jint nPrefix, jobject postfix, jint nPostfix) {
+  return demi_set_fuzzer(H(h), (const demi_fuzzer_config*)BUF(env, cfg), (const demi_ext_event*)BUF(env, prefix), (uint32_t)nPrefix,
+                         postfix ? (const demi_ext_event*)BUF(env, postfix) : 0, (uint32_t)nPostfix);
+}
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_fuzzCampaign(JNIEnv* env, jclass c, jlong h, jobject params,
+    jlong programSeedBase, jobject out) {
+  return demi_fuzz_campaign(H(h), (const demi_fuzz_params*)BUF(env, params), (int64_t)programSeedBase, (demi_fuzz_result*)BUF(env, out));
+}
 /* `exp` = a direct buffer laid out as demi_experiment whose pointer fields the Scala side fills with
  * GetDirectBufferAddress-style addresses (DemiNative.addressOf) */
 JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_experimentSave(JNIEnv* env, jclass c, jstring dir, jobject exp) {

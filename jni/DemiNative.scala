@@ -65,6 +65,9 @@ object DemiNative {
   /** Fuzzer.generateFuzzTest, seeded (fuzzing/Fuzzer.scala:123-174). */
   @native def fuzzerGenerate(cfg: ByteBuffer, seed: Long, prefix: ByteBuffer, nPrefix: Int, postfix: ByteBuffer, nPostfix: Int,
                              out: ByteBuffer, cap: Int, nOut: ByteBuffer): Int
+  /** demi_set_fuzzer / demi_fuzz_campaign: RunnerUtils.fuzz's loop (RunnerUtils.scala:75-91), a new program per execution */
+  @native def setFuzzer(h: Long, cfg: ByteBuffer, prefix: ByteBuffer, nPrefix: Int, postfix: ByteBuffer, nPostfix: Int): Int
+  @native def fuzzCampaign(h: Long, params: ByteBuffer, programSeedBase: Long, out: ByteBuffer): Int
   /** The flat experiment directory that replaces ExperimentSerializer's *.bin object streams (Serialization.scala:57-74). */
   @native def experimentSave(dir: String, exp: ByteBuffer): Int
   @native def experimentLoad(dir: String, exp: ByteBuffer): Int
