@@ -122,6 +122,7 @@ EXPORTS = [
     "demi_load_model", "demi_actor_index", "demi_actor_name", "demi_set_user_filter",
     "demi_set_clock_rules", "demi_wildcard_replay_batch", "demi_wildcard_replay_trace", "demi_wildcard_minimize",
     "demi_set_fuzzer", "demi_fuzz_campaign", "demi_fuzz_campaign_dev",
+    "demi_random_test_batch", "demi_random_ddmin", "demi_random_test_trace",
 ]
 FILTER_RULE_DTYPE = np.dtype([("src_mask", "<u4"), ("dst_mask", "<u4"), ("type_mask", "<u4"), ("flags", "<u4")])
 FRULE_DEADLETTERS = 1
@@ -134,6 +135,19 @@ class FuzzerConfig(C.Structure):
 
 
 FUZZER_MAX_EVENTS = 4096
+
+# DDMin with RandomScheduler as the TestOracle (demi_random_test_batch / demi_random_ddmin)
+RANDOM_TEST_DTYPE = np.dtype([("first_hit", "<i4"), ("executions_run", "<u4"), ("violation", "<u4"), ("status", "<u2"),
+                              ("reserved", "<u2")])
+
+
+class RandomDDMinOut(C.Structure):
+    _fields_ = [("mcs_size", C.c_uint32), ("tests", C.c_uint32), ("n_iterations", C.c_uint32), ("verified", C.c_uint32),
+                ("total_replays", C.c_uint64), ("executions_executed", C.c_uint64), ("tests_evaluated", C.c_uint32),
+                ("batches", C.c_uint32), ("mcs_first_hit", C.c_int32), ("reserved", C.c_uint32)]
+
+
+assert RANDOM_TEST_DTYPE.itemsize == 16 and C.sizeof(RandomDDMinOut) == 48
 
 
 def fuzzer_generate(cfg, seed, prefix, postfix=None):
@@ -287,6 +301,14 @@ def lib():
     L.demi_fuzz_campaign.argtypes = [vp, C.POINTER(FuzzParams), C.c_int64, vp]
     L.demi_fuzz_campaign_dev.restype = C.c_int32
     L.demi_fuzz_campaign_dev.argtypes = [vp, C.POINTER(FuzzParams), C.c_int64, vp, vp]
+    L.demi_random_test_batch.restype = C.c_int32
+    L.demi_random_test_batch.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.POINTER(FuzzParams), vp]
+    L.demi_random_ddmin.restype = C.c_int32
+    L.demi_random_ddmin.argtypes = [vp, C.POINTER(FuzzParams), C.c_int32, vp, C.c_uint32, vp, vp, C.c_uint32,
+                                    C.POINTER(RandomDDMinOut)]
+    L.demi_random_test_trace.restype = C.c_int32
+    L.demi_random_test_trace.argtypes = [vp, vp, C.c_uint32, C.POINTER(FuzzParams), C.c_int64, vp, C.c_uint32,
+                                         C.POINTER(C.c_uint32), vp]
     L.demi_stats.restype = C.c_int32
     L.demi_stats.argtypes = [vp, C.POINTER(Perf)]
     _lib = L

@@ -4,8 +4,9 @@
   oracle/liboracle.so        — the CPU oracle (gcc; test infrastructure only)
   oracle/liboracle_wildcard.so — the same oracle with the wildcard-minimization restatement (oracle/wildcard.mk)
   oracle/liboracle_campaign.so — the same oracle with the Fuzzer and the campaign loop (oracle/campaign.mk)
+  oracle/liboracle_random_ddmin.so — the same oracle with DDMin over RandomScheduler tests (oracle/random_ddmin.mk)
 
-All four are git-ignored build products.
+All five are git-ignored build products.
 """
 import os
 import subprocess
@@ -18,6 +19,7 @@ ORACLE_DIR = os.path.join(ROOT, "oracle")
 ORACLE_LIB = os.path.join(ORACLE_DIR, "liboracle.so")
 ORACLE_WILDCARD_LIB = os.path.join(ORACLE_DIR, "liboracle_wildcard.so")   # oracle/wildcard.mk
 ORACLE_CAMPAIGN_LIB = os.path.join(ORACLE_DIR, "liboracle_campaign.so")   # oracle/campaign.mk
+ORACLE_RANDOM_DDMIN_LIB = os.path.join(ORACLE_DIR, "liboracle_random_ddmin.so")   # oracle/random_ddmin.mk
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -105,15 +107,18 @@ def build_oracle(force=False):
     srcs.append(os.path.join(ORACLE_DIR, "Makefile"))
     srcs.append(os.path.join(ORACLE_DIR, "wildcard.mk"))
     srcs.append(os.path.join(ORACLE_DIR, "campaign.mk"))
+    srcs.append(os.path.join(ORACLE_DIR, "random_ddmin.mk"))
     stamp = _cpu_stamp()
     same_cpu = os.path.exists(ORACLE_STAMP) and open(ORACLE_STAMP).read().strip() == stamp
     if not force and same_cpu and _newer(ORACLE_LIB, srcs) and _newer(ORACLE_WILDCARD_LIB, srcs) \
-            and _newer(ORACLE_CAMPAIGN_LIB, srcs):
+            and _newer(ORACLE_CAMPAIGN_LIB, srcs) and _newer(ORACLE_RANDOM_DDMIN_LIB, srcs):
         return ORACLE_LIB
     # make's chatter goes to stderr: bench.py prints exactly one JSON line on stdout
     subprocess.check_call(["make", "-B", "-C", ORACLE_DIR, "liboracle.so"], stdout=sys.stderr)
     subprocess.check_call(["make", "-B", "-C", ORACLE_DIR, "-f", "wildcard.mk", "liboracle_wildcard.so"], stdout=sys.stderr)
     subprocess.check_call(["make", "-B", "-C", ORACLE_DIR, "-f", "campaign.mk", "liboracle_campaign.so"], stdout=sys.stderr)
+    subprocess.check_call(["make", "-B", "-C", ORACLE_DIR, "-f", "random_ddmin.mk", "liboracle_random_ddmin.so"],
+                          stdout=sys.stderr)
     with open(ORACLE_STAMP, "w") as f:
         f.write(stamp + "\n")
     return ORACLE_LIB

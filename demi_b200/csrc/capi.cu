@@ -29,13 +29,15 @@ struct Variant {
   int model; uint32_t pcap, tcap; bool pend_global, record;
   kernel_fn fn; size_t smem_per_warp;
   kernel_fn fn_prog;             // the campaign instantiation (PROG); none for the recording variants
+  kernel_fn fn_tests;            // the random-oracle test instantiation (PROG + TESTS); none for the recording variants
 };
 template <class MODEL, int PCAP, int TCAP, bool PG, bool REC>
 static Variant make_variant() {
   using M = Machine<MODEL, PCAP, TCAP, PG, REC>;
   return Variant{MODEL::ID, (uint32_t)PCAP, (uint32_t)TCAP, PG, REC,
                  fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS>, sizeof(typename M::Smem),
-                 REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC>};
+                 REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC>,
+                 REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC, !REC>};
 }
 static const std::vector<Variant>& variants() {
   static const std::vector<Variant> v = {
@@ -63,12 +65,14 @@ static const Variant* pick_variant(int model, uint32_t pcap, uint32_t tcap, bool
 }
 
 // lane-engine table
-struct LaneVariant { int model; int bd; uint32_t lpcap; kernel_fn fn; kernel_fn fn_rec; size_t smem_per_block; kernel_fn fn_prog; };
+struct LaneVariant { int model; int bd; uint32_t lpcap; kernel_fn fn; kernel_fn fn_rec; size_t smem_per_block; kernel_fn fn_prog;
+                     kernel_fn fn_tests; };
 template <class MODEL, int BD, int LPCAP>
 static LaneVariant make_lane_variant() {
   using M = LaneMachine<MODEL, BD, LPCAP>;
   return LaneVariant{MODEL::ID, BD, (uint32_t)LPCAP, fuzz_lane_kernel<MODEL, BD, LPCAP>, fuzz_lane_kernel<MODEL, BD, LPCAP, true>,
-                     (size_t)M::WORDS * BD * sizeof(uint32_t), fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>};
+                     (size_t)M::WORDS * BD * sizeof(uint32_t), fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>,
+                     fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true>};
 }
 static const LaneVariant* pick_lane_variant(const demi_handle* h, bool campaign = false);
 
@@ -286,8 +290,10 @@ static int32_t ensure(demi_handle* h, void** p, size_t* cap, size_t need) {
   return DEMI_OK;
 }
 
-// campaign: sized for the Fuzzer's largest program (fz_max_sends Sends); ext / n_ext are bound per execution
-static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool record, LaunchPlan* plan, bool campaign = false) {
+// campaign: sized for the Fuzzer's largest program (fz_max_sends Sends); ext / n_ext are bound per execution.
+// tests: the launch runs fn_tests (random-oracle tests over the handle's program)
+static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool record, LaunchPlan* plan, bool campaign = false,
+                           bool tests = false) {
   if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
   if (campaign && !h->has_fuzzer) return fail(h, DEMI_ERR_STATE, "demi_set_fuzzer has not been called");
   if (!campaign && h->ext_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
@@ -299,7 +305,7 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool recor
   const bool fifo = h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;          // SrcDstFIFO lives in the HBM-pending variants
   const Variant* v = pick_variant(h->cfg.model, pcap, tcap, record, fifo);
   if (!v) return fail(h, DEMI_ERR_CAPACITY, "no kernel variant for pending_cap=%u tosend_cap=%u", pcap, tcap);
-  const kernel_fn fn = campaign ? v->fn_prog : v->fn;
+  const kernel_fn fn = tests ? v->fn_tests : campaign ? v->fn_prog : v->fn;
   const size_t smem = v->smem_per_warp * WARPS;
   // the attribute and the occupancy of a variant are fixed per device: asked once, not on every launch
   int blocks_per_sm = 0;
@@ -903,6 +909,315 @@ extern "C" int32_t demi_fuzz_campaign(demi_handle* h, const demi_fuzz_params* p,
     q.n_prefixes = m;
     return launch_campaign(h, &q, program_seed_base + (int64_t)off, dst, h->stream, first);
   });
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Random-oracle tests: RandomScheduler.test(subsequence) (RandomScheduler.scala:597-612) for T masks over the handle's
+// program, N executions each, T x N executions per launch through the PROG engines.
+
+// One warp per test: the subsequence of the base program that the test's mask keeps, compacted (ballot + prefix sum)
+// into the arena layout of the campaigns: events[t * stride ..), hdr[t] = {length, Sends}, the lane-form Sends at
+// sends[t * send_stride ..).
+__global__ void __launch_bounds__(128)
+random_subseq_kernel(const demi_ext_event* base, uint32_t n_ext, const uint64_t* masks, uint32_t mask_words, uint32_t n_tests,
+                     demi_ext_event* events, uint32_t stride, uint2* hdr, uint4* sends, uint32_t send_stride) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (t >= n_tests) return;
+  const uint64_t* mask = masks + t * mask_words;
+  const uint32_t below = (1u << lane) - 1u;
+  uint32_t len = 0, ns = 0;
+  for (uint32_t b = 0; b < n_ext; b += 32) {
+    const uint32_t i = b + lane;
+    const bool in = i < n_ext && ((mask[i >> 6] >> (i & 63)) & 1ull);
+    demi_ext_event e{};
+    if (in) e = base[i];
+    const bool send = in && e.kind == DEMI_EXT_SEND;
+    const uint32_t m = __ballot_sync(FULL_MASK, in), ms = __ballot_sync(FULL_MASK, send);
+    if (in) events[t * stride + len + __popc(m & below)] = e;
+    if (send)
+      sends[t * send_stride + ns + __popc(ms & below)] =
+          make_uint4(DEMI_DEADLETTERS | ((uint32_t)e.a << 8) | ((uint32_t)e.type << 16) | ((uint32_t)DEMI_MF_EXTERNAL << 24), e.p0, e.p1, 0u);
+    len += __popc(m); ns += __popc(ms);
+  }
+  if (lane == 0) hdr[t] = make_uint2(len, ns);
+}
+
+// One warp per test over its N execution records: the test record, and the executions that ran (not skipped).
+__global__ void __launch_bounds__(128)
+random_test_reduce_kernel(const demi_fuzz_result* res, uint32_t n_tests, uint32_t n_execs, demi_random_test_result* out,
+                          unsigned long long* executed) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (t >= n_tests) return;
+  int32_t first = -1;
+  uint32_t status = 0, violation = 0, ran = 0;
+  for (uint32_t b = 0; b < n_execs; b += 32) {
+    const uint32_t j = b + lane;
+    uint32_t st = PS_SKIPPED, v = 0;
+    if (j < n_execs) { const demi_fuzz_result& r = res[t * n_execs + j]; st = r.status; v = r.violation; }
+    const uint32_t hit = __ballot_sync(FULL_MASK, st == 0 && v != 0);
+    const uint32_t bad = __ballot_sync(FULL_MASK, st != 0 && st != PS_SKIPPED);
+    ran += __popc(__ballot_sync(FULL_MASK, st != PS_SKIPPED));
+    if (first < 0) {
+      const uint32_t upto = hit ? (((hit & (0u - hit)) - 1u) | (hit & (0u - hit))) : FULL_MASK;   // lanes up to the first hit
+      const uint32_t first_bad = bad & upto;
+      const uint32_t sb = __shfl_sync(FULL_MASK, st, first_bad ? __ffs(first_bad) - 1 : 0);
+      if (!status && first_bad) status = sb;
+      const uint32_t vh = __shfl_sync(FULL_MASK, v, hit ? __ffs(hit) - 1 : 0);
+      if (hit) { first = (int32_t)(b + __ffs(hit) - 1); violation = vh; }
+    }
+  }
+  if (lane == 0) {
+    out[t] = demi_random_test_result{first, first >= 0 ? (uint32_t)first + 1 : n_execs, violation, (uint16_t)status, 0};
+    atomicAdd(executed, (unsigned long long)ran);
+  }
+}
+
+// tests per launch: at most RANDOM_EXECS_PER_LAUNCH executions (their records are 32 B each, 128 MB) and an arena of
+// at most 512 MB
+static constexpr uint64_t RANDOM_EXECS_PER_LAUNCH = 1u << 22;
+
+static int32_t check_random(demi_handle* h, const char* who, uint32_t mask_words, const demi_fuzz_params* p) {
+  if (!p) return fail(h, DEMI_ERR_INVALID, "%s: null params", who);
+  if (h->ext_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
+  if (p->n_prefixes == 0 || p->n_prefixes > RANDOM_EXECS_PER_LAUNCH)
+    return fail(h, DEMI_ERR_INVALID, "%s: N = n_prefixes must be in 1..%llu", who, (unsigned long long)RANDOM_EXECS_PER_LAUNCH);
+  if ((uint64_t)mask_words * 64 < h->ext_host.size()) return fail(h, DEMI_ERR_INVALID, "%s: mask_words too small", who);
+  return DEMI_OK;
+}
+
+// the tests of one call, in launches of `per` tests; *executed = executions that ran
+static int32_t random_tests(demi_handle* h, const uint64_t* masks, uint32_t n_tests, uint32_t mask_words, const demi_fuzz_params* p,
+                            demi_random_test_result* out, uint64_t* executed) {
+  const uint32_t N = (uint32_t)p->n_prefixes, n_ext = (uint32_t)h->ext_host.size();
+  const uint32_t stride = std::max(n_ext, 1u), send_stride = std::max(h->n_ext_sends, 1u);
+  const uint64_t per_test = (uint64_t)stride * sizeof(demi_ext_event) + sizeof(uint2) + (uint64_t)send_stride * sizeof(uint4) +
+                            (uint64_t)mask_words * 8 + sizeof(demi_random_test_result) + 4;
+  const uint64_t per = std::max<uint64_t>(1, std::min<uint64_t>(RANDOM_EXECS_PER_LAUNCH / N, ((uint64_t)512 << 20) / per_test));
+  const uint64_t cap_tests = std::min<uint64_t>(per, n_tests);
+  // arena: events | hdr | sends | masks | first_hit | test records | counter
+  const size_t b_ev = (size_t)cap_tests * stride * sizeof(demi_ext_event), b_hdr = ((size_t)cap_tests * sizeof(uint2) + 15) & ~(size_t)15,
+               b_snd = (size_t)cap_tests * send_stride * sizeof(uint4), b_mask = ((size_t)cap_tests * mask_words * 8 + 15) & ~(size_t)15,
+               b_fh = ((size_t)cap_tests * 4 + 15) & ~(size_t)15, b_out = ((size_t)cap_tests * sizeof(demi_random_test_result) + 15) & ~(size_t)15;
+  int32_t rc = ensure(h, &h->fz_arena, &h->fz_arena_bytes, b_ev + b_hdr + b_snd + b_mask + b_fh + b_out + 16);
+  if (rc != DEMI_OK) return rc;
+  if ((rc = ensure(h, (void**)&h->results_dev, &h->results_cap, std::max<size_t>((size_t)cap_tests * N * sizeof(demi_fuzz_result), 32))) != DEMI_OK)
+    return rc;
+  unsigned char* a0 = (unsigned char*)h->fz_arena;
+  demi_ext_event* ev = (demi_ext_event*)a0;
+  uint2* hdr = (uint2*)(a0 + b_ev);
+  uint4* sends = (uint4*)(a0 + b_ev + b_hdr);
+  uint64_t* mdev = (uint64_t*)(a0 + b_ev + b_hdr + b_snd);
+  uint32_t* first_hit = (uint32_t*)(a0 + b_ev + b_hdr + b_snd + b_mask);
+  demi_random_test_result* odev = (demi_random_test_result*)(a0 + b_ev + b_hdr + b_snd + b_mask + b_fh);
+  unsigned long long* cnt = (unsigned long long*)(a0 + b_ev + b_hdr + b_snd + b_mask + b_fh + b_out);
+  cudaStream_t s = h->stream;
+  CUDA_TRY(h, cudaMemsetAsync(cnt, 0, sizeof(unsigned long long), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
+  CUDA_TRY(h, cudaEventRecord(h->ev0, s));
+  h->perf.kernel_launches = 0;
+  for (uint64_t off = 0; off < n_tests; off += per) {
+    const uint32_t m = (uint32_t)std::min<uint64_t>(per, n_tests - off);
+    demi_fuzz_params q = *p;
+    q.n_prefixes = (uint64_t)m * N;
+    LaunchPlan plan;
+    if ((rc = plan_launch(h, &q, false, &plan, false, true)) != DEMI_OK) return rc;
+    CUDA_TRY(h, cudaMemcpyAsync(mdev, masks + off * mask_words, (size_t)m * mask_words * 8, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(h, cudaMemsetAsync(first_hit, 0xFF, (size_t)m * 4, s));
+    random_subseq_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(h->ext_dev, n_ext, mdev, mask_words, m, ev, stride,
+                                                                                     hdr, sends, send_stride);
+    CUDA_TRY(h, cudaGetLastError());
+    KernelArgs& a = plan.args;
+    a.results = h->results_dev;
+    a.prog_ext = ev; a.prog_hdr = hdr; a.prog_sends = sends;
+    a.prog_stride = stride; a.prog_send_stride = send_stride;
+    a.prog_model_key = demi_model_key(h);
+    a.prog_max_messages = p->max_messages;
+    a.prog_execs = N;
+    a.prog_first_hit = first_hit;
+    // lane eligibility is decided on the base program: every condition pick_lane_variant checks (distinct Sends, no
+    // HardKill, ...) holds for each of its subsequences
+    if (const LaneVariant* lv = pick_lane_variant(h)) {
+      if ((rc = launch_lane(h, lv, lv->fn_tests, a, q.n_prefixes, s)) != DEMI_OK) return rc;
+      a.index_list = h->ovf_list;
+      a.index_count = h->ovf_count;
+    }
+    if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
+    plan.v->fn_tests<<<plan.grid, WARPS * 32, plan.smem, s>>>(a);
+    CUDA_TRY(h, cudaGetLastError());
+    random_test_reduce_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(h->results_dev, m, N, odev, cnt);
+    CUDA_TRY(h, cudaGetLastError());
+    h->perf.kernel_launches += 3;        // launch_lane counts its own
+    CUDA_TRY(h, cudaMemcpyAsync(out + off, odev, (size_t)m * sizeof(demi_random_test_result), cudaMemcpyDeviceToHost, s));
+  }
+  unsigned long long c[4] = {0, 0, 0, 0}, ran = 0;
+  CUDA_TRY(h, cudaEventRecord(h->ev1, s));
+  CUDA_TRY(h, cudaMemcpyAsync(c, h->counters_dev, sizeof(c), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(&ran, cnt, sizeof(ran), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  float ms = 0;
+  CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+  h->perf.kernel_ms = ms;
+  h->perf.prefixes = ran;
+  h->perf.deliveries = c[0]; h->perf.violations = c[1];
+  h->perf.deferred = (uint32_t)std::min<unsigned long long>(c[2], 0xFFFFFFFFull);
+  h->perf.h2d_bytes = (uint64_t)n_tests * mask_words * 8;
+  h->perf.d2h_bytes = (uint64_t)n_tests * sizeof(demi_random_test_result);
+  *executed = ran;
+  return DEMI_OK;
+}
+
+extern "C" int32_t demi_random_test_batch(demi_handle* h, const uint64_t* masks, uint32_t n_tests, uint32_t mask_words,
+                                          const demi_fuzz_params* p, demi_random_test_result* out) {
+  if (!h) return DEMI_ERR_INVALID;
+  int32_t rc = check_random(h, "demi_random_test_batch", mask_words, p);
+  if (rc != DEMI_OK) return rc;
+  if (n_tests && (!masks || !out)) return fail(h, DEMI_ERR_INVALID, "demi_random_test_batch: null masks or output");
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  uint64_t executed = 0;
+  if (!n_tests) { h->perf.prefixes = 0; return DEMI_OK; }
+  return random_tests(h, masks, n_tests, mask_words, p, out, &executed);
+}
+
+// demi_fuzz_trace over a subsequence of the handle's program: the program's host and device copies are swapped for
+// the subsequence's for the one recording launch, then restored
+extern "C" int32_t demi_random_test_trace(demi_handle* h, const uint64_t* mask, uint32_t mask_words, const demi_fuzz_params* p,
+                                          int64_t seed, demi_event* events, uint32_t cap_events, uint32_t* n_events,
+                                          demi_fuzz_result* result) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!p || !mask) return fail(h, DEMI_ERR_INVALID, "demi_random_test_trace: null argument");
+  if (h->ext_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
+  if ((uint64_t)mask_words * 64 < h->ext_host.size()) return fail(h, DEMI_ERR_INVALID, "demi_random_test_trace: mask_words too small");
+  std::vector<demi_ext_event> sub;
+  uint32_t sends = 0;
+  bool hard_kill = false;
+  for (size_t i = 0; i < h->ext_host.size(); i++)
+    if ((mask[i >> 6] >> (i & 63)) & 1ull) {
+      sub.push_back(h->ext_host[i]);
+      sends += sub.back().kind == DEMI_EXT_SEND;
+      hard_kill |= sub.back().kind == DEMI_EXT_HARD_KILL;
+    }
+  if (sub.empty()) return fail(h, DEMI_ERR_INVALID, "demi_random_test_trace: the mask keeps no event");
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  demi_ext_event* dev = nullptr;
+  CUDA_TRY(h, cudaMalloc(&dev, sub.size() * sizeof(demi_ext_event)));
+  cudaError_t e = cudaMemcpy(dev, sub.data(), sub.size() * sizeof(demi_ext_event), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) { cudaFree(dev); return fail(h, DEMI_ERR_CUDA, "demi_random_test_trace: %s", cudaGetErrorString(e)); }
+  std::swap(h->ext_dev, dev); h->ext_host.swap(sub); std::swap(h->n_ext_sends, sends); std::swap(h->has_hard_kill, hard_kill);
+  const int32_t rc = demi_fuzz_trace(h, p, seed, events, cap_events, n_events, nullptr, 0, nullptr, result);
+  std::swap(h->ext_dev, dev); h->ext_host.swap(sub); std::swap(h->n_ext_sends, sends); std::swap(h->has_hard_kill, hard_kill);
+  cudaFree(dev);
+  return rc;
+}
+
+#include "ddmin_driver.hpp"
+namespace {
+
+// RandomScheduler as DDMin's TestOracle: a speculative batch of masks = one demi_random_test_batch
+struct RandomDDMinDriver : DDMinDriver {
+  demi_fuzz_params p{};
+  std::map<Mask, demi_random_test_result> records;
+  std::vector<uint32_t> consumed_runs;      // executions_run of each test the sequential walk consumed, in order
+  uint64_t executions_executed = 0;
+  int32_t evaluate_flat(const uint64_t* masks, size_t n, signed char* out) override {
+    std::vector<demi_random_test_result> res(n);
+    uint64_t executed = 0;
+    int32_t rc = random_tests(h, masks, (uint32_t)n, mw, &p, res.data(), &executed);
+    if (rc != DEMI_OK) return rc;
+    executions_executed += executed;
+    for (size_t i = 0; i < n; i++) {
+      records[Mask(masks + i * mw, masks + (i + 1) * mw)] = res[i];
+      out[i] = res[i].status == 0 && res[i].first_hit >= 0;
+    }
+    return DEMI_OK;
+  }
+  int32_t evaluate_batch(const std::vector<Mask>& want, std::vector<char>& out) override {
+    std::vector<uint64_t> flat(want.size() * mw);
+    for (size_t i = 0; i < want.size(); i++) std::copy(want[i].begin(), want[i].end(), flat.begin() + i * mw);
+    std::vector<signed char> r(want.size());
+    int32_t rc = evaluate_flat(flat.data(), want.size(), r.data());
+    for (size_t i = 0; i < want.size(); i++) out[i] = r[i];
+    return rc;
+  }
+  // a test's status fails the call only here, where the sequential walk uses its result
+  void consumed(const Mask& m) override {
+    const demi_random_test_result& r = records.at(m);
+    if (r.status) { error = fail(h, DEMI_ERR_CAPACITY, "demi_random_ddmin: a test execution reported status %u", (unsigned)r.status); return; }
+    consumed_runs.push_back(r.executions_run);
+  }
+};
+
+}  // namespace
+
+extern "C" int32_t demi_random_ddmin(demi_handle* h, const demi_fuzz_params* p, int32_t check_unmodified, uint64_t* mcs_mask,
+                                     uint32_t mask_words, uint32_t* iteration_sizes, uint64_t* iteration_keys, uint32_t cap,
+                                     demi_random_ddmin_out* out) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!mcs_mask || !out) return fail(h, DEMI_ERR_INVALID, "demi_random_ddmin: null output");
+  int32_t rc = check_random(h, "demi_random_ddmin", mask_words, p);
+  if (rc != DEMI_OK) return rc;
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  memset(out, 0, sizeof(*out));
+  const uint32_t n_ext = (uint32_t)h->ext_host.size();
+  RandomDDMinDriver d;
+  d.h = h; d.p = *p; d.looking_for = p->looking_for; d.mw = mask_words; d.n_ext = n_ext;
+  d.ext = h->ext_host.data();
+  // tests per speculative batch, sized by executions per launch: about 2^20 executions (a few milliseconds of the lane
+  // engine on raft5-sized programs, so the launch latency is amortised), and never more than the 6000 tests of the
+  // replay path (beyond that the host's batch building costs more than the launch)
+  d.wide_cap = std::max<size_t>(16, std::min<size_t>(6000, ((size_t)1 << 20) / p->n_prefixes));
+  if (getenv("DEMI_DDMIN_WIDE")) d.wide_cap = (size_t)atol(getenv("DEMI_DDMIN_WIDE"));
+  // DDMin.minimize's dag is the whole program, WaitQuiescence included (UnmodifiedEventDag, Minimizer.scala:15-20)
+  Mask dag(mask_words, 0), zero(mask_words, 0);
+  for (uint32_t i = 0; i < n_ext; i++) DDMinDriver::setbit(dag, i);
+  if (check_unmodified) {                                                 // DeltaDebugging.scala:41-47
+    bool v = d.test(dag, dag, zero);
+    if (d.error != DEMI_OK) return d.error;
+    if (!v) return fail(h, DEMI_ERR_INVALID, "Unmodified trace does not trigger violation");
+    d.consumed_runs.clear();                                              // _stats.reset() (:48)
+  }
+  d.original_num_events = n_ext;
+  Mask mcs = d.ddmin2(dag, zero);
+  if (d.error != DEMI_OK) return d.error;
+  d.iteration_sizes.push_back(d.original_num_events - d.total_inputs_pruned);     // fencepost :60
+  if (d.original_num_events - d.total_inputs_pruned != DDMinDriver::popcount(mcs))
+    return fail(h, DEMI_ERR_STATE, "demi_random_ddmin: bookkeeping assertion failed (DeltaDebugging.scala:58)");
+  const uint32_t tests = (uint32_t)d.consumed_runs.size();
+  std::vector<uint64_t> keys;
+  uint64_t total = 0;
+  for (uint32_t r : d.consumed_runs) { total += r; keys.push_back(total); }
+  keys.push_back(total);                                                  // the fencepost's key
+  out->mcs_size = DDMinDriver::popcount(mcs);
+  bool verified = true;                                                   // nothing pruned: the original trace stands
+  out->mcs_first_hit = -1;
+  if (out->mcs_size < n_ext) {                                            // verify_mcs (RunnerUtils.scala:612-620)
+    // the MCS's own test alone: taken from the tests already run, else evaluated by itself (no speculation below it)
+    auto it = d.records.find(mcs);
+    if (it == d.records.end()) {
+      signed char v;
+      if ((rc = d.evaluate_flat(mcs.data(), 1, &v)) != DEMI_OK) return rc;
+      d.replays_executed++;
+      it = d.records.find(mcs);
+    }
+    const demi_random_test_result& r = it->second;
+    if (r.status) return fail(h, DEMI_ERR_CAPACITY, "demi_random_ddmin: the MCS's test reported status %u", (unsigned)r.status);
+    verified = r.first_hit >= 0;
+    out->mcs_first_hit = r.first_hit;
+  }
+  std::copy(mcs.begin(), mcs.end(), mcs_mask);
+  out->tests = tests;
+  out->total_replays = total;
+  out->n_iterations = (uint32_t)d.iteration_sizes.size();
+  out->executions_executed = d.executions_executed;
+  out->tests_evaluated = d.replays_executed;
+  out->batches = d.batches;
+  out->verified = verified ? 1u : 0u;
+  for (uint32_t i = 0; i < cap && i < out->n_iterations; i++) {
+    if (iteration_sizes) iteration_sizes[i] = d.iteration_sizes[i];
+    if (iteration_keys) iteration_keys[i] = keys[i];
+  }
+  return DEMI_OK;
 }
 
 extern "C" int32_t demi_stats(const demi_handle* h, demi_perf* out) {

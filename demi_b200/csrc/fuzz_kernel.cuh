@@ -3,16 +3,20 @@
 // prefix indices assigned to it; a block is WARPS independent warps.
 // PROG (campaigns, demi_fuzz_campaign): prefix idx runs program idx of the arena in `args.prog_*`, with that
 // program's capacities; the launch's own ext / n_ext / caps are the campaign's largest and size the scratch.
+// PROG + TESTS (random-oracle tests, demi_random_test_batch): prefix idx is execution idx % prog_execs of program
+// idx / prog_execs (prog_test_bind), skipped above its program's first hit.  A separate instantiation, so that the
+// campaign kernels stay as they were.
 #pragma once
 #include "machine.cuh"
 #include "models/models.cuh"
 
 namespace demi {
 
-template <class MODEL, int PCAP, int TCAP, bool PEND_GLOBAL, bool RECORD, int WARPS, bool PROG = false>
+template <class MODEL, int PCAP, int TCAP, bool PEND_GLOBAL, bool RECORD, int WARPS, bool PROG = false, bool TESTS = false>
 __global__ void __launch_bounds__(WARPS * 32)
 fuzz_kernel(const __grid_constant__ KernelArgs args) {
   static_assert(!(PROG && RECORD), "a campaign execution is recorded through demi_fuzz_trace on its program");
+  static_assert(PROG || !TESTS, "random-oracle tests bind their programs as campaigns do");
   using M = Machine<MODEL, PCAP, TCAP, PEND_GLOBAL, RECORD>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const uint32_t warp = threadIdx.x >> 5;
@@ -43,8 +47,19 @@ fuzz_kernel(const __grid_constant__ KernelArgs args) {
     const uint64_t idx = args.index_list ? (uint64_t)args.index_list[it] : it;
     demi_fuzz_result r;
     if (RECORD) m.rec_ev = args.rec_events + it * (uint64_t)args.rec_cap;
-    if constexpr (PROG) prog_bind(la, args, idx, false);
-    m.run(args.seed_base + (int64_t)idx, r);
+    if constexpr (TESTS) {
+      uint64_t prog; int64_t seed;
+      if (prog_test_bind(la, args, idx, false, prog, seed)) {
+        m.run(seed, r);
+        if (lane == 0) prog_note_hit(args, idx, prog, r);
+      } else {
+        r = demi_fuzz_result{};
+        r.status = PS_SKIPPED;
+      }
+    } else {
+      if constexpr (PROG) prog_bind(la, args, idx, false);
+      m.run(args.seed_base + (int64_t)idx, r);
+    }
     const bool retry = args.ovf_list && (r.status == DEMI_PS_PENDING_OVF || r.status == DEMI_PS_NODE_OVF);
     if (retry) {
       if (lane == 0) { uint32_t pos = atomicAdd(args.ovf_count, 1u); args.ovf_list[pos] = (uint32_t)idx; }

@@ -587,13 +587,14 @@ struct LaneMachine {
 #endif
 // REC launches walk a work list (`index_list`): slot `it` of the list owns rec_events[it*rec_cap ..), rec_parent[it*cap ..),
 // rec_counts[it*4 ..) and results[it]; a deferred slot is handed to the general engine by POSITION (ovf_list holds `it`).
-// PROG (campaigns): prefix idx runs program idx of the arena in `args.prog_*` (see fuzz_kernel); the 0x80 | k entries
+// PROG (campaigns; with TESTS random-oracle tests, see fuzz_kernel): prefix idx runs its program of the arena in `args.prog_*`; the 0x80 | k entries
 // of messagesToSend resolve through that program's Send table.  A deferred prefix keeps its index, so the PROG
 // instantiation of the warp engine re-runs it on the same program.
-template <class MODEL, int BD, int LPCAP, bool REC = false, bool PROG = false>
+template <class MODEL, int BD, int LPCAP, bool REC = false, bool PROG = false, bool TESTS = false>
 __global__ void __launch_bounds__(BD, DEMI_K1_MIN_BLOCKS)
 fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
   static_assert(!(PROG && REC), "a campaign execution is recorded through demi_fuzz_trace on its program");
+  static_assert(PROG || !TESTS, "random-oracle tests bind their programs as campaigns do");
   using M = LaneMachine<MODEL, BD, LPCAP, REC>;
   extern __shared__ __align__(16) uint32_t lane_smem[];
   const uint32_t tid = threadIdx.x;
@@ -619,9 +620,20 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
       m.rec_par = args.rec_parent + it * (uint64_t)args.rec_parent_cap;
       m.rec_par[0] = 0;
     }
-    if constexpr (PROG) prog_bind(la, args, idx, true);
     demi_fuzz_result r;
-    m.run(args.seed_base + (int64_t)idx, r);
+    if constexpr (TESTS) {
+      uint64_t prog; int64_t seed;
+      if (prog_test_bind(la, args, idx, true, prog, seed)) {
+        m.run(seed, r);
+        prog_note_hit(args, idx, prog, r);
+      } else {
+        r = demi_fuzz_result{};
+        r.status = PS_SKIPPED;
+      }
+    } else {
+      if constexpr (PROG) prog_bind(la, args, idx, true);
+      m.run(args.seed_base + (int64_t)idx, r);
+    }
     if (r.status == LANE_DEFER) {
       uint32_t pos = atomicAdd(args.ovf_count, 1u);
       args.ovf_list[pos] = (uint32_t)(REC ? it : idx);

@@ -175,7 +175,15 @@ struct KernelArgs {
   int32_t  prog_model_key;             // the `model` argument of the capacity rules
   int32_t  prog_max_messages;          // max_messages as the caller gave it (the capacity rules read it unmapped)
   uint32_t prog_lane_pcap;             // lane engine: defer beyond this many pending messages (0 = no extra limit)
+  // random-oracle tests (demi_random_test_batch, the TESTS kernels): execution idx runs program idx / prog_execs under
+  // seed_base + idx % prog_execs; prog_first_hit[program] is the lowest execution index with a hit so far (atomicMin,
+  // 0xFFFFFFFF = none), and an execution whose index is above it is skipped (PS_SKIPPED)
+  uint32_t prog_execs;
+  uint32_t* prog_first_hit;
 };
+// the record status of an execution skipped because its program already has a hit at a lower index (never leaves
+// the device: the per-test reduction reads it)
+constexpr uint16_t PS_SKIPPED = 0xFFFEu;
 // The program view of a campaign execution: `la` is the executing thread's copy of the launch arguments.
 __device__ __forceinline__ void prog_bind(KernelArgs& la, const KernelArgs& args, uint64_t idx, bool lane) {
   const uint2 h = args.prog_hdr[idx];
@@ -186,6 +194,24 @@ __device__ __forceinline__ void prog_bind(KernelArgs& la, const KernelArgs& args
   la.tosend_cap = demi_tosend_cap(h.y);
   la.node_cap = demi_node_cap(demi_pending_cap(args.prog_model_key, args.prog_max_messages, h.y));
   la.ext_sends = args.prog_sends + idx * (uint64_t)args.prog_send_stride;
+}
+// A random-oracle test execution (the TESTS kernels): execution idx is execution j = idx % prog_execs of program
+// prog = idx / prog_execs, under seed_base + j.  Binds the program on every path (so that the copy stays in
+// registers) and returns false if the execution is skipped.  `lane`: one thread per execution (else a warp, kept
+// uniform).
+__device__ __forceinline__ bool prog_test_bind(KernelArgs& la, const KernelArgs& args, uint64_t idx, bool lane, uint64_t& prog,
+                                               int64_t& seed) {
+  const uint32_t p = (uint32_t)idx / args.prog_execs, j = (uint32_t)idx - p * args.prog_execs;
+  prog = p; seed = args.seed_base + (int64_t)j;
+  uint32_t fh = *(volatile const uint32_t*)(args.prog_first_hit + p);
+  if (!lane) fh = __shfl_sync(FULL_MASK, fh, 0);
+  prog_bind(la, args, p, lane);
+  return j <= fh;
+}
+// after a TESTS execution: a hit lowers its program's first_hit (the caller writes from one thread per execution)
+__device__ __forceinline__ void prog_note_hit(const KernelArgs& args, uint64_t idx, uint64_t prog, const demi_fuzz_result& r) {
+  if (r.status == 0 && r.violation)
+    atomicMin(args.prog_first_hit + prog, (uint32_t)idx - (uint32_t)prog * args.prog_execs);
 }
 
 // -----------------------------------------------------------------------------

@@ -276,6 +276,46 @@ class Engine(object):
                                        mcs.ctypes.data, mw, iters.ctypes.data, cap_iterations, C.byref(out)))
         return mcs, iters[:min(out.n_iterations, cap_iterations)].copy(), out
 
+    # ---- DDMin with RandomScheduler as the TestOracle (RunnerUtils.randomDDMin, RunnerUtils.scala:601-623)
+    def program_mask_words(self):
+        return max(1, (len(self._ext) + 63) // 64)
+
+    def random_test_batch(self, masks, n_execs, seed_base, max_messages, interval=0, looking_for=0):
+        """RandomScheduler.test of each mask's subsequence of the program (set_externals): N = n_execs executions,
+        execution j under FullyRandom(seed_base + j).  One RANDOM_TEST_DTYPE record per mask."""
+        mw = self.program_mask_words()
+        m = np.ascontiguousarray(masks, dtype=np.uint64).reshape(-1, mw)
+        out = np.zeros(len(m), dtype=N.RANDOM_TEST_DTYPE)
+        p = N.FuzzParams(seed_base, n_execs, max_messages, interval, looking_for or 0, 0)
+        self._check(N.lib().demi_random_test_batch(self._h, m.ctypes.data, len(m), mw, C.byref(p), out.ctypes.data))
+        return out
+
+    def random_ddmin(self, n_execs, seed_base, max_messages, looking_for, interval=0, check_unmodified=False,
+                     cap_iterations=1 << 16):
+        """demi_random_ddmin over the program: (MCS mask, iteration sizes, their keys, RandomDDMinOut)."""
+        mw = self.program_mask_words()
+        mcs = np.zeros(mw, dtype=np.uint64)
+        sizes = np.zeros(cap_iterations, dtype=np.uint32)
+        keys = np.zeros(cap_iterations, dtype=np.uint64)
+        out = N.RandomDDMinOut()
+        p = N.FuzzParams(seed_base, n_execs, max_messages, interval, looking_for or 0, 0)
+        self._check(N.lib().demi_random_ddmin(self._h, C.byref(p), 1 if check_unmodified else 0, mcs.ctypes.data, mw,
+                                              sizes.ctypes.data, keys.ctypes.data, cap_iterations, C.byref(out)))
+        n = min(out.n_iterations, cap_iterations)
+        return mcs, sizes[:n].copy(), keys[:n].copy(), out
+
+    def random_test_trace(self, mask, seed, max_messages, interval=0, looking_for=0, cap_events=65536):
+        """The EventTrace of execution `seed` of the mask's subsequence of the program (demi_random_test_trace): what
+        RandomScheduler.test returns for it.  Accepts adjacent WaitQuiescence.  (result, EventTrace)."""
+        m = np.ascontiguousarray(mask, dtype=np.uint64)
+        p = N.FuzzParams(seed, 1, max_messages, interval, looking_for or 0, 0)
+        ev = np.zeros(cap_events, dtype=N.EVENT_DTYPE)
+        n = C.c_uint32()
+        res = np.zeros(1, dtype=N.RESULT_DTYPE)
+        self._check(N.lib().demi_random_test_trace(self._h, m.ctypes.data, len(m), C.byref(p), seed, ev.ctypes.data,
+                                                   cap_events, C.byref(n), res.ctypes.data))
+        return res[0], ev[:n.value].copy()
+
     # ---- state-hash dedup + compaction (K5 / K4)
     def dedup_compact(self, results, mode=0):
         results = np.ascontiguousarray(results, dtype=N.RESULT_DTYPE)
@@ -616,7 +656,9 @@ class ReplayScheduler(STSScheduler):
 
 class DDMin(object):
     """DDMin(oracle, checkUnmodifed) — minification/DeltaDebugging.scala:7-109, with an
-    STSScheduler as the TestOracle (RunnerUtils.stsSchedDDMin, RunnerUtils.scala:642-707)."""
+    STSScheduler as the TestOracle (RunnerUtils.stsSchedDDMin, RunnerUtils.scala:642-707), or with a RandomScheduler
+    (RunnerUtils.randomDDMin, RunnerUtils.scala:601-623): minimize(violation, events) then minimizes `events`, the
+    whole program, WaitQuiescence included, with up to max_executions executions per test."""
 
     def __init__(self, oracle, checkUnmodifed=False, stats=None):
         self.oracle = oracle
@@ -632,16 +674,61 @@ class DDMin(object):
                 raise ValueError("No such external event:%r" % (e,))
         self.oracle.engine.conjoin_atoms(ext.index(e1), ext.index(e2))
 
-    def minimize(self, violation_fingerprint):
-        """Returns the MCS as a list of ExternalEvents (WaitQuiescence dropped, RunnerUtils.scala:678-684)."""
+    def minimize(self, violation_fingerprint, events=None):
+        """Returns the MCS as a list of ExternalEvents (under STSSched: WaitQuiescence dropped, RunnerUtils.scala:678-684)."""
+        if isinstance(self.oracle, RandomScheduler):
+            return self._minimize_random(violation_fingerprint, events)
         mcs, iters, out = self.oracle.engine.ddmin(violation_fingerprint, self.oracle.flags, self.checkUnmodifed)
         self._stats.record_series(iters)
         self._stats.total_replays = out.total_replays
         self.last = out
         return events_of(self.oracle.original_externals, mcs)
 
+    def _minimize_random(self, violation_fingerprint, events):
+        if events is None:
+            raise ValueError("DDMin over a RandomScheduler minimizes the `events` it is given")
+        o = self.oracle
+        if o.test_invariant is None:
+            raise ValueError("Must invoke setInvariant before test()")
+        events = list(events)
+        o.engine.set_externals(events)
+        self._stats.updateStrategy("DDMin", o.getName())
+        self._stats.record_prune_start()
+        mcs, sizes, keys, out = o.engine.random_ddmin(o.max_executions, o.seed, o.maxMessages, violation_fingerprint,
+                                                      o.invariant_check_interval, self.checkUnmodifed)
+        self._stats.record_prune_end()
+        base = self._stats.total_replays
+        for size, key in zip(sizes, keys):            # record_iteration_size keys by total_replays, counted in executions
+            self._stats.total_replays = base + int(key)
+            self._stats.record_iteration_size(size)
+        self._stats.total_replays = base + out.total_replays
+        self.last = out
+        return events_of(events, mcs)
+
     def verify_mcs(self, mcs, violation_fingerprint):
         return self.oracle.test(mcs, violation_fingerprint)
+
+
+def randomDDMin(schedulerConfig, trace, externals, violation, stats=None, max_executions=1, seed=0, engine=None):
+    """RunnerUtils.randomDDMin (RunnerUtils.scala:601-623) on a recorded experiment: `trace` is its EventTrace
+    (EVENT_DTYPE records), `externals` its program, `violation` the fingerprint code.  DDMin(RandomScheduler(
+    schedulerConfig, max_executions, seed), checkUnmodifed = false) with setMaxMessages(trace.size).  Returns
+    (MCS events, MinimizationStats, verified trace, violation); the verified trace is the EventTrace of the MCS's
+    first violating execution (None if it does not reproduce), or `trace` itself when nothing was pruned.
+    Execution j of every test runs FullyRandom(seed + j) (the reference keeps one Random running across tests)."""
+    sched = RandomScheduler(schedulerConfig, max_executions, 0, seed, engine=engine)
+    sched.setMaxMessages(len(trace))
+    ddmin = DDMin(sched, checkUnmodifed=False, stats=stats)
+    externals = list(externals)
+    mcs = ddmin.minimize(violation, externals)
+    if len(mcs) >= len(externals):
+        return mcs, ddmin._stats, trace, violation
+    out = ddmin.last                                  # verify_mcs ran in demi_random_ddmin (a throwaway stats object)
+    verified = None
+    if out.verified:
+        m = mask_of(externals, mcs)
+        _, verified = sched.engine.random_test_trace(m, seed + out.mcs_first_hit, len(trace), 0, violation)
+    return mcs, ddmin._stats, verified, violation
 
 
 class ProvenanceTracker:

@@ -355,6 +355,68 @@ int32_t demi_ddmin(demi_handle* h, uint32_t looking_for, uint32_t flags, int32_t
                    uint64_t* mcs_mask, uint32_t mask_words,
                    uint32_t* iteration_sizes, uint32_t cap_iterations, demi_ddmin_out* out);
 
+/* DDMin with a RandomScheduler as the TestOracle (RunnerUtils.randomDDMin, RunnerUtils.scala:601-623).  The dag is the
+ * handle's program (demi_set_externals) with every event in it, WaitQuiescence included: DDMin.minimize wraps the
+ * events in an UnmodifiedEventDag (Minimizer.scala:15-20).  Atoms as in demi_ddmin (Start..Kill, Partition..UnPartition;
+ * HardKill is a single atom); no conjoined atoms.
+ *
+ * A test is RandomScheduler.test(subsequence) (RandomScheduler.scala:597-612, explore :234-272): up to N =
+ * p->n_prefixes executions of the subsequence as written, which may leave WaitQuiescence adjacent, first or last (each
+ * runs as an empty quiescence segment).  Execution j of every test runs FullyRandom(p->seed_base + j), j < N: a
+ * documented deviation (the reference keeps one java.util.Random running across tests and executions), so that a
+ * test's outcome is a function of its subsequence alone.  p->max_messages, p->looking_for and
+ * p->invariant_check_interval are applied as in demi_fuzz_batch.
+ *
+ * first_hit is the lowest j whose execution ends with status 0 and a violation, -1 if none; executions_run is
+ * first_hit + 1, or N; status is the first nonzero DEMI_PS_* status among executions 0..executions_run-1 (the
+ * executions explore would have run); violation is the hit's code. */
+typedef struct {
+  int32_t  first_hit;
+  uint32_t executions_run;
+  uint32_t violation;
+  uint16_t status;
+  uint16_t reserved;
+} demi_random_test_result;
+/* n_tests masks of mask_words words each (bit i = event i of the handle's program).  Executions beyond a test's
+ * first hit may be skipped; the records are the same as without skipping.  demi_perf.prefixes is the number of
+ * executions that ran.  DEMI_ERR_STATE without a program; DEMI_ERR_INVALID for N = 0 or above 2^22, mask_words too
+ * small or null arguments. */
+int32_t demi_random_test_batch(demi_handle* h, const uint64_t* masks, uint32_t n_tests, uint32_t mask_words,
+                               const demi_fuzz_params* p, demi_random_test_result* out);
+/* The counters follow the reference's MinimizationStats, which count executions: explore calls increment_replays once
+ * per execution (:251-253) and record_iteration_size keys by total_replays (Minimizer.scala:183-185).  So
+ * total_replays is the sum of executions_run over the tests the sequential walk consumes, and iteration_sizes[i] is
+ * keyed by iteration_keys[i], the running sum after that test; the last entry is the fencepost (DeltaDebugging.scala:60).
+ * Sums of executions are 64-bit (N may be 2^22).  With check_unmodified the whole program is tested first and not
+ * counted (_stats.reset(), :48).  verify_mcs runs only if the MCS is shorter than the program (RunnerUtils.scala:
+ * 612-620): the MCS's own test, evaluated once (or taken from the tests already run) and not counted; verified = 1 when
+ * it reproduces, or when nothing was pruned (the original trace stands), and mcs_first_hit is that test's first_hit
+ * (-1 when it was not run or did not reproduce).  A test with a nonzero status fails the call with DEMI_ERR_CAPACITY
+ * only when the sequential walk (or verify_mcs) consumes it. */
+typedef struct {
+  uint32_t mcs_size;
+  uint32_t tests;                 /* tests the sequential walk consumed                                  */
+  uint32_t n_iterations;          /* entries of iteration_sizes / iteration_keys, fencepost included      */
+  uint32_t verified;
+  uint64_t total_replays;         /* executions those tests ran (stats.total_replays)                    */
+  uint64_t executions_executed;   /* executions that ran on the GPU, speculative tests included           */
+  uint32_t tests_evaluated;       /* tests evaluated on the GPU, speculative ones included                */
+  uint32_t batches;               /* speculative batches                                                  */
+  int32_t  mcs_first_hit;
+  uint32_t reserved;
+} demi_random_ddmin_out;
+int32_t demi_random_ddmin(demi_handle* h, const demi_fuzz_params* p, int32_t check_unmodified, uint64_t* mcs_mask,
+                          uint32_t mask_words, uint32_t* iteration_sizes, uint64_t* iteration_keys, uint32_t cap,
+                          demi_random_ddmin_out* out);
+/* The EventTrace RandomScheduler.test returns for a subsequence: execution `seed` of the mask's subsequence of the
+ * handle's program, recorded as demi_fuzz_trace records it (p->max_messages, p->looking_for and
+ * p->invariant_check_interval as there; p->seed_base and p->n_prefixes are not read).  Unlike demi_set_externals +
+ * demi_fuzz_trace it accepts the subsequences DDMin leaves, adjacent WaitQuiescence included; the handle's program is
+ * unchanged.  Errors as demi_fuzz_trace, DEMI_ERR_STATE without a program, DEMI_ERR_INVALID for mask_words too small. */
+int32_t demi_random_test_trace(demi_handle* h, const uint64_t* mask, uint32_t mask_words, const demi_fuzz_params* p,
+                               int64_t seed, demi_event* events, uint32_t cap_events, uint32_t* n_events,
+                               demi_fuzz_result* result);
+
 /* --------------------------------------------------------------------- DPOR */
 /* DPORwHeuristics(schedulerConfig, backtrackHeuristic = DefaultBacktrackOrdering,
  * depth_bound, stopIfViolationFound, trackHistory = true) driven like

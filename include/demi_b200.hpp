@@ -50,6 +50,7 @@ typedef std::vector<demi_event> EventTrace;
 inline uint32_t next_external_id() { static uint32_t id = 0; return ++id; }            // IDGenerator
 inline demi_ext_event Start(uint8_t name) { return {DEMI_EXT_START, name, 0, 0, 0, 0, next_external_id()}; }
 inline demi_ext_event Kill(uint8_t name) { return {DEMI_EXT_KILL, name, 0, 0, 0, 0, next_external_id()}; }
+inline demi_ext_event HardKill(uint8_t name) { return {DEMI_EXT_HARD_KILL, name, 0, 0, 0, 0, next_external_id()}; }
 inline demi_ext_event Send(uint8_t name, uint8_t type, uint32_t p0 = 0, uint32_t p1 = 0) {
   return {DEMI_EXT_SEND, name, 0, type, p0, p1, next_external_id()};
 }
@@ -255,6 +256,12 @@ class RandomScheduler {
   std::vector<demi_fuzz_result> results;
   std::vector<uint16_t> depGraph;      // depTracker.getGraph of the violating execution, as parent pointers
   uint32_t affectedNodes = 0;          // ... and its fingerprint's affectedNodes
+  // the test parameters DDMin uses when this scheduler is its oracle: N = max_executions, execution j under seed + j
+  demi_fuzz_params test_params(ViolationFingerprint fp) const {
+    return demi_fuzz_params{seed, max_executions, maxMessages, invariant_check_interval, fp, 0};
+  }
+  int64_t getSeed() const { return seed; }
+  int32_t getInvariantCheckInterval() const { return invariant_check_interval; }
  private:
   uint32_t max_executions; int32_t invariant_check_interval; int64_t seed;
   int32_t maxMessages = -1;                                           // Int.MaxValue (:54)
@@ -318,25 +325,88 @@ class ReplayScheduler : public STSScheduler {
 class DDMin {
  public:
   DDMin(STSScheduler& oracle, bool checkUnmodifed = false, MinimizationStats* stats = nullptr)
-      : oracle(oracle), checkUnmodifed(checkUnmodifed), _stats(stats ? stats : &own) {}
+      : _stats(stats ? stats : &own), oracle(&oracle), checkUnmodifed(checkUnmodifed) {}
+  // RunnerUtils.randomDDMin's DDMin (RunnerUtils.scala:601-623): a RandomScheduler as the TestOracle
+  DDMin(RandomScheduler& oracle, bool checkUnmodifed = false, MinimizationStats* stats = nullptr)
+      : _stats(stats ? stats : &own), random(&oracle), checkUnmodifed(checkUnmodifed) {}
   // the MCS (WaitQuiescence dropped, RunnerUtils.scala:678-684); throws std::invalid_argument
   // ("Unmodified trace does not trigger violation") like DeltaDebugging.scala:41-47
   ExternalEvents minimize(ViolationFingerprint fp) {
-    std::vector<uint64_t> mcs(oracle.mask_words(), 0);
+    if (!oracle) throw std::invalid_argument("DDMin over a RandomScheduler minimizes the events it is given");
+    std::vector<uint64_t> mcs(oracle->mask_words(), 0);
     std::vector<uint32_t> iters(1 << 16);
-    oracle.engine->check(demi_ddmin(oracle.engine->handle(), fp, oracle.flags, checkUnmodifed ? 1 : 0, mcs.data(),
-                                    oracle.mask_words(), iters.data(), (uint32_t)iters.size(), &last));
+    oracle->engine->check(demi_ddmin(oracle->engine->handle(), fp, oracle->flags, checkUnmodifed ? 1 : 0, mcs.data(),
+                                     oracle->mask_words(), iters.data(), (uint32_t)iters.size(), &last));
     _stats->iteration_size.clear();
     _stats->record_series(iters.data(), last.n_iterations, false);
     _stats->total_replays_ref() = last.total_replays;
-    return events_of(oracle.original_externals, mcs);
+    return events_of(oracle->original_externals, mcs);
   }
-  std::optional<EventTrace> verify_mcs(const ExternalEvents& mcs, ViolationFingerprint fp) { return oracle.test(mcs, fp); }
+  // over a RandomScheduler: the whole program `events`, WaitQuiescence included (demi_random_ddmin).  MinimizationStats
+  // counts executions: each iteration size is keyed by the running sum of the executions the tests ran.
+  ExternalEvents minimize(ViolationFingerprint fp, const ExternalEvents& events) {
+    if (!random) return minimize(fp);
+    Engine& e = *random->engine;
+    e.check(demi_set_externals(e.handle(), events.data(), (uint32_t)events.size()));
+    const uint32_t mw = events.size() ? (uint32_t)((events.size() + 63) / 64) : 1u;
+    std::vector<uint64_t> mcs(mw, 0), keys(1 << 16);
+    std::vector<uint32_t> sizes(1 << 16);
+    const demi_fuzz_params p = random->test_params(fp);
+    e.check(demi_random_ddmin(e.handle(), &p, checkUnmodifed ? 1 : 0, mcs.data(), mw, sizes.data(), keys.data(),
+                              (uint32_t)sizes.size(), &last_random));
+    _stats->updateStrategy("DDMin", random->getName());
+    const uint32_t base = _stats->total_replays_ref();
+    const uint32_t n = std::min<uint32_t>(last_random.n_iterations, (uint32_t)sizes.size());
+    for (uint32_t i = 0; i < n; i++) {
+      _stats->total_replays_ref() = base + (uint32_t)keys[i];
+      _stats->record_iteration_size(sizes[i]);
+    }
+    _stats->total_replays_ref() = base + (uint32_t)last_random.total_replays;
+    return events_of(events, mcs);
+  }
+  std::optional<EventTrace> verify_mcs(const ExternalEvents& mcs, ViolationFingerprint fp) {
+    if (random) return random->test(mcs, fp);
+    return oracle->test(mcs, fp);
+  }
   demi_ddmin_out last{};
+  demi_random_ddmin_out last_random{};
   MinimizationStats* _stats;
  private:
-  STSScheduler& oracle; bool checkUnmodifed; MinimizationStats own;
+  STSScheduler* oracle = nullptr;
+  RandomScheduler* random = nullptr;
+  bool checkUnmodifed; MinimizationStats own;
 };
+
+// RunnerUtils.randomDDMin (RunnerUtils.scala:601-623) on a recorded experiment: DDMin(RandomScheduler(cfg,
+// max_executions, seed), checkUnmodifed = false) with setMaxMessages(trace.size).  Returns (MCS, stats, verified trace,
+// violation); the verified trace is the EventTrace of the MCS's first violating execution (nullopt when it does not
+// reproduce), or `trace` itself when nothing was pruned.  Execution j of every test runs FullyRandom(seed + j).
+struct RandomDDMinResult {
+  ExternalEvents mcs; MinimizationStats stats; std::optional<EventTrace> verified; ViolationFingerprint violation;
+  demi_random_ddmin_out out;
+};
+inline RandomDDMinResult randomDDMin(const SchedulerConfig& cfg, const EventTrace& trace, const ExternalEvents& externals,
+                                     ViolationFingerprint violation, uint32_t max_executions = 1, int64_t seed = 0,
+                                     std::shared_ptr<Engine> engine = nullptr) {
+  RandomScheduler sched(cfg, max_executions, 0, seed, engine);
+  sched.setMaxMessages((int32_t)trace.size());
+  RandomDDMinResult r;
+  DDMin ddmin(sched, false, &r.stats);
+  r.mcs = ddmin.minimize(violation, externals);
+  r.out = ddmin.last_random;
+  r.violation = violation;
+  if (r.mcs.size() >= externals.size()) { r.verified = trace; return r; }
+  if (!r.out.verified) return r;
+  const std::vector<uint64_t> m = mask_of(externals, r.mcs);
+  const demi_fuzz_params p = sched.test_params(violation);
+  EventTrace ev(65536);
+  uint32_t n = 0; demi_fuzz_result res{};
+  sched.engine->check(demi_random_test_trace(sched.engine->handle(), m.data(), (uint32_t)m.size(), &p,
+                                             seed + r.out.mcs_first_hit, ev.data(), (uint32_t)ev.size(), &n, &res));
+  ev.resize(n);
+  r.verified = ev;
+  return r;
+}
 
 struct LeftToRightOneAtATime {};       // RemovalStrategy (OneAtATimeRemoval.scala:131-137)
 struct SrcDstFIFORemoval {};           // RemovalStrategy (OneAtATimeRemoval.scala:139-251)

@@ -190,6 +190,20 @@ JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_fuzzCampaign(J
     jlong programSeedBase, jobject out) {
   return demi_fuzz_campaign(H(h), (const demi_fuzz_params*)BUF(env, params), (int64_t)programSeedBase, (demi_fuzz_result*)BUF(env, out));
 }
+/* demi_random_ddmin / demi_random_test_trace: RunnerUtils.randomDDMin, DDMin with a RandomScheduler as the TestOracle,
+ * over the program of setExternals (the verified trace: randomTestTrace on the MCS mask at seed + mcs_first_hit) */
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_randomDDMin(JNIEnv* env, jclass c, jlong h, jobject params,
+    jint checkUnmodified, jobject mcsMask, jint maskWords, jobject iterationSizes, jobject iterationKeys, jint cap, jobject out) {
+  return demi_random_ddmin(H(h), (const demi_fuzz_params*)BUF(env, params), checkUnmodified, (uint64_t*)BUF(env, mcsMask),
+                           (uint32_t)maskWords, iterationSizes ? (uint32_t*)BUF(env, iterationSizes) : 0,
+                           iterationKeys ? (uint64_t*)BUF(env, iterationKeys) : 0, (uint32_t)cap, (demi_random_ddmin_out*)BUF(env, out));
+}
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_randomTestTrace(JNIEnv* env, jclass c, jlong h, jobject mask,
+    jint maskWords, jobject params, jlong seed, jobject events, jint capEvents, jobject count, jobject result) {
+  return demi_random_test_trace(H(h), (const uint64_t*)BUF(env, mask), (uint32_t)maskWords, (const demi_fuzz_params*)BUF(env, params),
+                                (int64_t)seed, (demi_event*)BUF(env, events), (uint32_t)capEvents, (uint32_t*)BUF(env, count),
+                                (demi_fuzz_result*)BUF(env, result));
+}
 /* `exp` = a direct buffer laid out as demi_experiment whose pointer fields the Scala side fills with
  * GetDirectBufferAddress-style addresses (DemiNative.addressOf) */
 JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_experimentSave(JNIEnv* env, jclass c, jstring dir, jobject exp) {

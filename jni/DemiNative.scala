@@ -68,6 +68,13 @@ object DemiNative {
   /** demi_set_fuzzer / demi_fuzz_campaign: RunnerUtils.fuzz's loop (RunnerUtils.scala:75-91), a new program per execution */
   @native def setFuzzer(h: Long, cfg: ByteBuffer, prefix: ByteBuffer, nPrefix: Int, postfix: ByteBuffer, nPostfix: Int): Int
   @native def fuzzCampaign(h: Long, params: ByteBuffer, programSeedBase: Long, out: ByteBuffer): Int
+  /** demi_random_ddmin: RunnerUtils.randomDDMin (RunnerUtils.scala:601-623), DDMin over RandomScheduler.test; params =
+    * demi_fuzz_params with n_prefixes = max_executions.  iterationKeys: uint64 running sums of executions. */
+  @native def randomDDMin(h: Long, params: ByteBuffer, checkUnmodified: Int, mcsMask: ByteBuffer, maskWords: Int,
+                          iterationSizes: ByteBuffer, iterationKeys: ByteBuffer, cap: Int, out: ByteBuffer): Int
+  /** demi_random_test_trace: the EventTrace RandomScheduler.test returns for a subsequence (the verified MCS trace) */
+  @native def randomTestTrace(h: Long, mask: ByteBuffer, maskWords: Int, params: ByteBuffer, seed: Long, events: ByteBuffer,
+                              capEvents: Int, count: ByteBuffer, result: ByteBuffer): Int
   /** The flat experiment directory that replaces ExperimentSerializer's *.bin object streams (Serialization.scala:57-74). */
   @native def experimentSave(dir: String, exp: ByteBuffer): Int
   @native def experimentLoad(dir: String, exp: ByteBuffer): Int
