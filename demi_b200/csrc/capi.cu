@@ -89,6 +89,20 @@ extern "C" const char* demi_last_error(const demi_handle* h) {
   return h ? h->err.c_str() : g_create_error.c_str();
 }
 
+#if DEMI_K1_PHASE_CLOCK
+// The lane engine's phase sums ([phase][cycles, active lanes, entries], LanePhase order) of every launch since the
+// last reset; only a library built with DEMI_K1_PHASE_CLOCK has this symbol.
+extern "C" int32_t demi_k1_phase_read(unsigned long long* out, int32_t reset) {
+  if (cudaDeviceSynchronize() != cudaSuccess) return DEMI_ERR_CUDA;
+  if (out && cudaMemcpyFromSymbol(out, demi_k1_phase_sums, sizeof(demi_k1_phase_sums)) != cudaSuccess) return DEMI_ERR_CUDA;
+  if (reset) {
+    static const unsigned long long zero[LP_COUNT * 3] = {};
+    if (cudaMemcpyToSymbol(demi_k1_phase_sums, zero, sizeof(zero)) != cudaSuccess) return DEMI_ERR_CUDA;
+  }
+  return LP_COUNT;
+}
+#endif
+
 extern "C" int32_t demi_device_count(void) {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }

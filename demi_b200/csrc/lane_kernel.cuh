@@ -40,8 +40,51 @@ namespace demi {
 #ifndef DEMI_K1_LPCAP_RAFT5
 #define DEMI_K1_LPCAP_RAFT5 96
 #endif
+#ifndef DEMI_K1_PHASE_CLOCK
+#define DEMI_K1_PHASE_CLOCK 0    // profiling builds only (tools/profile_lane_phases.py): per-phase clock64() sums
+#endif
 
 constexpr uint32_t LANE_DEFER = 0xFFFFu;      // internal status: hand over to the warp engine
+
+// The phase clock.  Lane 0 of each warp keeps, per phase of an execution step, the clock64() cycles from the phase's
+// entry to the next phase's entry, the active lanes at the entry (__popc(__activemask())) and the number of entries.
+// The warp adds them to demi_k1_phase_sums when it finishes; demi_k1_phase_read (capi.cu) copies them out.  Lanes
+// that diverge from lane 0 are seen only through lane 0's waits, so the figures say what the warp pays per phase.
+enum LanePhase : uint32_t { LP_FLUSH, LP_PICK, LP_RECEIVE, LP_SEND, LP_CANCEL, LP_SCHEDULE, LP_INVARIANT, LP_TAIL, LP_COUNT };
+#if DEMI_K1_PHASE_CLOCK
+static __device__ unsigned long long demi_k1_phase_sums[LP_COUNT * 3];     // [phase][cycles, lanes, entries]
+#endif
+struct LanePhaseClock {
+#if DEMI_K1_PHASE_CLOCK
+  unsigned long long cyc[LP_COUNT], lanes[LP_COUNT], n[LP_COUNT], t0;
+  uint32_t cur;
+  __device__ __forceinline__ void start() {
+    for (int p = 0; p < LP_COUNT; p++) cyc[p] = lanes[p] = n[p] = 0;
+    cur = LP_TAIL; t0 = clock64();
+  }
+  __device__ __forceinline__ void enter(uint32_t p) {
+    const uint32_t act = __activemask();
+    if ((threadIdx.x & 31u) == 0) {
+      const unsigned long long now = clock64();
+      cyc[cur] += now - t0; t0 = now; cur = p;
+      lanes[p] += __popc(act); n[p]++;
+    }
+  }
+  __device__ __forceinline__ void finish() {
+    enter(LP_TAIL);
+    if ((threadIdx.x & 31u) == 0)
+      for (int p = 0; p < LP_COUNT; p++) {
+        atomicAdd(&demi_k1_phase_sums[p * 3 + 0], cyc[p]);
+        atomicAdd(&demi_k1_phase_sums[p * 3 + 1], lanes[p]);
+        atomicAdd(&demi_k1_phase_sums[p * 3 + 2], n[p]);
+      }
+  }
+#else
+  __device__ __forceinline__ void start() {}
+  __device__ __forceinline__ void enter(uint32_t) {}
+  __device__ __forceinline__ void finish() {}
+#endif
+};
 
 // The pending arrays are the only data this kernel re-reads from global memory; the result records are written once.
 // An L2 evict_last policy on the former (and evict-first stores for the latter) keeps the arrays cache-resident, so
@@ -153,6 +196,10 @@ struct LaneDirectOutbox {
   __device__ __forceinline__ void schedule_repeating(uint32_t type, uint32_t p0, uint32_t p1) { m->schedule_timer(OP_SCHED_REPEAT, self, type, p0, p1); }
   __device__ __forceinline__ void cancel_timer(uint32_t type, uint32_t p0, uint32_t p1) { m->cancel_timer(self, type, p0, p1); }
 };
+template <class M>
+__device__ __forceinline__ void receive_phase(LaneDirectOutbox<M>& o, uint32_t rp) {
+  o.m->clk.enter(rp == RP_CANCEL ? LP_CANCEL : rp == RP_SEND ? LP_SEND : LP_SCHEDULE);
+}
 
 // REC: the execution's EventTrace and DepTracker parents are written out (provenance batches, demi_fuzz_provenance)
 template <class MODEL, int BD, int LPCAP, bool REC = false>
@@ -163,7 +210,9 @@ struct LaneMachine {
   // the outbox is staged in shared memory only when receive()'s operations are not applied as they are issued
   static constexpr bool DIRECT = DEMI_K1_DIRECT_OUTBOX && MODEL::LANE_SENDS_DISTINCT;
   static constexpr int OBW = DIRECT ? 0 : OB * 3;
-  static constexpr int WORDS = N * SW + OBW + N;       // states + outbox + partition rows
+  static constexpr uint32_t CT = MODEL::LANE_CANCEL_TYPE;            // 0: receive() cancels no timer
+  static constexpr int TW = CT ? (N + 1) / 2 : 0;
+  static constexpr int WORDS = N * SW + OBW + N + TW;      // states + outbox + partition rows + cancellable timer copies
 
   uint32_t* smw;             // &smem[tid]; word w at smw[w*BD]
   uint4* pend;               // entry i at pend[i*32]
@@ -189,8 +238,23 @@ struct LaneMachine {
   // the trace hash term of the next send with its dst, type, p0 and p1 words left out
   bool sends_open;
   uint64_t send_lin;
+  LanePhaseClock clk;        // empty unless DEMI_K1_PHASE_CLOCK
 
   __device__ __forceinline__ uint32_t& part_row(uint32_t a) { return smw[(N * SW + OBW + a) * BD]; }
+  // Where the timer message of type CT (the one timer receive() cancels) of each actor is in the pending array, so that
+  // Cancellable.cancel need not scan for it: 16 bits per actor (actor a in half a & 1 of word a >> 1), the low byte the
+  // number of its copies in the array, the high byte the index of the copy when there is exactly one and it is known
+  // (0xFF otherwise: after 2 -> 1 it is not).  Only timer_produced inserts timer messages (an external with a timer's
+  // key defers) and every removal goes through pending_remove_at, so these are exact.  Other timers are not tracked:
+  // the check on each removal is one compare of the header's flags and type.
+  __device__ __forceinline__ uint32_t& tcopy_word(uint32_t a) { return smw[(N * SW + OBW + N + (a >> 1)) * BD]; }
+  __device__ __forceinline__ uint32_t tcopy(uint32_t a) { return (tcopy_word(a) >> ((a & 1u) * 16)) & 0xFFFFu; }
+  __device__ __forceinline__ void tcopy_set(uint32_t a, uint32_t e) {
+    uint32_t& w = tcopy_word(a);
+    const uint32_t sh = (a & 1u) * 16;
+    w = (w & ~(0xFFFFu << sh)) | (e << sh);
+  }
+  __device__ __forceinline__ static bool cancellable_timer(uint32_t hdr) { return (hdr >> 16) == ((DEMI_MF_TIMER << 8) | CT); }
   __device__ __forceinline__ LaneState actor(uint32_t a) { return LaneState{smw + a * SW * BD, BD}; }
 
   __device__ __forceinline__ void defer() { status = LANE_DEFER; }
@@ -231,6 +295,16 @@ struct LaneMachine {
     uint4 last = ld_l2_hint(pend + (n_pending - 1) * 32, pol);
     st_l2_hint(pend + i * 32, last, pol);
     n_pending--;
+    if constexpr (CT != 0) {
+      if (cancellable_timer(v.x)) {
+        const uint32_t a = hdr_dst(v.x);
+        tcopy_set(a, ((tcopy(a) & 0xFFu) - 1u) | 0xFF00u);
+      }
+      if (cancellable_timer(last.x)) {                   // moved from index n_pending to i
+        const uint32_t a = hdr_dst(last.x), e = tcopy(a);
+        if ((e >> 8) == n_pending) tcopy_set(a, (e & 0xFFu) | (i << 8));
+      }
+    }
     return v;
   }
 
@@ -301,6 +375,11 @@ struct LaneMachine {
     if (!crosses_partition(DEMI_DEADLETTERS, dst)) {
       pending_insert(make_uint4(make_hdr(DEMI_DEADLETTERS, dst, type, DEMI_MF_TIMER), p0, p1, w3));
       if (status) return;
+      if constexpr (CT != 0)
+        if (type == CT) {
+          const uint32_t n = tcopy(dst) & 0xFFu;
+          tcopy_set(dst, n == 0 ? (1u | (n_pending - 1) << 8) : ((n + 1) | 0xFF00u));
+        }
     }
     record_event(DEMI_EV_MSG_SEND, DEMI_TIMER_SND, dst, type, p0, p1, w3, parent_event);
   }
@@ -389,8 +468,16 @@ struct LaneMachine {
     registry &= ~bit;
     for (uint32_t i = 0; i < tosend.n; i++)           // handle_timer_cancel (ExternalEventInjector.scala:601-610)
       if (tosend.get(i) == (uint32_t)slot) { tosend.remove_at(i); return; }
-    // FullyRandom.remove (RandomScheduler.scala:653-664): first match in array order.  Four entries are fetched per
-    // step so that their latencies overlap (this scan was 6 % of the kernel's stall samples when it fetched one).
+    // FullyRandom.remove (RandomScheduler.scala:653-664): first match in array order.  The only entries that match are
+    // the slot's timer messages: for the tracked type CT, with none pending there is nothing to remove, and a single
+    // copy at a known index is the first match.  Otherwise the array is scanned, four entries fetched per step so that
+    // their latencies overlap (this scan was 6 % of the kernel's stall samples when it fetched one).
+    if constexpr (CT != 0)
+      if (type == CT) {
+        const uint32_t e = tcopy(self);
+        if ((e & 0xFFu) == 0) return;
+        if ((e >> 8) != 0xFFu) { pending_remove_at(e >> 8); return; }
+      }
     const uint32_t want = make_hdr(DEMI_DEADLETTERS, self, type, 0);
 #pragma unroll 1
     for (uint32_t i = 0; i < n_pending; i += 4) {
@@ -528,6 +615,8 @@ struct LaneMachine {
 #pragma unroll 1
     for (uint32_t i = 0; i < N * SW; i++) smw[i * BD] = MODEL::init_word(i, A->model_flags);
     for (uint32_t a = 0; a < N; a++) part_row(a) = 0;
+    if constexpr (TW > 0)
+      for (uint32_t w = 0; w < (uint32_t)TW; w++) smw[(N * SW + OBW + N + w) * BD] = 0;
     n_pending = max_pending = 0;
     tosend.clear(); resend = 0; n_resend = 0;
     just = registry = cancelled = root_timers = window_timers = 0;
@@ -539,20 +628,26 @@ struct LaneMachine {
   }
 
   __device__ __forceinline__ void run(int64_t seed, demi_fuzz_result& out) {
+    clk.enter(LP_TAIL);
     reset(seed);
     uint32_t n_ops = 0, self = 0;          // outbox of the delivery that has not been drained yet
     for (;;) {
       inject_until_quiescence();
       for (;;) {
+        clk.enter(LP_INVARIANT);
         const bool go = may_continue();
+        clk.enter(LP_FLUSH);
         drain(n_ops, self, go);            // previous receive()'s sends, then (if going on) the flush
         n_ops = 0;
         uint4 pick;
+        clk.enter(LP_PICK);
         if (!go || !pick_next(pick)) break;
         self = hdr_dst(pick.x);
+        clk.enter(LP_RECEIVE);
         n_ops = dispatch_new_message(pick);
         if (status) break;
       }
+      clk.enter(LP_TAIL);
       if (status | violation) break;
       if (ext_idx < A->n_ext) {
         record_event(DEMI_EV_QUIESCENCE, DEMI_DEADLETTERS, DEMI_DEADLETTERS, 0, 0, 0, 0, 0);
@@ -609,6 +704,7 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
   if constexpr (PROG) { la = args; m.A = &la; } else m.A = &args;
   m.pol = l2_evict_last_policy();
   m.rec_ev = nullptr; m.rec_par = nullptr;
+  m.clk.start();
 
   const uint64_t count = (REC && args.index_list) ? (uint64_t)(*args.index_count) : args.n_prefixes;
   unsigned long long my_steps = 0;
@@ -662,6 +758,7 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
       my_viol += r.violation ? 1u : 0u;
     }
   }
+  m.clk.finish();
   // warp-aggregate the summary counters
   for (int o = 16; o > 0; o >>= 1) {
     my_steps += __shfl_xor_sync(FULL_MASK, my_steps, o);

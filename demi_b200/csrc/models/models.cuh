@@ -21,10 +21,18 @@
 //   timer_slot / slot_msg                    lane engine: the model's finite timer
 //                                            universe (<= 32 (receiver,msg) keys)
 //   LANE_OUTBOX                              lane engine: max ops of one receive()
+//   LANE_CANCEL_TYPE                         lane engine: the message type of the timers receive() may
+//                                            cancel, one slot per receiver (p0 = p1 = 0); 0: none
 #pragma once
 #include "../machine.cuh"
 
 namespace demi {
+
+// The points between a receive()'s handler, its cancel, its sends and its schedule.  An outbox that profiles them
+// (the lane engine's phase clock) overloads receive_phase; for every other outbox it is nothing.
+enum { RP_CANCEL = 0, RP_SEND = 1, RP_SCHEDULE = 2 };
+template <class O>
+__device__ __forceinline__ void receive_phase(O&, uint32_t) {}
 
 // ---------------------------------------------------------------- pingpong3
 // BASELINE.json configs[0].  Ping(k) to X => X sends Pong(k) to (X+1)%3.
@@ -37,6 +45,7 @@ struct PingPong3 {
   __device__ static __forceinline__ uint32_t init_word(uint32_t, uint32_t) { return 0; }
   static constexpr int LANE_OUTBOX = 2;
   static constexpr bool LANE_SENDS_DISTINCT = false;
+  static constexpr uint32_t LANE_CANCEL_TYPE = 0;
   static constexpr int REPLAY_OUTBOX = 2;
   template <class S, class O>
   __device__ static __forceinline__ void receive(O& out, uint32_t self, S st, uint32_t /*src*/,
@@ -91,6 +100,7 @@ struct Raft5 {
   // every receive() sends at most one message to each receiver (votes / AppendEntries per peer, one reply), so no two
   // sends of one delivery are equal and the lane engine's duplicate-send screen is skipped
   static constexpr bool LANE_SENDS_DISTINCT = true;
+  static constexpr uint32_t LANE_CANCEL_TYPE = HEARTBEAT_TICK;     // the only timer receive() cancels
   static constexpr int REPLAY_OUTBOX = 6;
   // timer universe: (actor, ELECTION_TICK) -> 2*actor, (actor, HEARTBEAT_TICK) -> 2*actor+1
   __device__ static __forceinline__ int timer_slot(uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) {
@@ -215,19 +225,34 @@ struct Raft5 {
         if (t < c[TERM]) { plan_p0 = (uint32_t)c[TERM]; break; }
         if (t > c[TERM] || c[ROLE] != FOLLOWER) cancel_heartbeat = step_down(c, t);
         c[HEARD] = 1;
-        bool ok = prev <= c[LOGLEN] && (prev == 0 || s[LOGTERM + prev - 1] == pt);
+        // The log as two 64-bit words, entry k in byte k: LOGTERM (state words 2-3) and LOGVAL (4-5).  LOGLEN <= LOG_CAP
+        // always, so with prev <= LOGLEN every entry read or written here is inside them.
+        const uint32_t len = c[LOGLEN];
+        uint64_t lt = (uint64_t)s.w(2) | (uint64_t)s.w(3) << 32;
+        bool ok = prev <= len && (prev == 0 || ((lt >> (8 * (prev - 1))) & 0xFFu) == pt);
         if (!ok) { plan_p0 = (uint32_t)c[TERM]; break; }
         uint32_t mi = prev;
         if (has) {
-          if (c[LOGLEN] > prev && s[LOGTERM + prev] != et) {          // conflict: truncate
-            for (uint32_t k = prev; k < LOG_CAP; k++) { s[LOGTERM + k] = 0; s[LOGVAL + k] = 0; }
-            c[LOGLEN] = (uint8_t)prev;
+          uint64_t lv = (uint64_t)s.w(4) | (uint64_t)s.w(5) << 32;
+          uint32_t nlen = len;
+          bool changed = false;
+          if (len > prev && ((lt >> (8 * prev)) & 0xFFu) != et) {        // conflict: truncate entries prev..LOG_CAP-1
+            const uint64_t keep = (1ull << (8 * prev)) - 1ull;            // prev < len <= LOG_CAP
+            lt &= keep; lv &= keep;
+            nlen = prev; changed = true;
           }
-          if (c[LOGLEN] == prev && prev < LOG_CAP) {
-            s[LOGTERM + prev] = (uint8_t)et; s[LOGVAL + prev] = (uint8_t)ev;
-            c[LOGLEN] = (uint8_t)(prev + 1);
+          if (nlen == prev && prev < LOG_CAP) {
+            const uint32_t sh = 8 * prev;
+            lt = (lt & ~(0xFFull << sh)) | ((uint64_t)et << sh);
+            lv = (lv & ~(0xFFull << sh)) | ((uint64_t)ev << sh);
+            nlen = prev + 1; changed = true;
           }
-          if (c[LOGLEN] > prev) mi = prev + 1;
+          if (changed) {
+            s.w(2) = (uint32_t)lt; s.w(3) = (uint32_t)(lt >> 32);
+            s.w(4) = (uint32_t)lv; s.w(5) = (uint32_t)(lv >> 32);
+            c[LOGLEN] = nlen;
+          }
+          if (nlen > prev) mi = prev + 1;
         }
         uint32_t nc = lc < mi ? lc : mi;
         if (nc > c[COMMIT]) c[COMMIT] = (uint8_t)nc;
@@ -241,12 +266,24 @@ struct Raft5 {
         if (ok) {
           if (mi > s[MATCH + src]) s[MATCH + src] = (uint8_t)mi;
           if (mi > s[NEXT + src]) s[NEXT + src] = (uint8_t)mi;
-          for (uint32_t idx = c[LOGLEN]; idx > c[COMMIT]; idx--) {
-            if (s[LOGTERM + idx - 1] != c[TERM] && !(flags & BUG_STALE_COMMIT)) continue;
-            uint32_t cnt = 1;
-            for (uint32_t k = 0; k < 5; k++) if (k != self && s[MATCH + k] >= idx) cnt++;
-            if (cnt >= 3) { c[COMMIT] = (uint8_t)idx; break; }
+          // The largest idx in (COMMIT, LOGLEN] whose entry is of this term (any entry with BUG_STALE_COMMIT) and that
+          // two peers match, as bit idx-1 of masks over the (at most LOG_CAP) entries.  A peer's MATCH >= idx for the
+          // low min(MATCH, LOG_CAP) bits; `two` keeps the bits that two peers have.  MATCH is bytes 1-3 of word 7
+          // and bytes 0-1 of word 8.
+          const uint32_t m03 = __funnelshift_r(s.w(7), s.w(8), 8), m4 = (s.w(8) >> 8) & 0xFFu;
+          uint32_t one = 0, two = 0;
+#pragma unroll
+          for (uint32_t k = 0; k < 5; k++) {
+            const uint32_t m = k < 4 ? (m03 >> (8 * k)) & 0xFFu : m4;
+            const uint32_t bits = k == self ? 0u : (1u << (m < LOG_CAP ? m : LOG_CAP)) - 1u;
+            two |= one & bits; one |= bits;
           }
+          const uint32_t rep = (uint32_t)c[TERM] * 0x01010101u;
+          const uint32_t same_term = (flags & BUG_STALE_COMMIT) ? 0xFFu
+              : byte_msbs(__vcmpeq4(s.w(2), rep)) | byte_msbs(__vcmpeq4(s.w(3), rep)) << 4;
+          const uint32_t len = c[LOGLEN], cm = c[COMMIT];
+          const uint32_t cand = same_term & two & ((1u << len) - 1u) & ~((1u << (cm < LOG_CAP ? cm : LOG_CAP)) - 1u);
+          if (cand) c[COMMIT] = 32u - __clz(cand);
         } else if (s[NEXT + src] > 0) {
           s[NEXT + src]--;
         }
@@ -254,7 +291,9 @@ struct Raft5 {
       }
       default: break;
     }
+    receive_phase(out, RP_CANCEL);
     if (cancel_heartbeat) out.cancel_timer(HEARTBEAT_TICK, 0, 0);
+    receive_phase(out, RP_SEND);
     // A broadcast goes to the four peers in ascending order: trip k sends to k + (k >= self), so no trip is spent on
     // skipping `self`.  The outbox is told the number of sends first (out.reserve), so an engine that applies them as
     // they are issued checks its capacities once per delivery; it returns false when they do not fit (the execution
@@ -278,6 +317,7 @@ struct Raft5 {
         out.send(j, qt, q0, q1);
       }
     }
+    receive_phase(out, RP_SCHEDULE);
     if (sched) out.schedule_repeating(sched, 0, 0);
   }
 
@@ -311,23 +351,46 @@ struct Raft5 {
       }
     return 0;
   }
+  // the low n bytes of a word (n >= 4: all of it)
+  __device__ static __forceinline__ uint32_t low_bytes(uint32_t n) { return n >= 4 ? 0xFFFFFFFFu : (1u << (n * 8)) - 1u; }
+  // bit k = the top bit of byte k (the four products land on bits 24-27 and never overlap)
+  __device__ static __forceinline__ uint32_t byte_msbs(uint32_t x) { return (((x >> 7) & 0x01010101u) * 0x01020408u) >> 24; }
+  // Code 1 if some pair is two leaders in one term, else 2 if some pair's committed prefixes disagree.  Word 0 of the
+  // five actors (ROLE, TERM) is loaded once and the ten pairs are compared in registers; the logs are compared only
+  // when two actors have committed something, a pair's first c = min(COMMIT) entries as masked LOGTERM and LOGVAL
+  // words (words 2-3 and 4-5).
   template <class A>
   __device__ static __forceinline__ uint32_t invariant(A all, uint32_t) {
-    uint32_t code = 0;
-#pragma unroll 1
+    uint32_t w0[5], committed = 0;
+#pragma unroll
+    for (uint32_t i = 0; i < 5; i++) {
+      w0[i] = all.actor(i).w(0);
+      committed |= ((all.actor(i).w(1) >> 8) & 0xFFu) ? 1u << i : 0u;
+    }
+    bool two_leaders = false;
+#pragma unroll
     for (uint32_t i = 0; i < 5; i++)
+#pragma unroll
+      for (uint32_t j = i + 1; j < 5; j++)
+        two_leaders |= (w0[i] & 0xFFu) == LEADER && ((w0[i] ^ w0[j]) & 0xFFFFu) == 0;
+    if (two_leaders) return 1;
+    if (__popc(committed) < 2) return 0;
+#pragma unroll 1
+    for (uint32_t i = 0; i < 4; i++) {
+      if (!((committed >> i) & 1u)) continue;
+      auto a = all.actor(i);
+      const uint32_t ca = (a.w(1) >> 8) & 0xFFu;
+      const uint32_t t0 = a.w(2), t1 = a.w(3), v0 = a.w(4), v1 = a.w(5);
 #pragma unroll 1
       for (uint32_t j = i + 1; j < 5; j++) {
-        auto a = all.actor(i);
+        if (!((committed >> j) & 1u)) continue;
         auto b = all.actor(j);
-        if (a[ROLE] == LEADER && b[ROLE] == LEADER && a[TERM] == b[TERM]) return 1;
-        if (code) continue;
-        uint32_t c = a[COMMIT] < b[COMMIT] ? a[COMMIT] : b[COMMIT];
-#pragma unroll 1
-        for (uint32_t k = 0; k < c; k++)
-          if (a[LOGTERM + k] != b[LOGTERM + k] || a[LOGVAL + k] != b[LOGVAL + k]) code = 2;
+        const uint32_t cb = (b.w(1) >> 8) & 0xFFu, c = ca < cb ? ca : cb;
+        const uint32_t m0 = low_bytes(c), m1 = low_bytes(c > 4 ? c - 4 : 0u);
+        if ((((t0 ^ b.w(2)) | (v0 ^ b.w(4))) & m0) | (((t1 ^ b.w(3)) | (v1 ^ b.w(5))) & m1)) return 2;
       }
-    return code;
+    }
+    return 0;
   }
 };
 
@@ -352,6 +415,7 @@ struct Bcast32 {
   static constexpr int REPLAY_OUTBOX = 32;
   static constexpr int LANE_OUTBOX = 32;
   static constexpr bool LANE_SENDS_DISTINCT = false;
+  static constexpr uint32_t LANE_CANCEL_TYPE = 0;
   template <class A>
   __device__ static __forceinline__ uint32_t invariant(A all, uint32_t flags) {
     if (!flags) return 0;
