@@ -12,8 +12,8 @@
 //                  thread-interleaved (word w of thread t at [w*BD + t]: every
 //                  access is bank-conflict free whatever each lane indexes)
 //   HBM / L1 / L2  the pending-message array (RandomizedHashSet.arr), 16-byte
-//                  entries interleaved per warp (entry i of lane l at
-//                  [(i*32 + l)])
+//                  entries, LPCAP contiguous ones per thread (entry i of
+//                  thread t at [t*LPCAP + i])
 //
 // Exactness: every structure here is a bounded, duplicate-free restatement.
 // Whenever an execution could leave that regime (a capacity would overflow, or
@@ -215,7 +215,7 @@ struct LaneMachine {
   static constexpr int WORDS = N * SW + OBW + N + TW;      // states + outbox + partition rows + cancellable timer copies
 
   uint32_t* smw;             // &smem[tid]; word w at smw[w*BD]
-  uint4* pend;               // entry i at pend[i*32]
+  uint4* pend;               // entry i at pend[i]
   uint4* rec_ev; uint16_t* rec_par;   // REC: this execution's EventTrace slot and parent array
   uint64_t pol;              // L2 cache policy of the pending array
   const KernelArgs* A;
@@ -281,7 +281,7 @@ struct LaneMachine {
   // and at the end of the execution, the only points where the set can be at a maximum.
   __device__ __forceinline__ bool pending_full(uint32_t k) const { return n_pending + k > A->pending_cap || n_pending + k > LPCAP; }
   __device__ __forceinline__ void pending_push(uint4 e) {          // the caller has checked pending_full
-    st_l2_hint(pend + n_pending * 32, e, pol);
+    st_l2_hint(pend + n_pending, e, pol);
     n_pending++;
   }
   __device__ __forceinline__ void pending_insert(uint4 e) {
@@ -291,9 +291,9 @@ struct LaneMachine {
   // RandomizedHashSet.remove (schedulers/Util.scala:146-163)
   __device__ __forceinline__ uint4 pending_remove_at(uint32_t i) {
     if (n_pending > max_pending) max_pending = n_pending;
-    uint4 v = ld_l2_hint(pend + i * 32, pol);
-    uint4 last = ld_l2_hint(pend + (n_pending - 1) * 32, pol);
-    st_l2_hint(pend + i * 32, last, pol);
+    uint4 v = ld_l2_hint(pend + i, pol);
+    uint4 last = ld_l2_hint(pend + (n_pending - 1), pol);
+    st_l2_hint(pend + i, last, pol);
     n_pending--;
     if constexpr (CT != 0) {
       if (cancellable_timer(v.x)) {
@@ -483,7 +483,7 @@ struct LaneMachine {
     for (uint32_t i = 0; i < n_pending; i += 4) {
       uint4 q[4];
 #pragma unroll
-      for (uint32_t k = 0; k < 4; k++) q[k] = (i + k < n_pending) ? ld_l2_hint(pend + (i + k) * 32, pol) : make_uint4(0, 0, 0, 0);
+      for (uint32_t k = 0; k < 4; k++) q[k] = (i + k < n_pending) ? ld_l2_hint(pend + (i + k), pol) : make_uint4(0, 0, 0, 0);
 #pragma unroll
       for (uint32_t k = 0; k < 4; k++)
         if ((q[k].x & 0x00FFFFFFu) == want && q[k].y == p0 && q[k].z == p1) { pending_remove_at(i + k); return; }
@@ -665,7 +665,7 @@ struct LaneMachine {
       if (A->fuzz_flags & DEMI_FF_HASH_PENDING)
 #pragma unroll 1
         for (uint32_t i = 0; i < n_pending; i++) {
-          uint4 q = ld_l2_hint(pend + i * 32, pol);
+          uint4 q = ld_l2_hint(pend + i, pol);
           sh += demi_pending_term(q.x & 0x00FFFFFFu, q.y, q.z);
         }
       out.violation = violation; out.steps = (uint32_t)nsched;
@@ -695,11 +695,10 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
   const uint32_t tid = threadIdx.x;
   const uint64_t gthread = (uint64_t)blockIdx.x * BD + tid;
   const uint64_t total = (uint64_t)gridDim.x * BD;
-  const uint64_t gwarp = gthread >> 5;
 
   M m;
   m.smw = lane_smem + tid;
-  m.pend = args.lane_pend + gwarp * (uint64_t)LPCAP * 32 + (tid & 31);
+  m.pend = args.lane_pend + gthread * (uint64_t)LPCAP;
   KernelArgs la;
   if constexpr (PROG) { la = args; m.A = &la; } else m.A = &args;
   m.pol = l2_evict_last_policy();
