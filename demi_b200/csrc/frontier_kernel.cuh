@@ -660,7 +660,10 @@ __global__ void __launch_bounds__(1024) fr_sel_blockscan_kernel(const __grid_con
   if (threadIdx.x == 0) {
     S.info->total_winners = carry_s;
     S.info->taken = carry_s < S.quota ? carry_s : S.quota;
-    if (carry_s <= S.quota) S.info->cut = S.win_n;                             // the whole window is consumed
+    // fewer winners than the quota: the whole window is consumed and getNext goes on into the next one; otherwise the
+    // round ends at its quota-th winner (fr_sel_assign_kernel) and the explored points behind it stay queued, to be
+    // dropped by the round that dequeues them, as getNext drops them (:1156-1160)
+    if (carry_s < S.quota) S.info->cut = S.win_n;
   }
 }
 // the first `quota` winners are dequeued: marked explored (:1169-1171) and handed to the executor
@@ -682,7 +685,7 @@ __global__ void __launch_bounds__(256) fr_sel_assign_kernel(const __grid_constan
   const ulonglong2 k = S.win[i];
   if (!S.no_history && fr_e_insert(S.E, S.e_slots, k.y, S.ctr)) { atomicAdd(&S.ctr[FRC_EXPLORED], 1ull); fr_log_key(S.log, k.y, S.ctr); }
   S.sel[S.sel_base + rank] = k;
-  if (rank == q - 1 && total > S.quota) S.info->cut = i + 1;
+  if (rank == q - 1 && total >= S.quota) S.info->cut = i + 1;
 }
 
 // ------------------------------------------------------------------ explored pairs learned from the other ranks

@@ -157,6 +157,8 @@ struct Raft5 {
   // as it is issued (the lane engine) then carry one copy of that code instead of one per handler, and the threads of
   // a warp that handle different message types meet again at those sites.
   enum { PLAN_NONE = 0, PLAN_REPLY = 1, PLAN_REQUEST_VOTES = 2, PLAN_APPEND_ALL = 3 };
+  // DESIGN §3 raft5 R1: no reply to a non-actor (deadLetters, the sender of an external message)
+  __device__ static __forceinline__ uint32_t reply_plan(uint32_t src) { return src < N_ACTORS ? PLAN_REPLY : PLAN_NONE; }
   template <class S, class C, class O>
   __device__ static __forceinline__ void receive_body(O& out, uint32_t self, S& s, C& c, uint32_t src,
                                                       uint32_t type, uint32_t p0, uint32_t p1, uint32_t flags) {
@@ -194,12 +196,13 @@ struct Raft5 {
         bool can_vote = (c[VOTED] == NONE || c[VOTED] == src) || (flags & BUG_DOUBLE_VOTE);
         uint32_t grant = (t == c[TERM] && can_vote && up_to_date) ? 1u : 0u;
         if (grant) { c[VOTED] = (uint8_t)src; c[HEARD] = 1; }
-        plan = PLAN_REPLY; plan_type = VOTE_REPLY; plan_p0 = (uint32_t)c[TERM] | (grant << 8);
+        plan = reply_plan(src); plan_type = VOTE_REPLY; plan_p0 = (uint32_t)c[TERM] | (grant << 8);
         break;
       }
       case VOTE_REPLY: {
         uint32_t g = (p0 >> 8) & 1u;
         if (t > c[TERM]) { cancel_heartbeat = step_down(c, t); break; }
+        if (src >= N_ACTORS) break;                          // DESIGN §3 raft5 R2: no vote from a non-actor
         if (c[ROLE] == CANDIDATE && t == c[TERM] && g) {
           c[VOTES] |= (uint8_t)(1u << src);
           if (__popc((uint32_t)c[VOTES]) >= 3) {
@@ -221,7 +224,7 @@ struct Raft5 {
       case APPEND_ENTRIES: {
         uint32_t prev = (p0 >> 8) & 0xFF, pt = (p0 >> 16) & 0xFF, lc = (p0 >> 24) & 0xFF;
         uint32_t has = p1 & 1u, et = (p1 >> 8) & 0xFF, ev = (p1 >> 16) & 0xFF;
-        plan = PLAN_REPLY; plan_type = APPEND_REPLY;
+        plan = reply_plan(src); plan_type = APPEND_REPLY;
         if (t < c[TERM]) { plan_p0 = (uint32_t)c[TERM]; break; }
         if (t > c[TERM] || c[ROLE] != FOLLOWER) cancel_heartbeat = step_down(c, t);
         c[HEARD] = 1;
@@ -262,7 +265,7 @@ struct Raft5 {
       case APPEND_REPLY: {
         uint32_t ok = (p0 >> 8) & 1u, mi = (p0 >> 16) & 0xFF;
         if (t > c[TERM]) { cancel_heartbeat = step_down(c, t); break; }
-        if (c[ROLE] != LEADER || t != c[TERM]) break;
+        if (c[ROLE] != LEADER || t != c[TERM] || src >= N_ACTORS) break;   // DESIGN §3 raft5 R2
         if (ok) {
           if (mi > s[MATCH + src]) s[MATCH + src] = (uint8_t)mi;
           if (mi > s[NEXT + src]) s[NEXT + src] = (uint8_t)mi;

@@ -78,6 +78,11 @@ static void raft_send_append(om_machine* m, int self, const uint8_t* s, int j) {
           (uint32_t)s[R_TERM] | (prev << 8) | (pt << 16) | ((uint32_t)s[R_COMMIT] << 24),
           has | (et << 8) | (ev << 16));
 }
+/* DESIGN.md §3, raft5 R1: a reply to a non-actor (deadLetters, the sender of an external message) is not issued */
+static void raft_reply(om_machine* m, int self, int src, uint8_t type, uint32_t p0) {
+  if (src >= RAFT_N) return;
+  om_send(m, self, src, type, p0, 0);
+}
 static void raft_receive(om_machine* m, int self, uint32_t* stw, const demi_msg* msg) {
   uint8_t* s = (uint8_t*)stw;
   uint32_t flags = m->model_flags;
@@ -119,7 +124,7 @@ static void raft_receive(om_machine* m, int self, uint32_t* stw, const demi_msg*
       int can_vote = (s[R_VOTED] == RAFT_NONE || s[R_VOTED] == c) || (flags & RAFT_BUG_DOUBLE_VOTE);
       uint32_t grant = (t == s[R_TERM] && can_vote && up_to_date) ? 1u : 0u;
       if (grant) { s[R_VOTED] = (uint8_t)c; s[R_HEARD] = 1; }
-      om_send(m, self, c, RM_VOTE_REPLY, (uint32_t)s[R_TERM] | (grant << 8), 0);
+      raft_reply(m, self, c, RM_VOTE_REPLY, (uint32_t)s[R_TERM] | (grant << 8));
       break;
     }
     case RM_VOTE_REPLY: {
@@ -127,6 +132,7 @@ static void raft_receive(om_machine* m, int self, uint32_t* stw, const demi_msg*
       uint8_t t = (uint8_t)(msg->p0 & 0xFF);
       uint32_t g = (msg->p0 >> 8) & 1u;
       if (t > s[R_TERM]) { raft_step_down(m, self, s, t); break; }
+      if (msg->src >= RAFT_N) break;                  /* DESIGN.md §3, raft5 R2: no vote from a non-actor */
       if (s[R_ROLE] == ROLE_CANDIDATE && t == s[R_TERM] && g) {
         s[R_VOTES] |= (uint8_t)(1u << msg->src);
         if (__builtin_popcount(s[R_VOTES]) >= 3) {
@@ -153,11 +159,11 @@ static void raft_receive(om_machine* m, int self, uint32_t* stw, const demi_msg*
       uint8_t t = (uint8_t)(msg->p0 & 0xFF);
       uint32_t prev = (msg->p0 >> 8) & 0xFF, pt = (msg->p0 >> 16) & 0xFF, lc = (msg->p0 >> 24) & 0xFF;
       uint32_t has = msg->p1 & 1u, et = (msg->p1 >> 8) & 0xFF, ev = (msg->p1 >> 16) & 0xFF;
-      if (t < s[R_TERM]) { om_send(m, self, l, RM_APPEND_REPLY, (uint32_t)s[R_TERM], 0); break; }
+      if (t < s[R_TERM]) { raft_reply(m, self, l, RM_APPEND_REPLY, (uint32_t)s[R_TERM]); break; }
       if (t > s[R_TERM] || s[R_ROLE] != ROLE_FOLLOWER) raft_step_down(m, self, s, t);
       s[R_HEARD] = 1;
       int ok = prev <= s[R_LOGLEN] && (prev == 0 || s[R_LOGTERM + prev - 1] == pt);
-      if (!ok) { om_send(m, self, l, RM_APPEND_REPLY, (uint32_t)s[R_TERM], 0); break; }
+      if (!ok) { raft_reply(m, self, l, RM_APPEND_REPLY, (uint32_t)s[R_TERM]); break; }
       uint32_t mi = prev;
       if (has) {
         if (s[R_LOGLEN] > prev && s[R_LOGTERM + prev] != et) {      /* conflict: truncate */
@@ -172,7 +178,7 @@ static void raft_receive(om_machine* m, int self, uint32_t* stw, const demi_msg*
       }
       uint32_t nc = lc < mi ? lc : mi;
       if (nc > s[R_COMMIT]) s[R_COMMIT] = (uint8_t)nc;
-      om_send(m, self, l, RM_APPEND_REPLY, (uint32_t)s[R_TERM] | (1u << 8) | (mi << 16), 0);
+      raft_reply(m, self, l, RM_APPEND_REPLY, (uint32_t)s[R_TERM] | (1u << 8) | (mi << 16));
       break;
     }
     case RM_APPEND_REPLY: {
@@ -182,6 +188,7 @@ static void raft_receive(om_machine* m, int self, uint32_t* stw, const demi_msg*
       uint32_t ok = (msg->p0 >> 8) & 1u, mi = (msg->p0 >> 16) & 0xFF;
       if (t > s[R_TERM]) { raft_step_down(m, self, s, t); break; }
       if (s[R_ROLE] != ROLE_LEADER || t != s[R_TERM]) break;
+      if (j >= RAFT_N) break;                         /* DESIGN.md §3, raft5 R2: nothing indexed by a non-actor */
       if (ok) {
         if (mi > s[R_MATCH + j]) s[R_MATCH + j] = (uint8_t)mi;
         if (mi > s[R_NEXT + j]) s[R_NEXT + j] = (uint8_t)mi;

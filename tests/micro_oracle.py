@@ -14,6 +14,7 @@ schedulers/ExternalEventInjector.scala:258-365, :367-441, :541-580, :601-610; In
 """
 
 DEADLETTERS = "deadLetters"
+INJECTED = "injected"                            # messagesToSend's sender of an external Send (deadLetters on the wire)
 
 
 class JavaRandom(object):                       # java.util.Random, Java SE specification
@@ -128,7 +129,8 @@ class Execution(object):
         self.lookingFor = looking_for
         self.depTracker = DepTracker()
         # ExternalEventInjector
-        self.messagesToSend = []                 # (sender or None, receiver, msg)
+        self.messagesToSend = []                 # (sender, None for a timer or INJECTED for an external Send, receiver, msg)
+        self.injecting = False                   # event_produced is handling an injected Send
         self.enqueuedExternalMessages = []       # MultiSet
         # RandomScheduler
         self.justScheduledTimers = set()
@@ -175,7 +177,7 @@ class Execution(object):
                 self.actors[e[1]] = self.fresh_actor(e[1])
             elif e[0] == "Send":
                 self.enqueuedExternalMessages.append(e[2])           # enqueue_message :258-268
-                self.messagesToSend.append((None, e[1], e[2]))
+                self.messagesToSend.append((INJECTED, e[1], e[2]))
             elif e[0] == "Partition":
                 self.events.append(("Partition", e[1], e[2])); self.partitioned.add((e[1], e[2]))
             elif e[0] == "UnPartition":
@@ -216,7 +218,9 @@ class Execution(object):
         self.uniq_counter += 1
         uniq = self.uniq_counter
         is_timer = False
-        if msg in self.enqueuedExternalMessages:                     # handle_event_produced :504-507
+        # handle_event_produced :504-507 asks enqueuedExternalMessages.contains(msg); this project classifies a message
+        # by where it came from, an injected Send (DESIGN.md §3, raft5)
+        if self.injecting:
             unique = self.depTracker.reportNewlyEnabledExternal(snd, rcv, msg)
             self.pendingEvents.insert((uniq, unique, snd, rcv, msg))
         else:
@@ -253,7 +257,9 @@ class Execution(object):
         for sender, rcv, msg in queue:
             if rcv in self.dead:                                     # "Dropping message to non-existent receiver" (:343-346)
                 continue
-            self.tell(DEADLETTERS if sender is None else sender, rcv, msg)
+            self.injecting = sender is INJECTED
+            self.tell(DEADLETTERS if sender in (None, INJECTED) else sender, rcv, msg)
+            self.injecting = False
 
     def violationMatches(self, v):               # :138-154
         if v is None:
@@ -474,6 +480,10 @@ class RaftActor(object):
         et, ev = self.log[prev] if has else (0, 0)
         ctx.send(str(j), (APPEND_ENTRIES, self.term | (prev << 8) | (pt << 16) | (self.commit << 24), has | (et << 8) | (ev << 16)))
 
+    def reply(self, ctx, src, msg):
+        if src is not None:                      # DESIGN.md §3 raft5 R1: no reply to deadLetters
+            ctx.send(str(src), msg)
+
     def receive(self, ctx, sender, msg):
         ty, p0, p1 = msg
         src = int(sender) if sender.isdigit() else None
@@ -511,10 +521,12 @@ class RaftActor(object):
             grant = 1 if (t == self.term and can_vote and up_to_date) else 0
             if grant:
                 self.voted, self.heard = src, True
-            ctx.send(str(src), (VOTE_REPLY, self.term | (grant << 8), 0))
+            self.reply(ctx, src, (VOTE_REPLY, self.term | (grant << 8), 0))
         elif ty == VOTE_REPLY:
             if t > self.term:
                 self.step_down(ctx, t)
+                return
+            if src is None:                      # R2: no vote from deadLetters
                 return
             if self.role == CANDIDATE and t == self.term and (p0 >> 8) & 1:
                 self.votes.add(src)
@@ -536,14 +548,14 @@ class RaftActor(object):
             prev, pt, lc = (p0 >> 8) & 0xFF, (p0 >> 16) & 0xFF, (p0 >> 24) & 0xFF
             has, et, ev = p1 & 1, (p1 >> 8) & 0xFF, (p1 >> 16) & 0xFF
             if t < self.term:
-                ctx.send(str(src), (APPEND_REPLY, self.term, 0))
+                self.reply(ctx, src, (APPEND_REPLY, self.term, 0))
                 return
             if t > self.term or self.role != FOLLOWER:
                 self.step_down(ctx, t)
             self.heard = True
             ok = prev <= len(self.log) and (prev == 0 or self.log[prev - 1][0] == pt)
             if not ok:
-                ctx.send(str(src), (APPEND_REPLY, self.term, 0))
+                self.reply(ctx, src, (APPEND_REPLY, self.term, 0))
                 return
             mi = prev
             if has:
@@ -554,13 +566,13 @@ class RaftActor(object):
                 if len(self.log) > prev:
                     mi = prev + 1
             self.commit = max(self.commit, min(lc, mi))
-            ctx.send(str(src), (APPEND_REPLY, self.term | (1 << 8) | (mi << 16), 0))
+            self.reply(ctx, src, (APPEND_REPLY, self.term | (1 << 8) | (mi << 16), 0))
         elif ty == APPEND_REPLY:
             ok, mi = (p0 >> 8) & 1, (p0 >> 16) & 0xFF
             if t > self.term:
                 self.step_down(ctx, t)
                 return
-            if self.role != LEADER or t != self.term:
+            if self.role != LEADER or t != self.term or src is None:   # R2: nothing indexed by deadLetters
                 return
             if ok:
                 self.match[src] = max(self.match[src], mi)
@@ -583,9 +595,9 @@ def raft_invariant(actors):
         for j in range(i + 1, 5):
             if a[i].role == LEADER and a[j].role == LEADER and a[i].term == a[j].term:
                 return 1
-            if code is None:
+            if code is None:                     # entries past the log's end are the cleared (0, 0) of the state bytes
                 c = min(a[i].commit, a[j].commit)
-                if a[i].log[:c] != a[j].log[:c]:
+                if (a[i].log + [(0, 0)] * 8)[:c] != (a[j].log + [(0, 0)] * 8)[:c]:
                     code = 2
     return code
 
