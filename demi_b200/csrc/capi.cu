@@ -380,6 +380,15 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool recor
 
 static int32_t launch_fuzz(demi_handle* h, const demi_fuzz_params* p, void* out_dev, void* stream, bool reset_counters);
 
+// The counts of a new batch start from zero; demi_fuzz_summary_dev, or the host path once it syncs, fills the rest.
+static void reset_batch_perf(demi_handle* h) {
+  h->perf.kernel_launches = 0;
+  h->perf.prefixes = 0;
+  h->perf.deliveries = 0;
+  h->perf.violations = 0;
+  h->perf.deferred = 0;
+}
+
 extern "C" int32_t demi_fuzz_batch_dev(demi_handle* h, const demi_fuzz_params* p, void* out_dev, void* stream) {
   return launch_fuzz(h, p, out_dev, stream, true);
 }
@@ -425,14 +434,13 @@ static int32_t launch_fuzz(demi_handle* h, const demi_fuzz_params* p, void* out_
   LaunchPlan plan;
   int32_t rc = plan_launch(h, p, false, &plan);
   if (rc != DEMI_OK) return rc;
-  if (p->n_prefixes == 0) return DEMI_OK;
   cudaStream_t s = (cudaStream_t)stream;
-  plan.args.results = (demi_fuzz_result*)out_dev;
-  if (reset_counters) {
+  if (reset_counters) {                                        // an empty batch, too, reports its own (zero) counts
     CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
-    h->perf.kernel_launches = 0;
-    h->perf.prefixes = 0;
+    reset_batch_perf(h);
   }
+  if (p->n_prefixes == 0) return DEMI_OK;
+  plan.args.results = (demi_fuzz_result*)out_dev;
   const LaneVariant* lv = pick_lane_variant(h);
   if (lv) {
     // K1-lane handles every prefix it can prove exact; the rest are deferred to the warp engine
@@ -841,6 +849,10 @@ static int32_t launch_campaign(demi_handle* h, const demi_fuzz_params* p, int64_
   int32_t rc = plan_launch(h, p, false, &plan, true);
   if (rc != DEMI_OK) return rc;
   const uint64_t n = p->n_prefixes;
+  if (reset_counters) {                                        // an empty batch, too, reports its own (zero) counts
+    CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
+    reset_batch_perf(h);
+  }
   if (n == 0) return DEMI_OK;
   uint32_t stride, send_stride;
   campaign_chunk(h, &stride, &send_stride);
@@ -849,11 +861,6 @@ static int32_t launch_campaign(demi_handle* h, const demi_fuzz_params* p, int64_
   demi_ext_event* ev = (demi_ext_event*)h->fz_arena;
   uint2* hdr = (uint2*)((unsigned char*)h->fz_arena + b_ev);
   uint4* sends = (uint4*)((unsigned char*)h->fz_arena + b_ev + b_hdr);
-  if (reset_counters) {
-    CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
-    h->perf.kernel_launches = 0;
-    h->perf.prefixes = 0;
-  }
   fuzzer_gen_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(h->fuzzer, program_seed_base, n, h->fz_fixed_dev, h->fz_n_prefix,
                                                                  h->fz_n_postfix, ev, stride, hdr, sends, send_stride);
   CUDA_TRY(h, cudaGetLastError());

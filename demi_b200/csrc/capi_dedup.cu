@@ -18,9 +18,9 @@ extern "C" int32_t demi_dedup_compact_dev(demi_handle* h, const void* results_de
   while (slots < 2 * n) slots <<= 1;
   const uint32_t n_blocks = (uint32_t)((n + DD_BLOCK - 1) / DD_BLOCK);
   int32_t rc;
-  if (mode == DEMI_DM_UNIQUE) {
-    if ((rc = ensure_bytes(h, &S.keys, &S.keys_b, slots * sizeof(DDSlot))) != DEMI_OK) return rc;
-    CUDA_TRY(h, cudaMemsetAsync(S.keys, 0xFF, slots * sizeof(DDSlot), s));
+  if (mode == DEMI_DM_UNIQUE) {                                 // + table[slots]: the records whose hash is ~0
+    if ((rc = ensure_bytes(h, &S.keys, &S.keys_b, (slots + 1) * sizeof(DDSlot))) != DEMI_OK) return rc;
+    CUDA_TRY(h, cudaMemsetAsync(S.keys, 0xFF, (slots + 1) * sizeof(DDSlot), s));
   }
   if ((rc = ensure_bytes(h, &S.keep, &S.keep_b, n)) != DEMI_OK) return rc;
   if ((rc = ensure_bytes(h, &S.counts, &S.counts_b, (size_t)n_blocks * 4)) != DEMI_OK) return rc;

@@ -7,6 +7,8 @@
 //   K5b dedup_flag   : keep[i] = (value[slot(key_i)] == i)  (or violation != 0); per-block counts
 //   scan             : exclusive scan of the block counts (one block)
 //   K4  compact      : ballot + prefix inside the block, coalesced 32-byte record writes
+// A state hash of ~0 is the empty-slot marker, so it cannot be a key: its records share one extra slot past the
+// table (table[slots], emptied by the same 0xFF memset) that only holds their min index.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -26,8 +28,11 @@ __global__ void __launch_bounds__(DD_BLOCK)
 dedup_insert_kernel(const demi_fuzz_result* __restrict__ rec, uint64_t n, DDSlot* table, uint64_t slots) {
   for (uint64_t i = (uint64_t)blockIdx.x * DD_BLOCK + threadIdx.x; i < n; i += (uint64_t)gridDim.x * DD_BLOCK) {
     const uint4 a = __ldg(reinterpret_cast<const uint4*>(rec + i));          // {violation, steps, state_hash lo, hi}
-    uint64_t key = (uint64_t)a.z | ((uint64_t)a.w << 32);
-    if (key == DD_EMPTY) key = 0x5D5D5D5D5D5D5D5Dull;                         // reserve the sentinel
+    const uint64_t key = (uint64_t)a.z | ((uint64_t)a.w << 32);
+    if (key == DD_EMPTY) {                                                    // the marker's own slot
+      if (__ldcg(&table[slots].val) > (uint32_t)i) atomicMin(&table[slots].val, (uint32_t)i);
+      continue;
+    }
     uint64_t s = dd_slot(key, slots);
     for (;;) {
       // one 16-byte read shows the slot's key and current index.  A slot never changes once it holds a key, so a
@@ -58,13 +63,16 @@ dedup_flag_kernel(const demi_fuzz_result* __restrict__ rec, uint64_t n, int mode
     if (mode == DEMI_DM_VIOLATING) {
       k = a.x != 0;
     } else {
-      uint64_t key = (uint64_t)a.z | ((uint64_t)a.w << 32);
-      if (key == DD_EMPTY) key = 0x5D5D5D5D5D5D5D5Dull;
-      uint64_t s = dd_slot(key, slots);
-      for (;;) {
-        const ulonglong2 q = __ldg(reinterpret_cast<const ulonglong2*>(table + s));
-        if (q.x == key) { k = (uint32_t)q.y == (uint32_t)i; break; }
-        s = (s + 1) & (slots - 1);
+      const uint64_t key = (uint64_t)a.z | ((uint64_t)a.w << 32);
+      if (key == DD_EMPTY) {
+        k = __ldg(&table[slots].val) == (uint32_t)i;
+      } else {
+        uint64_t s = dd_slot(key, slots);
+        for (;;) {
+          const ulonglong2 q = __ldg(reinterpret_cast<const ulonglong2*>(table + s));
+          if (q.x == key) { k = (uint32_t)q.y == (uint32_t)i; break; }
+          s = (s + 1) & (slots - 1);
+        }
       }
     }
     keep[i] = k ? 1 : 0;

@@ -224,7 +224,7 @@ int32_t demi_fuzz_batch(demi_handle* h, const demi_fuzz_params* p,
 int32_t demi_fuzz_batch_dev(demi_handle* h, const demi_fuzz_params* p,
                             void* out_dev, void* stream);
 /* Device-side summary of a finished batch without copying the records:
- * number of violating prefixes and sum of steps. */
+ * number of violating prefixes and sum of steps (0 and 0 after an empty batch). */
 int32_t demi_fuzz_summary_dev(demi_handle* h, const void* results_dev, uint64_t n,
                               void* stream, uint64_t* n_violations, uint64_t* sum_steps);
 /* Re-run one seed in recording mode and return its EventTrace

@@ -48,6 +48,13 @@ def test_dedup_edge_cases():
     one = np.zeros(1, dtype=N.RESULT_DTYPE); one["state_hash"] = 0xFFFFFFFFFFFFFFFF   # the table's sentinel value
     u, i = eng.dedup_compact(np.repeat(one, 777), 0)
     assert len(u) == 1 and i[0] == 0
+    # ~0 marks an empty slot; it must stay distinct from every real key, whichever of the two comes first
+    ones, other = 0xFFFFFFFFFFFFFFFF, 0x5D5D5D5D5D5D5D5D
+    for a, b in ((ones, other), (other, ones)):
+        alias = np.zeros(5, dtype=N.RESULT_DTYPE); alias["state_hash"] = [a, b, a, b, 0]
+        alias["steps"] = np.arange(5)
+        u, i = eng.dedup_compact(alias, 0)
+        assert i.tolist() == [0, 1, 4] and u.tobytes() == alias[[0, 1, 4]].tobytes()
     ragged = np.zeros(1025, dtype=N.RESULT_DTYPE); ragged["state_hash"] = np.arange(1025) % 7
     u, i = eng.dedup_compact(ragged, 0)
     assert (i == np.arange(7)).all()
