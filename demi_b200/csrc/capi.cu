@@ -317,7 +317,10 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool recor
   const uint32_t pcap = demi_pending_cap(demi_model_key(h), p->max_messages, n_sends);
   const uint32_t tcap = demi_tosend_cap(n_sends);
   const bool fifo = h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;          // SrcDstFIFO lives in the HBM-pending variants
-  const Variant* v = pick_variant(h->cfg.model, pcap, tcap, record, fifo);
+  // so does every program with a HardKill: Machine::hard_kill needs room for n_pending + matches <= 2 * pcap entries,
+  // which only the HBM variants (PCAP = 16384 >= 2 * 8192) have.  A random-oracle test decides on the base program.
+  const bool hard_kill = campaign ? h->fz_has_hard_kill : h->has_hard_kill;
+  const Variant* v = pick_variant(h->cfg.model, pcap, tcap, record, fifo || hard_kill);
   if (!v) return fail(h, DEMI_ERR_CAPACITY, "no kernel variant for pending_cap=%u tosend_cap=%u", pcap, tcap);
   const kernel_fn fn = tests ? v->fn_tests : campaign ? v->fn_prog : v->fn;
   const size_t smem = v->smem_per_warp * WARPS;
@@ -361,7 +364,7 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool recor
                      total_warps * (uint64_t)(v->pcap / 2 + 3 * FIFO_PAIRS) * sizeof(uint16_t))) != DEMI_OK) return rc;
     a.fifo_scratch = h->fifo_scratch;
   }
-  if (fifo && ((campaign ? h->fz_has_hard_kill : h->has_hard_kill) || !h->filter.empty()))
+  if (fifo && (hard_kill || !h->filter.empty()))
     return fail(h, DEMI_ERR_INVALID, "HardKill and userDefinedFilter are offered for FullyRandom only");
   a.n_filter = (uint32_t)h->filter.size();
   for (uint32_t i = 0; i < a.n_filter; i++) a.filter[i] = make_uint4(h->filter[i].src_mask, h->filter[i].dst_mask, h->filter[i].type_mask, h->filter[i].flags);

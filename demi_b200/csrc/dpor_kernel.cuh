@@ -77,6 +77,7 @@ struct DporMachine {
   uint32_t* smw; const DporArgs* A;
   uint4* nodes; uint32_t* child_hash; uint32_t* queues; uint64_t* explored; DporKey* heap;
   uint32_t* traces; uint32_t* trace_len; uint32_t* cur_trace; uint32_t* next_trace;
+  const uint32_t* next_rd;      // the nextTrace the schedule follows: next_trace, or the whole initial trace
   uint32_t* node_pos; uint32_t* scan; uint32_t scan_stride; uint32_t* heap_dist; int32_t* path;
   uint32_t* bk_head; uint32_t* bk_tail; uint32_t pool_top, free_head, max_branch;   // bucket queue (see bq_push)
   uint16_t qlen[NQ];            // local memory (small)
@@ -243,9 +244,9 @@ struct DporMachine {
       if (A->P.max_messages >= 0 && nsched > A->P.max_messages) return 0;       // :583-586
       uint32_t pick = 0;
       do {                                                                       // getNextMatchingMessage :542-555
-        while (next_pos < next_len && next_trace[next_pos] == 0) next_pos++;     // getNextTraceMessage :363-372
+        while (next_pos < next_len && next_rd[next_pos] == 0) next_pos++;     // getNextTraceMessage :363-372
         if (next_pos >= next_len) break;
-        uint32_t want = next_trace[next_pos++];                                  // getMatchingMessage :516-524
+        uint32_t want = next_rd[next_pos++];                                  // getMatchingMessage :516-524
         uint4 c = nodes[want];
         uint32_t dst = hdr_dst(c.x);
         if (!((A->blocked_mask >> dst) & 1u)) {
@@ -453,7 +454,7 @@ struct DporMachine {
     explored_add(e1, e2);                                                       // :1169-1171
     if (status) return false;
     // nextTrace = trace.take(maxIndex+1) ++ replayThis (:1180, :1060-1063)
-    next_len = 0; next_pos = 0;
+    next_len = 0; next_pos = 0; next_rd = next_trace;
     for (uint32_t i = 0; i <= kb && i < n; i++) next_trace[next_len++] = cur_trace[i];
     for (uint32_t i = kb + 1; i <= kl; i++) {
       const uint32_t id = kt[i];
@@ -499,7 +500,7 @@ struct DporMachine {
         if (!analyse(n_traces - 1, R)) next_len = 0;                              // None: run() clears nextTrace :757-759
         R.exhausted = 0;
       } else if (A->n_init_trace) {
-        for (uint32_t i = 0; i < A->n_init_trace && i < A->T1; i++) next_trace[next_len++] = __ldg(A->init_trace + i);
+        next_rd = A->init_trace; next_len = A->n_init_trace;                     // followed whole, however long
       }
       started = true;
       while (!status) {
@@ -554,6 +555,7 @@ dpor_kernel(const __grid_constant__ DporArgs args) {
   m.trace_len = args.trace_len + (size_t)sid * (args.P.max_interleavings + 1);
   m.cur_trace = args.cur_trace + (size_t)sid * args.T1;
   m.next_trace = args.next_trace + (size_t)sid * args.T1;
+  m.next_rd = m.next_trace;
   m.node_pos = args.node_pos + (size_t)sid * args.P.node_cap;
   if (args.scan_in_smem) { m.scan = lane_smem + (size_t)M::WORDS * BD + threadIdx.x; m.scan_stride = BD; }
   else { m.scan = args.scan + (size_t)sid * args.T1; m.scan_stride = 1; }

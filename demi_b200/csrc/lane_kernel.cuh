@@ -259,7 +259,9 @@ struct LaneMachine {
 
   __device__ __forceinline__ void defer() { status = LANE_DEFER; }
 
-  // EventTrace.+= (EventTrace.scala:88-110); w3 = uniq | node << 16
+  // EventTrace.+= (EventTrace.scala:88-110); w3 = uniq | node << 16.  Here uniq == node < node_cap <= 65535, so the
+  // 16-bit Uniq wrap (DESIGN.md §2) is never reached: an execution with more ids is one with identical Sends, which
+  // only the warp engine runs.
   __device__ __forceinline__ void record_event(uint32_t kind, uint32_t src, uint32_t dst, uint32_t type,
                                                uint32_t p0, uint32_t p1, uint32_t w3, uint32_t parent) {
     uint32_t w0 = kind | (src << 8) | (dst << 16) | (type << 24);

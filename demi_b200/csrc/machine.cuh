@@ -394,7 +394,9 @@ struct Machine {
       int ci = cancelled.find(lane, timer_key(dst, type), p0, p1);
       if (ci >= 0) { cancelled.remove_at(lane, (uint32_t)ci); return; }
     }
-    uint32_t uniq = ++n_uniq;                                   // Uniq(...) :283
+    // Uniq(...) :283.  Ids are 16-bit and wrap modulo 2^16 (DESIGN.md §2), as the oracle and demi_event have them;
+    // unmasked, bit 16 would land in the node field of the pending entry and of the trace word.
+    uint32_t uniq = ++n_uniq & 0xFFFFu;
     uint32_t hdr_nf = hdr & 0x00FFFFFFu;
     bool is_timer = false;
     uint32_t node;
@@ -517,6 +519,10 @@ struct Machine {
     // scheduler.actorTerminated(name) -> FullyRandom.removeAll (RandomScheduler.scala:686-696): every element of the
     // array as it was when the loop started is visited once, in position order, and a match is swap-removed at its
     // CURRENT index.  Pass 1 lists the Uniq ids of the matches in position order (in the free top of the array).
+    // That needs n_pending + matches <= 2 * pending_cap entries, so plan_launch sends every program with a HardKill to
+    // the HBM variants (PCAP = 16384 >= 2 * 8192); the PENDING_OVF below is never reached there.  Pass 2 removes, for
+    // each listed id, the first entry carrying it; after the 16-bit wrap that can be an entry of another receiver, as
+    // in the oracle (DESIGN.md §2).
     __syncwarp();
     const uint32_t n0 = n_pending, TOP = (uint32_t)PCAP;
     uint32_t r = 0;

@@ -246,7 +246,7 @@ struct ReplayMachine {
     if (cancelled && slot >= 0 && ((cancelled >> slot) & 1u)) { cancelled &= ~(1u << slot); return; }
     uint32_t uniq = 0;
     if (LIST) {
-      uniq = ++n_uniq;                                              // Uniq(...) :570; appendMsgSend :620-622
+      uniq = ++n_uniq & 0xFFFFu;                                    // Uniq(...) :570, 16-bit (DESIGN.md §2); appendMsgSend :620-622
       rec_push(DEMI_EV_MSG_SEND, (!external && src == DEMI_DEADLETTERS) ? DEMI_TIMER_SND : src, dst, type, p0, p1, uniq);
     }
     if (!external && crosses_partition(src, dst)) return;

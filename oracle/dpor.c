@@ -61,6 +61,7 @@ typedef struct {
   uint32_t parent_event, current_depth;
   uint32_t cur_trace[DP_MAX_T]; uint32_t cur_len;
   uint32_t next_trace[DP_MAX_T]; uint32_t next_len, next_pos;
+  const uint32_t* next_rd;                                 /* the nextTrace followed: next_trace or the initial trace */
   int32_t nsched;
   int status;
   /* instance state that survives test() calls */
@@ -242,9 +243,9 @@ static uint32_t dpor_schedule(dpor_t* d) {
      * prioritizePendingUponDivergence, getNextMatchingMessage (:542-555) keeps popping nextTrace until an
      * expected message is pending */
     do {
-      while (d->next_pos < d->next_len && d->next_trace[d->next_pos] == 0) d->next_pos++;
+      while (d->next_pos < d->next_len && d->next_rd[d->next_pos] == 0) d->next_pos++;
       if (d->next_pos >= d->next_len) break;
-      uint32_t want = d->next_trace[d->next_pos++];
+      uint32_t want = d->next_rd[d->next_pos++];
       const demi_msg* c = &d->nodes[want].msg;
       if (!((d->m.blocked_mask >> c->dst) & 1u)) {
         uint32_t q = qindex(d, c->src, c->dst);
@@ -390,7 +391,7 @@ static int dpor_analyse(dpor_t* d, uint32_t k, demi_dpor_result* out) {
   if (d->status) return 0;
   /* nextTrace = trace.take(maxIndex+1) ++ replayThis (:1180); replayThis =
    * keyTrace.drop(branchI+1).dropRight(size-laterI-1).filter(_.id != earlier.id) (:1060-1063) */
-  d->next_len = 0; d->next_pos = 0;
+  d->next_len = 0; d->next_pos = 0; d->next_rd = d->next_trace;
   for (uint32_t i = 0; i <= key.branch && i < n; i++) d->next_trace[d->next_len++] = tr[i];
   const uint32_t* kt = d->traces + (size_t)key.trace_ref * d->T1;
   for (uint32_t i = key.branch + 1; i <= key.later_i; i++)
@@ -466,7 +467,7 @@ int oracle_dpor_test(void* s, int32_t max_distance, demi_dpor_result* out,
   if (d->started && d->n_heap) {
     if (!dpor_analyse(d, d->n_traces - 1, out)) d->next_len = 0;                 /* None: run() clears nextTrace :757-759 */
   } else if (d->opts.n_init_trace) {
-    for (uint32_t i = 0; i < d->opts.n_init_trace && i < DP_MAX_T; i++) d->next_trace[d->next_len++] = d->opts.init_trace[i];
+    d->next_rd = d->opts.init_trace; d->next_len = d->opts.n_init_trace;      /* followed whole, however long */
   }
   d->started = 1;
   out->exhausted = 0;

@@ -55,8 +55,11 @@ int oracle_fuzz_trace(const demi_config* cfg, const demi_ext_event* ext, uint32_
                       demi_fuzz_result* result) {
   if (!oracle_get_model(cfg->model)) return DEMI_ERR_INVALID;
   demi_fuzz_result r;
-  oracle_run_prefix(cfg, ext, n_ext, p, seed, &r, events, cap_events, dep_parent, cap_nodes, 0);
-  if (n_events) *n_events = r.n_events;
+  om_machine* m = (om_machine*)malloc(sizeof(om_machine));
+  if (!m) return DEMI_ERR_INVALID;
+  oracle_run_prefix(cfg, ext, n_ext, p, seed, &r, events, cap_events, dep_parent, cap_nodes, m);
+  if (n_events) *n_events = r.status ? r.n_events : m->n_events;   /* the whole trace: r.n_events saturates at 65535 */
+  free(m);
   if (n_nodes) *n_nodes = r.n_nodes;
   if (result) *result = r;
   return r.status ? DEMI_ERR_CAPACITY : DEMI_OK;

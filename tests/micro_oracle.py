@@ -216,7 +216,7 @@ class Execution(object):
     # ---- RandomScheduler
     def event_produced(self, snd, rcv, msg):     # :274-321
         self.uniq_counter += 1
-        uniq = self.uniq_counter
+        uniq = self.uniq_counter & 0xFFFF                            # Uniq ids are 16-bit and wrap (DESIGN.md §2)
         is_timer = False
         # handle_event_produced :504-507 asks enqueuedExternalMessages.contains(msg); this project classifies a message
         # by where it came from, an injected Send (DESIGN.md §3, raft5)
@@ -853,7 +853,7 @@ class STSReplay(Execution):
     # ---- scheduler callbacks
     def event_produced(self, snd, rcv, msg):     # :561-623
         self.uniq_counter += 1
-        uniq = self.uniq_counter
+        uniq = self.uniq_counter & 0xFFFF                            # Uniq ids are 16-bit and wrap (DESIGN.md §2)
         is_timer = False
         if msg in self.enqueuedExternalMessages:                     # handle_event_produced: ExternalMessage
             self.pending.setdefault((snd, rcv), {}).setdefault(msg, []).append((uniq, msg))
