@@ -25,19 +25,24 @@ thread_local std::string g_create_error;
 // ------------------------------------------------------------ kernel table
 constexpr int WARPS = 4;
 typedef void (*kernel_fn)(const KernelArgs);
+// What a fuzz launch runs: a batch of prefixes over the handle's program, the recording of chosen prefixes
+// (provenance, traces), a campaign's generated programs (PROG), or random-oracle tests over subsequences (PROG + TESTS).
+// Both engines have one instantiation per mode.
+enum LaunchMode { LM_BATCH, LM_RECORD, LM_PROGRAM, LM_TESTS, LM_COUNT };
 struct Variant {
-  int model; uint32_t pcap, tcap; bool pend_global, record;
-  kernel_fn fn; size_t smem_per_warp;
-  kernel_fn fn_prog;             // the campaign instantiation (PROG); none for the recording variants
-  kernel_fn fn_tests;            // the random-oracle test instantiation (PROG + TESTS); none for the recording variants
+  int model; uint32_t pcap, tcap; bool pend_global;
+  size_t smem_per_warp;
+  kernel_fn fn[LM_COUNT];        // a recording variant has LM_RECORD alone, the others every mode but it
 };
 template <class MODEL, int PCAP, int TCAP, bool PG, bool REC>
 static Variant make_variant() {
   using M = Machine<MODEL, PCAP, TCAP, PG, REC>;
-  return Variant{MODEL::ID, (uint32_t)PCAP, (uint32_t)TCAP, PG, REC,
-                 fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS>, sizeof(typename M::Smem),
-                 REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC>,
-                 REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC, !REC>};
+  Variant v{MODEL::ID, (uint32_t)PCAP, (uint32_t)TCAP, PG, sizeof(typename M::Smem),
+            {fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS>, nullptr,
+             REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC>,
+             REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC, !REC>}};
+  if (REC) std::swap(v.fn[LM_BATCH], v.fn[LM_RECORD]);
+  return v;
 }
 static const std::vector<Variant>& variants() {
   static const std::vector<Variant> v = {
@@ -58,23 +63,21 @@ static const std::vector<Variant>& variants() {
   };
   return v;
 }
-static const Variant* pick_variant(int model, uint32_t pcap, uint32_t tcap, bool record, bool need_global) {
+static const Variant* pick_variant(int model, LaunchMode mode, uint32_t pcap, uint32_t tcap, bool need_global) {
   for (const Variant& v : variants())
-    if (v.model == model && v.record == record && v.pcap >= pcap && v.tcap >= tcap && (v.pend_global || !need_global)) return &v;
+    if (v.model == model && v.fn[mode] && v.pcap >= pcap && v.tcap >= tcap && (v.pend_global || !need_global)) return &v;
   return nullptr;
 }
 
 // lane-engine table
-struct LaneVariant { int model; int bd; uint32_t lpcap; kernel_fn fn; kernel_fn fn_rec; size_t smem_per_block; kernel_fn fn_prog;
-                     kernel_fn fn_tests; };
+struct LaneVariant { int model; int bd; uint32_t lpcap; size_t smem_per_block; kernel_fn fn[LM_COUNT]; };
 template <class MODEL, int BD, int LPCAP>
 static LaneVariant make_lane_variant() {
   using M = LaneMachine<MODEL, BD, LPCAP>;
-  return LaneVariant{MODEL::ID, BD, (uint32_t)LPCAP, fuzz_lane_kernel<MODEL, BD, LPCAP>, fuzz_lane_kernel<MODEL, BD, LPCAP, true>,
-                     (size_t)M::WORDS * BD * sizeof(uint32_t), fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>,
-                     fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true>};
+  return LaneVariant{MODEL::ID, BD, (uint32_t)LPCAP, (size_t)M::WORDS * BD * sizeof(uint32_t),
+                     {fuzz_lane_kernel<MODEL, BD, LPCAP>, fuzz_lane_kernel<MODEL, BD, LPCAP, true>,
+                      fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>, fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true>}};
 }
-static const LaneVariant* pick_lane_variant(const demi_handle* h, bool campaign = false);
 
 // ---------------------------------------------------------------- lifecycle
 #ifndef DEMI_BUILD_ID
@@ -219,46 +222,42 @@ extern "C" const char* demi_actor_name(const demi_handle* h, uint32_t index) {
   return digits[index];
 }
 
+// A Send external in the form the lane engine reads from its Send table (LaneMachine::external_produced decodes it,
+// lane_kernel.cuh:452): a message from deadLetters, flagged external.
+__host__ __device__ inline uint4 lane_send(const demi_ext_event& e) {
+  return make_uint4(DEMI_DEADLETTERS | ((uint32_t)e.a << 8) | ((uint32_t)e.type << 16) | ((uint32_t)DEMI_MF_EXTERNAL << 24),
+                    e.p0, e.p1, 0u);
+}
+
+// Adds event e of a program to *info; `sends` collects the program's Sends in the lane engine's form.
+static void describe_event(ProgramInfo* info, std::vector<uint4>* sends, const demi_ext_event& e) {
+  if (e.kind == DEMI_EXT_PARTITION || e.kind == DEMI_EXT_UNPARTITION) info->partitions = true;
+  if (e.kind == DEMI_EXT_HARD_KILL) info->hard_kill = true;
+  if (e.kind != DEMI_EXT_SEND) return;
+  const uint4 m = lane_send(e);
+  for (const uint4& o : *sends) if (o.x == m.x && o.y == m.y && o.z == m.z) info->sends_distinct = false;
+  sends->push_back(m);
+  info->sends++;
+}
+
 extern "C" int32_t demi_set_externals(demi_handle* h, const demi_ext_event* ev, uint32_t n) {
   if (!h) return DEMI_ERR_INVALID;
   if (!ev && n) return fail(h, DEMI_ERR_INVALID, "demi_set_externals: null events");
   { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
-  const int n_actors = demi_model_actors(h);
-  uint32_t sends = 0;
+  ProgramInfo info;
+  std::vector<uint4> sv;                 // the lane engine's Send table
   for (uint32_t i = 0; i < n; i++) {
-    const demi_ext_event& e = ev[i];
-    if (e.kind < DEMI_EXT_START || e.kind > DEMI_EXT_HARD_KILL)
-      return fail(h, DEMI_ERR_INVALID, "demi_set_externals: event %u has unknown kind %u", i, e.kind);
-    bool needs_a = e.kind != DEMI_EXT_WAIT_QUIESCENCE;
-    bool needs_b = e.kind == DEMI_EXT_PARTITION || e.kind == DEMI_EXT_UNPARTITION;
-    if ((needs_a && e.a >= n_actors) || (needs_b && e.b >= n_actors))
-      return fail(h, DEMI_ERR_INVALID, "demi_set_externals: event %u names an unknown actor", i);
-    // MessageTypes.sanityCheckTrace (ExternalEvents.scala:138-149): no two consecutive WaitQuiescence
-    if (e.kind == DEMI_EXT_WAIT_QUIESCENCE && i > 0 && ev[i - 1].kind == DEMI_EXT_WAIT_QUIESCENCE)
-      return fail(h, DEMI_ERR_INVALID, "demi_set_externals: consecutive WaitQuiescence at %u", i);
-    if (e.kind == DEMI_EXT_SEND) sends++;
+    const int32_t rc = demi_check_external(h, "demi_set_externals", "", ev, i, true, true);
+    if (rc != DEMI_OK) return rc;
+    describe_event(&info, &sv, ev[i]);
   }
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   cudaFree(h->ext_dev); h->ext_dev = nullptr;
   h->ext_host.assign(ev, ev + n);
-  h->n_ext_sends = sends;
+  h->ext_info = info;
   if (n) {
     CUDA_TRY(h, cudaMalloc(&h->ext_dev, n * sizeof(demi_ext_event)));
     CUDA_TRY(h, cudaMemcpy(h->ext_dev, ev, n * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
-  }
-  // lane-engine side tables: the Send events in order; whether two Sends are
-  // identical (they would share a DepTracker Unique under the root)
-  std::vector<uint4> sv;
-  h->has_partitions = false; h->ext_sends_distinct = true; h->has_hard_kill = false;
-  for (uint32_t i = 0; i < n; i++) {
-    const demi_ext_event& e = ev[i];
-    if (e.kind == DEMI_EXT_PARTITION || e.kind == DEMI_EXT_UNPARTITION) h->has_partitions = true;
-    if (e.kind == DEMI_EXT_HARD_KILL) h->has_hard_kill = true;
-    if (e.kind != DEMI_EXT_SEND) continue;
-    uint4 m = make_uint4(DEMI_DEADLETTERS | ((uint32_t)e.a << 8) | ((uint32_t)e.type << 16) |
-                         ((uint32_t)DEMI_MF_EXTERNAL << 24), e.p0, e.p1, 0u);
-    for (const uint4& o : sv) if (o.x == m.x && o.y == m.y && o.z == m.z) h->ext_sends_distinct = false;
-    sv.push_back(m);
   }
   cudaFree(h->ext_sends_dev); h->ext_sends_dev = nullptr;
   if (!sv.empty()) {
@@ -275,8 +274,9 @@ extern "C" int32_t demi_set_user_filter(demi_handle* h, const demi_filter_rule* 
   return DEMI_OK;
 }
 
-// campaign: the same conditions, over the handle's Fuzzer (demi_set_fuzzer) instead of its program
-static const LaneVariant* pick_lane_variant(const demi_handle* h, bool campaign) {
+// The lane engine for a launch over a program `prog` describes (for a campaign, the Fuzzer's; a random-oracle test
+// decides on the base program, and each of its subsequences meets every condition the base program meets)
+static const LaneVariant* pick_lane_variant(const demi_handle* h, const ProgramInfo& prog) {
   static const std::vector<LaneVariant> v = {
 #ifndef DEMI_K1_BD_RAFT5
 #define DEMI_K1_BD_RAFT5 256
@@ -285,55 +285,35 @@ static const LaneVariant* pick_lane_variant(const demi_handle* h, bool campaign)
     make_lane_variant<PingPong3, 256, 128>(),
     make_lane_variant<Bcast32, 128, 8192>(),
   };
-  const bool distinct = campaign ? h->fz_sends_distinct : h->ext_sends_distinct;
-  const bool hard_kill = campaign ? h->fz_has_hard_kill : h->has_hard_kill;
-  if (!h->use_lane_engine || h->cfg.blocked_mask || !distinct || h->cfg.strategy != DEMI_RS_FULLY_RANDOM ||
-      hard_kill || !h->filter.empty()) return nullptr;          // actor termination and user filters: the general engine
+  if (!h->use_lane_engine || h->cfg.blocked_mask || !prog.sends_distinct || h->cfg.strategy != DEMI_RS_FULLY_RANDOM ||
+      prog.hard_kill || !h->filter.empty()) return nullptr;          // actor termination and user filters: the general engine
   for (const LaneVariant& lv : v) if (lv.model == h->cfg.model) return &lv;
   return nullptr;
 }
 
 // ------------------------------------------------------------------- launch
-struct LaunchPlan { const Variant* v; int grid; size_t smem; KernelArgs args; };
+struct LaunchPlan { const Variant* v; LaunchMode mode; const ProgramInfo* prog; int grid; size_t smem; KernelArgs args; };
 
-static int32_t ensure(demi_handle* h, void** p, size_t* cap, size_t need) {
-  if (*cap >= need) return DEMI_OK;
-  cudaFree(*p); *p = nullptr; *cap = 0;
-  CUDA_TRY(h, cudaMalloc(p, need));
-  *cap = need;
-  return DEMI_OK;
-}
-
-// campaign: sized for the Fuzzer's largest program (fz_max_sends Sends); ext / n_ext are bound per execution.
-// tests: the launch runs fn_tests (random-oracle tests over the handle's program)
-static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool record, LaunchPlan* plan, bool campaign = false,
-                           bool tests = false) {
+// A launch of `mode` over the program (ext, n_ext) that `prog` describes.  A campaign has no one program: `prog` is
+// its Fuzzer's, sized for the largest program, and each execution binds its own events.
+static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, LaunchMode mode, const ProgramInfo& prog,
+                           const demi_ext_event* ext, uint32_t n_ext, LaunchPlan* plan) {
   if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
-  if (campaign && !h->has_fuzzer) return fail(h, DEMI_ERR_STATE, "demi_set_fuzzer has not been called");
-  if (!campaign && h->ext_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
+  if (mode == LM_PROGRAM && !h->has_fuzzer) return fail(h, DEMI_ERR_STATE, "demi_set_fuzzer has not been called");
+  if (mode != LM_PROGRAM && h->ext_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
   if (p->n_prefixes > 0xFFFFFFFFull) return fail(h, DEMI_ERR_INVALID, "n_prefixes > 2^32-1 per call");
   { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
-  const uint32_t n_sends = campaign ? h->fz_max_sends : h->n_ext_sends;
-  const uint32_t pcap = demi_pending_cap(demi_model_key(h), p->max_messages, n_sends);
-  const uint32_t tcap = demi_tosend_cap(n_sends);
+  const uint32_t pcap = demi_pending_cap(demi_model_key(h), p->max_messages, prog.sends);
+  const uint32_t tcap = demi_tosend_cap(prog.sends);
   const bool fifo = h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;          // SrcDstFIFO lives in the HBM-pending variants
   // so does every program with a HardKill: Machine::hard_kill needs room for n_pending + matches <= 2 * pcap entries,
   // which only the HBM variants (PCAP = 16384 >= 2 * 8192) have.  A random-oracle test decides on the base program.
-  const bool hard_kill = campaign ? h->fz_has_hard_kill : h->has_hard_kill;
-  const Variant* v = pick_variant(h->cfg.model, pcap, tcap, record, fifo || hard_kill);
+  const Variant* v = pick_variant(h->cfg.model, mode, pcap, tcap, fifo || prog.hard_kill);
   if (!v) return fail(h, DEMI_ERR_CAPACITY, "no kernel variant for pending_cap=%u tosend_cap=%u", pcap, tcap);
-  const kernel_fn fn = tests ? v->fn_tests : campaign ? v->fn_prog : v->fn;
   const size_t smem = v->smem_per_warp * WARPS;
-  // the attribute and the occupancy of a variant are fixed per device: asked once, not on every launch
+  int32_t rc;
   int blocks_per_sm = 0;
-  {
-    auto it = h->occupancy.find((const void*)fn);
-    if (it == h->occupancy.end()) {
-      CUDA_TRY(h, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, fn, WARPS * 32, smem));
-      h->occupancy[(const void*)fn] = blocks_per_sm;
-    } else blocks_per_sm = it->second;
-  }
+  if ((rc = demi_occupancy(h, (const void*)v->fn[mode], WARPS * 32, smem, &blocks_per_sm)) != DEMI_OK) return rc;
   if (blocks_per_sm < 1) return fail(h, DEMI_ERR_CAPACITY, "kernel variant does not fit on an SM (smem %zu)", smem);
   uint64_t want = (p->n_prefixes + WARPS - 1) / WARPS;
   uint64_t full = (uint64_t)h->sm_count * (uint64_t)blocks_per_sm;
@@ -341,12 +321,11 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool recor
   const uint64_t total_warps = (uint64_t)grid * WARPS;
   const uint32_t node_cap = demi_node_cap(pcap);
 
-  int32_t rc;
-  if ((rc = ensure(h, (void**)&h->node_scratch, &h->node_scratch_bytes,
-                   total_warps * node_cap * sizeof(uint4))) != DEMI_OK) return rc;
+  if ((rc = ensure_bytes(h, (void**)&h->node_scratch, &h->node_scratch_bytes,
+                         total_warps * node_cap * sizeof(uint4))) != DEMI_OK) return rc;
   if (v->pend_global)
-    if ((rc = ensure(h, (void**)&h->pend_scratch, &h->pend_scratch_bytes,
-                     total_warps * (uint64_t)v->pcap * sizeof(uint4))) != DEMI_OK) return rc;
+    if ((rc = ensure_bytes(h, (void**)&h->pend_scratch, &h->pend_scratch_bytes,
+                           total_warps * (uint64_t)v->pcap * sizeof(uint4))) != DEMI_OK) return rc;
 
   KernelArgs a{};
   a.model_flags = h->cfg.model_flags;
@@ -360,16 +339,16 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool recor
   a.fuzz_flags = p->flags;
   a.strategy = h->cfg.strategy;
   if (fifo) {
-    if ((rc = ensure(h, (void**)&h->fifo_scratch, &h->fifo_scratch_bytes,
-                     total_warps * (uint64_t)(v->pcap / 2 + 3 * FIFO_PAIRS) * sizeof(uint16_t))) != DEMI_OK) return rc;
+    if ((rc = ensure_bytes(h, (void**)&h->fifo_scratch, &h->fifo_scratch_bytes,
+                           total_warps * (uint64_t)(v->pcap / 2 + 3 * FIFO_PAIRS) * sizeof(uint16_t))) != DEMI_OK) return rc;
     a.fifo_scratch = h->fifo_scratch;
   }
-  if (fifo && (hard_kill || !h->filter.empty()))
+  if (fifo && (prog.hard_kill || !h->filter.empty()))
     return fail(h, DEMI_ERR_INVALID, "HardKill and userDefinedFilter are offered for FullyRandom only");
   a.n_filter = (uint32_t)h->filter.size();
   for (uint32_t i = 0; i < a.n_filter; i++) a.filter[i] = make_uint4(h->filter[i].src_mask, h->filter[i].dst_mask, h->filter[i].type_mask, h->filter[i].flags);
-  a.ext = campaign ? nullptr : h->ext_dev;
-  a.n_ext = campaign ? 0u : (uint32_t)h->ext_host.size();
+  a.ext = ext;
+  a.n_ext = n_ext;
   a.node_cap = node_cap;
   a.pending_cap = pcap;
   a.tosend_cap = tcap;
@@ -377,57 +356,65 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, bool recor
   a.pend_scratch = h->pend_scratch;
   a.sum_steps = h->counters_dev;
   a.n_violations = h->counters_dev + 1;
-  plan->v = v; plan->grid = grid; plan->smem = smem; plan->args = a;
+  plan->v = v; plan->mode = mode; plan->prog = &prog; plan->grid = grid; plan->smem = smem; plan->args = a;
   return DEMI_OK;
 }
 
-static int32_t launch_fuzz(demi_handle* h, const demi_fuzz_params* p, void* out_dev, void* stream, bool reset_counters);
+// The lane engine over the plan's `n_items` work items when one applies, then the warp engine on the items it deferred
+// (on every item otherwise).  Counts both launches.
+static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, cudaStream_t s) {
+  KernelArgs& a = plan.args;
+  if (const LaneVariant* lv = pick_lane_variant(h, *plan.prog)) {
+    const kernel_fn lfn = lv->fn[plan.mode];
+    const size_t lsmem = lv->smem_per_block;
+    int32_t rc;
+    int bps = 0;
+    if ((rc = demi_occupancy(h, (const void*)lfn, lv->bd, lsmem, &bps)) != DEMI_OK) return rc;
+    if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "lane kernel does not fit on an SM");
+    uint64_t want = (n_items + lv->bd - 1) / lv->bd;
+    int lgrid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * bps));
+    const uint64_t lwarps = (uint64_t)lgrid * (lv->bd / 32);
+    if ((rc = ensure_bytes(h, (void**)&h->lane_pend, &h->lane_pend_bytes, lwarps * lv->lpcap * 32 * sizeof(uint4))) != DEMI_OK) return rc;
+    if ((rc = ensure_bytes(h, (void**)&h->ovf_list, &h->ovf_list_bytes, std::max<size_t>(n_items * sizeof(uint32_t), 64))) != DEMI_OK) return rc;
+    CUDA_TRY(h, cudaMemsetAsync(h->ovf_count, 0, sizeof(uint32_t), s));
+    KernelArgs la = a;
+    la.lane_pend = h->lane_pend;
+    la.ext_sends = plan.mode == LM_PROGRAM ? nullptr : h->ext_sends_dev;     // a campaign binds each program's table
+    la.has_partitions = plan.prog->partitions ? 1u : 0u;
+    la.prog_lane_pcap = h->lane_pending_cap;
+    la.ovf_list = h->ovf_list; la.ovf_count = h->ovf_count;
+    if (h->lane_pending_cap) la.pending_cap = std::min(la.pending_cap, h->lane_pending_cap);     // deferring is always exact
+    lfn<<<lgrid, lv->bd, lsmem, s>>>(la);
+    CUDA_TRY(h, cudaGetLastError());
+    h->perf.kernel_launches++;
+    // what the lane engine could not prove exact: a recording launch numbers its outputs by work-list position
+    if (plan.mode == LM_RECORD) { a.pos_list = h->ovf_list; a.pos_count = h->ovf_count; }
+    else { a.index_list = h->ovf_list; a.index_count = h->ovf_count; }
+  }
+  if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
+  plan.v->fn[plan.mode]<<<plan.grid, WARPS * 32, plan.smem, s>>>(a);
+  CUDA_TRY(h, cudaGetLastError());
+  h->perf.kernel_launches++;
+  return DEMI_OK;
+}
 
-// The counts of a new batch start from zero; demi_fuzz_summary_dev, or the host path once it syncs, fills the rest.
-static void reset_batch_perf(demi_handle* h) {
+// A new batch: its counters and counts start from zero (an empty batch, too, reports its own); demi_fuzz_summary_dev,
+// or the host path once it syncs, fills the rest.
+static int32_t reset_batch(demi_handle* h, cudaStream_t s) {
+  CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
   h->perf.kernel_launches = 0;
   h->perf.prefixes = 0;
   h->perf.deliveries = 0;
   h->perf.violations = 0;
   h->perf.deferred = 0;
-}
-
-extern "C" int32_t demi_fuzz_batch_dev(demi_handle* h, const demi_fuzz_params* p, void* out_dev, void* stream) {
-  return launch_fuzz(h, p, out_dev, stream, true);
-}
-
-// One launch of the lane engine over `n_items` work items; what it defers is appended to h->ovf_list / h->ovf_count.
-static int32_t launch_lane(demi_handle* h, const LaneVariant* lv, kernel_fn lfn, const KernelArgs& base, uint64_t n_items, cudaStream_t s,
-                           bool campaign = false) {
-  const size_t lsmem = lv->smem_per_block;
-  int bps = 0;
-  {
-    auto it = h->occupancy.find((const void*)lfn);
-    if (it == h->occupancy.end()) {
-      CUDA_TRY(h, cudaFuncSetAttribute(lfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsmem));
-      CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, lfn, lv->bd, lsmem));
-      h->occupancy[(const void*)lfn] = bps;
-    } else bps = it->second;
-  }
-  if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "lane kernel does not fit on an SM");
-  uint64_t want = (n_items + lv->bd - 1) / lv->bd;
-  int lgrid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * bps));
-  const uint64_t lwarps = (uint64_t)lgrid * (lv->bd / 32);
-  int32_t rc2;
-  if ((rc2 = ensure(h, (void**)&h->lane_pend, &h->lane_pend_bytes, lwarps * lv->lpcap * 32 * sizeof(uint4))) != DEMI_OK) return rc2;
-  if ((rc2 = ensure(h, (void**)&h->ovf_list, &h->ovf_list_bytes, std::max<size_t>(n_items * sizeof(uint32_t), 64))) != DEMI_OK) return rc2;
-  CUDA_TRY(h, cudaMemsetAsync(h->ovf_count, 0, sizeof(uint32_t), s));
-  KernelArgs la = base;
-  la.lane_pend = h->lane_pend;
-  la.ext_sends = campaign ? nullptr : h->ext_sends_dev;           // a campaign binds each program's table
-  la.has_partitions = (campaign ? h->fz_has_partitions : h->has_partitions) ? 1u : 0u;
-  la.prog_lane_pcap = h->lane_pending_cap;
-  la.ovf_list = h->ovf_list; la.ovf_count = h->ovf_count;
-  if (h->lane_pending_cap) la.pending_cap = std::min(la.pending_cap, h->lane_pending_cap);     // deferring is always exact
-  lfn<<<lgrid, lv->bd, lsmem, s>>>(la);
-  CUDA_TRY(h, cudaGetLastError());
-  h->perf.kernel_launches++;
   return DEMI_OK;
+}
+
+// demi_perf's counts from the engines' counters: deliveries, violations, and prefixes deferred to the warp engine
+static void read_counters(demi_handle* h, const unsigned long long* c) {
+  h->perf.deliveries = c[0];
+  h->perf.violations = c[1];
+  h->perf.deferred = (uint32_t)std::min<unsigned long long>(c[2], 0xFFFFFFFFull);
 }
 
 static int32_t launch_fuzz(demi_handle* h, const demi_fuzz_params* p, void* out_dev, void* stream, bool reset_counters) {
@@ -435,29 +422,19 @@ static int32_t launch_fuzz(demi_handle* h, const demi_fuzz_params* p, void* out_
   if (!out_dev) return fail(h, DEMI_ERR_INVALID, "demi_fuzz_batch_dev: null output");
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   LaunchPlan plan;
-  int32_t rc = plan_launch(h, p, false, &plan);
+  int32_t rc = plan_launch(h, p, LM_BATCH, h->ext_info, h->ext_dev, (uint32_t)h->ext_host.size(), &plan);
   if (rc != DEMI_OK) return rc;
   cudaStream_t s = (cudaStream_t)stream;
-  if (reset_counters) {                                        // an empty batch, too, reports its own (zero) counts
-    CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
-    reset_batch_perf(h);
-  }
+  if (reset_counters && (rc = reset_batch(h, s)) != DEMI_OK) return rc;
   if (p->n_prefixes == 0) return DEMI_OK;
   plan.args.results = (demi_fuzz_result*)out_dev;
-  const LaneVariant* lv = pick_lane_variant(h);
-  if (lv) {
-    // K1-lane handles every prefix it can prove exact; the rest are deferred to the warp engine
-    int32_t rc2 = launch_lane(h, lv, lv->fn, plan.args, p->n_prefixes, s);
-    if (rc2 != DEMI_OK) return rc2;
-    plan.args.index_list = h->ovf_list;
-    plan.args.index_count = h->ovf_count;
-  }
-  if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
-  plan.v->fn<<<plan.grid, WARPS * 32, plan.smem, s>>>(plan.args);
-  CUDA_TRY(h, cudaGetLastError());
-  h->perf.kernel_launches++;
+  if ((rc = launch_plan(h, plan, p->n_prefixes, s)) != DEMI_OK) return rc;
   h->perf.prefixes += p->n_prefixes;
   return DEMI_OK;
+}
+
+extern "C" int32_t demi_fuzz_batch_dev(demi_handle* h, const demi_fuzz_params* p, void* out_dev, void* stream) {
+  return launch_fuzz(h, p, out_dev, stream, true);
 }
 
 // Runs n records in chunks of `per` through launch(off, m, dst, first_chunk) on h->stream; chunk i's records travel to
@@ -465,7 +442,7 @@ static int32_t launch_fuzz(demi_handle* h, const demi_fuzz_params* p, void* out_
 template <class Launch>
 static int32_t run_pipelined(demi_handle* h, const char* who, uint64_t n, uint64_t per, demi_fuzz_result* out_host, Launch launch) {
   const size_t bytes = (size_t)n * sizeof(demi_fuzz_result);
-  int32_t rc = ensure(h, (void**)&h->results_dev, &h->results_cap, std::max<size_t>(bytes, 32));
+  int32_t rc = ensure_bytes(h, (void**)&h->results_dev, &h->results_cap, std::max<size_t>(bytes, 32));
   if (rc != DEMI_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev0, h->stream));
   if (n == 0) { rc = launch(0, 0, h->results_dev, true); if (rc != DEMI_OK) return rc; }
@@ -496,9 +473,7 @@ static int32_t run_pipelined(demi_handle* h, const char* who, uint64_t n, uint64
   float ms = 0;
   CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
   h->perf.kernel_ms = ms;
-  h->perf.deliveries = cnt[0];
-  h->perf.violations = cnt[1];
-  h->perf.deferred = (uint32_t)std::min<unsigned long long>(cnt[2], 0xFFFFFFFFull);      // deferred to the general engine
+  read_counters(h, cnt);
   h->perf.d2h_bytes = bytes + sizeof(cnt);
   h->perf.h2d_bytes = 0;
   return DEMI_OK;
@@ -531,29 +506,26 @@ extern "C" int32_t demi_fuzz_summary_dev(demi_handle* h, const void* /*results_d
   CUDA_TRY(h, cudaStreamSynchronize((cudaStream_t)stream));
   if (sum_steps) *sum_steps = c[0];
   if (n_violations) *n_violations = c[1];
-  h->perf.deliveries = c[0];
-  h->perf.violations = c[1];
-  h->perf.deferred = (uint32_t)std::min<unsigned long long>(c[2], 0xFFFFFFFFull);
+  read_counters(h, c);
   return DEMI_OK;
 }
 
-extern "C" int32_t demi_fuzz_trace(demi_handle* h, const demi_fuzz_params* p, int64_t seed,
-                                   demi_event* events, uint32_t cap_events, uint32_t* n_events,
-                                   uint16_t* dep_parent, uint32_t cap_nodes, uint32_t* n_nodes,
-                                   demi_fuzz_result* result) {
-  if (!h) return DEMI_ERR_INVALID;
+// demi_fuzz_trace over the program (ext, n_ext) that `prog` describes: one prefix, recorded by the warp engine
+static int32_t fuzz_trace(demi_handle* h, const demi_fuzz_params* p, int64_t seed, demi_event* events, uint32_t cap_events,
+                          uint32_t* n_events, uint16_t* dep_parent, uint32_t cap_nodes, uint32_t* n_nodes, demi_fuzz_result* result,
+                          const demi_ext_event* ext, uint32_t n_ext, const ProgramInfo& prog) {
   if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
   if (!events || !cap_events) return fail(h, DEMI_ERR_INVALID, "demi_fuzz_trace: events buffer required");
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   demi_fuzz_params q = *p;
   q.seed_base = seed; q.n_prefixes = 1;
   LaunchPlan plan;
-  int32_t rc = plan_launch(h, &q, true, &plan);
+  int32_t rc = plan_launch(h, &q, LM_RECORD, prog, ext, n_ext, &plan);
   if (rc != DEMI_OK) return rc;
   const uint32_t cap_ev = std::max<uint32_t>(cap_events, 1), cap_n = std::max<uint32_t>(cap_nodes, 1);
   // one recording buffer, kept in the handle: events | parents | result
   const size_t o_par = (size_t)cap_ev * sizeof(demi_event), o_res = (o_par + (size_t)cap_n * 2 + 15) & ~(size_t)15;
-  if ((rc = ensure(h, &h->trace_rec, &h->trace_rec_bytes, o_res + sizeof(demi_fuzz_result))) != DEMI_OK) return rc;
+  if ((rc = ensure_bytes(h, &h->trace_rec, &h->trace_rec_bytes, o_res + sizeof(demi_fuzz_result))) != DEMI_OK) return rc;
   demi_event* ev_dev = (demi_event*)h->trace_rec;
   uint16_t* par_dev = (uint16_t*)((unsigned char*)h->trace_rec + o_par);
   demi_fuzz_result* res_dev = (demi_fuzz_result*)((unsigned char*)h->trace_rec + o_res);
@@ -562,8 +534,8 @@ extern "C" int32_t demi_fuzz_trace(demi_handle* h, const demi_fuzz_params* p, in
   plan.args.rec_counts = h->rec_counts_dev;
   plan.args.rec_parent = dep_parent ? par_dev : nullptr; plan.args.rec_parent_cap = cap_nodes;
   CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), h->stream));
-  if (h->cfg.model == DEMI_MODEL_IR) ir_bind(h->ir_dev, h->stream);
-  plan.v->fn<<<1, WARPS * 32, plan.smem, h->stream>>>(plan.args);
+  if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, h->stream));
+  plan.v->fn[LM_RECORD]<<<1, WARPS * 32, plan.smem, h->stream>>>(plan.args);
   cudaError_t e = cudaGetLastError();
   demi_fuzz_result r{}; uint32_t counts[4] = {0, 0, 0, 0};
   if (e == cudaSuccess) e = cudaMemcpyAsync(&r, res_dev, sizeof(r), cudaMemcpyDeviceToHost, h->stream);
@@ -582,6 +554,15 @@ extern "C" int32_t demi_fuzz_trace(demi_handle* h, const demi_fuzz_params* p, in
   return DEMI_OK;
 }
 
+extern "C" int32_t demi_fuzz_trace(demi_handle* h, const demi_fuzz_params* p, int64_t seed,
+                                   demi_event* events, uint32_t cap_events, uint32_t* n_events,
+                                   uint16_t* dep_parent, uint32_t cap_nodes, uint32_t* n_nodes,
+                                   demi_fuzz_result* result) {
+  if (!h) return DEMI_ERR_INVALID;
+  return fuzz_trace(h, p, seed, events, cap_events, n_events, dep_parent, cap_nodes, n_nodes, result, h->ext_dev,
+                    (uint32_t)h->ext_host.size(), h->ext_info);
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Provenance pruning (ProvenanceTracker, schedulers/Util.scala:267-376)
 static int32_t launch_provenance(demi_handle* h, ProvArgs a, cudaStream_t s) {
@@ -590,7 +571,7 @@ static int32_t launch_provenance(demi_handle* h, ProvArgs a, cudaStream_t s) {
   const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * 8));
   a.t_cap = a.mask_words * 64;
   a.scratch_stride = a.t_cap + 3 * a.par_stride;
-  int32_t rc = ensure(h, (void**)&h->prov_scratch, &h->prov_scratch_bytes,
+  int32_t rc = ensure_bytes(h, (void**)&h->prov_scratch, &h->prov_scratch_bytes,
                       (uint64_t)grid * PW * a.scratch_stride * sizeof(uint32_t));
   if (rc != DEMI_OK) return rc;
   a.scratch = (uint32_t*)h->prov_scratch;
@@ -653,7 +634,7 @@ extern "C" int32_t demi_fuzz_provenance(demi_handle* h, const demi_fuzz_params* 
   demi_fuzz_params q = *p;
   q.n_prefixes = n;
   LaunchPlan plan;
-  int32_t rc = plan_launch(h, &q, true, &plan);
+  int32_t rc = plan_launch(h, &q, LM_RECORD, h->ext_info, h->ext_dev, (uint32_t)h->ext_host.size(), &plan);
   if (rc != DEMI_OK) return rc;
   // an execution records at most one MsgSend + one MsgEvent per message, plus the external markers
   const uint32_t node_cap = plan.args.node_cap;
@@ -685,6 +666,7 @@ extern "C" int32_t demi_fuzz_provenance(demi_handle* h, const demi_fuzz_params* 
   if (e == cudaSuccess) e = cudaMemcpyAsync(d_n, &n, 4, cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = cudaMemsetAsync(d_cnt, 0, b_cnt, s);
   if (e == cudaSuccess) e = cudaMemsetAsync(d_res, 0xFF, b_res, s);
+  if (e == cudaSuccess) e = cudaEventRecord(h->ev0, s);
   if (e == cudaSuccess) {
     plan.args.results = (demi_fuzz_result*)d_res;
     plan.args.index_list = (const uint32_t*)d_idx; plan.args.index_count = (const uint32_t*)d_n;
@@ -692,21 +674,9 @@ extern "C" int32_t demi_fuzz_provenance(demi_handle* h, const demi_fuzz_params* 
     plan.args.rec_counts = (uint32_t*)d_cnt;
     plan.args.rec_parent = (uint16_t*)d_par; plan.args.rec_parent_cap = node_cap;
     plan.args.sum_steps = nullptr; plan.args.n_violations = nullptr;
-    cudaEvent_t t0, t1; cudaEventCreate(&t0); cudaEventCreate(&t1);
-    cudaEventRecord(t0, s);
-    if (h->cfg.model == DEMI_MODEL_IR) ir_bind(h->ir_dev, s);
     // the lane engine records every execution it can prove exact; the slots it defers go to the general engine
-    const LaneVariant* lv = pick_lane_variant(h);
-    if (lv) {
-      rc = launch_lane(h, lv, lv->fn_rec, plan.args, n, s);
-      plan.args.pos_list = h->ovf_list; plan.args.pos_count = h->ovf_count;
-    }
+    rc = launch_plan(h, plan, n, s);
     if (rc == DEMI_OK) {
-      plan.v->fn<<<plan.grid, WARPS * 32, plan.smem, s>>>(plan.args);
-      e = cudaGetLastError();
-      h->perf.kernel_launches++;
-    }
-    if (rc == DEMI_OK && e == cudaSuccess) {
       ProvArgs a{};
       a.events = (const demi_event*)buf; a.ev_stride = ev_cap;
       a.parent = (const uint16_t*)d_par; a.par_stride = node_cap;
@@ -714,14 +684,13 @@ extern "C" int32_t demi_fuzz_provenance(demi_handle* h, const demi_fuzz_params* 
       a.keep = (uint64_t*)d_keep; a.mask_words = mask_words; a.out = (demi_provenance_out*)d_out; a.n = n;
       rc = launch_provenance(h, a, s);
     }
-    cudaEventRecord(t1, s);
+    e = cudaEventRecord(h->ev1, s);
     if (rc == DEMI_OK && e == cudaSuccess) e = cudaMemcpyAsync(keep_masks, d_keep, b_keep, cudaMemcpyDeviceToHost, s);
     if (rc == DEMI_OK && e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, b_out, cudaMemcpyDeviceToHost, s);
     if (rc == DEMI_OK && e == cudaSuccess && results) e = cudaMemcpyAsync(results, d_res, b_res, cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     float ms = 0.f;
-    if (e == cudaSuccess && cudaEventElapsedTime(&ms, t0, t1) == cudaSuccess) h->perf.kernel_ms = ms;
-    cudaEventDestroy(t0); cudaEventDestroy(t1);
+    if (e == cudaSuccess && (e = cudaEventElapsedTime(&ms, h->ev0, h->ev1)) == cudaSuccess) h->perf.kernel_ms = ms;
   }
   cudaFree(buf);
   if (rc != DEMI_OK) return rc;
@@ -750,36 +719,23 @@ extern "C" int32_t demi_set_fuzzer(demi_handle* h, const demi_fuzzer_config* cfg
   if (!h) return DEMI_ERR_INVALID;
   if (!cfg || (!prefix && n_prefix) || (!postfix && n_postfix)) return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: null argument");
   { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
-  const int na = demi_model_actors(h);
-  uint32_t starts = 0, sends = 0;
-  bool hard_kill = false, partitions = false, distinct = true;
+  uint32_t starts = 0;
+  ProgramInfo info;
   std::vector<uint4> sv;
   for (int part = 0; part < 2; part++) {
     const demi_ext_event* ev = part ? postfix : prefix;
     const uint32_t n = part ? n_postfix : n_prefix;
-    const char* where = part ? "postfix" : "prefix";
     for (uint32_t i = 0; i < n; i++) {
       const demi_ext_event& e = ev[i];
-      if (e.kind < DEMI_EXT_START || e.kind > DEMI_EXT_HARD_KILL)
-        return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: %s event %u has unknown kind %u", where, i, e.kind);
-      const bool needs_a = e.kind != DEMI_EXT_WAIT_QUIESCENCE;
-      const bool needs_b = e.kind == DEMI_EXT_PARTITION || e.kind == DEMI_EXT_UNPARTITION;
-      if ((needs_a && e.a >= na) || (needs_b && e.b >= na))
-        return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: %s event %u names an unknown actor", where, i);
-      if (e.kind == DEMI_EXT_WAIT_QUIESCENCE && i > 0 && ev[i - 1].kind == DEMI_EXT_WAIT_QUIESCENCE)
-        return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: consecutive WaitQuiescence at %s event %u", where, i);
+      const int32_t rc = demi_check_external(h, "demi_set_fuzzer", part ? "postfix " : "prefix ", ev, i, true, true);
+      if (rc != DEMI_OK) return rc;
       if (!part && e.kind == DEMI_EXT_START) starts++;
-      if (e.kind == DEMI_EXT_HARD_KILL) hard_kill = true;
-      if (needs_b) partitions = true;
-      if (e.kind != DEMI_EXT_SEND) continue;
-      sends++;
+      describe_event(&info, &sv, e);
       // the lane engine's screen (demi_set_externals): no two Sends of a program may be equal.  A generated Send is
       // (alive actor, send_type, p0 = counter in 1..num_events, p1 = 0); a fixed Send that could equal one screens
       // the campaign out, whichever actor the generated one picks.
-      const uint4 m = make_uint4((uint32_t)e.a | ((uint32_t)e.type << 8), e.p0, e.p1, 0u);
-      for (const uint4& o : sv) if (o.x == m.x && o.y == m.y && o.z == m.z) distinct = false;
-      if (cfg->send > 0.0 && e.type == cfg->send_type && e.p1 == 0 && e.p0 >= 1 && e.p0 <= cfg->num_events) distinct = false;
-      sv.push_back(m);
+      if (e.kind == DEMI_EXT_SEND && cfg->send > 0.0 && e.type == cfg->send_type && e.p1 == 0 && e.p0 >= 1 && e.p0 <= cfg->num_events)
+        info.sends_distinct = false;
     }
   }
   if (!starts) return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: the prefix has no Start (the Fuzzer's actors are the prefix's Starts, Fuzzer.scala:60)");
@@ -806,10 +762,9 @@ extern "C" int32_t demi_set_fuzzer(demi_handle* h, const demi_fuzzer_config* cfg
       CUDA_TRY(h, cudaMemcpy(h->fz_fixed_dev + n_prefix, postfix, (size_t)n_postfix * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
   }
   h->fuzzer = *cfg; h->fz_n_prefix = n_prefix; h->fz_n_postfix = n_postfix;
-  h->fz_max_sends = sends + cfg->num_events;
-  h->fz_has_hard_kill = hard_kill;
-  h->fz_has_partitions = partitions || cfg->partition > 0.0;
-  h->fz_sends_distinct = distinct;
+  info.sends += cfg->num_events;                 // the largest program's
+  info.partitions |= cfg->partition > 0.0;
+  h->fz_info = info;
   h->has_fuzzer = true;
   return DEMI_OK;
 }
@@ -831,15 +786,35 @@ fuzzer_gen_kernel(const demi_fuzzer_config cfg, int64_t seed_base, uint64_t n, c
   uint4* st = sends + i * send_stride;
   for (uint32_t j = 0, k = 0; j < len; j++) {
     const demi_ext_event e = out[j];
-    if (e.kind == DEMI_EXT_SEND)
-      st[k++] = make_uint4(DEMI_DEADLETTERS | ((uint32_t)e.a << 8) | ((uint32_t)e.type << 16) | ((uint32_t)DEMI_MF_EXTERNAL << 24), e.p0, e.p1, 0u);
+    if (e.kind == DEMI_EXT_SEND) st[k++] = lane_send(e);
   }
+}
+
+// The arena in h->fz_arena of `n` programs, as the PROG engines read them: program i's events at ev[i * stride ..),
+// hdr[i] = {length, Sends}, its lane-form Sends at sends[i * send_stride ..); then `extra` bytes for the caller at *rest.
+struct ProgramArena { demi_ext_event* ev; uint2* hdr; uint4* sends; uint32_t stride, send_stride; };
+static int32_t carve_programs(demi_handle* h, uint64_t n, uint32_t stride, uint32_t send_stride, size_t extra, ProgramArena* pa,
+                              unsigned char** rest = nullptr) {
+  const size_t b_ev = (size_t)n * stride * sizeof(demi_ext_event), b_hdr = ((size_t)n * sizeof(uint2) + 15) & ~(size_t)15,
+               b_snd = (size_t)n * send_stride * sizeof(uint4);
+  int32_t rc = ensure_bytes(h, &h->fz_arena, &h->fz_arena_bytes, b_ev + b_hdr + b_snd + extra);
+  if (rc != DEMI_OK) return rc;
+  unsigned char* a0 = (unsigned char*)h->fz_arena;
+  *pa = ProgramArena{(demi_ext_event*)a0, (uint2*)(a0 + b_ev), (uint4*)(a0 + b_ev + b_hdr), stride, send_stride};
+  if (rest) *rest = a0 + b_ev + b_hdr + b_snd;
+  return DEMI_OK;
+}
+static void bind_programs(const demi_handle* h, KernelArgs& a, const ProgramArena& pa, int32_t max_messages) {
+  a.prog_ext = pa.ev; a.prog_hdr = pa.hdr; a.prog_sends = pa.sends;
+  a.prog_stride = pa.stride; a.prog_send_stride = pa.send_stride;
+  a.prog_model_key = demi_model_key(h);
+  a.prog_max_messages = max_messages;
 }
 
 // programs per launch: the arena of one chunk stays under 512 MB
 static uint64_t campaign_chunk(const demi_handle* h, uint32_t* stride, uint32_t* send_stride) {
   *stride = (uint32_t)demi::fuzzer_program_room(h->fuzzer, h->fz_n_prefix, h->fz_n_postfix);
-  *send_stride = std::max(h->fz_max_sends, 1u);
+  *send_stride = std::max(h->fz_info.sends, 1u);
   const uint64_t per = (uint64_t)*stride * sizeof(demi_ext_event) + sizeof(uint2) + (uint64_t)*send_stride * sizeof(uint4);
   return std::max<uint64_t>(1, std::min<uint64_t>(2u << 20, ((uint64_t)512 << 20) / per));
 }
@@ -849,40 +824,22 @@ static uint64_t campaign_chunk(const demi_handle* h, uint32_t* stride, uint32_t*
 static int32_t launch_campaign(demi_handle* h, const demi_fuzz_params* p, int64_t program_seed_base, void* out_dev, cudaStream_t s,
                                bool reset_counters) {
   LaunchPlan plan;
-  int32_t rc = plan_launch(h, p, false, &plan, true);
+  int32_t rc = plan_launch(h, p, LM_PROGRAM, h->fz_info, nullptr, 0, &plan);
   if (rc != DEMI_OK) return rc;
   const uint64_t n = p->n_prefixes;
-  if (reset_counters) {                                        // an empty batch, too, reports its own (zero) counts
-    CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
-    reset_batch_perf(h);
-  }
+  if (reset_counters && (rc = reset_batch(h, s)) != DEMI_OK) return rc;
   if (n == 0) return DEMI_OK;
   uint32_t stride, send_stride;
   campaign_chunk(h, &stride, &send_stride);
-  const size_t b_ev = (size_t)n * stride * sizeof(demi_ext_event), b_hdr = ((size_t)n * sizeof(uint2) + 15) & ~(size_t)15;
-  if ((rc = ensure(h, &h->fz_arena, &h->fz_arena_bytes, b_ev + b_hdr + (size_t)n * send_stride * sizeof(uint4))) != DEMI_OK) return rc;
-  demi_ext_event* ev = (demi_ext_event*)h->fz_arena;
-  uint2* hdr = (uint2*)((unsigned char*)h->fz_arena + b_ev);
-  uint4* sends = (uint4*)((unsigned char*)h->fz_arena + b_ev + b_hdr);
+  ProgramArena pa;
+  if ((rc = carve_programs(h, n, stride, send_stride, 0, &pa)) != DEMI_OK) return rc;
   fuzzer_gen_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(h->fuzzer, program_seed_base, n, h->fz_fixed_dev, h->fz_n_prefix,
-                                                                 h->fz_n_postfix, ev, stride, hdr, sends, send_stride);
+                                                                 h->fz_n_postfix, pa.ev, stride, pa.hdr, pa.sends, send_stride);
   CUDA_TRY(h, cudaGetLastError());
   h->perf.kernel_launches++;
-  KernelArgs& a = plan.args;
-  a.results = (demi_fuzz_result*)out_dev;
-  a.prog_ext = ev; a.prog_hdr = hdr; a.prog_sends = sends;
-  a.prog_stride = stride; a.prog_send_stride = send_stride;
-  a.prog_model_key = demi_model_key(h);
-  a.prog_max_messages = p->max_messages;
-  if (const LaneVariant* lv = pick_lane_variant(h, true)) {
-    if ((rc = launch_lane(h, lv, lv->fn_prog, a, n, s, true)) != DEMI_OK) return rc;
-    a.index_list = h->ovf_list;
-    a.index_count = h->ovf_count;
-  }
-  if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
-  plan.v->fn_prog<<<plan.grid, WARPS * 32, plan.smem, s>>>(a);
-  CUDA_TRY(h, cudaGetLastError());
-  h->perf.kernel_launches++;
+  plan.args.results = (demi_fuzz_result*)out_dev;
+  bind_programs(h, plan.args, pa, p->max_messages);
+  if ((rc = launch_plan(h, plan, n, s)) != DEMI_OK) return rc;
   h->perf.prefixes += n;
   return DEMI_OK;
 }
@@ -959,9 +916,7 @@ random_subseq_kernel(const demi_ext_event* base, uint32_t n_ext, const uint64_t*
     const bool send = in && e.kind == DEMI_EXT_SEND;
     const uint32_t m = __ballot_sync(FULL_MASK, in), ms = __ballot_sync(FULL_MASK, send);
     if (in) events[t * stride + len + __popc(m & below)] = e;
-    if (send)
-      sends[t * send_stride + ns + __popc(ms & below)] =
-          make_uint4(DEMI_DEADLETTERS | ((uint32_t)e.a << 8) | ((uint32_t)e.type << 16) | ((uint32_t)DEMI_MF_EXTERNAL << 24), e.p0, e.p1, 0u);
+    if (send) sends[t * send_stride + ns + __popc(ms & below)] = lane_send(e);
     len += __popc(m); ns += __popc(ms);
   }
   if (lane == 0) hdr[t] = make_uint2(len, ns);
@@ -1015,27 +970,24 @@ static int32_t check_random(demi_handle* h, const char* who, uint32_t mask_words
 static int32_t random_tests(demi_handle* h, const uint64_t* masks, uint32_t n_tests, uint32_t mask_words, const demi_fuzz_params* p,
                             demi_random_test_result* out, uint64_t* executed) {
   const uint32_t N = (uint32_t)p->n_prefixes, n_ext = (uint32_t)h->ext_host.size();
-  const uint32_t stride = std::max(n_ext, 1u), send_stride = std::max(h->n_ext_sends, 1u);
+  const uint32_t stride = std::max(n_ext, 1u), send_stride = std::max(h->ext_info.sends, 1u);
   const uint64_t per_test = (uint64_t)stride * sizeof(demi_ext_event) + sizeof(uint2) + (uint64_t)send_stride * sizeof(uint4) +
                             (uint64_t)mask_words * 8 + sizeof(demi_random_test_result) + 4;
   const uint64_t per = std::max<uint64_t>(1, std::min<uint64_t>(RANDOM_EXECS_PER_LAUNCH / N, ((uint64_t)512 << 20) / per_test));
   const uint64_t cap_tests = std::min<uint64_t>(per, n_tests);
-  // arena: events | hdr | sends | masks | first_hit | test records | counter
-  const size_t b_ev = (size_t)cap_tests * stride * sizeof(demi_ext_event), b_hdr = ((size_t)cap_tests * sizeof(uint2) + 15) & ~(size_t)15,
-               b_snd = (size_t)cap_tests * send_stride * sizeof(uint4), b_mask = ((size_t)cap_tests * mask_words * 8 + 15) & ~(size_t)15,
-               b_fh = ((size_t)cap_tests * 4 + 15) & ~(size_t)15, b_out = ((size_t)cap_tests * sizeof(demi_random_test_result) + 15) & ~(size_t)15;
-  int32_t rc = ensure(h, &h->fz_arena, &h->fz_arena_bytes, b_ev + b_hdr + b_snd + b_mask + b_fh + b_out + 16);
+  // arena: the programs | masks | first_hit | test records | counter
+  const size_t b_mask = ((size_t)cap_tests * mask_words * 8 + 15) & ~(size_t)15, b_fh = ((size_t)cap_tests * 4 + 15) & ~(size_t)15,
+               b_out = ((size_t)cap_tests * sizeof(demi_random_test_result) + 15) & ~(size_t)15;
+  ProgramArena pa;
+  unsigned char* rest;
+  int32_t rc = carve_programs(h, cap_tests, stride, send_stride, b_mask + b_fh + b_out + 16, &pa, &rest);
   if (rc != DEMI_OK) return rc;
-  if ((rc = ensure(h, (void**)&h->results_dev, &h->results_cap, std::max<size_t>((size_t)cap_tests * N * sizeof(demi_fuzz_result), 32))) != DEMI_OK)
+  if ((rc = ensure_bytes(h, (void**)&h->results_dev, &h->results_cap, std::max<size_t>((size_t)cap_tests * N * sizeof(demi_fuzz_result), 32))) != DEMI_OK)
     return rc;
-  unsigned char* a0 = (unsigned char*)h->fz_arena;
-  demi_ext_event* ev = (demi_ext_event*)a0;
-  uint2* hdr = (uint2*)(a0 + b_ev);
-  uint4* sends = (uint4*)(a0 + b_ev + b_hdr);
-  uint64_t* mdev = (uint64_t*)(a0 + b_ev + b_hdr + b_snd);
-  uint32_t* first_hit = (uint32_t*)(a0 + b_ev + b_hdr + b_snd + b_mask);
-  demi_random_test_result* odev = (demi_random_test_result*)(a0 + b_ev + b_hdr + b_snd + b_mask + b_fh);
-  unsigned long long* cnt = (unsigned long long*)(a0 + b_ev + b_hdr + b_snd + b_mask + b_fh + b_out);
+  uint64_t* mdev = (uint64_t*)rest;
+  uint32_t* first_hit = (uint32_t*)(rest + b_mask);
+  demi_random_test_result* odev = (demi_random_test_result*)(rest + b_mask + b_fh);
+  unsigned long long* cnt = (unsigned long long*)(rest + b_mask + b_fh + b_out);
   cudaStream_t s = h->stream;
   CUDA_TRY(h, cudaMemsetAsync(cnt, 0, sizeof(unsigned long long), s));
   CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
@@ -1046,33 +998,22 @@ static int32_t random_tests(demi_handle* h, const uint64_t* masks, uint32_t n_te
     demi_fuzz_params q = *p;
     q.n_prefixes = (uint64_t)m * N;
     LaunchPlan plan;
-    if ((rc = plan_launch(h, &q, false, &plan, false, true)) != DEMI_OK) return rc;
+    if ((rc = plan_launch(h, &q, LM_TESTS, h->ext_info, h->ext_dev, n_ext, &plan)) != DEMI_OK) return rc;
     CUDA_TRY(h, cudaMemcpyAsync(mdev, masks + off * mask_words, (size_t)m * mask_words * 8, cudaMemcpyHostToDevice, s));
     CUDA_TRY(h, cudaMemsetAsync(first_hit, 0xFF, (size_t)m * 4, s));
-    random_subseq_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(h->ext_dev, n_ext, mdev, mask_words, m, ev, stride,
-                                                                                     hdr, sends, send_stride);
+    random_subseq_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(h->ext_dev, n_ext, mdev, mask_words, m, pa.ev, stride,
+                                                                                     pa.hdr, pa.sends, send_stride);
     CUDA_TRY(h, cudaGetLastError());
+    h->perf.kernel_launches++;
     KernelArgs& a = plan.args;
     a.results = h->results_dev;
-    a.prog_ext = ev; a.prog_hdr = hdr; a.prog_sends = sends;
-    a.prog_stride = stride; a.prog_send_stride = send_stride;
-    a.prog_model_key = demi_model_key(h);
-    a.prog_max_messages = p->max_messages;
+    bind_programs(h, a, pa, p->max_messages);
     a.prog_execs = N;
     a.prog_first_hit = first_hit;
-    // lane eligibility is decided on the base program: every condition pick_lane_variant checks (distinct Sends, no
-    // HardKill, ...) holds for each of its subsequences
-    if (const LaneVariant* lv = pick_lane_variant(h)) {
-      if ((rc = launch_lane(h, lv, lv->fn_tests, a, q.n_prefixes, s)) != DEMI_OK) return rc;
-      a.index_list = h->ovf_list;
-      a.index_count = h->ovf_count;
-    }
-    if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
-    plan.v->fn_tests<<<plan.grid, WARPS * 32, plan.smem, s>>>(a);
-    CUDA_TRY(h, cudaGetLastError());
+    if ((rc = launch_plan(h, plan, q.n_prefixes, s)) != DEMI_OK) return rc;
     random_test_reduce_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(h->results_dev, m, N, odev, cnt);
     CUDA_TRY(h, cudaGetLastError());
-    h->perf.kernel_launches += 3;        // launch_lane counts its own
+    h->perf.kernel_launches++;
     CUDA_TRY(h, cudaMemcpyAsync(out + off, odev, (size_t)m * sizeof(demi_random_test_result), cudaMemcpyDeviceToHost, s));
   }
   unsigned long long c[4] = {0, 0, 0, 0}, ran = 0;
@@ -1084,8 +1025,7 @@ static int32_t random_tests(demi_handle* h, const uint64_t* masks, uint32_t n_te
   CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
   h->perf.kernel_ms = ms;
   h->perf.prefixes = ran;
-  h->perf.deliveries = c[0]; h->perf.violations = c[1];
-  h->perf.deferred = (uint32_t)std::min<unsigned long long>(c[2], 0xFFFFFFFFull);
+  read_counters(h, c);
   h->perf.h2d_bytes = (uint64_t)n_tests * mask_words * 8;
   h->perf.d2h_bytes = (uint64_t)n_tests * sizeof(demi_random_test_result);
   *executed = ran;
@@ -1104,8 +1044,7 @@ extern "C" int32_t demi_random_test_batch(demi_handle* h, const uint64_t* masks,
   return random_tests(h, masks, n_tests, mask_words, p, out, &executed);
 }
 
-// demi_fuzz_trace over a subsequence of the handle's program: the program's host and device copies are swapped for
-// the subsequence's for the one recording launch, then restored
+// demi_fuzz_trace over the subsequence of the handle's program that `mask` keeps
 extern "C" int32_t demi_random_test_trace(demi_handle* h, const uint64_t* mask, uint32_t mask_words, const demi_fuzz_params* p,
                                           int64_t seed, demi_event* events, uint32_t cap_events, uint32_t* n_events,
                                           demi_fuzz_result* result) {
@@ -1114,13 +1053,12 @@ extern "C" int32_t demi_random_test_trace(demi_handle* h, const uint64_t* mask, 
   if (h->ext_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
   if ((uint64_t)mask_words * 64 < h->ext_host.size()) return fail(h, DEMI_ERR_INVALID, "demi_random_test_trace: mask_words too small");
   std::vector<demi_ext_event> sub;
-  uint32_t sends = 0;
-  bool hard_kill = false;
+  ProgramInfo info;
+  std::vector<uint4> sv;
   for (size_t i = 0; i < h->ext_host.size(); i++)
     if ((mask[i >> 6] >> (i & 63)) & 1ull) {
       sub.push_back(h->ext_host[i]);
-      sends += sub.back().kind == DEMI_EXT_SEND;
-      hard_kill |= sub.back().kind == DEMI_EXT_HARD_KILL;
+      describe_event(&info, &sv, sub.back());
     }
   if (sub.empty()) return fail(h, DEMI_ERR_INVALID, "demi_random_test_trace: the mask keeps no event");
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
@@ -1128,9 +1066,7 @@ extern "C" int32_t demi_random_test_trace(demi_handle* h, const uint64_t* mask, 
   CUDA_TRY(h, cudaMalloc(&dev, sub.size() * sizeof(demi_ext_event)));
   cudaError_t e = cudaMemcpy(dev, sub.data(), sub.size() * sizeof(demi_ext_event), cudaMemcpyHostToDevice);
   if (e != cudaSuccess) { cudaFree(dev); return fail(h, DEMI_ERR_CUDA, "demi_random_test_trace: %s", cudaGetErrorString(e)); }
-  std::swap(h->ext_dev, dev); h->ext_host.swap(sub); std::swap(h->n_ext_sends, sends); std::swap(h->has_hard_kill, hard_kill);
-  const int32_t rc = demi_fuzz_trace(h, p, seed, events, cap_events, n_events, nullptr, 0, nullptr, result);
-  std::swap(h->ext_dev, dev); h->ext_host.swap(sub); std::swap(h->n_ext_sends, sends); std::swap(h->has_hard_kill, hard_kill);
+  const int32_t rc = fuzz_trace(h, p, seed, events, cap_events, n_events, nullptr, 0, nullptr, result, dev, (uint32_t)sub.size(), info);
   cudaFree(dev);
   return rc;
 }

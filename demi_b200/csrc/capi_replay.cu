@@ -134,9 +134,11 @@ static int32_t launch_replay(demi_handle* h, const void* masks_dev, const void* 
   const ReplayVariant* rv = pick_rv(h->cfg.model);
   if (!rv) return fail(h, DEMI_ERR_INVALID, "no replay kernel for model %d", h->cfg.model);
   cudaStream_t s = (cudaStream_t)stream;
-  CUDA_TRY(h, cudaFuncSetAttribute(rv->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rv->smem));
-  int bps = 0;
-  CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, rv->fn, rv->bd, rv->smem));
+  // the grid (and the table's size) is the batch kernel's; the recording kernel runs one block of it
+  int32_t rc;
+  int bps = 0, rec_bps = 0;
+  if ((rc = demi_occupancy(h, (const void*)rv->fn, rv->bd, rv->smem, &bps)) != DEMI_OK) return rc;
+  if (record && (rc = demi_occupancy(h, (const void*)rv->fn_rec, rv->bd, rv->smem, &rec_bps)) != DEMI_OK) return rc;
   if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
   uint64_t want = ((uint64_t)n_masks + rv->bd - 1) / rv->bd;
   int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * bps));
@@ -158,7 +160,6 @@ static int32_t launch_replay(demi_handle* h, const void* masks_dev, const void* 
   a.pending_cap = demi_replay_pending_cap(h->trace_n_send_events);
   a.tosend_cap = demi_tosend_cap(h->trace_n_ext_sends);
   a.table_slots = demi_pow2_at_least(2 * a.pending_cap, 256, 1u << 16);
-  int32_t rc;
   const size_t table_bytes = warps * a.table_slots * 32 * sizeof(uint4);
   const bool fresh_table = h->rp_table_bytes < table_bytes;
   if ((rc = ensure_bytes(h, &h->rp_table, &h->rp_table_bytes, table_bytes)) != DEMI_OK) return rc;
@@ -181,14 +182,8 @@ static int32_t launch_replay(demi_handle* h, const void* masks_dev, const void* 
   a.table = (uint4*)h->rp_table; a.tosend = (uint32_t*)h->rp_tosend;
   a.pruned = (flags & DEMI_RF_FILTER_KNOWN_ABSENTS) ? (uint32_t*)h->rp_pruned : nullptr;
   a.counters = h->rp_counters;
-  if (record) {
-    CUDA_TRY(h, cudaFuncSetAttribute(rv->fn_rec, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rv->smem));
-    if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
-    rv->fn_rec<<<1, rv->bd, rv->smem, s>>>(a);
-  } else {
-    if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
-    rv->fn<<<grid, rv->bd, rv->smem, s>>>(a);
-  }
+  if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
+  (record ? rv->fn_rec : rv->fn)<<<record ? 1 : grid, rv->bd, rv->smem, s>>>(a);
   CUDA_TRY(h, cudaGetLastError());
   h->perf.kernel_launches = 1;
   h->perf.prefixes = n_masks;

@@ -85,9 +85,9 @@ int32_t wc_launch(demi_handle* h, const WcTrace& t, const uint64_t* include_host
   const bool record = rec_host != nullptr;
   cudaStream_t s = h->stream;
   wild_fn fn = record ? wv->fn_rec : wv->fn;
-  CUDA_TRY(h, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wv->smem));
+  int32_t rc;
   int bps = 0;
-  CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, fn, wv->bd, wv->smem));
+  if ((rc = demi_occupancy(h, (const void*)fn, wv->bd, wv->smem, &bps)) != DEMI_OK) return rc;
   if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
   const uint32_t n_ext = (uint32_t)h->trace_ext_host.size();
   ReplayArgs a{};
@@ -112,7 +112,6 @@ int32_t wc_launch(demi_handle* h, const WcTrace& t, const uint64_t* include_host
   a.gen_base = 1;
   a.wc_words = t.words;
   std::copy(h->clock_incr, h->clock_incr + 8, a.wc_incr);
-  int32_t rc;
   const size_t ev_bytes = t.ev.size() * sizeof(uint32_t), inc_bytes = (size_t)n_tests * t.words * sizeof(uint64_t);
   // staging in rp_masks: include masks | per-event modes | the two REC counters
   const size_t ev_off = (inc_bytes + 15) & ~(size_t)15, cnt_off = (ev_off + ev_bytes + 15) & ~(size_t)15;

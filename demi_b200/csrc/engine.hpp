@@ -19,6 +19,11 @@ extern thread_local std::string g_create_error;
 struct DedupScratch { void* keys = nullptr; size_t keys_b = 0; void* vals = nullptr; size_t vals_b = 0;
                       void* keep = nullptr; size_t keep_b = 0; void* counts = nullptr; size_t counts_b = 0; };
 
+// What the fuzz launches need to know about an external program: its Sends (for a Fuzzer, those of its largest
+// program), whether it has a HardKill or a Partition / UnPartition, and whether no two of its Sends are equal (two
+// equal Sends would share a DepTracker Unique under the root).
+struct ProgramInfo { uint32_t sends = 0; bool hard_kill = false, partitions = false, sends_distinct = true; };
+
 struct demi_handle {
   DedupScratch dedup;
   demi_config cfg{};
@@ -27,7 +32,7 @@ struct demi_handle {
   // external program
   std::vector<demi_ext_event> ext_host;
   demi_ext_event* ext_dev = nullptr;
-  uint32_t n_ext_sends = 0;
+  ProgramInfo ext_info;
   // device buffers
   demi_fuzz_result* results_dev = nullptr; size_t results_cap = 0;
   uint4* node_scratch = nullptr; size_t node_scratch_bytes = 0;
@@ -35,7 +40,6 @@ struct demi_handle {
   unsigned long long* counters_dev = nullptr;      // [0]=sum_steps [1]=n_violations
   // lane engine
   uint4* ext_sends_dev = nullptr;
-  bool has_partitions = false, ext_sends_distinct = true;
   uint4* lane_pend = nullptr; size_t lane_pend_bytes = 0;
   uint32_t* ovf_list = nullptr; size_t ovf_list_bytes = 0;
   uint32_t* ovf_count = nullptr;
@@ -75,7 +79,6 @@ struct demi_handle {
   std::vector<std::string> names;      // actor names, then message-type names
   // ---- FullyRandom's userDefinedFilter as rules (demi_set_user_filter); HardKill in the external program
   std::vector<demi_filter_rule> filter;
-  bool has_hard_kill = false;
   // ---- FingerprintFactory.getLogicalClock / causesClockIncrement as data (demi_set_clock_rules, capi_wildcard.cu):
   // per type the packed rule (0 = no clock; a valid rule has bits >= 1, so it is never 0) and the incrementing set
   uint32_t clock_rule[256] = {};
@@ -85,8 +88,7 @@ struct demi_handle {
   demi_fuzzer_config fuzzer{};
   uint32_t fz_n_prefix = 0, fz_n_postfix = 0;
   demi_ext_event* fz_fixed_dev = nullptr;                 // prefix | postfix
-  uint32_t fz_max_sends = 0;                              // Sends of the largest program: prefix + postfix + num_events
-  bool fz_has_hard_kill = false, fz_has_partitions = false, fz_sends_distinct = true;
+  ProgramInfo fz_info;                                    // sends: prefix + postfix + num_events
   void* fz_arena = nullptr; size_t fz_arena_bytes = 0;
   // ---- launch bookkeeping
   std::map<const void*, int> occupancy;          // kernel -> resident blocks per SM (asked once per handle)
@@ -95,8 +97,6 @@ struct demi_handle {
 void demi_replay_free(demi_handle* h);
 void demi_comm_free(demi_handle* h);
 void demi_frontier_free(demi_handle* h);
-
-inline int32_t ensure_bytes(demi_handle* h, void** p, size_t* cap, size_t need);
 
 inline int32_t fail(demi_handle* h, int32_t code, const char* fmt, ...) {
   char buf[512];
@@ -122,15 +122,27 @@ inline int32_t demi_need_model(demi_handle* h) {
   if (h->cfg.model == DEMI_MODEL_IR && !h->ir_loaded) return fail(h, DEMI_ERR_STATE, "demi_load_model has not been called");
   return DEMI_OK;
 }
-inline int32_t demi_check_externals(demi_handle* h, const char* who, const demi_ext_event* ev, uint32_t n) {
+// External event ev[i] of a program `who` was handed: a kind it accepts (HardKill only with `hard_kill`: RandomScheduler
+// fuzzing has it, replay and DPOR do not), actors of the model, and with `single_wait` no WaitQuiescence right after
+// another (MessageTypes.sanityCheckTrace, ExternalEvents.scala:138-149).  `where` names the part of the program, or is "".
+inline int32_t demi_check_external(demi_handle* h, const char* who, const char* where, const demi_ext_event* ev, uint32_t i,
+                                   bool hard_kill, bool single_wait) {
+  const demi_ext_event& e = ev[i];
   const uint32_t na = (uint32_t)demi_model_actors(h);
+  if (e.kind < DEMI_EXT_START || e.kind > (hard_kill ? DEMI_EXT_HARD_KILL : DEMI_EXT_UNPARTITION))
+    return fail(h, DEMI_ERR_INVALID, "%s: %sevent %u has kind %u, which this entry point does not accept", who, where, i, (unsigned)e.kind);
+  const bool needs_a = e.kind != DEMI_EXT_WAIT_QUIESCENCE;
+  const bool needs_b = e.kind == DEMI_EXT_PARTITION || e.kind == DEMI_EXT_UNPARTITION;
+  if ((needs_a && e.a >= na) || (needs_b && e.b >= na)) return fail(h, DEMI_ERR_INVALID, "%s: %sevent %u names an unknown actor", who, where, i);
+  if (single_wait && e.kind == DEMI_EXT_WAIT_QUIESCENCE && i > 0 && ev[i - 1].kind == DEMI_EXT_WAIT_QUIESCENCE)
+    return fail(h, DEMI_ERR_INVALID, "%s: consecutive WaitQuiescence at %sevent %u", who, where, i);
+  return DEMI_OK;
+}
+// a program to replay: no HardKill, consecutive WaitQuiescence allowed
+inline int32_t demi_check_externals(demi_handle* h, const char* who, const demi_ext_event* ev, uint32_t n) {
   for (uint32_t i = 0; i < n; i++) {
-    const demi_ext_event& e = ev[i];
-    if (e.kind < DEMI_EXT_START || e.kind > DEMI_EXT_UNPARTITION)      // HardKill: RandomScheduler fuzzing only
-      return fail(h, DEMI_ERR_INVALID, "%s: external %u has kind %u, which this entry point does not accept", who, i, (unsigned)e.kind);
-    const bool needs_a = e.kind != DEMI_EXT_WAIT_QUIESCENCE;
-    const bool needs_b = e.kind == DEMI_EXT_PARTITION || e.kind == DEMI_EXT_UNPARTITION;
-    if ((needs_a && e.a >= na) || (needs_b && e.b >= na)) return fail(h, DEMI_ERR_INVALID, "%s: external %u names an unknown actor", who, i);
+    const int32_t rc = demi_check_external(h, who, "", ev, i, false, false);
+    if (rc != DEMI_OK) return rc;
   }
   return DEMI_OK;
 }
@@ -167,5 +179,17 @@ inline int32_t ensure_bytes(demi_handle* h, void** p, size_t* cap, size_t need) 
   cudaFree(*p); *p = nullptr; *cap = 0;
   CUDA_TRY(h, cudaMalloc(p, need));
   *cap = need;
+  return DEMI_OK;
+}
+
+// Resident blocks per SM of kernel `fn` at `block` threads and `smem` bytes of dynamic shared memory (which it is
+// allowed first).  Both are fixed per device, so they are asked once per handle; the cache is keyed on the kernel
+// alone, so `smem` must be fixed per kernel too.
+inline int32_t demi_occupancy(demi_handle* h, const void* fn, int block, size_t smem, int* blocks_per_sm) {
+  auto it = h->occupancy.find(fn);
+  if (it != h->occupancy.end()) { *blocks_per_sm = it->second; return DEMI_OK; }
+  CUDA_TRY(h, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, fn, block, smem));
+  h->occupancy[fn] = *blocks_per_sm;
   return DEMI_OK;
 }
