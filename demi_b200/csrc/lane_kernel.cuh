@@ -154,20 +154,41 @@ struct LaneOutbox {
 };
 
 // small FIFO of bytes in four 32-bit registers: entry i is byte (i & 3) of w[i >> 2], and the bytes at and above n
-// are zero.  Every operation is a few byte permutes (PRMT) or bitwise ops on the words; none loops over the entries.
+// are zero.  Every operation is a few byte permutes (PRMT), funnel shifts or bitwise ops on the words; none loops over
+// the entries.
 struct ByteQueue16 {
   uint32_t w[4]; uint32_t n;
   __device__ __forceinline__ void clear() { w[0] = w[1] = w[2] = w[3] = 0; n = 0; }
-  __device__ __forceinline__ uint32_t get(uint32_t i) const {
-    const uint32_t q = i >> 2;
-    const uint32_t x = q == 0 ? w[0] : q == 1 ? w[1] : q == 2 ? w[2] : w[3];
-    return __byte_perm(x, 0u, 0x4440u | (i & 3u));
-  }
-  __device__ __forceinline__ void push(uint32_t b) {      // caller checks n < 16
-    const uint32_t v = b << ((n & 3u) * 8u);
+  // Word k takes byte b at bit 8n - 32k: a clamping funnel shift of b gives 0 wherever that is not in 0..24 (a
+  // "negative" amount wraps to a large one).  Caller checks n < 16.
+  __device__ __forceinline__ void push(uint32_t b) {
 #pragma unroll
-    for (uint32_t k = 0; k < 4; k++) if ((n >> 2) == k) w[k] |= v;
+    for (uint32_t k = 0; k < 4; k++) w[k] |= __funnelshift_lc(0u, b, n * 8u - 32u * k);
     n++;
+  }
+  // An empty queue takes the `len` bytes of hi:lo (those at and above len zero) as its entries.
+  __device__ __forceinline__ void assign(uint32_t lo, uint32_t hi, uint32_t len) { w[0] = lo; w[1] = hi; n = len; }
+  // Removes and returns entry 0: the queue shifts down one byte, and the zero bytes above n shift in behind it.
+  // Caller checks n > 0.
+  __device__ __forceinline__ uint32_t pop() {
+    const uint32_t b = w[0] & 0xFFu;
+    w[0] = __funnelshift_r(w[0], w[1], 8);
+    w[1] = __funnelshift_r(w[1], w[2], 8);
+    w[2] = __funnelshift_r(w[2], w[3], 8);
+    w[3] >>= 8;
+    n--;
+    return b;
+  }
+  // The index of the first entry equal to b (b < 0x80), or a value >= n when there is none.  All 16 bytes are compared
+  // at once (a SIMD byte compare per word, its byte masks gathered into one bit per entry); the zero bytes above n
+  // can match only b = 0, and only after every entry that does.
+  __device__ __forceinline__ uint32_t find(uint32_t b) const {
+    const uint32_t pat = b * 0x01010101u;
+    uint32_t bits = 0x10000u;
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++)
+      bits |= (((__vcmpeq4(w[k], pat) & 0x80808080u) * 0x00204081u) >> 28) << (4 * k);
+    return __ffs(bits) - 1u;
   }
   // Order preserving: every entry above i moves down one byte.  Word k is permuted with the word above it (byte 0 of
   // w[k+1] is byte 4 of the pair); it keeps its `keep` bytes below i and takes the next byte for each one above:
@@ -212,6 +233,7 @@ struct LaneMachine {
   static constexpr int OBW = DIRECT ? 0 : OB * 3;
   static constexpr uint32_t CT = MODEL::LANE_CANCEL_TYPE;            // 0: receive() cancels no timer
   static constexpr int TW = CT ? (N + 1) / 2 : 0;
+  static_assert(CT == 0 || LPCAP < 0xFF, "tcopy keeps a pending index in one byte, 0xFF meaning unknown");
   static constexpr int WORDS = N * SW + OBW + N + TW;      // states + outbox + partition rows + cancellable timer copies
 
   uint32_t* smw;             // &smem[tid]; word w at smw[w*BD]
@@ -298,13 +320,15 @@ struct LaneMachine {
     st_l2_hint(pend + i, last, pol);
     n_pending--;
     if constexpr (CT != 0) {
-      if (cancellable_timer(v.x)) {
-        const uint32_t a = hdr_dst(v.x);
-        tcopy_set(a, ((tcopy(a) & 0xFFu) - 1u) | 0xFF00u);
+      // in place on the actor's half of the word: the count is at least 1 here, and indices stay below LPCAP < 0xFF
+      if (cancellable_timer(v.x)) {                      // one copy fewer, its index no longer known
+        const uint32_t a = hdr_dst(v.x), sh = (a & 1u) * 16;
+        tcopy_word(a) = (tcopy_word(a) - (1u << sh)) | (0xFF00u << sh);
       }
       if (cancellable_timer(last.x)) {                   // moved from index n_pending to i
-        const uint32_t a = hdr_dst(last.x), e = tcopy(a);
-        if ((e >> 8) == n_pending) tcopy_set(a, (e & 0xFFu) | (i << 8));
+        const uint32_t a = hdr_dst(last.x), sh = (a & 1u) * 16 + 8;
+        uint32_t& w = tcopy_word(a);
+        if (((w >> sh) & 0xFFu) == n_pending) w ^= (n_pending ^ i) << sh;
       }
     }
     return v;
@@ -401,23 +425,15 @@ struct LaneMachine {
     record_event(DEMI_EV_MSG_SEND, hdr_src(hdr), dst, type, p0, p1, w3, 0u);
   }
 
-  // ExternalEventInjector.handle_timer (ExternalEventInjector.scala:282-297)
-  __device__ __forceinline__ void handle_timer(uint32_t slot) {
-    if (A->ignore_timers) return;
-    if (tosend.n >= LANE_TOSEND_CAP || tosend.n >= A->tosend_cap) { defer(); return; }
-    tosend.push(slot);
+  // RandomScheduler.enqueue_timer (RandomScheduler.scala:549-559) of a slot whose justScheduledTimers bit is set
+  __device__ __forceinline__ void resend_push(uint32_t slot) {
+    if (n_resend >= LANE_RESEND_CAP) { defer(); return; }
+    resend |= (uint64_t)slot << (n_resend * 8);
+    n_resend++;
   }
-  // RandomScheduler.enqueue_timer (RandomScheduler.scala:549-559)
-  __device__ __forceinline__ void enqueue_timer(uint32_t slot) {
-    if ((just >> slot) & 1u) {
-      if (n_resend >= LANE_RESEND_CAP) { defer(); return; }
-      resend |= (uint64_t)slot << (n_resend * 8);
-      n_resend++;
-      return;
-    }
-    handle_timer(slot);
-  }
-  // scheduler.scheduleOnce / schedule (Instrumenter.scala:1126-1190)
+  // scheduler.scheduleOnce / schedule (Instrumenter.scala:1126-1190), then RandomScheduler.enqueue_timer ->
+  // ExternalEventInjector.handle_timer (ExternalEventInjector.scala:282-297).  This is the only place a single timer
+  // enters messagesToSend.
   __device__ __forceinline__ void schedule_timer(uint32_t kind, uint32_t self, uint32_t type, uint32_t p0, uint32_t p1) {
     if (status) return;
     const int s2 = MODEL::timer_slot(self, type, p0, p1);
@@ -427,7 +443,10 @@ struct LaneMachine {
       if (__popc(registry) >= DEMI_TIMERSET_CAP) { defer(); return; }
       registry |= 1u << s2;
     }
-    enqueue_timer((uint32_t)s2);
+    if ((just >> s2) & 1u) { resend_push((uint32_t)s2); return; }
+    if (A->ignore_timers) return;
+    if (tosend.n >= LANE_TOSEND_CAP || tosend.n >= A->tosend_cap) { defer(); return; }
+    tosend.push((uint32_t)s2);
   }
   // First the ops receive() left in the outbox (`n_ops`, sender `self`), in program order; then, if `do_flush`,
   // ExternalEventInjector.send_external_messages (ExternalEventInjector.scala:306-365).  Two loops, so that the
@@ -445,9 +464,11 @@ struct LaneMachine {
       }
     }
     if (status || !do_flush) return;
+    // in order from the front; a flush that runs to the end leaves the queue empty (a deferred prefix's queue is
+    // never read again)
 #pragma unroll 1
-    for (uint32_t i = 0; i < tosend.n && !status; i++) {
-      const uint32_t b = tosend.get(i);
+    while (tosend.n != 0 && !status) {
+      const uint32_t b = tosend.pop();
       if (b & 0x80u) {
         const uint4 raw = __ldg(reinterpret_cast<const uint4*>(A->ext_sends) + (b & 0x7Fu));
         external_produced(raw.x, raw.y, raw.z);
@@ -455,7 +476,6 @@ struct LaneMachine {
         timer_produced(b);
       }
     }
-    if (!status) tosend.clear();
   }
 
   // Cancellable.cancel(): Instrumenter.cancelTimer (Instrumenter.scala:159-168) ->
@@ -468,8 +488,8 @@ struct LaneMachine {
     if (!(cancelled & bit) && __popc(cancelled) >= DEMI_TIMERSET_CAP) { defer(); return; }
     cancelled |= bit;
     registry &= ~bit;
-    for (uint32_t i = 0; i < tosend.n; i++)           // handle_timer_cancel (ExternalEventInjector.scala:601-610)
-      if (tosend.get(i) == (uint32_t)slot) { tosend.remove_at(i); return; }
+    const uint32_t at = tosend.find((uint32_t)slot);  // handle_timer_cancel (ExternalEventInjector.scala:601-610)
+    if (at < tosend.n) { tosend.remove_at(at); return; }
     // FullyRandom.remove (RandomScheduler.scala:653-664): first match in array order.  The only entries that match are
     // the slot's timer messages: for the tracked type CT, with none pending there is nothing to remove, and a single
     // copy at a known index is the first match.  Otherwise the array is scanned, four entries fetched per step so that
@@ -563,24 +583,27 @@ struct LaneMachine {
     parent_event = pick.w >> 16;                                // reportNewlyDelivered (DepTracker.scala:132-135)
     window_timers = 0;
     // updateRepeatingTimer :405-421
-    int slot = MODEL::timer_slot(dst, type, pick.y, pick.z);
+    const int slot = MODEL::timer_slot(dst, type, pick.y, pick.z);
     if (slot >= 0 && ((registry >> slot) & 1u)) {
       just |= 1u << slot;
+      // Instrumenter.dispatch_new_message's re-arm of the repeating timer (Instrumenter.scala:1008-1016), applied
+      // here, before receive() as there: its enqueue_timer finds the just-set bit, so the slot goes to resend
+      resend_push((uint32_t)slot);
     } else {
-      for (uint32_t i = 0; i < n_resend; i++) handle_timer((uint32_t)(resend >> (i * 8)) & 0xFFu);
+      // handle_timer of each re-send entry, in order.  messagesToSend is empty here: run() flushed it to the end just
+      // before this pick (a flush that defers ends the execution), so the list becomes the whole queue, and its at most
+      // LANE_RESEND_CAP entries always fit.
+      if (!A->ignore_timers) tosend.assign((uint32_t)resend, (uint32_t)(resend >> 32), n_resend);
       resend = 0; n_resend = 0;
       just = 0;
     }
     return !status;
   }
 
-  // Instrumenter.dispatch_new_message (Instrumenter.scala:913-1017)
+  // Instrumenter.dispatch_new_message (Instrumenter.scala:913-1017); pick_next has re-armed a repeating timer
   // returns the number of outbox ops receive() produced (applied by drain())
   __device__ __forceinline__ uint32_t dispatch_new_message(const uint4& pick) {
     uint32_t src = hdr_src(pick.x), dst = hdr_dst(pick.x), type = hdr_type(pick.x);
-    int slot = MODEL::timer_slot(dst, type, pick.y, pick.z);
-    if (slot >= 0 && ((registry >> slot) & 1u)) enqueue_timer((uint32_t)slot);     // re-arm :1008-1016
-    if (status) return 0;
     if constexpr (DIRECT) {
       LaneDirectOutbox<LaneMachine> direct{this, dst};
       MODEL::receive(direct, dst, actor(dst), src, type, pick.y, pick.z, A->model_flags);
