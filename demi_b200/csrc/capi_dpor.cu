@@ -84,7 +84,7 @@ int32_t dpor_run(demi_handle* h, const demi_ext_event* ext, const uint32_t* ext_
     if (ext[i].a >= n_actors) return fail(h, DEMI_ERR_INVALID, "demi_dpor_batch: external %u names an unknown actor", i);
   }
   DporArgs a{};
-  a.model_flags = h->cfg.model_flags; a.blocked_mask = h->cfg.blocked_mask; a.ignore_timers = h->cfg.ignore_timers;
+  a.model_flags = h->cfg.model_flags; a.blocked_mask = h->cfg.blocked_mask;
   a.P = P; a.n_searches = n_searches; a.cap_viol = cap_viol; a.cap_hashes = cap_hashes;
   a.T1 = (uint32_t)P.max_messages + 2;
   a.child_slots = demi_pow2_at_least(2 * P.node_cap, 4, 1u << 22);

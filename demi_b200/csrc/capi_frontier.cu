@@ -224,7 +224,7 @@ int32_t fr_setup(FrState& st, const demi_ext_event* ext, uint32_t n_ext, bool re
   CUDA_TRY(h, cudaFuncSetAttribute(fr_scatter_kernel<SCAN_WPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cnt_smem));
   st.brq.assign(st.T1, {}); st.branch_live.assign(st.T1, 0);
   FrArgs& A = st.A;
-  A.model_flags = h->cfg.model_flags; A.blocked_mask = h->cfg.blocked_mask; A.ignore_timers = h->cfg.ignore_timers;
+  A.model_flags = h->cfg.model_flags; A.blocked_mask = h->cfg.blocked_mask;
   A.max_messages = F.max_messages; A.looking_for = F.looking_for; A.no_history = (F.flags & DEMI_FR_NO_HISTORY) ? 1u : 0u;
   A.ext = st.ext_dev; A.n_ext = n_ext; A.T1 = st.T1;
   A.tr = st.tr; A.tr_meta = st.tr_meta; A.E = st.E; A.e_slots = F.explored_slots;

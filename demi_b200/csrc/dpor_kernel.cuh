@@ -36,7 +36,7 @@ __host__ __device__ __forceinline__ uint32_t dpor_key_later(DporKey q) { return 
 __host__ __device__ __forceinline__ uint32_t dpor_key_earlier(DporKey q) { return 0xFFFu - (uint32_t)(q & 0xFFFu); }
 
 struct DporArgs {
-  uint32_t model_flags, blocked_mask; int32_t ignore_timers;
+  uint32_t model_flags, blocked_mask;
   demi_dpor_params P;
   const uint4* ext; const uint32_t* ext_offsets; uint32_t n_searches;
   demi_dpor_result* results;
@@ -127,8 +127,9 @@ struct DporMachine {
       qlen[q]++;
     }
   }
-  __device__ __forceinline__ void timer_send(uint32_t slot) {        // enqueue_timer = enqueue_message (Scheduler.scala:73)
-    if (A->ignore_timers) return;
+  // enqueue_timer = enqueue_message (Scheduler.scala:73): sent at once, whatever ignoreTimers says — the reference reads
+  // that flag only in ExternalEventInjector.handle_timer (ExternalEventInjector.scala:283-285), which DPOR never calls
+  __device__ __forceinline__ void timer_send(uint32_t slot) {
     uint32_t dst, type, p0, p1;
     MODEL::slot_msg(slot, dst, type, p0, p1);
     event_produced(DEMI_DEADLETTERS, dst, type, p0, p1);

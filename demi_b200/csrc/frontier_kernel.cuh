@@ -42,7 +42,7 @@ enum { FRC_DELIVERIES = 0, FRC_VIOLATIONS = 1, FRC_RACES = 2, FRC_EXPLORED = 3, 
 
 struct FrArgs {
   FrLog log;
-  uint32_t model_flags, blocked_mask; int32_t ignore_timers;
+  uint32_t model_flags, blocked_mask;
   int32_t max_messages; uint32_t looking_for;
   const uint4* ext; uint32_t n_ext;
   uint32_t T1;
@@ -161,8 +161,8 @@ struct FrExec {
       if (prev == NIL) qmask[q >> 5] &= ~(1u << (q & 31));
     }
   }
-  __device__ __forceinline__ void timer_send(uint32_t slot) {          // enqueue_timer = enqueue_message (Scheduler.scala:73)
-    if (A->ignore_timers) return;
+  // enqueue_timer = enqueue_message (Scheduler.scala:73), whatever ignoreTimers says (see DporMachine::timer_send)
+  __device__ __forceinline__ void timer_send(uint32_t slot) {
     uint32_t dst, type, p0, p1;
     MODEL::slot_msg(slot, dst, type, p0, p1);
     event_produced(DEMI_DEADLETTERS, dst, type, p0, p1);

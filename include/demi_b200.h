@@ -127,7 +127,13 @@ typedef struct demi_config {
   int32_t  model;             /* DEMI_MODEL_*                                   */
   uint32_t model_flags;       /* model-defined (raft5: seeded-bug bits)        */
   uint32_t blocked_mask;      /* Instrumenter.blockedActors as a bitmask       */
-  int32_t  ignore_timers;     /* SchedulerConfig.ignoreTimers                  */
+  int32_t  ignore_timers;     /* SchedulerConfig.ignoreTimers, read where the reference reads it,
+                                 ExternalEventInjector.handle_timer (ExternalEventInjector.scala:283-285):
+                                 RandomScheduler, STSScheduler, ReplayScheduler and the wildcard replays
+                                 never send a timer when it is set.  DPORwHeuristics sends its timers at once
+                                 (enqueue_timer = enqueue_message, Scheduler.scala:73; DPORwHeuristics.scala
+                                 :946-955) without reading it, so demi_dpor_batch(_ex), demi_incremental_ddmin
+                                 and demi_dpor_frontier(_multi) deliver timers whatever it says. */
   int32_t  strategy;          /* RandomizationStrategy of RandomScheduler: DEMI_RS_FULLY_RANDOM / DEMI_RS_SRC_DST_FIFO */
   int32_t  reserved[2];
 } demi_config;

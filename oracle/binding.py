@@ -192,9 +192,10 @@ def set_conjoined(pairs, n_ext):
 _conj_keep = None
 
 
-def ddmin_sts(model, events, ext, looking_for, flags=0, model_flags=0, check_unmodified=True, cap_iter=65536):
+def ddmin_sts(model, events, ext, looking_for, flags=0, model_flags=0, check_unmodified=True, cap_iter=65536, blocked_mask=0,
+              ignore_timers=0):
     ri = make_replay_input(model, events, ext)
-    cfg = Config(0, model, model_flags, 0, 0)
+    cfg = Config(0, model, model_flags, blocked_mask, ignore_timers)
     mw = mask_words(len(ext))
     mcs = np.zeros(mw, dtype=np.uint64)
     iters = np.zeros(cap_iter, dtype=np.uint32)
@@ -241,9 +242,10 @@ DPOR_VIOL_DTYPE = np.dtype([("schedule_hash", "<u8"), ("interleaving", "<u4"), (
 
 
 def dpor_search(model, ext, max_messages, max_interleavings, looking_for=0, stop_if_found=0, depth_bound=-1,
-                model_flags=0, node_cap=1 << 16, explored_slots=1 << 20, heap_cap=1 << 18, cap_viol=4096):
+                model_flags=0, node_cap=1 << 16, explored_slots=1 << 20, heap_cap=1 << 18, cap_viol=4096, blocked_mask=0,
+                ignore_timers=0):
     ext = np.ascontiguousarray(ext, dtype=EXT_DTYPE)
-    cfg = Config(0, model, model_flags, 0, 0)
+    cfg = Config(0, model, model_flags, blocked_mask, ignore_timers)
     P = DporParams(max_messages, depth_bound, max_interleavings, looking_for, stop_if_found, node_cap,
                    explored_slots, heap_cap)
     res = np.zeros(1, dtype=DPOR_RESULT_DTYPE)
@@ -257,9 +259,10 @@ def dpor_search(model, ext, max_messages, max_interleavings, looking_for=0, stop
 
 
 # ------------------------------------------------ recorded STS replay / internal minimization
-def replay_trace(model, events, ext, mask, looking_for=0, flags=0, model_flags=0, skip_event=0xFFFFFFFF, cap=65536):
+def replay_trace(model, events, ext, mask, looking_for=0, flags=0, model_flags=0, skip_event=0xFFFFFFFF, cap=65536,
+                 blocked_mask=0, ignore_timers=0):
     ri = make_replay_input(model, events, ext)
-    cfg = Config(0, model, model_flags, 0, 0, 0)
+    cfg = Config(0, model, model_flags, blocked_mask, ignore_timers, 0)
     mask = np.ascontiguousarray(mask, dtype=np.uint64)
     out = np.zeros(1, dtype=REPLAY_DTYPE)
     rec = np.zeros(cap, dtype=EVENT_DTYPE)
@@ -270,10 +273,11 @@ def replay_trace(model, events, ext, mask, looking_for=0, flags=0, model_flags=0
     return out[0], rec[:n.value].copy()
 
 
-def internal_minimize(model, verified, mcs_ext, looking_for, flags=0, model_flags=0, cap=65536):
+def internal_minimize(model, verified, mcs_ext, looking_for, flags=0, model_flags=0, cap=65536, blocked_mask=0,
+                      ignore_timers=0):
     verified = np.ascontiguousarray(verified, dtype=EVENT_DTYPE)
     mcs_ext = np.ascontiguousarray(mcs_ext, dtype=EXT_DTYPE)
-    cfg = Config(0, model, model_flags, 0, 0, 0)
+    cfg = Config(0, model, model_flags, blocked_mask, ignore_timers, 0)
     out = np.zeros(cap, dtype=EVENT_DTYPE)
     sizes = np.zeros(cap, dtype=np.uint32)
     n_out, total, n_sizes, unig = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32()
@@ -301,9 +305,10 @@ def provenance(events, dep_parent, affected_mask, mask_words):
     return keep, out[0]
 
 
-def fuzz_provenance(model, ext, seed, max_messages, interval, mask_words, model_flags=0, looking_for=0, strategy=0):
+def fuzz_provenance(model, ext, seed, max_messages, interval, mask_words, model_flags=0, looking_for=0, strategy=0,
+                    blocked_mask=0, ignore_timers=0):
     ext = np.ascontiguousarray(ext, dtype=EXT_DTYPE)
-    cfg = Config(0, model, model_flags, 0, 0, strategy)
+    cfg = Config(0, model, model_flags, blocked_mask, ignore_timers, strategy)
     p = FuzzParams(seed, 1, max_messages, interval, looking_for, 0)
     keep = np.zeros(mask_words, dtype=np.uint64)
     out = np.zeros(1, dtype=PROVENANCE_DTYPE)
@@ -337,9 +342,9 @@ class DporInstance:
 
     def __init__(self, model, ext, max_messages, max_interleavings, seed=None, arvind=0, prioritize_pending=0,
                  looking_for=0, stop_if_found=1, model_flags=0, node_cap=1 << 12, explored_slots=1 << 16,
-                 heap_cap=1 << 17):
+                 heap_cap=1 << 17, blocked_mask=0, ignore_timers=0):
         ext = np.ascontiguousarray(ext, dtype=EXT_DTYPE)
-        cfg = Config(0, model, model_flags, 0, 0)
+        cfg = Config(0, model, model_flags, blocked_mask, ignore_timers)
         self.P = DporParams(max_messages, -1, max_interleavings, looking_for, stop_if_found, node_cap, explored_slots,
                             heap_cap)
         self.max_interleavings = max_interleavings
@@ -370,10 +375,10 @@ class DporInstance:
 
 def incremental_ddmin(model, ext, max_messages, max_interleavings, seed, max_max_distance=8, stop_at_size=6,
                       looking_for=0, model_flags=0, node_cap=1 << 12, explored_slots=1 << 16, heap_cap=1 << 17,
-                      cap_instances=4096):
+                      cap_instances=4096, blocked_mask=0, ignore_timers=0):
     """RunnerUtils.editDistanceDporDDMin's minimisation (RunnerUtils.scala:822-842)."""
     ext = np.ascontiguousarray(ext, dtype=EXT_DTYPE)
-    cfg = Config(0, model, model_flags, 0, 0)
+    cfg = Config(0, model, model_flags, blocked_mask, ignore_timers)
     P = DporParams(max_messages, -1, max_interleavings, looking_for, 1, node_cap, explored_slots, heap_cap)
     nodes = np.ascontiguousarray(seed[0], dtype=np.uint32)
     trace = np.ascontiguousarray(seed[1], dtype=np.uint32)

@@ -128,9 +128,10 @@ void dpor_om_send(om_machine* m, int src, int dst, uint8_t type, uint32_t p0, ui
 }
 void dpor_queue_overflow(void) { if (!g_dpor->status) g_dpor->status = DEMI_DS_QUEUE_OVF; }
 /* Scheduler.enqueue_timer default = enqueue_message: the timer message is sent at
- * once (Scheduler.scala:73; DPORwHeuristics.scala:946-955) */
+ * once (Scheduler.scala:73; DPORwHeuristics.scala:946-955).  SchedulerConfig.ignoreTimers
+ * is not read here: the reference reads it only in ExternalEventInjector.handle_timer
+ * (ExternalEventInjector.scala:283-285), which DPORwHeuristics never calls. */
 static void dpor_timer_send(dpor_t* d, int rcv, uint8_t type, uint32_t p0, uint32_t p1) {
-  if (d->m.ignore_timers) return;
   demi_msg t; t.src = DEMI_DEADLETTERS; t.dst = (uint8_t)rcv; t.type = type; t.flags = 0; t.p0 = p0; t.p1 = p1;
   dpor_event_produced(d, &t);
 }
@@ -410,7 +411,7 @@ void* oracle_dpor_open(const demi_config* cfg, const demi_ext_event* ext, uint32
   d->params = *P; d->P = &d->params;
   d->ext = (demi_ext_event*)malloc(sizeof(demi_ext_event) * (n_ext + 1)); memcpy(d->ext, ext, sizeof(demi_ext_event) * n_ext); d->n_ext = n_ext;
   if (opts) d->opts = *opts;
-  d->m.model = model; d->m.model_flags = cfg->model_flags; d->m.blocked_mask = cfg->blocked_mask; d->m.ignore_timers = cfg->ignore_timers;
+  d->m.model = model; d->m.model_flags = cfg->model_flags; d->m.blocked_mask = cfg->blocked_mask;
   d->cap_nodes = P->node_cap; d->nodes = (dnode*)calloc(d->cap_nodes, sizeof(dnode)); d->n_nodes = 1;
   d->explored_slots = P->explored_slots; d->explored = (uint64_t*)malloc(8ull * d->explored_slots);
   memset(d->explored, 0xFF, 8ull * d->explored_slots);

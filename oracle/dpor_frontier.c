@@ -100,8 +100,8 @@ void front_om_send(om_machine* m, int src, int dst, uint8_t type, uint32_t p0, u
   f_event_produced(g_fx, &msg);
 }
 void front_queue_overflow(void) { if (!g_fx->status) g_fx->status = DEMI_DS_QUEUE_OVF; }
-static void f_timer_send(fexec* x, int rcv, uint8_t type, uint32_t p0, uint32_t p1) {   /* enqueue_timer = enqueue_message */
-  if (x->m.ignore_timers) return;
+/* enqueue_timer = enqueue_message, whatever ignoreTimers says (see dpor.c's dpor_timer_send) */
+static void f_timer_send(fexec* x, int rcv, uint8_t type, uint32_t p0, uint32_t p1) {
   demi_msg t; t.src = DEMI_DEADLETTERS; t.dst = (uint8_t)rcv; t.type = type; t.flags = 0; t.p0 = p0; t.p1 = p1;
   f_event_produced(x, &t);
 }
@@ -326,7 +326,7 @@ int oracle_dpor_frontier(const demi_config* cfg, const demi_ext_event* ext, uint
   const uint32_t S = F->rounds_per_exchange ? F->rounds_per_exchange : 1;
   frank* R = (frank*)calloc(n_ranks, sizeof(frank));
   fexec* x = (fexec*)calloc(1, sizeof(fexec));
-  x->m.model = model; x->m.model_flags = cfg->model_flags; x->m.blocked_mask = cfg->blocked_mask; x->m.ignore_timers = cfg->ignore_timers;
+  x->m.model = model; x->m.model_flags = cfg->model_flags; x->m.blocked_mask = cfg->blocked_mask;
   x->F = F; x->ext = ext; x->n_ext = n_ext;
   x->cap_pend = demi_fr_pool_entries(oracle_model_key(cfg->model), F->max_messages, n_sends);
   x->pend = (fpend*)malloc(sizeof(fpend) * x->cap_pend);

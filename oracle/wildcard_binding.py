@@ -51,13 +51,13 @@ def _type_set(types):
 
 
 def wildcard_replay(model, events, ext, include, increment_types, looking_for=0, flags=0, model_flags=0, blocked_mask=0,
-                    cap=65536):
+                    cap=65536, ignore_timers=0):
     """One STSScheduler.test of ClockClusterizer's trace: (result, recorded EventTrace, ignored trace positions)."""
     ev = np.ascontiguousarray(events, dtype=EVENT_DTYPE)
     ext = np.ascontiguousarray(ext, dtype=EXT_DTYPE)
     inc = np.ascontiguousarray(include, dtype=np.uint64)
     incr = _type_set(increment_types)
-    cfg = Config(0, model, model_flags, blocked_mask, 0, 0)
+    cfg = Config(0, model, model_flags, blocked_mask, ignore_timers, 0)
     out = np.zeros(1, dtype=REPLAY_DTYPE)
     rec = np.zeros(cap, dtype=EVENT_DTYPE)
     ign = np.zeros(len(ev) + 1, dtype=np.uint32)
@@ -90,12 +90,13 @@ def wildcard_cluster_sequence(events, rules, increment_types, outcomes=(), ignor
     return masks[:n].copy()
 
 
-def wildcard_minimize(model, verified, mcs_ext, rules, increment_types, looking_for, flags=0, model_flags=0, cap=65536):
+def wildcard_minimize(model, verified, mcs_ext, rules, increment_types, looking_for, flags=0, model_flags=0, cap=65536,
+                      blocked_mask=0, ignore_timers=0):
     """WildcardMinimizer (STSSched, ClockClusterizer), sequential: (rc, minTrace, total_replays, internal sizes)."""
     verified = np.ascontiguousarray(verified, dtype=EVENT_DTYPE)
     mcs_ext = np.ascontiguousarray(mcs_ext, dtype=EXT_DTYPE)
     rt, incr = _rule_table(rules), _type_set(increment_types)
-    cfg = Config(0, model, model_flags, 0, 0, 0)
+    cfg = Config(0, model, model_flags, blocked_mask, ignore_timers, 0)
     out = np.zeros(cap, dtype=EVENT_DTYPE)
     sizes = np.zeros(cap, dtype=np.uint32)
     n_out, total, n_sizes = C.c_uint32(), C.c_uint32(), C.c_uint32()

@@ -114,7 +114,7 @@ class Execution(object):
     """One RandomScheduler.explore(trace) with max_executions = 1, FullyRandom(seed), checkpointing off."""
 
     def __init__(self, actors, externals, seed, max_messages, invariant_check_interval, invariant, external_filter,
-                 blocked=(), looking_for=None, user_filter=None, fresh_actor=None):
+                 blocked=(), looking_for=None, user_filter=None, fresh_actor=None, ignore_timers=False):
         self.userDefinedFilter = user_filter or (lambda snd, rcv, msg: True)      # FullyRandom ctor arg (:636)
         self.fresh_actor = fresh_actor                                             # name -> new instance (HardKill + Start)
         self.dead = set()
@@ -126,6 +126,7 @@ class Execution(object):
         self.invariant = invariant
         self.is_external = external_filter
         self.blockedActors = set(blocked)
+        self.ignoreTimers = ignore_timers        # SchedulerConfig.ignoreTimers
         self.lookingFor = looking_for
         self.depTracker = DepTracker()
         # ExternalEventInjector
@@ -233,6 +234,8 @@ class Execution(object):
         self.events.append(("MsgSend", "Timer" if is_timer else snd, rcv, msg, uniq, unique.id))
 
     def handle_timer(self, rcv, msg):            # ExternalEventInjector :282-297
+        if self.ignoreTimers:                    # the one place the reference reads ignoreTimers (:283-285)
+            return
         self.messagesToSend.append((None, rcv, msg))
 
     def enqueue_timer(self, rcv, msg):           # :549-559
@@ -843,8 +846,9 @@ class STSReplay(Execution):
     notify_timer_cancel (:846-868).  The Instrumenter side (`!`, timers, dispatch) is Execution's."""
 
     def __init__(self, actors, original_events, original_externals, invariant, is_external, filter_known_absents=False,
-                 looking_for=None):
-        Execution.__init__(self, actors, [], 0, -1, 0, invariant, is_external, looking_for=looking_for)
+                 looking_for=None, blocked=(), ignore_timers=False):
+        Execution.__init__(self, actors, [], 0, -1, 0, invariant, is_external, blocked=blocked, looking_for=looking_for,
+                           ignore_timers=ignore_timers)
         self.original_events, self.original_externals = original_events, original_externals
         self.filterKnownAbsents = filter_known_absents
         self.pending = {}                        # (snd, rcv) -> {fingerprint -> [(uniq, msg)]}   (:112-114)
@@ -1133,10 +1137,14 @@ class DPORSearch(object):
     checkpointing off (invariant at the end of every interleaving), prioritizePendingUponDivergence off, no depth
     bound.  Two choices the Scala leaves to scala-library internals are fixed as DESIGN.md §6 fixes them: the divergent
     choice (`pendingEvents.find` over a HashMap, :454-456) takes the first non-empty queue in (sender, receiver) order
-    with deadLetters last, and backtrack points of equal branch depth leave the PriorityQueue oldest first."""
+    with deadLetters last, and backtrack points of equal branch depth leave the PriorityQueue oldest first.
+    `blocked` is the blockedActors set schedule_new_message is called with (:421); nothing here reads ignoreTimers,
+    because DPORwHeuristics sends a timer at once (enqueue_timer = enqueue_message, Scheduler.scala:73) and never
+    reaches ExternalEventInjector.handle_timer."""
 
-    def __init__(self, make_actors, externals, invariant, max_messages, stop_if_found=True, looking_for=None):
+    def __init__(self, make_actors, externals, invariant, max_messages, stop_if_found=True, looking_for=None, blocked=()):
         self.make_actors, self.externals, self.invariant = make_actors, externals, invariant
+        self.blockedActors = set(blocked)
         self.max_messages, self.stopIfViolationFound, self.lookingFor = max_messages, stop_if_found, looking_for
         # the dependency graph (child -> parent edges), ids from one counter, root = Unique(MsgEvent("null","null",null), 0)
         self.event = {0: ("null", "null", None)}
@@ -1220,6 +1228,8 @@ class DPORSearch(object):
             if u == 0:
                 continue                                             # "All system messages need to ignored" (the root)
             snd, rcv, _ = self.event[u]
+            if rcv in self.blockedActors:
+                return None                                          # :478, :518: the entry is consumed all the same
             q = self.pending.get((snd, rcv))
             if q is not None:
                 for i, (v, m) in enumerate(q):
@@ -1235,7 +1245,7 @@ class DPORSearch(object):
             return (10 ** 6 if snd == DEADLETTERS else int(snd), int(rcv))
         for key in sorted(self.pending, key=order):
             q = self.pending[key]
-            if q:
+            if q and key[1] not in self.blockedActors:             # :455
                 u, m = q.pop(0)
                 return (u, key[0], key[1], m)
         return None
@@ -1349,8 +1359,8 @@ class ResumableDPORInstance(DPORSearch):
     called repeatedly (:1193-1242)."""
 
     def __init__(self, make_actors, externals, invariant, max_messages, init_nodes=None, init_trace=None, arvind=False,
-                 prioritize_pending=False, stop_if_found=True, looking_for=None):
-        DPORSearch.__init__(self, make_actors, externals, invariant, max_messages, stop_if_found, looking_for)
+                 prioritize_pending=False, stop_if_found=True, looking_for=None, blocked=()):
+        DPORSearch.__init__(self, make_actors, externals, invariant, max_messages, stop_if_found, looking_for, blocked)
         self.arvind, self.prioritize = arvind, prioritize_pending
         self.init_trace = list(init_trace) if init_trace is not None else None
         self.originalIndices = {}
