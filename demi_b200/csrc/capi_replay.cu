@@ -16,20 +16,37 @@
 
 using namespace demi;
 
-typedef void (*replay_fn)(const ReplayArgs);
-struct ReplayVariant { int model; int bd; replay_fn fn; replay_fn fn_rec; size_t smem; int n_actors; };
 template <class MODEL, int BD>
 static ReplayVariant make_rv() {
-  using M = ReplayMachine<MODEL, BD>;
-  return ReplayVariant{MODEL::ID, BD, replay_lane_kernel<MODEL, BD, false>, replay_lane_kernel<MODEL, BD, true>,
+  using M = ReplayMachine<MODEL, BD>;     // WORDS does not depend on REC or WILD
+  return ReplayVariant{MODEL::ID, BD,
+                       {{replay_lane_kernel<MODEL, BD, false, false>, replay_lane_kernel<MODEL, BD, true, false>},
+                        {replay_lane_kernel<MODEL, BD, false, true>, replay_lane_kernel<MODEL, BD, true, true>}},
                        (size_t)M::WORDS * BD * sizeof(uint32_t), MODEL::N_ACTORS};
 }
-static const ReplayVariant* pick_rv(int model) {
+const ReplayVariant* pick_rv(int model) {
   static const std::vector<ReplayVariant> v = {
     make_rv<PingPong3, 256>(), make_rv<Raft5, 256>(), make_rv<Bcast32, 128>(), make_rv<IrModel, 128>(),
   };
   for (const ReplayVariant& r : v) if (r.model == model) return &r;
   return nullptr;
+}
+
+ReplayArgs replay_args(const demi_handle* h, uint32_t looking_for, uint32_t flags) {
+  ReplayArgs a{};
+  a.model_flags = h->cfg.model_flags; a.blocked_mask = h->cfg.blocked_mask; a.ignore_timers = h->cfg.ignore_timers;
+  a.looking_for = looking_for; a.flags = flags;
+  a.events = (const uint4*)h->trace_dev; a.n_events = (uint32_t)h->trace_host.size();
+  a.ev_ordinal = h->ev_ordinal_dev;
+  a.ext = (const uint4*)h->trace_ext_dev; a.n_ext = (uint32_t)h->trace_ext_host.size();
+  a.send_ext_index = h->send_ext_index_dev; a.n_sends = h->trace_n_ext_sends;
+  a.external_type_mask = demi_ext_type_mask(h);
+  a.n_uniq_words = (h->trace_n_uniq + 31) / 32;
+  return a;
+}
+
+cudaError_t replay_ir_bind(const demi_handle* h, cudaStream_t s) {
+  return h->cfg.model == DEMI_MODEL_IR ? ir_bind(h->ir_dev, s) : cudaSuccess;
 }
 
 void demi_replay_free(demi_handle* h) {
@@ -137,22 +154,14 @@ static int32_t launch_replay(demi_handle* h, const void* masks_dev, const void* 
   // the grid (and the table's size) is the batch kernel's; the recording kernel runs one block of it
   int32_t rc;
   int bps = 0, rec_bps = 0;
-  if ((rc = demi_occupancy(h, (const void*)rv->fn, rv->bd, rv->smem, &bps)) != DEMI_OK) return rc;
-  if (record && (rc = demi_occupancy(h, (const void*)rv->fn_rec, rv->bd, rv->smem, &rec_bps)) != DEMI_OK) return rc;
+  if ((rc = demi_occupancy(h, (const void*)rv->fn[0][0], rv->bd, rv->smem, &bps)) != DEMI_OK) return rc;
+  if (record && (rc = demi_occupancy(h, (const void*)rv->fn[0][1], rv->bd, rv->smem, &rec_bps)) != DEMI_OK) return rc;
   if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
   uint64_t want = ((uint64_t)n_masks + rv->bd - 1) / rv->bd;
   int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * bps));
   const uint64_t warps = (uint64_t)grid * (rv->bd / 32);
 
-  ReplayArgs a{};
-  a.model_flags = h->cfg.model_flags; a.blocked_mask = h->cfg.blocked_mask; a.ignore_timers = h->cfg.ignore_timers;
-  a.looking_for = looking_for; a.flags = flags;
-  a.events = (const uint4*)h->trace_dev; a.n_events = (uint32_t)h->trace_host.size();
-  a.ev_ordinal = h->ev_ordinal_dev;
-  a.ext = (const uint4*)h->trace_ext_dev; a.n_ext = n_ext;
-  a.send_ext_index = h->send_ext_index_dev; a.n_sends = h->trace_n_ext_sends;
-  a.external_type_mask = demi_ext_type_mask(h);
-  a.n_uniq_words = (h->trace_n_uniq + 31) / 32;
+  ReplayArgs a = replay_args(h, looking_for, flags);
   a.masks = (const uint64_t*)masks_dev; a.n_masks = n_masks; a.mask_words = mask_words;
   a.skips = (const uint32_t*)skips_dev;
   a.rec_events = rec_dev; a.rec_cap = rec_cap; a.rec_count = rec_count_dev;
@@ -182,8 +191,8 @@ static int32_t launch_replay(demi_handle* h, const void* masks_dev, const void* 
   a.table = (uint4*)h->rp_table; a.tosend = (uint32_t*)h->rp_tosend;
   a.pruned = (flags & DEMI_RF_FILTER_KNOWN_ABSENTS) ? (uint32_t*)h->rp_pruned : nullptr;
   a.counters = h->rp_counters;
-  if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
-  (record ? rv->fn_rec : rv->fn)<<<record ? 1 : grid, rv->bd, rv->smem, s>>>(a);
+  CUDA_TRY(h, replay_ir_bind(h, s));
+  rv->fn[0][record]<<<record ? 1 : grid, rv->bd, rv->smem, s>>>(a);
   CUDA_TRY(h, cudaGetLastError());
   h->perf.kernel_launches = 1;
   h->perf.prefixes = n_masks;

@@ -11,27 +11,10 @@
 #include <set>
 #include "replay_kernel.cuh"
 #include "engine.hpp"
-#include "models/model_ir.cuh"
 
 using namespace demi;
 
 namespace {
-typedef void (*wild_fn)(const ReplayArgs);
-struct WildVariant { int model; int bd; wild_fn fn; wild_fn fn_rec; size_t smem; int n_actors; };
-template <class MODEL, int BD>
-WildVariant make_wv() {
-  using M = ReplayMachine<MODEL, BD, false, true>;
-  return WildVariant{MODEL::ID, BD, replay_lane_kernel<MODEL, BD, false, true>, replay_lane_kernel<MODEL, BD, true, true>,
-                     (size_t)M::WORDS * BD * sizeof(uint32_t), MODEL::N_ACTORS};
-}
-const WildVariant* pick_wv(int model) {
-  static const std::vector<WildVariant> v = {
-    make_wv<PingPong3, 256>(), make_wv<Raft5, 256>(), make_wv<Bcast32, 128>(), make_wv<IrModel, 128>(),
-  };
-  for (const WildVariant& r : v) if (r.model == model) return &r;
-  return nullptr;
-}
-
 inline bool incr_of(const demi_handle* h, uint32_t type) { return (h->clock_incr[type >> 5] >> (type & 31)) & 1u; }
 // FingerprintFactory.getLogicalClock as data: false = None
 inline bool clock_of(const demi_handle* h, const demi_event& e, uint32_t& clock) {
@@ -80,17 +63,17 @@ int32_t wc_launch(demi_handle* h, const WcTrace& t, const uint64_t* include_host
                   demi_event* rec_host, uint32_t rec_cap, uint32_t* n_rec,
                   uint32_t* ign_host, uint32_t ign_cap, uint32_t* n_ign) {
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  const WildVariant* wv = pick_wv(h->cfg.model);
+  const ReplayVariant* wv = pick_rv(h->cfg.model);
   if (!wv) return fail(h, DEMI_ERR_INVALID, "no replay kernel for model %d", h->cfg.model);
   const bool record = rec_host != nullptr;
   cudaStream_t s = h->stream;
-  wild_fn fn = record ? wv->fn_rec : wv->fn;
+  replay_fn fn = wv->fn[1][record];
   int32_t rc;
   int bps = 0;
   if ((rc = demi_occupancy(h, (const void*)fn, wv->bd, wv->smem, &bps)) != DEMI_OK) return rc;
   if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
   const uint32_t n_ext = (uint32_t)h->trace_ext_host.size();
-  ReplayArgs a{};
+  ReplayArgs a = replay_args(h, looking_for, flags);
   a.pending_cap = demi_wildcard_pending_cap(demi_model_key(h), (uint32_t)t.pos.size(), h->trace_n_ext_sends);
   a.table_slots = a.pending_cap;                        // list storage (the kernel compacts it in place)
   a.tosend_cap = demi_tosend_cap(h->trace_n_ext_sends);
@@ -100,14 +83,6 @@ int32_t wc_launch(demi_handle* h, const WcTrace& t, const uint64_t* include_host
   const uint64_t want = ((uint64_t)n_tests + wv->bd - 1) / wv->bd;
   const int grid = record ? 1 : (int)std::max<uint64_t>(1, std::min<uint64_t>({want, (uint64_t)h->sm_count * bps, max_blocks}));
   const uint64_t warps = (uint64_t)grid * (wv->bd / 32);
-  a.model_flags = h->cfg.model_flags; a.blocked_mask = h->cfg.blocked_mask; a.ignore_timers = h->cfg.ignore_timers;
-  a.looking_for = looking_for; a.flags = flags;
-  a.events = (const uint4*)h->trace_dev; a.n_events = (uint32_t)h->trace_host.size();
-  a.ev_ordinal = h->ev_ordinal_dev;
-  a.ext = (const uint4*)h->trace_ext_dev; a.n_ext = n_ext;
-  a.send_ext_index = h->send_ext_index_dev; a.n_sends = h->trace_n_ext_sends;
-  a.external_type_mask = demi_ext_type_mask(h);
-  a.n_uniq_words = (h->trace_n_uniq + 31) / 32;
   a.masks = nullptr; a.n_masks = n_tests; a.mask_words = std::max<uint32_t>(1, (n_ext + 63) / 64);   // the full MCS
   a.gen_base = 1;
   a.wc_words = t.words;
@@ -142,7 +117,7 @@ int32_t wc_launch(demi_handle* h, const WcTrace& t, const uint64_t* include_host
     a.rec_events = (demi_event*)d_rec; a.rec_cap = rec_cap; a.rec_count = counts;
     a.wc_ignored = (uint32_t*)d_ign; a.wc_ignored_cap = ign_cap; a.wc_ignored_count = counts + 1;
   }
-  if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
+  CUDA_TRY(h, replay_ir_bind(h, s));
   CUDA_TRY(h, cudaEventRecord(h->ev0, s));
   fn<<<grid, wv->bd, wv->smem, s>>>(a);
   cudaError_t e = cudaGetLastError();

@@ -16,7 +16,7 @@
 // finished interleavings (backtrack keys reference them instead of copying
 // `needToReplay`).  Actor states / outbox: thread-interleaved shared memory.
 #pragma once
-#include "lane_kernel.cuh"
+#include "actor_step.cuh"
 
 namespace demi {
 
@@ -68,11 +68,14 @@ struct DporArgs {
 
 template <class MODEL, int BD>
 struct DporMachine {
+  using Model = MODEL;
+  static constexpr int BLOCK = BD;
   static constexpr int N = MODEL::N_ACTORS;
   static constexpr int SW = MODEL::STATE_WORDS;
   static constexpr int OB = MODEL::REPLAY_OUTBOX;
   static constexpr int WORDS = N * SW + OB * 3;
   static constexpr int NQ = (N + 1) * N;
+  static constexpr uint32_t UNSUPPORTED = DEMI_DS_UNSUPPORTED, QUEUE_OVF = DEMI_DS_QUEUE_OVF;
 
   uint32_t* smw; const DporArgs* A;
   uint4* nodes; uint32_t* child_hash; uint32_t* queues; uint64_t* explored; DporKey* heap;
@@ -113,11 +116,10 @@ struct DporMachine {
     return id;
   }
 
-  // DPORwHeuristics.event_produced (:803-847) after the cancelled-timer drop (Instrumenter.scala:1090-1096)
+  // DPORwHeuristics.event_produced (:803-847) after the cancelled-timer drop
   __device__ __forceinline__ void event_produced(uint32_t src, uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) {
     if (status) return;
-    int slot = MODEL::timer_slot(dst, type, p0, p1);
-    if (cancelled && slot >= 0 && ((cancelled >> slot) & 1u)) { cancelled &= ~(1u << slot); return; }
+    if (timer_dropped(*this, dst, type, p0, p1)) return;
     uint32_t id = get_message(make_hdr(src, dst, type, 0), p0, p1);
     if (status) return;
     if (A->P.depth_bound < 0 || (int32_t)current_depth < A->P.depth_bound) {     // depth-bound gate :832
@@ -129,7 +131,7 @@ struct DporMachine {
   }
   // enqueue_timer = enqueue_message (Scheduler.scala:73): sent at once, whatever ignoreTimers says — the reference reads
   // that flag only in ExternalEventInjector.handle_timer (ExternalEventInjector.scala:283-285), which DPOR never calls
-  __device__ __forceinline__ void timer_send(uint32_t slot) {
+  __device__ __forceinline__ void enqueue_timer(uint32_t slot) {
     uint32_t dst, type, p0, p1;
     MODEL::slot_msg(slot, dst, type, p0, p1);
     event_produced(DEMI_DEADLETTERS, dst, type, p0, p1);
@@ -138,12 +140,8 @@ struct DporMachine {
     for (uint32_t j = i; j + 1 < qlen[q]; j++) queues[q * DPOR_QCAP + j] = queues[q * DPOR_QCAP + j + 1];
     qlen[q]--;
   }
-  // DPORwHeuristics.notify_timer_cancel (:961-985)
-  __device__ __forceinline__ void cancel_timer(uint32_t self, uint32_t type, uint32_t p0, uint32_t p1) {
-    int slot = MODEL::timer_slot(self, type, p0, p1);
-    if (slot < 0) { status = DEMI_DS_UNSUPPORTED; return; }
-    cancelled |= 1u << slot;
-    registry &= ~(1u << slot);
+  // the cancelled timer's pending copy (DPORwHeuristics.notify_timer_cancel :961-985)
+  __device__ __forceinline__ void cancel_pending(uint32_t self, uint32_t, uint32_t type, uint32_t p0, uint32_t p1) {
     uint32_t q = qindex(DEMI_DEADLETTERS, self);
     for (uint32_t i = 0; i < qlen[q]; i++) {
       uint4 c = nodes[queues[q * DPOR_QCAP + i]];
@@ -277,7 +275,7 @@ struct DporMachine {
   }
 
   __device__ __forceinline__ uint32_t run_interleaving(uint32_t ext_lo, uint32_t ext_hi) {
-    for (uint32_t i = 0; i < N * SW; i++) smw[i * BD] = MODEL::init_word(i, A->model_flags);
+    actor_init(*this);
     registry = cancelled = 0;
     for (int q = 0; q < NQ; q++) qlen[q] = 0;
     isolated = (N >= 32) ? 0xFFFFFFFFu : ((1u << N) - 1u);
@@ -294,29 +292,9 @@ struct DporMachine {
     while (!status && (pick = schedule()) != 0) {
       uint4 c = nodes[pick];
       uint32_t src = hdr_src(c.x), dst = hdr_dst(c.x), type = hdr_type(c.x);
-      int slot = MODEL::timer_slot(dst, type, c.y, c.z);
-      if (slot >= 0 && ((registry >> slot) & 1u)) timer_send((uint32_t)slot);    // re-arm (Instrumenter.scala:1008-1016)
+      timer_rearm(*this, dst, type, c.y, c.z);
       if (status) break;
-      LaneOutbox<OB> ob;
-      ob.base = smw + N * SW * BD; ob.bd = BD; ob.n = 0; ob.self = dst; ob.overflow = false;
-      MODEL::receive(ob, dst, actor(dst), src, type, c.y, c.z, A->model_flags);
-      if (ob.overflow) { status = DEMI_DS_QUEUE_OVF; break; }
-      for (uint32_t i = 0; i < ob.n && !status; i++) {
-        uint32_t w0 = ob.base[(i * 3) * BD], q0 = ob.base[(i * 3 + 1) * BD], q1 = ob.base[(i * 3 + 2) * BD];
-        uint32_t kind = w0 & 0xFF, odst = (w0 >> 8) & 0xFF, otype = (w0 >> 16) & 0xFF;
-        if (kind == OP_SEND) event_produced(dst, odst, otype, q0, q1);
-        else if (kind == OP_CANCEL) cancel_timer(odst, otype, q0, q1);
-        else {
-          int s2 = MODEL::timer_slot(odst, otype, q0, q1);
-          if (s2 < 0) { status = DEMI_DS_UNSUPPORTED; break; }
-          if ((registry >> s2) & 1u) continue;
-          if (kind == OP_SCHED_REPEAT) {
-            if (__popc(registry) >= DEMI_TIMERSET_CAP) { status = DEMI_DS_QUEUE_OVF; break; }
-            registry |= 1u << s2;
-          }
-          timer_send((uint32_t)s2);
-        }
-      }
+      actor_receive<false>(*this, src, dst, type, c.y, c.z);
     }
     if (status) return 0;
     uint32_t v = MODEL::invariant(LaneAll<SW>{smw, BD}, A->model_flags);          // checkInvariant :394-418

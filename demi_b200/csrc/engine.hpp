@@ -95,6 +95,16 @@ struct demi_handle {
   void* trace_rec = nullptr; size_t trace_rec_bytes = 0;   // demi_fuzz_trace's recording buffer
 };
 void demi_replay_free(demi_handle* h);
+// K2, STSSched replay (capi_replay.cu), for both the exact replays and the wildcard replays (capi_wildcard.cu): per
+// model the block size, the shared memory and the four instantiations of replay_lane_kernel, fn[WILD][REC]
+namespace demi { struct ReplayArgs; }
+typedef void (*replay_fn)(const demi::ReplayArgs);
+struct ReplayVariant { int model; int bd; replay_fn fn[2][2]; size_t smem; int n_actors; };
+const ReplayVariant* pick_rv(int model);
+// the ReplayArgs fields that follow from the handle's configuration and its trace (demi_set_trace); the rest are zero
+demi::ReplayArgs replay_args(const demi_handle* h, uint32_t looking_for, uint32_t flags);
+// binds the handle's loaded model to the replay kernels: model_ir.cuh keeps one copy of it per translation unit
+cudaError_t replay_ir_bind(const demi_handle* h, cudaStream_t s);
 void demi_comm_free(demi_handle* h);
 void demi_frontier_free(demi_handle* h);
 

@@ -25,9 +25,7 @@
 //                      pair (hash table of minimum window index), prefix-sum, cut at the round's quota, mark (:1169-1171).
 //   fr_pack / fr_unpack     a stolen record = point + trace prefix; what moves over NVLink in the steal round.
 #pragma once
-#include "lane_kernel.cuh"
-#include "models/model_traits.cuh"
-#include "models/models.cuh"
+#include "actor_step.cuh"
 
 namespace demi {
 
@@ -98,26 +96,17 @@ __device__ __forceinline__ void fr_log_key(const FrLog& log, unsigned long long 
 }
 
 // ------------------------------------------------------------------ executor
-// receive()'s view when its operations are applied as they are issued (built-in models: a receive() never exceeds the
-// outbox, so nothing observable depends on staging it)
-template <class M>
-struct FrDirectOutbox {
-  M* m; uint32_t self;
-  __device__ __forceinline__ bool reserve(uint32_t) { return true; }     // each send checks its own capacities
-  __device__ __forceinline__ void send(uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) { m->event_produced(self, dst, type, p0, p1); }
-  __device__ __forceinline__ void schedule_once(uint32_t type, uint32_t p0, uint32_t p1) { m->schedule_timer(OP_SCHED_ONCE, self, type, p0, p1); }
-  __device__ __forceinline__ void schedule_repeating(uint32_t type, uint32_t p0, uint32_t p1) { m->schedule_timer(OP_SCHED_REPEAT, self, type, p0, p1); }
-  __device__ __forceinline__ void cancel_timer(uint32_t type, uint32_t p0, uint32_t p1) { m->cancel_timer(self, type, p0, p1); }
-};
-
 template <class MODEL, int BD>
 struct FrExec {
+  using Model = MODEL;
+  static constexpr int BLOCK = BD;
   static constexpr int N = MODEL::N_ACTORS;
   static constexpr int SW = MODEL::STATE_WORDS;
   static constexpr int OB = MODEL::REPLAY_OUTBOX;
   static constexpr bool DIRECT = model_replay_direct<MODEL>::value;
   static constexpr int WORDS = N * SW + (DIRECT ? 0 : OB * 3);
   static constexpr int NQ = (N + 1) * N;
+  static constexpr uint32_t UNSUPPORTED = DEMI_DS_UNSUPPORTED, QUEUE_OVF = DEMI_DS_QUEUE_OVF;
   static constexpr int QW = (NQ + 31) / 32;
   static constexpr uint32_t NIL = 0xFFFFu;
 
@@ -133,12 +122,11 @@ struct FrExec {
     return (src == DEMI_DEADLETTERS ? (uint32_t)N : src) * N + dst;
   }
 
-  // DPORwHeuristics.event_produced (:803-847) after the cancelled-timer drop (Instrumenter.scala:1090-1096);
+  // DPORwHeuristics.event_produced (:803-847) after the cancelled-timer drop;
   // getMessage (:773-801): same parent + same (snd, rcv, fingerprint) = same Unique, here the same hash
   __device__ __forceinline__ void event_produced(uint32_t src, uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) {
     if (status) return;
-    const int slot = MODEL::timer_slot(dst, type, p0, p1);
-    if (cancelled && slot >= 0 && ((cancelled >> slot) & 1u)) { cancelled &= ~(1u << slot); return; }
+    if (timer_dropped(*this, dst, type, p0, p1)) return;
     if (n_ent >= A->cap_pend) { status = DEMI_DS_QUEUE_OVF; return; }
     const uint32_t e = n_ent++;
     const uint32_t hdr = make_hdr(src, dst, type, 0);
@@ -161,31 +149,14 @@ struct FrExec {
       if (prev == NIL) qmask[q >> 5] &= ~(1u << (q & 31));
     }
   }
-  // enqueue_timer = enqueue_message (Scheduler.scala:73), whatever ignoreTimers says (see DporMachine::timer_send)
-  __device__ __forceinline__ void timer_send(uint32_t slot) {
+  // enqueue_timer = enqueue_message (Scheduler.scala:73), whatever ignoreTimers says (see DporMachine::enqueue_timer)
+  __device__ __forceinline__ void enqueue_timer(uint32_t slot) {
     uint32_t dst, type, p0, p1;
     MODEL::slot_msg(slot, dst, type, p0, p1);
     event_produced(DEMI_DEADLETTERS, dst, type, p0, p1);
   }
-  // DPORwHeuristics.notify_timer_cancel (:961-985)
-  // scheduler.scheduleOnce / schedule (Instrumenter.scala:1126-1190)
-  __device__ __forceinline__ void schedule_timer(uint32_t kind, uint32_t self, uint32_t type, uint32_t p0, uint32_t p1) {
-    if (status) return;
-    const int s2 = MODEL::timer_slot(self, type, p0, p1);
-    if (s2 < 0) { status = DEMI_DS_UNSUPPORTED; return; }
-    if ((registry >> s2) & 1u) return;                                  // "Non-unique timer"
-    if (kind == OP_SCHED_REPEAT) {
-      if (__popc(registry) >= DEMI_TIMERSET_CAP) { status = DEMI_DS_QUEUE_OVF; return; }
-      registry |= 1u << s2;
-    }
-    timer_send((uint32_t)s2);
-  }
-  __device__ __forceinline__ void cancel_timer(uint32_t self, uint32_t type, uint32_t p0, uint32_t p1) {
-    if (status) return;
-    const int slot = MODEL::timer_slot(self, type, p0, p1);
-    if (slot < 0) { status = DEMI_DS_UNSUPPORTED; return; }
-    cancelled |= 1u << slot;
-    registry &= ~(1u << slot);
+  // the cancelled timer's pending copy (DPORwHeuristics.notify_timer_cancel :961-985)
+  __device__ __forceinline__ void cancel_pending(uint32_t self, uint32_t, uint32_t type, uint32_t p0, uint32_t p1) {
     const uint32_t q = qindex(DEMI_DEADLETTERS, self);
     uint32_t prev = NIL;
     for (uint32_t e = qhead[q]; e != NIL; prev = e, e = nxa[(size_t)e * 32] & 0xFFFFu) {
@@ -198,8 +169,7 @@ struct FrExec {
   // kt == nullptr: no nextTrace.  Else nextTrace = kt[1..branch] ++ (kt[branch+1..li] minus the entries whose id is
   // kt[ei]'s) (:1060-1063, :1180).  Returns the violation code.
   __device__ uint32_t run(const uint4* kt, uint32_t branch, uint32_t li, uint32_t ei, uint4* out, unsigned long long& sh) {
-#pragma unroll 1
-    for (uint32_t i = 0; i < N * SW; i++) smw[i * BD] = MODEL::init_word(i, A->model_flags);
+    actor_init(*this);
     registry = cancelled = 0;
 #pragma unroll 1
     for (int q = 0; q < NQ; q++) { qhead[q] = NIL; qtail[q] = NIL; }
@@ -268,26 +238,9 @@ struct FrExec {
       sh += demi_event_term(c.z & 0x00FFFFFFu, c.w, p1, cur_len, 0, 0);
       cur_pos = cur_len++;
       parent_id = (unsigned long long)c.x | ((unsigned long long)c.y << 32);
-      const int slot = MODEL::timer_slot(dst, type, c.w, p1);
-      if (slot >= 0 && ((registry >> slot) & 1u)) timer_send((uint32_t)slot);      // re-arm (Instrumenter.scala:1008-1016)
+      timer_rearm(*this, dst, type, c.w, p1);
       if (status) break;
-      if constexpr (DIRECT) {
-        FrDirectOutbox<FrExec> direct{this, dst};
-        MODEL::receive(direct, dst, actor(dst), src, type, c.w, p1, A->model_flags);
-      } else {
-        LaneOutbox<OB> ob;
-        ob.base = smw + N * SW * BD; ob.bd = BD; ob.n = 0; ob.self = dst; ob.overflow = false;
-        MODEL::receive(ob, dst, actor(dst), src, type, c.w, p1, A->model_flags);
-        if (ob.overflow) { status = DEMI_DS_QUEUE_OVF; break; }
-#pragma unroll 1
-        for (uint32_t i = 0; i < ob.n && !status; i++) {
-          const uint32_t w0 = ob.base[(i * 3) * BD], q0 = ob.base[(i * 3 + 1) * BD], q1 = ob.base[(i * 3 + 2) * BD];
-          const uint32_t kind = w0 & 0xFF, odst = (w0 >> 8) & 0xFF, otype = (w0 >> 16) & 0xFF;
-          if (kind == OP_SEND) event_produced(dst, odst, otype, q0, q1);
-          else if (kind == OP_CANCEL) cancel_timer(odst, otype, q0, q1);
-          else schedule_timer(kind, odst, otype, q0, q1);
-        }
-      }
+      actor_receive<DIRECT>(*this, src, dst, type, c.w, p1);
     }
     if (status) return 0;
     uint32_t v = MODEL::invariant(LaneAll<SW>{smw, BD}, A->model_flags);   // checkInvariant :394-418

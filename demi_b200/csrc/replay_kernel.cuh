@@ -19,8 +19,7 @@
 // STSScheduler.scala:112-114) is an open-addressing hash table of
 // {hdr,p0,p1,generation|count} in HBM, interleaved per warp.
 #pragma once
-#include "lane_kernel.cuh"
-#include "models/model_traits.cuh"
+#include "actor_step.cuh"
 
 namespace demi {
 
@@ -58,28 +57,19 @@ struct ReplayArgs {
 };
 enum : uint32_t { WC_EXACT = 0, WC_CLASS = 1, WC_CLOCK = 2 };   // match mode of one delivery of the base trace
 
-// receive()'s view when its operations are applied as they are issued (program order is the reference's order:
-// `!`, scheduleOnce and cancel() act synchronously inside receive()); no staging in shared memory.
-template <class M>
-struct ReplayDirectOutbox {
-  M* m; uint32_t self;
-  __device__ __forceinline__ bool reserve(uint32_t) { return true; }     // each send checks its own capacities
-  __device__ __forceinline__ void send(uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) { m->event_produced(self, dst, type, p0, p1, false); }
-  __device__ __forceinline__ void schedule_once(uint32_t type, uint32_t p0, uint32_t p1) { m->schedule_timer(OP_SCHED_ONCE, self, type, p0, p1); }
-  __device__ __forceinline__ void schedule_repeating(uint32_t type, uint32_t p0, uint32_t p1) { m->schedule_timer(OP_SCHED_REPEAT, self, type, p0, p1); }
-  __device__ __forceinline__ void cancel_timer(uint32_t type, uint32_t p0, uint32_t p1) { m->cancel_timer(self, type, p0, p1); }
-};
-
 // WILD: ClockClusterizer's wildcarded trace (capi_wildcard.cu).  The pending set is the insertion-ordered list of
 // the REC variant (Uniq order = list order), compacted in place when taken entries dominate it.
 template <class MODEL, int BD, bool REC = false, bool WILD = false>
 struct ReplayMachine {
+  using Model = MODEL;
+  static constexpr int BLOCK = BD;
   static constexpr bool LIST = REC || WILD;
   static constexpr int N = MODEL::N_ACTORS;
   static constexpr int SW = MODEL::STATE_WORDS;
   static constexpr int OB = MODEL::REPLAY_OUTBOX;
   static constexpr bool DIRECT = model_replay_direct<MODEL>::value;
   static constexpr int OBW = DIRECT ? 0 : OB * 3;      // the outbox is staged in shared memory only when it can overflow
+  static constexpr uint32_t UNSUPPORTED = DEMI_RS_UNSUPPORTED, QUEUE_OVF = DEMI_PS_QUEUE_OVF;
   static constexpr int WORDS = N * SW + OBW + N;
 
   uint32_t* smw;
@@ -237,13 +227,11 @@ struct ReplayMachine {
     return false;
   }
 
-  // STSScheduler.event_produced (STSScheduler.scala:561-623) after the
-  // cancelled-timer drop of Instrumenter.aroundDispatch (Instrumenter.scala:1090-1096)
+  // STSScheduler.event_produced (STSScheduler.scala:561-623) after the cancelled-timer drop
   __device__ __forceinline__ void event_produced(uint32_t src, uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1,
-                                                 bool external) {
+                                                 bool external = false) {
     if (status) return;
-    int slot = MODEL::timer_slot(dst, type, p0, p1);
-    if (cancelled && slot >= 0 && ((cancelled >> slot) & 1u)) { cancelled &= ~(1u << slot); return; }
+    if (timer_dropped(*this, dst, type, p0, p1)) return;
     uint32_t uniq = 0;
     if (LIST) {
       uniq = ++n_uniq & 0xFFFFu;                                    // Uniq(...) :570, 16-bit (DESIGN.md §2); appendMsgSend :620-622
@@ -273,21 +261,15 @@ struct ReplayMachine {
     }
     n_tosend = 0;
   }
-  __device__ __forceinline__ void handle_timer(uint32_t slot) {   // STSScheduler.enqueue_timer (:870)
+  // ExternalEventInjector.handle_timer: into messagesToSend unless ignoreTimers (STSScheduler.enqueue_timer :870)
+  __device__ __forceinline__ void enqueue_timer(uint32_t slot) {
     if (A->ignore_timers) return;
     tosend_push(slot);
   }
-  // STSScheduler.notify_timer_cancel (STSScheduler.scala:846-868)
-  __device__ __forceinline__ void cancel_timer(uint32_t self, uint32_t type, uint32_t p0, uint32_t p1) {
-    if (status) return;
-    int slot = MODEL::timer_slot(self, type, p0, p1);
-    if (slot < 0) { status = DEMI_RS_UNSUPPORTED; return; }
-    uint32_t bit = 1u << slot;
-    if (!(cancelled & bit) && __popc(cancelled) >= DEMI_TIMERSET_CAP) { status = DEMI_PS_QUEUE_OVF; return; }
-    cancelled |= bit;
-    registry &= ~bit;
+  // the cancelled timer's pending copy (STSScheduler.notify_timer_cancel :846-868)
+  __device__ __forceinline__ void cancel_pending(uint32_t self, uint32_t slot, uint32_t type, uint32_t p0, uint32_t p1) {
     for (uint32_t i = 0; i < n_tosend; i++)
-      if (tosend[(size_t)i * 32] == (uint32_t)slot) {               // order-preserving removal
+      if (tosend[(size_t)i * 32] == slot) {                         // order-preserving removal
         for (uint32_t j = i; j + 1 < n_tosend; j++) tosend[(size_t)j * 32] = tosend[(size_t)(j + 1) * 32];
         n_tosend--;
         return;
@@ -295,42 +277,13 @@ struct ReplayMachine {
     pending_take(make_hdr(DEMI_DEADLETTERS, self, type, 0), p0, p1);
   }
 
-  // Instrumenter.dispatch_new_message: re-arm a repeating timer, then receive()
   __device__ __forceinline__ void deliver(uint32_t src, uint32_t dst, uint32_t type, uint32_t p0, uint32_t p1) {
     rhash += demi_event_term(src | (dst << 8) | (type << 16), p0, p1, delivered, 0, 0);
     delivered++;
-    int slot = MODEL::timer_slot(dst, type, p0, p1);
-    if (slot >= 0 && ((registry >> slot) & 1u)) handle_timer((uint32_t)slot);
+    timer_rearm(*this, dst, type, p0, p1);
     if (status) return;
-    if constexpr (DIRECT) {
-      ReplayDirectOutbox<ReplayMachine> direct{this, dst};
-      MODEL::receive(direct, dst, actor(dst), src, type, p0, p1, A->model_flags);
-    } else {
-      LaneOutbox<OB> ob;
-      ob.base = smw + N * SW * BD; ob.bd = BD; ob.n = 0; ob.self = dst; ob.overflow = false;
-      MODEL::receive(ob, dst, actor(dst), src, type, p0, p1, A->model_flags);
-      if (ob.overflow) { status = DEMI_PS_QUEUE_OVF; return; }
-      for (uint32_t i = 0; i < ob.n && !status; i++) {
-        uint32_t w0 = ob.base[(i * 3) * BD], q0 = ob.base[(i * 3 + 1) * BD], q1 = ob.base[(i * 3 + 2) * BD];
-        uint32_t kind = w0 & 0xFF, odst = (w0 >> 8) & 0xFF, otype = (w0 >> 16) & 0xFF;
-        if (kind == OP_SEND) event_produced(dst, odst, otype, q0, q1, false);
-        else if (kind == OP_CANCEL) cancel_timer(odst, otype, q0, q1);
-        else schedule_timer(kind, odst, otype, q0, q1);
-      }
-    }
+    actor_receive<DIRECT>(*this, src, dst, type, p0, p1);
     flush();     // schedule_new_message begins with send_external_messages (:655)
-  }
-  // scheduler.scheduleOnce / schedule (Instrumenter.scala:1126-1190)
-  __device__ __forceinline__ void schedule_timer(uint32_t kind, uint32_t self, uint32_t type, uint32_t p0, uint32_t p1) {
-    if (status) return;
-    const int s2 = MODEL::timer_slot(self, type, p0, p1);
-    if (s2 < 0) { status = DEMI_RS_UNSUPPORTED; return; }
-    if ((registry >> s2) & 1u) return;
-    if (kind == OP_SCHED_REPEAT) {
-      if (__popc(registry) >= DEMI_TIMERSET_CAP) { status = DEMI_PS_QUEUE_OVF; return; }
-      registry |= 1u << s2;
-    }
-    handle_timer((uint32_t)s2);
   }
 
   // WILD + REC: the trace positions of ignored deliveries, from which WildcardMinimizer takes ignoredAbsentIds
@@ -349,7 +302,7 @@ struct ReplayMachine {
     n_rec = n_uniq = n_list = 0;
     if constexpr (WILD) { wc_inc = A->wc_include + (size_t)test_idx * A->wc_words; list_lo = 0; n_ign = 0; }
     gen = generation;
-    for (uint32_t i = 0; i < N * SW; i++) smw[i * BD] = MODEL::init_word(i, A->model_flags);
+    actor_init(*this);
     for (uint32_t a = 0; a < N; a++) part_row(a) = 0;
     n_pending = n_tosend = 0; registry = cancelled = 0;
     inaccessible = (N >= 32) ? 0xFFFFFFFFu : ((1u << N) - 1u);
