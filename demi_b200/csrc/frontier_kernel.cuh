@@ -97,7 +97,7 @@ __device__ __forceinline__ void fr_log_key(const FrLog& log, unsigned long long 
 
 // ------------------------------------------------------------------ executor
 template <class MODEL, int BD>
-struct FrExec {
+struct FrExec : TimerTable<MODEL> {
   using Model = MODEL;
   static constexpr int BLOCK = BD;
   static constexpr int N = MODEL::N_ACTORS;
@@ -113,7 +113,9 @@ struct FrExec {
   const FrArgs* A; uint32_t* smw;
   uint4* pa; uint32_t* p1a; uint32_t* nxa;       // this lane's entry e at [e * 32]
   uint16_t qhead[NQ], qtail[NQ]; uint32_t qmask[QW];
-  uint32_t n_ent, registry, cancelled, isolated, cur_len, cur_pos, status;
+  uint32_t n_ent;
+  typename TimerTable<MODEL>::mask_t registry, cancelled;
+  uint32_t isolated, cur_len, cur_pos, status;
   unsigned long long parent_id;
   int32_t nsched;
 
@@ -152,7 +154,7 @@ struct FrExec {
   // enqueue_timer = enqueue_message (Scheduler.scala:73), whatever ignoreTimers says (see DporMachine::enqueue_timer)
   __device__ __forceinline__ void enqueue_timer(uint32_t slot) {
     uint32_t dst, type, p0, p1;
-    MODEL::slot_msg(slot, dst, type, p0, p1);
+    timer_msg(*this, slot, dst, type, p0, p1);
     event_produced(DEMI_DEADLETTERS, dst, type, p0, p1);
   }
   // the cancelled timer's pending copy (DPORwHeuristics.notify_timer_cancel :961-985)
@@ -170,7 +172,7 @@ struct FrExec {
   // kt[ei]'s) (:1060-1063, :1180).  Returns the violation code.
   __device__ uint32_t run(const uint4* kt, uint32_t branch, uint32_t li, uint32_t ei, uint4* out, unsigned long long& sh) {
     actor_init(*this);
-    registry = cancelled = 0;
+    registry = cancelled = 0; timer_reset(*this);
 #pragma unroll 1
     for (int q = 0; q < NQ; q++) { qhead[q] = NIL; qtail[q] = NIL; }
     for (int w = 0; w < QW; w++) qmask[w] = 0;

@@ -60,7 +60,7 @@ enum : uint32_t { WC_EXACT = 0, WC_CLASS = 1, WC_CLOCK = 2 };   // match mode of
 // WILD: ClockClusterizer's wildcarded trace (capi_wildcard.cu).  The pending set is the insertion-ordered list of
 // the REC variant (Uniq order = list order), compacted in place when taken entries dominate it.
 template <class MODEL, int BD, bool REC = false, bool WILD = false>
-struct ReplayMachine {
+struct ReplayMachine : TimerTable<MODEL> {
   using Model = MODEL;
   static constexpr int BLOCK = BD;
   static constexpr bool LIST = REC || WILD;
@@ -79,7 +79,7 @@ struct ReplayMachine {
 
   uint32_t gen;                      // hash-table generation of this test
   uint32_t n_pending, n_tosend;
-  uint32_t registry, cancelled;      // timer-slot bitmasks
+  typename TimerTable<MODEL>::mask_t registry, cancelled;      // timer-slot bitmasks
   uint32_t inaccessible, killed;
   uint32_t status;
   uint32_t delivered, ignored;
@@ -255,15 +255,17 @@ struct ReplayMachine {
         event_produced(DEMI_DEADLETTERS, (e.x >> 16) & 0xFF, e.x >> 24, e.y, e.z, true);
       } else {
         uint32_t dst, type, p0, p1;
-        MODEL::slot_msg(code, dst, type, p0, p1);
+        timer_msg(*this, code, dst, type, p0, p1);
         event_produced(DEMI_DEADLETTERS, dst, type, p0, p1, false);
       }
     }
     n_tosend = 0;
+    timer_flushed(*this);
   }
   // ExternalEventInjector.handle_timer: into messagesToSend unless ignoreTimers (STSScheduler.enqueue_timer :870)
   __device__ __forceinline__ void enqueue_timer(uint32_t slot) {
     if (A->ignore_timers) return;
+    timer_queued(*this, slot);
     tosend_push(slot);
   }
   // the cancelled timer's pending copy (STSScheduler.notify_timer_cancel :846-868)
@@ -304,7 +306,7 @@ struct ReplayMachine {
     gen = generation;
     actor_init(*this);
     for (uint32_t a = 0; a < N; a++) part_row(a) = 0;
-    n_pending = n_tosend = 0; registry = cancelled = 0;
+    n_pending = n_tosend = 0; registry = cancelled = 0; timer_reset(*this);
     inaccessible = (N >= 32) ? 0xFFFFFFFFu : ((1u << N) - 1u);
     killed = 0; status = 0; delivered = ignored = 0; rhash = 0;
     rem_cursor = 0; alive = 0;

@@ -32,6 +32,11 @@
  *    operations that reach the scheduler.  One more ends the execution with the queue-overflow status of the engine
  *    that runs it (DEMI_PS_QUEUE_OVF for fuzzing and replay, DEMI_DS_QUEUE_OVF for DPOR); none of that receive()'s
  *    operations is applied.  Header word 8 is only the capacity hint the pending-set size is derived from.
+ *  - Timers: SCHED_ONCE / SCHED_REPEAT / CANCEL name a timer by (type, p0, p1) of the actor that issues them; any
+ *    values may be used.  Fuzzing, replay, the minimizers and frontier DPOR all run them.  Per execution at most
+ *    DEMI_TIMERSET_CAP (16) repeating timers can be registered at a time and at most 16 cancelled timers can be waiting
+ *    for their message to be dropped; one more ends the execution with the queue-overflow status, as for the compiled
+ *    models.  Scheduling a repeating timer that is already registered does nothing.
  *  - External types: the external-message filter is a 32-bit mask; type t is external iff t < 32 and bit t of the mask
  *    is set (demi_type_is_external, demi_limits.h).  Types 32..255 are always internal.
  */
