@@ -132,15 +132,16 @@ extern "C" int32_t demi_create(const demi_config* cfg, demi_handle** out) {
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaEventCreate(&h->ev0);
   if (e == cudaSuccess) e = cudaEventCreate(&h->ev1);
-  if (e == cudaSuccess) e = cudaMalloc(&h->counters_dev, 4 * sizeof(unsigned long long));
-  if (e == cudaSuccess) e = cudaMalloc(&h->rec_counts_dev, 4 * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&h->ovf_count, sizeof(uint32_t));
   if (getenv("DEMI_DISABLE_LANE_ENGINE")) h->use_lane_engine = 0;
   if (const char* e = getenv("DEMI_LANE_PENDING_CAP")) h->lane_pending_cap = (uint32_t)atoi(e);   // tests: make the lane engine defer early
-  if (e != cudaSuccess) {
-    fail(nullptr, DEMI_ERR_CUDA, "demi_create: %s", cudaGetErrorString(e));
+  int32_t rc = e == cudaSuccess ? DEMI_OK : fail(nullptr, DEMI_ERR_CUDA, "demi_create: %s", cudaGetErrorString(e));
+  // no handle yet: a failure goes to demi_last_error(NULL)
+  if (rc == DEMI_OK) rc = h->counters_dev.grow(nullptr, 4 * sizeof(unsigned long long));
+  if (rc == DEMI_OK) rc = h->rec_counts_dev.grow(nullptr, 4 * sizeof(uint32_t));
+  if (rc == DEMI_OK) rc = h->ovf_count.grow(nullptr, sizeof(uint32_t));
+  if (rc != DEMI_OK) {
     demi_destroy(h);                       // frees whatever was created before the failure
-    return DEMI_ERR_CUDA;
+    return rc;
   }
   *out = h;
   return DEMI_OK;
@@ -149,22 +150,13 @@ extern "C" int32_t demi_create(const demi_config* cfg, demi_handle** out) {
 extern "C" void demi_destroy(demi_handle* h) {
   if (!h) return;
   cudaSetDevice(h->cfg.device);
-  cudaFree(h->ext_dev); cudaFree(h->results_dev); cudaFree(h->node_scratch); cudaFree(h->pend_scratch);
-  cudaFree(h->counters_dev); cudaFree(h->rec_counts_dev); cudaFree(h->prov_scratch);
-  for (void* b : h->dpor_buf) cudaFree(b);
-  cudaFree(h->ext_sends_dev); cudaFree(h->lane_pend); cudaFree(h->ovf_list); cudaFree(h->ovf_count); cudaFree(h->fifo_scratch);
-  demi_replay_free(h);
   demi_frontier_free(h);
   demi_comm_free(h);
-  cudaFree(h->ir_blob_dev); cudaFree(h->trace_rec);
-  cudaFree(h->fz_fixed_dev); cudaFree(h->fz_arena);
-  cudaFree(h->dedup.keys); cudaFree(h->dedup.vals); cudaFree(h->dedup.keep); cudaFree(h->dedup.counts);
-  if (h->pinned) cudaFreeHost(h->pinned);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-  delete h;
+  delete h;                                // its device buffers free themselves
 }
 
 // demi_load_model: validate, keep the name table on the host, put programs + initial states on the device
@@ -197,13 +189,14 @@ extern "C" int32_t demi_load_model(demi_handle* h, const void* model_blob, size_
   while (off < nb && names.size() < (size_t)na + nt) { const size_t l = strnlen(nm + off, nb - off); names.emplace_back(nm + off, l); off += l + 1; }
   if (names.size() != (size_t)na + nt) return fail(h, DEMI_ERR_INVALID, "demi_load_model: %zu names for %u actors + %u message types", names.size(), na, nt);
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  cudaFree(h->ir_blob_dev); h->ir_blob_dev = nullptr; h->ir_loaded = false;
-  CUDA_TRY(h, cudaMalloc(&h->ir_blob_dev, words * 4));
-  CUDA_TRY(h, cudaMemcpy(h->ir_blob_dev, w, words * 4, cudaMemcpyHostToDevice));
-  h->ir_dev.recv = h->ir_blob_dev + DEMI_IR_HEADER_WORDS; h->ir_dev.inv = h->ir_dev.recv + rl; h->ir_dev.init = h->ir_dev.inv + il;
+  DevBuf blob;
+  const int32_t rc = blob.upload(h, w, words * 4);
+  if (rc != DEMI_OK) return rc;
+  h->ir_blob_dev = std::move(blob);
+  h->ir_dev.recv = h->ir_blob_dev.get<uint32_t>() + DEMI_IR_HEADER_WORDS; h->ir_dev.inv = h->ir_dev.recv + rl; h->ir_dev.init = h->ir_dev.inv + il;
   h->ir_dev.recv_len = rl; h->ir_dev.inv_len = il; h->ir_dev.n_actors = na; h->ir_dev.state_words = sw;
   h->ir_ext_mask = w[7]; h->ir_fanout = w[8]; h->ir_n_actors = na; h->ir_n_types = nt;
-  h->names = names;
+  h->names = std::move(names);
   h->ir_loaded = true;
   return DEMI_OK;
 }
@@ -252,18 +245,14 @@ extern "C" int32_t demi_set_externals(demi_handle* h, const demi_ext_event* ev, 
     describe_event(&info, &sv, ev[i]);
   }
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  cudaFree(h->ext_dev); h->ext_dev = nullptr;
+  DevBuf ext_dev, sends_dev;
+  int32_t rc;
+  if (n && (rc = ext_dev.upload(h, ev, n * sizeof(demi_ext_event))) != DEMI_OK) return rc;
+  if (!sv.empty() && (rc = sends_dev.upload(h, sv.data(), sv.size() * sizeof(uint4))) != DEMI_OK) return rc;
   h->ext_host.assign(ev, ev + n);
   h->ext_info = info;
-  if (n) {
-    CUDA_TRY(h, cudaMalloc(&h->ext_dev, n * sizeof(demi_ext_event)));
-    CUDA_TRY(h, cudaMemcpy(h->ext_dev, ev, n * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
-  }
-  cudaFree(h->ext_sends_dev); h->ext_sends_dev = nullptr;
-  if (!sv.empty()) {
-    CUDA_TRY(h, cudaMalloc(&h->ext_sends_dev, sv.size() * sizeof(uint4)));
-    CUDA_TRY(h, cudaMemcpy(h->ext_sends_dev, sv.data(), sv.size() * sizeof(uint4), cudaMemcpyHostToDevice));
-  }
+  h->ext_dev = std::move(ext_dev);
+  h->ext_sends_dev = std::move(sends_dev);
   return DEMI_OK;
 }
 
@@ -321,11 +310,9 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, LaunchMode
   const uint64_t total_warps = (uint64_t)grid * WARPS;
   const uint32_t node_cap = demi_node_cap(pcap);
 
-  if ((rc = ensure_bytes(h, (void**)&h->node_scratch, &h->node_scratch_bytes,
-                         total_warps * node_cap * sizeof(uint4))) != DEMI_OK) return rc;
+  if ((rc = h->node_scratch.grow(h, total_warps * node_cap * sizeof(uint4))) != DEMI_OK) return rc;
   if (v->pend_global)
-    if ((rc = ensure_bytes(h, (void**)&h->pend_scratch, &h->pend_scratch_bytes,
-                           total_warps * (uint64_t)v->pcap * sizeof(uint4))) != DEMI_OK) return rc;
+    if ((rc = h->pend_scratch.grow(h, total_warps * (uint64_t)v->pcap * sizeof(uint4))) != DEMI_OK) return rc;
 
   KernelArgs a{};
   a.model_flags = h->cfg.model_flags;
@@ -339,9 +326,8 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, LaunchMode
   a.fuzz_flags = p->flags;
   a.strategy = h->cfg.strategy;
   if (fifo) {
-    if ((rc = ensure_bytes(h, (void**)&h->fifo_scratch, &h->fifo_scratch_bytes,
-                           total_warps * (uint64_t)(v->pcap / 2 + 3 * FIFO_PAIRS) * sizeof(uint16_t))) != DEMI_OK) return rc;
-    a.fifo_scratch = h->fifo_scratch;
+    if ((rc = h->fifo_scratch.grow(h, total_warps * (uint64_t)(v->pcap / 2 + 3 * FIFO_PAIRS) * sizeof(uint16_t))) != DEMI_OK) return rc;
+    a.fifo_scratch = h->fifo_scratch.get<uint16_t>();
   }
   if (fifo && (prog.hard_kill || !h->filter.empty()))
     return fail(h, DEMI_ERR_INVALID, "HardKill and userDefinedFilter are offered for FullyRandom only");
@@ -352,10 +338,10 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, LaunchMode
   a.node_cap = node_cap;
   a.pending_cap = pcap;
   a.tosend_cap = tcap;
-  a.node_scratch = h->node_scratch;
-  a.pend_scratch = h->pend_scratch;
-  a.sum_steps = h->counters_dev;
-  a.n_violations = h->counters_dev + 1;
+  a.node_scratch = h->node_scratch.get<uint4>();
+  a.pend_scratch = h->pend_scratch.get<uint4>();
+  a.sum_steps = h->counters_dev.get<unsigned long long>();
+  a.n_violations = a.sum_steps + 1;
   plan->v = v; plan->mode = mode; plan->prog = &prog; plan->grid = grid; plan->smem = smem; plan->args = a;
   return DEMI_OK;
 }
@@ -374,22 +360,22 @@ static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, c
     uint64_t want = (n_items + lv->bd - 1) / lv->bd;
     int lgrid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * bps));
     const uint64_t lwarps = (uint64_t)lgrid * (lv->bd / 32);
-    if ((rc = ensure_bytes(h, (void**)&h->lane_pend, &h->lane_pend_bytes, lwarps * lv->lpcap * 32 * sizeof(uint4))) != DEMI_OK) return rc;
-    if ((rc = ensure_bytes(h, (void**)&h->ovf_list, &h->ovf_list_bytes, std::max<size_t>(n_items * sizeof(uint32_t), 64))) != DEMI_OK) return rc;
-    CUDA_TRY(h, cudaMemsetAsync(h->ovf_count, 0, sizeof(uint32_t), s));
+    if ((rc = h->lane_pend.grow(h, lwarps * lv->lpcap * 32 * sizeof(uint4))) != DEMI_OK) return rc;
+    if ((rc = h->ovf_list.grow(h, std::max<size_t>(n_items * sizeof(uint32_t), 64))) != DEMI_OK) return rc;
+    CUDA_TRY(h, cudaMemsetAsync(h->ovf_count.get(), 0, sizeof(uint32_t), s));
     KernelArgs la = a;
-    la.lane_pend = h->lane_pend;
-    la.ext_sends = plan.mode == LM_PROGRAM ? nullptr : h->ext_sends_dev;     // a campaign binds each program's table
+    la.lane_pend = h->lane_pend.get<uint4>();
+    la.ext_sends = plan.mode == LM_PROGRAM ? nullptr : h->ext_sends_dev.get<uint4>();     // a campaign binds each program's table
     la.has_partitions = plan.prog->partitions ? 1u : 0u;
     la.prog_lane_pcap = h->lane_pending_cap;
-    la.ovf_list = h->ovf_list; la.ovf_count = h->ovf_count;
+    la.ovf_list = h->ovf_list.get<uint32_t>(); la.ovf_count = h->ovf_count.get<uint32_t>();
     if (h->lane_pending_cap) la.pending_cap = std::min(la.pending_cap, h->lane_pending_cap);     // deferring is always exact
     lfn<<<lgrid, lv->bd, lsmem, s>>>(la);
     CUDA_TRY(h, cudaGetLastError());
     h->perf.kernel_launches++;
     // what the lane engine could not prove exact: a recording launch numbers its outputs by work-list position
-    if (plan.mode == LM_RECORD) { a.pos_list = h->ovf_list; a.pos_count = h->ovf_count; }
-    else { a.index_list = h->ovf_list; a.index_count = h->ovf_count; }
+    if (plan.mode == LM_RECORD) { a.pos_list = la.ovf_list; a.pos_count = la.ovf_count; }
+    else { a.index_list = la.ovf_list; a.index_count = la.ovf_count; }
   }
   if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
   plan.v->fn[plan.mode]<<<plan.grid, WARPS * 32, plan.smem, s>>>(a);
@@ -401,7 +387,7 @@ static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, c
 // A new batch: its counters and counts start from zero (an empty batch, too, reports its own); demi_fuzz_summary_dev,
 // or the host path once it syncs, fills the rest.
 static int32_t reset_batch(demi_handle* h, cudaStream_t s) {
-  CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->counters_dev.get(), 0, 4 * sizeof(unsigned long long), s));
   h->perf.kernel_launches = 0;
   h->perf.prefixes = 0;
   h->perf.deliveries = 0;
@@ -422,7 +408,7 @@ static int32_t launch_fuzz(demi_handle* h, const demi_fuzz_params* p, void* out_
   if (!out_dev) return fail(h, DEMI_ERR_INVALID, "demi_fuzz_batch_dev: null output");
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   LaunchPlan plan;
-  int32_t rc = plan_launch(h, p, LM_BATCH, h->ext_info, h->ext_dev, (uint32_t)h->ext_host.size(), &plan);
+  int32_t rc = plan_launch(h, p, LM_BATCH, h->ext_info, h->ext_dev.get<demi_ext_event>(), (uint32_t)h->ext_host.size(), &plan);
   if (rc != DEMI_OK) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   if (reset_counters && (rc = reset_batch(h, s)) != DEMI_OK) return rc;
@@ -442,14 +428,15 @@ extern "C" int32_t demi_fuzz_batch_dev(demi_handle* h, const demi_fuzz_params* p
 template <class Launch>
 static int32_t run_pipelined(demi_handle* h, const char* who, uint64_t n, uint64_t per, demi_fuzz_result* out_host, Launch launch) {
   const size_t bytes = (size_t)n * sizeof(demi_fuzz_result);
-  int32_t rc = ensure_bytes(h, (void**)&h->results_dev, &h->results_cap, std::max<size_t>(bytes, 32));
+  int32_t rc = h->results_dev.grow(h, std::max<size_t>(bytes, 32));
   if (rc != DEMI_OK) return rc;
+  demi_fuzz_result* results = h->results_dev.get<demi_fuzz_result>();
   CUDA_TRY(h, cudaEventRecord(h->ev0, h->stream));
-  if (n == 0) { rc = launch(0, 0, h->results_dev, true); if (rc != DEMI_OK) return rc; }
+  if (n == 0) { rc = launch(0, 0, results, true); if (rc != DEMI_OK) return rc; }
   std::vector<cudaEvent_t> evs;
   for (uint64_t off = 0; off < n; off += per) {
     const uint64_t m = std::min<uint64_t>(per, n - off);
-    rc = launch(off, m, h->results_dev + off, off == 0);
+    rc = launch(off, m, results + off, off == 0);
     if (rc != DEMI_OK) break;
     cudaEvent_t ev;
     cudaError_t ce = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
@@ -457,14 +444,14 @@ static int32_t run_pipelined(demi_handle* h, const char* who, uint64_t n, uint64
       evs.push_back(ev);
       ce = cudaEventRecord(ev, h->stream);
       if (ce == cudaSuccess) ce = cudaStreamWaitEvent(h->copy_stream, ev, 0);
-      if (ce == cudaSuccess) ce = cudaMemcpyAsync(out_host + off, h->results_dev + off, m * sizeof(demi_fuzz_result),
+      if (ce == cudaSuccess) ce = cudaMemcpyAsync(out_host + off, results + off, m * sizeof(demi_fuzz_result),
                                                   cudaMemcpyDeviceToHost, h->copy_stream);
     }
     if (ce != cudaSuccess) { rc = fail(h, DEMI_ERR_CUDA, "%s: %s", who, cudaGetErrorString(ce)); break; }   // events freed below
   }
   cudaError_t e = cudaEventRecord(h->ev1, h->stream);
   unsigned long long cnt[3] = {0, 0, 0};
-  if (e == cudaSuccess) e = cudaMemcpyAsync(cnt, h->counters_dev, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(cnt, h->counters_dev.get(), sizeof(cnt), cudaMemcpyDeviceToHost, h->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->copy_stream);
   for (cudaEvent_t ev : evs) cudaEventDestroy(ev);
@@ -502,7 +489,7 @@ extern "C" int32_t demi_fuzz_summary_dev(demi_handle* h, const void* /*results_d
   if (!h) return DEMI_ERR_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   unsigned long long c[3] = {0, 0, 0};
-  CUDA_TRY(h, cudaMemcpyAsync(c, h->counters_dev, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  CUDA_TRY(h, cudaMemcpyAsync(c, h->counters_dev.get(), sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   CUDA_TRY(h, cudaStreamSynchronize((cudaStream_t)stream));
   if (sum_steps) *sum_steps = c[0];
   if (n_violations) *n_violations = c[1];
@@ -525,21 +512,21 @@ static int32_t fuzz_trace(demi_handle* h, const demi_fuzz_params* p, int64_t see
   const uint32_t cap_ev = std::max<uint32_t>(cap_events, 1), cap_n = std::max<uint32_t>(cap_nodes, 1);
   // one recording buffer, kept in the handle: events | parents | result
   const size_t o_par = (size_t)cap_ev * sizeof(demi_event), o_res = (o_par + (size_t)cap_n * 2 + 15) & ~(size_t)15;
-  if ((rc = ensure_bytes(h, &h->trace_rec, &h->trace_rec_bytes, o_res + sizeof(demi_fuzz_result))) != DEMI_OK) return rc;
-  demi_event* ev_dev = (demi_event*)h->trace_rec;
-  uint16_t* par_dev = (uint16_t*)((unsigned char*)h->trace_rec + o_par);
-  demi_fuzz_result* res_dev = (demi_fuzz_result*)((unsigned char*)h->trace_rec + o_res);
+  if ((rc = h->trace_rec.grow(h, o_res + sizeof(demi_fuzz_result))) != DEMI_OK) return rc;
+  demi_event* ev_dev = h->trace_rec.get<demi_event>();
+  uint16_t* par_dev = (uint16_t*)(h->trace_rec.get<unsigned char>() + o_par);
+  demi_fuzz_result* res_dev = (demi_fuzz_result*)(h->trace_rec.get<unsigned char>() + o_res);
   plan.args.results = res_dev;
   plan.args.rec_events = ev_dev; plan.args.rec_cap = cap_events;
-  plan.args.rec_counts = h->rec_counts_dev;
+  plan.args.rec_counts = h->rec_counts_dev.get<uint32_t>();
   plan.args.rec_parent = dep_parent ? par_dev : nullptr; plan.args.rec_parent_cap = cap_nodes;
-  CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->counters_dev.get(), 0, 4 * sizeof(unsigned long long), h->stream));
   if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, h->stream));
   plan.v->fn[LM_RECORD]<<<1, WARPS * 32, plan.smem, h->stream>>>(plan.args);
   cudaError_t e = cudaGetLastError();
   demi_fuzz_result r{}; uint32_t counts[4] = {0, 0, 0, 0};
   if (e == cudaSuccess) e = cudaMemcpyAsync(&r, res_dev, sizeof(r), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(counts, h->rec_counts_dev, sizeof(counts), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(counts, h->rec_counts_dev.get(), sizeof(counts), cudaMemcpyDeviceToHost, h->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
   if (e == cudaSuccess && r.status == 0) {
     e = cudaMemcpy(events, ev_dev, (size_t)std::min(counts[0], cap_events) * sizeof(demi_event), cudaMemcpyDeviceToHost);
@@ -559,7 +546,7 @@ extern "C" int32_t demi_fuzz_trace(demi_handle* h, const demi_fuzz_params* p, in
                                    uint16_t* dep_parent, uint32_t cap_nodes, uint32_t* n_nodes,
                                    demi_fuzz_result* result) {
   if (!h) return DEMI_ERR_INVALID;
-  return fuzz_trace(h, p, seed, events, cap_events, n_events, dep_parent, cap_nodes, n_nodes, result, h->ext_dev,
+  return fuzz_trace(h, p, seed, events, cap_events, n_events, dep_parent, cap_nodes, n_nodes, result, h->ext_dev.get<demi_ext_event>(),
                     (uint32_t)h->ext_host.size(), h->ext_info);
 }
 
@@ -571,10 +558,9 @@ static int32_t launch_provenance(demi_handle* h, ProvArgs a, cudaStream_t s) {
   const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * 8));
   a.t_cap = a.mask_words * 64;
   a.scratch_stride = a.t_cap + 3 * a.par_stride;
-  int32_t rc = ensure_bytes(h, (void**)&h->prov_scratch, &h->prov_scratch_bytes,
-                      (uint64_t)grid * PW * a.scratch_stride * sizeof(uint32_t));
+  int32_t rc = h->prov_scratch.grow(h, (uint64_t)grid * PW * a.scratch_stride * sizeof(uint32_t));
   if (rc != DEMI_OK) return rc;
-  a.scratch = (uint32_t*)h->prov_scratch;
+  a.scratch = h->prov_scratch.get<uint32_t>();
   provenance_kernel<PW><<<grid, PW * 32, 0, s>>>(a);
   CUDA_TRY(h, cudaGetLastError());
   h->perf.kernel_launches++;
@@ -593,30 +579,27 @@ extern "C" int32_t demi_provenance(demi_handle* h, const demi_event* events, uin
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   const size_t ev_b = (size_t)std::max(n_events, 1u) * sizeof(demi_event), par_b = (size_t)n_nodes * 2;
   const size_t keep_b = (size_t)mask_words * 8;
-  unsigned char* buf = nullptr;                      // events | parents | counts | keep | out
+  // events | parents | counts | keep | out
   const size_t o_par = (ev_b + 15) & ~(size_t)15, o_cnt = (o_par + par_b + 15) & ~(size_t)15, o_keep = o_cnt + 16,
                o_out = o_keep + ((keep_b + 15) & ~(size_t)15), total = o_out + sizeof(demi_provenance_out);
-  CUDA_TRY(h, cudaMalloc(&buf, total));
-  const uint32_t counts[4] = {n_events, n_nodes, affected_mask, 0};
-  cudaError_t e = cudaMemcpyAsync(buf, events, (size_t)n_events * sizeof(demi_event), cudaMemcpyHostToDevice, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(buf + o_par, dep_parent, par_b, cudaMemcpyHostToDevice, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(buf + o_cnt, counts, sizeof(counts), cudaMemcpyHostToDevice, h->stream);
-  int32_t rc = DEMI_OK;
-  if (e == cudaSuccess) {
-    ProvArgs a{};
-    a.events = (const demi_event*)buf; a.ev_stride = std::max(n_events, 1u);
-    a.parent = (const uint16_t*)(buf + o_par); a.par_stride = n_nodes;
-    a.counts = (const uint32_t*)(buf + o_cnt); a.results = nullptr;
-    a.keep = (uint64_t*)(buf + o_keep); a.mask_words = mask_words;
-    a.out = (demi_provenance_out*)(buf + o_out); a.n = 1;
-    rc = launch_provenance(h, a, h->stream);
-  }
-  if (rc == DEMI_OK && e == cudaSuccess) e = cudaMemcpyAsync(keep_mask, buf + o_keep, keep_b, cudaMemcpyDeviceToHost, h->stream);
-  if (rc == DEMI_OK && e == cudaSuccess) e = cudaMemcpyAsync(out, buf + o_out, sizeof(*out), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-  cudaFree(buf);
+  DevBuf tmp;
+  int32_t rc = tmp.grow(h, total);
   if (rc != DEMI_OK) return rc;
-  if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "demi_provenance: %s", cudaGetErrorString(e));
+  unsigned char* buf = tmp.get<unsigned char>();
+  const uint32_t counts[4] = {n_events, n_nodes, affected_mask, 0};
+  CUDA_TRY(h, cudaMemcpyAsync(buf, events, (size_t)n_events * sizeof(demi_event), cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(buf + o_par, dep_parent, par_b, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(buf + o_cnt, counts, sizeof(counts), cudaMemcpyHostToDevice, h->stream));
+  ProvArgs a{};
+  a.events = (const demi_event*)buf; a.ev_stride = std::max(n_events, 1u);
+  a.parent = (const uint16_t*)(buf + o_par); a.par_stride = n_nodes;
+  a.counts = (const uint32_t*)(buf + o_cnt); a.results = nullptr;
+  a.keep = (uint64_t*)(buf + o_keep); a.mask_words = mask_words;
+  a.out = (demi_provenance_out*)(buf + o_out); a.n = 1;
+  if ((rc = launch_provenance(h, a, h->stream)) != DEMI_OK) return rc;
+  CUDA_TRY(h, cudaMemcpyAsync(keep_mask, buf + o_keep, keep_b, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(out, buf + o_out, sizeof(*out), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   return DEMI_OK;
 }
 
@@ -634,7 +617,7 @@ extern "C" int32_t demi_fuzz_provenance(demi_handle* h, const demi_fuzz_params* 
   demi_fuzz_params q = *p;
   q.n_prefixes = n;
   LaunchPlan plan;
-  int32_t rc = plan_launch(h, &q, LM_RECORD, h->ext_info, h->ext_dev, (uint32_t)h->ext_host.size(), &plan);
+  int32_t rc = plan_launch(h, &q, LM_RECORD, h->ext_info, h->ext_dev.get<demi_ext_event>(), (uint32_t)h->ext_host.size(), &plan);
   if (rc != DEMI_OK) return rc;
   // an execution records at most one MsgSend + one MsgEvent per message, plus the external markers
   const uint32_t node_cap = plan.args.node_cap;
@@ -656,45 +639,40 @@ extern "C" int32_t demi_fuzz_provenance(demi_handle* h, const demi_fuzz_params* 
   const size_t b_ev = (size_t)n * ev_cap * sizeof(demi_event), b_par = (((size_t)n * node_cap * 2) + 15) & ~(size_t)15,
                b_cnt = (size_t)n * 16, b_res = (size_t)n * sizeof(demi_fuzz_result), b_idx = (((size_t)n * 4) + 15) & ~(size_t)15,
                b_keep = (size_t)n * mask_words * 8, b_out = (size_t)n * sizeof(demi_provenance_out);
-  unsigned char* buf = nullptr;
-  CUDA_TRY(h, cudaMalloc(&buf, b_ev + b_par + b_cnt + b_res + b_idx + 16 + b_keep + b_out));
+  DevBuf tmp;
+  if ((rc = tmp.grow(h, b_ev + b_par + b_cnt + b_res + b_idx + 16 + b_keep + b_out)) != DEMI_OK) return rc;
+  unsigned char* buf = tmp.get<unsigned char>();
   unsigned char* d_par = buf + b_ev; unsigned char* d_cnt = d_par + b_par; unsigned char* d_res = d_cnt + b_cnt;
   unsigned char* d_idx = d_res + b_res; unsigned char* d_n = d_idx + b_idx; unsigned char* d_keep = d_n + 16;
   unsigned char* d_out = d_keep + b_keep;
   cudaStream_t s = h->stream;
-  cudaError_t e = cudaMemcpyAsync(d_idx, prefix_index, (size_t)n * 4, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_n, &n, 4, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_cnt, 0, b_cnt, s);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_res, 0xFF, b_res, s);
-  if (e == cudaSuccess) e = cudaEventRecord(h->ev0, s);
-  if (e == cudaSuccess) {
-    plan.args.results = (demi_fuzz_result*)d_res;
-    plan.args.index_list = (const uint32_t*)d_idx; plan.args.index_count = (const uint32_t*)d_n;
-    plan.args.rec_events = (demi_event*)buf; plan.args.rec_cap = ev_cap;
-    plan.args.rec_counts = (uint32_t*)d_cnt;
-    plan.args.rec_parent = (uint16_t*)d_par; plan.args.rec_parent_cap = node_cap;
-    plan.args.sum_steps = nullptr; plan.args.n_violations = nullptr;
-    // the lane engine records every execution it can prove exact; the slots it defers go to the general engine
-    rc = launch_plan(h, plan, n, s);
-    if (rc == DEMI_OK) {
-      ProvArgs a{};
-      a.events = (const demi_event*)buf; a.ev_stride = ev_cap;
-      a.parent = (const uint16_t*)d_par; a.par_stride = node_cap;
-      a.counts = (const uint32_t*)d_cnt; a.results = (const demi_fuzz_result*)d_res;
-      a.keep = (uint64_t*)d_keep; a.mask_words = mask_words; a.out = (demi_provenance_out*)d_out; a.n = n;
-      rc = launch_provenance(h, a, s);
-    }
-    e = cudaEventRecord(h->ev1, s);
-    if (rc == DEMI_OK && e == cudaSuccess) e = cudaMemcpyAsync(keep_masks, d_keep, b_keep, cudaMemcpyDeviceToHost, s);
-    if (rc == DEMI_OK && e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, b_out, cudaMemcpyDeviceToHost, s);
-    if (rc == DEMI_OK && e == cudaSuccess && results) e = cudaMemcpyAsync(results, d_res, b_res, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    float ms = 0.f;
-    if (e == cudaSuccess && (e = cudaEventElapsedTime(&ms, h->ev0, h->ev1)) == cudaSuccess) h->perf.kernel_ms = ms;
-  }
-  cudaFree(buf);
-  if (rc != DEMI_OK) return rc;
-  if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "demi_fuzz_provenance: %s", cudaGetErrorString(e));
+  CUDA_TRY(h, cudaMemcpyAsync(d_idx, prefix_index, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(h, cudaMemcpyAsync(d_n, &n, 4, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(h, cudaMemsetAsync(d_cnt, 0, b_cnt, s));
+  CUDA_TRY(h, cudaMemsetAsync(d_res, 0xFF, b_res, s));
+  CUDA_TRY(h, cudaEventRecord(h->ev0, s));
+  plan.args.results = (demi_fuzz_result*)d_res;
+  plan.args.index_list = (const uint32_t*)d_idx; plan.args.index_count = (const uint32_t*)d_n;
+  plan.args.rec_events = (demi_event*)buf; plan.args.rec_cap = ev_cap;
+  plan.args.rec_counts = (uint32_t*)d_cnt;
+  plan.args.rec_parent = (uint16_t*)d_par; plan.args.rec_parent_cap = node_cap;
+  plan.args.sum_steps = nullptr; plan.args.n_violations = nullptr;
+  // the lane engine records every execution it can prove exact; the slots it defers go to the general engine
+  if ((rc = launch_plan(h, plan, n, s)) != DEMI_OK) return rc;
+  ProvArgs a{};
+  a.events = (const demi_event*)buf; a.ev_stride = ev_cap;
+  a.parent = (const uint16_t*)d_par; a.par_stride = node_cap;
+  a.counts = (const uint32_t*)d_cnt; a.results = (const demi_fuzz_result*)d_res;
+  a.keep = (uint64_t*)d_keep; a.mask_words = mask_words; a.out = (demi_provenance_out*)d_out; a.n = n;
+  if ((rc = launch_provenance(h, a, s)) != DEMI_OK) return rc;
+  CUDA_TRY(h, cudaEventRecord(h->ev1, s));
+  CUDA_TRY(h, cudaMemcpyAsync(keep_masks, d_keep, b_keep, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(out, d_out, b_out, cudaMemcpyDeviceToHost, s));
+  if (results) CUDA_TRY(h, cudaMemcpyAsync(results, d_res, b_res, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  float ms = 0.f;
+  CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+  h->perf.kernel_ms = ms;
   return DEMI_OK;
 }
 
@@ -754,13 +732,12 @@ extern "C" int32_t demi_set_fuzzer(demi_handle* h, const demi_fuzzer_config* cfg
   if (cfg->num_events > DEMI_FUZZER_MAX_EVENTS)
     return fail(h, DEMI_ERR_INVALID, "demi_set_fuzzer: num_events %u, at most %d", cfg->num_events, DEMI_FUZZER_MAX_EVENTS);
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  cudaFree(h->fz_fixed_dev); h->fz_fixed_dev = nullptr; h->has_fuzzer = false;
-  if (n_prefix + n_postfix) {
-    CUDA_TRY(h, cudaMalloc(&h->fz_fixed_dev, (size_t)(n_prefix + n_postfix) * sizeof(demi_ext_event)));
-    CUDA_TRY(h, cudaMemcpy(h->fz_fixed_dev, prefix, (size_t)n_prefix * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
-    if (n_postfix)
-      CUDA_TRY(h, cudaMemcpy(h->fz_fixed_dev + n_prefix, postfix, (size_t)n_postfix * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
-  }
+  std::vector<demi_ext_event> fixed(prefix, prefix + n_prefix);
+  if (n_postfix) fixed.insert(fixed.end(), postfix, postfix + n_postfix);
+  DevBuf fixed_dev;                      // n_prefix >= 1: the prefix has a Start
+  const int32_t rc = fixed_dev.upload(h, fixed.data(), fixed.size() * sizeof(demi_ext_event));
+  if (rc != DEMI_OK) return rc;
+  h->fz_fixed_dev = std::move(fixed_dev);
   h->fuzzer = *cfg; h->fz_n_prefix = n_prefix; h->fz_n_postfix = n_postfix;
   info.sends += cfg->num_events;                 // the largest program's
   info.partitions |= cfg->partition > 0.0;
@@ -797,9 +774,9 @@ static int32_t carve_programs(demi_handle* h, uint64_t n, uint32_t stride, uint3
                               unsigned char** rest = nullptr) {
   const size_t b_ev = (size_t)n * stride * sizeof(demi_ext_event), b_hdr = ((size_t)n * sizeof(uint2) + 15) & ~(size_t)15,
                b_snd = (size_t)n * send_stride * sizeof(uint4);
-  int32_t rc = ensure_bytes(h, &h->fz_arena, &h->fz_arena_bytes, b_ev + b_hdr + b_snd + extra);
+  int32_t rc = h->fz_arena.grow(h, b_ev + b_hdr + b_snd + extra);
   if (rc != DEMI_OK) return rc;
-  unsigned char* a0 = (unsigned char*)h->fz_arena;
+  unsigned char* a0 = h->fz_arena.get<unsigned char>();
   *pa = ProgramArena{(demi_ext_event*)a0, (uint2*)(a0 + b_ev), (uint4*)(a0 + b_ev + b_hdr), stride, send_stride};
   if (rest) *rest = a0 + b_ev + b_hdr + b_snd;
   return DEMI_OK;
@@ -833,7 +810,7 @@ static int32_t launch_campaign(demi_handle* h, const demi_fuzz_params* p, int64_
   campaign_chunk(h, &stride, &send_stride);
   ProgramArena pa;
   if ((rc = carve_programs(h, n, stride, send_stride, 0, &pa)) != DEMI_OK) return rc;
-  fuzzer_gen_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(h->fuzzer, program_seed_base, n, h->fz_fixed_dev, h->fz_n_prefix,
+  fuzzer_gen_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(h->fuzzer, program_seed_base, n, h->fz_fixed_dev.get<demi_ext_event>(), h->fz_n_prefix,
                                                                  h->fz_n_postfix, pa.ev, stride, pa.hdr, pa.sends, send_stride);
   CUDA_TRY(h, cudaGetLastError());
   h->perf.kernel_launches++;
@@ -982,15 +959,16 @@ static int32_t random_tests(demi_handle* h, const uint64_t* masks, uint32_t n_te
   unsigned char* rest;
   int32_t rc = carve_programs(h, cap_tests, stride, send_stride, b_mask + b_fh + b_out + 16, &pa, &rest);
   if (rc != DEMI_OK) return rc;
-  if ((rc = ensure_bytes(h, (void**)&h->results_dev, &h->results_cap, std::max<size_t>((size_t)cap_tests * N * sizeof(demi_fuzz_result), 32))) != DEMI_OK)
-    return rc;
+  if ((rc = h->results_dev.grow(h, std::max<size_t>((size_t)cap_tests * N * sizeof(demi_fuzz_result), 32))) != DEMI_OK) return rc;
+  demi_fuzz_result* results = h->results_dev.get<demi_fuzz_result>();
+  const demi_ext_event* ext = h->ext_dev.get<demi_ext_event>();
   uint64_t* mdev = (uint64_t*)rest;
   uint32_t* first_hit = (uint32_t*)(rest + b_mask);
   demi_random_test_result* odev = (demi_random_test_result*)(rest + b_mask + b_fh);
   unsigned long long* cnt = (unsigned long long*)(rest + b_mask + b_fh + b_out);
   cudaStream_t s = h->stream;
   CUDA_TRY(h, cudaMemsetAsync(cnt, 0, sizeof(unsigned long long), s));
-  CUDA_TRY(h, cudaMemsetAsync(h->counters_dev, 0, 4 * sizeof(unsigned long long), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->counters_dev.get(), 0, 4 * sizeof(unsigned long long), s));
   CUDA_TRY(h, cudaEventRecord(h->ev0, s));
   h->perf.kernel_launches = 0;
   for (uint64_t off = 0; off < n_tests; off += per) {
@@ -998,27 +976,27 @@ static int32_t random_tests(demi_handle* h, const uint64_t* masks, uint32_t n_te
     demi_fuzz_params q = *p;
     q.n_prefixes = (uint64_t)m * N;
     LaunchPlan plan;
-    if ((rc = plan_launch(h, &q, LM_TESTS, h->ext_info, h->ext_dev, n_ext, &plan)) != DEMI_OK) return rc;
+    if ((rc = plan_launch(h, &q, LM_TESTS, h->ext_info, ext, n_ext, &plan)) != DEMI_OK) return rc;
     CUDA_TRY(h, cudaMemcpyAsync(mdev, masks + off * mask_words, (size_t)m * mask_words * 8, cudaMemcpyHostToDevice, s));
     CUDA_TRY(h, cudaMemsetAsync(first_hit, 0xFF, (size_t)m * 4, s));
-    random_subseq_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(h->ext_dev, n_ext, mdev, mask_words, m, pa.ev, stride,
+    random_subseq_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(ext, n_ext, mdev, mask_words, m, pa.ev, stride,
                                                                                      pa.hdr, pa.sends, send_stride);
     CUDA_TRY(h, cudaGetLastError());
     h->perf.kernel_launches++;
     KernelArgs& a = plan.args;
-    a.results = h->results_dev;
+    a.results = results;
     bind_programs(h, a, pa, p->max_messages);
     a.prog_execs = N;
     a.prog_first_hit = first_hit;
     if ((rc = launch_plan(h, plan, q.n_prefixes, s)) != DEMI_OK) return rc;
-    random_test_reduce_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(h->results_dev, m, N, odev, cnt);
+    random_test_reduce_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(results, m, N, odev, cnt);
     CUDA_TRY(h, cudaGetLastError());
     h->perf.kernel_launches++;
     CUDA_TRY(h, cudaMemcpyAsync(out + off, odev, (size_t)m * sizeof(demi_random_test_result), cudaMemcpyDeviceToHost, s));
   }
   unsigned long long c[4] = {0, 0, 0, 0}, ran = 0;
   CUDA_TRY(h, cudaEventRecord(h->ev1, s));
-  CUDA_TRY(h, cudaMemcpyAsync(c, h->counters_dev, sizeof(c), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(c, h->counters_dev.get(), sizeof(c), cudaMemcpyDeviceToHost, s));
   CUDA_TRY(h, cudaMemcpyAsync(&ran, cnt, sizeof(ran), cudaMemcpyDeviceToHost, s));
   CUDA_TRY(h, cudaStreamSynchronize(s));
   float ms = 0;
@@ -1062,13 +1040,10 @@ extern "C" int32_t demi_random_test_trace(demi_handle* h, const uint64_t* mask, 
     }
   if (sub.empty()) return fail(h, DEMI_ERR_INVALID, "demi_random_test_trace: the mask keeps no event");
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  demi_ext_event* dev = nullptr;
-  CUDA_TRY(h, cudaMalloc(&dev, sub.size() * sizeof(demi_ext_event)));
-  cudaError_t e = cudaMemcpy(dev, sub.data(), sub.size() * sizeof(demi_ext_event), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) { cudaFree(dev); return fail(h, DEMI_ERR_CUDA, "demi_random_test_trace: %s", cudaGetErrorString(e)); }
-  const int32_t rc = fuzz_trace(h, p, seed, events, cap_events, n_events, nullptr, 0, nullptr, result, dev, (uint32_t)sub.size(), info);
-  cudaFree(dev);
-  return rc;
+  DevBuf dev;
+  const int32_t rc = dev.upload(h, sub.data(), sub.size() * sizeof(demi_ext_event));
+  if (rc != DEMI_OK) return rc;
+  return fuzz_trace(h, p, seed, events, cap_events, n_events, nullptr, 0, nullptr, result, dev.get<demi_ext_event>(), (uint32_t)sub.size(), info);
 }
 
 #include "ddmin_driver.hpp"

@@ -19,20 +19,20 @@ extern "C" int32_t demi_dedup_compact_dev(demi_handle* h, const void* results_de
   const uint32_t n_blocks = (uint32_t)((n + DD_BLOCK - 1) / DD_BLOCK);
   int32_t rc;
   if (mode == DEMI_DM_UNIQUE) {                                 // + table[slots]: the records whose hash is ~0
-    if ((rc = ensure_bytes(h, &S.keys, &S.keys_b, (slots + 1) * sizeof(DDSlot))) != DEMI_OK) return rc;
-    CUDA_TRY(h, cudaMemsetAsync(S.keys, 0xFF, (slots + 1) * sizeof(DDSlot), s));
+    if ((rc = S.keys.grow(h, (slots + 1) * sizeof(DDSlot))) != DEMI_OK) return rc;
+    CUDA_TRY(h, cudaMemsetAsync(S.keys.get(), 0xFF, (slots + 1) * sizeof(DDSlot), s));
   }
-  if ((rc = ensure_bytes(h, &S.keep, &S.keep_b, n)) != DEMI_OK) return rc;
-  if ((rc = ensure_bytes(h, &S.counts, &S.counts_b, (size_t)n_blocks * 4)) != DEMI_OK) return rc;
+  if ((rc = S.keep.grow(h, n)) != DEMI_OK) return rc;
+  if ((rc = S.counts.grow(h, (size_t)n_blocks * 4)) != DEMI_OK) return rc;
   const demi_fuzz_result* rec = (const demi_fuzz_result*)results_dev;
   if (mode == DEMI_DM_UNIQUE) {
     int grid = (int)std::min<uint64_t>(n_blocks, (uint64_t)h->sm_count * 8);
-    dedup_insert_kernel<<<grid, DD_BLOCK, 0, s>>>(rec, n, (DDSlot*)S.keys, slots);
+    dedup_insert_kernel<<<grid, DD_BLOCK, 0, s>>>(rec, n, S.keys.get<DDSlot>(), slots);
   }
-  dedup_flag_kernel<<<n_blocks, DD_BLOCK, 0, s>>>(rec, n, mode, (const DDSlot*)S.keys, slots,
-                                                  (uint8_t*)S.keep, (uint32_t*)S.counts);
-  dedup_scan_kernel<<<1, 1024, 0, s>>>((uint32_t*)S.counts, n_blocks, (unsigned long long*)out_count_dev);
-  compact_kernel<<<n_blocks, DD_BLOCK, 0, s>>>(rec, n, (const uint8_t*)S.keep, (const uint32_t*)S.counts,
+  dedup_flag_kernel<<<n_blocks, DD_BLOCK, 0, s>>>(rec, n, mode, S.keys.get<const DDSlot>(), slots,
+                                                  S.keep.get<uint8_t>(), S.counts.get<uint32_t>());
+  dedup_scan_kernel<<<1, 1024, 0, s>>>(S.counts.get<uint32_t>(), n_blocks, (unsigned long long*)out_count_dev);
+  compact_kernel<<<n_blocks, DD_BLOCK, 0, s>>>(rec, n, S.keep.get<const uint8_t>(), S.counts.get<const uint32_t>(),
                                                (demi_fuzz_result*)out_records_dev, (uint32_t*)out_index_dev);
   CUDA_TRY(h, cudaGetLastError());
   h->perf.kernel_launches = mode == DEMI_DM_UNIQUE ? 4 : 3;
@@ -46,24 +46,21 @@ extern "C" int32_t demi_dedup_compact(demi_handle* h, const demi_fuzz_result* re
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   *out_count = 0;
   if (n == 0) return DEMI_OK;
-  void *d_in = 0, *d_out = 0, *d_idx = 0, *d_cnt = 0;
-  cudaError_t e = cudaMalloc(&d_in, n * sizeof(demi_fuzz_result));
-  if (e == cudaSuccess) e = cudaMalloc(&d_out, n * sizeof(demi_fuzz_result));
-  if (e == cudaSuccess) e = cudaMalloc(&d_idx, n * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&d_cnt, 8);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_in, results, n * sizeof(demi_fuzz_result), cudaMemcpyHostToDevice, h->stream);
-  int32_t rc = DEMI_OK;
-  if (e == cudaSuccess) rc = demi_dedup_compact_dev(h, d_in, n, mode, d_out, d_idx, d_cnt, h->stream);
+  DevBuf d_in, d_out, d_idx, d_cnt;
+  int32_t rc;
+  if ((rc = d_in.grow(h, n * sizeof(demi_fuzz_result))) != DEMI_OK) return rc;
+  if ((rc = d_out.grow(h, n * sizeof(demi_fuzz_result))) != DEMI_OK) return rc;
+  if ((rc = d_idx.grow(h, n * sizeof(uint32_t))) != DEMI_OK) return rc;
+  if ((rc = d_cnt.grow(h, 8)) != DEMI_OK) return rc;
+  CUDA_TRY(h, cudaMemcpyAsync(d_in.get(), results, n * sizeof(demi_fuzz_result), cudaMemcpyHostToDevice, h->stream));
+  if ((rc = demi_dedup_compact_dev(h, d_in.get(), n, mode, d_out.get(), d_idx.get(), d_cnt.get(), h->stream)) != DEMI_OK) return rc;
   unsigned long long cnt = 0;
-  if (e == cudaSuccess && rc == DEMI_OK) e = cudaMemcpyAsync(&cnt, d_cnt, 8, cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess && rc == DEMI_OK) e = cudaStreamSynchronize(h->stream);
-  if (e == cudaSuccess && rc == DEMI_OK && cnt) {
-    e = cudaMemcpy(out_records, d_out, cnt * sizeof(demi_fuzz_result), cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && out_index) e = cudaMemcpy(out_index, d_idx, cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost);
+  CUDA_TRY(h, cudaMemcpyAsync(&cnt, d_cnt.get(), 8, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (cnt) {
+    CUDA_TRY(h, cudaMemcpy(out_records, d_out.get(), cnt * sizeof(demi_fuzz_result), cudaMemcpyDeviceToHost));
+    if (out_index) CUDA_TRY(h, cudaMemcpy(out_index, d_idx.get(), cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   }
-  cudaFree(d_in); cudaFree(d_out); cudaFree(d_idx); cudaFree(d_cnt);
-  if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "demi_dedup_compact: %s", cudaGetErrorString(e));
-  if (rc != DEMI_OK) return rc;
   *out_count = cnt;
   return DEMI_OK;
 }

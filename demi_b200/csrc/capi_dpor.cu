@@ -116,26 +116,18 @@ int32_t dpor_run(demi_handle* h, const demi_ext_event* ext, const uint32_t* ext_
     {&d_bk, use_buckets ? S * 2 * (size_t)a.T1 * sizeof(uint32_t) : 16, -1},
   };
   // the buffers live in the handle and only grow: a DDMin run issues many launches of similar size
-  cudaError_t e = cudaSuccess;
-  size_t total = 0;
   constexpr size_t NB = sizeof(bufs) / sizeof(bufs[0]);
   static_assert(NB <= sizeof(h->dpor_buf) / sizeof(h->dpor_buf[0]), "dpor_buf too small");
   for (size_t i = 0; i < NB; i++) {
     Buf& b = bufs[i];
-    total += b.bytes;
-    if (e != cudaSuccess) break;
-    if (h->dpor_buf_bytes[i] < b.bytes) {
-      cudaFree(h->dpor_buf[i]); h->dpor_buf[i] = nullptr; h->dpor_buf_bytes[i] = 0;
-      e = cudaMalloc(&h->dpor_buf[i], b.bytes);
-      if (e == cudaSuccess) h->dpor_buf_bytes[i] = b.bytes;
+    if (const int32_t rc = h->dpor_buf[i].grow(h, b.bytes); rc != DEMI_OK) {
+      for (DevBuf& d : h->dpor_buf) d.reset();     // all of them: a smaller retry then finds the memory free
+      return rc;
     }
-    *b.p = h->dpor_buf[i];
-    if (e == cudaSuccess && b.fill >= 0) e = cudaMemsetAsync(*b.p, b.fill, b.bytes, h->stream);
+    *b.p = h->dpor_buf[i].get();
+    if (b.fill >= 0) CUDA_TRY(h, cudaMemsetAsync(*b.p, b.fill, b.bytes, h->stream));
   }
-  if (e != cudaSuccess) {
-    for (size_t i = 0; i < NB; i++) { cudaFree(h->dpor_buf[i]); h->dpor_buf[i] = nullptr; h->dpor_buf_bytes[i] = 0; }
-    return fail(h, DEMI_ERR_CUDA, "demi_dpor_batch: %s (%.1f MB of search state)", cudaGetErrorString(e), total / 1e6);
-  }
+  cudaError_t e = cudaSuccess;
   auto up = [&](void* dst, const void* src, size_t bytes) {
     if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream);
   };

@@ -127,7 +127,7 @@ struct FrState {
   demi_handle* h = nullptr; FrComm* comm = nullptr; const FrVariant* v = nullptr;
   demi_frontier_params F{}; uint32_t T1 = 0, W = 0, cap_pend = 0, rcap = 0, win_cap = 0, s_slots = 0, rec_u4 = 0;
   cudaStream_t s = nullptr;
-  std::vector<void*> allocs;
+  std::vector<DevBuf> allocs;
   // device
   uint4* tr = nullptr; uint32_t* tr_meta = nullptr; unsigned long long* E = nullptr; ulonglong2* pool = nullptr;
   ulonglong2* sel = nullptr; unsigned long long* out_hash = nullptr; uint32_t* out_viol = nullptr;
@@ -152,13 +152,12 @@ struct FrState {
   FrArgs A{};
 
   template <class T> int32_t dalloc(T** p, size_t n) {
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, std::max<size_t>(n * sizeof(T), 256));
-    if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "demi_dpor_frontier: cudaMalloc of %zu bytes: %s", n * sizeof(T), cudaGetErrorString(e));
-    allocs.push_back(q); *p = (T*)q;
-    return DEMI_OK;
+    allocs.emplace_back();
+    const int32_t rc = allocs.back().grow(h, std::max<size_t>(n * sizeof(T), 256));
+    *p = allocs.back().get<T>();
+    return rc;
   }
-  ~FrState() { for (void* q : allocs) cudaFree(q); for (auto& e : ev) if (e) cudaEventDestroy(e); }
+  ~FrState() { for (auto& e : ev) if (e) cudaEventDestroy(e); }
 };
 
 // device buffers are kept in the handle between calls with the same geometry (a search of a few hundred
@@ -591,21 +590,18 @@ int32_t fr_run(FrState& st, demi_dpor_violation* viol, uint32_t cap_viol, uint64
     // on the device, then put back in execution order)
     if (hashes) CUDA_TRY(h, cudaMemcpy(hashes, st.out_hash, std::min<unsigned long long>(st.n_exec, cap_hashes) * 8, cudaMemcpyDeviceToHost));
     if (viol && cap_viol) {
-      demi_dpor_violation* vd = nullptr; unsigned int* cnt = nullptr;
-      CUDA_TRY(h, cudaMalloc(&vd, (size_t)cap_viol * sizeof(demi_dpor_violation) + 16));
-      cnt = (unsigned int*)(vd + cap_viol);
-      cudaError_t e = cudaMemsetAsync(cnt, 0, 4, st.s);
-      if (e == cudaSuccess) {
-        fr_collect_viol_kernel<<<(unsigned)((st.n_exec + 255) / 256), 256, 0, st.s>>>(st.out_hash, st.out_viol, st.n_exec, vd, cap_viol, cnt);
-        e = cudaGetLastError();
-      }
+      DevBuf buf;
+      if ((rc = buf.grow(h, (size_t)cap_viol * sizeof(demi_dpor_violation) + 16)) != DEMI_OK) return rc;
+      demi_dpor_violation* vd = buf.get<demi_dpor_violation>();
+      unsigned int* cnt = (unsigned int*)(vd + cap_viol);
+      CUDA_TRY(h, cudaMemsetAsync(cnt, 0, 4, st.s));
+      fr_collect_viol_kernel<<<(unsigned)((st.n_exec + 255) / 256), 256, 0, st.s>>>(st.out_hash, st.out_viol, st.n_exec, vd, cap_viol, cnt);
+      CUDA_TRY(h, cudaGetLastError());
       unsigned int nv = 0;
-      if (e == cudaSuccess) e = cudaMemcpyAsync(&nv, cnt, 4, cudaMemcpyDeviceToHost, st.s);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(st.s);
+      CUDA_TRY(h, cudaMemcpyAsync(&nv, cnt, 4, cudaMemcpyDeviceToHost, st.s));
+      CUDA_TRY(h, cudaStreamSynchronize(st.s));
       const unsigned int got = std::min<unsigned int>(nv, cap_viol);
-      if (e == cudaSuccess && got) e = cudaMemcpy(viol, vd, (size_t)got * sizeof(demi_dpor_violation), cudaMemcpyDeviceToHost);
-      cudaFree(vd);
-      if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "demi_dpor_frontier: %s", cudaGetErrorString(e));
+      if (got) CUDA_TRY(h, cudaMemcpy(viol, vd, (size_t)got * sizeof(demi_dpor_violation), cudaMemcpyDeviceToHost));
       std::sort(viol, viol + got, [](const demi_dpor_violation& a, const demi_dpor_violation& b) { return a.interleaving < b.interleaving; });
       h->perf.kernel_launches++;
     }

@@ -36,10 +36,10 @@ ReplayArgs replay_args(const demi_handle* h, uint32_t looking_for, uint32_t flag
   ReplayArgs a{};
   a.model_flags = h->cfg.model_flags; a.blocked_mask = h->cfg.blocked_mask; a.ignore_timers = h->cfg.ignore_timers;
   a.looking_for = looking_for; a.flags = flags;
-  a.events = (const uint4*)h->trace_dev; a.n_events = (uint32_t)h->trace_host.size();
-  a.ev_ordinal = h->ev_ordinal_dev;
-  a.ext = (const uint4*)h->trace_ext_dev; a.n_ext = (uint32_t)h->trace_ext_host.size();
-  a.send_ext_index = h->send_ext_index_dev; a.n_sends = h->trace_n_ext_sends;
+  a.events = h->trace_dev.get<const uint4>(); a.n_events = (uint32_t)h->trace_host.size();
+  a.ev_ordinal = h->ev_ordinal_dev.get<uint16_t>();
+  a.ext = h->trace_ext_dev.get<const uint4>(); a.n_ext = (uint32_t)h->trace_ext_host.size();
+  a.send_ext_index = h->send_ext_index_dev.get<uint16_t>(); a.n_sends = h->trace_n_ext_sends;
   a.external_type_mask = demi_ext_type_mask(h);
   a.n_uniq_words = (h->trace_n_uniq + 31) / 32;
   return a;
@@ -47,12 +47,6 @@ ReplayArgs replay_args(const demi_handle* h, uint32_t looking_for, uint32_t flag
 
 cudaError_t replay_ir_bind(const demi_handle* h, cudaStream_t s) {
   return h->cfg.model == DEMI_MODEL_IR ? ir_bind(h->ir_dev, s) : cudaSuccess;
-}
-
-void demi_replay_free(demi_handle* h) {
-  cudaFree(h->trace_dev); cudaFree(h->trace_ext_dev); cudaFree(h->ev_ordinal_dev); cudaFree(h->send_ext_index_dev);
-  cudaFree(h->rp_table); cudaFree(h->rp_tosend); cudaFree(h->rp_pruned); cudaFree(h->rp_masks); cudaFree(h->rp_results);
-  cudaFree(h->rp_counters);
 }
 
 extern "C" int32_t demi_set_trace(demi_handle* h, const demi_event* events, uint32_t n_events,
@@ -92,6 +86,15 @@ extern "C" int32_t demi_set_trace(demi_handle* h, const demi_event* events, uint
     }
   std::vector<uint16_t> sidx;
   for (uint32_t i = 0; i < n_externals; i++) if (externals[i].kind == DEMI_EXT_SEND) sidx.push_back((uint16_t)i);
+  DevBuf ext_dev, ord_dev, sidx_dev, trace_dev;
+  int32_t rc;
+  if ((rc = ext_dev.upload(h, externals, n_externals * sizeof(demi_ext_event))) != DEMI_OK) return rc;
+  if ((rc = ord_dev.upload(h, ordinal.data(), n_events * sizeof(uint16_t))) != DEMI_OK) return rc;
+  if ((rc = sidx_dev.grow(h, std::max<size_t>(sidx.size(), 1) * sizeof(uint16_t))) != DEMI_OK) return rc;
+  if (!sidx.empty())
+    CUDA_TRY(h, cudaMemcpy(sidx_dev.get(), sidx.data(), sidx.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
+  if ((rc = trace_dev.upload(h, events, n_events * sizeof(demi_event))) != DEMI_OK) return rc;
+  if ((rc = h->rp_counters.grow(h, 2 * sizeof(unsigned long long))) != DEMI_OK) return rc;     // allocated once per handle
   h->trace_host.assign(events, events + n_events);
   h->trace_ext_host.assign(externals, externals + n_externals);
   h->send_ext_index_host = sidx;
@@ -99,18 +102,8 @@ extern "C" int32_t demi_set_trace(demi_handle* h, const demi_event* events, uint
   h->trace_n_uniq = max_uniq + 1;
   h->trace_n_send_events = n_send_events;
   h->trace_n_ext_sends = (uint32_t)sidx.size();
-  cudaFree(h->trace_dev); cudaFree(h->trace_ext_dev); cudaFree(h->ev_ordinal_dev); cudaFree(h->send_ext_index_dev);
-  h->trace_dev = h->trace_ext_dev = nullptr; h->ev_ordinal_dev = h->send_ext_index_dev = nullptr;
-  CUDA_TRY(h, cudaMalloc(&h->trace_dev, n_events * sizeof(demi_event)));
-  CUDA_TRY(h, cudaMalloc(&h->trace_ext_dev, n_externals * sizeof(demi_ext_event)));
-  CUDA_TRY(h, cudaMalloc(&h->ev_ordinal_dev, n_events * sizeof(uint16_t)));
-  CUDA_TRY(h, cudaMalloc(&h->send_ext_index_dev, std::max<size_t>(sidx.size(), 1) * sizeof(uint16_t)));
-  CUDA_TRY(h, cudaMemcpy(h->trace_dev, events, n_events * sizeof(demi_event), cudaMemcpyHostToDevice));
-  CUDA_TRY(h, cudaMemcpy(h->trace_ext_dev, externals, n_externals * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
-  CUDA_TRY(h, cudaMemcpy(h->ev_ordinal_dev, ordinal.data(), n_events * sizeof(uint16_t), cudaMemcpyHostToDevice));
-  if (!sidx.empty())
-    CUDA_TRY(h, cudaMemcpy(h->send_ext_index_dev, sidx.data(), sidx.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-  if (!h->rp_counters) CUDA_TRY(h, cudaMalloc(&h->rp_counters, 2 * sizeof(unsigned long long)));
+  h->trace_dev = std::move(trace_dev); h->trace_ext_dev = std::move(ext_dev);
+  h->ev_ordinal_dev = std::move(ord_dev); h->send_ext_index_dev = std::move(sidx_dev);
   return DEMI_OK;
 }
 
@@ -170,27 +163,26 @@ static int32_t launch_replay(demi_handle* h, const void* masks_dev, const void* 
   a.tosend_cap = demi_tosend_cap(h->trace_n_ext_sends);
   a.table_slots = demi_pow2_at_least(2 * a.pending_cap, 256, 1u << 16);
   const size_t table_bytes = warps * a.table_slots * 32 * sizeof(uint4);
-  const bool fresh_table = h->rp_table_bytes < table_bytes;
-  if ((rc = ensure_bytes(h, &h->rp_table, &h->rp_table_bytes, table_bytes)) != DEMI_OK) return rc;
-  if ((rc = ensure_bytes(h, &h->rp_tosend, &h->rp_tosend_bytes, warps * a.tosend_cap * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
+  const bool fresh_table = h->rp_table.bytes() < table_bytes;
+  if ((rc = h->rp_table.grow(h, table_bytes)) != DEMI_OK) return rc;
+  if ((rc = h->rp_tosend.grow(h, warps * a.tosend_cap * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
   if (flags & DEMI_RF_FILTER_KNOWN_ABSENTS)
-    if ((rc = ensure_bytes(h, &h->rp_pruned, &h->rp_pruned_bytes,
-                           warps * (a.n_uniq_words + rv->n_actors) * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
+    if ((rc = h->rp_pruned.grow(h, warps * (a.n_uniq_words + rv->n_actors) * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
   // Generation stamps: each launch gets a fresh range [gen_base, gen_base + tests per thread]; the table is
   // cleared only when it was (re)allocated, its geometry changed, or the 16-bit range is exhausted.
   const uint32_t per_thread = (uint32_t)(((uint64_t)n_masks + (uint64_t)grid * rv->bd - 1) / ((uint64_t)grid * rv->bd)) + 1;
   const uint64_t geometry = ((uint64_t)a.table_slots << 32) ^ warps;
   if (fresh_table || h->rp_gen_next == 0 || h->rp_table_geometry != geometry || h->rp_gen_next + per_thread >= 0xFFF0u || record) {
-    CUDA_TRY(h, cudaMemsetAsync(h->rp_table, 0, table_bytes, s));
+    CUDA_TRY(h, cudaMemsetAsync(h->rp_table.get(), 0, table_bytes, s));
     h->rp_gen_next = 1;
     h->rp_table_geometry = geometry;
   }
   a.gen_base = h->rp_gen_next;
   h->rp_gen_next = record ? 0 : h->rp_gen_next + per_thread;   // the recording variant leaves list entries behind: clear next time
-  CUDA_TRY(h, cudaMemsetAsync(h->rp_counters, 0, 2 * sizeof(unsigned long long), s));
-  a.table = (uint4*)h->rp_table; a.tosend = (uint32_t*)h->rp_tosend;
-  a.pruned = (flags & DEMI_RF_FILTER_KNOWN_ABSENTS) ? (uint32_t*)h->rp_pruned : nullptr;
-  a.counters = h->rp_counters;
+  CUDA_TRY(h, cudaMemsetAsync(h->rp_counters.get(), 0, 2 * sizeof(unsigned long long), s));
+  a.table = h->rp_table.get<uint4>(); a.tosend = h->rp_tosend.get<uint32_t>();
+  a.pruned = (flags & DEMI_RF_FILTER_KNOWN_ABSENTS) ? h->rp_pruned.get<uint32_t>() : nullptr;
+  a.counters = h->rp_counters.get<unsigned long long>();
   CUDA_TRY(h, replay_ir_bind(h, s));
   rv->fn[0][record]<<<record ? 1 : grid, rv->bd, rv->smem, s>>>(a);
   CUDA_TRY(h, cudaGetLastError());
@@ -208,17 +200,17 @@ extern "C" int32_t demi_replay_batch_ex(demi_handle* h, const uint64_t* masks, c
   int32_t rc;
   const size_t mbytes = masks ? (size_t)n_tests * mask_words * sizeof(uint64_t) : 0, rbytes = (size_t)n_tests * sizeof(demi_replay_result);
   const size_t sbytes = skip_events ? (size_t)n_tests * sizeof(uint32_t) : 0;
-  if ((rc = ensure_bytes(h, &h->rp_masks, &h->rp_masks_bytes, std::max<size_t>(mbytes + sbytes, 8))) != DEMI_OK) return rc;
-  if ((rc = ensure_bytes(h, &h->rp_results, &h->rp_results_bytes, rbytes)) != DEMI_OK) return rc;
-  char* base = (char*)h->rp_masks;
+  if ((rc = h->rp_masks.grow(h, std::max<size_t>(mbytes + sbytes, 8))) != DEMI_OK) return rc;
+  if ((rc = h->rp_results.grow(h, rbytes)) != DEMI_OK) return rc;
+  char* base = h->rp_masks.get<char>();
   if (masks) CUDA_TRY(h, cudaMemcpyAsync(base, masks, mbytes, cudaMemcpyHostToDevice, h->stream));
   if (skip_events) CUDA_TRY(h, cudaMemcpyAsync(base + mbytes, skip_events, sbytes, cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaEventRecord(h->ev0, h->stream));
   rc = launch_replay(h, masks ? base : nullptr, skip_events ? base + mbytes : nullptr, n_tests, mask_words, looking_for, flags,
-                     h->rp_results, h->stream, nullptr, 0, nullptr);
+                     h->rp_results.get(), h->stream, nullptr, 0, nullptr);
   if (rc != DEMI_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev1, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(out_host, h->rp_results, rbytes, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(out_host, h->rp_results.get(), rbytes, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   float ms = 0;
   CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
@@ -232,26 +224,23 @@ extern "C" int32_t demi_replay_trace(demi_handle* h, const uint64_t* mask, uint3
   if (!h) return DEMI_ERR_INVALID;
   if (!events || !cap_events || !result) return fail(h, DEMI_ERR_INVALID, "demi_replay_trace: null buffer");
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  void *d_mask = 0, *d_skip = 0, *d_rec = 0, *d_cnt = 0, *d_res = 0;
-  cudaError_t e = cudaMalloc(&d_rec, (size_t)cap_events * sizeof(demi_event));
-  if (e == cudaSuccess) e = cudaMalloc(&d_cnt, 4);
-  if (e == cudaSuccess) e = cudaMalloc(&d_res, sizeof(demi_replay_result));
-  if (e == cudaSuccess) e = cudaMalloc(&d_skip, 4);
-  if (e == cudaSuccess && mask) e = cudaMalloc(&d_mask, (size_t)mask_words * 8);
-  if (e == cudaSuccess && mask) e = cudaMemcpyAsync(d_mask, mask, (size_t)mask_words * 8, cudaMemcpyHostToDevice, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_skip, &skip_event, 4, cudaMemcpyHostToDevice, h->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_cnt, 0, 4, h->stream);
-  int32_t rc = DEMI_OK;
-  if (e == cudaSuccess) rc = launch_replay(h, d_mask, d_skip, 1, mask_words, looking_for, flags, d_res, h->stream,
-                                           (demi_event*)d_rec, cap_events, (uint32_t*)d_cnt);
+  DevBuf d_mask, d_skip, d_rec, d_cnt, d_res;
+  int32_t rc;
+  if ((rc = d_rec.grow(h, (size_t)cap_events * sizeof(demi_event))) != DEMI_OK) return rc;
+  if ((rc = d_cnt.grow(h, 4)) != DEMI_OK) return rc;
+  if ((rc = d_res.grow(h, sizeof(demi_replay_result))) != DEMI_OK) return rc;
+  if ((rc = d_skip.grow(h, 4)) != DEMI_OK) return rc;
+  if (mask && (rc = d_mask.grow(h, (size_t)mask_words * 8)) != DEMI_OK) return rc;
+  if (mask) CUDA_TRY(h, cudaMemcpyAsync(d_mask.get(), mask, (size_t)mask_words * 8, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(d_skip.get(), &skip_event, 4, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(d_cnt.get(), 0, 4, h->stream));
+  if ((rc = launch_replay(h, d_mask.get(), d_skip.get(), 1, mask_words, looking_for, flags, d_res.get(), h->stream,
+                          d_rec.get<demi_event>(), cap_events, d_cnt.get<uint32_t>())) != DEMI_OK) return rc;
   uint32_t cnt = 0;
-  if (e == cudaSuccess && rc == DEMI_OK) e = cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess && rc == DEMI_OK) e = cudaMemcpyAsync(result, d_res, sizeof(demi_replay_result), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess && rc == DEMI_OK) e = cudaStreamSynchronize(h->stream);
-  if (e == cudaSuccess && rc == DEMI_OK && cnt) e = cudaMemcpy(events, d_rec, (size_t)std::min(cnt, cap_events) * sizeof(demi_event), cudaMemcpyDeviceToHost);
-  cudaFree(d_mask); cudaFree(d_skip); cudaFree(d_rec); cudaFree(d_cnt); cudaFree(d_res);
-  if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "demi_replay_trace: %s", cudaGetErrorString(e));
-  if (rc != DEMI_OK) return rc;
+  CUDA_TRY(h, cudaMemcpyAsync(&cnt, d_cnt.get(), 4, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(result, d_res.get(), sizeof(demi_replay_result), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (cnt) CUDA_TRY(h, cudaMemcpy(events, d_rec.get(), (size_t)std::min(cnt, cap_events) * sizeof(demi_event), cudaMemcpyDeviceToHost));
   if (n_events) *n_events = cnt;
   return DEMI_OK;
 }
@@ -264,16 +253,16 @@ extern "C" int32_t demi_replay_batch(demi_handle* h, const uint64_t* masks, uint
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   int32_t rc;
   const size_t mbytes = (size_t)n_masks * mask_words * sizeof(uint64_t), rbytes = (size_t)n_masks * sizeof(demi_replay_result);
-  if ((rc = ensure_bytes(h, &h->rp_masks, &h->rp_masks_bytes, mbytes)) != DEMI_OK) return rc;
-  if ((rc = ensure_bytes(h, &h->rp_results, &h->rp_results_bytes, rbytes)) != DEMI_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(h->rp_masks, masks, mbytes, cudaMemcpyHostToDevice, h->stream));
+  if ((rc = h->rp_masks.grow(h, mbytes)) != DEMI_OK) return rc;
+  if ((rc = h->rp_results.grow(h, rbytes)) != DEMI_OK) return rc;
+  CUDA_TRY(h, cudaMemcpyAsync(h->rp_masks.get(), masks, mbytes, cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaEventRecord(h->ev0, h->stream));
-  rc = demi_replay_batch_dev(h, h->rp_masks, n_masks, mask_words, looking_for, flags, h->rp_results, h->stream);
+  rc = demi_replay_batch_dev(h, h->rp_masks.get(), n_masks, mask_words, looking_for, flags, h->rp_results.get(), h->stream);
   if (rc != DEMI_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev1, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(out_host, h->rp_results, rbytes, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(out_host, h->rp_results.get(), rbytes, cudaMemcpyDeviceToHost, h->stream));
   unsigned long long c[2] = {0, 0};
-  CUDA_TRY(h, cudaMemcpyAsync(c, h->rp_counters, sizeof(c), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(c, h->rp_counters.get(), sizeof(c), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   float ms = 0;
   CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));

@@ -90,46 +90,42 @@ int32_t wc_launch(demi_handle* h, const WcTrace& t, const uint64_t* include_host
   const size_t ev_bytes = t.ev.size() * sizeof(uint32_t), inc_bytes = (size_t)n_tests * t.words * sizeof(uint64_t);
   // staging in rp_masks: include masks | per-event modes | the two REC counters
   const size_t ev_off = (inc_bytes + 15) & ~(size_t)15, cnt_off = (ev_off + ev_bytes + 15) & ~(size_t)15;
-  if ((rc = ensure_bytes(h, &h->rp_masks, &h->rp_masks_bytes, cnt_off + 16)) != DEMI_OK) return rc;
-  if ((rc = ensure_bytes(h, &h->rp_results, &h->rp_results_bytes, (size_t)n_tests * sizeof(demi_replay_result))) != DEMI_OK) return rc;
-  if ((rc = ensure_bytes(h, &h->rp_table, &h->rp_table_bytes, warps * warp_bytes)) != DEMI_OK) return rc;
-  if ((rc = ensure_bytes(h, &h->rp_tosend, &h->rp_tosend_bytes, warps * a.tosend_cap * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
+  if ((rc = h->rp_masks.grow(h, cnt_off + 16)) != DEMI_OK) return rc;
+  if ((rc = h->rp_results.grow(h, (size_t)n_tests * sizeof(demi_replay_result))) != DEMI_OK) return rc;
+  if ((rc = h->rp_table.grow(h, warps * warp_bytes)) != DEMI_OK) return rc;
+  if ((rc = h->rp_tosend.grow(h, warps * a.tosend_cap * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
   if (flags & DEMI_RF_FILTER_KNOWN_ABSENTS)
-    if ((rc = ensure_bytes(h, &h->rp_pruned, &h->rp_pruned_bytes, warps * (a.n_uniq_words + wv->n_actors) * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
+    if ((rc = h->rp_pruned.grow(h, warps * (a.n_uniq_words + wv->n_actors) * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
   h->rp_gen_next = 0;
-  char* base = (char*)h->rp_masks;
+  char* base = h->rp_masks.get<char>();
   uint32_t* counts = (uint32_t*)(base + cnt_off);
   CUDA_TRY(h, cudaMemcpyAsync(base, include_host, inc_bytes, cudaMemcpyHostToDevice, s));
   CUDA_TRY(h, cudaMemcpyAsync(base + ev_off, t.ev.data(), ev_bytes, cudaMemcpyHostToDevice, s));
   a.wc_include = (const uint64_t*)base; a.wc_ev = (const uint32_t*)(base + ev_off);
-  a.results = (demi_replay_result*)h->rp_results;
-  a.table = (uint4*)h->rp_table; a.tosend = (uint32_t*)h->rp_tosend;
-  a.pruned = (flags & DEMI_RF_FILTER_KNOWN_ABSENTS) ? (uint32_t*)h->rp_pruned : nullptr;
-  CUDA_TRY(h, cudaMemsetAsync(h->rp_counters, 0, 2 * sizeof(unsigned long long), s));
-  a.counters = h->rp_counters;
-  void *d_rec = nullptr, *d_ign = nullptr;
+  a.results = h->rp_results.get<demi_replay_result>();
+  a.table = h->rp_table.get<uint4>(); a.tosend = h->rp_tosend.get<uint32_t>();
+  a.pruned = (flags & DEMI_RF_FILTER_KNOWN_ABSENTS) ? h->rp_pruned.get<uint32_t>() : nullptr;
+  CUDA_TRY(h, cudaMemsetAsync(h->rp_counters.get(), 0, 2 * sizeof(unsigned long long), s));
+  a.counters = h->rp_counters.get<unsigned long long>();
+  DevBuf d_rec, d_ign;
   if (record) {
-    CUDA_TRY(h, cudaMalloc(&d_rec, (size_t)rec_cap * sizeof(demi_event)));
-    if (cudaMalloc(&d_ign, (size_t)std::max<uint32_t>(ign_cap, 1) * sizeof(uint32_t)) != cudaSuccess) {
-      cudaFree(d_rec); return fail(h, DEMI_ERR_CUDA, "wildcard: cudaMalloc failed");
-    }
+    if ((rc = d_rec.grow(h, (size_t)rec_cap * sizeof(demi_event))) != DEMI_OK) return rc;
+    if ((rc = d_ign.grow(h, (size_t)std::max<uint32_t>(ign_cap, 1) * sizeof(uint32_t))) != DEMI_OK) return rc;
     CUDA_TRY(h, cudaMemsetAsync(counts, 0, 8, s));
-    a.rec_events = (demi_event*)d_rec; a.rec_cap = rec_cap; a.rec_count = counts;
-    a.wc_ignored = (uint32_t*)d_ign; a.wc_ignored_cap = ign_cap; a.wc_ignored_count = counts + 1;
+    a.rec_events = d_rec.get<demi_event>(); a.rec_cap = rec_cap; a.rec_count = counts;
+    a.wc_ignored = d_ign.get<uint32_t>(); a.wc_ignored_cap = ign_cap; a.wc_ignored_count = counts + 1;
   }
   CUDA_TRY(h, replay_ir_bind(h, s));
   CUDA_TRY(h, cudaEventRecord(h->ev0, s));
   fn<<<grid, wv->bd, wv->smem, s>>>(a);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaEventRecord(h->ev1, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out_host, h->rp_results, (size_t)n_tests * sizeof(demi_replay_result), cudaMemcpyDeviceToHost, s);
+  CUDA_TRY(h, cudaGetLastError());
+  CUDA_TRY(h, cudaEventRecord(h->ev1, s));
+  CUDA_TRY(h, cudaMemcpyAsync(out_host, a.results, (size_t)n_tests * sizeof(demi_replay_result), cudaMemcpyDeviceToHost, s));
   uint32_t c[2] = {0, 0};
-  if (e == cudaSuccess && record) e = cudaMemcpyAsync(c, counts, sizeof(c), cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  if (e == cudaSuccess && record && c[0]) e = cudaMemcpy(rec_host, d_rec, (size_t)std::min(c[0], rec_cap) * sizeof(demi_event), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && record && c[1] && ign_host) e = cudaMemcpy(ign_host, d_ign, (size_t)std::min(c[1], ign_cap) * sizeof(uint32_t), cudaMemcpyDeviceToHost);
-  cudaFree(d_rec); cudaFree(d_ign);
-  if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "wildcard replay: %s", cudaGetErrorString(e));
+  if (record) CUDA_TRY(h, cudaMemcpyAsync(c, counts, sizeof(c), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  if (record && c[0]) CUDA_TRY(h, cudaMemcpy(rec_host, d_rec.get(), (size_t)std::min(c[0], rec_cap) * sizeof(demi_event), cudaMemcpyDeviceToHost));
+  if (record && c[1] && ign_host) CUDA_TRY(h, cudaMemcpy(ign_host, d_ign.get(), (size_t)std::min(c[1], ign_cap) * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   float ms = 0;
   CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
   h->perf.kernel_ms = ms; h->perf.kernel_launches = 1; h->perf.prefixes = n_tests;

@@ -16,8 +16,30 @@
 
 extern thread_local std::string g_create_error;
 
-struct DedupScratch { void* keys = nullptr; size_t keys_b = 0; void* vals = nullptr; size_t vals_b = 0;
-                      void* keep = nullptr; size_t keep_b = 0; void* counts = nullptr; size_t counts_b = 0; };
+struct demi_handle;
+// A device allocation with one owner, which frees it: moved, never copied.  Every device buffer of the library is one.
+class DevBuf {
+ public:
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : p_(o.p_), bytes_(o.bytes_) { o.p_ = nullptr; o.bytes_ = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) { reset(); std::swap(p_, o.p_); std::swap(bytes_, o.bytes_); }
+    return *this;
+  }
+  ~DevBuf() { reset(); }
+  void reset() { if (p_) cudaFree(p_); p_ = nullptr; bytes_ = 0; }
+  // At least `bytes`: the buffer is kept when it is big enough, else freed and allocated anew.  On failure it is empty
+  // and the call returns DEMI_ERR_CUDA through fail().
+  int32_t grow(demi_handle* h, size_t bytes);
+  // grow(bytes), then a synchronous copy of host `src`
+  int32_t upload(demi_handle* h, const void* src, size_t bytes);
+  template <class T = void> T* get() const { return (T*)p_; }
+  size_t bytes() const { return bytes_; }
+ private:
+  void* p_ = nullptr; size_t bytes_ = 0;
+};
+
+struct DedupScratch { DevBuf keys, keep, counts; };
 
 // What the fuzz launches need to know about an external program: its Sends (for a Fuzzer, those of its largest
 // program), whether it has a HardKill or a Partition / UnPartition, and whether no two of its Sends are equal (two
@@ -31,26 +53,21 @@ struct demi_handle {
   int sm_count = 0;
   // external program
   std::vector<demi_ext_event> ext_host;
-  demi_ext_event* ext_dev = nullptr;
+  DevBuf ext_dev;                                  // demi_ext_event[ext_host.size()]
   ProgramInfo ext_info;
   // device buffers
-  demi_fuzz_result* results_dev = nullptr; size_t results_cap = 0;
-  uint4* node_scratch = nullptr; size_t node_scratch_bytes = 0;
-  uint4* pend_scratch = nullptr; size_t pend_scratch_bytes = 0;
-  unsigned long long* counters_dev = nullptr;      // [0]=sum_steps [1]=n_violations
+  DevBuf results_dev;                              // demi_fuzz_result
+  DevBuf node_scratch, pend_scratch;               // uint4
+  DevBuf counters_dev;                             // unsigned long long: [0]=sum_steps [1]=n_violations
   // lane engine
-  uint4* ext_sends_dev = nullptr;
-  uint4* lane_pend = nullptr; size_t lane_pend_bytes = 0;
-  uint32_t* ovf_list = nullptr; size_t ovf_list_bytes = 0;
-  uint32_t* ovf_count = nullptr;
-  uint16_t* fifo_scratch = nullptr; size_t fifo_scratch_bytes = 0;
+  DevBuf ext_sends_dev, lane_pend;                 // uint4
+  DevBuf ovf_list, ovf_count;                      // uint32_t
+  DevBuf fifo_scratch;                             // uint16_t
   int use_lane_engine = 1;
   uint32_t lane_pending_cap = 0;      // DEMI_LANE_PENDING_CAP (tests): the lane engine defers beyond this many pending messages
-  uint32_t* rec_counts_dev = nullptr;
-  void* prov_scratch = nullptr; size_t prov_scratch_bytes = 0;
-  void* dpor_buf[24] = {}; size_t dpor_buf_bytes[24] = {};     // K3 per-search structures (capi_dpor.cu)
-  // pinned staging for host transfers
-  void* pinned = nullptr; size_t pinned_bytes = 0;
+  DevBuf rec_counts_dev;                           // uint32_t
+  DevBuf prov_scratch;
+  DevBuf dpor_buf[24];                             // K3 per-search structures (capi_dpor.cu)
   cudaStream_t stream = nullptr, copy_stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   demi_perf perf{};
@@ -59,21 +76,18 @@ struct demi_handle {
   std::vector<demi_ext_event> trace_ext_host;
   std::vector<uint16_t> send_ext_index_host;
   std::vector<int32_t> conjoined;          // UnmodifiedEventDag._conjoinedAtoms over trace_ext_host (demi_conjoin_atoms)
-  void* trace_dev = nullptr; void* trace_ext_dev = nullptr;
-  uint16_t* ev_ordinal_dev = nullptr; uint16_t* send_ext_index_dev = nullptr;
+  DevBuf trace_dev, trace_ext_dev;                 // trace_host, trace_ext_host
+  DevBuf ev_ordinal_dev, send_ext_index_dev;       // uint16_t
   uint32_t trace_n_uniq = 0, trace_n_send_events = 0, trace_n_ext_sends = 0;
-  void* rp_table = nullptr; size_t rp_table_bytes = 0; uint32_t rp_gen_next = 0; uint64_t rp_table_geometry = 0;
-  void* rp_tosend = nullptr; size_t rp_tosend_bytes = 0;
-  void* rp_pruned = nullptr; size_t rp_pruned_bytes = 0;
-  void* rp_masks = nullptr; size_t rp_masks_bytes = 0;
-  void* rp_results = nullptr; size_t rp_results_bytes = 0;
-  unsigned long long* rp_counters = nullptr;
+  DevBuf rp_table; uint32_t rp_gen_next = 0; uint64_t rp_table_geometry = 0;
+  DevBuf rp_tosend, rp_pruned, rp_masks, rp_results;
+  DevBuf rp_counters;                              // unsigned long long[2]
   // ---- communicator (capi_frontier.cu): NCCL inside the library
   void* comm = nullptr;
   void* frontier = nullptr;      // cached K3F buffers
   // ---- a model loaded with demi_load_model (model == DEMI_MODEL_IR)
   bool ir_loaded = false;
-  uint32_t* ir_blob_dev = nullptr;
+  DevBuf ir_blob_dev;                              // the blob's header and programs (ir_dev points into it)
   demi_ir_device ir_dev{};
   uint32_t ir_ext_mask = 0, ir_fanout = 0, ir_n_actors = 0, ir_n_types = 0;
   std::vector<std::string> names;      // actor names, then message-type names
@@ -87,14 +101,13 @@ struct demi_handle {
   bool has_fuzzer = false;
   demi_fuzzer_config fuzzer{};
   uint32_t fz_n_prefix = 0, fz_n_postfix = 0;
-  demi_ext_event* fz_fixed_dev = nullptr;                 // prefix | postfix
+  DevBuf fz_fixed_dev;                                    // demi_ext_event: prefix | postfix
   ProgramInfo fz_info;                                    // sends: prefix + postfix + num_events
-  void* fz_arena = nullptr; size_t fz_arena_bytes = 0;
+  DevBuf fz_arena;
   // ---- launch bookkeeping
   std::map<const void*, int> occupancy;          // kernel -> resident blocks per SM (asked once per handle)
-  void* trace_rec = nullptr; size_t trace_rec_bytes = 0;   // demi_fuzz_trace's recording buffer
+  DevBuf trace_rec;                              // demi_fuzz_trace's recording buffer
 };
-void demi_replay_free(demi_handle* h);
 // K2, STSSched replay (capi_replay.cu), for both the exact replays and the wildcard replays (capi_wildcard.cu): per
 // model the block size, the shared memory and the four instantiations of replay_lane_kernel, fn[WILD][REC]
 namespace demi { struct ReplayArgs; }
@@ -184,11 +197,21 @@ inline int32_t demi_check_parents(demi_handle* h, const char* who, const uint16_
   return DEMI_OK;
 }
 
-inline int32_t ensure_bytes(demi_handle* h, void** p, size_t* cap, size_t need) {
-  if (*cap >= need) return DEMI_OK;
-  cudaFree(*p); *p = nullptr; *cap = 0;
-  CUDA_TRY(h, cudaMalloc(p, need));
-  *cap = need;
+// DEMI_TEST_ALLOC_LIMIT=n (tests): an allocation of more than n bytes fails as a full device would, without asking the
+// driver.  It is read only when a buffer is about to be allocated, so a test can set it around one call.
+inline int32_t DevBuf::grow(demi_handle* h, size_t bytes) {
+  if (bytes_ >= bytes) return DEMI_OK;
+  reset();
+  const char* limit = getenv("DEMI_TEST_ALLOC_LIMIT");
+  const cudaError_t e = limit && *limit && bytes > strtoull(limit, nullptr, 10) ? cudaErrorMemoryAllocation : cudaMalloc(&p_, bytes);
+  if (e != cudaSuccess) { p_ = nullptr; return fail(h, DEMI_ERR_CUDA, "cudaMalloc of %zu bytes: %s", bytes, cudaGetErrorString(e)); }
+  bytes_ = bytes;
+  return DEMI_OK;
+}
+inline int32_t DevBuf::upload(demi_handle* h, const void* src, size_t bytes) {
+  const int32_t rc = grow(h, bytes);
+  if (rc != DEMI_OK) return rc;
+  CUDA_TRY(h, cudaMemcpy(p_, src, bytes, cudaMemcpyHostToDevice));
   return DEMI_OK;
 }
 

@@ -81,8 +81,8 @@ class Engine(object):
     def set_externals(self, events):
         arr = events if isinstance(events, np.ndarray) else pack_externals(events)
         arr = np.ascontiguousarray(arr, dtype=N.EXT_DTYPE)
-        self._ext = arr
         self._check(N.lib().demi_set_externals(self._h, arr.ctypes.data, len(arr)))
+        self._ext = arr
 
     def fuzz_batch(self, seed_base, n, max_messages, interval, looking_for=0, out=None, flags=0):
         p = N.FuzzParams(seed_base, n, max_messages, interval, looking_for or 0, flags)
@@ -104,9 +104,9 @@ class Engine(object):
         post = postfix if isinstance(postfix, np.ndarray) else pack_externals(list(postfix))
         pre = np.ascontiguousarray(pre, dtype=N.EXT_DTYPE)
         post = np.ascontiguousarray(post, dtype=N.EXT_DTYPE)
-        self._fuzzer = (config, pre, post)
         self._check(N.lib().demi_set_fuzzer(self._h, C.byref(config), pre.ctypes.data if len(pre) else None, len(pre),
                                             post.ctypes.data if len(post) else None, len(post)))
+        self._fuzzer = (config, pre, post)
 
     def fuzzer_program(self, program_seed):
         """The program the campaign execution with this program seed runs (demi_fuzzer_generate on the host)."""
@@ -172,8 +172,8 @@ class Engine(object):
         ev = np.ascontiguousarray(events, dtype=N.EVENT_DTYPE)
         ext = externals if isinstance(externals, np.ndarray) else pack_externals(externals)
         ext = np.ascontiguousarray(ext, dtype=N.EXT_DTYPE)
-        self._trace, self._trace_ext = ev, ext
         self._check(N.lib().demi_set_trace(self._h, ev.ctypes.data, len(ev), ext.ctypes.data, len(ext)))
+        self._trace, self._trace_ext = ev, ext
 
     def mask_words(self):
         return max(1, (len(self._trace_ext) + 63) // 64)

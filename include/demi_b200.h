@@ -200,7 +200,8 @@ void    demi_destroy(demi_handle* h);
  * (TestOracle.scala:27) when the host's application is not one of the compiled models.  The blob is copied.
  * A loaded model may use timers in every entry point that takes one (fuzzing, replay, DDMin, internal and wildcard
  * minimization, frontier DPOR), within the limits of the compiled models: 16 repeating timers registered and 16
- * cancelled timers not yet dropped per execution, then DEMI_PS_QUEUE_OVF / DEMI_DS_QUEUE_OVF. */
+ * cancelled timers not yet dropped per execution, then DEMI_PS_QUEUE_OVF / DEMI_DS_QUEUE_OVF.  A call that fails, for
+ * any reason, leaves the handle as it was: the previously loaded model, if any, stays loaded. */
 int32_t demi_load_model(demi_handle* h, const void* model_blob, size_t size);
 /* The name table: the reference addresses actors by name (Scheduler.scala:13-104: blockedActors: Set[String], ...),
  * the C ABI by index.  Built-in models name their actors "0", "1", ...; a loaded model brings its own names. */
@@ -208,7 +209,8 @@ int32_t demi_actor_index(const demi_handle* h, const char* name);         /* -1 
 const char* demi_actor_name(const demi_handle* h, uint32_t index);        /* NULL if out of range */
 
 /* The external-event program == the `_trace: Seq[ExternalEvent]` argument of
- * RandomScheduler.explore (RandomScheduler.scala:234) / TestOracle.test. */
+ * RandomScheduler.explore (RandomScheduler.scala:234) / TestOracle.test.  A call that fails, for any reason (a
+ * device allocation included), leaves the handle as it was: the previous program stays set. */
 int32_t demi_set_externals(demi_handle* h, const demi_ext_event* ev, uint32_t n);
 
 /* FullyRandom(userDefinedFilter = ...) (RandomScheduler.scala:633-684): "userDefinedFilter can throw out entries to
@@ -261,7 +263,8 @@ typedef struct demi_replay_result {
 
 /* The recorded execution to minimise: STSScheduler.original_trace
  * (STSScheduler.scala:85) and EventTrace.original_externals (EventTrace.scala:20).
- * Usually the output of demi_fuzz_trace for a violating seed. */
+ * Usually the output of demi_fuzz_trace for a violating seed.  A call that fails, for any reason (a device allocation
+ * included), leaves the handle as it was: the previous trace and its conjoined atoms stay set. */
 int32_t demi_set_trace(demi_handle* h, const demi_event* events, uint32_t n_events,
                        const demi_ext_event* externals, uint32_t n_externals);
 /* n_masks independent STSScheduler.test(subseq, fingerprint) calls.  Mask i is
@@ -673,7 +676,9 @@ int32_t demi_fuzzer_generate(const demi_fuzzer_config* cfg, int64_t seed,
  * Start (the Fuzzer's actors are the prefix's Starts, :60) or with more than DEMI_MAX_ACTORS Start events (a restart
  * after Kill or HardKill counts too: the generator's sets hold one entry per Start), consecutive
  * WaitQuiescence in the prefix or postfix, a postfix that begins with WaitQuiescence, a send_type the model does not
- * define, weights that are negative, not finite or add up to 0, and num_events above DEMI_FUZZER_MAX_EVENTS. */
+ * define, weights that are negative, not finite or add up to 0, and num_events above DEMI_FUZZER_MAX_EVENTS.  A call
+ * that fails, for any reason (a device allocation included), leaves the handle as it was: the previous Fuzzer, if any,
+ * stays set. */
 #define DEMI_FUZZER_MAX_EVENTS 4096
 int32_t demi_set_fuzzer(demi_handle* h, const demi_fuzzer_config* cfg, const demi_ext_event* prefix, uint32_t n_prefix,
                         const demi_ext_event* postfix, uint32_t n_postfix);
