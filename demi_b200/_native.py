@@ -112,7 +112,7 @@ PV_OK, PV_CYCLE, PV_OVERFLOW, PV_PREFIX_FAILED = 0, 1, 2, 3
 EXPORTS = [
     "demi_version", "demi_last_error", "demi_device_count", "demi_create", "demi_destroy",
     "demi_set_externals", "demi_fuzz_batch", "demi_fuzz_batch_dev", "demi_fuzz_summary_dev",
-    "demi_fuzz_trace", "demi_stats",
+    "demi_fuzz_trace", "demi_stats", "demi_lane_kernel",
     "demi_set_trace", "demi_replay_batch", "demi_replay_batch_dev", "demi_ddmin", "demi_dpor_batch",
     "demi_dedup_compact_dev", "demi_dedup_compact",
     "demi_replay_batch_ex", "demi_replay_trace", "demi_internal_minimize",
@@ -127,6 +127,7 @@ EXPORTS = [
 FILTER_RULE_DTYPE = np.dtype([("src_mask", "<u4"), ("dst_mask", "<u4"), ("type_mask", "<u4"), ("flags", "<u4")])
 FRULE_DEADLETTERS = 1
 MODEL_IR = 100
+LANE_NONE, LANE_GENERIC, LANE_STEADY = 0, 1, 2
 
 
 class FuzzerConfig(C.Structure):
@@ -311,5 +312,7 @@ def lib():
                                          C.POINTER(C.c_uint32), vp]
     L.demi_stats.restype = C.c_int32
     L.demi_stats.argtypes = [vp, C.POINTER(Perf)]
+    L.demi_lane_kernel.restype = C.c_int32
+    L.demi_lane_kernel.argtypes = [vp]
     _lib = L
     return L

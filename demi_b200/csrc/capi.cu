@@ -70,13 +70,34 @@ static const Variant* pick_variant(int model, LaunchMode mode, uint32_t pcap, ui
 }
 
 // lane-engine table
-struct LaneVariant { int model; int bd; uint32_t lpcap; size_t smem_per_block; kernel_fn fn[LM_COUNT]; };
+// `steady`: the LM_BATCH instantiation that starts from the program's snapshot (`snapshot` takes it); `ops` is the
+// model's operations per receive(), which the node-capacity proof of lane_steady_eligible counts with.
+typedef void (*snapshot_fn)(const KernelArgs, LaneSnapshot*);
+struct LaneVariant {
+  int model; int bd; uint32_t lpcap; size_t smem_per_block; kernel_fn fn[LM_COUNT];
+  kernel_fn steady; size_t steady_smem; snapshot_fn snapshot; uint32_t ops;
+};
 template <class MODEL, int BD, int LPCAP>
 static LaneVariant make_lane_variant() {
   using M = LaneMachine<MODEL, BD, LPCAP>;
+  using S = LaneMachine<MODEL, BD, LPCAP, false, true>;
   return LaneVariant{MODEL::ID, BD, (uint32_t)LPCAP, (size_t)M::WORDS * BD * sizeof(uint32_t),
                      {fuzz_lane_kernel<MODEL, BD, LPCAP>, fuzz_lane_kernel<MODEL, BD, LPCAP, true>,
-                      fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>, fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true>}};
+                      fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>, fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true>},
+                     fuzz_lane_kernel<MODEL, BD, LPCAP, false, false, false, true>, (size_t)S::WORDS * BD * sizeof(uint32_t),
+                     lane_snapshot_kernel<MODEL>, (uint32_t)MODEL::LANE_OUTBOX};
+}
+#ifndef DEMI_K1_BD_RAFT5
+#define DEMI_K1_BD_RAFT5 256
+#endif
+static const LaneVariant* lane_variant_of(int model) {
+  static const std::vector<LaneVariant> v = {
+    make_lane_variant<Raft5, DEMI_K1_BD_RAFT5, DEMI_K1_LPCAP_RAFT5>(),
+    make_lane_variant<PingPong3, 256, 128>(),
+    make_lane_variant<Bcast32, 128, 8192>(),
+  };
+  for (const LaneVariant& lv : v) if (lv.model == model) return &lv;
+  return nullptr;
 }
 
 // ---------------------------------------------------------------- lifecycle
@@ -245,14 +266,37 @@ extern "C" int32_t demi_set_externals(demi_handle* h, const demi_ext_event* ev, 
     describe_event(&info, &sv, ev[i]);
   }
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  DevBuf ext_dev, sends_dev;
+  DevBuf ext_dev, sends_dev, snap_dev;
+  LaneSnapshot snap{};
+  snap.status = LANE_DEFER;                // no lane engine for the model: no snapshot
   int32_t rc;
   if (n && (rc = ext_dev.upload(h, ev, n * sizeof(demi_ext_event))) != DEMI_OK) return rc;
   if (!sv.empty() && (rc = sends_dev.upload(h, sv.data(), sv.size() * sizeof(uint4))) != DEMI_OK) return rc;
+  if (const LaneVariant* lv = lane_variant_of(h->cfg.model)) {
+    // The program's pre-delivery snapshot, under the physical limits: a batch compares its counts with its own
+    // capacities (launch_plan).  It depends on the program and the model alone (no actor has received anything, and
+    // the snapshot holds no actor state, so neither model_flags nor ignoreTimers shows in it), hence it is taken here
+    // and not per batch.
+    if ((rc = snap_dev.grow(h, sizeof(LaneSnapshot))) != DEMI_OK) return rc;
+    KernelArgs a{};
+    a.ext = ext_dev.get<demi_ext_event>(); a.n_ext = n;
+    a.ext_sends = sends_dev.get<uint4>();
+    a.has_partitions = info.partitions ? 1u : 0u;
+    a.model_flags = h->cfg.model_flags;
+    a.max_messages = INT_MAX;
+    a.node_cap = 65535u; a.pending_cap = 0xFFFFu; a.tosend_cap = 0xFFFFu;
+    CUDA_TRY(h, cudaMemsetAsync(snap_dev.get(), 0, sizeof(LaneSnapshot), h->stream));
+    lv->snapshot<<<1, 1, 0, h->stream>>>(a, snap_dev.get<LaneSnapshot>());
+    CUDA_TRY(h, cudaGetLastError());
+    CUDA_TRY(h, cudaMemcpyAsync(&snap, snap_dev.get(), sizeof(LaneSnapshot), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
   h->ext_host.assign(ev, ev + n);
   h->ext_info = info;
   h->ext_dev = std::move(ext_dev);
   h->ext_sends_dev = std::move(sends_dev);
+  h->lane_snap_dev = std::move(snap_dev);
+  h->lane_snap = snap;
   return DEMI_OK;
 }
 
@@ -266,18 +310,9 @@ extern "C" int32_t demi_set_user_filter(demi_handle* h, const demi_filter_rule* 
 // The lane engine for a launch over a program `prog` describes (for a campaign, the Fuzzer's; a random-oracle test
 // decides on the base program, and each of its subsequences meets every condition the base program meets)
 static const LaneVariant* pick_lane_variant(const demi_handle* h, const ProgramInfo& prog) {
-  static const std::vector<LaneVariant> v = {
-#ifndef DEMI_K1_BD_RAFT5
-#define DEMI_K1_BD_RAFT5 256
-#endif
-    make_lane_variant<Raft5, DEMI_K1_BD_RAFT5, DEMI_K1_LPCAP_RAFT5>(),
-    make_lane_variant<PingPong3, 256, 128>(),
-    make_lane_variant<Bcast32, 128, 8192>(),
-  };
   if (!h->use_lane_engine || h->cfg.blocked_mask || !prog.sends_distinct || h->cfg.strategy != DEMI_RS_FULLY_RANDOM ||
       prog.hard_kill || !h->filter.empty()) return nullptr;          // actor termination and user filters: the general engine
-  for (const LaneVariant& lv : v) if (lv.model == h->cfg.model) return &lv;
-  return nullptr;
+  return lane_variant_of(h->cfg.model);
 }
 
 // ------------------------------------------------------------------- launch
@@ -350,9 +385,22 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, LaunchMode
 // (on every item otherwise).  Counts both launches.
 static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, cudaStream_t s) {
   KernelArgs& a = plan.args;
+  h->lane_kernel = DEMI_LANE_NONE;
   if (const LaneVariant* lv = pick_lane_variant(h, *plan.prog)) {
-    const kernel_fn lfn = lv->fn[plan.mode];
-    const size_t lsmem = lv->smem_per_block;
+    const uint32_t lane_pcap = std::min(h->lane_pending_cap ? std::min(a.pending_cap, h->lane_pending_cap) : a.pending_cap, lv->lpcap);
+    // A batch over the handle's program starts every execution from the program's snapshot when the rule of
+    // lane_steady.hpp allows it; every other launch runs the generic instantiation.
+    bool steady = false;
+    if (plan.mode == LM_BATCH && plan.prog == &h->ext_info) {
+      LaneSteadyLaunch l{};
+      l.n_ext = a.n_ext; l.partitions = plan.prog->partitions; l.ignore_timers = a.ignore_timers != 0;
+      l.looking_for = a.looking_for; l.max_messages = a.max_messages;
+      l.pending_cap = lane_pcap; l.node_cap = a.node_cap; l.tosend_cap = a.tosend_cap;
+      l.lane_tosend_cap = LANE_TOSEND_CAP; l.ops_per_delivery = lv->ops;
+      steady = lane_steady_eligible(h->lane_snap, l);
+    }
+    const kernel_fn lfn = steady ? lv->steady : lv->fn[plan.mode];
+    const size_t lsmem = steady ? lv->steady_smem : lv->smem_per_block;
     int32_t rc;
     int bps = 0;
     if ((rc = demi_occupancy(h, (const void*)lfn, lv->bd, lsmem, &bps)) != DEMI_OK) return rc;
@@ -370,8 +418,10 @@ static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, c
     la.prog_lane_pcap = h->lane_pending_cap;
     la.ovf_list = h->ovf_list.get<uint32_t>(); la.ovf_count = h->ovf_count.get<uint32_t>();
     if (h->lane_pending_cap) la.pending_cap = std::min(la.pending_cap, h->lane_pending_cap);     // deferring is always exact
+    if (steady) { la.pending_cap = lane_pcap; la.lane_snap = h->lane_snap_dev.get<LaneSnapshot>(); }   // one bound, rows included
     lfn<<<lgrid, lv->bd, lsmem, s>>>(la);
     CUDA_TRY(h, cudaGetLastError());
+    h->lane_kernel = steady ? DEMI_LANE_STEADY : DEMI_LANE_GENERIC;
     h->perf.kernel_launches++;
     // what the lane engine could not prove exact: a recording launch numbers its outputs by work-list position
     if (plan.mode == LM_RECORD) { a.pos_list = la.ovf_list; a.pos_count = la.ovf_count; }
@@ -1154,6 +1204,8 @@ extern "C" int32_t demi_random_ddmin(demi_handle* h, const demi_fuzz_params* p, 
   }
   return DEMI_OK;
 }
+
+extern "C" int32_t demi_lane_kernel(const demi_handle* h) { return h ? h->lane_kernel : DEMI_ERR_INVALID; }
 
 extern "C" int32_t demi_stats(const demi_handle* h, demi_perf* out) {
   if (!h || !out) return DEMI_ERR_INVALID;

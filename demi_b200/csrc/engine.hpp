@@ -13,6 +13,7 @@
 #include "../../include/demi_b200.h"
 #include "../../include/demi_limits.h"
 #include "../../include/demi_model_ir.h"
+#include "lane_steady.hpp"
 
 extern thread_local std::string g_create_error;
 
@@ -65,6 +66,9 @@ struct demi_handle {
   DevBuf fifo_scratch;                             // uint16_t
   int use_lane_engine = 1;
   uint32_t lane_pending_cap = 0;      // DEMI_LANE_PENDING_CAP (tests): the lane engine defers beyond this many pending messages
+  DevBuf lane_snap_dev;                            // demi::LaneSnapshot of ext_host (demi_set_externals takes it)
+  demi::LaneSnapshot lane_snap{};                  // its host copy: what launch_plan decides on
+  int32_t lane_kernel = DEMI_LANE_NONE;            // the lane instantiation the last fuzz launch ran (demi_lane_kernel)
   DevBuf rec_counts_dev;                           // uint32_t
   DevBuf prov_scratch;
   DevBuf dpor_buf[24];                             // K3 per-search structures (capi_dpor.cu)

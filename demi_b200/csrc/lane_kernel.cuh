@@ -25,6 +25,7 @@
 #pragma once
 #include "machine.cuh"
 #include "models/models.cuh"
+#include "lane_steady.hpp"
 
 namespace demi {
 
@@ -223,8 +224,14 @@ __device__ __forceinline__ void receive_phase(LaneDirectOutbox<M>& o, uint32_t r
 }
 
 // REC: the execution's EventTrace and DepTracker parents are written out (provenance batches, demi_fuzz_provenance)
-template <class MODEL, int BD, int LPCAP, bool REC = false>
+// STEADY: every execution starts from the launch's pre-delivery snapshot (lane_steady.hpp) and nothing external
+// happens after it.  The host has checked lane_steady_eligible, so this instantiation carries no code for externals,
+// partitions, isolated or killed actors, ignoreTimers, a violation filter or the node capacity, and tests the
+// pending array against one bound (A->pending_cap, which the host has clamped to LPCAP).  Every rule is the generic
+// one with those cases compiled out.
+template <class MODEL, int BD, int LPCAP, bool REC = false, bool STEADY = false>
 struct LaneMachine {
+  static_assert(!(STEADY && REC), "recording launches run the generic instantiation");
   static constexpr int N = MODEL::N_ACTORS;
   static constexpr int SW = MODEL::STATE_WORDS;
   static constexpr int OB = MODEL::LANE_OUTBOX;
@@ -234,7 +241,8 @@ struct LaneMachine {
   static constexpr uint32_t CT = MODEL::LANE_CANCEL_TYPE;            // 0: receive() cancels no timer
   static constexpr int TW = CT ? (N + 1) / 2 : 0;
   static_assert(CT == 0 || LPCAP < 0xFF, "tcopy keeps a pending index in one byte, 0xFF meaning unknown");
-  static constexpr int WORDS = N * SW + OBW + N + TW;      // states + outbox + partition rows + cancellable timer copies
+  static constexpr int PW = STEADY ? 0 : N;               // partition rows: none when the program has no partition
+  static constexpr int WORDS = N * SW + OBW + PW + TW;     // states + outbox + partition rows + cancellable timer copies
 
   uint32_t* smw;             // &smem[tid]; word w at smw[w*BD]
   uint4* pend;               // entry i at pend[i]
@@ -269,7 +277,7 @@ struct LaneMachine {
   // (0xFF otherwise: after 2 -> 1 it is not).  Only timer_produced inserts timer messages (an external with a timer's
   // key defers) and every removal goes through pending_remove_at, so these are exact.  Other timers are not tracked:
   // the check on each removal is one compare of the header's flags and type.
-  __device__ __forceinline__ uint32_t& tcopy_word(uint32_t a) { return smw[(N * SW + OBW + N + (a >> 1)) * BD]; }
+  __device__ __forceinline__ uint32_t& tcopy_word(uint32_t a) { return smw[(N * SW + OBW + PW + (a >> 1)) * BD]; }
   __device__ __forceinline__ uint32_t tcopy(uint32_t a) { return (tcopy_word(a) >> ((a & 1u) * 16)) & 0xFFFFu; }
   __device__ __forceinline__ void tcopy_set(uint32_t a, uint32_t e) {
     uint32_t& w = tcopy_word(a);
@@ -303,7 +311,10 @@ struct LaneMachine {
 
   // RandomizedHashSet.insert (schedulers/Util.scala:126-136).  max_pending is brought up to date before each removal
   // and at the end of the execution, the only points where the set can be at a maximum.
-  __device__ __forceinline__ bool pending_full(uint32_t k) const { return n_pending + k > A->pending_cap || n_pending + k > LPCAP; }
+  __device__ __forceinline__ bool pending_full(uint32_t k) const {
+    if constexpr (STEADY) return n_pending + k > A->pending_cap;
+    return n_pending + k > A->pending_cap || n_pending + k > LPCAP;
+  }
   __device__ __forceinline__ void pending_push(uint4 e) {          // the caller has checked pending_full
     st_l2_hint(pend + n_pending, e, pol);
     n_pending++;
@@ -335,7 +346,10 @@ struct LaneMachine {
   }
 
   // EventOrchestrator.crosses_partition (EventOrchestrator.scala:345-351)
-  __device__ __forceinline__ bool network_open() { return !(inaccessible | killed) && !A->has_partitions; }   // everyone started, no one isolated
+  __device__ __forceinline__ bool network_open() {           // everyone started, no one isolated
+    if constexpr (STEADY) return true;
+    return !(inaccessible | killed) && !A->has_partitions;
+  }
   __device__ __forceinline__ bool crosses_partition(uint32_t snd, uint32_t rcv) {
     return !network_open() && crosses_partition_closed(snd, rcv);
   }
@@ -364,7 +378,7 @@ struct LaneMachine {
   // exact: the general engine re-runs the prefix).  Only REC's trace capacity is still checked per event.
   __device__ __forceinline__ bool reserve_sends(uint32_t self, uint32_t k) {
     if (status) return false;
-    if (n_nodes + k > A->node_cap || pending_full(k)) { defer(); return false; }
+    if ((!STEADY && n_nodes + k > A->node_cap) || pending_full(k)) { defer(); return false; }
     sends_open = network_open();
     // demi_event_term of the first send, dst / type / payload terms left out: word 0 = kind | self << 8, word 3 =
     // node | node << 16 (node <= 0xFFFE, as n_nodes + k <= node_cap <= 0xFFFF), sequence n_events
@@ -378,7 +392,7 @@ struct LaneMachine {
       if (slot >= 0 && ((cancelled >> slot) & 1u)) { cancelled &= ~(1u << slot); return; }
     }
     const uint32_t w3 = n_nodes++ * 0x10001u;
-    if (sends_open || !crosses_partition_closed(self, dst)) pending_push(make_uint4(make_hdr(self, dst, type, 0), p0, p1, w3));
+    if (STEADY || sends_open || !crosses_partition_closed(self, dst)) pending_push(make_uint4(make_hdr(self, dst, type, 0), p0, p1, w3));
     // the hash term of this send: word 0 adds dst << 16 | type << 24 to the reserved kind | self << 8, and the next
     // send's word 3 and sequence number are one node (0x10001) and one event further on
     const uint32_t w0_tail = (dst << 16) | (type << 24);
@@ -391,9 +405,10 @@ struct LaneMachine {
   __device__ __forceinline__ void timer_produced(uint32_t slot) {
     const uint32_t bit = 1u << slot;
     if (cancelled & bit) { cancelled &= ~bit; return; }
-    if (n_nodes >= A->node_cap) { defer(); return; }
-    // two equal timer sends under one parent would share a Unique: defer those
-    if (parent_event == 0) { if (root_timers & bit) { defer(); return; } root_timers |= bit; }
+    if (!STEADY && n_nodes >= A->node_cap) { defer(); return; }
+    // two equal timer sends under one parent would share a Unique: defer those.  (STEADY: a timer is flushed only
+    // after a delivery, whose node is the parent.)
+    if (!STEADY && parent_event == 0) { if (root_timers & bit) { defer(); return; } root_timers |= bit; }
     else { if (window_timers & bit) { defer(); return; } window_timers |= bit; }
     const uint32_t w3 = n_nodes++ * 0x10001u;
     uint32_t dst, type, p0, p1;
@@ -444,8 +459,8 @@ struct LaneMachine {
       registry |= 1u << s2;
     }
     if ((just >> s2) & 1u) { resend_push((uint32_t)s2); return; }
-    if (A->ignore_timers) return;
-    if (tosend.n >= LANE_TOSEND_CAP || tosend.n >= A->tosend_cap) { defer(); return; }
+    if (!STEADY && A->ignore_timers) return;
+    if (tosend.n >= LANE_TOSEND_CAP || (!STEADY && tosend.n >= A->tosend_cap)) { defer(); return; }
     tosend.push((uint32_t)s2);
   }
   // First the ops receive() left in the outbox (`n_ops`, sender `self`), in program order; then, if `do_flush`,
@@ -469,7 +484,7 @@ struct LaneMachine {
 #pragma unroll 1
     while (tosend.n != 0 && !status) {
       const uint32_t b = tosend.pop();
-      if (b & 0x80u) {
+      if (!STEADY && (b & 0x80u)) {
         const uint4 raw = __ldg(reinterpret_cast<const uint4*>(A->ext_sends) + (b & 0x7Fu));
         external_produced(raw.x, raw.y, raw.z);
       } else {
@@ -514,7 +529,7 @@ struct LaneMachine {
 
   __device__ __forceinline__ uint32_t check_invariant() {
     uint32_t v = MODEL::invariant(LaneAll<SW>{smw, BD}, A->model_flags);
-    if (!A->looking_for) return v;                    // violationMatches (RandomScheduler.scala:138-154)
+    if (STEADY || !A->looking_for) return v;                    // violationMatches (RandomScheduler.scala:138-154)
     return (v && v == A->looking_for) ? A->looking_for : 0u;
   }
 
@@ -564,7 +579,7 @@ struct LaneMachine {
   // delivery's outbox is drained (drain() then flushes only if we go on)
   __device__ __forceinline__ bool may_continue() {
     if (status | violation) return false;
-    if (nsched > A->max_messages) { ext_idx = A->n_ext; return false; }
+    if (nsched > A->max_messages) { if (!STEADY) ext_idx = A->n_ext; return false; }
     if (A->interval > 0 && nmod == 0 && nsched != 0) {
       violation = check_invariant();
       if (violation) return false;
@@ -593,7 +608,7 @@ struct LaneMachine {
       // handle_timer of each re-send entry, in order.  messagesToSend is empty here: run() flushed it to the end just
       // before this pick (a flush that defers ends the execution), so the list becomes the whole queue, and its at most
       // LANE_RESEND_CAP entries always fit.
-      if (!A->ignore_timers) tosend.assign((uint32_t)resend, (uint32_t)(resend >> 32), n_resend);
+      if (STEADY || !A->ignore_timers) tosend.assign((uint32_t)resend, (uint32_t)(resend >> 32), n_resend);
       resend = 0; n_resend = 0;
       just = 0;
     }
@@ -639,9 +654,10 @@ struct LaneMachine {
     rng.seed(seed);
 #pragma unroll 1
     for (uint32_t i = 0; i < N * SW; i++) smw[i * BD] = MODEL::init_word(i, A->model_flags);
-    for (uint32_t a = 0; a < N; a++) part_row(a) = 0;
+    if constexpr (!STEADY)
+      for (uint32_t a = 0; a < N; a++) part_row(a) = 0;
     if constexpr (TW > 0)
-      for (uint32_t w = 0; w < (uint32_t)TW; w++) smw[(N * SW + OBW + N + w) * BD] = 0;
+      for (uint32_t w = 0; w < (uint32_t)TW; w++) smw[(N * SW + OBW + PW + w) * BD] = 0;
     n_pending = max_pending = 0;
     tosend.clear(); resend = 0; n_resend = 0;
     just = registry = cancelled = root_timers = window_timers = 0;
@@ -652,12 +668,31 @@ struct LaneMachine {
     killed = 0; thash = 0;
   }
 
-  __device__ __forceinline__ void run(int64_t seed, demi_fuzz_result& out) {
-    clk.enter(LP_TAIL);
-    reset(seed);
+  // An execution up to its first pick: the externals up to the first WaitQuiescence and the flush of their Sends.
+  // It draws no random number, so it is the same for every seed; lane_snapshot_kernel runs it once per program.
+  __device__ __forceinline__ void first_flush() {
+    inject_until_quiescence();
+    const bool go = may_continue();
+    drain(0, 0, go);
+  }
+  // STEADY: the machine reset() left becomes the one first_flush() would have left.  Nothing has been delivered, so
+  // the actor states and every timer structure are as reset() set them; tosend is empty after a flush.
+  __device__ __forceinline__ void restore() {
+    const LaneSnapshot* s = A->lane_snap;
+    const uint4* sp = reinterpret_cast<const uint4*>(s->pend);
+    n_pending = __ldg(&s->n_pending);
+#pragma unroll 1
+    for (uint32_t i = 0; i < n_pending; i++) st_l2_hint(pend + i, __ldg(sp + i), pol);
+    n_nodes = __ldg(&s->n_nodes); n_events = __ldg(&s->n_events);
+    thash = __ldg(reinterpret_cast<const unsigned long long*>(&s->thash));
+  }
+
+  // The deliveries of an execution, segment by segment.  STEADY has one segment and starts it at the top of the
+  // delivery loop: with nothing scheduled and tosend empty, may_continue() and drain() do nothing before the first pick.
+  __device__ __forceinline__ void deliver() {
     uint32_t n_ops = 0, self = 0;          // outbox of the delivery that has not been drained yet
     for (;;) {
-      inject_until_quiescence();
+      if constexpr (!STEADY) inject_until_quiescence();
       for (;;) {
         clk.enter(LP_INVARIANT);
         const bool go = may_continue();
@@ -673,6 +708,7 @@ struct LaneMachine {
         if (status) break;
       }
       clk.enter(LP_TAIL);
+      if constexpr (STEADY) break;
       if (status | violation) break;
       if (ext_idx < A->n_ext) {
         record_event(DEMI_EV_QUIESCENCE, DEMI_DEADLETTERS, DEMI_DEADLETTERS, 0, 0, 0, 0, 0);
@@ -680,6 +716,9 @@ struct LaneMachine {
       }
       break;
     }
+  }
+  // The final invariant check and the result record.
+  __device__ __forceinline__ void finish(demi_fuzz_result& out) {
     if (!status && nsched <= A->max_messages && !violation) violation = check_invariant();
     if (n_pending > max_pending) max_pending = n_pending;
     out.status = (uint16_t)status;
@@ -700,7 +739,38 @@ struct LaneMachine {
       out.max_pending = (uint16_t)max_pending;
     }
   }
+
+  __device__ __forceinline__ void run(int64_t seed, demi_fuzz_result& out) {
+    clk.enter(LP_TAIL);
+    reset(seed);
+    if constexpr (STEADY) restore();
+    deliver();
+    finish(out);
+  }
 };
+
+// The pre-delivery snapshot of the launch's program (lane_steady.hpp): one thread runs reset() and first_flush() of
+// the generic machine with the physical limits in place of a batch's capacities (a batch compares the recorded
+// counts with its own), LANE_SNAP_CAP pending rows (a program that enables more defers, and is not snapshotted),
+// and stores the machine.  Launched when the program is set, not per batch.
+template <class MODEL>
+__global__ void lane_snapshot_kernel(const __grid_constant__ KernelArgs args, LaneSnapshot* out) {
+  using M = LaneMachine<MODEL, 1, (int)LANE_SNAP_CAP>;
+  __shared__ uint32_t smem[M::WORDS];
+  M m;
+  m.smw = smem;
+  m.pend = reinterpret_cast<uint4*>(out->pend);
+  m.A = &args;
+  m.pol = l2_evict_last_policy();
+  m.rec_ev = nullptr; m.rec_par = nullptr;
+  m.reset(0);
+  m.first_flush();
+  out->thash = m.thash;
+  out->n_pending = m.n_pending; out->n_nodes = m.n_nodes; out->n_events = m.n_events; out->parent_event = m.parent_event;
+  out->root_timers = m.root_timers; out->registry = m.registry; out->cancelled = m.cancelled; out->tosend_n = m.tosend.n;
+  out->ext_idx = m.ext_idx; out->ext_send_idx = m.ext_send_idx; out->inaccessible = m.inaccessible; out->killed = m.killed;
+  out->status = m.status;
+}
 
 #ifndef DEMI_K1_MIN_BLOCKS
 #define DEMI_K1_MIN_BLOCKS 3
@@ -710,12 +780,13 @@ struct LaneMachine {
 // PROG (campaigns; with TESTS random-oracle tests, see fuzz_kernel): prefix idx runs its program of the arena in `args.prog_*`; the 0x80 | k entries
 // of messagesToSend resolve through that program's Send table.  A deferred prefix keeps its index, so the PROG
 // instantiation of the warp engine re-runs it on the same program.
-template <class MODEL, int BD, int LPCAP, bool REC = false, bool PROG = false, bool TESTS = false>
+template <class MODEL, int BD, int LPCAP, bool REC = false, bool PROG = false, bool TESTS = false, bool STEADY = false>
 __global__ void __launch_bounds__(BD, DEMI_K1_MIN_BLOCKS)
 fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
   static_assert(!(PROG && REC), "a campaign execution is recorded through demi_fuzz_trace on its program");
   static_assert(PROG || !TESTS, "random-oracle tests bind their programs as campaigns do");
-  using M = LaneMachine<MODEL, BD, LPCAP, REC>;
+  static_assert(!STEADY || !(REC || PROG), "a steady launch runs one fixed program, unrecorded");
+  using M = LaneMachine<MODEL, BD, LPCAP, REC, STEADY>;
   extern __shared__ __align__(16) uint32_t lane_smem[];
   const uint32_t tid = threadIdx.x;
   const uint64_t gthread = (uint64_t)blockIdx.x * BD + tid;

@@ -120,6 +120,7 @@ struct JRandom {
   }
 };
 
+struct LaneSnapshot;
 struct KernelArgs {
   // configuration
   uint32_t model_flags;
@@ -161,7 +162,12 @@ struct KernelArgs {
   unsigned long long* sum_steps; unsigned long long* n_violations;
   // lane engine (lane_kernel.cuh)
   uint4*    lane_pend;        // [total_warps][LPCAP][32] pending entries
-  const uint4* ext_sends;     // the program's Send events as {hdr|EXTERNAL, p0, p1, 0}, in order
+  union {
+    const uint4* ext_sends;   // the program's Send events as {hdr|EXTERNAL, p0, p1, 0}, in order
+    // STEADY launches inject nothing and have no Send table: they read the program's pre-delivery snapshot
+    // (lane_steady.hpp) through the same slot, so that the struct, and with it every other kernel, stays as it was
+    const LaneSnapshot* lane_snap;
+  };
   uint32_t  has_partitions;   // program contains Partition/UnPartition events
   // FullyRandom's userDefinedFilter as rules (demi_set_user_filter): {src_mask, dst_mask, type_mask, flags}
   uint4     filter[DEMI_MAX_FILTER_RULES]; uint32_t n_filter;

@@ -442,6 +442,10 @@ class Engine(object):
         r = res[0]
         return r, viol[:min(int(r["violations"]), cap_viol)].copy(), hashes[:min(int(r["interleavings"]), cap_h)].copy()
 
+    def lane_kernel(self):
+        """Which lane-engine instantiation the last fuzz launch ran: N.LANE_NONE, LANE_GENERIC or LANE_STEADY."""
+        return N.lib().demi_lane_kernel(self._h)
+
     def stats(self):
         s = N.Perf()
         self._check(N.lib().demi_stats(self._h, C.byref(s)))

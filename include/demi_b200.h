@@ -707,6 +707,13 @@ int32_t demi_experiment_load(const char* dir, demi_experiment* e);
 
 /* ------------------------------------------------------------- statistics */
 int32_t demi_stats(const demi_handle* h, demi_perf* out);
+/* Which instantiation of the lane engine the handle's last fuzz launch ran (batch, campaign, random test or
+ * provenance): none (the warp engine ran every execution), the generic one, or the steady one, which starts every
+ * execution from the program's pre-delivery snapshot.  The records are the same whichever ran. */
+#define DEMI_LANE_NONE    0
+#define DEMI_LANE_GENERIC 1
+#define DEMI_LANE_STEADY  2
+int32_t demi_lane_kernel(const demi_handle* h);
 
 #ifdef __cplusplus
 }

@@ -162,6 +162,7 @@ class Engine {
   // UnmodifiedEventDag.conjoinAtoms (minification/Util.scala:167-178): DDMin treats the two externals as one atom
   void conjoin_atoms(uint32_t i1, uint32_t i2) { check(demi_conjoin_atoms(h, i1, i2)); }      // indices into the trace's externals
   demi_perf stats() const { demi_perf p{}; demi_stats(h, &p); return p; }
+  int32_t lane_kernel() const { return demi_lane_kernel(h); }      // DEMI_LANE_*: what the last fuzz launch ran
   // ---- campaigns: a new Fuzzer program per execution (RunnerUtils.fuzz's loop, RunnerUtils.scala:75-91)
   // demi_set_fuzzer: new Fuzzer(num_events, weights, message_gen, prefix, postfix) (Fuzzer.scala:61-82)
   void set_fuzzer(const demi_fuzzer_config& c, const ExternalEvents& prefix, const ExternalEvents& postfix = {}) {
