@@ -148,6 +148,8 @@ struct FrState {
   unsigned long long pool_top = 0, pool_live = 0, n_exec = 0;
   uint32_t n_slots = 0;
   unsigned long long cap_exec = 0;
+  unsigned long long explored_sel = 0;            // explored pairs after the last getNext (history on)
+  bool round_failed = false;                      // a round ended in a capacity status: R.explored_pairs is final
   demi_frontier_result R{};
   FrArgs A{};
 
@@ -166,7 +168,8 @@ struct FrGeom { int model, world; demi_frontier_params F; uint32_t n_sends, ext_
 bool fr_same_geom(const FrGeom& a, const FrGeom& b, uint32_t n_ext) {
   return a.model == b.model && a.world == b.world && a.F.max_messages == b.F.max_messages && a.F.width == b.F.width &&
          a.F.max_interleavings == b.F.max_interleavings && a.F.explored_slots == b.F.explored_slots && a.F.pool_cap == b.F.pool_cap &&
-         a.F.trace_cap == b.F.trace_cap && a.F.steal_max == b.F.steal_max && a.n_sends == b.n_sends && n_ext <= a.ext_cap;
+         a.F.trace_cap == b.F.trace_cap && a.F.steal_max == b.F.steal_max && a.F.flags == b.F.flags &&   // flags: the explored-key log
+         a.n_sends == b.n_sends && n_ext <= a.ext_cap;
 }
 
 int32_t fr_setup(FrState& st, const demi_ext_event* ext, uint32_t n_ext, bool reuse) {
@@ -210,6 +213,7 @@ int32_t fr_setup(FrState& st, const demi_ext_event* ext, uint32_t n_ext, bool re
   for (auto& e : st.ev) CUDA_TRY(h, cudaEventCreate(&e));
   }
   st.runs.clear(); st.pool_top = st.pool_live = st.n_exec = 0; st.n_slots = 0;
+  st.explored_sel = 0; st.round_failed = false;
   memset(&st.R, 0, sizeof(st.R));
   if (!(F.flags & DEMI_FR_NO_HISTORY)) CUDA_TRY(h, cudaMemsetAsync(st.E, 0, F.explored_slots * 8, st.s));
   CUDA_TRY(h, cudaMemsetAsync(st.ctr, 0, FRC_N * 8, st.s));
@@ -271,6 +275,7 @@ int32_t fr_select_window(FrState& st, const std::vector<FrSeg>& segs, uint32_t w
   CUDA_TRY(h, cudaGetLastError());
   FrInfo info;
   CUDA_TRY(h, cudaMemcpyAsync(&info, st.info, sizeof(info), cudaMemcpyDeviceToHost, st.s));
+  if (!S.no_history) CUDA_TRY(h, cudaMemcpyAsync(&st.explored_sel, st.ctr + FRC_EXPLORED, 8, cudaMemcpyDeviceToHost, st.s));
   CUDA_TRY(h, cudaStreamSynchronize(st.s));
   *taken = info.taken; *cut = info.cut;
   h->perf.kernel_launches += 4;
@@ -355,10 +360,19 @@ int32_t fr_select_tail(FrState& st, unsigned long long m, uint32_t* n_out) {
   return DEMI_OK;
 }
 
+// a round that ends in a capacity status adds nothing to the executed work (st.R still holds the last completed
+// round's counters); keys_dropped and pool_left already are the failed round's getNext, explored_pairs becomes it
+int32_t fr_round_fail(FrState& st, uint32_t status) {
+  st.R.status = status;
+  st.R.explored_pairs = st.explored_sel;
+  st.round_failed = true;
+  return DEMI_OK;
+}
+
 // execute st.A.n_sel points (or the root), scan the new traces, enqueue their backtrack points as a new run
 int32_t fr_execute_and_scan(FrState& st, uint32_t n_sel, bool root) {
   demi_handle* h = st.h;
-  if ((unsigned long long)st.n_slots + n_sel > st.F.trace_cap) { st.R.status = DEMI_DS_TRACE_OVF; return DEMI_OK; }
+  if ((unsigned long long)st.n_slots + n_sel > st.F.trace_cap) return fr_round_fail(st, DEMI_DS_TRACE_OVF);   // the whole round, before it runs
   FrArgs& A = st.A;
   A.n_sel = n_sel; A.root = root ? 1u : 0u; A.first_slot = st.n_slots; A.exec_base = st.n_exec; A.pool_top = st.pool_top;
   if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, st.s));
@@ -384,11 +398,11 @@ int32_t fr_execute_and_scan(FrState& st, uint32_t n_sel, bool root) {
   float ms = 0;
   cudaEventElapsedTime(&ms, st.ev[0], st.ev[1]); st.R.exec_ms += ms;
   cudaEventElapsedTime(&ms, st.ev[1], st.ev[2]); st.R.scan_ms += ms;
-  if (ctr[FRC_STATUS]) { st.R.status = (uint32_t)ctr[FRC_STATUS]; return DEMI_OK; }
-  if (ctr[FRC_EXPLORED] * 2 >= st.F.explored_slots) { st.R.status = DEMI_DS_EXPLORED_OVF; return DEMI_OK; }
+  if (ctr[FRC_STATUS]) return fr_round_fail(st, (uint32_t)ctr[FRC_STATUS]);
+  if (ctr[FRC_EXPLORED] * 2 >= st.F.explored_slots) return fr_round_fail(st, DEMI_DS_EXPLORED_OVF);   // after the round's scan
   unsigned long long added = 0;
   for (uint32_t b = 0; b < st.T1; b++) added += tot[b];
-  if (st.pool_top + added > st.F.pool_cap) { st.R.status = DEMI_DS_HEAP_OVF; return DEMI_OK; }
+  if (st.pool_top + added > st.F.pool_cap) return fr_round_fail(st, DEMI_DS_HEAP_OVF);   // pool_cap bounds the arena: every point enqueued or received
   fr_add_run(st, st.pool_top, tot.data());
   st.pool_top += added;
   st.R.keys_enqueued += added;
@@ -578,7 +592,7 @@ int32_t fr_run(FrState& st, demi_dpor_violation* viol, uint32_t cap_viol, uint64
     }
   }
   // results
-  {
+  if (!st.round_failed) {
     unsigned long long ctr[FRC_N];                          // a steal round marks the points it hands over
     CUDA_TRY(h, cudaMemcpy(ctr, st.ctr, sizeof(ctr), cudaMemcpyDeviceToHost));
     st.R.explored_pairs = ctr[FRC_EXPLORED];

@@ -62,14 +62,17 @@ struct FrArgs {
 };
 
 // ------------------------------------------------------------------ explored set
+// at most `slots` probes: on a full table an absent key answers "absent", and the host's check after the round
+// (explored pairs · 2 ≥ slots) reports DEMI_DS_EXPLORED_OVF
 __device__ __forceinline__ bool fr_e_has(const unsigned long long* E, unsigned long long slots, unsigned long long key) {
   unsigned long long s = demi_fr_explored_slot(key, slots);
-  for (;;) {
+  for (unsigned long long probes = 0; probes < slots; probes++) {
     const unsigned long long v = E[s];
     if (v == 0ull) return false;
     if (v == key) return true;
     s = (s + 1) & (slots - 1);
   }
+  return false;
 }
 // returns true when the key was new
 __device__ __forceinline__ bool fr_e_insert(unsigned long long* E, unsigned long long slots, unsigned long long key, unsigned long long* ctr) {

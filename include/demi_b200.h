@@ -551,8 +551,9 @@ typedef struct demi_frontier_params {
   uint32_t stop_if_found;         /* stopIfViolationFound (:82), applied at round granularity            */
   uint32_t width;                 /* backtrack points replayed per round per rank                        */
   uint64_t max_interleavings;     /* exploration budget over all ranks                                    */
-  uint64_t explored_slots;        /* per rank, power of two                                              */
-  uint64_t pool_cap;              /* per rank: queued backtrack points                                   */
+  uint64_t explored_slots;        /* per rank, power of two; a round leaving explored_pairs·2 ≥ this fails */
+  uint64_t pool_cap;              /* per rank: backtrack points enqueued + received over the search (the
+                                     arena is append-only: dequeued points are not reclaimed)            */
   uint32_t trace_cap;             /* per rank: trace slots (executed + imported)                         */
   uint32_t rounds_per_exchange;   /* steal period in rounds (ignored on one rank)                        */
   uint32_t steal_max;             /* most records one rank sends to one other rank per exchange          */
@@ -586,7 +587,14 @@ typedef struct demi_frontier_entry {    /* one delivered event of a trace, 16 by
 /* Runs on this handle's device; with a communicator (demi_comm_init) every rank calls it collectively.
  * hashes (cap_hashes, may be NULL): schedule hash of every interleaving executed on this rank, in slot order;
  * viol (cap_viol): this rank's violating interleavings in execution order (`interleaving` indexes `hashes`); when more
- * than cap_viol violate, result->violations still counts them all and which cap_viol records are returned is unspecified. */
+ * than cap_viol violate, result->violations still counts them all and which cap_viol records are returned is unspecified.
+ * Capacities (result->status, the call returns DEMI_ERR_CAPACITY): a round needs its trace slots before it executes
+ * (TRACE_OVF); after its scan the explored table must stay below half full (EXPLORED_OVF) and its new points must fit
+ * the arena (HEAP_OVF); an execution may fail with QUEUE_OVF / UNSUPPORTED.  A round that fails adds nothing to the
+ * executed work: interleavings, deliveries, violations, races, keys_enqueued, rounds, trace_slots, the hashes and the
+ * violation records are those after the last completed round (the same as a search whose budget ends there), while
+ * keys_dropped, pool_left and explored_pairs are those after the failed round's getNext.  On a steal, a receiver takes
+ * a donor's batch whole or, when its trace slots or arena cannot hold it, not at all. */
 int32_t demi_dpor_frontier(demi_handle* h, const demi_ext_event* ext, uint32_t n_ext,
                            const demi_frontier_params* params, demi_frontier_result* result,
                            demi_dpor_violation* viol, uint32_t cap_viol, uint64_t* hashes, uint64_t cap_hashes);

@@ -28,17 +28,21 @@ typedef struct { uint64_t ord, pk; } fkey;                          /* queue ent
 typedef struct { uint64_t id; demi_msg msg; uint16_t ppos; } fpend;  /* a pending message and the position that created it */
 
 typedef struct {
-  /* explored ordered pairs */
-  uint64_t* E; uint64_t e_slots, n_E; int no_history;     /* trackHistory = false (:86): the set stays empty */
-  uint64_t* log; uint64_t n_log, cap_log;                  /* pair keys marked since the last exchange (shared with the other ranks there) */
+  /* explored ordered pairs.  The table is private and grows, so it never fills; `e_cap` (explored_slots) is the
+   * engine's table, and a round after which n_E·2 ≥ e_cap ends the search with DEMI_DS_EXPLORED_OVF */
+  uint64_t* E; uint64_t e_slots, n_E, e_cap; int no_history;   /* trackHistory = false (:86): the set stays empty */
+  uint64_t* log; uint64_t n_log, cap_log, log_alloc;       /* pair keys marked since the last exchange (shared with the other ranks there) */
   /* trace store */
   demi_frontier_entry* tr; uint32_t* tr_len; uint32_t* tr_branch; uint32_t n_slots, cap_slots, T1;
-  /* backtrack queue, ascending ord */
-  fkey* pool; uint64_t n_pool, cap_pool;
+  /* backtrack queue, ascending ord; pool_top = points enqueued + received so far, bounded by pool_cap (the arena) */
+  fkey* pool; uint64_t n_pool, cap_pool, pool_top;
   demi_frontier_result R;
   demi_dpor_violation* viol; uint32_t cap_viol;
   uint64_t* hashes; uint64_t cap_hashes, n_hashes;
   uint32_t round_first_slot, round_n;                                /* the traces executed in the current round */
+  /* the counters after the current round's getNext: a round that ends in a capacity status goes back to them */
+  demi_frontier_result snap; uint32_t snap_slots; uint64_t snap_hashes, snap_E;
+  int explored_fixed;                                                /* R.explored_pairs was set by a failed round */
 } frank;
 
 typedef struct {
@@ -63,13 +67,25 @@ static int e_has(const frank* r, uint64_t key) {
   while (r->E[s]) { if (r->E[s] == key) return 1; s = (s + 1) & (r->e_slots - 1); }
   return 0;
 }
+static void e_place(uint64_t* E, uint64_t slots, uint64_t key) {
+  uint64_t s = demi_fr_explored_slot(key, slots);
+  while (E[s]) s = (s + 1) & (slots - 1);
+  E[s] = key;
+}
 static void e_add(frank* r, uint64_t key) {
   if (r->no_history) return;
   uint64_t s = demi_fr_explored_slot(key, r->e_slots);
   while (r->E[s]) { if (r->E[s] == key) return; s = (s + 1) & (r->e_slots - 1); }
-  if (r->n_E * 2 >= r->e_slots) { r->R.status = DEMI_DS_EXPLORED_OVF; return; }
   r->E[s] = key; r->n_E++;
-  if (r->log) { if (r->n_log >= r->cap_log) { r->R.status = DEMI_DS_EXPLORED_OVF; return; } r->log[r->n_log++] = key; }
+  if (r->n_E * 2 >= r->e_slots) {                                         /* keep the private table at most half full */
+    uint64_t* E2 = (uint64_t*)calloc(r->e_slots * 2, 8);
+    for (uint64_t i = 0; i < r->e_slots; i++) if (r->E[i]) e_place(E2, r->e_slots * 2, r->E[i]);
+    free(r->E); r->E = E2; r->e_slots *= 2;
+  }
+  if (r->log) {                                                           /* its capacity is checked after the round */
+    if (r->n_log == r->log_alloc) { r->log_alloc *= 2; r->log = (uint64_t*)realloc(r->log, 8 * r->log_alloc); }
+    r->log[r->n_log++] = key;
+  }
 }
 
 /* --------------------------------------------- DPORwHeuristics.event_produced */
@@ -215,15 +231,30 @@ static uint32_t f_execute(fexec* x, const demi_frontier_entry* kt, uint32_t bran
 }
 
 /* ------------------------------------------------------------ rank state */
-static int pool_insert_sorted(frank* r, const fkey* add, uint64_t n) {      /* `add` ascending; merge */
-  if (r->n_pool + n > r->cap_pool) { r->R.status = DEMI_DS_HEAP_OVF; return 0; }
+/* `add` ascending; merge.  pool_cap bounds the arena (every point enqueued or received over the search), not the live
+ * queue: DEMI_DS_HEAP_OVF when these `n` would take the total past it.  The live queue never exceeds the arena. */
+static int pool_insert_sorted(frank* r, const fkey* add, uint64_t n) {
+  if (r->pool_top + n > r->cap_pool) { r->R.status = DEMI_DS_HEAP_OVF; return 0; }
   uint64_t i = r->n_pool, j = n, k = r->n_pool + n;
   while (j > 0) {
     if (i > 0 && r->pool[i - 1].ord > add[j - 1].ord) r->pool[--k] = r->pool[--i];
     else r->pool[--k] = add[--j];
   }
-  r->n_pool += n;
+  r->n_pool += n; r->pool_top += n;
   return 1;
+}
+/* the counters after getNext, before the round executes */
+static void round_snapshot(frank* r) {
+  r->snap = r->R; r->snap_slots = r->n_slots; r->snap_hashes = r->n_hashes; r->snap_E = r->n_E;
+}
+/* a round that ends in a capacity status adds nothing to the executed work: interleavings, deliveries, violations,
+ * races, keys_enqueued, rounds, trace slots and hashes go back to the last completed round; keys_dropped, pool_left
+ * and explored_pairs keep the failed round's getNext */
+static void round_fail(frank* r, uint32_t status) {
+  r->R = r->snap; r->n_slots = r->snap_slots; r->n_hashes = r->snap_hashes;
+  r->R.explored_pairs = r->snap_E; r->explored_fixed = 1;
+  r->R.status = status;
+  r->round_n = 0;
 }
 static int fkey_cmp(const void* a, const void* b) {
   const fkey* x = (const fkey*)a; const fkey* y = (const fkey*)b;
@@ -257,8 +288,8 @@ static void f_scan(frank* r, uint32_t slot, int pass, fkey* out, uint64_t* n_out
     }
 }
 
-/* one round on one rank: dequeue up to `quota` unexplored points, execute, scan */
-static void f_round(frank* r, fexec* x, uint32_t quota, fkey* scratch) {
+/* one round on one rank: dequeue up to `quota` unexplored points, execute (the scan follows); returns the points run */
+static uint32_t f_round(frank* r, fexec* x, uint32_t quota, fkey* scratch) {
   /* getNext (:1142-1162), `quota` times without an intervening scan */
   uint64_t taken = 0; uint32_t n_sel = 0;
   fkey* sel = scratch;                                                      /* the selected points, queue order */
@@ -270,17 +301,19 @@ static void f_round(frank* r, fexec* x, uint32_t quota, fkey* scratch) {
   }
   memmove(r->pool, r->pool + taken, sizeof(fkey) * (r->n_pool - taken));
   r->n_pool -= taken;
-  if (r->R.status) return;
   r->round_first_slot = r->n_slots; r->round_n = 0;
-  for (uint32_t s = 0; s < n_sel && !r->R.status; s++) {
-    if (r->n_slots >= r->cap_slots) { r->R.status = DEMI_DS_TRACE_OVF; break; }
+  if (!n_sel) { r->R.rounds++; return 0; }
+  round_snapshot(r);
+  /* the whole round needs its trace slots before any point runs */
+  if ((uint64_t)r->n_slots + n_sel > r->cap_slots) { round_fail(r, DEMI_DS_TRACE_OVF); return n_sel; }
+  for (uint32_t s = 0; s < n_sel; s++) {
     const uint32_t kslot = demi_fr_ord_slot(sel[s].ord), branch = demi_fr_ord_branch(sel[s].ord);
     const uint32_t li = demi_fr_ord_later(sel[s].ord), ei = demi_fr_ord_earlier(sel[s].ord);
     const uint32_t slot = r->n_slots++;
     x->cur = r->tr + (size_t)slot * r->T1;
     uint64_t sh;
     uint32_t v = f_execute(x, r->tr + (size_t)kslot * r->T1, branch, li, ei, &sh);
-    if (x->status) { r->R.status = (uint32_t)x->status; break; }
+    if (x->status) { round_fail(r, (uint32_t)x->status); return n_sel; }
     r->tr_len[slot] = x->cur_len; r->tr_branch[slot] = branch;
     r->round_n++;
     if (r->hashes && r->n_hashes < r->cap_hashes) r->hashes[r->n_hashes] = sh;
@@ -295,15 +328,19 @@ static void f_round(frank* r, fexec* x, uint32_t quota, fkey* scratch) {
     }
   }
   r->R.rounds++;
+  return n_sel;
 }
+/* the scan of the round's traces and the enqueue; the explored table's and the arena's capacities are decided here,
+ * for the whole round (cap_scratch holds any round: at most rcap < T1²/2 points per trace) */
 static void f_scan_round(frank* r, fkey* scratch, uint64_t cap_scratch) {
-  for (uint32_t s = 0; s < r->round_n && !r->R.status; s++) f_scan(r, r->round_first_slot + s, 0, 0, 0);
+  for (uint32_t s = 0; s < r->round_n; s++) f_scan(r, r->round_first_slot + s, 0, 0, 0);
   uint64_t n_new = 0;
-  for (uint32_t s = 0; s < r->round_n && !r->R.status; s++) {
-    if (n_new + (uint64_t)r->T1 * r->T1 > cap_scratch) { r->R.status = DEMI_DS_HEAP_OVF; break; }
+  for (uint32_t s = 0; s < r->round_n; s++) {
+    if (n_new + (uint64_t)r->T1 * r->T1 > cap_scratch) { round_fail(r, DEMI_DS_HEAP_OVF); return; }
     f_scan(r, r->round_first_slot + s, 1, scratch, &n_new);
   }
-  if (r->R.status) return;
+  if (r->n_E * 2 >= r->e_cap || (r->log && r->n_log > r->cap_log)) { round_fail(r, DEMI_DS_EXPLORED_OVF); return; }
+  if (r->pool_top + n_new > r->cap_pool) { round_fail(r, DEMI_DS_HEAP_OVF); return; }
   qsort(scratch, n_new, sizeof(fkey), fkey_cmp);                            /* already ascending per slot; slots ascending per branch */
   r->R.keys_enqueued += n_new;
   pool_insert_sorted(r, scratch, n_new);
@@ -335,8 +372,12 @@ int oracle_dpor_frontier(const demi_config* cfg, const demi_ext_event* ext, uint
   fkey* sbuf = (fkey*)malloc(sizeof(fkey) * (2 * (size_t)F->steal_max + 2));
   for (uint32_t q = 0; q < n_ranks; q++) {
     frank* r = &R[q];
-    r->e_slots = F->explored_slots; r->E = (uint64_t*)calloc(r->e_slots, 8); r->no_history = (F->flags & DEMI_FR_NO_HISTORY) != 0;
-    if (n_ranks > 1 && !r->no_history) { r->cap_log = F->explored_slots / 2 < (1ull << 22) ? F->explored_slots / 2 : (1ull << 22); r->log = (uint64_t*)malloc(8 * r->cap_log); }
+    r->no_history = (F->flags & DEMI_FR_NO_HISTORY) != 0;
+    r->e_cap = F->explored_slots; r->e_slots = r->no_history ? 1 : 1024; r->E = (uint64_t*)calloc(r->e_slots, 8);
+    if (n_ranks > 1 && !r->no_history) {
+      r->cap_log = F->explored_slots / 2 < (1ull << 22) ? F->explored_slots / 2 : (1ull << 22);
+      r->log_alloc = 1024; r->log = (uint64_t*)malloc(8 * r->log_alloc);
+    }
     r->T1 = T1; r->cap_slots = F->trace_cap;
     r->tr = (demi_frontier_entry*)malloc(sizeof(demi_frontier_entry) * (size_t)r->cap_slots * T1);
     r->tr_len = (uint32_t*)calloc(r->cap_slots, 4); r->tr_branch = (uint32_t*)calloc(r->cap_slots, 4);
@@ -349,11 +390,13 @@ int oracle_dpor_frontier(const demi_config* cfg, const demi_ext_event* ext, uint
   /* the first execution: no nextTrace (:1219-1221 with an empty backtrack set), on rank 0 */
   {
     frank* r = &R[0];
-    if (r->cap_slots < 1) r->R.status = DEMI_DS_TRACE_OVF;
-    else if (F->max_interleavings >= 1) {
+    round_snapshot(r);
+    if (F->max_interleavings < 1) {}
+    else if (r->cap_slots < 1) round_fail(r, DEMI_DS_TRACE_OVF);
+    else {
       x->cur = r->tr; uint64_t sh;
       uint32_t v = f_execute(x, 0, 0, 0, 0, &sh);
-      if (x->status) r->R.status = (uint32_t)x->status;
+      if (x->status) round_fail(r, (uint32_t)x->status);
       else {
         r->tr_len[0] = x->cur_len; r->tr_branch[0] = 0; r->n_slots = 1;
         r->round_first_slot = 0; r->round_n = 1;
@@ -377,6 +420,9 @@ int oracle_dpor_frontier(const demi_config* cfg, const demi_ext_event* ext, uint
     if (!total_pool) { exhausted = 1; break; }
     /* ---- the pair keys every rank marked since the last exchange become known to all ranks (a set union) */
     if (n_ranks > 1 && R[0].log) {
+      int log_ovf = 0;                                                      /* a log past its capacity fails every rank */
+      for (uint32_t q = 0; q < n_ranks; q++) log_ovf |= R[q].n_log > R[q].cap_log;
+      if (log_ovf) { for (uint32_t q = 0; q < n_ranks; q++) R[q].R.status = DEMI_DS_EXPLORED_OVF; any_status = 1; break; }
       for (uint32_t q = 0; q < n_ranks; q++) R[q].R.bytes_sent += R[q].n_log * 8ull * (n_ranks - 1);
       for (uint32_t rcv = 0; rcv < n_ranks; rcv++)
         for (uint32_t src = 0; src < n_ranks; src++) {
@@ -418,9 +464,14 @@ int oracle_dpor_frontier(const demi_config* cfg, const demi_ext_event* ext, uint
             moved[n_moved++] = d->pool[i];
           }
           d->n_pool = lo;
+          d->R.records_sent += n_moved; d->R.bytes_sent += 16ull * (T1 + 2) * n_moved;   /* fixed-stride records on the wire */
+          /* a receiver takes a donor's batch whole or, when its trace slots or its arena cannot hold it, not at all
+           * (and no later batch) */
+          if (r->R.status || !n_moved) continue;
+          if ((uint64_t)r->n_slots + n_moved > r->cap_slots) { r->R.status = DEMI_DS_TRACE_OVF; continue; }
+          if (r->pool_top + n_moved > r->cap_pool) { r->R.status = DEMI_DS_HEAP_OVF; continue; }
           /* each record = the point + its trace prefix [0..later]; the receiver stores the prefix in a new slot */
-          for (uint64_t i = 0; i < n_moved && !r->R.status; i++) {
-            if (r->n_slots >= r->cap_slots) { r->R.status = DEMI_DS_TRACE_OVF; break; }
+          for (uint64_t i = 0; i < n_moved; i++) {
             const uint32_t kslot = demi_fr_ord_slot(moved[i].ord), li = demi_fr_ord_later(moved[i].ord);
             const uint32_t slot = r->n_slots++;
             memcpy(r->tr + (size_t)slot * T1, d->tr + (size_t)kslot * T1, sizeof(demi_frontier_entry) * (li + 1));
@@ -428,14 +479,11 @@ int oracle_dpor_frontier(const demi_config* cfg, const demi_ext_event* ext, uint
             fkey k; k.pk = moved[i].pk;
             k.ord = demi_fr_ord(demi_fr_ord_branch(moved[i].ord), slot, li, demi_fr_ord_earlier(moved[i].ord));
             sbuf[F->steal_max + i] = k;
-            d->R.records_sent++; d->R.bytes_sent += 16ull * (T1 + 2);   /* fixed-stride records on the wire */
-            r->R.records_received++;
           }
-          if (!r->R.status && n_moved) {
-            fkey* in = sbuf + F->steal_max;
-            qsort(in, n_moved, sizeof(fkey), fkey_cmp);
-            pool_insert_sorted(r, in, n_moved);
-          }
+          r->R.records_received += n_moved;
+          fkey* in = sbuf + F->steal_max;
+          qsort(in, n_moved, sizeof(fkey), fkey_cmp);
+          pool_insert_sorted(r, in, n_moved);
         }
       }
       any_status = 0;
@@ -453,10 +501,9 @@ int oracle_dpor_frontier(const demi_config* cfg, const demi_ext_event* ext, uint
       left -= allow;
       for (uint32_t s = 0; s < S && allow && r->n_pool && !r->R.status; s++) {
         uint32_t quota = allow < F->width ? (uint32_t)allow : F->width;
-        const uint64_t before = r->R.interleavings;
-        f_round(r, x, quota, scratch);
-        allow -= r->R.interleavings - before;
-        if (!r->R.status) f_scan_round(r, scratch, cap_scratch);
+        const uint32_t n_run = f_round(r, x, quota, scratch);
+        allow -= n_run;
+        if (n_run && !r->R.status) f_scan_round(r, scratch, cap_scratch);
         if (F->stop_if_found && r->R.violations) break;
       }
     }
@@ -464,7 +511,8 @@ int oracle_dpor_frontier(const demi_config* cfg, const demi_ext_event* ext, uint
   g_fx = 0;
   for (uint32_t q = 0; q < n_ranks; q++) {
     frank* r = &R[q];
-    r->R.explored_pairs = r->n_E; r->R.pool_left = r->n_pool; r->R.trace_slots = r->n_slots;
+    if (!r->explored_fixed) r->R.explored_pairs = r->n_E;
+    r->R.pool_left = r->n_pool; r->R.trace_slots = r->n_slots;
     r->R.exhausted = (uint32_t)exhausted; r->R.budget_exhausted = (uint32_t)budget;
     results[q] = r->R;
     free(r->log); free(r->E); free(r->tr); free(r->tr_len); free(r->tr_branch); free(r->pool);
