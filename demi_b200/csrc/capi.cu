@@ -2,6 +2,7 @@
 // No CPU fallback: every compute entry point needs a CUDA device.
 #include <climits>
 #include <cmath>
+#include <cstddef>
 #include <cstdlib>
 #include <cstdio>
 #include <cstdarg>
@@ -70,12 +71,14 @@ static const Variant* pick_variant(int model, LaunchMode mode, uint32_t pcap, ui
 }
 
 // lane-engine table
-// `steady`: the LM_BATCH instantiation that starts from the program's snapshot (`snapshot` takes it); `ops` is the
-// model's operations per receive(), which the node-capacity proof of lane_steady_eligible counts with.
+// `steady`: the LM_BATCH instantiation that starts from the program's tree (`snapshot` takes its root, `tree` builds
+// one level, of records `node_bytes` long); `ops` is the model's operations per receive(), which the node-capacity
+// proof of lane_steady_eligible counts with.
 typedef void (*snapshot_fn)(const KernelArgs, LaneSnapshot*);
+typedef void (*tree_fn)(const KernelArgs, uint32_t*, const uint2*, uint32_t, uint32_t);
 struct LaneVariant {
   int model; int bd; uint32_t lpcap; size_t smem_per_block; kernel_fn fn[LM_COUNT];
-  kernel_fn steady; size_t steady_smem; snapshot_fn snapshot; uint32_t ops;
+  kernel_fn steady; size_t steady_smem; snapshot_fn snapshot; tree_fn tree; uint32_t node_bytes; uint32_t ops;
 };
 template <class MODEL, int BD, int LPCAP>
 static LaneVariant make_lane_variant() {
@@ -85,7 +88,7 @@ static LaneVariant make_lane_variant() {
                      {fuzz_lane_kernel<MODEL, BD, LPCAP>, fuzz_lane_kernel<MODEL, BD, LPCAP, true>,
                       fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>, fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true>},
                      fuzz_lane_kernel<MODEL, BD, LPCAP, false, false, false, true>, (size_t)S::WORDS * BD * sizeof(uint32_t),
-                     lane_snapshot_kernel<MODEL>, (uint32_t)MODEL::LANE_OUTBOX};
+                     lane_snapshot_kernel<MODEL>, lane_tree_kernel<MODEL, LPCAP>, S::NODE_WORDS * 4u, (uint32_t)MODEL::LANE_OUTBOX};
 }
 #ifndef DEMI_K1_BD_RAFT5
 #define DEMI_K1_BD_RAFT5 256
@@ -265,6 +268,8 @@ extern "C" int32_t demi_set_externals(demi_handle* h, const demi_ext_event* ev, 
     if (rc != DEMI_OK) return rc;
     describe_event(&info, &sv, ev[i]);
   }
+  // the program the handle has: everything below would compute what it holds, the tree included
+  if (n && n == h->ext_host.size() && memcmp(ev, h->ext_host.data(), n * sizeof(demi_ext_event)) == 0) return DEMI_OK;
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   DevBuf ext_dev, sends_dev, snap_dev;
   LaneSnapshot snap{};
@@ -277,7 +282,8 @@ extern "C" int32_t demi_set_externals(demi_handle* h, const demi_ext_event* ev, 
     // capacities (launch_plan).  It depends on the program and the model alone (no actor has received anything, and
     // the snapshot holds no actor state, so neither model_flags nor ignoreTimers shows in it), hence it is taken here
     // and not per batch.
-    if ((rc = snap_dev.grow(h, sizeof(LaneSnapshot))) != DEMI_OK) return rc;
+    const size_t snap_bytes = sizeof(LaneSnapshot) + lv->node_bytes;      // the snapshot, then the tree's root
+    if ((rc = snap_dev.grow(h, snap_bytes)) != DEMI_OK) return rc;
     KernelArgs a{};
     a.ext = ext_dev.get<demi_ext_event>(); a.n_ext = n;
     a.ext_sends = sends_dev.get<uint4>();
@@ -285,7 +291,7 @@ extern "C" int32_t demi_set_externals(demi_handle* h, const demi_ext_event* ev, 
     a.model_flags = h->cfg.model_flags;
     a.max_messages = INT_MAX;
     a.node_cap = 65535u; a.pending_cap = 0xFFFFu; a.tosend_cap = 0xFFFFu;
-    CUDA_TRY(h, cudaMemsetAsync(snap_dev.get(), 0, sizeof(LaneSnapshot), h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(snap_dev.get(), 0, snap_bytes, h->stream));
     lv->snapshot<<<1, 1, 0, h->stream>>>(a, snap_dev.get<LaneSnapshot>());
     CUDA_TRY(h, cudaGetLastError());
     CUDA_TRY(h, cudaMemcpyAsync(&snap, snap_dev.get(), sizeof(LaneSnapshot), cudaMemcpyDeviceToHost, h->stream));
@@ -297,6 +303,7 @@ extern "C" int32_t demi_set_externals(demi_handle* h, const demi_ext_event* ev, 
   h->ext_sends_dev = std::move(sends_dev);
   h->lane_snap_dev = std::move(snap_dev);
   h->lane_snap = snap;
+  h->lane_tree_built = false;
   return DEMI_OK;
 }
 
@@ -381,11 +388,58 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, LaunchMode
   return DEMI_OK;
 }
 
+// The tree of the handle's program for a steady launch with arguments `la` (lane_steady.hpp), kept on the handle and
+// built again only when the program or the key changes.  Level by level: the host reads the new level's first 16
+// bytes per record, decides with lane_tree_extend whether the next level is built, and lists its children; one thread
+// builds each.  The root is the record the snapshot kernel stored after the snapshot.
+static int32_t lane_tree(demi_handle* h, const LaneVariant* lv, const KernelArgs& la, cudaStream_t s) {
+  const LaneTreeKey key = lane_tree_key(la.model_flags, la.interval, la.max_messages, la.pending_cap);
+  if (h->lane_tree_built && h->lane_tree_key == key) return DEMI_OK;
+  h->lane_tree_built = false;
+  const size_t nb = lv->node_bytes;
+  int32_t rc;
+  if ((rc = h->lane_tree.grow(h, std::max<size_t>(LANE_TREE_BUDGET, nb))) != DEMI_OK) return rc;
+  uint8_t* tree = h->lane_tree.get<uint8_t>();
+  CUDA_TRY(h, cudaMemcpyAsync(tree, h->lane_snap_dev.get<uint8_t>() + sizeof(LaneSnapshot), nb, cudaMemcpyDeviceToDevice, s));
+  KernelArgs ba = la;
+  ba.pending_cap = std::min(la.pending_cap, LANE_NODE_ROWS);
+  uint64_t lo = 0, hi = 1;                           // the deepest level's records
+  uint32_t depth = 0;
+  std::vector<uint4> head;
+  std::vector<uint2> kids;
+  for (;;) {
+    head.resize(hi - lo);
+    CUDA_TRY(h, cudaMemcpy2DAsync(head.data(), sizeof(uint4), tree + lo * nb, nb, sizeof(uint4), hi - lo, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(h, cudaStreamSynchronize(s));
+    kids.clear();
+    for (uint64_t j = 0; j < hi - lo; j++)
+      if (lane_node_expands(head[j].y, (int32_t)head[j].z, head[j].w, la.max_messages))
+        for (uint32_t i = 0; i < head[j].y; i++) kids.push_back(make_uint2((uint32_t)(lo + j), i));
+    if (!lane_tree_extend(depth, hi, kids.size(), (uint32_t)nb)) break;
+    if ((rc = h->lane_tree_kids.grow(h, kids.size() * sizeof(uint2))) != DEMI_OK) return rc;
+    CUDA_TRY(h, cudaMemcpyAsync(h->lane_tree_kids.get(), kids.data(), kids.size() * sizeof(uint2), cudaMemcpyHostToDevice, s));
+    const uint32_t n = (uint32_t)kids.size();
+    lv->tree<<<(n + LANE_TREE_BD - 1) / LANE_TREE_BD, LANE_TREE_BD, 0, s>>>(ba, reinterpret_cast<uint32_t*>(tree),
+                                                                         h->lane_tree_kids.get<uint2>(), (uint32_t)hi, n);
+    CUDA_TRY(h, cudaGetLastError());
+    lo = hi; hi += n; depth++;
+  }
+  h->lane_snap.depth = depth;
+  h->lane_snap.tree = (uint64_t)(uintptr_t)tree;
+  CUDA_TRY(h, cudaMemcpyAsync(h->lane_snap_dev.get<uint8_t>() + offsetof(LaneSnapshot, depth), &h->lane_snap.depth,
+                              sizeof(LaneSnapshot) - offsetof(LaneSnapshot, depth), cudaMemcpyHostToDevice, s));
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  h->lane_tree_key = key;
+  h->lane_tree_built = true;
+  return DEMI_OK;
+}
+
 // The lane engine over the plan's `n_items` work items when one applies, then the warp engine on the items it deferred
 // (on every item otherwise).  Counts both launches.
 static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, cudaStream_t s) {
   KernelArgs& a = plan.args;
   h->lane_kernel = DEMI_LANE_NONE;
+  h->lane_tree_depth = -1;
   if (const LaneVariant* lv = pick_lane_variant(h, *plan.prog)) {
     const uint32_t lane_pcap = std::min(h->lane_pending_cap ? std::min(a.pending_cap, h->lane_pending_cap) : a.pending_cap, lv->lpcap);
     // A batch over the handle's program starts every execution from the program's snapshot when the rule of
@@ -418,10 +472,15 @@ static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, c
     la.prog_lane_pcap = h->lane_pending_cap;
     la.ovf_list = h->ovf_list.get<uint32_t>(); la.ovf_count = h->ovf_count.get<uint32_t>();
     if (h->lane_pending_cap) la.pending_cap = std::min(la.pending_cap, h->lane_pending_cap);     // deferring is always exact
-    if (steady) { la.pending_cap = lane_pcap; la.lane_snap = h->lane_snap_dev.get<LaneSnapshot>(); }   // one bound, rows included
+    if (steady) {
+      la.pending_cap = lane_pcap;                    // one bound, rows included
+      la.lane_snap = h->lane_snap_dev.get<LaneSnapshot>();
+      if ((rc = lane_tree(h, lv, la, s)) != DEMI_OK) return rc;
+    }
     lfn<<<lgrid, lv->bd, lsmem, s>>>(la);
     CUDA_TRY(h, cudaGetLastError());
     h->lane_kernel = steady ? DEMI_LANE_STEADY : DEMI_LANE_GENERIC;
+    h->lane_tree_depth = steady ? (int32_t)h->lane_snap.depth : -1;
     h->perf.kernel_launches++;
     // what the lane engine could not prove exact: a recording launch numbers its outputs by work-list position
     if (plan.mode == LM_RECORD) { a.pos_list = la.ovf_list; a.pos_count = la.ovf_count; }
@@ -1206,6 +1265,7 @@ extern "C" int32_t demi_random_ddmin(demi_handle* h, const demi_fuzz_params* p, 
 }
 
 extern "C" int32_t demi_lane_kernel(const demi_handle* h) { return h ? h->lane_kernel : DEMI_ERR_INVALID; }
+extern "C" int32_t demi_lane_tree_depth(const demi_handle* h) { return h ? h->lane_tree_depth : DEMI_ERR_INVALID; }
 
 extern "C" int32_t demi_stats(const demi_handle* h, demi_perf* out) {
   if (!h || !out) return DEMI_ERR_INVALID;

@@ -69,6 +69,11 @@ struct demi_handle {
   DevBuf lane_snap_dev;                            // demi::LaneSnapshot of ext_host (demi_set_externals takes it)
   demi::LaneSnapshot lane_snap{};                  // its host copy: what launch_plan decides on
   int32_t lane_kernel = DEMI_LANE_NONE;            // the lane instantiation the last fuzz launch ran (demi_lane_kernel)
+  // the tree of the steady instantiation (lane_steady.hpp): node records, built for ext_host under lane_tree_key
+  DevBuf lane_tree, lane_tree_kids;                // uint32_t records; uint2 (parent, pending index) of a level's children
+  bool lane_tree_built = false;
+  demi::LaneTreeKey lane_tree_key{};
+  int32_t lane_tree_depth = -1;                    // the depth the last fuzz launch walked (-1: not the steady one)
   DevBuf rec_counts_dev;                           // uint32_t
   DevBuf prov_scratch;
   DevBuf dpor_buf[24];                             // K3 per-search structures (capi_dpor.cu)

@@ -589,7 +589,11 @@ struct LaneMachine {
   __device__ __forceinline__ bool pick_next(uint4& pick) {
     if (status) return false;
     if (n_pending == 0) return false;
-    pick = pending_remove_at(rng.next_int(n_pending));          // Util.scala:171-176
+    return pick_at(rng.next_int(n_pending), pick);              // Util.scala:171-176
+  }
+  // The pick of pending index i: what pick_next does once it has drawn i.  lane_tree_kernel picks each i in turn.
+  __device__ __forceinline__ bool pick_at(uint32_t i, uint4& pick) {
+    pick = pending_remove_at(i);
     nsched++;
     if (nsched == 0x7FFFFFFF) nsched = 1;
     if (++nmod == A->interval) nmod = 0;
@@ -675,16 +679,62 @@ struct LaneMachine {
     const bool go = may_continue();
     drain(0, 0, go);
   }
-  // STEADY: the machine reset() left becomes the one first_flush() would have left.  Nothing has been delivered, so
-  // the actor states and every timer structure are as reset() set them; tosend is empty after a flush.
-  __device__ __forceinline__ void restore() {
-    const LaneSnapshot* s = A->lane_snap;
-    const uint4* sp = reinterpret_cast<const uint4*>(s->pend);
-    n_pending = __ldg(&s->n_pending);
+  // A node record of the tree (lane_steady.hpp): the header, the state and timer-copy words, then the pending rows.
+  static constexpr uint32_t NODE_WORDS = lane_node_words(N * SW + TW);
+  static constexpr uint32_t NODE_ROWS_AT = NODE_WORDS - LANE_NODE_ROWS * 4;
+  __device__ __forceinline__ uint32_t& machine_word(uint32_t i) {      // i < N * SW: a state word, else a timer copy
+    return smw[(i < (uint32_t)(N * SW) ? i : i + OBW + PW) * BD];
+  }
+  // Stores the machine as a node without children.  pend may already be the record's rows (lane_tree_kernel).
+  __device__ __forceinline__ void store_node(uint32_t* r) {
+    r[LN_CHILD] = LANE_NODE_LEAF; r[LN_N_PENDING] = n_pending; r[LN_NSCHED] = (uint32_t)nsched; r[LN_VIOLATION] = violation;
+    r[LN_NMOD] = (uint32_t)nmod; r[LN_MAX_PENDING] = max_pending; r[LN_N_NODES] = n_nodes; r[LN_N_EVENTS] = n_events;
+    r[LN_PARENT_EVENT] = parent_event; r[LN_REGISTRY] = registry; r[LN_CANCELLED] = cancelled; r[LN_JUST] = just;
+    r[LN_WINDOW_TIMERS] = window_timers; r[LN_N_RESEND] = n_resend;
+    r[LN_RESEND_LO] = (uint32_t)resend; r[LN_RESEND_HI] = (uint32_t)(resend >> 32);
+    r[LN_THASH_LO] = (uint32_t)thash; r[LN_THASH_HI] = (uint32_t)(thash >> 32);
+    for (uint32_t i = 0; i < (uint32_t)(N * SW + TW); i++) r[LANE_NODE_HEAD + i] = machine_word(i);
+    uint4* rows = reinterpret_cast<uint4*>(r + NODE_ROWS_AT);
+    if (rows != pend)
+      for (uint32_t i = 0; i < n_pending; i++) rows[i] = ld_l2_hint(pend + i, pol);
+  }
+  // The steady machine becomes the one stored in record r (status 0): every register and shared word the rest of an
+  // execution reads.  tosend is empty at a stored pick point, or never read again when the execution stops there.
+  __device__ __forceinline__ void load_node(const uint32_t* r) {
+    static_assert(STEADY, "a node is the steady machine");
+    const uint4* q = reinterpret_cast<const uint4*>(r);
+    const uint4 h0 = __ldg(q), h1 = __ldg(q + 1), h2 = __ldg(q + 2), h3 = __ldg(q + 3), h4 = __ldg(q + 4);
+    n_pending = h0.y; nsched = (int32_t)h0.z; violation = h0.w;
+    nmod = (int32_t)h1.x; max_pending = h1.y; n_nodes = h1.z; n_events = h1.w;
+    parent_event = h2.x; registry = h2.y; cancelled = h2.z; just = h2.w;
+    window_timers = h3.x; n_resend = h3.y; resend = h3.z | (uint64_t)h3.w << 32;
+    thash = h4.x | (uint64_t)h4.y << 32;
+    status = 0;
+    tosend.clear();
 #pragma unroll 1
-    for (uint32_t i = 0; i < n_pending; i++) st_l2_hint(pend + i, __ldg(sp + i), pol);
-    n_nodes = __ldg(&s->n_nodes); n_events = __ldg(&s->n_events);
-    thash = __ldg(reinterpret_cast<const unsigned long long*>(&s->thash));
+    for (uint32_t i = 0; i < (uint32_t)(N * SW + TW); i++) machine_word(i) = __ldg(r + LANE_NODE_HEAD + i);
+    const uint4* rows = reinterpret_cast<const uint4*>(r + NODE_ROWS_AT);
+#pragma unroll 1
+    for (uint32_t i = 0; i < n_pending; i++) st_l2_hint(pend + i, __ldg(rows + i), pol);
+  }
+  // STEADY: the machine after the execution's first picks.  Each level of the tree draws the index pick_next would
+  // draw; the walk stops at a node without children, or before a child that is not stored, and leaves the generator
+  // as it is before the draw that the delivery loop then makes again.  The loop re-enters at its top, where
+  // may_continue() repeats a pure check (or stops the execution, as it did when the node was stored) and drain()
+  // finds tosend empty.
+  __device__ __forceinline__ void restore() {
+    const uint32_t* tree = reinterpret_cast<const uint32_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&A->lane_snap->tree)));
+    const uint32_t* at = tree;
+    uint4 h = __ldg(reinterpret_cast<const uint4*>(at));
+#pragma unroll 1
+    while (h.x != LANE_NODE_LEAF) {
+      JRandom r = rng;
+      const uint32_t* c = tree + (size_t)(h.x + r.next_int(h.y)) * NODE_WORDS;
+      const uint4 hc = __ldg(reinterpret_cast<const uint4*>(c));
+      if (hc.y == LANE_NODE_ABSENT) break;
+      rng = r; at = c; h = hc;
+    }
+    load_node(at);
   }
 
   // The deliveries of an execution, segment by segment.  STEADY has one segment and starts it at the top of the
@@ -742,8 +792,8 @@ struct LaneMachine {
 
   __device__ __forceinline__ void run(int64_t seed, demi_fuzz_result& out) {
     clk.enter(LP_TAIL);
-    reset(seed);
-    if constexpr (STEADY) restore();
+    if constexpr (STEADY) { rng.seed(seed); restore(); }
+    else reset(seed);
     deliver();
     finish(out);
   }
@@ -752,10 +802,12 @@ struct LaneMachine {
 // The pre-delivery snapshot of the launch's program (lane_steady.hpp): one thread runs reset() and first_flush() of
 // the generic machine with the physical limits in place of a batch's capacities (a batch compares the recorded
 // counts with its own), LANE_SNAP_CAP pending rows (a program that enables more defers, and is not snapshotted),
-// and stores the machine.  Launched when the program is set, not per batch.
+// and stores the machine, both as the snapshot's scalars (what the host decides on) and as the root record of the
+// tree, which follows the snapshot.  Launched when the program is set, not per batch.
 template <class MODEL>
 __global__ void lane_snapshot_kernel(const __grid_constant__ KernelArgs args, LaneSnapshot* out) {
   using M = LaneMachine<MODEL, 1, (int)LANE_SNAP_CAP>;
+  static_assert(M::NODE_WORDS == LaneMachine<MODEL, 1, 1, false, true>::NODE_WORDS, "one record layout per model");
   __shared__ uint32_t smem[M::WORDS];
   M m;
   m.smw = smem;
@@ -770,6 +822,44 @@ __global__ void lane_snapshot_kernel(const __grid_constant__ KernelArgs args, La
   out->root_timers = m.root_timers; out->registry = m.registry; out->cancelled = m.cancelled; out->tosend_n = m.tosend.n;
   out->ext_idx = m.ext_idx; out->ext_send_idx = m.ext_send_idx; out->inaccessible = m.inaccessible; out->killed = m.killed;
   out->status = m.status;
+  m.store_node(reinterpret_cast<uint32_t*>(out + 1));
+}
+
+// One level of the tree: thread c builds child c of the level, the machine after its parent picks pending index
+// kids[c].y, delivers it and reaches its next pick point (the top of the delivery loop: may_continue() and the flush),
+// exactly as the steady kernel does.  The launch's pending bound is lowered to the record's rows: an execution that
+// would exceed them defers here and is not stored, like every deferred one, so the walk stops at its parent and the
+// steady kernel runs that delivery itself.  The first child of each parent links the parent to its children.
+constexpr int LANE_TREE_BD = 32;
+template <class MODEL, int LPCAP>
+__global__ void __launch_bounds__(LANE_TREE_BD)
+lane_tree_kernel(const __grid_constant__ KernelArgs args, uint32_t* tree, const uint2* kids, uint32_t first, uint32_t n) {
+  using M = LaneMachine<MODEL, LANE_TREE_BD, LPCAP, false, true>;
+  __shared__ uint32_t smem[M::WORDS * LANE_TREE_BD];
+  const uint32_t c = blockIdx.x * LANE_TREE_BD + threadIdx.x;
+  if (c >= n) return;
+  const uint2 k = kids[c];
+  uint32_t* r = tree + (size_t)(first + c) * M::NODE_WORDS;
+  M m;
+  m.smw = smem + threadIdx.x;
+  m.pend = reinterpret_cast<uint4*>(r + M::NODE_ROWS_AT);
+  m.A = &args;
+  m.pol = l2_evict_last_policy();
+  m.rec_ev = nullptr; m.rec_par = nullptr;
+  m.clk.start();
+  m.rng.seed(0);
+  m.load_node(tree + (size_t)k.x * M::NODE_WORDS);
+  uint4 pick;
+  if (m.pick_at(k.y, pick)) {
+    const uint32_t n_ops = m.dispatch_new_message(pick);
+    if (!m.status) {
+      const bool go = m.may_continue();
+      m.drain(n_ops, hdr_dst(pick.x), go);
+    }
+  }
+  if (m.status) r[LN_N_PENDING] = LANE_NODE_ABSENT;
+  else m.store_node(r);
+  if (k.y == 0) tree[(size_t)k.x * M::NODE_WORDS + LN_CHILD] = first + c;
 }
 
 #ifndef DEMI_K1_MIN_BLOCKS

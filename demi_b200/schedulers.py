@@ -446,6 +446,10 @@ class Engine(object):
         """Which lane-engine instantiation the last fuzz launch ran: N.LANE_NONE, LANE_GENERIC or LANE_STEADY."""
         return N.lib().demi_lane_kernel(self._h)
 
+    def lane_tree_depth(self):
+        """The depth of the tree the last fuzz launch walked when it ran LANE_STEADY, else -1."""
+        return N.lib().demi_lane_tree_depth(self._h)
+
     def stats(self):
         s = N.Perf()
         self._check(N.lib().demi_stats(self._h, C.byref(s)))

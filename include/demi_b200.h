@@ -722,6 +722,10 @@ int32_t demi_stats(const demi_handle* h, demi_perf* out);
 #define DEMI_LANE_GENERIC 1
 #define DEMI_LANE_STEADY  2
 int32_t demi_lane_kernel(const demi_handle* h);
+/* The depth of the tree the handle's last fuzz launch started its executions from when it ran the steady instantiation:
+ * each execution skips up to that many of its first deliveries, whose machines the tree holds.  -1 for every other
+ * launch. */
+int32_t demi_lane_tree_depth(const demi_handle* h);
 
 #ifdef __cplusplus
 }
