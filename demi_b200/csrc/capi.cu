@@ -586,7 +586,7 @@ extern "C" int32_t demi_fuzz_batch(demi_handle* h, const demi_fuzz_params* p, de
   const uint64_t per = n_chunks ? (n + n_chunks - 1) / n_chunks : 0;
   return run_pipelined(h, "demi_fuzz_batch", n, per, out_host, [&](uint64_t off, uint64_t m, demi_fuzz_result* dst, bool first) {
     demi_fuzz_params q = *p;
-    q.seed_base = p->seed_base + (int64_t)off;
+    q.seed_base = seed_at(p->seed_base, off);
     q.n_prefixes = m;
     return launch_fuzz(h, &q, dst, h->stream, first);
   });
@@ -866,7 +866,7 @@ fuzzer_gen_kernel(const demi_fuzzer_config cfg, int64_t seed_base, uint64_t n, c
   uint16_t pairs[2 * (DEMI_MAX_ACTORS * (DEMI_MAX_ACTORS - 1) / 2)];
   demi_ext_event* out = events + i * stride;
   uint32_t n_sends = 0;
-  const uint32_t len = demi::fuzzer_generate(cfg, seed_base + (int64_t)i, fixed, n_prefix, fixed + n_prefix, n_postfix, alive, pairs,
+  const uint32_t len = demi::fuzzer_generate(cfg, seed_at(seed_base, i), fixed, n_prefix, fixed + n_prefix, n_postfix, alive, pairs,
                                              out, &n_sends);
   hdr[i] = make_uint2(len, n_sends);
   uint4* st = sends + i * send_stride;
@@ -953,9 +953,9 @@ extern "C" int32_t demi_fuzz_campaign_dev(demi_handle* h, const demi_fuzz_params
   if (n == 0) return launch_campaign(h, p, program_seed_base, out_dev, (cudaStream_t)stream, true);
   for (uint64_t off = 0; off < n; off += chunk) {
     demi_fuzz_params q = *p;
-    q.seed_base = p->seed_base + (int64_t)off;
+    q.seed_base = seed_at(p->seed_base, off);
     q.n_prefixes = std::min(chunk, n - off);
-    rc = launch_campaign(h, &q, program_seed_base + (int64_t)off, (demi_fuzz_result*)out_dev + off, (cudaStream_t)stream, off == 0);
+    rc = launch_campaign(h, &q, seed_at(program_seed_base, off), (demi_fuzz_result*)out_dev + off, (cudaStream_t)stream, off == 0);
     if (rc != DEMI_OK) return rc;
   }
   return DEMI_OK;
@@ -972,9 +972,9 @@ extern "C" int32_t demi_fuzz_campaign(demi_handle* h, const demi_fuzz_params* p,
   const uint64_t chunk = campaign_chunk(h, &stride, &send_stride);
   return run_pipelined(h, "demi_fuzz_campaign", p->n_prefixes, chunk, out_host, [&](uint64_t off, uint64_t m, demi_fuzz_result* dst, bool first) {
     demi_fuzz_params q = *p;
-    q.seed_base = p->seed_base + (int64_t)off;
+    q.seed_base = seed_at(p->seed_base, off);
     q.n_prefixes = m;
-    return launch_campaign(h, &q, program_seed_base + (int64_t)off, dst, h->stream, first);
+    return launch_campaign(h, &q, seed_at(program_seed_base, off), dst, h->stream, first);
   });
 }
 

@@ -58,7 +58,7 @@ fuzz_kernel(const __grid_constant__ KernelArgs args) {
       }
     } else {
       if constexpr (PROG) prog_bind(la, args, idx, false);
-      m.run(args.seed_base + (int64_t)idx, r);
+      m.run(seed_at(args.seed_base, idx), r);
     }
     const bool retry = args.ovf_list && (r.status == DEMI_PS_PENDING_OVF || r.status == DEMI_PS_NODE_OVF);
     if (retry) {

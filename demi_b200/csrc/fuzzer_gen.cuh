@@ -16,7 +16,8 @@ struct FzJavaRandom {
   DEMI_HD int32_t next_int(int32_t bound) {
     int32_t r = next(31), m = bound - 1;
     if ((bound & m) == 0) return (int32_t)(((int64_t)bound * (int64_t)r) >> 31);
-    for (int32_t u = r; u - (r = u % bound) + m < 0; u = next(31)) {}
+    // Java's `u - (r = u % bound) + m < 0` wraps in int; here in uint32_t, where the wrap is defined
+    for (int32_t u = r; (int32_t)((uint32_t)u - (uint32_t)(r = u % bound) + (uint32_t)m) < 0; u = next(31)) {}
     return r;
   }
   DEMI_HD double next_double() { return (double)(((int64_t)next(26) << 27) + next(27)) * (1.0 / (double)(1ll << 53)); }

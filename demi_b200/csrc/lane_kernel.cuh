@@ -913,7 +913,7 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
       }
     } else {
       if constexpr (PROG) prog_bind(la, args, idx, true);
-      m.run(args.seed_base + (int64_t)idx, r);
+      m.run(seed_at(args.seed_base, idx), r);
     }
     if (r.status == LANE_DEFER) {
       uint32_t pos = atomicAdd(args.ovf_count, 1u);

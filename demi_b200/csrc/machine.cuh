@@ -119,6 +119,9 @@ struct JRandom {
     return r;
   }
 };
+// The seed of execution `off` of a batch that starts at `base`.  Java's long addition wraps, and only the low 48 bits
+// reach the generator, so the sum is taken in uint64_t: int64_t addition would be undefined past INT64_MAX.
+__host__ __device__ __forceinline__ int64_t seed_at(int64_t base, uint64_t off) { return (int64_t)((uint64_t)base + off); }
 
 struct LaneSnapshot;
 struct KernelArgs {
@@ -208,7 +211,7 @@ __device__ __forceinline__ void prog_bind(KernelArgs& la, const KernelArgs& args
 __device__ __forceinline__ bool prog_test_bind(KernelArgs& la, const KernelArgs& args, uint64_t idx, bool lane, uint64_t& prog,
                                                int64_t& seed) {
   const uint32_t p = (uint32_t)idx / args.prog_execs, j = (uint32_t)idx - p * args.prog_execs;
-  prog = p; seed = args.seed_base + (int64_t)j;
+  prog = p; seed = seed_at(args.seed_base, j);
   uint32_t fh = *(volatile const uint32_t*)(args.prog_first_hit + p);
   if (!lane) fh = __shfl_sync(FULL_MASK, fh, 0);
   prog_bind(la, args, p, lane);

@@ -81,6 +81,16 @@ def kat_jrandom(seed, bound, n):
     return list(out)
 
 
+def jrandom_rejections():
+    """Redraws of nextInt(bound)'s rejection loop in this library since reset_jrandom_rejections()."""
+    lib().oracle_jrandom_rejections.restype = C.c_uint64
+    return int(lib().oracle_jrandom_rejections())
+
+
+def reset_jrandom_rejections():
+    lib().oracle_jrandom_reset_rejections()
+
+
 def kat_hashset(seed, ops, blocked_mask=0):
     ops_a = (C.c_int32 * len(ops))(*ops)
     arr = (C.c_int32 * (len(ops) + 1))()

@@ -152,8 +152,8 @@ static void* campaign_worker(void* arg) {
   om_machine* m = (om_machine*)malloc(sizeof(om_machine));
   demi_ext_event* prog = (demi_ext_event*)malloc(sizeof(demi_ext_event) * (j->n_prefix + j->fz->num_events + j->n_postfix + 1));
   for (uint64_t i = j->lo; i < j->hi; i++) {
-    uint32_t n = oracle_fuzzer_generate(j->fz, j->program_seed_base + (int64_t)i, j->prefix, j->n_prefix, j->postfix, j->n_postfix, prog);
-    oracle_run_prefix(j->cfg, prog, n, j->p, j->p->seed_base + (int64_t)i, &j->out[i], 0, 0, 0, 0, m);
+    uint32_t n = oracle_fuzzer_generate(j->fz, jr_seed_at(j->program_seed_base, i), j->prefix, j->n_prefix, j->postfix, j->n_postfix, prog);
+    oracle_run_prefix(j->cfg, prog, n, j->p, jr_seed_at(j->p->seed_base, i), &j->out[i], 0, 0, 0, 0, m);
   }
   free(prog);
   free(m);

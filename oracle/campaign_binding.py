@@ -41,6 +41,16 @@ def load_model(blob):
         raise RuntimeError("oracle_load_model: %d" % rc)
 
 
+def jrandom_rejections():
+    """Redraws of nextInt(bound)'s rejection loop in this library since reset_jrandom_rejections()."""
+    lib().oracle_jrandom_rejections.restype = C.c_uint64
+    return int(lib().oracle_jrandom_rejections())
+
+
+def reset_jrandom_rejections():
+    lib().oracle_jrandom_reset_rejections()
+
+
 def _ext(a):
     return np.ascontiguousarray(a if a is not None else np.zeros(0, dtype=EXT_DTYPE), dtype=EXT_DTYPE)
 

@@ -19,7 +19,7 @@ static void* fuzz_worker(void* arg) {
   fuzz_job* j = (fuzz_job*)arg;
   om_machine* m = (om_machine*)malloc(sizeof(om_machine));
   for (uint64_t i = j->lo; i < j->hi; i++)
-    oracle_run_prefix(j->cfg, j->ext, j->n_ext, j->p, j->p->seed_base + (int64_t)i,
+    oracle_run_prefix(j->cfg, j->ext, j->n_ext, j->p, jr_seed_at(j->p->seed_base, i),
                       &j->out[i], 0, 0, 0, 0, m);
   free(m);
   return 0;
@@ -66,6 +66,11 @@ int oracle_fuzz_trace(const demi_config* cfg, const demi_ext_event* ext, uint32_
 }
 
 /* ------------------------------------------------------------------- KATs */
+uint64_t oracle_jr_rejections;
+uint64_t oracle_jrandom_rejections(void) { return __atomic_load_n(&oracle_jr_rejections, __ATOMIC_RELAXED); }
+void oracle_jrandom_reset_rejections(void) { __atomic_store_n(&oracle_jr_rejections, 0, __ATOMIC_RELAXED); }
+
+
 /* java.util.Random: out[i] = nextInt() if bound <= 0 else nextInt(bound) */
 void oracle_kat_jrandom(int64_t seed, int32_t bound, int32_t n, int32_t* out) {
   jrandom r; jr_seed(&r, seed);

@@ -13,6 +13,15 @@
 
 typedef struct { uint64_t s; } jrandom;
 
+/* Redraws of nextInt(bound)'s rejection loop since the last oracle_jrandom_reset_rejections(), over every generator
+ * and thread of the library (fuzz.c).  Tests read it to show that a crafted seed took the loop.  It is counted on the
+ * loop's body only, which runs about once in 10^9 draws at this project's bounds. */
+extern uint64_t oracle_jr_rejections;
+
+/* The seed of execution `off` of a batch at `base`.  Java's long addition wraps, and only the low 48 bits reach the
+ * generator, so the sum is taken in uint64_t: int64_t addition would be undefined past INT64_MAX. */
+static inline int64_t jr_seed_at(int64_t base, uint64_t off) { return (int64_t)((uint64_t)base + off); }
+
 #define JR_MULT 0x5DEECE66DULL
 #define JR_ADD  0xBULL
 #define JR_MASK ((1ULL << 48) - 1)
@@ -36,6 +45,7 @@ static inline int32_t jr_next_int_bound(jrandom* r, int32_t bound) {
   int32_t u = v;
   /* (u - (v = u % bound) + m) overflows to negative => reject */
   while ((int32_t)((uint32_t)u - (uint32_t)(v = u % bound) + (uint32_t)m) < 0) {
+    __atomic_fetch_add(&oracle_jr_rejections, 1, __ATOMIC_RELAXED);
     u = jr_next(r, 31);
   }
   return v;

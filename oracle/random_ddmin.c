@@ -30,7 +30,7 @@ static void random_test(const demi_config* cfg, const demi_ext_event* ext, uint3
   out->executions_run = (uint32_t)p->n_prefixes;
   for (uint32_t j = 0; j < (uint32_t)p->n_prefixes; j++) {
     demi_fuzz_result r;
-    oracle_run_prefix(cfg, buf, n, p, p->seed_base + (int64_t)j, &r, NULL, 0, NULL, 0, scratch);
+    oracle_run_prefix(cfg, buf, n, p, jr_seed_at(p->seed_base, j), &r, NULL, 0, NULL, 0, scratch);
     if (r.status && !out->status) out->status = r.status;
     if (!r.status && r.violation) { out->first_hit = (int32_t)j; out->executions_run = j + 1; out->violation = r.violation; return; }
   }

@@ -38,6 +38,16 @@ def load_model(blob):
         raise RuntimeError("oracle_load_model: %d" % rc)
 
 
+def jrandom_rejections():
+    """Redraws of nextInt(bound)'s rejection loop in this library since reset_jrandom_rejections()."""
+    lib().oracle_jrandom_rejections.restype = C.c_uint64
+    return int(lib().oracle_jrandom_rejections())
+
+
+def reset_jrandom_rejections():
+    lib().oracle_jrandom_reset_rejections()
+
+
 def set_user_filter(rules):
     arr = np.ascontiguousarray(np.array(list(rules), dtype=np.uint32).reshape(-1, 4))
     lib().oracle_set_user_filter(C.c_void_p(arr.ctypes.data) if len(arr) else None, len(arr))
