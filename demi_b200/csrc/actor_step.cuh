@@ -45,9 +45,9 @@ struct TimerTable {
 // DYNAMIC_TIMERS: a key's index in the table is its slot.  A slot is live while it is in the machine's registry or
 // cancelled mask or in `held`; any other slot is free and is reused, so a slot number means nothing outside the
 // execution and must never reach a result, a hash, a recorded event or an ordering.  `held` are the slots a machine
-// has queued for its next flush (K2's messagesToSend; K3F sends a fired timer at once and holds none): timer_queued()
-// adds one, timer_flushed() drops them all when the queue has been emptied.  A copy that cancel() takes out of the
-// queue stays held until that flush, which costs nothing but the slot.
+// has queued for its next flush (K2's messagesToSend; K3 and K3F send a fired timer at once and hold none):
+// timer_queued() adds one, timer_flushed() drops them all when the queue has been emptied.  A copy that cancel() takes
+// out of the queue stays held until that flush, which costs nothing but the slot.
 // Bound: registry and cancelled hold at most DEMI_TIMERSET_CAP (16) slots each, and between two flushes lies one
 // delivery, which queues at most one re-arm and DEMI_IR_OUTBOX (16) scheduled timers: 16 + 16 + 17 = 49 live slots at
 // most, so a table of 64 never fills and the capacity that ends an execution is always one of the reference's.

@@ -1,6 +1,7 @@
 // capi_dpor.cu — C ABI for batched DPORwHeuristics searches (K3), the edit-distance bounded / resumable
 // configuration of RunnerUtils.editDistanceDporDDMin, and IncrementalDDMin on top of it.
 #include "dpor_kernel.cuh"
+#include "models/model_ir.cuh"
 #include "engine.hpp"
 #include "ddmin_driver.hpp"
 
@@ -13,8 +14,15 @@ static DporVariant make_dv() {
   using M = DporMachine<MODEL, BD>;
   return DporVariant{MODEL::ID, BD, dpor_kernel<MODEL, BD>, (size_t)M::WORDS * BD * sizeof(uint32_t), M::NQ};
 }
+// A loaded model (IrModel) has the geometry of DEMI_IR_ACTORS actors, whatever it loads: 16 x 8 state words and a
+// staged outbox of 16 x 3 words per search (22 528 B of shared memory per block of 32), and NQ = 17 * 16 FIFOs per
+// search in HBM.  The canonical order of getPendingEvent (the scan over q = src * 16 + dst, deadLetters in row 16) is
+// the oracle's (src * DEMI_MAX_ACTORS + dst, deadLetters in row n_actors): no queue whose sender or receiver lies in
+// [n_actors, 16) ever holds a message, because the interpreter drops a SEND to such an index and every external is
+// range-checked against the loaded actor count, so both scans meet the non-empty queues in the same order.
 static const DporVariant* pick_dv(int model) {
-  static const std::vector<DporVariant> v = { make_dv<PingPong3, 32>(), make_dv<Raft5, 32>(), make_dv<Bcast32, 32>() };
+  static const std::vector<DporVariant> v = { make_dv<PingPong3, 32>(), make_dv<Raft5, 32>(), make_dv<Bcast32, 32>(),
+                                              make_dv<IrModel, 32>() };
   for (const DporVariant& d : v) if (d.model == model) return &d;
   return nullptr;
 }
@@ -151,6 +159,7 @@ int32_t dpor_run(demi_handle* h, const demi_ext_event* ext, const uint32_t* ext_
   a.init_nodes = (const uint4*)d_sn; a.n_init_nodes = (uint32_t)n_seed_nodes;
   a.init_trace = (const uint32_t*)d_st; a.n_init_trace = (uint32_t)n_seed_trace;
   a.orig_index = (const int32_t*)d_oi;
+  if (e == cudaSuccess && h->cfg.model == DEMI_MODEL_IR) e = ir_bind(h->ir_dev, h->stream);   // this unit's copy of g_ir
   // the race scan's position table goes to shared memory when it leaves room for >= 8 blocks per SM
   size_t smem = dv->smem;
   const size_t scan_bytes = (size_t)a.T1 * dv->bd * sizeof(uint32_t);
@@ -185,6 +194,7 @@ extern "C" int32_t demi_dpor_batch_ex(demi_handle* h, const demi_ext_event* ext,
   if (!h) return DEMI_ERR_INVALID;
   if (!ext || !ext_offsets || !params || !results) return fail(h, DEMI_ERR_INVALID, "demi_dpor_batch: null argument");
   if (n_searches == 0) return DEMI_OK;
+  { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
   SeedHost seed;
   const bool have_seed = ex && ex->seed;
   if (have_seed) { int32_t rc = build_seed(h, ex->seed, seed); if (rc != DEMI_OK) return rc; }
@@ -247,6 +257,7 @@ extern "C" int32_t demi_incremental_ddmin(demi_handle* h, const demi_ext_event* 
                                           uint64_t* mcs_mask, uint32_t mask_words, demi_incddmin_out* out) {
   if (!h) return DEMI_ERR_INVALID;
   if (!externals || !params || !mcs_mask || !out) return fail(h, DEMI_ERR_INVALID, "demi_incremental_ddmin: null argument");
+  { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
   if ((uint64_t)mask_words * 64 < n_externals) return fail(h, DEMI_ERR_INVALID, "mask_words too small");
   for (uint32_t i = 0; i < n_externals; i++)
     if (externals[i].kind != DEMI_EXT_START && externals[i].kind != DEMI_EXT_SEND)

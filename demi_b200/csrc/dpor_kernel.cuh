@@ -67,7 +67,7 @@ struct DporArgs {
 };
 
 template <class MODEL, int BD>
-struct DporMachine {
+struct DporMachine : TimerTable<MODEL> {
   using Model = MODEL;
   static constexpr int BLOCK = BD;
   static constexpr int N = MODEL::N_ACTORS;
@@ -86,7 +86,8 @@ struct DporMachine {
   uint16_t qlen[NQ];            // local memory (small)
   uint32_t n_nodes, n_explored, n_heap, n_traces, found;
   int32_t max_distance;         // setMaxDistance (:128-134); < 0 = no cap
-  uint32_t registry, cancelled, isolated;
+  typename TimerTable<MODEL>::mask_t registry, cancelled;
+  uint32_t isolated;
   uint32_t parent_event, current_depth, cur_len, next_len, next_pos;
   int32_t nsched;
   uint32_t status;
@@ -133,7 +134,7 @@ struct DporMachine {
   // that flag only in ExternalEventInjector.handle_timer (ExternalEventInjector.scala:283-285), which DPOR never calls
   __device__ __forceinline__ void enqueue_timer(uint32_t slot) {
     uint32_t dst, type, p0, p1;
-    MODEL::slot_msg(slot, dst, type, p0, p1);
+    timer_msg(*this, slot, dst, type, p0, p1);
     event_produced(DEMI_DEADLETTERS, dst, type, p0, p1);
   }
   __device__ __forceinline__ void queue_remove(uint32_t q, uint32_t i) {
@@ -276,7 +277,7 @@ struct DporMachine {
 
   __device__ __forceinline__ uint32_t run_interleaving(uint32_t ext_lo, uint32_t ext_hi) {
     actor_init(*this);
-    registry = cancelled = 0;
+    registry = cancelled = 0; timer_reset(*this);
     for (int q = 0; q < NQ; q++) qlen[q] = 0;
     isolated = (N >= 32) ? 0xFFFFFFFFu : ((1u << N) - 1u);
     cur_len = 0; cur_trace[cur_len++] = 0;                                       // currentTrace += root :343

@@ -5,8 +5,9 @@
 // dropped here, before any engine sees it; more than DEMI_IR_OUTBOX operations in one receive() set the outbox's
 // overflow flag, which every engine reports as its queue-overflow status.  Timers are available through the outbox like in any model.  A
 // loaded program can arm any (type, p0, p1), so the model has no compile-time timer numbering: DYNAMIC_TIMERS makes
-// replay (K2) and frontier DPOR (K3F) intern the keys per execution (TimerTable, actor_step.cuh); timer_slot stays −1
-// for the lane fuzz engine, which hands a loaded model that arms timers to the general warp engine.
+// replay (K2), DPOR batches and IncrementalDDMin (K3) and frontier DPOR (K3F) intern the keys per execution
+// (TimerTable, actor_step.cuh); timer_slot stays −1 for the lane fuzz engine, which hands a loaded model that arms
+// timers to the general warp engine.
 #pragma once
 #include "../machine.cuh"
 #include "../../../include/demi_model_ir.h"
@@ -28,7 +29,7 @@ struct IrModel {
   static constexpr int LANE_OUTBOX = DEMI_IR_OUTBOX;
   static constexpr int REPLAY_OUTBOX = DEMI_IR_OUTBOX;
   static constexpr bool REPLAY_DIRECT = false;    // a loaded program can overflow the outbox: DEMI_PS_QUEUE_OVF is observable
-  static constexpr bool DYNAMIC_TIMERS = true;    // a loaded program arms any (type, p0, p1): replay and frontier DPOR intern the keys
+  static constexpr bool DYNAMIC_TIMERS = true;    // a loaded program arms any (type, p0, p1): replay and DPOR intern the keys
 
   __device__ static __forceinline__ uint32_t init_word(uint32_t i, uint32_t) {
     const uint32_t a = i / STATE_WORDS, w = i % STATE_WORDS;

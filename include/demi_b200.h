@@ -199,9 +199,10 @@ void    demi_destroy(demi_handle* h);
  * is what stands in for "the application's receive()" (Instrumenter.scala:913-1017) and `setInvariant`
  * (TestOracle.scala:27) when the host's application is not one of the compiled models.  The blob is copied.
  * A loaded model may use timers in every entry point that takes one (fuzzing, replay, DDMin, internal and wildcard
- * minimization, frontier DPOR), within the limits of the compiled models: 16 repeating timers registered and 16
- * cancelled timers not yet dropped per execution, then DEMI_PS_QUEUE_OVF / DEMI_DS_QUEUE_OVF.  A call that fails, for
- * any reason, leaves the handle as it was: the previously loaded model, if any, stays loaded. */
+ * minimization, frontier DPOR, DPOR batches and IncrementalDDMin), within the limits of the compiled models: 16
+ * repeating timers registered and 16 cancelled timers not yet dropped per execution, then DEMI_PS_QUEUE_OVF /
+ * DEMI_DS_QUEUE_OVF.  A call that fails, for any reason, leaves the handle as it was: the previously loaded model, if
+ * any, stays loaded. */
 int32_t demi_load_model(demi_handle* h, const void* model_blob, size_t size);
 /* The name table: the reference addresses actors by name (Scheduler.scala:13-104: blockedActors: Set[String], ...),
  * the C ABI by index.  Built-in models name their actors "0", "1", ...; a loaded model brings its own names. */
