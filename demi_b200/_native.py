@@ -54,6 +54,11 @@ class DDMinOut(C.Structure):
                 ("reserved", C.c_uint32 * 2)]
 
 
+DDMIN_OUT_DTYPE = np.dtype([("mcs_size", "<u4"), ("total_replays", "<u4"), ("n_iterations", "<u4"),
+                            ("replays_executed", "<u4"), ("batches", "<u4"), ("verified", "<u4"), ("reserved", "<u4", (2,))])
+assert DDMIN_OUT_DTYPE.itemsize == C.sizeof(DDMinOut)
+
+
 class IntMinOut(C.Structure):
     _fields_ = [("n_events", C.c_uint32), ("deliveries_before", C.c_uint32), ("deliveries_after", C.c_uint32),
                 ("total_replays", C.c_uint32), ("n_internal_sizes", C.c_uint32), ("unignorable", C.c_uint32),
@@ -123,6 +128,7 @@ EXPORTS = [
     "demi_set_clock_rules", "demi_wildcard_replay_batch", "demi_wildcard_replay_trace", "demi_wildcard_minimize",
     "demi_set_fuzzer", "demi_fuzz_campaign", "demi_fuzz_campaign_dev",
     "demi_random_test_batch", "demi_random_ddmin", "demi_random_test_trace",
+    "demi_fuzz_traces", "demi_set_traces", "demi_replay_batch_many", "demi_ddmin_many",
 ]
 FILTER_RULE_DTYPE = np.dtype([("src_mask", "<u4"), ("dst_mask", "<u4"), ("type_mask", "<u4"), ("flags", "<u4")])
 FRULE_DEADLETTERS = 1
@@ -310,6 +316,14 @@ def lib():
     L.demi_random_test_trace.restype = C.c_int32
     L.demi_random_test_trace.argtypes = [vp, vp, C.c_uint32, C.POINTER(FuzzParams), C.c_int64, vp, C.c_uint32,
                                          C.POINTER(C.c_uint32), vp]
+    L.demi_fuzz_traces.restype = C.c_int32
+    L.demi_fuzz_traces.argtypes = [vp, C.POINTER(FuzzParams), vp, C.c_uint32, vp, C.c_uint32, vp, vp]
+    L.demi_set_traces.restype = C.c_int32
+    L.demi_set_traces.argtypes = [vp, C.c_uint32, vp, vp, vp, vp, vp, vp]
+    L.demi_replay_batch_many.restype = C.c_int32
+    L.demi_replay_batch_many.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp]
+    L.demi_ddmin_many.restype = C.c_int32
+    L.demi_ddmin_many.argtypes = [vp, vp, C.c_uint32, C.c_int32, vp, C.c_uint32, vp, C.c_uint32, vp, vp]
     L.demi_stats.restype = C.c_int32
     L.demi_stats.argtypes = [vp, C.POINTER(Perf)]
     L.demi_lane_kernel.restype = C.c_int32

@@ -785,6 +785,95 @@ extern "C" int32_t demi_fuzz_provenance(demi_handle* h, const demi_fuzz_params* 
   return DEMI_OK;
 }
 
+// The EventTraces of executions seed_base + prefix_index[i], recorded as demi_fuzz_provenance records them (the lane
+// engine first, the slots it defers on the general engine) without the dep tree: the events of execution i go to
+// events + i*cap_events, its count to n_events[i] and its record to results[i] (may be NULL).
+extern "C" int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, const uint32_t* prefix_index, uint32_t n,
+                                    demi_event* events, uint32_t cap_events, uint32_t* n_events, demi_fuzz_result* results) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
+  if (!n) return DEMI_OK;
+  if (!prefix_index || !events || !cap_events || !n_events)
+    return fail(h, DEMI_ERR_INVALID, "demi_fuzz_traces: prefix_index, events, cap_events and n_events are required");
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  // bound the per-slot recording buffers to ~4 GB per launch: larger requests run in chunks
+  const size_t per_slot = (size_t)cap_events * sizeof(demi_event) + 2 + 16 + sizeof(demi_fuzz_result) + 4;
+  const uint32_t chunk = (uint32_t)std::max<size_t>(1, ((size_t)4 << 30) / per_slot);
+  int32_t rc;
+  uint32_t launches = 0;
+  float ms_all = 0.f;
+  int64_t bad = -1;
+  uint32_t bad_status = 0;
+  std::vector<demi_fuzz_result> res;
+  std::vector<uint32_t> cnt;
+  for (uint32_t off = 0; off < n; off += chunk) {
+    const uint32_t m = std::min(chunk, n - off);
+    demi_fuzz_params q = *p;
+    q.n_prefixes = m;
+    LaunchPlan plan;
+    if ((rc = plan_launch(h, &q, LM_RECORD, h->ext_info, h->ext_dev.get<demi_ext_event>(), (uint32_t)h->ext_host.size(), &plan)) != DEMI_OK)
+      return rc;
+    // events | parents (one entry per slot: the tree is not returned) | counts | results | work list | its length
+    const size_t b_ev = (size_t)m * cap_events * sizeof(demi_event), b_par = (((size_t)m * 2) + 15) & ~(size_t)15,
+                 b_cnt = (size_t)m * 16, b_res = (size_t)m * sizeof(demi_fuzz_result), b_idx = (((size_t)m * 4) + 15) & ~(size_t)15;
+    DevBuf tmp;
+    if ((rc = tmp.grow(h, b_ev + b_par + b_cnt + b_res + b_idx + 16)) != DEMI_OK) return rc;
+    unsigned char* buf = tmp.get<unsigned char>();
+    unsigned char* d_par = buf + b_ev; unsigned char* d_cnt = d_par + b_par; unsigned char* d_res = d_cnt + b_cnt;
+    unsigned char* d_idx = d_res + b_res; unsigned char* d_n = d_idx + b_idx;
+    cudaStream_t s = h->stream;
+    CUDA_TRY(h, cudaMemcpyAsync(d_idx, prefix_index + off, (size_t)m * 4, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(h, cudaMemcpyAsync(d_n, &m, 4, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(h, cudaMemsetAsync(d_cnt, 0, b_cnt, s));
+    CUDA_TRY(h, cudaMemsetAsync(d_res, 0xFF, b_res, s));
+    CUDA_TRY(h, cudaEventRecord(h->ev0, s));
+    plan.args.results = (demi_fuzz_result*)d_res;
+    plan.args.index_list = (const uint32_t*)d_idx; plan.args.index_count = (const uint32_t*)d_n;
+    plan.args.rec_events = (demi_event*)buf; plan.args.rec_cap = cap_events;
+    plan.args.rec_counts = (uint32_t*)d_cnt;
+    plan.args.rec_parent = (uint16_t*)d_par; plan.args.rec_parent_cap = 1;
+    plan.args.sum_steps = nullptr; plan.args.n_violations = nullptr;
+    h->perf.kernel_launches = 0;
+    if ((rc = launch_plan(h, plan, m, s)) != DEMI_OK) return rc;
+    launches += h->perf.kernel_launches;
+    CUDA_TRY(h, cudaEventRecord(h->ev1, s));
+    res.resize(m); cnt.resize((size_t)m * 4);
+    CUDA_TRY(h, cudaMemcpyAsync(cnt.data(), d_cnt, b_cnt, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(h, cudaMemcpyAsync(res.data(), d_res, b_res, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(h, cudaStreamSynchronize(s));
+    float ms = 0.f;
+    CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+    ms_all += ms;
+    // the events travel as rows as wide as the longest successful recording; a failing execution's partial recording
+    // is zeroed first, so that it returns no events
+    uint32_t width = 0;
+    for (uint32_t i = 0; i < m; i++) {
+      n_events[off + i] = cnt[(size_t)i * 4];
+      if (results) results[off + i] = res[i];
+      if (res[i].status) {
+        if (bad < 0) { bad = off + i; bad_status = res[i].status; }
+        CUDA_TRY(h, cudaMemsetAsync(buf + (size_t)i * cap_events * sizeof(demi_event), 0, (size_t)cap_events * sizeof(demi_event), s));
+      } else {
+        width = std::max(width, std::min(cnt[(size_t)i * 4], cap_events));
+      }
+    }
+    if (width) {
+      const size_t pitch = (size_t)cap_events * sizeof(demi_event);
+      CUDA_TRY(h, cudaMemcpy2DAsync(events + (size_t)off * cap_events, pitch, buf, pitch, (size_t)width * sizeof(demi_event), m,
+                                    cudaMemcpyDeviceToHost, s));
+      CUDA_TRY(h, cudaStreamSynchronize(s));
+    }
+  }
+  h->perf.kernel_launches = launches;
+  h->perf.prefixes = n;
+  h->perf.kernel_ms = ms_all;
+  // as demi_fuzz_trace fails for that seed; every record is filled all the same
+  if (bad >= 0)
+    return fail(h, DEMI_ERR_CAPACITY, "demi_fuzz_traces: execution %lld (prefix %u) status %u", (long long)bad,
+                prefix_index[bad], bad_status);
+  return DEMI_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Campaigns: RunnerUtils.fuzz's loop (RunnerUtils.scala:75-91) with a fresh Fuzzer program per execution.
 // Execution i runs program fuzzer_generate(program_seed_base + i) under FullyRandom(seed_base + i).

@@ -49,47 +49,62 @@ cudaError_t replay_ir_bind(const demi_handle* h, cudaStream_t s) {
   return h->cfg.model == DEMI_MODEL_IR ? ir_bind(h->ir_dev, s) : cudaSuccess;
 }
 
-extern "C" int32_t demi_set_trace(demi_handle* h, const demi_event* events, uint32_t n_events,
-                                  const demi_ext_event* externals, uint32_t n_externals) {
-  if (!h) return DEMI_ERR_INVALID;
+int32_t check_trace(demi_handle* h, const char* who, const demi_event* events, uint32_t n_events,
+                    const demi_ext_event* externals, uint32_t n_externals) {
   if (!events || !n_events || !externals || !n_externals)
-    return fail(h, DEMI_ERR_INVALID, "demi_set_trace: empty trace or externals");   // assume(!original_trace.isEmpty)
-  if (n_externals > 4096) return fail(h, DEMI_ERR_INVALID, "demi_set_trace: more than 4096 external events");
-  if (n_events >= (1u << 31)) return fail(h, DEMI_ERR_INVALID, "demi_set_trace: trace too long");
-  { int32_t vrc = demi_check_events(h, "demi_set_trace", events, n_events, 0); if (vrc != DEMI_OK) return vrc;
-    vrc = demi_check_externals(h, "demi_set_trace", externals, n_externals); if (vrc != DEMI_OK) return vrc; }   // (rejects HardKill)
-  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
+    return fail(h, DEMI_ERR_INVALID, "%s: empty trace or externals", who);   // assume(!original_trace.isEmpty)
+  if (n_externals > 4096) return fail(h, DEMI_ERR_INVALID, "%s: more than 4096 external events", who);
+  if (n_events >= (1u << 31)) return fail(h, DEMI_ERR_INVALID, "%s: trace too long", who);
+  int32_t vrc = demi_check_events(h, who, events, n_events, 0); if (vrc != DEMI_OK) return vrc;
+  return demi_check_externals(h, who, externals, n_externals);   // (rejects HardKill)
+}
+
+int32_t trace_tables(demi_handle* h, const char* who, const demi_event* events, uint32_t n_events,
+                     const demi_ext_event* externals, uint32_t n_externals, TraceTables& t) {
   const uint32_t ext_mask = demi_ext_type_mask(h);
   // FIFO correspondence of external MsgSends and original Sends (EventTrace.scala:385-386, :419-436)
-  std::vector<uint16_t> ordinal(n_events, 0xFFFF);
+  t.ordinal.assign(n_events, 0xFFFF);
   std::map<uint32_t, uint16_t> uniq_to_ord;
   uint32_t ord = 0, max_uniq = 0, n_send_events = 0;
   for (uint32_t i = 0; i < n_events; i++) {
     const demi_event& e = events[i];
     if (e.kind < DEMI_EV_MSG_SEND || e.kind > DEMI_EV_QUIESCENCE)
-      return fail(h, DEMI_ERR_INVALID, "demi_set_trace: event %u has unknown kind %u", i, e.kind);
+      return fail(h, DEMI_ERR_INVALID, "%s: event %u has unknown kind %u", who, i, e.kind);
     if (e.kind == DEMI_EV_MSG_SEND) {
       n_send_events++;
       if (e.uniq > max_uniq) max_uniq = e.uniq;
       if (demi_type_is_external(ext_mask, e.type)) {
-        if (ord >= 0xFFFF) return fail(h, DEMI_ERR_INVALID, "demi_set_trace: too many external sends");
-        ordinal[i] = (uint16_t)ord; uniq_to_ord[e.uniq] = (uint16_t)ord; ord++;
+        if (ord >= 0xFFFF) return fail(h, DEMI_ERR_INVALID, "%s: too many external sends", who);
+        t.ordinal[i] = (uint16_t)ord; uniq_to_ord[e.uniq] = (uint16_t)ord; ord++;
       }
     }
   }
   for (uint32_t i = 0; i < n_events; i++)
     if (events[i].kind == DEMI_EV_MSG_EVENT) {
       auto it = uniq_to_ord.find(events[i].uniq);
-      if (it != uniq_to_ord.end()) ordinal[i] = it->second;
+      if (it != uniq_to_ord.end()) t.ordinal[i] = it->second;
       if (events[i].uniq > max_uniq) max_uniq = events[i].uniq;
     }
-  std::vector<uint16_t> sidx;
-  for (uint32_t i = 0; i < n_externals; i++) if (externals[i].kind == DEMI_EXT_SEND) sidx.push_back((uint16_t)i);
-  DevBuf ext_dev, ord_dev, sidx_dev, trace_dev;
+  t.sidx.clear();
+  for (uint32_t i = 0; i < n_externals; i++) if (externals[i].kind == DEMI_EXT_SEND) t.sidx.push_back((uint16_t)i);
+  t.n_uniq = max_uniq + 1;
+  t.n_send_events = n_send_events;
+  return DEMI_OK;
+}
+
+extern "C" int32_t demi_set_trace(demi_handle* h, const demi_event* events, uint32_t n_events,
+                                  const demi_ext_event* externals, uint32_t n_externals) {
+  if (!h) return DEMI_ERR_INVALID;
+  { int32_t vrc = check_trace(h, "demi_set_trace", events, n_events, externals, n_externals); if (vrc != DEMI_OK) return vrc; }
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
+  TraceTables t;
   int32_t rc;
+  if ((rc = trace_tables(h, "demi_set_trace", events, n_events, externals, n_externals, t)) != DEMI_OK) return rc;
+  const std::vector<uint16_t>& sidx = t.sidx;
+  DevBuf ext_dev, ord_dev, sidx_dev, trace_dev;
   if ((rc = ext_dev.upload(h, externals, n_externals * sizeof(demi_ext_event))) != DEMI_OK) return rc;
-  if ((rc = ord_dev.upload(h, ordinal.data(), n_events * sizeof(uint16_t))) != DEMI_OK) return rc;
+  if ((rc = ord_dev.upload(h, t.ordinal.data(), n_events * sizeof(uint16_t))) != DEMI_OK) return rc;
   if ((rc = sidx_dev.grow(h, std::max<size_t>(sidx.size(), 1) * sizeof(uint16_t))) != DEMI_OK) return rc;
   if (!sidx.empty())
     CUDA_TRY(h, cudaMemcpy(sidx_dev.get(), sidx.data(), sidx.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
@@ -99,8 +114,8 @@ extern "C" int32_t demi_set_trace(demi_handle* h, const demi_event* events, uint
   h->trace_ext_host.assign(externals, externals + n_externals);
   h->send_ext_index_host = sidx;
   h->conjoined.assign(n_externals, -1);                       // a new EventDag has no conjoined atoms
-  h->trace_n_uniq = max_uniq + 1;
-  h->trace_n_send_events = n_send_events;
+  h->trace_n_uniq = t.n_uniq;
+  h->trace_n_send_events = t.n_send_events;
   h->trace_n_ext_sends = (uint32_t)sidx.size();
   h->trace_dev = std::move(trace_dev); h->trace_ext_dev = std::move(ext_dev);
   h->ev_ordinal_dev = std::move(ord_dev); h->send_ext_index_dev = std::move(sidx_dev);
@@ -128,6 +143,34 @@ extern "C" int32_t demi_replay_batch_dev(demi_handle* h, const void* masks_dev, 
   if (!h) return DEMI_ERR_INVALID;
   if (!masks_dev) return fail(h, DEMI_ERR_INVALID, "demi_replay_batch_dev: null buffer");
   return launch_replay(h, masks_dev, nullptr, n_masks, mask_words, looking_for, flags, out_dev, stream, nullptr, 0, nullptr);
+}
+
+// The per-warp scratch of a K2 launch of `warps` warps with a's geometry (table_slots, tosend_cap, n_uniq_words, flags),
+// its first generation and its counters, all in a.  Generation stamps: each launch gets a fresh range [gen_base,
+// gen_base + tests per thread]; the table is cleared only when it was (re)allocated, its geometry changed, or the
+// 16-bit range is exhausted.
+int32_t replay_scratch(demi_handle* h, ReplayArgs& a, uint64_t warps, int n_actors, uint32_t per_thread, bool record,
+                       cudaStream_t s) {
+  int32_t rc;
+  const size_t table_bytes = warps * a.table_slots * 32 * sizeof(uint4);
+  const bool fresh_table = h->rp_table.bytes() < table_bytes;
+  if ((rc = h->rp_table.grow(h, table_bytes)) != DEMI_OK) return rc;
+  if ((rc = h->rp_tosend.grow(h, warps * a.tosend_cap * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
+  if (a.flags & DEMI_RF_FILTER_KNOWN_ABSENTS)
+    if ((rc = h->rp_pruned.grow(h, warps * (a.n_uniq_words + n_actors) * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
+  const uint64_t geometry = ((uint64_t)a.table_slots << 32) ^ warps;
+  if (fresh_table || h->rp_gen_next == 0 || h->rp_table_geometry != geometry || h->rp_gen_next + per_thread >= 0xFFF0u || record) {
+    CUDA_TRY(h, cudaMemsetAsync(h->rp_table.get(), 0, table_bytes, s));
+    h->rp_gen_next = 1;
+    h->rp_table_geometry = geometry;
+  }
+  a.gen_base = h->rp_gen_next;
+  h->rp_gen_next = record ? 0 : h->rp_gen_next + per_thread;   // the recording variant leaves list entries behind: clear next time
+  CUDA_TRY(h, cudaMemsetAsync(h->rp_counters.get(), 0, 2 * sizeof(unsigned long long), s));
+  a.table = h->rp_table.get<uint4>(); a.tosend = h->rp_tosend.get<uint32_t>();
+  a.pruned = (a.flags & DEMI_RF_FILTER_KNOWN_ABSENTS) ? h->rp_pruned.get<uint32_t>() : nullptr;
+  a.counters = h->rp_counters.get<unsigned long long>();
+  return DEMI_OK;
 }
 
 static int32_t launch_replay(demi_handle* h, const void* masks_dev, const void* skips_dev, uint32_t n_masks, uint32_t mask_words,
@@ -162,27 +205,8 @@ static int32_t launch_replay(demi_handle* h, const void* masks_dev, const void* 
   a.pending_cap = demi_replay_pending_cap(h->trace_n_send_events);
   a.tosend_cap = demi_tosend_cap(h->trace_n_ext_sends);
   a.table_slots = demi_pow2_at_least(2 * a.pending_cap, 256, 1u << 16);
-  const size_t table_bytes = warps * a.table_slots * 32 * sizeof(uint4);
-  const bool fresh_table = h->rp_table.bytes() < table_bytes;
-  if ((rc = h->rp_table.grow(h, table_bytes)) != DEMI_OK) return rc;
-  if ((rc = h->rp_tosend.grow(h, warps * a.tosend_cap * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
-  if (flags & DEMI_RF_FILTER_KNOWN_ABSENTS)
-    if ((rc = h->rp_pruned.grow(h, warps * (a.n_uniq_words + rv->n_actors) * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
-  // Generation stamps: each launch gets a fresh range [gen_base, gen_base + tests per thread]; the table is
-  // cleared only when it was (re)allocated, its geometry changed, or the 16-bit range is exhausted.
   const uint32_t per_thread = (uint32_t)(((uint64_t)n_masks + (uint64_t)grid * rv->bd - 1) / ((uint64_t)grid * rv->bd)) + 1;
-  const uint64_t geometry = ((uint64_t)a.table_slots << 32) ^ warps;
-  if (fresh_table || h->rp_gen_next == 0 || h->rp_table_geometry != geometry || h->rp_gen_next + per_thread >= 0xFFF0u || record) {
-    CUDA_TRY(h, cudaMemsetAsync(h->rp_table.get(), 0, table_bytes, s));
-    h->rp_gen_next = 1;
-    h->rp_table_geometry = geometry;
-  }
-  a.gen_base = h->rp_gen_next;
-  h->rp_gen_next = record ? 0 : h->rp_gen_next + per_thread;   // the recording variant leaves list entries behind: clear next time
-  CUDA_TRY(h, cudaMemsetAsync(h->rp_counters.get(), 0, 2 * sizeof(unsigned long long), s));
-  a.table = h->rp_table.get<uint4>(); a.tosend = h->rp_tosend.get<uint32_t>();
-  a.pruned = (flags & DEMI_RF_FILTER_KNOWN_ABSENTS) ? h->rp_pruned.get<uint32_t>() : nullptr;
-  a.counters = h->rp_counters.get<unsigned long long>();
+  if ((rc = replay_scratch(h, a, warps, rv->n_actors, per_thread, record, s)) != DEMI_OK) return rc;
   CUDA_TRY(h, replay_ir_bind(h, s));
   rv->fn[0][record]<<<record ? 1 : grid, rv->bd, rv->smem, s>>>(a);
   CUDA_TRY(h, cudaGetLastError());
@@ -303,19 +327,10 @@ struct StsDDMinDriver : DDMinDriver {
 
 }  // namespace
 
-extern "C" int32_t demi_ddmin(demi_handle* h, uint32_t looking_for, uint32_t flags, int32_t check_unmodified,
-                              uint64_t* mcs_mask, uint32_t mask_words,
-                              uint32_t* iteration_sizes, uint32_t cap_iterations, demi_ddmin_out* out) {
-  if (!h) return DEMI_ERR_INVALID;
-  if (!mcs_mask || !out) return fail(h, DEMI_ERR_INVALID, "demi_ddmin: null output");
-  if (h->trace_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_trace has not been called");
-  const uint32_t n_ext = (uint32_t)h->trace_ext_host.size();
-  if (mask_words * 64 < n_ext) return fail(h, DEMI_ERR_INVALID, "mask_words too small");
-  memset(out, 0, sizeof(*out));
-  StsDDMinDriver d;
-  d.h = h; d.looking_for = looking_for; d.flags = flags; d.mw = mask_words; d.n_ext = n_ext;
-  d.ext = h->trace_ext_host.data();
-  d.conjoined = &h->conjoined;
+int32_t ddmin_sts(DDMinDriver& d, int32_t check_unmodified, uint64_t* mcs_mask, uint32_t* iteration_sizes,
+                  uint32_t cap_iterations, demi_ddmin_out* out) {
+  demi_handle* h = d.h;
+  const uint32_t mask_words = d.mw, n_ext = d.n_ext;
   // tests per speculative batch: a launch costs ~3 ms of latency whatever its size (one test walks the whole trace),
   // building a batch ~0.2 us per test on the host; ~6000 tests = five to six levels of the decision tree per launch
   d.wide_cap = getenv("DEMI_DDMIN_WIDE") ? (size_t)atol(getenv("DEMI_DDMIN_WIDE")) : 6000;
@@ -348,4 +363,20 @@ extern "C" int32_t demi_ddmin(demi_handle* h, uint32_t looking_for, uint32_t fla
   if (iteration_sizes)
     for (uint32_t i = 0; i < cap_iterations && i < out->n_iterations; i++) iteration_sizes[i] = d.iteration_sizes[i];
   return DEMI_OK;
+}
+
+extern "C" int32_t demi_ddmin(demi_handle* h, uint32_t looking_for, uint32_t flags, int32_t check_unmodified,
+                              uint64_t* mcs_mask, uint32_t mask_words,
+                              uint32_t* iteration_sizes, uint32_t cap_iterations, demi_ddmin_out* out) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!mcs_mask || !out) return fail(h, DEMI_ERR_INVALID, "demi_ddmin: null output");
+  if (h->trace_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_trace has not been called");
+  const uint32_t n_ext = (uint32_t)h->trace_ext_host.size();
+  if (mask_words * 64 < n_ext) return fail(h, DEMI_ERR_INVALID, "mask_words too small");
+  memset(out, 0, sizeof(*out));
+  StsDDMinDriver d;
+  d.h = h; d.looking_for = looking_for; d.flags = flags; d.mw = mask_words; d.n_ext = n_ext;
+  d.ext = h->trace_ext_host.data();
+  d.conjoined = &h->conjoined;
+  return ddmin_sts(d, check_unmodified, mcs_mask, iteration_sizes, cap_iterations, out);
 }

@@ -1,0 +1,370 @@
+// capi_replay_many.cu — STSSched replay and DDMin over a set of traces (demi_set_traces): the tests of many traces in
+// one K2 launch, and one DDMin per trace, their speculative batches served together.
+//
+// A minimisation of a small trace asks for tens to a few hundred tests at a time, a small fraction of one wave of the
+// replay kernel, and waits for each launch.  Here the drivers of many traces run side by side, each on a host thread
+// with a rendezvous: every driver in flight runs until it asks for an evaluation or finishes, then one launch evaluates
+// the union of their requests and each gets its own slice back.  A driver sees exactly the answers it would get alone,
+// so its decisions, MCS and counters do not depend on which other drivers share its launches.
+#include <atomic>
+#include <condition_variable>
+#include <mutex>
+#include <new>
+#include <system_error>
+#include <thread>
+#include "replay_kernel.cuh"
+#include "engine.hpp"
+#include "ddmin_driver.hpp"
+#include "models/model_ir.cuh"
+
+using namespace demi;
+
+namespace {
+
+typedef void (*replay_many_fn)(const ReplayArgs, const ReplayTraceView*, const uint4*, uint32_t, ReplayArgs*);
+struct ManyVariant { int model; int bd; replay_many_fn fn; size_t smem; int n_actors; };
+template <class MODEL, int BD>
+ManyVariant make_mv() {
+  using M = ReplayMachine<MODEL, BD>;
+  return ManyVariant{MODEL::ID, BD, replay_many_kernel<MODEL, BD>, (size_t)M::WORDS * BD * sizeof(uint32_t), MODEL::N_ACTORS};
+}
+// the block sizes of the single-trace kernels (capi_replay.cu)
+const ManyVariant* pick_mv(int model) {
+  static const std::vector<ManyVariant> v = {
+    make_mv<PingPong3, 256>(), make_mv<Raft5, 256>(), make_mv<Bcast32, 128>(), make_mv<IrModel, 128>(),
+  };
+  for (const ManyVariant& r : v) if (r.model == model) return &r;
+  return nullptr;
+}
+
+// tests per launch: larger unions are evaluated in several launches
+constexpr uint32_t MANY_MAX_TESTS = 1u << 20;
+// host threads demi_ddmin_many may run at once
+constexpr uint32_t MANY_MAX_WINDOW = 4096;
+
+struct LaunchCounts { uint32_t launches = 0; uint64_t tests = 0, violations = 0, deliveries = 0; double ms = 0; };
+
+// One K2 launch over tests [0, n) of the set: test i replays mask i on trace trace_of_test[i] (validated by the
+// caller).  Tests are grouped by trace into warp tiles, longest trace first; results come back in input order.
+int32_t launch_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks, uint32_t n, uint32_t mw,
+                    const uint32_t* looking_for, uint32_t flags, demi_replay_result* out, LaunchCounts& lc) {
+  const auto& S = h->set;
+  const ManyVariant* mv = pick_mv(h->cfg.model);
+  if (!mv) return fail(h, DEMI_ERR_INVALID, "no replay kernel for model %d", h->cfg.model);
+  // counting sort of the tests by the rank of their trace (longer traces first, then by index)
+  std::vector<uint32_t> count(S.n + 1, 0);
+  for (uint32_t i = 0; i < n; i++) count[trace_of_test[i]]++;
+  std::vector<uint32_t> order_t;
+  for (uint32_t t = 0; t < S.n; t++) if (count[t]) order_t.push_back(t);
+  std::stable_sort(order_t.begin(), order_t.end(), [&](uint32_t a, uint32_t b) { return S.n_events[a] > S.n_events[b]; });
+  std::vector<uint32_t> first(S.n, 0);
+  std::vector<uint4> tiles;
+  ReplayArgs a = replay_args(h, 0, flags);
+  a.table_slots = a.tosend_cap = a.n_uniq_words = a.pending_cap = 0;
+  uint32_t pos = 0;
+  for (uint32_t t : order_t) {
+    first[t] = pos;
+    for (uint32_t k = 0; k < count[t]; k += 32) tiles.push_back(make_uint4(t, pos + k, std::min(32u, count[t] - k), looking_for[t]));
+    pos += count[t];
+    a.table_slots = std::max(a.table_slots, S.table_slots[t]);
+    a.tosend_cap = std::max(a.tosend_cap, S.tosend_cap[t]);
+    a.n_uniq_words = std::max(a.n_uniq_words, S.n_uniq_words[t]);
+    a.pending_cap = std::max(a.pending_cap, S.pending_cap[t]);
+  }
+  std::vector<uint32_t> slot(n);                    // test i runs at position slot[i] of the grouped order
+  std::vector<uint64_t> grouped((size_t)n * mw);
+  for (uint32_t i = 0; i < n; i++) {
+    slot[i] = first[trace_of_test[i]]++;
+    std::copy(masks + (size_t)i * mw, masks + (size_t)(i + 1) * mw, grouped.begin() + (size_t)slot[i] * mw);
+  }
+  cudaStream_t s = h->stream;
+  int32_t rc;
+  int bps = 0;
+  if ((rc = demi_occupancy(h, (const void*)mv->fn, mv->bd, mv->smem, &bps)) != DEMI_OK) return rc;
+  if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
+  const uint32_t n_tiles = (uint32_t)tiles.size(), wpb = (uint32_t)mv->bd / 32;
+  const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((n_tiles + wpb - 1) / wpb, (uint64_t)h->sm_count * bps));
+  const uint64_t warps = (uint64_t)grid * wpb;
+  const uint32_t per_thread = (uint32_t)((n_tiles + warps - 1) / warps) + 1;
+  if ((rc = replay_scratch(h, a, warps, mv->n_actors, per_thread, false, s)) != DEMI_OK) return rc;
+  const size_t mbytes = grouped.size() * sizeof(uint64_t), tbytes = tiles.size() * sizeof(uint4);
+  const size_t rbytes = (size_t)n * sizeof(demi_replay_result);
+  if ((rc = h->rp_masks.grow(h, mbytes + tbytes)) != DEMI_OK) return rc;
+  if ((rc = h->rp_results.grow(h, rbytes)) != DEMI_OK) return rc;
+  if ((rc = h->rp_bound.grow(h, warps * sizeof(ReplayArgs))) != DEMI_OK) return rc;
+  char* base = h->rp_masks.get<char>();
+  CUDA_TRY(h, cudaMemcpyAsync(base, tiles.data(), tbytes, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(h, cudaMemcpyAsync(base + tbytes, grouped.data(), mbytes, cudaMemcpyHostToDevice, s));
+  a.masks = (const uint64_t*)(base + tbytes); a.n_masks = n; a.mask_words = mw;
+  a.results = h->rp_results.get<demi_replay_result>();
+  if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
+  CUDA_TRY(h, cudaEventRecord(h->ev0, s));
+  mv->fn<<<grid, mv->bd, mv->smem, s>>>(a, S.views.get<ReplayTraceView>(), (const uint4*)base, n_tiles, h->rp_bound.get<ReplayArgs>());
+  CUDA_TRY(h, cudaGetLastError());
+  CUDA_TRY(h, cudaEventRecord(h->ev1, s));
+  std::vector<demi_replay_result> res(n);
+  unsigned long long c[2] = {0, 0};
+  CUDA_TRY(h, cudaMemcpyAsync(res.data(), a.results, rbytes, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(c, a.counters, sizeof(c), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  float ms = 0;
+  CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+  for (uint32_t i = 0; i < n; i++) out[i] = res[slot[i]];
+  lc.launches++; lc.tests += n; lc.ms += ms; lc.violations += c[0]; lc.deliveries += c[1];
+  return DEMI_OK;
+}
+
+void set_perf(demi_handle* h, const LaunchCounts& lc) {
+  h->perf.kernel_launches = lc.launches; h->perf.prefixes = lc.tests; h->perf.kernel_ms = lc.ms;
+  h->perf.violations = lc.violations; h->perf.deliveries = lc.deliveries;
+}
+
+// n tests in launches of at most MANY_MAX_TESTS
+int32_t replay_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks, uint32_t n, uint32_t mw,
+                    const uint32_t* looking_for, uint32_t flags, demi_replay_result* out, LaunchCounts& lc) {
+  for (uint32_t off = 0; off < n; off += MANY_MAX_TESTS) {
+    const uint32_t m = std::min(MANY_MAX_TESTS, n - off);
+    const int32_t rc = launch_many(h, trace_of_test + off, masks + (size_t)off * mw, m, mw, looking_for, flags, out + off, lc);
+    if (rc != DEMI_OK) return rc;
+  }
+  return DEMI_OK;
+}
+
+// ---------------------------------------------------------------------- rounds of DDMin drivers
+// A driver's request for an evaluation: its masks (a slice of its arena, which stays put while it waits) and, once
+// served, their results or the launch's error.
+struct Request {
+  uint32_t trace; const uint64_t* masks; size_t n;
+  std::vector<demi_replay_result> res;
+  int32_t rc = DEMI_OK; bool done = false;
+};
+struct Rendezvous {
+  std::mutex mu;
+  std::condition_variable coord, work;
+  uint32_t running = 0;            // workers executing driver code; the others wait on a request or have left
+  std::vector<Request*> queue;
+};
+
+// STSSched as DDMin's TestOracle on trace `trace` of the set, as StsDDMinDriver (capi_replay.cu) on the single trace
+struct SetDDMinDriver : DDMinDriver {
+  Rendezvous* R; uint32_t trace;
+  int32_t ask(const uint64_t* masks, size_t n, signed char* out) {
+    Request q; q.trace = trace; q.masks = masks; q.n = n;
+    {
+      std::unique_lock<std::mutex> lk(R->mu);
+      R->queue.push_back(&q);
+      R->running--;
+      R->coord.notify_one();
+      R->work.wait(lk, [&] { return q.done; });
+    }
+    if (q.rc != DEMI_OK) return q.rc;
+    for (size_t i = 0; i < n; i++) {
+      if (q.res[i].status != 0) return fail(h, DEMI_ERR_CAPACITY, "demi_ddmin: a replay reported status %u", (unsigned)q.res[i].status);
+      out[i] = q.res[i].violation != 0;
+    }
+    return DEMI_OK;
+  }
+  int32_t evaluate_flat(const uint64_t* masks, size_t n, signed char* out) override { return ask(masks, n, out); }
+  int32_t evaluate_batch(const std::vector<Mask>& want, std::vector<char>& out) override {
+    std::vector<uint64_t> flat(want.size() * mw);
+    for (size_t i = 0; i < want.size(); i++) std::copy(want[i].begin(), want[i].end(), flat.begin() + i * mw);
+    std::vector<signed char> r(want.size(), 0);
+    const int32_t rc = ask(flat.data(), want.size(), r.data());
+    for (size_t i = 0; i < want.size(); i++) out[i] = r[i];
+    return rc;
+  }
+};
+
+}  // namespace
+
+extern "C" int32_t demi_set_traces(demi_handle* h, uint32_t n_traces,
+                                   const demi_event* events, const uint32_t* event_offsets, const uint32_t* n_events,
+                                   const demi_ext_event* externals, const uint32_t* ext_offsets, const uint32_t* n_externals) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!n_traces) return fail(h, DEMI_ERR_INVALID, "demi_set_traces: no traces");
+  if (!events || !event_offsets || !n_events || !externals || !ext_offsets || !n_externals)
+    return fail(h, DEMI_ERR_INVALID, "demi_set_traces: null buffer");
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
+  // the new set is built aside and replaces the old one only when every trace passed and every upload succeeded
+  std::vector<demi_event> ev_all; std::vector<uint16_t> ord_all, sidx_all; std::vector<demi_ext_event> ext_all;
+  std::vector<size_t> ev_off(n_traces), ext_off(n_traces), sidx_off(n_traces);
+  std::vector<uint32_t> n_sends(n_traces);
+  std::map<std::pair<uint32_t, uint32_t>, std::pair<size_t, size_t>> ext_seen;   // a program shared by traces is stored once
+  demi_handle::TraceSet S;
+  S.n = n_traces;
+  S.ext.resize(n_traces); S.n_events.resize(n_traces);
+  S.n_uniq_words.resize(n_traces); S.pending_cap.resize(n_traces); S.tosend_cap.resize(n_traces); S.table_slots.resize(n_traces);
+  char who[64];
+  TraceTables t;
+  for (uint32_t i = 0; i < n_traces; i++) {
+    snprintf(who, sizeof(who), "demi_set_traces: trace %u", i);
+    const demi_event* ev = events + event_offsets[i];
+    const demi_ext_event* ex = externals + ext_offsets[i];
+    int32_t rc = check_trace(h, who, ev, n_events[i], ex, n_externals[i]);
+    if (rc == DEMI_OK) rc = trace_tables(h, who, ev, n_events[i], ex, n_externals[i], t);
+    if (rc != DEMI_OK) return rc;
+    ev_off[i] = ev_all.size();
+    ev_all.insert(ev_all.end(), ev, ev + n_events[i]);
+    ord_all.insert(ord_all.end(), t.ordinal.begin(), t.ordinal.end());
+    auto key = std::make_pair(ext_offsets[i], n_externals[i]);
+    auto it = ext_seen.find(key);
+    if (it == ext_seen.end()) {
+      it = ext_seen.emplace(key, std::make_pair(ext_all.size(), sidx_all.size())).first;
+      ext_all.insert(ext_all.end(), ex, ex + n_externals[i]);
+      sidx_all.insert(sidx_all.end(), t.sidx.begin(), t.sidx.end());
+    }
+    ext_off[i] = it->second.first; sidx_off[i] = it->second.second;
+    n_sends[i] = (uint32_t)t.sidx.size();
+    S.ext[i].assign(ex, ex + n_externals[i]);
+    S.n_events[i] = n_events[i];
+    S.n_uniq_words[i] = (t.n_uniq + 31) / 32;
+    S.pending_cap[i] = demi_replay_pending_cap(t.n_send_events);
+    S.tosend_cap[i] = demi_tosend_cap(n_sends[i]);
+    S.table_slots[i] = demi_pow2_at_least(2 * S.pending_cap[i], 256, 1u << 16);
+  }
+  if (sidx_all.empty()) sidx_all.push_back(0);
+  int32_t rc;
+  if ((rc = S.events.upload(h, ev_all.data(), ev_all.size() * sizeof(demi_event))) != DEMI_OK) return rc;
+  if ((rc = S.ordinal.upload(h, ord_all.data(), ord_all.size() * sizeof(uint16_t))) != DEMI_OK) return rc;
+  if ((rc = S.externals.upload(h, ext_all.data(), ext_all.size() * sizeof(demi_ext_event))) != DEMI_OK) return rc;
+  if ((rc = S.send_index.upload(h, sidx_all.data(), sidx_all.size() * sizeof(uint16_t))) != DEMI_OK) return rc;
+  std::vector<ReplayTraceView> views(n_traces);
+  for (uint32_t i = 0; i < n_traces; i++) {
+    ReplayTraceView& v = views[i];
+    v.events = S.events.get<const uint4>() + ev_off[i]; v.ev_ordinal = S.ordinal.get<const uint16_t>() + ev_off[i];
+    v.ext = S.externals.get<const uint4>() + ext_off[i]; v.send_ext_index = S.send_index.get<const uint16_t>() + sidx_off[i];
+    v.n_events = n_events[i]; v.n_ext = n_externals[i]; v.n_sends = n_sends[i]; v.n_uniq_words = S.n_uniq_words[i];
+    v.pending_cap = S.pending_cap[i]; v.tosend_cap = S.tosend_cap[i]; v.table_slots = S.table_slots[i]; v.pad = 0;
+  }
+  if ((rc = S.views.upload(h, views.data(), views.size() * sizeof(ReplayTraceView))) != DEMI_OK) return rc;
+  if ((rc = h->rp_counters.grow(h, 2 * sizeof(unsigned long long))) != DEMI_OK) return rc;
+  h->set = std::move(S);
+  return DEMI_OK;
+}
+
+extern "C" int32_t demi_replay_batch_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks, uint32_t n_tests,
+                                          uint32_t mask_words, const uint32_t* looking_for, uint32_t flags,
+                                          demi_replay_result* out) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!trace_of_test || !masks || !looking_for || !out) return fail(h, DEMI_ERR_INVALID, "demi_replay_batch_many: null buffer");
+  if (!h->set.n) return fail(h, DEMI_ERR_STATE, "demi_set_traces has not been called");
+  for (uint32_t i = 0; i < n_tests; i++) {
+    const uint32_t t = trace_of_test[i];
+    if (t >= h->set.n) return fail(h, DEMI_ERR_INVALID, "demi_replay_batch_many: test %u names trace %u of %u", i, t, h->set.n);
+    if ((uint64_t)mask_words * 64 < h->set.ext[t].size())
+      return fail(h, DEMI_ERR_INVALID, "mask_words %u too small for the %zu externals of trace %u", mask_words, h->set.ext[t].size(), t);
+  }
+  if (n_tests == 0) return DEMI_OK;
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  LaunchCounts lc;
+  const int32_t rc = replay_many(h, trace_of_test, masks, n_tests, mask_words, looking_for, flags, out, lc);
+  set_perf(h, lc);
+  return rc;
+}
+
+extern "C" int32_t demi_ddmin_many(demi_handle* h, const uint32_t* looking_for, uint32_t flags, int32_t check_unmodified,
+                                   uint64_t* mcs_masks, uint32_t mask_words, uint32_t* iteration_sizes, uint32_t cap_iterations,
+                                   demi_ddmin_out* out, int32_t* status) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!looking_for || !mcs_masks || !out || !status) return fail(h, DEMI_ERR_INVALID, "demi_ddmin_many: null buffer");
+  const uint32_t n = h->set.n;
+  if (!n) return fail(h, DEMI_ERR_STATE, "demi_set_traces has not been called");
+  for (uint32_t t = 0; t < n; t++)
+    if ((uint64_t)mask_words * 64 < h->set.ext[t].size())
+      return fail(h, DEMI_ERR_INVALID, "mask_words %u too small for the %zu externals of trace %u", mask_words, h->set.ext[t].size(), t);
+  // drivers in flight: DEMI_DDMIN_MANY_WINDOW, 1..MANY_MAX_WINDOW (default 512); a thread that finishes a driver takes
+  // the next trace
+  uint32_t window = 512;
+  if (const char* w = getenv("DEMI_DDMIN_MANY_WINDOW")) {
+    char* end = nullptr;
+    const long v = strtol(w, &end, 10);
+    if (end == w || *end || v < 1 || v > (long)MANY_MAX_WINDOW)
+      return fail(h, DEMI_ERR_INVALID, "DEMI_DDMIN_MANY_WINDOW=%s: expected 1..%u", w, MANY_MAX_WINDOW);
+    window = (uint32_t)v;
+  }
+  window = std::min(window, n);
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  memset(out, 0, (size_t)n * sizeof(demi_ddmin_out));
+  Rendezvous R;
+  std::atomic<uint32_t> next{0};
+  std::vector<std::string> msg(n);
+  auto worker = [&]() {
+    // fail() records a message on the handle it is given: each worker's drivers get a handle of their own for that,
+    // so that the message of each failing trace is kept
+    demi_handle eh;
+    for (uint32_t t; (t = next.fetch_add(1)) < n;) {
+      try {
+        SetDDMinDriver d;
+        d.R = &R; d.trace = t;
+        d.h = &eh; d.looking_for = looking_for[t]; d.flags = flags; d.mw = mask_words;
+        d.n_ext = (uint32_t)h->set.ext[t].size(); d.ext = h->set.ext[t].data();
+        status[t] = ddmin_sts(d, check_unmodified, mcs_masks + (size_t)t * mask_words,
+                              iteration_sizes ? iteration_sizes + (size_t)t * cap_iterations : nullptr, cap_iterations, out + t);
+        if (status[t] != DEMI_OK) msg[t] = eh.err;
+      } catch (const std::bad_alloc&) {                // a driver out of host memory fails its trace alone
+        status[t] = DEMI_ERR_CAPACITY;
+        msg[t] = "demi_ddmin_many: out of host memory";
+      }
+    }
+    std::lock_guard<std::mutex> lk(R.mu);
+    R.running--;
+    R.coord.notify_one();
+  };
+  LaunchCounts lc;
+  int32_t call_rc = DEMI_OK;
+  std::string call_msg;
+  std::vector<std::thread> threads;
+  {
+    std::unique_lock<std::mutex> lk(R.mu);
+    // the workers are counted before any of them can take the lock; when the system refuses a thread, the ones already
+    // started carry the window (the results do not depend on it)
+    try {
+      threads.reserve(window);
+      for (uint32_t i = 0; i < window; i++) threads.emplace_back(worker);
+    } catch (const std::system_error&) {
+    } catch (const std::bad_alloc&) {
+    }
+    R.running = (uint32_t)threads.size();
+    if (threads.empty()) return fail(h, DEMI_ERR_CAPACITY, "demi_ddmin_many: could not start a worker thread");
+    for (;;) {
+      R.coord.wait(lk, [&] { return R.running == 0; });
+      if (R.queue.empty()) break;                  // no driver waits and none runs: every trace is done
+      std::vector<Request*> batch;
+      batch.swap(R.queue);
+      lk.unlock();
+      size_t total = 0;
+      for (const Request* q : batch) total += q->n;
+      std::vector<uint32_t> tr(total);
+      std::vector<uint64_t> flat(total * mask_words);
+      std::vector<demi_replay_result> res(total);
+      size_t k = 0;
+      for (const Request* q : batch) {
+        std::fill(tr.begin() + k, tr.begin() + k + q->n, q->trace);
+        std::copy(q->masks, q->masks + q->n * mask_words, flat.begin() + k * mask_words);
+        k += q->n;
+      }
+      int32_t rc = call_rc;
+      if (rc == DEMI_OK) {
+        rc = replay_many(h, tr.data(), flat.data(), (uint32_t)total, mask_words, looking_for, flags, res.data(), lc);
+        if (rc != DEMI_OK) { call_rc = rc; call_msg = h->err; }
+      }
+      k = 0;
+      for (Request* q : batch) {
+        q->rc = rc;
+        if (rc == DEMI_OK) q->res.assign(res.begin() + k, res.begin() + k + q->n);
+        k += q->n;
+      }
+      lk.lock();
+      for (Request* q : batch) q->done = true;
+      R.running += (uint32_t)batch.size();
+      R.work.notify_all();
+    }
+  }
+  for (std::thread& th : threads) th.join();
+  set_perf(h, lc);
+  if (call_rc != DEMI_OK) { h->err = call_msg; return call_rc; }
+  for (uint32_t t = 0; t < n; t++)
+    if (status[t] != DEMI_OK) { h->err = msg[t]; break; }
+  return DEMI_OK;
+}

@@ -76,8 +76,11 @@ struct DDMinDriver {
     auto it = dag_index.find(dag);
     if (it != dag_index.end()) return it->second;
     DagNode n; n.dag = dag; n.child[0] = n.child[1] = -1; n.ok = halves(dag, n.hv, n.na);
+    // `dag` may live in dag_nodes (child_of passes a node's half), which push_back can move: key on the copy first
+    const int32_t id = (int32_t)dag_nodes.size();
+    dag_index.emplace(n.dag, id);
     dag_nodes.push_back(std::move(n));
-    return dag_index[dag] = (int32_t)dag_nodes.size() - 1;
+    return id;
   }
   int32_t child_of(int32_t d, int k) {
     if (dag_nodes[d].child[k] < 0) { const int32_t c = dag_of(dag_nodes[d].hv[k]); dag_nodes[d].child[k] = c; }

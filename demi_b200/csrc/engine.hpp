@@ -91,6 +91,16 @@ struct demi_handle {
   DevBuf rp_table; uint32_t rp_gen_next = 0; uint64_t rp_table_geometry = 0;
   DevBuf rp_tosend, rp_pruned, rp_masks, rp_results;
   DevBuf rp_counters;                              // unsigned long long[2]
+  DevBuf rp_bound;                                 // demi::ReplayArgs per warp of a multi-trace K2 launch
+  // ---- the trace set (demi_set_traces, capi_replay_many.cu): independent of the single trace above
+  struct TraceSet {
+    uint32_t n = 0;
+    std::vector<std::vector<demi_ext_event>> ext;      // per trace: its externals (DDMin's atoms)
+    std::vector<uint32_t> n_events;
+    DevBuf events, ordinal, externals, send_index;   // every trace's records, one after the other
+    DevBuf views;                                    // demi::ReplayTraceView[n]
+    std::vector<uint32_t> n_uniq_words, pending_cap, tosend_cap, table_slots;
+  } set;
   // ---- communicator (capi_frontier.cu): NCCL inside the library
   void* comm = nullptr;
   void* frontier = nullptr;      // cached K3F buffers
@@ -127,6 +137,21 @@ const ReplayVariant* pick_rv(int model);
 demi::ReplayArgs replay_args(const demi_handle* h, uint32_t looking_for, uint32_t flags);
 // binds the handle's loaded model to the replay kernels: model_ir.cuh keeps one copy of it per translation unit
 cudaError_t replay_ir_bind(const demi_handle* h, cudaStream_t s);
+// what demi_set_trace checks of a trace before it builds its side tables; `who` leads every message
+int32_t check_trace(demi_handle* h, const char* who, const demi_event* events, uint32_t n_events,
+                    const demi_ext_event* externals, uint32_t n_externals);
+// the side tables of a trace K2 reads: per event the FIFO ordinal of its external Send, the index of each Send among
+// the externals, the Uniq-id bound and the number of MsgSends
+struct TraceTables { std::vector<uint16_t> ordinal, sidx; uint32_t n_uniq = 0, n_send_events = 0; };
+int32_t trace_tables(demi_handle* h, const char* who, const demi_event* events, uint32_t n_events,
+                     const demi_ext_event* externals, uint32_t n_externals, TraceTables& t);
+// the per-warp scratch, generation range and counters of a K2 launch (capi_replay.cu)
+int32_t replay_scratch(demi_handle* h, demi::ReplayArgs& a, uint64_t warps, int n_actors, uint32_t per_thread, bool record,
+                       cudaStream_t s);
+// demi_ddmin's walk over a driver whose oracle, trace and flags are set: check_unmodified, ddmin2, verify_mcs, outputs
+namespace demi { struct DDMinDriver; }
+int32_t ddmin_sts(demi::DDMinDriver& d, int32_t check_unmodified, uint64_t* mcs_mask, uint32_t* iteration_sizes,
+                  uint32_t cap_iterations, demi_ddmin_out* out);
 void demi_comm_free(demi_handle* h);
 void demi_frontier_free(demi_handle* h);
 

@@ -482,4 +482,78 @@ replay_lane_kernel(const __grid_constant__ ReplayArgs args) {
   }
 }
 
+// One trace of a set (demi_set_traces): the ReplayArgs fields that differ from trace to trace.  The capacities are the
+// trace's own, so that every test reports the status it would report with that trace alone.
+struct ReplayTraceView {
+  const uint4* events; const uint16_t* ev_ordinal; const uint4* ext; const uint16_t* send_ext_index;
+  uint32_t n_events, n_ext, n_sends, n_uniq_words;
+  uint32_t pending_cap, tosend_cap, table_slots, pad;
+};
+
+// K2 over many traces.  A tile {trace, first test, tests (<= 32), looking_for} belongs to one warp, so the trace stays
+// warp-uniform and the lanes walk it in lock-step as in replay_lane_kernel; warps take tiles grid-stride.  `args`
+// carries what the tiles share (flags, masks, results) and the scratch geometry, which is the largest of the launch's
+// traces; each tile binds its trace's view into the warp's copy of it, bound[warp] in global memory.  The copy is in
+// neither registers (they would come out of the per-event loop's) nor shared memory (a block's copies would cost raft5
+// one of its four resident blocks per SM); its fields are read through L1.
+template <class MODEL, int BD>
+__global__ void __launch_bounds__(BD, (model_replay_direct<MODEL>::value && MODEL::N_ACTORS <= 8) ? 1024 / BD : 1)
+replay_many_kernel(const __grid_constant__ ReplayArgs args, const ReplayTraceView* __restrict__ views,
+                   const uint4* __restrict__ tiles, uint32_t n_tiles, ReplayArgs* bound) {
+  using M = ReplayMachine<MODEL, BD>;
+  extern __shared__ __align__(16) uint32_t lane_smem[];
+  const uint32_t tid = threadIdx.x;
+  const uint64_t gwarp = ((uint64_t)blockIdx.x * BD + tid) >> 5;
+  const uint64_t total_warps = (uint64_t)gridDim.x * (BD / 32);
+  const uint32_t lane = tid & 31;
+
+  ReplayArgs& la = bound[gwarp];
+  if (lane == 0) la = args;
+  __syncwarp();
+  M m;
+  m.smw = lane_smem + tid;
+  m.A = &la;
+  m.table = args.table + gwarp * (uint64_t)args.table_slots * 32 + lane;
+  m.tosend = args.tosend + gwarp * (uint64_t)args.tosend_cap * 32 + lane;
+  m.pruned = args.pruned ? args.pruned + gwarp * (uint64_t)(args.n_uniq_words + M::N) * 32 + lane : nullptr;
+
+  unsigned long long my_repro = 0, my_deliv = 0;
+  uint32_t generation = args.gen_base - 1;
+  for (uint64_t t = gwarp; t < n_tiles; t += total_warps) {
+    const uint4 tile = tiles[t];
+    __syncwarp();                                  // every lane is done with the previous tile's trace
+    if (lane == 0) {
+      const ReplayTraceView& v = views[tile.x];
+      la.events = v.events; la.n_events = v.n_events; la.ev_ordinal = v.ev_ordinal;
+      la.ext = v.ext; la.n_ext = v.n_ext; la.send_ext_index = v.send_ext_index; la.n_sends = v.n_sends;
+      la.n_uniq_words = v.n_uniq_words; la.pending_cap = v.pending_cap; la.tosend_cap = v.tosend_cap;
+      la.table_slots = v.table_slots; la.looking_for = tile.w;
+    }
+    __syncwarp();
+    if (lane >= tile.z) continue;
+    generation++;
+    if (generation >= 0xFFFFu) {
+      for (uint32_t s = 0; s < args.table_slots; s++) m.table[(size_t)s * 32] = make_uint4(0, 0, 0, 0);
+      generation = 1;
+    }
+    const uint32_t idx = tile.y + lane;
+    demi_replay_result r;
+    m.run(idx, generation, r);
+    uint4* dst = reinterpret_cast<uint4*>(args.results + idx);
+    dst[0] = make_uint4((uint32_t)r.violation | ((uint32_t)r.status << 16),
+                        (uint32_t)r.delivered | ((uint32_t)r.ignored << 16),
+                        (uint32_t)r.state_hash, (uint32_t)(r.state_hash >> 32));
+    my_repro += (r.status == 0 && r.violation) ? 1u : 0u;
+    my_deliv += r.delivered;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    my_repro += __shfl_xor_sync(FULL_MASK, my_repro, o);
+    my_deliv += __shfl_xor_sync(FULL_MASK, my_deliv, o);
+  }
+  if (lane == 0 && args.counters && (my_repro | my_deliv)) {
+    atomicAdd(args.counters, my_repro);
+    atomicAdd(args.counters + 1, my_deliv);
+  }
+}
+
 }  // namespace demi

@@ -46,6 +46,7 @@ class Engine(object):
         if rc != N.OK:
             raise DemiError(rc, N.lib().demi_last_error(None).decode())
         self._ext = None
+        self._set_ext = []                 # the externals count of each trace of the set (set_traces)
 
     def close(self):
         if self._h:
@@ -140,6 +141,18 @@ class Engine(object):
         self._check(N.lib().demi_fuzz_trace(self._h, C.byref(p), seed, ev.ctypes.data, cap_events, C.byref(ne),
                                             par.ctypes.data, cap_nodes, C.byref(nn), res.ctypes.data))
         return ev[:ne.value].copy(), par[:nn.value].copy(), res[0]
+
+    def fuzz_traces(self, seed_base, prefix_index, max_messages, interval, looking_for=0, cap_events=1024):
+        """demi_fuzz_traces: the EventTraces of executions seed_base + prefix_index[i], recorded in one launch.
+        Returns (events [n, cap_events], n_events [n], results [n]); row i holds n_events[i] events."""
+        idx = np.ascontiguousarray(prefix_index, dtype=np.uint32)
+        p = N.FuzzParams(seed_base, len(idx), max_messages, interval, looking_for or 0, 0)
+        ev = np.zeros((len(idx), cap_events), dtype=N.EVENT_DTYPE)
+        ne = np.zeros(len(idx), dtype=np.uint32)
+        res = np.zeros(len(idx), dtype=N.RESULT_DTYPE)
+        self._check(N.lib().demi_fuzz_traces(self._h, C.byref(p), idx.ctypes.data, len(idx), ev.ctypes.data, cap_events,
+                                             ne.ctypes.data, res.ctypes.data))
+        return ev, ne, res
 
     # ---- provenance pruning (ProvenanceTracker, schedulers/Util.scala:267-376)
     def provenance(self, events, dep_parent, affected_mask, mask_words=None):
@@ -275,6 +288,68 @@ class Engine(object):
         self._check(N.lib().demi_ddmin(self._h, looking_for or 0, flags, 1 if check_unmodified else 0,
                                        mcs.ctypes.data, mw, iters.ctypes.data, cap_iterations, C.byref(out)))
         return mcs, iters[:min(out.n_iterations, cap_iterations)].copy(), out
+
+    # ---- a set of traces: replay and DDMin with many traces' tests in shared launches
+    def set_traces(self, traces, externals):
+        """demi_set_traces.  `traces` is a list of EVENT_DTYPE arrays, or (events [n, cap], n_events) as fuzz_traces
+        returns them; `externals` is one program shared by every trace, or a list of one per trace."""
+        if isinstance(traces, tuple):
+            ev, ne = np.ascontiguousarray(traces[0], dtype=N.EVENT_DTYPE), np.ascontiguousarray(traces[1], dtype=np.uint32)
+            n = len(ne)
+            ev_off = (np.arange(n, dtype=np.uint64) * ev.shape[1]).astype(np.uint32)
+            ev = ev.reshape(-1)
+        else:
+            n = len(traces)
+            ne = np.array([len(t) for t in traces], dtype=np.uint32)
+            ev_off = np.concatenate([[0], np.cumsum(ne)[:-1]]).astype(np.uint32)
+            ev = np.ascontiguousarray(np.concatenate(traces) if n else np.zeros(0, N.EVENT_DTYPE), dtype=N.EVENT_DTYPE)
+        if isinstance(externals, (list, tuple)) and len(externals) and isinstance(externals[0], np.ndarray):
+            exts = [np.ascontiguousarray(e, dtype=N.EXT_DTYPE) for e in externals]
+        else:
+            one = externals if isinstance(externals, np.ndarray) else pack_externals(externals)
+            exts = [np.ascontiguousarray(one, dtype=N.EXT_DTYPE)] * n
+        if exts and all(e is exts[0] for e in exts):
+            ext, nx, ext_off = exts[0], np.full(n, len(exts[0]), dtype=np.uint32), np.zeros(n, dtype=np.uint32)
+        else:
+            nx = np.array([len(e) for e in exts], dtype=np.uint32)
+            ext_off = np.concatenate([[0], np.cumsum(nx)[:-1]]).astype(np.uint32)
+            ext = np.ascontiguousarray(np.concatenate(exts), dtype=N.EXT_DTYPE)
+        ev_off, ne, ext_off, nx = (np.ascontiguousarray(a, dtype=np.uint32) for a in (ev_off, ne, ext_off, nx))
+        self._check(N.lib().demi_set_traces(self._h, n, ev.ctypes.data if len(ev) else None, ev_off.ctypes.data,
+                                            ne.ctypes.data, ext.ctypes.data if len(ext) else None, ext_off.ctypes.data,
+                                            nx.ctypes.data))
+        self._set_ext = [len(e) for e in exts]
+
+    def set_mask_words(self):
+        return max(1, (max(self._set_ext, default=0) + 63) // 64)
+
+    def replay_batch_many(self, trace_of_test, masks, looking_for, flags=0, mask_words=None):
+        """demi_replay_batch_many: test i replays masks[i] on trace trace_of_test[i]; looking_for[t] per trace."""
+        mw = mask_words or self.set_mask_words()
+        tr = np.ascontiguousarray(trace_of_test, dtype=np.uint32)
+        m = np.ascontiguousarray(masks, dtype=np.uint64).reshape(-1, mw)
+        lf = np.ascontiguousarray(looking_for, dtype=np.uint32)
+        out = np.empty(len(tr), dtype=N.REPLAY_DTYPE)
+        self._check(N.lib().demi_replay_batch_many(self._h, tr.ctypes.data, m.ctypes.data, len(tr), mw, lf.ctypes.data,
+                                                   flags, out.ctypes.data))
+        return out
+
+    def ddmin_many(self, looking_for, flags=0, check_unmodified=True, cap_iterations=256, mask_words=None):
+        """demi_ddmin_many over the set: (MCS masks [n, mw], iteration sizes [n, cap], DDMIN_OUT_DTYPE [n], status [n]).
+        A trace whose status is not OK has no outputs; the call raises only for call-level errors."""
+        n = len(self._set_ext)
+        mw = mask_words or self.set_mask_words()
+        lf = np.ascontiguousarray(looking_for, dtype=np.uint32)
+        mcs = np.zeros((n, mw), dtype=np.uint64)
+        iters = np.zeros((n, cap_iterations), dtype=np.uint32)
+        out = np.zeros(n, dtype=N.DDMIN_OUT_DTYPE)
+        status = np.zeros(n, dtype=np.int32)
+        self._check(N.lib().demi_ddmin_many(self._h, lf.ctypes.data, flags, 1 if check_unmodified else 0, mcs.ctypes.data,
+                                            mw, iters.ctypes.data, cap_iterations, out.ctypes.data, status.ctypes.data))
+        return mcs, iters, out, status
+
+    def last_error(self):
+        return N.lib().demi_last_error(self._h).decode()
 
     # ---- DDMin with RandomScheduler as the TestOracle (RunnerUtils.randomDDMin, RunnerUtils.scala:601-623)
     def program_mask_words(self):

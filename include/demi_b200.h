@@ -368,6 +368,44 @@ int32_t demi_ddmin(demi_handle* h, uint32_t looking_for, uint32_t flags, int32_t
                    uint64_t* mcs_mask, uint32_t mask_words,
                    uint32_t* iteration_sizes, uint32_t cap_iterations, demi_ddmin_out* out);
 
+/* ------------------------------------------- many traces: recording, replay and DDMin in shared launches
+ * The EventTraces of n executions of the handle's program, recorded in one launch as demi_fuzz_provenance records them:
+ * execution i is seed p->seed_base + prefix_index[i].  Its events go to events + i*cap_events, its count to
+ * n_events[i] and its demi_fuzz_result to results[i] (results may be NULL).  Each record equals what demi_fuzz_trace
+ * returns for that seed with the same cap_events.  An execution with a nonzero status (DEMI_PS_EVENT_OVF when
+ * cap_events is too small) has its count and result but no events: the call writes zeros where they would be.  The call
+ * then returns DEMI_ERR_CAPACITY naming the lowest such execution, with every record filled.  Each row is written only
+ * as far as the longest successful recording of the call reaches; past n_events[i], row i's content is unspecified. */
+int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, const uint32_t* prefix_index, uint32_t n,
+                         demi_event* events, uint32_t cap_events, uint32_t* n_events, demi_fuzz_result* results);
+/* A set of n_traces recorded executions to minimise, separate from the single trace of demi_set_trace (which it leaves
+ * as it is).  Trace t is events[event_offsets[t] ..] (n_events[t] records) with the externals
+ * externals[ext_offsets[t] ..] (n_externals[t] records); offsets are in elements, so the strided output of
+ * demi_fuzz_traces and one program shared by every trace (all ext_offsets 0) are taken as they are.  Each trace is
+ * validated as demi_set_trace validates its trace; a failure names the trace's index.  A call that fails leaves the
+ * previous set in place.  Traces of a set have no conjoined atoms. */
+int32_t demi_set_traces(demi_handle* h, uint32_t n_traces,
+                        const demi_event* events, const uint32_t* event_offsets, const uint32_t* n_events,
+                        const demi_ext_event* externals, const uint32_t* ext_offsets, const uint32_t* n_externals);
+/* n_tests STSScheduler.test calls over the set: test i replays mask i (mask_words words) on trace trace_of_test[i],
+ * looking for looking_for[trace_of_test[i]].  Record i equals demi_replay_batch's record for that mask with that trace
+ * alone, for every flag.  demi_perf counts the launches, the tests and their kernel time. */
+int32_t demi_replay_batch_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks, uint32_t n_tests,
+                               uint32_t mask_words, const uint32_t* looking_for, uint32_t flags,
+                               demi_replay_result* out);
+/* demi_ddmin on every trace t of the set, looking for looking_for[t]: status[t] is what demi_set_trace(trace t) then
+ * demi_ddmin(h, looking_for[t], flags, check_unmodified, ...) would return, and when it is DEMI_OK, mcs_masks[t*mask_words
+ * ..], iteration_sizes[t*cap_iterations ..] (may be NULL) and out[t] equal that call's outputs, replays_executed and
+ * batches included (they count that trace's own speculative batches); out[t].reserved holds host microseconds.  The
+ * minimisations of many traces run side by side and their tests share launches; the results do not depend on how the
+ * traces are grouped.  The call fails only on invalid arguments, without a set (DEMI_ERR_STATE) or on a CUDA error; when
+ * some traces fail, it returns DEMI_OK and demi_last_error holds the message of the lowest-indexed one.
+ * DEMI_DDMIN_MANY_WINDOW bounds the minimisations in flight, one host thread each: 1..4096, default 512; any other
+ * value fails the call with DEMI_ERR_INVALID. */
+int32_t demi_ddmin_many(demi_handle* h, const uint32_t* looking_for, uint32_t flags, int32_t check_unmodified,
+                        uint64_t* mcs_masks, uint32_t mask_words, uint32_t* iteration_sizes, uint32_t cap_iterations,
+                        demi_ddmin_out* out, int32_t* status);
+
 /* DDMin with a RandomScheduler as the TestOracle (RunnerUtils.randomDDMin, RunnerUtils.scala:601-623).  The dag is the
  * handle's program (demi_set_externals) with every event in it, WaitQuiescence included: DDMin.minimize wraps the
  * events in an UnmodifiedEventDag (Minimizer.scala:15-20).  Atoms as in demi_ddmin (Start..Kill, Partition..UnPartition;

@@ -188,9 +188,72 @@ class Engine {
     check(demi_fuzz_campaign(h, &p, program_seed_base, out.data()));
     return out;
   }
+  // ---- many traces: recording, replay and DDMin with their tests in shared launches
+  // demi_fuzz_traces: the EventTraces of executions seed_base + prefix_index[i] of the program (demi_set_externals)
+  std::vector<EventTrace> fuzz_traces(int64_t seed_base, const std::vector<uint32_t>& prefix_index, int32_t max_messages,
+                                      int32_t interval, uint32_t looking_for = 0, uint32_t cap_events = 4096) {
+    demi_fuzz_params p{seed_base, prefix_index.size(), max_messages, interval, looking_for, 0};
+    std::vector<demi_event> ev(prefix_index.size() * (size_t)cap_events);
+    std::vector<uint32_t> n(prefix_index.size());
+    check(demi_fuzz_traces(h, &p, prefix_index.data(), (uint32_t)prefix_index.size(), ev.data(), cap_events, n.data(), nullptr));
+    std::vector<EventTrace> out(n.size());
+    for (size_t i = 0; i < n.size(); i++) out[i].assign(ev.begin() + i * cap_events, ev.begin() + i * cap_events + n[i]);
+    return out;
+  }
+  // demi_set_traces: trace i with externals[i] (or one program shared by all when externals has one entry)
+  void set_traces(const std::vector<EventTrace>& traces, const std::vector<ExternalEvents>& externals) {
+    const bool shared = externals.size() == 1;
+    std::vector<demi_event> ev; std::vector<demi_ext_event> ex;
+    std::vector<uint32_t> eo, ne, xo, nx;
+    for (size_t i = 0; i < traces.size(); i++) {
+      eo.push_back((uint32_t)ev.size()); ne.push_back((uint32_t)traces[i].size());
+      ev.insert(ev.end(), traces[i].begin(), traces[i].end());
+      const ExternalEvents& x = externals.at(shared ? 0 : i);
+      xo.push_back(shared ? 0u : (uint32_t)ex.size()); nx.push_back((uint32_t)x.size());
+      if (!shared || i == 0) ex.insert(ex.end(), x.begin(), x.end());
+    }
+    check(demi_set_traces(h, (uint32_t)traces.size(), ev.data(), eo.data(), ne.data(), ex.data(), xo.data(), nx.data()));
+    set_ext.clear();
+    for (size_t i = 0; i < traces.size(); i++) set_ext.push_back(externals.at(shared ? 0 : i));
+  }
+  uint32_t set_mask_words() const {
+    size_t m = 1;
+    for (const ExternalEvents& x : set_ext) m = std::max(m, x.size());
+    return (uint32_t)((m + 63) / 64);
+  }
+  // demi_replay_batch_many: masks[i] (set_mask_words() words) on trace trace_of_test[i]
+  std::vector<demi_replay_result> replay_batch_many(const std::vector<uint32_t>& trace_of_test, const std::vector<uint64_t>& masks,
+                                                    const std::vector<ViolationFingerprint>& looking_for, uint32_t flags = 0) {
+    std::vector<demi_replay_result> out(trace_of_test.size());
+    check(demi_replay_batch_many(h, trace_of_test.data(), masks.data(), (uint32_t)trace_of_test.size(), set_mask_words(),
+                                 looking_for.data(), flags, out.data()));
+    return out;
+  }
+  // demi_ddmin_many: per trace of the set, its MCS (WaitQuiescence dropped) and the DDMin record, or the error code
+  struct DDMinManyResult { ExternalEvents mcs; demi_ddmin_out out; int32_t status; std::vector<uint32_t> iteration_sizes; };
+  std::vector<DDMinManyResult> ddmin_many(const std::vector<ViolationFingerprint>& looking_for, uint32_t flags = 0,
+                                          bool checkUnmodifed = true, uint32_t cap_iterations = 256) {
+    const size_t n = set_ext.size();
+    const uint32_t mw = set_mask_words();
+    std::vector<uint64_t> mcs(n * mw);
+    std::vector<uint32_t> iters(n * cap_iterations);
+    std::vector<demi_ddmin_out> out(n);
+    std::vector<int32_t> status(n);
+    check(demi_ddmin_many(h, looking_for.data(), flags, checkUnmodifed ? 1 : 0, mcs.data(), mw, iters.data(), cap_iterations,
+                          out.data(), status.data()));
+    std::vector<DDMinManyResult> r(n);
+    for (size_t t = 0; t < n; t++) {
+      r[t].out = out[t]; r[t].status = status[t];
+      if (status[t] != DEMI_OK) continue;
+      for (size_t i = 0; i < set_ext[t].size(); i++) if ((mcs[t * mw + (i >> 6)] >> (i & 63)) & 1ull) r[t].mcs.push_back(set_ext[t][i]);
+      r[t].iteration_sizes.assign(iters.begin() + t * cap_iterations, iters.begin() + t * cap_iterations + std::min(out[t].n_iterations, cap_iterations));
+    }
+    return r;
+  }
   const SchedulerConfig cfg;
  private:
   demi_handle* h = nullptr;
+  std::vector<ExternalEvents> set_ext;         // the externals of each trace of the set (demi_set_traces)
   demi_fuzzer_config fz_cfg{};
   ExternalEvents fz_prefix, fz_postfix;
 };

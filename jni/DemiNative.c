@@ -204,6 +204,33 @@ JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_randomTestTrac
                                 (int64_t)seed, (demi_event*)BUF(env, events), (uint32_t)capEvents, (uint32_t*)BUF(env, count),
                                 (demi_fuzz_result*)BUF(env, result));
 }
+/* demi_fuzz_traces / demi_set_traces / demi_replay_batch_many / demi_ddmin_many: many violating executions recorded,
+ * replayed and minimized with their tests in shared launches */
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_fuzzTraces(JNIEnv* env, jclass c, jlong h, jobject params,
+    jobject prefixIndex, jint n, jobject events, jint capEvents, jobject nEvents, jobject results) {
+  return demi_fuzz_traces(H(h), (const demi_fuzz_params*)BUF(env, params), (const uint32_t*)BUF(env, prefixIndex), (uint32_t)n,
+                          (demi_event*)BUF(env, events), (uint32_t)capEvents, (uint32_t*)BUF(env, nEvents),
+                          results ? (demi_fuzz_result*)BUF(env, results) : 0);
+}
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_setTraces(JNIEnv* env, jclass c, jlong h, jint nTraces,
+    jobject events, jobject eventOffsets, jobject nEvents, jobject externals, jobject extOffsets, jobject nExternals) {
+  return demi_set_traces(H(h), (uint32_t)nTraces, (const demi_event*)BUF(env, events), (const uint32_t*)BUF(env, eventOffsets),
+                         (const uint32_t*)BUF(env, nEvents), (const demi_ext_event*)BUF(env, externals),
+                         (const uint32_t*)BUF(env, extOffsets), (const uint32_t*)BUF(env, nExternals));
+}
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_replayBatchMany(JNIEnv* env, jclass c, jlong h, jobject traceOfTest,
+    jobject masks, jint nTests, jint maskWords, jobject lookingFor, jint flags, jobject out) {
+  return demi_replay_batch_many(H(h), (const uint32_t*)BUF(env, traceOfTest), (const uint64_t*)BUF(env, masks), (uint32_t)nTests,
+                                (uint32_t)maskWords, (const uint32_t*)BUF(env, lookingFor), (uint32_t)flags,
+                                (demi_replay_result*)BUF(env, out));
+}
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_ddminMany(JNIEnv* env, jclass c, jlong h, jobject lookingFor,
+    jint flags, jint checkUnmodified, jobject mcsMasks, jint maskWords, jobject iterationSizes, jint capIterations, jobject out,
+    jobject status) {
+  return demi_ddmin_many(H(h), (const uint32_t*)BUF(env, lookingFor), (uint32_t)flags, checkUnmodified, (uint64_t*)BUF(env, mcsMasks),
+                         (uint32_t)maskWords, iterationSizes ? (uint32_t*)BUF(env, iterationSizes) : 0, (uint32_t)capIterations,
+                         (demi_ddmin_out*)BUF(env, out), (int32_t*)BUF(env, status));
+}
 /* `exp` = a direct buffer laid out as demi_experiment whose pointer fields the Scala side fills with
  * GetDirectBufferAddress-style addresses (DemiNative.addressOf) */
 JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_experimentSave(JNIEnv* env, jclass c, jstring dir, jobject exp) {

@@ -75,6 +75,18 @@ object DemiNative {
   /** demi_random_test_trace: the EventTrace RandomScheduler.test returns for a subsequence (the verified MCS trace) */
   @native def randomTestTrace(h: Long, mask: ByteBuffer, maskWords: Int, params: ByteBuffer, seed: Long, events: ByteBuffer,
                               capEvents: Int, count: ByteBuffer, result: ByteBuffer): Int
+  /** demi_fuzz_traces: the EventTraces of executions seed_base + prefixIndex(i), execution i at events + i*capEvents */
+  @native def fuzzTraces(h: Long, params: ByteBuffer, prefixIndex: ByteBuffer, n: Int, events: ByteBuffer, capEvents: Int,
+                         nEvents: ByteBuffer, results: ByteBuffer): Int
+  /** demi_set_traces: a set of traces to minimise (offsets in elements), separate from setTrace's single trace */
+  @native def setTraces(h: Long, nTraces: Int, events: ByteBuffer, eventOffsets: ByteBuffer, nEvents: ByteBuffer,
+                        externals: ByteBuffer, extOffsets: ByteBuffer, nExternals: ByteBuffer): Int
+  /** demi_replay_batch_many: test i replays mask i on trace traceOfTest(i); lookingFor holds one code per trace */
+  @native def replayBatchMany(h: Long, traceOfTest: ByteBuffer, masks: ByteBuffer, nTests: Int, maskWords: Int,
+                              lookingFor: ByteBuffer, flags: Int, out: ByteBuffer): Int
+  /** demi_ddmin_many: RunnerUtils.stsSchedDDMin on every trace of the set; status(t) is that trace's return code */
+  @native def ddminMany(h: Long, lookingFor: ByteBuffer, flags: Int, checkUnmodified: Int, mcsMasks: ByteBuffer, maskWords: Int,
+                        iterationSizes: ByteBuffer, capIterations: Int, out: ByteBuffer, status: ByteBuffer): Int
   /** The flat experiment directory that replaces ExperimentSerializer's *.bin object streams (Serialization.scala:57-74). */
   @native def experimentSave(dir: String, exp: ByteBuffer): Int
   @native def experimentLoad(dir: String, exp: ByteBuffer): Int
