@@ -1253,7 +1253,7 @@ struct RandomDDMinDriver : DDMinDriver {
   std::map<Mask, demi_random_test_result> records;
   std::vector<uint32_t> consumed_runs;      // executions_run of each test the sequential walk consumed, in order
   uint64_t executions_executed = 0;
-  int32_t evaluate_flat(const uint64_t* masks, size_t n, signed char* out) override {
+  int32_t evaluate(const uint64_t* masks, size_t n, signed char* out) override {
     std::vector<demi_random_test_result> res(n);
     uint64_t executed = 0;
     int32_t rc = random_tests(h, masks, (uint32_t)n, mw, &p, res.data(), &executed);
@@ -1264,14 +1264,6 @@ struct RandomDDMinDriver : DDMinDriver {
       out[i] = res[i].status == 0 && res[i].first_hit >= 0;
     }
     return DEMI_OK;
-  }
-  int32_t evaluate_batch(const std::vector<Mask>& want, std::vector<char>& out) override {
-    std::vector<uint64_t> flat(want.size() * mw);
-    for (size_t i = 0; i < want.size(); i++) std::copy(want[i].begin(), want[i].end(), flat.begin() + i * mw);
-    std::vector<signed char> r(want.size());
-    int32_t rc = evaluate_flat(flat.data(), want.size(), r.data());
-    for (size_t i = 0; i < want.size(); i++) out[i] = r[i];
-    return rc;
   }
   // a test's status fails the call only here, where the sequential walk uses its result
   void consumed(const Mask& m) override {
@@ -1329,7 +1321,7 @@ extern "C" int32_t demi_random_ddmin(demi_handle* h, const demi_fuzz_params* p, 
     auto it = d.records.find(mcs);
     if (it == d.records.end()) {
       signed char v;
-      if ((rc = d.evaluate_flat(mcs.data(), 1, &v)) != DEMI_OK) return rc;
+      if ((rc = d.evaluate(mcs.data(), 1, &v)) != DEMI_OK) return rc;
       d.replays_executed++;
       it = d.records.find(mcs);
     }

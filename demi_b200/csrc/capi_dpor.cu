@@ -222,23 +222,24 @@ struct DporDDMinDriver : DDMinDriver {
   std::map<Mask, std::vector<int32_t>> history;
   uint64_t interleavings = 0;
 
-  int32_t evaluate_batch(const std::vector<Mask>& want, std::vector<char>& out) override {
+  int32_t evaluate(const uint64_t* masks, size_t n, signed char* out) override {
     std::vector<demi_ext_event> flat;
     std::vector<uint32_t> off(1, 0), coff(1, 0);
     std::vector<int32_t> caps;
-    for (const Mask& m : want) {
-      for (uint32_t i = 0; i < n_ext; i++) if (bit(m, i)) flat.push_back(ext[i]);
+    for (size_t k = 0; k < n; k++) {
+      const uint64_t* m = masks + k * mw;
+      for (uint32_t i = 0; i < n_ext; i++) if ((m[i >> 6] >> (i & 63)) & 1ull) flat.push_back(ext[i]);
       off.push_back((uint32_t)flat.size());
-      auto it = history.find(m);
+      auto it = history.find(Mask(m, m + mw));
       if (it != history.end()) caps.insert(caps.end(), it->second.begin(), it->second.end());
       caps.push_back(cap);
       coff.push_back((uint32_t)caps.size());
     }
-    std::vector<demi_dpor_result> res(want.size());
-    int32_t rc = dpor_run(h, flat.data(), off.data(), (uint32_t)want.size(), P, dflags, seed, caps.data(), coff.data(),
+    std::vector<demi_dpor_result> res(n);
+    int32_t rc = dpor_run(h, flat.data(), off.data(), (uint32_t)n, P, dflags, seed, caps.data(), coff.data(),
                           res.data(), nullptr, 0, nullptr, 0);
     if (rc != DEMI_OK) return rc;
-    for (size_t i = 0; i < want.size(); i++) {
+    for (size_t i = 0; i < n; i++) {
       if (res[i].status) return fail(h, DEMI_ERR_CAPACITY, "demi_incremental_ddmin: a DPOR instance reported status %u", res[i].status);
       out[i] = res[i].violations != 0;
       interleavings += res[i].interleavings;

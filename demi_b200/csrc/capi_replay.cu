@@ -16,37 +16,36 @@
 
 using namespace demi;
 
-template <class MODEL, int BD>
-static ReplayVariant make_rv() {
+namespace {
+typedef void (*replay_fn)(const ReplayArgs);
+typedef void (*replay_many_fn)(const ReplayArgs, const ReplayTraceView*, const uint4*, uint32_t, ReplayArgs*);
+// K2 per model: the four instantiations of replay_lane_kernel, fn[WILD][REC], and replay_many_kernel, at the model's
+// block size and shared memory.  Every K2 instantiation is in this unit, so that its copy of model_ir.cuh's loaded model
+// is the one K2 reads.
+struct ReplayVariant { int model; int bd; replay_fn fn[2][2]; replay_many_fn many; size_t smem; int n_actors; };
+template <class MODEL>
+ReplayVariant make_rv() {
+  constexpr int BD = replay_block<MODEL>;
   using M = ReplayMachine<MODEL, BD>;     // WORDS does not depend on REC or WILD
   return ReplayVariant{MODEL::ID, BD,
                        {{replay_lane_kernel<MODEL, BD, false, false>, replay_lane_kernel<MODEL, BD, true, false>},
                         {replay_lane_kernel<MODEL, BD, false, true>, replay_lane_kernel<MODEL, BD, true, true>}},
-                       (size_t)M::WORDS * BD * sizeof(uint32_t), MODEL::N_ACTORS};
+                       replay_many_kernel<MODEL, BD>, (size_t)M::WORDS * BD * sizeof(uint32_t), MODEL::N_ACTORS};
 }
 const ReplayVariant* pick_rv(int model) {
-  static const std::vector<ReplayVariant> v = {
-    make_rv<PingPong3, 256>(), make_rv<Raft5, 256>(), make_rv<Bcast32, 128>(), make_rv<IrModel, 128>(),
-  };
+  static const std::vector<ReplayVariant> v = {make_rv<PingPong3>(), make_rv<Raft5>(), make_rv<Bcast32>(), make_rv<IrModel>()};
   for (const ReplayVariant& r : v) if (r.model == model) return &r;
   return nullptr;
 }
+}  // namespace
 
-ReplayArgs replay_args(const demi_handle* h, uint32_t looking_for, uint32_t flags) {
+ReplayArgs replay_args(const demi_handle* h, const ReplayTraceView& trace, uint32_t looking_for, uint32_t flags) {
   ReplayArgs a{};
   a.model_flags = h->cfg.model_flags; a.blocked_mask = h->cfg.blocked_mask; a.ignore_timers = h->cfg.ignore_timers;
   a.looking_for = looking_for; a.flags = flags;
-  a.events = h->trace_dev.get<const uint4>(); a.n_events = (uint32_t)h->trace_host.size();
-  a.ev_ordinal = h->ev_ordinal_dev.get<uint16_t>();
-  a.ext = h->trace_ext_dev.get<const uint4>(); a.n_ext = (uint32_t)h->trace_ext_host.size();
-  a.send_ext_index = h->send_ext_index_dev.get<uint16_t>(); a.n_sends = h->trace_n_ext_sends;
   a.external_type_mask = demi_ext_type_mask(h);
-  a.n_uniq_words = (h->trace_n_uniq + 31) / 32;
+  bind_trace(a, trace);
   return a;
-}
-
-cudaError_t replay_ir_bind(const demi_handle* h, cudaStream_t s) {
-  return h->cfg.model == DEMI_MODEL_IR ? ir_bind(h->ir_dev, s) : cudaSuccess;
 }
 
 int32_t check_trace(demi_handle* h, const char* who, const demi_event* events, uint32_t n_events,
@@ -92,6 +91,16 @@ int32_t trace_tables(demi_handle* h, const char* who, const demi_event* events, 
   return DEMI_OK;
 }
 
+ReplayTraceView trace_view(const TraceTables& t, uint32_t n_events, uint32_t n_externals) {
+  ReplayTraceView v{};
+  v.n_events = n_events; v.n_ext = n_externals; v.n_sends = (uint32_t)t.sidx.size();
+  v.n_uniq_words = (t.n_uniq + 31) / 32;
+  v.pending_cap = demi_replay_pending_cap(t.n_send_events);
+  v.tosend_cap = demi_tosend_cap(v.n_sends);
+  v.table_slots = demi_pow2_at_least(2 * v.pending_cap, 256, 1u << 16);
+  return v;
+}
+
 extern "C" int32_t demi_set_trace(demi_handle* h, const demi_event* events, uint32_t n_events,
                                   const demi_ext_event* externals, uint32_t n_externals) {
   if (!h) return DEMI_ERR_INVALID;
@@ -112,19 +121,14 @@ extern "C" int32_t demi_set_trace(demi_handle* h, const demi_event* events, uint
   if ((rc = h->rp_counters.grow(h, 2 * sizeof(unsigned long long))) != DEMI_OK) return rc;     // allocated once per handle
   h->trace_host.assign(events, events + n_events);
   h->trace_ext_host.assign(externals, externals + n_externals);
-  h->send_ext_index_host = sidx;
   h->conjoined.assign(n_externals, -1);                       // a new EventDag has no conjoined atoms
-  h->trace_n_uniq = t.n_uniq;
-  h->trace_n_send_events = t.n_send_events;
-  h->trace_n_ext_sends = (uint32_t)sidx.size();
+  h->trace = trace_view(t, n_events, n_externals);
+  h->trace.events = trace_dev.get<const uint4>(); h->trace.ev_ordinal = ord_dev.get<const uint16_t>();
+  h->trace.ext = ext_dev.get<const uint4>(); h->trace.send_ext_index = sidx_dev.get<const uint16_t>();
   h->trace_dev = std::move(trace_dev); h->trace_ext_dev = std::move(ext_dev);
   h->ev_ordinal_dev = std::move(ord_dev); h->send_ext_index_dev = std::move(sidx_dev);
   return DEMI_OK;
 }
-
-static int32_t launch_replay(demi_handle* h, const void* masks_dev, const void* skips_dev, uint32_t n_masks, uint32_t mask_words,
-                             uint32_t looking_for, uint32_t flags, void* out_dev, void* stream,
-                             demi_event* rec_dev, uint32_t rec_cap, uint32_t* rec_count_dev);
 
 extern "C" int32_t demi_conjoin_atoms(demi_handle* h, uint32_t e1, uint32_t e2) {
   if (!h) return DEMI_ERR_INVALID;
@@ -138,18 +142,21 @@ extern "C" int32_t demi_conjoin_atoms(demi_handle* h, uint32_t e1, uint32_t e2) 
   return DEMI_OK;
 }
 
-extern "C" int32_t demi_replay_batch_dev(demi_handle* h, const void* masks_dev, uint32_t n_masks, uint32_t mask_words,
-                                         uint32_t looking_for, uint32_t flags, void* out_dev, void* stream) {
-  if (!h) return DEMI_ERR_INVALID;
-  if (!masks_dev) return fail(h, DEMI_ERR_INVALID, "demi_replay_batch_dev: null buffer");
-  return launch_replay(h, masks_dev, nullptr, n_masks, mask_words, looking_for, flags, out_dev, stream, nullptr, 0, nullptr);
+namespace {
+// How a launch uses the table: hash tables stamped with the launch's generations (exact replays), or the insertion-
+// ordered list of the REC variant (a recording) or of the WILD variants
+enum class TableUse { GENERATIONS, RECORD, LIST };
+
+cudaError_t replay_ir_bind(const demi_handle* h, cudaStream_t s) {
+  return h->cfg.model == DEMI_MODEL_IR ? ir_bind(h->ir_dev, s) : cudaSuccess;
 }
 
 // The per-warp scratch of a K2 launch of `warps` warps with a's geometry (table_slots, tosend_cap, n_uniq_words, flags),
 // its first generation and its counters, all in a.  Generation stamps: each launch gets a fresh range [gen_base,
 // gen_base + tests per thread]; the table is cleared only when it was (re)allocated, its geometry changed, or the
-// 16-bit range is exhausted.
-int32_t replay_scratch(demi_handle* h, ReplayArgs& a, uint64_t warps, int n_actors, uint32_t per_thread, bool record,
+// 16-bit range is exhausted.  A list leaves its entries behind, so the launch after it clears the table
+// (rp_gen_next = 0); a recording clears it first too, a wildcard list needs no clearing of its own.
+int32_t replay_scratch(demi_handle* h, ReplayArgs& a, uint64_t warps, int n_actors, uint32_t per_thread, TableUse use,
                        cudaStream_t s) {
   int32_t rc;
   const size_t table_bytes = warps * a.table_slots * 32 * sizeof(uint4);
@@ -158,18 +165,55 @@ int32_t replay_scratch(demi_handle* h, ReplayArgs& a, uint64_t warps, int n_acto
   if ((rc = h->rp_tosend.grow(h, warps * a.tosend_cap * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
   if (a.flags & DEMI_RF_FILTER_KNOWN_ABSENTS)
     if ((rc = h->rp_pruned.grow(h, warps * (a.n_uniq_words + n_actors) * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
-  const uint64_t geometry = ((uint64_t)a.table_slots << 32) ^ warps;
-  if (fresh_table || h->rp_gen_next == 0 || h->rp_table_geometry != geometry || h->rp_gen_next + per_thread >= 0xFFF0u || record) {
-    CUDA_TRY(h, cudaMemsetAsync(h->rp_table.get(), 0, table_bytes, s));
-    h->rp_gen_next = 1;
-    h->rp_table_geometry = geometry;
+  if (use == TableUse::LIST) {
+    a.gen_base = 1;
+  } else {
+    const uint64_t geometry = ((uint64_t)a.table_slots << 32) ^ warps;
+    if (fresh_table || h->rp_gen_next == 0 || h->rp_table_geometry != geometry || h->rp_gen_next + per_thread >= 0xFFF0u ||
+        use == TableUse::RECORD) {
+      CUDA_TRY(h, cudaMemsetAsync(h->rp_table.get(), 0, table_bytes, s));
+      h->rp_gen_next = 1;
+      h->rp_table_geometry = geometry;
+    }
+    a.gen_base = h->rp_gen_next;
   }
-  a.gen_base = h->rp_gen_next;
-  h->rp_gen_next = record ? 0 : h->rp_gen_next + per_thread;   // the recording variant leaves list entries behind: clear next time
+  h->rp_gen_next = use == TableUse::GENERATIONS ? h->rp_gen_next + per_thread : 0;
   CUDA_TRY(h, cudaMemsetAsync(h->rp_counters.get(), 0, 2 * sizeof(unsigned long long), s));
   a.table = h->rp_table.get<uint4>(); a.tosend = h->rp_tosend.get<uint32_t>();
   a.pruned = (a.flags & DEMI_RF_FILTER_KNOWN_ABSENTS) ? h->rp_pruned.get<uint32_t>() : nullptr;
   a.counters = h->rp_counters.get<unsigned long long>();
+  return DEMI_OK;
+}
+}  // namespace
+
+int32_t replay_launch(demi_handle* h, ReplayArgs& a, bool wild, bool record, const ReplayTiles* many, bool timed,
+                      cudaStream_t s) {
+  const ReplayVariant* rv = pick_rv(h->cfg.model);
+  if (!rv) return fail(h, DEMI_ERR_INVALID, "no replay kernel for model %d", h->cfg.model);
+  int32_t rc;
+  int bps = 0;
+  const void* fn = many ? (const void*)rv->many : (const void*)rv->fn[wild][record];
+  if ((rc = demi_occupancy(h, fn, rv->bd, rv->smem, &bps)) != DEMI_OK) return rc;
+  if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
+  // a block takes a test per thread of the single-trace kernel, a tile per warp of the multi-trace one; a recording
+  // runs one test, so one block
+  const uint32_t wpb = (uint32_t)rv->bd / 32, per_block = many ? wpb : (uint32_t)rv->bd;
+  const uint64_t items = many ? many->n_tiles : a.n_masks;
+  uint64_t blocks = std::min<uint64_t>((items + per_block - 1) / per_block, (uint64_t)h->sm_count * bps);
+  // a wildcard list holds table_slots uint4 per lane: keep the scratch under 4 GiB
+  if (wild) blocks = std::min<uint64_t>(blocks, std::max<uint64_t>(1, (4ull << 30) / ((uint64_t)a.table_slots * 32 * sizeof(uint4)) / wpb));
+  const int grid = (int)std::max<uint64_t>(1, blocks);
+  const uint64_t warps = (uint64_t)grid * wpb;
+  const uint32_t per_thread = (uint32_t)((items + (uint64_t)grid * per_block - 1) / ((uint64_t)grid * per_block)) + 1;
+  const TableUse use = wild ? TableUse::LIST : record ? TableUse::RECORD : TableUse::GENERATIONS;
+  if ((rc = replay_scratch(h, a, warps, rv->n_actors, per_thread, use, s)) != DEMI_OK) return rc;
+  if (many && (rc = h->rp_bound.grow(h, warps * sizeof(ReplayArgs))) != DEMI_OK) return rc;
+  CUDA_TRY(h, replay_ir_bind(h, s));
+  if (timed) CUDA_TRY(h, cudaEventRecord(h->ev0, s));
+  if (many) rv->many<<<grid, rv->bd, rv->smem, s>>>(a, many->views, many->tiles, many->n_tiles, h->rp_bound.get<ReplayArgs>());
+  else rv->fn[wild][record]<<<grid, rv->bd, rv->smem, s>>>(a);
+  CUDA_TRY(h, cudaGetLastError());
+  if (timed) CUDA_TRY(h, cudaEventRecord(h->ev1, s));
   return DEMI_OK;
 }
 
@@ -179,40 +223,27 @@ static int32_t launch_replay(demi_handle* h, const void* masks_dev, const void* 
   if (!h) return DEMI_ERR_INVALID;
   if (h->trace_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_trace has not been called");
   if (!out_dev) return fail(h, DEMI_ERR_INVALID, "replay: null output buffer");
-  const bool record = rec_dev != nullptr;
   const uint32_t n_ext = (uint32_t)h->trace_ext_host.size();
   if (masks_dev && mask_words * 64 < n_ext) return fail(h, DEMI_ERR_INVALID, "mask_words %u too small for %u externals", mask_words, n_ext);
   if (n_masks == 0) return DEMI_OK;
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  const ReplayVariant* rv = pick_rv(h->cfg.model);
-  if (!rv) return fail(h, DEMI_ERR_INVALID, "no replay kernel for model %d", h->cfg.model);
-  cudaStream_t s = (cudaStream_t)stream;
-  // the grid (and the table's size) is the batch kernel's; the recording kernel runs one block of it
-  int32_t rc;
-  int bps = 0, rec_bps = 0;
-  if ((rc = demi_occupancy(h, (const void*)rv->fn[0][0], rv->bd, rv->smem, &bps)) != DEMI_OK) return rc;
-  if (record && (rc = demi_occupancy(h, (const void*)rv->fn[0][1], rv->bd, rv->smem, &rec_bps)) != DEMI_OK) return rc;
-  if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
-  uint64_t want = ((uint64_t)n_masks + rv->bd - 1) / rv->bd;
-  int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * bps));
-  const uint64_t warps = (uint64_t)grid * (rv->bd / 32);
-
-  ReplayArgs a = replay_args(h, looking_for, flags);
+  ReplayArgs a = replay_args(h, h->trace, looking_for, flags);
   a.masks = (const uint64_t*)masks_dev; a.n_masks = n_masks; a.mask_words = mask_words;
   a.skips = (const uint32_t*)skips_dev;
   a.rec_events = rec_dev; a.rec_cap = rec_cap; a.rec_count = rec_count_dev;
   a.results = (demi_replay_result*)out_dev;
-  a.pending_cap = demi_replay_pending_cap(h->trace_n_send_events);
-  a.tosend_cap = demi_tosend_cap(h->trace_n_ext_sends);
-  a.table_slots = demi_pow2_at_least(2 * a.pending_cap, 256, 1u << 16);
-  const uint32_t per_thread = (uint32_t)(((uint64_t)n_masks + (uint64_t)grid * rv->bd - 1) / ((uint64_t)grid * rv->bd)) + 1;
-  if ((rc = replay_scratch(h, a, warps, rv->n_actors, per_thread, record, s)) != DEMI_OK) return rc;
-  CUDA_TRY(h, replay_ir_bind(h, s));
-  rv->fn[0][record]<<<record ? 1 : grid, rv->bd, rv->smem, s>>>(a);
-  CUDA_TRY(h, cudaGetLastError());
+  const int32_t rc = replay_launch(h, a, false, rec_dev != nullptr, nullptr, false, (cudaStream_t)stream);
+  if (rc != DEMI_OK) return rc;
   h->perf.kernel_launches = 1;
   h->perf.prefixes = n_masks;
   return DEMI_OK;
+}
+
+extern "C" int32_t demi_replay_batch_dev(demi_handle* h, const void* masks_dev, uint32_t n_masks, uint32_t mask_words,
+                                         uint32_t looking_for, uint32_t flags, void* out_dev, void* stream) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!masks_dev) return fail(h, DEMI_ERR_INVALID, "demi_replay_batch_dev: null buffer");
+  return launch_replay(h, masks_dev, nullptr, n_masks, mask_words, looking_for, flags, out_dev, stream, nullptr, 0, nullptr);
 }
 
 extern "C" int32_t demi_replay_batch_ex(demi_handle* h, const uint64_t* masks, const uint32_t* skip_events, uint32_t n_tests,
@@ -297,31 +328,23 @@ extern "C" int32_t demi_replay_batch(demi_handle* h, const uint64_t* masks, uint
 
 // ---------------------------------------------------------------------- DDMin
 #include "ddmin_driver.hpp"
+
+int32_t replay_verdicts(demi_handle* h, const demi_replay_result* res, size_t n, signed char* out) {
+  for (size_t i = 0; i < n; i++) {
+    if (res[i].status != 0) return fail(h, DEMI_ERR_CAPACITY, "demi_ddmin: a replay reported status %u", (unsigned)res[i].status);
+    out[i] = res[i].violation != 0;
+  }
+  return DEMI_OK;
+}
+
 namespace {
 
 // STSSched as DDMin's TestOracle: a batch of masks = one replay launch
 struct StsDDMinDriver : DDMinDriver {
-  int32_t evaluate_flat(const uint64_t* masks, size_t n, signed char* out) override {   // the arena slice goes to the kernel as is
+  int32_t evaluate(const uint64_t* masks, size_t n, signed char* out) override {   // the slice goes to the kernel as is
     std::vector<demi_replay_result> res(n);
-    int32_t rc = demi_replay_batch(h, masks, (uint32_t)n, mw, looking_for, flags, res.data());
-    if (rc != DEMI_OK) return rc;
-    for (size_t i = 0; i < n; i++) {
-      if (res[i].status != 0) return fail(h, DEMI_ERR_CAPACITY, "demi_ddmin: a replay reported status %u", (unsigned)res[i].status);
-      out[i] = res[i].violation != 0;
-    }
-    return DEMI_OK;
-  }
-  int32_t evaluate_batch(const std::vector<Mask>& want, std::vector<char>& out) override {
-    std::vector<uint64_t> flat(want.size() * mw);
-    for (size_t i = 0; i < want.size(); i++) std::copy(want[i].begin(), want[i].end(), flat.begin() + i * mw);
-    std::vector<demi_replay_result> res(want.size());
-    int32_t rc = demi_replay_batch(h, flat.data(), (uint32_t)want.size(), mw, looking_for, flags, res.data());
-    if (rc != DEMI_OK) return rc;
-    for (size_t i = 0; i < want.size(); i++) {
-      if (res[i].status != 0) return fail(h, DEMI_ERR_CAPACITY, "demi_ddmin: a replay reported status %u", (unsigned)res[i].status);
-      out[i] = res[i].violation != 0;
-    }
-    return DEMI_OK;
+    const int32_t rc = demi_replay_batch(h, masks, (uint32_t)n, mw, looking_for, flags, res.data());
+    return rc != DEMI_OK ? rc : replay_verdicts(h, res.data(), n, out);
   }
 };
 

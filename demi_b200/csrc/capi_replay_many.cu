@@ -15,27 +15,10 @@
 #include "replay_kernel.cuh"
 #include "engine.hpp"
 #include "ddmin_driver.hpp"
-#include "models/model_ir.cuh"
 
 using namespace demi;
 
 namespace {
-
-typedef void (*replay_many_fn)(const ReplayArgs, const ReplayTraceView*, const uint4*, uint32_t, ReplayArgs*);
-struct ManyVariant { int model; int bd; replay_many_fn fn; size_t smem; int n_actors; };
-template <class MODEL, int BD>
-ManyVariant make_mv() {
-  using M = ReplayMachine<MODEL, BD>;
-  return ManyVariant{MODEL::ID, BD, replay_many_kernel<MODEL, BD>, (size_t)M::WORDS * BD * sizeof(uint32_t), MODEL::N_ACTORS};
-}
-// the block sizes of the single-trace kernels (capi_replay.cu)
-const ManyVariant* pick_mv(int model) {
-  static const std::vector<ManyVariant> v = {
-    make_mv<PingPong3, 256>(), make_mv<Raft5, 256>(), make_mv<Bcast32, 128>(), make_mv<IrModel, 128>(),
-  };
-  for (const ManyVariant& r : v) if (r.model == model) return &r;
-  return nullptr;
-}
 
 // tests per launch: larger unions are evaluated in several launches
 constexpr uint32_t MANY_MAX_TESTS = 1u << 20;
@@ -49,27 +32,25 @@ struct LaunchCounts { uint32_t launches = 0; uint64_t tests = 0, violations = 0,
 int32_t launch_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks, uint32_t n, uint32_t mw,
                     const uint32_t* looking_for, uint32_t flags, demi_replay_result* out, LaunchCounts& lc) {
   const auto& S = h->set;
-  const ManyVariant* mv = pick_mv(h->cfg.model);
-  if (!mv) return fail(h, DEMI_ERR_INVALID, "no replay kernel for model %d", h->cfg.model);
   // counting sort of the tests by the rank of their trace (longer traces first, then by index)
   std::vector<uint32_t> count(S.n + 1, 0);
   for (uint32_t i = 0; i < n; i++) count[trace_of_test[i]]++;
   std::vector<uint32_t> order_t;
   for (uint32_t t = 0; t < S.n; t++) if (count[t]) order_t.push_back(t);
-  std::stable_sort(order_t.begin(), order_t.end(), [&](uint32_t a, uint32_t b) { return S.n_events[a] > S.n_events[b]; });
+  std::stable_sort(order_t.begin(), order_t.end(), [&](uint32_t a, uint32_t b) { return S.view[a].n_events > S.view[b].n_events; });
   std::vector<uint32_t> first(S.n, 0);
   std::vector<uint4> tiles;
-  ReplayArgs a = replay_args(h, 0, flags);
-  a.table_slots = a.tosend_cap = a.n_uniq_words = a.pending_cap = 0;
+  ReplayTraceView geometry{};                       // the scratch's: the largest of the launch's traces
   uint32_t pos = 0;
   for (uint32_t t : order_t) {
     first[t] = pos;
     for (uint32_t k = 0; k < count[t]; k += 32) tiles.push_back(make_uint4(t, pos + k, std::min(32u, count[t] - k), looking_for[t]));
     pos += count[t];
-    a.table_slots = std::max(a.table_slots, S.table_slots[t]);
-    a.tosend_cap = std::max(a.tosend_cap, S.tosend_cap[t]);
-    a.n_uniq_words = std::max(a.n_uniq_words, S.n_uniq_words[t]);
-    a.pending_cap = std::max(a.pending_cap, S.pending_cap[t]);
+    const ReplayTraceView& v = S.view[t];
+    geometry.table_slots = std::max(geometry.table_slots, v.table_slots);
+    geometry.tosend_cap = std::max(geometry.tosend_cap, v.tosend_cap);
+    geometry.n_uniq_words = std::max(geometry.n_uniq_words, v.n_uniq_words);
+    geometry.pending_cap = std::max(geometry.pending_cap, v.pending_cap);
   }
   std::vector<uint32_t> slot(n);                    // test i runs at position slot[i] of the grouped order
   std::vector<uint64_t> grouped((size_t)n * mw);
@@ -79,29 +60,18 @@ int32_t launch_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_
   }
   cudaStream_t s = h->stream;
   int32_t rc;
-  int bps = 0;
-  if ((rc = demi_occupancy(h, (const void*)mv->fn, mv->bd, mv->smem, &bps)) != DEMI_OK) return rc;
-  if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
-  const uint32_t n_tiles = (uint32_t)tiles.size(), wpb = (uint32_t)mv->bd / 32;
-  const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((n_tiles + wpb - 1) / wpb, (uint64_t)h->sm_count * bps));
-  const uint64_t warps = (uint64_t)grid * wpb;
-  const uint32_t per_thread = (uint32_t)((n_tiles + warps - 1) / warps) + 1;
-  if ((rc = replay_scratch(h, a, warps, mv->n_actors, per_thread, false, s)) != DEMI_OK) return rc;
   const size_t mbytes = grouped.size() * sizeof(uint64_t), tbytes = tiles.size() * sizeof(uint4);
   const size_t rbytes = (size_t)n * sizeof(demi_replay_result);
   if ((rc = h->rp_masks.grow(h, mbytes + tbytes)) != DEMI_OK) return rc;
   if ((rc = h->rp_results.grow(h, rbytes)) != DEMI_OK) return rc;
-  if ((rc = h->rp_bound.grow(h, warps * sizeof(ReplayArgs))) != DEMI_OK) return rc;
   char* base = h->rp_masks.get<char>();
   CUDA_TRY(h, cudaMemcpyAsync(base, tiles.data(), tbytes, cudaMemcpyHostToDevice, s));
   CUDA_TRY(h, cudaMemcpyAsync(base + tbytes, grouped.data(), mbytes, cudaMemcpyHostToDevice, s));
+  ReplayArgs a = replay_args(h, geometry, 0, flags);
   a.masks = (const uint64_t*)(base + tbytes); a.n_masks = n; a.mask_words = mw;
   a.results = h->rp_results.get<demi_replay_result>();
-  if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
-  CUDA_TRY(h, cudaEventRecord(h->ev0, s));
-  mv->fn<<<grid, mv->bd, mv->smem, s>>>(a, S.views.get<ReplayTraceView>(), (const uint4*)base, n_tiles, h->rp_bound.get<ReplayArgs>());
-  CUDA_TRY(h, cudaGetLastError());
-  CUDA_TRY(h, cudaEventRecord(h->ev1, s));
+  const ReplayTiles many{S.views.get<ReplayTraceView>(), (const uint4*)base, (uint32_t)tiles.size()};
+  if ((rc = replay_launch(h, a, false, false, &many, true, s)) != DEMI_OK) return rc;
   std::vector<demi_replay_result> res(n);
   unsigned long long c[2] = {0, 0};
   CUDA_TRY(h, cudaMemcpyAsync(res.data(), a.results, rbytes, cudaMemcpyDeviceToHost, s));
@@ -148,7 +118,7 @@ struct Rendezvous {
 // STSSched as DDMin's TestOracle on trace `trace` of the set, as StsDDMinDriver (capi_replay.cu) on the single trace
 struct SetDDMinDriver : DDMinDriver {
   Rendezvous* R; uint32_t trace;
-  int32_t ask(const uint64_t* masks, size_t n, signed char* out) {
+  int32_t evaluate(const uint64_t* masks, size_t n, signed char* out) override {
     Request q; q.trace = trace; q.masks = masks; q.n = n;
     {
       std::unique_lock<std::mutex> lk(R->mu);
@@ -157,21 +127,7 @@ struct SetDDMinDriver : DDMinDriver {
       R->coord.notify_one();
       R->work.wait(lk, [&] { return q.done; });
     }
-    if (q.rc != DEMI_OK) return q.rc;
-    for (size_t i = 0; i < n; i++) {
-      if (q.res[i].status != 0) return fail(h, DEMI_ERR_CAPACITY, "demi_ddmin: a replay reported status %u", (unsigned)q.res[i].status);
-      out[i] = q.res[i].violation != 0;
-    }
-    return DEMI_OK;
-  }
-  int32_t evaluate_flat(const uint64_t* masks, size_t n, signed char* out) override { return ask(masks, n, out); }
-  int32_t evaluate_batch(const std::vector<Mask>& want, std::vector<char>& out) override {
-    std::vector<uint64_t> flat(want.size() * mw);
-    for (size_t i = 0; i < want.size(); i++) std::copy(want[i].begin(), want[i].end(), flat.begin() + i * mw);
-    std::vector<signed char> r(want.size(), 0);
-    const int32_t rc = ask(flat.data(), want.size(), r.data());
-    for (size_t i = 0; i < want.size(); i++) out[i] = r[i];
-    return rc;
+    return q.rc != DEMI_OK ? q.rc : replay_verdicts(h, q.res.data(), n, out);
   }
 };
 
@@ -189,12 +145,10 @@ extern "C" int32_t demi_set_traces(demi_handle* h, uint32_t n_traces,
   // the new set is built aside and replaces the old one only when every trace passed and every upload succeeded
   std::vector<demi_event> ev_all; std::vector<uint16_t> ord_all, sidx_all; std::vector<demi_ext_event> ext_all;
   std::vector<size_t> ev_off(n_traces), ext_off(n_traces), sidx_off(n_traces);
-  std::vector<uint32_t> n_sends(n_traces);
   std::map<std::pair<uint32_t, uint32_t>, std::pair<size_t, size_t>> ext_seen;   // a program shared by traces is stored once
   demi_handle::TraceSet S;
   S.n = n_traces;
-  S.ext.resize(n_traces); S.n_events.resize(n_traces);
-  S.n_uniq_words.resize(n_traces); S.pending_cap.resize(n_traces); S.tosend_cap.resize(n_traces); S.table_slots.resize(n_traces);
+  S.ext.resize(n_traces); S.view.resize(n_traces);
   char who[64];
   TraceTables t;
   for (uint32_t i = 0; i < n_traces; i++) {
@@ -215,13 +169,8 @@ extern "C" int32_t demi_set_traces(demi_handle* h, uint32_t n_traces,
       sidx_all.insert(sidx_all.end(), t.sidx.begin(), t.sidx.end());
     }
     ext_off[i] = it->second.first; sidx_off[i] = it->second.second;
-    n_sends[i] = (uint32_t)t.sidx.size();
     S.ext[i].assign(ex, ex + n_externals[i]);
-    S.n_events[i] = n_events[i];
-    S.n_uniq_words[i] = (t.n_uniq + 31) / 32;
-    S.pending_cap[i] = demi_replay_pending_cap(t.n_send_events);
-    S.tosend_cap[i] = demi_tosend_cap(n_sends[i]);
-    S.table_slots[i] = demi_pow2_at_least(2 * S.pending_cap[i], 256, 1u << 16);
+    S.view[i] = trace_view(t, n_events[i], n_externals[i]);
   }
   if (sidx_all.empty()) sidx_all.push_back(0);
   int32_t rc;
@@ -229,15 +178,12 @@ extern "C" int32_t demi_set_traces(demi_handle* h, uint32_t n_traces,
   if ((rc = S.ordinal.upload(h, ord_all.data(), ord_all.size() * sizeof(uint16_t))) != DEMI_OK) return rc;
   if ((rc = S.externals.upload(h, ext_all.data(), ext_all.size() * sizeof(demi_ext_event))) != DEMI_OK) return rc;
   if ((rc = S.send_index.upload(h, sidx_all.data(), sidx_all.size() * sizeof(uint16_t))) != DEMI_OK) return rc;
-  std::vector<ReplayTraceView> views(n_traces);
   for (uint32_t i = 0; i < n_traces; i++) {
-    ReplayTraceView& v = views[i];
+    ReplayTraceView& v = S.view[i];
     v.events = S.events.get<const uint4>() + ev_off[i]; v.ev_ordinal = S.ordinal.get<const uint16_t>() + ev_off[i];
     v.ext = S.externals.get<const uint4>() + ext_off[i]; v.send_ext_index = S.send_index.get<const uint16_t>() + sidx_off[i];
-    v.n_events = n_events[i]; v.n_ext = n_externals[i]; v.n_sends = n_sends[i]; v.n_uniq_words = S.n_uniq_words[i];
-    v.pending_cap = S.pending_cap[i]; v.tosend_cap = S.tosend_cap[i]; v.table_slots = S.table_slots[i]; v.pad = 0;
   }
-  if ((rc = S.views.upload(h, views.data(), views.size() * sizeof(ReplayTraceView))) != DEMI_OK) return rc;
+  if ((rc = S.views.upload(h, S.view.data(), S.view.size() * sizeof(ReplayTraceView))) != DEMI_OK) return rc;
   if ((rc = h->rp_counters.grow(h, 2 * sizeof(unsigned long long))) != DEMI_OK) return rc;
   h->set = std::move(S);
   return DEMI_OK;

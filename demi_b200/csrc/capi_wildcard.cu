@@ -57,34 +57,20 @@ int32_t wc_check_flags(demi_handle* h, const char* who, uint32_t flags) {
 }
 
 // One launch of n_tests wildcard tests.  Device inputs live in the replay buffers of capi_replay.cu; the list this
-// variant leaves in the table means the exact path clears the table before its next launch (rp_gen_next = 0).
+// variant leaves in the table means the exact path clears the table before its next launch.
 int32_t wc_launch(demi_handle* h, const WcTrace& t, const uint64_t* include_host, uint32_t n_tests, uint32_t looking_for,
                   uint32_t flags, demi_replay_result* out_host,
                   demi_event* rec_host, uint32_t rec_cap, uint32_t* n_rec,
                   uint32_t* ign_host, uint32_t ign_cap, uint32_t* n_ign) {
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  const ReplayVariant* wv = pick_rv(h->cfg.model);
-  if (!wv) return fail(h, DEMI_ERR_INVALID, "no replay kernel for model %d", h->cfg.model);
   const bool record = rec_host != nullptr;
   cudaStream_t s = h->stream;
-  replay_fn fn = wv->fn[1][record];
   int32_t rc;
-  int bps = 0;
-  if ((rc = demi_occupancy(h, (const void*)fn, wv->bd, wv->smem, &bps)) != DEMI_OK) return rc;
-  if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
   const uint32_t n_ext = (uint32_t)h->trace_ext_host.size();
-  ReplayArgs a = replay_args(h, looking_for, flags);
-  a.pending_cap = demi_wildcard_pending_cap(demi_model_key(h), (uint32_t)t.pos.size(), h->trace_n_ext_sends);
+  ReplayArgs a = replay_args(h, h->trace, looking_for, flags);
+  a.pending_cap = demi_wildcard_pending_cap(demi_model_key(h), (uint32_t)t.pos.size(), h->trace.n_sends);
   a.table_slots = a.pending_cap;                        // list storage (the kernel compacts it in place)
-  a.tosend_cap = demi_tosend_cap(h->trace_n_ext_sends);
-  // one list of table_slots uint4 per lane: keep the scratch under 4 GiB
-  const uint64_t warp_bytes = (uint64_t)a.table_slots * 32 * sizeof(uint4);
-  const uint64_t max_blocks = std::max<uint64_t>(1, (4ull << 30) / warp_bytes / (wv->bd / 32));
-  const uint64_t want = ((uint64_t)n_tests + wv->bd - 1) / wv->bd;
-  const int grid = record ? 1 : (int)std::max<uint64_t>(1, std::min<uint64_t>({want, (uint64_t)h->sm_count * bps, max_blocks}));
-  const uint64_t warps = (uint64_t)grid * (wv->bd / 32);
   a.masks = nullptr; a.n_masks = n_tests; a.mask_words = std::max<uint32_t>(1, (n_ext + 63) / 64);   // the full MCS
-  a.gen_base = 1;
   a.wc_words = t.words;
   std::copy(h->clock_incr, h->clock_incr + 8, a.wc_incr);
   const size_t ev_bytes = t.ev.size() * sizeof(uint32_t), inc_bytes = (size_t)n_tests * t.words * sizeof(uint64_t);
@@ -92,21 +78,12 @@ int32_t wc_launch(demi_handle* h, const WcTrace& t, const uint64_t* include_host
   const size_t ev_off = (inc_bytes + 15) & ~(size_t)15, cnt_off = (ev_off + ev_bytes + 15) & ~(size_t)15;
   if ((rc = h->rp_masks.grow(h, cnt_off + 16)) != DEMI_OK) return rc;
   if ((rc = h->rp_results.grow(h, (size_t)n_tests * sizeof(demi_replay_result))) != DEMI_OK) return rc;
-  if ((rc = h->rp_table.grow(h, warps * warp_bytes)) != DEMI_OK) return rc;
-  if ((rc = h->rp_tosend.grow(h, warps * a.tosend_cap * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
-  if (flags & DEMI_RF_FILTER_KNOWN_ABSENTS)
-    if ((rc = h->rp_pruned.grow(h, warps * (a.n_uniq_words + wv->n_actors) * 32 * sizeof(uint32_t))) != DEMI_OK) return rc;
-  h->rp_gen_next = 0;
   char* base = h->rp_masks.get<char>();
   uint32_t* counts = (uint32_t*)(base + cnt_off);
   CUDA_TRY(h, cudaMemcpyAsync(base, include_host, inc_bytes, cudaMemcpyHostToDevice, s));
   CUDA_TRY(h, cudaMemcpyAsync(base + ev_off, t.ev.data(), ev_bytes, cudaMemcpyHostToDevice, s));
   a.wc_include = (const uint64_t*)base; a.wc_ev = (const uint32_t*)(base + ev_off);
   a.results = h->rp_results.get<demi_replay_result>();
-  a.table = h->rp_table.get<uint4>(); a.tosend = h->rp_tosend.get<uint32_t>();
-  a.pruned = (flags & DEMI_RF_FILTER_KNOWN_ABSENTS) ? h->rp_pruned.get<uint32_t>() : nullptr;
-  CUDA_TRY(h, cudaMemsetAsync(h->rp_counters.get(), 0, 2 * sizeof(unsigned long long), s));
-  a.counters = h->rp_counters.get<unsigned long long>();
   DevBuf d_rec, d_ign;
   if (record) {
     if ((rc = d_rec.grow(h, (size_t)rec_cap * sizeof(demi_event))) != DEMI_OK) return rc;
@@ -115,11 +92,7 @@ int32_t wc_launch(demi_handle* h, const WcTrace& t, const uint64_t* include_host
     a.rec_events = d_rec.get<demi_event>(); a.rec_cap = rec_cap; a.rec_count = counts;
     a.wc_ignored = d_ign.get<uint32_t>(); a.wc_ignored_cap = ign_cap; a.wc_ignored_count = counts + 1;
   }
-  CUDA_TRY(h, replay_ir_bind(h, s));
-  CUDA_TRY(h, cudaEventRecord(h->ev0, s));
-  fn<<<grid, wv->bd, wv->smem, s>>>(a);
-  CUDA_TRY(h, cudaGetLastError());
-  CUDA_TRY(h, cudaEventRecord(h->ev1, s));
+  if ((rc = replay_launch(h, a, true, record, nullptr, true, s)) != DEMI_OK) return rc;
   CUDA_TRY(h, cudaMemcpyAsync(out_host, a.results, (size_t)n_tests * sizeof(demi_replay_result), cudaMemcpyDeviceToHost, s));
   uint32_t c[2] = {0, 0};
   if (record) CUDA_TRY(h, cudaMemcpyAsync(c, counts, sizeof(c), cudaMemcpyDeviceToHost, s));

@@ -86,14 +86,8 @@ struct DDMinDriver {
     if (dag_nodes[d].child[k] < 0) { const int32_t c = dag_of(dag_nodes[d].hv[k]); dag_nodes[d].child[k] = c; }
     return dag_nodes[d].child[k];
   }
-  // the oracle over a flat slice of masks (default: through evaluate_batch)
-  virtual int32_t evaluate_flat(const uint64_t* masks, size_t n, signed char* out) {
-    std::vector<Mask> want(n, Mask(mw)); std::vector<char> r(n, 0);
-    for (size_t i = 0; i < n; i++) std::copy(masks + i * mw, masks + (i + 1) * mw, want[i].begin());
-    int32_t rc = evaluate_batch(want, r);
-    for (size_t i = 0; i < n; i++) out[i] = r[i];
-    return rc;
-  }
+  // the oracle: out[i] = "test(mask i) reproduces the violation" for the n masks of mw words each at `masks`
+  virtual int32_t evaluate(const uint64_t* masks, size_t n, signed char* out) = 0;
   struct Frame { int32_t dag; uint32_t rem; };                  // rem: index into rem_arena
   std::vector<uint64_t> rem_arena;
   // evaluates m and, level by level, the tests the recursion below (dag, rem) — and the waiting siblings — can ask for
@@ -132,7 +126,7 @@ struct DDMinDriver {
     const size_t n_new = wt.size() - first_new;
     if (!n_new) return;
     const auto tq1 = std::chrono::steady_clock::now();
-    int32_t rc = evaluate_flat(&wt.arena[first_new * mw], n_new, &wt.res[first_new]);
+    int32_t rc = evaluate(&wt.arena[first_new * mw], n_new, &wt.res[first_new]);
     const auto tq2 = std::chrono::steady_clock::now();
     spec_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(tq1 - tq0).count();
     eval_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(tq2 - tq1).count();
@@ -217,18 +211,19 @@ struct DDMinDriver {
     expand(hv[1], unite(hv[0], rem), depth - 1, want);
   }
 
-  // the oracle: fill `out[i]` = "test(want[i]) reproduces the violation" for the whole batch
-  virtual int32_t evaluate_batch(const std::vector<Mask>& want, std::vector<char>& out) = 0;
   // the sequential walk consumed the result of test(m)
   virtual void consumed(const Mask&) {}
   virtual ~DDMinDriver() {}
 
-  void evaluate(std::vector<Mask>& want) {
+  // fills the memo with the results of the distinct masks of `want`
+  void evaluate_memo(std::vector<Mask>& want) {
     std::sort(want.begin(), want.end());
     want.erase(std::unique(want.begin(), want.end()), want.end());
     if (want.empty()) return;
-    std::vector<char> res(want.size(), 0);
-    int32_t rc = evaluate_batch(want, res);
+    std::vector<uint64_t> flat(want.size() * mw);
+    for (size_t i = 0; i < want.size(); i++) std::copy(want[i].begin(), want[i].end(), flat.begin() + i * mw);
+    std::vector<signed char> res(want.size(), 0);
+    int32_t rc = evaluate(flat.data(), want.size(), res.data());
     if (rc != DEMI_OK) { error = rc; return; }
     for (size_t i = 0; i < want.size(); i++) memo[want[i]] = res[i] != 0;
     replays_executed += (uint32_t)want.size();
@@ -253,7 +248,7 @@ struct DDMinDriver {
       expand(cur_dag, cur_rem, depth, want);
       for (auto it2 = pending_siblings.rbegin(); it2 != pending_siblings.rend() && want.size() < BATCH_TARGET; ++it2)
         expand(it2->first, it2->second, 3, want);
-      evaluate(want);
+      evaluate_memo(want);
       if (error != DEMI_OK) return false;
       it = memo.find(m);
     }

@@ -14,6 +14,7 @@
 #include "../../include/demi_limits.h"
 #include "../../include/demi_model_ir.h"
 #include "lane_steady.hpp"
+#include "replay_trace.hpp"
 
 extern thread_local std::string g_create_error;
 
@@ -83,11 +84,10 @@ struct demi_handle {
   // ---- STSSched replay / DDMin (capi_replay.cu)
   std::vector<demi_event> trace_host;
   std::vector<demi_ext_event> trace_ext_host;
-  std::vector<uint16_t> send_ext_index_host;
   std::vector<int32_t> conjoined;          // UnmodifiedEventDag._conjoinedAtoms over trace_ext_host (demi_conjoin_atoms)
   DevBuf trace_dev, trace_ext_dev;                 // trace_host, trace_ext_host
   DevBuf ev_ordinal_dev, send_ext_index_dev;       // uint16_t
-  uint32_t trace_n_uniq = 0, trace_n_send_events = 0, trace_n_ext_sends = 0;
+  demi::ReplayTraceView trace{};                   // the trace as K2 reads it: its counts, capacities and the buffers above
   DevBuf rp_table; uint32_t rp_gen_next = 0; uint64_t rp_table_geometry = 0;
   DevBuf rp_tosend, rp_pruned, rp_masks, rp_results;
   DevBuf rp_counters;                              // unsigned long long[2]
@@ -96,10 +96,9 @@ struct demi_handle {
   struct TraceSet {
     uint32_t n = 0;
     std::vector<std::vector<demi_ext_event>> ext;      // per trace: its externals (DDMin's atoms)
-    std::vector<uint32_t> n_events;
     DevBuf events, ordinal, externals, send_index;   // every trace's records, one after the other
-    DevBuf views;                                    // demi::ReplayTraceView[n]
-    std::vector<uint32_t> n_uniq_words, pending_cap, tosend_cap, table_slots;
+    std::vector<demi::ReplayTraceView> view;         // per trace: its view of the buffers above
+    DevBuf views;                                    // view, on the device
   } set;
   // ---- communicator (capi_frontier.cu): NCCL inside the library
   void* comm = nullptr;
@@ -127,16 +126,17 @@ struct demi_handle {
   std::map<const void*, int> occupancy;          // kernel -> resident blocks per SM (asked once per handle)
   DevBuf trace_rec;                              // demi_fuzz_trace's recording buffer
 };
-// K2, STSSched replay (capi_replay.cu), for both the exact replays and the wildcard replays (capi_wildcard.cu): per
-// model the block size, the shared memory and the four instantiations of replay_lane_kernel, fn[WILD][REC]
+// K2, STSSched replay (capi_replay.cu): the ReplayArgs fields that follow from the handle's configuration and `trace`;
+// the rest are zero
 namespace demi { struct ReplayArgs; }
-typedef void (*replay_fn)(const demi::ReplayArgs);
-struct ReplayVariant { int model; int bd; replay_fn fn[2][2]; size_t smem; int n_actors; };
-const ReplayVariant* pick_rv(int model);
-// the ReplayArgs fields that follow from the handle's configuration and its trace (demi_set_trace); the rest are zero
-demi::ReplayArgs replay_args(const demi_handle* h, uint32_t looking_for, uint32_t flags);
-// binds the handle's loaded model to the replay kernels: model_ir.cuh keeps one copy of it per translation unit
-cudaError_t replay_ir_bind(const demi_handle* h, cudaStream_t s);
+demi::ReplayArgs replay_args(const demi_handle* h, const demi::ReplayTraceView& trace, uint32_t looking_for, uint32_t flags);
+// the multi-trace kernel's own arguments: the set's views and the launch's tiles (capi_replay_many.cu)
+struct ReplayTiles { const demi::ReplayTraceView* views; const uint4* tiles; uint32_t n_tiles; };
+// Every K2 launch: the WILD or exact, REC or batch single-trace kernel, or with `many` the multi-trace kernel, on a's
+// tests; the grid, the per-warp scratch, the generation range and the counters, the loaded model's binding.  `timed`
+// records h->ev0 and h->ev1 around the kernel alone.
+int32_t replay_launch(demi_handle* h, demi::ReplayArgs& a, bool wild, bool record, const ReplayTiles* many, bool timed,
+                      cudaStream_t s);
 // what demi_set_trace checks of a trace before it builds its side tables; `who` leads every message
 int32_t check_trace(demi_handle* h, const char* who, const demi_event* events, uint32_t n_events,
                     const demi_ext_event* externals, uint32_t n_externals);
@@ -145,9 +145,10 @@ int32_t check_trace(demi_handle* h, const char* who, const demi_event* events, u
 struct TraceTables { std::vector<uint16_t> ordinal, sidx; uint32_t n_uniq = 0, n_send_events = 0; };
 int32_t trace_tables(demi_handle* h, const char* who, const demi_event* events, uint32_t n_events,
                      const demi_ext_event* externals, uint32_t n_externals, TraceTables& t);
-// the per-warp scratch, generation range and counters of a K2 launch (capi_replay.cu)
-int32_t replay_scratch(demi_handle* h, demi::ReplayArgs& a, uint64_t warps, int n_actors, uint32_t per_thread, bool record,
-                       cudaStream_t s);
+// the counts and capacities of a trace's view (its buffers are the caller's)
+demi::ReplayTraceView trace_view(const TraceTables& t, uint32_t n_events, uint32_t n_externals);
+// DDMin's verdicts on n replays: out[i] = "replay i reproduced the violation"; a replay that reported a status fails
+int32_t replay_verdicts(demi_handle* h, const demi_replay_result* res, size_t n, signed char* out);
 // demi_ddmin's walk over a driver whose oracle, trace and flags are set: check_unmodified, ddmin2, verify_mcs, outputs
 namespace demi { struct DDMinDriver; }
 int32_t ddmin_sts(demi::DDMinDriver& d, int32_t check_unmodified, uint64_t* mcs_mask, uint32_t* iteration_sizes,

@@ -20,6 +20,7 @@
 // {hdr,p0,p1,generation|count} in HBM, interleaved per warp.
 #pragma once
 #include "actor_step.cuh"
+#include "replay_trace.hpp"
 
 namespace demi {
 
@@ -56,6 +57,18 @@ struct ReplayArgs {
   uint32_t* wc_ignored; uint32_t wc_ignored_cap; uint32_t* wc_ignored_count;
 };
 enum : uint32_t { WC_EXACT = 0, WC_CLASS = 1, WC_CLOCK = 2 };   // match mode of one delivery of the base trace
+
+// a's trace: the host binds the single trace (demi_set_trace), replay_many_kernel each tile's trace of a set
+__host__ __device__ __forceinline__ void bind_trace(ReplayArgs& a, const ReplayTraceView& v) {
+  a.events = v.events; a.n_events = v.n_events; a.ev_ordinal = v.ev_ordinal;
+  a.ext = v.ext; a.n_ext = v.n_ext; a.send_ext_index = v.send_ext_index; a.n_sends = v.n_sends;
+  a.n_uniq_words = v.n_uniq_words; a.pending_cap = v.pending_cap; a.tosend_cap = v.tosend_cap;
+  a.table_slots = v.table_slots;
+}
+
+// K2's block size per model: a test's actor states are thread-interleaved in shared memory, so the models of more than
+// eight actors (bcast32, a loaded model) run half the threads per block
+template <class MODEL> constexpr int replay_block = MODEL::N_ACTORS <= 8 ? 256 : 128;
 
 // WILD: ClockClusterizer's wildcarded trace (capi_wildcard.cu).  The pending set is the insertion-ordered list of
 // the REC variant (Uniq order = list order), compacted in place when taken entries dominate it.
@@ -433,7 +446,52 @@ struct ReplayMachine : TimerTable<MODEL> {
     for (uint32_t i = 0; i < N * SW; i++) sh += demi_state_term(smw[i * BD], i);
     out.state_hash = sh + rhash;
   }
+
+  // ---- the per-thread skeleton of K2's kernels.  This thread's shared memory and its lane of warp gwarp's scratch,
+  // laid out by `scratch`'s geometry; A is what the tests read.
+  __device__ __forceinline__ void bind(uint32_t* smem, const ReplayArgs* a, const ReplayArgs& scratch, uint64_t gwarp,
+                                       uint32_t lane) {
+    smw = smem;
+    A = a;
+    table = scratch.table + gwarp * (uint64_t)scratch.table_slots * 32 + lane;
+    tosend = scratch.tosend + gwarp * (uint64_t)scratch.tosend_cap * 32 + lane;
+    pruned = scratch.pruned ? scratch.pruned + gwarp * (uint64_t)(scratch.n_uniq_words + N) * 32 + lane : nullptr;
+  }
+  // The next test's generation.  Generations continue across launches (the host hands out disjoint ranges), so the
+  // table needs no clearing between launches; on wrap-around this thread clears its own slots.
+  __device__ __forceinline__ void next_generation(uint32_t& generation, const ReplayArgs& scratch) {
+    generation++;
+    if (generation >= 0xFFFFu) {
+      for (uint32_t s = 0; s < scratch.table_slots; s++) table[(size_t)s * 32] = make_uint4(0, 0, 0, 0);
+      generation = 1;
+    }
+  }
+  // runs test idx, stores its result to launch.results[idx] in one 16-byte store and counts it
+  template <class IDX>
+  __device__ __forceinline__ void run_store(IDX idx, uint32_t generation, const ReplayArgs& launch,
+                                            unsigned long long& repro, unsigned long long& deliv) {
+    demi_replay_result r;
+    run((uint32_t)idx, generation, r);
+    reinterpret_cast<uint4*>(launch.results + idx)[0] =
+        make_uint4((uint32_t)r.violation | ((uint32_t)r.status << 16), (uint32_t)r.delivered | ((uint32_t)r.ignored << 16),
+                   (uint32_t)r.state_hash, (uint32_t)(r.state_hash >> 32));
+    repro += (r.status == 0 && r.violation) ? 1u : 0u;
+    deliv += r.delivered;
+  }
 };
+
+// adds a warp's counts to the launch's counters: [0] reproduced, [1] delivered
+__device__ __forceinline__ void replay_count(const ReplayArgs& args, unsigned long long& repro, unsigned long long& deliv,
+                                             uint32_t lane) {
+  for (int o = 16; o > 0; o >>= 1) {
+    repro += __shfl_xor_sync(FULL_MASK, repro, o);
+    deliv += __shfl_xor_sync(FULL_MASK, deliv, o);
+  }
+  if (lane == 0 && args.counters && (repro | deliv)) {
+    atomicAdd(args.counters, repro);
+    atomicAdd(args.counters + 1, deliv);
+  }
+}
 
 template <class MODEL, int BD, bool REC = false, bool WILD = false>
 __global__ void __launch_bounds__(BD, (model_replay_direct<MODEL>::value && MODEL::N_ACTORS <= 8) ? 1024 / BD : 1)
@@ -443,52 +501,18 @@ replay_lane_kernel(const __grid_constant__ ReplayArgs args) {
   const uint32_t tid = threadIdx.x;
   const uint64_t gthread = (uint64_t)blockIdx.x * BD + tid;
   const uint64_t total = (uint64_t)gridDim.x * BD;
-  const uint64_t gwarp = gthread >> 5;
   const uint32_t lane = tid & 31;
 
   M m;
-  m.smw = lane_smem + tid;
-  m.A = &args;
-  m.table = args.table + gwarp * (uint64_t)args.table_slots * 32 + lane;
-  m.tosend = args.tosend + gwarp * (uint64_t)args.tosend_cap * 32 + lane;
-  m.pruned = args.pruned ? args.pruned + gwarp * (uint64_t)(args.n_uniq_words + M::N) * 32 + lane : nullptr;
-
+  m.bind(lane_smem + tid, &args, args, gthread >> 5, lane);
   unsigned long long my_repro = 0, my_deliv = 0;
-  // generations continue across launches (the host hands out disjoint ranges), so the table needs no
-  // clearing between launches; on wrap-around this thread clears its own slots
   uint32_t generation = args.gen_base - 1;
   for (uint64_t idx = gthread; idx < args.n_masks; idx += total) {
-    generation++;
-    if (generation >= 0xFFFFu) {
-      for (uint32_t s = 0; s < args.table_slots; s++) m.table[(size_t)s * 32] = make_uint4(0, 0, 0, 0);
-      generation = 1;
-    }
-    demi_replay_result r;
-    m.run((uint32_t)idx, generation, r);
-    uint4* dst = reinterpret_cast<uint4*>(args.results + idx);
-    dst[0] = make_uint4((uint32_t)r.violation | ((uint32_t)r.status << 16),
-                        (uint32_t)r.delivered | ((uint32_t)r.ignored << 16),
-                        (uint32_t)r.state_hash, (uint32_t)(r.state_hash >> 32));
-    my_repro += (r.status == 0 && r.violation) ? 1u : 0u;
-    my_deliv += r.delivered;
+    m.next_generation(generation, args);
+    m.run_store(idx, generation, args, my_repro, my_deliv);
   }
-  for (int o = 16; o > 0; o >>= 1) {
-    my_repro += __shfl_xor_sync(FULL_MASK, my_repro, o);
-    my_deliv += __shfl_xor_sync(FULL_MASK, my_deliv, o);
-  }
-  if (lane == 0 && args.counters && (my_repro | my_deliv)) {
-    atomicAdd(args.counters, my_repro);
-    atomicAdd(args.counters + 1, my_deliv);
-  }
+  replay_count(args, my_repro, my_deliv, lane);
 }
-
-// One trace of a set (demi_set_traces): the ReplayArgs fields that differ from trace to trace.  The capacities are the
-// trace's own, so that every test reports the status it would report with that trace alone.
-struct ReplayTraceView {
-  const uint4* events; const uint16_t* ev_ordinal; const uint4* ext; const uint16_t* send_ext_index;
-  uint32_t n_events, n_ext, n_sends, n_uniq_words;
-  uint32_t pending_cap, tosend_cap, table_slots, pad;
-};
 
 // K2 over many traces.  A tile {trace, first test, tests (<= 32), looking_for} belongs to one warp, so the trace stays
 // warp-uniform and the lanes walk it in lock-step as in replay_lane_kernel; warps take tiles grid-stride.  `args`
@@ -511,49 +535,20 @@ replay_many_kernel(const __grid_constant__ ReplayArgs args, const ReplayTraceVie
   if (lane == 0) la = args;
   __syncwarp();
   M m;
-  m.smw = lane_smem + tid;
-  m.A = &la;
-  m.table = args.table + gwarp * (uint64_t)args.table_slots * 32 + lane;
-  m.tosend = args.tosend + gwarp * (uint64_t)args.tosend_cap * 32 + lane;
-  m.pruned = args.pruned ? args.pruned + gwarp * (uint64_t)(args.n_uniq_words + M::N) * 32 + lane : nullptr;
-
+  m.bind(lane_smem + tid, &la, args, gwarp, lane);
   unsigned long long my_repro = 0, my_deliv = 0;
   uint32_t generation = args.gen_base - 1;
   for (uint64_t t = gwarp; t < n_tiles; t += total_warps) {
     const uint4 tile = tiles[t];
     __syncwarp();                                  // every lane is done with the previous tile's trace
-    if (lane == 0) {
-      const ReplayTraceView& v = views[tile.x];
-      la.events = v.events; la.n_events = v.n_events; la.ev_ordinal = v.ev_ordinal;
-      la.ext = v.ext; la.n_ext = v.n_ext; la.send_ext_index = v.send_ext_index; la.n_sends = v.n_sends;
-      la.n_uniq_words = v.n_uniq_words; la.pending_cap = v.pending_cap; la.tosend_cap = v.tosend_cap;
-      la.table_slots = v.table_slots; la.looking_for = tile.w;
-    }
+    if (lane == 0) { bind_trace(la, views[tile.x]); la.looking_for = tile.w; }
     __syncwarp();
     if (lane >= tile.z) continue;
-    generation++;
-    if (generation >= 0xFFFFu) {
-      for (uint32_t s = 0; s < args.table_slots; s++) m.table[(size_t)s * 32] = make_uint4(0, 0, 0, 0);
-      generation = 1;
-    }
+    m.next_generation(generation, args);
     const uint32_t idx = tile.y + lane;
-    demi_replay_result r;
-    m.run(idx, generation, r);
-    uint4* dst = reinterpret_cast<uint4*>(args.results + idx);
-    dst[0] = make_uint4((uint32_t)r.violation | ((uint32_t)r.status << 16),
-                        (uint32_t)r.delivered | ((uint32_t)r.ignored << 16),
-                        (uint32_t)r.state_hash, (uint32_t)(r.state_hash >> 32));
-    my_repro += (r.status == 0 && r.violation) ? 1u : 0u;
-    my_deliv += r.delivered;
+    m.run_store(idx, generation, args, my_repro, my_deliv);
   }
-  for (int o = 16; o > 0; o >>= 1) {
-    my_repro += __shfl_xor_sync(FULL_MASK, my_repro, o);
-    my_deliv += __shfl_xor_sync(FULL_MASK, my_deliv, o);
-  }
-  if (lane == 0 && args.counters && (my_repro | my_deliv)) {
-    atomicAdd(args.counters, my_repro);
-    atomicAdd(args.counters + 1, my_deliv);
-  }
+  replay_count(args, my_repro, my_deliv, lane);
 }
 
 }  // namespace demi

@@ -13,10 +13,10 @@ using namespace demi;
 
 struct SupersetDriver : DDMinDriver {
   Mask K;
-  int32_t evaluate_batch(const std::vector<Mask>& want, std::vector<char>& out) override {
-    for (size_t i = 0; i < want.size(); i++) {
+  int32_t evaluate(const uint64_t* masks, size_t n, signed char* out) override {
+    for (size_t i = 0; i < n; i++) {
       bool all = true;
-      for (uint32_t w = 0; w < mw; w++) all = all && (want[i][w] & K[w]) == K[w];
+      for (uint32_t w = 0; w < mw; w++) all = all && (masks[i * mw + w] & K[w]) == K[w];
       out[i] = all;
     }
     return DEMI_OK;

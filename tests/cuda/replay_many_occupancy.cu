@@ -1,5 +1,5 @@
 // Resident blocks per SM of the multi-trace K2 kernel next to the single-trace one, per model, at the block size and
-// dynamic shared memory the C ABI launches them with (capi_replay.cu, capi_replay_many.cu).  Prints one line per model:
+// dynamic shared memory the C ABI launches them with (replay_block, capi_replay.cu).  Prints one line per model:
 // "<model> <single> <many>".
 #include <cstdio>
 #include "../../demi_b200/csrc/replay_kernel.cuh"
@@ -7,8 +7,9 @@
 
 using namespace demi;
 
-template <class MODEL, int BD>
+template <class MODEL>
 static int report(const char* name) {
+  constexpr int BD = replay_block<MODEL>;
   const size_t smem = (size_t)ReplayMachine<MODEL, BD>::WORDS * BD * sizeof(uint32_t);
   const void* fns[2] = {(const void*)replay_lane_kernel<MODEL, BD, false, false>, (const void*)replay_many_kernel<MODEL, BD>};
   int bps[2] = {0, 0};
@@ -21,7 +22,6 @@ static int report(const char* name) {
 }
 
 int main() {
-  int rc = report<PingPong3, 256>("pingpong3") | report<Raft5, 256>("raft5") | report<Bcast32, 128>("bcast32") |
-           report<IrModel, 128>("ir");
+  int rc = report<PingPong3>("pingpong3") | report<Raft5>("raft5") | report<Bcast32>("bcast32") | report<IrModel>("ir");
   return rc;
 }

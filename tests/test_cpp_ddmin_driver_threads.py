@@ -7,7 +7,7 @@ SRC = os.path.join(ROOT, "tests", "cpp", "ddmin_driver_threads_test.cpp")
 CUDA = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 
 
-def test_ddmin_driver_threads_asan(tmp_path):
+def test_ddmin_drivers_on_threads_match_solo_runs_asan(tmp_path):
     exe = os.path.join(str(tmp_path), "ddmin_driver_threads_test")
     subprocess.check_call(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=address", "-fno-omit-frame-pointer", "-pthread",
                            "-I" + os.path.join(CUDA, "include"), SRC, "-o", exe, "-L" + os.path.join(CUDA, "lib64"),
