@@ -161,7 +161,6 @@ extern "C" int32_t demi_create(const demi_config* cfg, demi_handle** out) {
   int32_t rc = e == cudaSuccess ? DEMI_OK : fail(nullptr, DEMI_ERR_CUDA, "demi_create: %s", cudaGetErrorString(e));
   // no handle yet: a failure goes to demi_last_error(NULL)
   if (rc == DEMI_OK) rc = h->counters_dev.grow(nullptr, 4 * sizeof(unsigned long long));
-  if (rc == DEMI_OK) rc = h->rec_counts_dev.grow(nullptr, 4 * sizeof(uint32_t));
   if (rc == DEMI_OK) rc = h->ovf_count.grow(nullptr, sizeof(uint32_t));
   if (rc != DEMI_OK) {
     demi_destroy(h);                       // frees whatever was created before the failure
@@ -606,6 +605,57 @@ extern "C" int32_t demi_fuzz_summary_dev(demi_handle* h, const void* /*results_d
   return DEMI_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Recording: the records both engines write in an LM_RECORD launch (KernelArgs::rec_*) and the provenance kernel
+// reads.  Slot i owns events[i*rec_cap ..), parents[i*par_cap ..), counts[i*4 ..) = {n_events, n_nodes, affectedNodes,
+// violation} and results[i]; with a work list it runs execution seed_base + list[i], else seed_base + i.
+struct Records {
+  demi_event* events; uint16_t* parents; uint32_t* counts; demi_fuzz_result* results;
+  unsigned char* extra; uint32_t rec_cap, par_cap;      // extra: the caller's bytes per slot, after the records
+};
+
+static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+
+// Slots per recording launch, so that what stage_records lays out (`extra` per slot included) stays within ~4 GB
+static uint32_t record_chunk(uint32_t rec_cap, uint32_t par_cap, size_t extra) {
+  const size_t per_slot = (size_t)rec_cap * sizeof(demi_event) + (size_t)par_cap * 2 + 16 + sizeof(demi_fuzz_result) + 4;
+  return (uint32_t)std::max<size_t>(1, ((size_t)4 << 30) / (per_slot + extra));
+}
+
+// Lays out the records of n slots in `buf`, grown to fit, each region 16-byte aligned: events | parents | counts |
+// results | work list | its length | `extra` bytes per slot.  par_cap 0 records no parents (the warp engine alone
+// allows it).  With a work list (`list`, n host entries) the list is uploaded, counts and results start cleared and
+// the launch leaves the handle's counters alone.  Binds plan->args when a plan is given.
+static int32_t stage_records(demi_handle* h, LaunchPlan* plan, uint32_t n, const uint32_t* list, uint32_t rec_cap,
+                             uint32_t par_cap, size_t extra, DevBuf& buf, Records* r, cudaStream_t s) {
+  const size_t b_ev = (size_t)n * rec_cap * sizeof(demi_event), b_par = align16((size_t)n * par_cap * 2), b_cnt = (size_t)n * 16,
+               b_res = (size_t)n * sizeof(demi_fuzz_result), b_list = align16((size_t)n * 4);
+  const int32_t rc = buf.grow(h, b_ev + b_par + b_cnt + b_res + b_list + 16 + (size_t)n * extra);
+  if (rc != DEMI_OK) return rc;
+  unsigned char* p = buf.get<unsigned char>();
+  r->events = (demi_event*)p;          p += b_ev;
+  r->parents = (uint16_t*)p;           p += b_par;
+  r->counts = (uint32_t*)p;            p += b_cnt;
+  r->results = (demi_fuzz_result*)p;   p += b_res;
+  uint32_t* d_list = (uint32_t*)p;     p += b_list;
+  uint32_t* d_len = (uint32_t*)p;      p += 16;
+  r->extra = p; r->rec_cap = rec_cap; r->par_cap = par_cap;
+  if (list) {
+    CUDA_TRY(h, cudaMemcpyAsync(d_list, list, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(h, cudaMemcpyAsync(d_len, &n, 4, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(h, cudaMemsetAsync(r->counts, 0, b_cnt, s));
+    CUDA_TRY(h, cudaMemsetAsync(r->results, 0xFF, b_res, s));
+  }
+  if (plan) {
+    KernelArgs& a = plan->args;
+    a.results = r->results; a.rec_counts = r->counts;
+    a.rec_events = r->events; a.rec_cap = rec_cap;
+    a.rec_parent = par_cap ? r->parents : nullptr; a.rec_parent_cap = par_cap;
+    if (list) { a.index_list = d_list; a.index_count = d_len; a.sum_steps = nullptr; a.n_violations = nullptr; }
+  }
+  return DEMI_OK;
+}
+
 // demi_fuzz_trace over the program (ext, n_ext) that `prog` describes: one prefix, recorded by the warp engine
 static int32_t fuzz_trace(demi_handle* h, const demi_fuzz_params* p, int64_t seed, demi_event* events, uint32_t cap_events,
                           uint32_t* n_events, uint16_t* dep_parent, uint32_t cap_nodes, uint32_t* n_nodes, demi_fuzz_result* result,
@@ -618,35 +668,25 @@ static int32_t fuzz_trace(demi_handle* h, const demi_fuzz_params* p, int64_t see
   LaunchPlan plan;
   int32_t rc = plan_launch(h, &q, LM_RECORD, prog, ext, n_ext, &plan);
   if (rc != DEMI_OK) return rc;
-  const uint32_t cap_ev = std::max<uint32_t>(cap_events, 1), cap_n = std::max<uint32_t>(cap_nodes, 1);
-  // one recording buffer, kept in the handle: events | parents | result
-  const size_t o_par = (size_t)cap_ev * sizeof(demi_event), o_res = (o_par + (size_t)cap_n * 2 + 15) & ~(size_t)15;
-  if ((rc = h->trace_rec.grow(h, o_res + sizeof(demi_fuzz_result))) != DEMI_OK) return rc;
-  demi_event* ev_dev = h->trace_rec.get<demi_event>();
-  uint16_t* par_dev = (uint16_t*)(h->trace_rec.get<unsigned char>() + o_par);
-  demi_fuzz_result* res_dev = (demi_fuzz_result*)(h->trace_rec.get<unsigned char>() + o_res);
-  plan.args.results = res_dev;
-  plan.args.rec_events = ev_dev; plan.args.rec_cap = cap_events;
-  plan.args.rec_counts = h->rec_counts_dev.get<uint32_t>();
-  plan.args.rec_parent = dep_parent ? par_dev : nullptr; plan.args.rec_parent_cap = cap_nodes;
+  Records rec;
+  if ((rc = stage_records(h, &plan, 1, nullptr, cap_events, dep_parent ? cap_nodes : 0, 0, h->trace_rec, &rec, h->stream)) != DEMI_OK) return rc;
   CUDA_TRY(h, cudaMemsetAsync(h->counters_dev.get(), 0, 4 * sizeof(unsigned long long), h->stream));
   if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, h->stream));
   plan.v->fn[LM_RECORD]<<<1, WARPS * 32, plan.smem, h->stream>>>(plan.args);
   cudaError_t e = cudaGetLastError();
-  demi_fuzz_result r{}; uint32_t counts[4] = {0, 0, 0, 0};
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&r, res_dev, sizeof(r), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(counts, h->rec_counts_dev.get(), sizeof(counts), cudaMemcpyDeviceToHost, h->stream);
+  struct { uint32_t counts[4]; demi_fuzz_result r; } got{};          // one slot's counts and result lie side by side
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&got, rec.counts, sizeof(got), cudaMemcpyDeviceToHost, h->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-  if (e == cudaSuccess && r.status == 0) {
-    e = cudaMemcpy(events, ev_dev, (size_t)std::min(counts[0], cap_events) * sizeof(demi_event), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess && got.r.status == 0) {
+    e = cudaMemcpy(events, rec.events, (size_t)std::min(got.counts[0], cap_events) * sizeof(demi_event), cudaMemcpyDeviceToHost);
     if (e == cudaSuccess && dep_parent)
-      e = cudaMemcpy(dep_parent, par_dev, (size_t)std::min(counts[1], cap_nodes) * sizeof(uint16_t), cudaMemcpyDeviceToHost);
+      e = cudaMemcpy(dep_parent, rec.parents, (size_t)std::min(got.counts[1], cap_nodes) * sizeof(uint16_t), cudaMemcpyDeviceToHost);
   }
   if (e != cudaSuccess) return fail(h, DEMI_ERR_CUDA, "demi_fuzz_trace: %s", cudaGetErrorString(e));
-  if (n_events) *n_events = counts[0];
-  if (n_nodes) *n_nodes = counts[1];
-  if (result) *result = r;
-  if (r.status) return fail(h, DEMI_ERR_CAPACITY, "demi_fuzz_trace: prefix status %u", (unsigned)r.status);
+  if (n_events) *n_events = got.counts[0];
+  if (n_nodes) *n_nodes = got.counts[1];
+  if (result) *result = got.r;
+  if (got.r.status) return fail(h, DEMI_ERR_CAPACITY, "demi_fuzz_trace: prefix status %u", (unsigned)got.r.status);
   return DEMI_OK;
 }
 
@@ -661,18 +701,34 @@ extern "C" int32_t demi_fuzz_trace(demi_handle* h, const demi_fuzz_params* p, in
 
 // ---------------------------------------------------------------------------------------------------------
 // Provenance pruning (ProvenanceTracker, schedulers/Util.scala:267-376)
-static int32_t launch_provenance(demi_handle* h, ProvArgs a, cudaStream_t s) {
+static size_t prune_bytes(uint32_t mask_words) { return (size_t)mask_words * 8 + sizeof(demi_provenance_out); }
+
+// Prunes n staged records into their `extra` bytes, prune_bytes(mask_words) per slot: keep masks | outputs (a record with
+// a status is skipped unless r.results is null).  Queues their copies to the host, the results' when `results` is given;
+// `timed` records h->ev1 after the kernel.
+static int32_t prune_records(demi_handle* h, const Records& r, uint32_t n, uint32_t mask_words, uint64_t* keep_masks,
+                             demi_provenance_out* out, demi_fuzz_result* results, bool timed, cudaStream_t s) {
   constexpr int PW = 4;
-  const uint64_t want = ((uint64_t)a.n + PW - 1) / PW;
-  const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * 8));
-  a.t_cap = a.mask_words * 64;
+  ProvArgs a{};
+  a.events = r.events; a.ev_stride = r.rec_cap;
+  a.parent = r.parents; a.par_stride = r.par_cap;
+  a.counts = r.counts; a.results = r.results;
+  a.keep = (uint64_t*)r.extra; a.mask_words = mask_words;
+  a.out = (demi_provenance_out*)(r.extra + (size_t)n * mask_words * 8); a.n = n;
+  a.t_cap = mask_words * 64;
   a.scratch_stride = a.t_cap + 3 * a.par_stride;
+  const uint64_t want = ((uint64_t)n + PW - 1) / PW;
+  const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)h->sm_count * 8));
   int32_t rc = h->prov_scratch.grow(h, (uint64_t)grid * PW * a.scratch_stride * sizeof(uint32_t));
   if (rc != DEMI_OK) return rc;
   a.scratch = h->prov_scratch.get<uint32_t>();
   provenance_kernel<PW><<<grid, PW * 32, 0, s>>>(a);
   CUDA_TRY(h, cudaGetLastError());
   h->perf.kernel_launches++;
+  if (timed) CUDA_TRY(h, cudaEventRecord(h->ev1, s));
+  CUDA_TRY(h, cudaMemcpyAsync(keep_masks, a.keep, (size_t)n * mask_words * 8, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(out, a.out, (size_t)n * sizeof(demi_provenance_out), cudaMemcpyDeviceToHost, s));
+  if (results) CUDA_TRY(h, cudaMemcpyAsync(results, r.results, (size_t)n * sizeof(demi_fuzz_result), cudaMemcpyDeviceToHost, s));
   return DEMI_OK;
 }
 
@@ -686,28 +742,17 @@ extern "C" int32_t demi_provenance(demi_handle* h, const demi_event* events, uin
   { int32_t vrc = demi_check_events(h, "demi_provenance", events, n_events, n_nodes, DEMI_MAX_ACTORS); if (vrc != DEMI_OK) return vrc;
     vrc = demi_check_parents(h, "demi_provenance", dep_parent, n_nodes); if (vrc != DEMI_OK) return vrc; }
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  const size_t ev_b = (size_t)std::max(n_events, 1u) * sizeof(demi_event), par_b = (size_t)n_nodes * 2;
-  const size_t keep_b = (size_t)mask_words * 8;
-  // events | parents | counts | keep | out
-  const size_t o_par = (ev_b + 15) & ~(size_t)15, o_cnt = (o_par + par_b + 15) & ~(size_t)15, o_keep = o_cnt + 16,
-               o_out = o_keep + ((keep_b + 15) & ~(size_t)15), total = o_out + sizeof(demi_provenance_out);
+  // the caller's trace as the record of one slot: its events, its parents and the counts a recording would have
   DevBuf tmp;
-  int32_t rc = tmp.grow(h, total);
+  Records rec;
+  int32_t rc = stage_records(h, nullptr, 1, nullptr, std::max(n_events, 1u), n_nodes, prune_bytes(mask_words), tmp, &rec, h->stream);
   if (rc != DEMI_OK) return rc;
-  unsigned char* buf = tmp.get<unsigned char>();
+  rec.results = nullptr;                   // no result record: nothing is skipped
   const uint32_t counts[4] = {n_events, n_nodes, affected_mask, 0};
-  CUDA_TRY(h, cudaMemcpyAsync(buf, events, (size_t)n_events * sizeof(demi_event), cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(buf + o_par, dep_parent, par_b, cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(buf + o_cnt, counts, sizeof(counts), cudaMemcpyHostToDevice, h->stream));
-  ProvArgs a{};
-  a.events = (const demi_event*)buf; a.ev_stride = std::max(n_events, 1u);
-  a.parent = (const uint16_t*)(buf + o_par); a.par_stride = n_nodes;
-  a.counts = (const uint32_t*)(buf + o_cnt); a.results = nullptr;
-  a.keep = (uint64_t*)(buf + o_keep); a.mask_words = mask_words;
-  a.out = (demi_provenance_out*)(buf + o_out); a.n = 1;
-  if ((rc = launch_provenance(h, a, h->stream)) != DEMI_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(keep_mask, buf + o_keep, keep_b, cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(out, buf + o_out, sizeof(*out), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(rec.events, events, (size_t)n_events * sizeof(demi_event), cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(rec.parents, dep_parent, (size_t)n_nodes * 2, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(rec.counts, counts, sizeof(counts), cudaMemcpyHostToDevice, h->stream));
+  if ((rc = prune_records(h, rec, 1, mask_words, keep_mask, out, nullptr, false, h->stream)) != DEMI_OK) return rc;
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   return DEMI_OK;
 }
@@ -731,57 +776,31 @@ extern "C" int32_t demi_fuzz_provenance(demi_handle* h, const demi_fuzz_params* 
   // an execution records at most one MsgSend + one MsgEvent per message, plus the external markers
   const uint32_t node_cap = plan.args.node_cap;
   const uint32_t ev_cap = 2 * node_cap + 2 * plan.args.n_ext + 16;
-  {
-    // bound the per-slot recording buffers to ~4 GB per launch: larger requests run in chunks
-    const size_t per_slot = (size_t)ev_cap * sizeof(demi_event) + (size_t)node_cap * 2 + 64 + (size_t)mask_words * 8;
-    const uint32_t chunk = (uint32_t)std::max<size_t>(1, ((size_t)4 << 30) / per_slot);
-    if (n > chunk) {
-      for (uint32_t off = 0; off < n; off += chunk) {
-        const uint32_t m = std::min(chunk, n - off);
-        rc = demi_fuzz_provenance(h, p, prefix_index + off, m, keep_masks + (size_t)off * mask_words, mask_words, out + off,
-                                  results ? results + off : nullptr);
-        if (rc != DEMI_OK) return rc;
-      }
-      return DEMI_OK;
-    }
-  }
-  const size_t b_ev = (size_t)n * ev_cap * sizeof(demi_event), b_par = (((size_t)n * node_cap * 2) + 15) & ~(size_t)15,
-               b_cnt = (size_t)n * 16, b_res = (size_t)n * sizeof(demi_fuzz_result), b_idx = (((size_t)n * 4) + 15) & ~(size_t)15,
-               b_keep = (size_t)n * mask_words * 8, b_out = (size_t)n * sizeof(demi_provenance_out);
-  DevBuf tmp;
-  if ((rc = tmp.grow(h, b_ev + b_par + b_cnt + b_res + b_idx + 16 + b_keep + b_out)) != DEMI_OK) return rc;
-  unsigned char* buf = tmp.get<unsigned char>();
-  unsigned char* d_par = buf + b_ev; unsigned char* d_cnt = d_par + b_par; unsigned char* d_res = d_cnt + b_cnt;
-  unsigned char* d_idx = d_res + b_res; unsigned char* d_n = d_idx + b_idx; unsigned char* d_keep = d_n + 16;
-  unsigned char* d_out = d_keep + b_keep;
+  const size_t extra = prune_bytes(mask_words);
+  const uint32_t chunk = record_chunk(ev_cap, node_cap, extra);
   cudaStream_t s = h->stream;
-  CUDA_TRY(h, cudaMemcpyAsync(d_idx, prefix_index, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-  CUDA_TRY(h, cudaMemcpyAsync(d_n, &n, 4, cudaMemcpyHostToDevice, s));
-  CUDA_TRY(h, cudaMemsetAsync(d_cnt, 0, b_cnt, s));
-  CUDA_TRY(h, cudaMemsetAsync(d_res, 0xFF, b_res, s));
-  CUDA_TRY(h, cudaEventRecord(h->ev0, s));
-  plan.args.results = (demi_fuzz_result*)d_res;
-  plan.args.index_list = (const uint32_t*)d_idx; plan.args.index_count = (const uint32_t*)d_n;
-  plan.args.rec_events = (demi_event*)buf; plan.args.rec_cap = ev_cap;
-  plan.args.rec_counts = (uint32_t*)d_cnt;
-  plan.args.rec_parent = (uint16_t*)d_par; plan.args.rec_parent_cap = node_cap;
-  plan.args.sum_steps = nullptr; plan.args.n_violations = nullptr;
-  // the lane engine records every execution it can prove exact; the slots it defers go to the general engine
-  if ((rc = launch_plan(h, plan, n, s)) != DEMI_OK) return rc;
-  ProvArgs a{};
-  a.events = (const demi_event*)buf; a.ev_stride = ev_cap;
-  a.parent = (const uint16_t*)d_par; a.par_stride = node_cap;
-  a.counts = (const uint32_t*)d_cnt; a.results = (const demi_fuzz_result*)d_res;
-  a.keep = (uint64_t*)d_keep; a.mask_words = mask_words; a.out = (demi_provenance_out*)d_out; a.n = n;
-  if ((rc = launch_provenance(h, a, s)) != DEMI_OK) return rc;
-  CUDA_TRY(h, cudaEventRecord(h->ev1, s));
-  CUDA_TRY(h, cudaMemcpyAsync(keep_masks, d_keep, b_keep, cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaMemcpyAsync(out, d_out, b_out, cudaMemcpyDeviceToHost, s));
-  if (results) CUDA_TRY(h, cudaMemcpyAsync(results, d_res, b_res, cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  float ms = 0.f;
-  CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
-  h->perf.kernel_ms = ms;
+  DevBuf buf;
+  float ms_all = 0.f;
+  h->perf.kernel_launches = 0;
+  for (uint32_t off = 0; off < n; off += chunk) {
+    const uint32_t m = std::min(chunk, n - off);
+    q.n_prefixes = m;                      // a chunk of a larger request plans its own grid
+    if (m < n && (rc = plan_launch(h, &q, LM_RECORD, h->ext_info, h->ext_dev.get<demi_ext_event>(), (uint32_t)h->ext_host.size(), &plan)))
+      return rc;
+    Records rec;
+    if ((rc = stage_records(h, &plan, m, prefix_index + off, ev_cap, node_cap, extra, buf, &rec, s)) != DEMI_OK) return rc;
+    CUDA_TRY(h, cudaEventRecord(h->ev0, s));
+    // the lane engine records every execution it can prove exact; the slots it defers go to the general engine
+    if ((rc = launch_plan(h, plan, m, s)) != DEMI_OK) return rc;
+    if ((rc = prune_records(h, rec, m, mask_words, keep_masks + (size_t)off * mask_words, out + off, results ? results + off : nullptr,
+                            true, s)) != DEMI_OK) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(s));
+    float ms = 0.f;
+    CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+    ms_all += ms;
+  }
+  h->perf.prefixes = n;
+  h->perf.kernel_ms = ms_all;
   return DEMI_OK;
 }
 
@@ -796,16 +815,16 @@ extern "C" int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, c
   if (!prefix_index || !events || !cap_events || !n_events)
     return fail(h, DEMI_ERR_INVALID, "demi_fuzz_traces: prefix_index, events, cap_events and n_events are required");
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  // bound the per-slot recording buffers to ~4 GB per launch: larger requests run in chunks
-  const size_t per_slot = (size_t)cap_events * sizeof(demi_event) + 2 + 16 + sizeof(demi_fuzz_result) + 4;
-  const uint32_t chunk = (uint32_t)std::max<size_t>(1, ((size_t)4 << 30) / per_slot);
+  const uint32_t chunk = record_chunk(cap_events, 1, 0);
+  cudaStream_t s = h->stream;
+  DevBuf buf;
   int32_t rc;
-  uint32_t launches = 0;
   float ms_all = 0.f;
   int64_t bad = -1;
   uint32_t bad_status = 0;
   std::vector<demi_fuzz_result> res;
   std::vector<uint32_t> cnt;
+  h->perf.kernel_launches = 0;
   for (uint32_t off = 0; off < n; off += chunk) {
     const uint32_t m = std::min(chunk, n - off);
     demi_fuzz_params q = *p;
@@ -813,33 +832,15 @@ extern "C" int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, c
     LaunchPlan plan;
     if ((rc = plan_launch(h, &q, LM_RECORD, h->ext_info, h->ext_dev.get<demi_ext_event>(), (uint32_t)h->ext_host.size(), &plan)) != DEMI_OK)
       return rc;
-    // events | parents (one entry per slot: the tree is not returned) | counts | results | work list | its length
-    const size_t b_ev = (size_t)m * cap_events * sizeof(demi_event), b_par = (((size_t)m * 2) + 15) & ~(size_t)15,
-                 b_cnt = (size_t)m * 16, b_res = (size_t)m * sizeof(demi_fuzz_result), b_idx = (((size_t)m * 4) + 15) & ~(size_t)15;
-    DevBuf tmp;
-    if ((rc = tmp.grow(h, b_ev + b_par + b_cnt + b_res + b_idx + 16)) != DEMI_OK) return rc;
-    unsigned char* buf = tmp.get<unsigned char>();
-    unsigned char* d_par = buf + b_ev; unsigned char* d_cnt = d_par + b_par; unsigned char* d_res = d_cnt + b_cnt;
-    unsigned char* d_idx = d_res + b_res; unsigned char* d_n = d_idx + b_idx;
-    cudaStream_t s = h->stream;
-    CUDA_TRY(h, cudaMemcpyAsync(d_idx, prefix_index + off, (size_t)m * 4, cudaMemcpyHostToDevice, s));
-    CUDA_TRY(h, cudaMemcpyAsync(d_n, &m, 4, cudaMemcpyHostToDevice, s));
-    CUDA_TRY(h, cudaMemsetAsync(d_cnt, 0, b_cnt, s));
-    CUDA_TRY(h, cudaMemsetAsync(d_res, 0xFF, b_res, s));
+    // one parent entry per slot: the tree is not returned
+    Records rec;
+    if ((rc = stage_records(h, &plan, m, prefix_index + off, cap_events, 1, 0, buf, &rec, s)) != DEMI_OK) return rc;
     CUDA_TRY(h, cudaEventRecord(h->ev0, s));
-    plan.args.results = (demi_fuzz_result*)d_res;
-    plan.args.index_list = (const uint32_t*)d_idx; plan.args.index_count = (const uint32_t*)d_n;
-    plan.args.rec_events = (demi_event*)buf; plan.args.rec_cap = cap_events;
-    plan.args.rec_counts = (uint32_t*)d_cnt;
-    plan.args.rec_parent = (uint16_t*)d_par; plan.args.rec_parent_cap = 1;
-    plan.args.sum_steps = nullptr; plan.args.n_violations = nullptr;
-    h->perf.kernel_launches = 0;
     if ((rc = launch_plan(h, plan, m, s)) != DEMI_OK) return rc;
-    launches += h->perf.kernel_launches;
     CUDA_TRY(h, cudaEventRecord(h->ev1, s));
     res.resize(m); cnt.resize((size_t)m * 4);
-    CUDA_TRY(h, cudaMemcpyAsync(cnt.data(), d_cnt, b_cnt, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(h, cudaMemcpyAsync(res.data(), d_res, b_res, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(h, cudaMemcpyAsync(cnt.data(), rec.counts, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(h, cudaMemcpyAsync(res.data(), rec.results, res.size() * sizeof(demi_fuzz_result), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(h, cudaStreamSynchronize(s));
     float ms = 0.f;
     CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
@@ -852,19 +853,18 @@ extern "C" int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, c
       if (results) results[off + i] = res[i];
       if (res[i].status) {
         if (bad < 0) { bad = off + i; bad_status = res[i].status; }
-        CUDA_TRY(h, cudaMemsetAsync(buf + (size_t)i * cap_events * sizeof(demi_event), 0, (size_t)cap_events * sizeof(demi_event), s));
+        CUDA_TRY(h, cudaMemsetAsync(rec.events + (size_t)i * cap_events, 0, (size_t)cap_events * sizeof(demi_event), s));
       } else {
         width = std::max(width, std::min(cnt[(size_t)i * 4], cap_events));
       }
     }
     if (width) {
       const size_t pitch = (size_t)cap_events * sizeof(demi_event);
-      CUDA_TRY(h, cudaMemcpy2DAsync(events + (size_t)off * cap_events, pitch, buf, pitch, (size_t)width * sizeof(demi_event), m,
+      CUDA_TRY(h, cudaMemcpy2DAsync(events + (size_t)off * cap_events, pitch, rec.events, pitch, (size_t)width * sizeof(demi_event), m,
                                     cudaMemcpyDeviceToHost, s));
       CUDA_TRY(h, cudaStreamSynchronize(s));
     }
   }
-  h->perf.kernel_launches = launches;
   h->perf.prefixes = n;
   h->perf.kernel_ms = ms_all;
   // as demi_fuzz_trace fails for that seed; every record is filled all the same

@@ -75,7 +75,6 @@ struct demi_handle {
   bool lane_tree_built = false;
   demi::LaneTreeKey lane_tree_key{};
   int32_t lane_tree_depth = -1;                    // the depth the last fuzz launch walked (-1: not the steady one)
-  DevBuf rec_counts_dev;                           // uint32_t
   DevBuf prov_scratch;
   DevBuf dpor_buf[24];                             // K3 per-search structures (capi_dpor.cu)
   cudaStream_t stream = nullptr, copy_stream = nullptr;
@@ -124,7 +123,7 @@ struct demi_handle {
   DevBuf fz_arena;
   // ---- launch bookkeeping
   std::map<const void*, int> occupancy;          // kernel -> resident blocks per SM (asked once per handle)
-  DevBuf trace_rec;                              // demi_fuzz_trace's recording buffer
+  DevBuf trace_rec;                              // demi_fuzz_trace's records (stage_records, one slot); only grows
 };
 // K2, STSSched replay (capi_replay.cu): the ReplayArgs fields that follow from the handle's configuration and `trace`;
 // the rest are zero

@@ -141,6 +141,7 @@ def cases(recorded):
                                   lambda e: e.wildcard_replay_trace(full_mask(n_deliveries), looking_for=code)),
         "provenance": (raft_engine, lambda e: e.provenance(ev, par, 1)),
         "fuzz_provenance": (raft_engine, lambda e: e.fuzz_provenance(1, np.arange(64), MAXM, INTERVAL)),
+        "fuzz_traces": (raft_engine, lambda e: e.fuzz_traces(1, np.arange(64), MAXM, INTERVAL)),
         "random_test_trace": (raft_engine, lambda e: e.random_test_trace(full_mask(n_ext), 5, MAXM, INTERVAL)),
         "dedup_compact": (raft_engine, lambda e: e.dedup_compact(records, 0)),
         "dpor_batch": (raft_engine, lambda e: e.dpor_batch(dpor_programs(), 30, 200, cap_viol=8, want_hashes=True)),
@@ -149,7 +150,7 @@ def cases(recorded):
 
 
 CASES = ["fuzz_batch", "fuzz_trace", "replay_trace", "wildcard_replay_trace", "provenance", "fuzz_provenance",
-         "random_test_trace", "dedup_compact", "dpor_batch", "dpor_frontier"]
+         "fuzz_traces", "random_test_trace", "dedup_compact", "dpor_batch", "dpor_frontier"]
 
 
 def as_bytes(x):

@@ -95,6 +95,19 @@ def test_fuzz_provenance_batch_matches_oracle(eng):
     assert out["n_kept"][:300].sum() < 0.9 * out["n_trace"][:300].sum()
 
 
+def test_fuzz_provenance_reports_its_own_launches_and_prefixes(eng):
+    """demi_perf after fuzz_provenance describes that call alone: the same call gives the same launch count, and
+    `prefixes` counts its executions, not those of the batch before it."""
+    res = eng.fuzz_batch(1, 20000, 50, 5)
+    idx = np.nonzero(res["violation"])[0][:100].astype(np.uint32)
+    assert 0 < len(idx) < 20000
+    seen = []
+    for _ in range(2):
+        eng.fuzz_provenance(1, idx, 50, 5)
+        seen.append((eng.stats().kernel_launches, eng.stats().prefixes))
+    assert seen[0] == seen[1] and seen[0][1] == len(idx) and seen[0][0] >= 2
+
+
 def test_fuzz_provenance_slots_deferred_by_the_lane_engine(monkeypatch):
     """The lane engine records what it can prove exact; slots it defers (here: more than 24 pending messages, a bound
     lowered for the test) are recorded by the general engine, addressed by work-list position.  Both kinds in one
