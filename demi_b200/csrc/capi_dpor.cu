@@ -84,13 +84,7 @@ int32_t dpor_run(demi_handle* h, const demi_ext_event* ext, const uint32_t* ext_
   const DporVariant* dv = pick_dv(h->cfg.model);
   if (!dv) return fail(h, DEMI_ERR_INVALID, "no DPOR kernel for model %d", h->cfg.model);
   const uint32_t n_ext = ext_offsets[n_searches];
-  const int n_actors = demi_model_actors(h);
-  for (uint32_t i = 0; i < n_ext; i++) {
-    // "unsuported external event" (DPORwHeuristics.scala:710)
-    if (ext[i].kind != DEMI_EXT_START && ext[i].kind != DEMI_EXT_SEND)
-      return fail(h, DEMI_ERR_INVALID, "demi_dpor_batch: external %u: DPOR accepts Start and Send only", i);
-    if (ext[i].a >= n_actors) return fail(h, DEMI_ERR_INVALID, "demi_dpor_batch: external %u names an unknown actor", i);
-  }
+  { int32_t vrc = demi_check_dpor_program(h, "demi_dpor_batch", ext, n_ext); if (vrc != DEMI_OK) return vrc; }
   DporArgs a{};
   a.model_flags = h->cfg.model_flags; a.blocked_mask = h->cfg.blocked_mask;
   a.P = P; a.n_searches = n_searches; a.cap_viol = cap_viol; a.cap_hashes = cap_hashes;
@@ -104,61 +98,60 @@ int32_t dpor_run(demi_handle* h, const demi_ext_event* ext, const uint32_t* ext_
   const size_t S = n_searches, NI = (size_t)P.max_interleavings + 1;
   const size_t n_caps = caps ? cap_offsets[n_searches] : 0;
   const size_t n_seed_nodes = seed ? seed->nodes.size() : 0, n_seed_trace = seed ? seed->trace.size() : 0;
-  struct Buf { void** p; size_t bytes; int fill; };
-  void *d_ext = 0, *d_off = 0, *d_res = 0, *d_viol = 0, *d_hash = 0, *d_nodes = 0, *d_child = 0, *d_q = 0, *d_ex = 0, *d_heap = 0,
-       *d_tr = 0, *d_tl = 0, *d_cur = 0, *d_next = 0, *d_npos = 0, *d_scan = 0, *d_hd = 0, *d_path = 0, *d_caps = 0, *d_coff = 0,
-       *d_sn = 0, *d_st = 0, *d_oi = 0, *d_bk = 0;
-  Buf bufs[] = {
-    {&d_ext, std::max<size_t>(n_ext, 1) * sizeof(demi_ext_event), -1}, {&d_off, (S + 1) * sizeof(uint32_t), -1},
-    {&d_res, S * sizeof(demi_dpor_result), 0}, {&d_viol, std::max<size_t>(S * cap_viol, 1) * sizeof(demi_dpor_violation), 0},
-    {&d_hash, std::max<size_t>(S * cap_hashes, 1) * sizeof(uint64_t), 0},
-    {&d_nodes, S * P.node_cap * sizeof(uint4), -1}, {&d_child, S * a.child_slots * sizeof(uint32_t), 0},
-    {&d_q, S * dv->nq * DPOR_QCAP * sizeof(uint32_t), -1}, {&d_ex, S * P.explored_slots * sizeof(uint64_t), 0xFF},
-    {&d_heap, S * P.heap_cap * sizeof(DporKey), -1}, {&d_tr, S * NI * a.T1 * sizeof(uint32_t), -1},
-    {&d_tl, S * NI * sizeof(uint32_t), -1}, {&d_cur, S * a.T1 * sizeof(uint32_t), -1}, {&d_next, S * a.T1 * sizeof(uint32_t), -1},
-    {&d_npos, S * P.node_cap * sizeof(uint32_t), 0}, {&d_scan, S * a.T1 * sizeof(uint32_t), -1},
-    {&d_hd, (arv || use_buckets) ? S * P.heap_cap * sizeof(uint32_t) : 16, -1}, {&d_path, arv ? S * (2 * (size_t)a.T1 + 4) * sizeof(int32_t) : 16, -1},
-    {&d_caps, std::max<size_t>(n_caps, 1) * sizeof(int32_t), -1}, {&d_coff, (S + 1) * sizeof(uint32_t), -1},
-    {&d_sn, std::max<size_t>(n_seed_nodes, 1) * sizeof(uint4), -1}, {&d_st, std::max<size_t>(n_seed_trace, 1) * sizeof(uint32_t), -1},
-    {&d_oi, std::max<size_t>(n_seed_nodes, 1) * sizeof(int32_t), -1},
-    {&d_bk, use_buckets ? S * 2 * (size_t)a.T1 * sizeof(uint32_t) : 16, -1},
-  };
-  // the buffers live in the handle and only grow: a DDMin run issues many launches of similar size
-  constexpr size_t NB = sizeof(bufs) / sizeof(bufs[0]);
-  static_assert(NB <= sizeof(h->dpor_buf) / sizeof(h->dpor_buf[0]), "dpor_buf too small");
-  for (size_t i = 0; i < NB; i++) {
-    Buf& b = bufs[i];
-    if (const int32_t rc = h->dpor_buf[i].grow(h, b.bytes); rc != DEMI_OK) {
-      for (DevBuf& d : h->dpor_buf) d.reset();     // all of them: a smaller retry then finds the memory free
-      return rc;
-    }
-    *b.p = h->dpor_buf[i].get();
-    if (b.fill >= 0) CUDA_TRY(h, cudaMemsetAsync(*b.p, b.fill, b.bytes, h->stream));
-  }
+  a.n_init_nodes = (uint32_t)n_seed_nodes; a.n_init_trace = (uint32_t)n_seed_trace;
+  // Every per-search buffer once: the field it binds, its bytes, its fill (-1: none) and whether the field is bound
+  // (an unbound one stays null).  The buffers live in the handle, one per entry, and only grow: a DDMin run issues many
+  // launches of similar size.
+  int32_t rc = DEMI_OK;
   cudaError_t e = cudaSuccess;
-  auto up = [&](void* dst, const void* src, size_t bytes) {
-    if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream);
+  size_t nb = 0;
+  auto buf = [&](auto*& field, size_t bytes, int fill, bool bound = true) {
+    if (nb == h->dpor_buf.size()) h->dpor_buf.emplace_back();
+    DevBuf& d = h->dpor_buf[nb++];
+    if (rc == DEMI_OK) rc = d.grow(h, bytes);
+    if (rc != DEMI_OK) return;
+    if (fill >= 0 && e == cudaSuccess) e = cudaMemsetAsync(d.get(), fill, bytes, h->stream);
+    field = bound ? d.get<std::remove_reference_t<decltype(*field)>>() : nullptr;
   };
-  up(d_ext, ext, n_ext * sizeof(demi_ext_event));
-  up(d_off, ext_offsets, (S + 1) * sizeof(uint32_t));
-  if (caps) { up(d_caps, caps, n_caps * sizeof(int32_t)); up(d_coff, cap_offsets, (S + 1) * sizeof(uint32_t)); }
-  if (seed) {
-    up(d_sn, seed->nodes.data(), n_seed_nodes * sizeof(uint4));
-    up(d_st, seed->trace.data(), n_seed_trace * sizeof(uint32_t));
-    up(d_oi, seed->orig_index.data(), n_seed_nodes * sizeof(int32_t));
+  buf(a.ext, std::max<size_t>(n_ext, 1) * sizeof(demi_ext_event), -1);
+  buf(a.ext_offsets, (S + 1) * sizeof(uint32_t), -1);
+  buf(a.results, S * sizeof(demi_dpor_result), 0);
+  buf(a.viol, std::max<size_t>(S * cap_viol, 1) * sizeof(demi_dpor_violation), 0, viol != nullptr);
+  buf(a.hashes, std::max<size_t>(S * cap_hashes, 1) * sizeof(uint64_t), 0, hashes != nullptr);
+  buf(a.nodes, S * P.node_cap * sizeof(uint4), -1);
+  buf(a.child_hash, S * a.child_slots * sizeof(uint32_t), 0);
+  buf(a.queues, S * dv->nq * DPOR_QCAP * sizeof(uint32_t), -1);
+  buf(a.explored, S * P.explored_slots * sizeof(uint64_t), 0xFF);
+  buf(a.heap, S * P.heap_cap * sizeof(DporKey), -1);
+  buf(a.traces, S * NI * a.T1 * sizeof(uint32_t), -1);
+  buf(a.trace_len, S * NI * sizeof(uint32_t), -1);
+  buf(a.cur_trace, S * a.T1 * sizeof(uint32_t), -1);
+  buf(a.next_trace, S * a.T1 * sizeof(uint32_t), -1);
+  buf(a.node_pos, S * P.node_cap * sizeof(uint32_t), 0);
+  buf(a.scan, S * a.T1 * sizeof(uint32_t), -1);
+  buf(a.heap_dist, (arv || use_buckets) ? S * P.heap_cap * sizeof(uint32_t) : 16, -1, arv || use_buckets);
+  buf(a.path, arv ? S * (2 * (size_t)a.T1 + 4) * sizeof(int32_t) : 16, -1, arv);
+  buf(a.caps, std::max<size_t>(n_caps, 1) * sizeof(int32_t), -1, caps != nullptr);
+  buf(a.cap_offsets, (S + 1) * sizeof(uint32_t), -1);
+  buf(a.init_nodes, std::max<size_t>(n_seed_nodes, 1) * sizeof(uint4), -1);
+  buf(a.init_trace, std::max<size_t>(n_seed_trace, 1) * sizeof(uint32_t), -1);
+  buf(a.orig_index, std::max<size_t>(n_seed_nodes, 1) * sizeof(int32_t), -1);
+  buf(a.buckets, use_buckets ? S * 2 * (size_t)a.T1 * sizeof(uint32_t) : 16, -1, use_buckets);
+  if (rc != DEMI_OK) {
+    for (DevBuf& d : h->dpor_buf) d.reset();       // all of them: a smaller retry then finds the memory free
+    return rc;
   }
-  a.ext = (const uint4*)d_ext; a.ext_offsets = (const uint32_t*)d_off; a.results = (demi_dpor_result*)d_res;
-  a.viol = viol ? (demi_dpor_violation*)d_viol : nullptr; a.hashes = hashes ? (uint64_t*)d_hash : nullptr;
-  a.nodes = (uint4*)d_nodes; a.child_hash = (uint32_t*)d_child; a.queues = (uint32_t*)d_q; a.explored = (uint64_t*)d_ex;
-  a.heap = (DporKey*)d_heap; a.traces = (uint32_t*)d_tr; a.trace_len = (uint32_t*)d_tl;
-  a.cur_trace = (uint32_t*)d_cur; a.next_trace = (uint32_t*)d_next;
-  a.node_pos = (uint32_t*)d_npos; a.scan = (uint32_t*)d_scan;
-  a.heap_dist = (arv || use_buckets) ? (uint32_t*)d_hd : nullptr;
-  a.buckets = use_buckets ? (uint32_t*)d_bk : nullptr; a.path = arv ? (int32_t*)d_path : nullptr;
-  a.caps = caps ? (const int32_t*)d_caps : nullptr; a.cap_offsets = (const uint32_t*)d_coff;
-  a.init_nodes = (const uint4*)d_sn; a.n_init_nodes = (uint32_t)n_seed_nodes;
-  a.init_trace = (const uint32_t*)d_st; a.n_init_trace = (uint32_t)n_seed_trace;
-  a.orig_index = (const int32_t*)d_oi;
+  auto up = [&](const void* dst, const void* src, size_t bytes) {
+    if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(const_cast<void*>(dst), src, bytes, cudaMemcpyHostToDevice, h->stream);
+  };
+  up(a.ext, ext, n_ext * sizeof(demi_ext_event));
+  up(a.ext_offsets, ext_offsets, (S + 1) * sizeof(uint32_t));
+  if (caps) { up(a.caps, caps, n_caps * sizeof(int32_t)); up(a.cap_offsets, cap_offsets, (S + 1) * sizeof(uint32_t)); }
+  if (seed) {
+    up(a.init_nodes, seed->nodes.data(), n_seed_nodes * sizeof(uint4));
+    up(a.init_trace, seed->trace.data(), n_seed_trace * sizeof(uint32_t));
+    up(a.orig_index, seed->orig_index.data(), n_seed_nodes * sizeof(int32_t));
+  }
   if (e == cudaSuccess && h->cfg.model == DEMI_MODEL_IR) e = ir_bind(h->ir_dev, h->stream);   // this unit's copy of g_ir
   // the race scan's position table goes to shared memory when it leaves room for >= 8 blocks per SM
   size_t smem = dv->smem;
@@ -172,9 +165,9 @@ int32_t dpor_run(demi_handle* h, const demi_ext_event* ext, const uint32_t* ext_
     e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaEventRecord(h->ev1, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(results, d_res, S * sizeof(demi_dpor_result), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess && viol && cap_viol) e = cudaMemcpyAsync(viol, d_viol, S * cap_viol * sizeof(demi_dpor_violation), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess && hashes && cap_hashes) e = cudaMemcpyAsync(hashes, d_hash, S * cap_hashes * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(results, a.results, S * sizeof(demi_dpor_result), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess && viol && cap_viol) e = cudaMemcpyAsync(viol, a.viol, S * cap_viol * sizeof(demi_dpor_violation), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess && hashes && cap_hashes) e = cudaMemcpyAsync(hashes, a.hashes, S * cap_hashes * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
   float ms = 0;
   if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, h->ev0, h->ev1);
@@ -260,10 +253,7 @@ extern "C" int32_t demi_incremental_ddmin(demi_handle* h, const demi_ext_event* 
   if (!externals || !params || !mcs_mask || !out) return fail(h, DEMI_ERR_INVALID, "demi_incremental_ddmin: null argument");
   { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
   if ((uint64_t)mask_words * 64 < n_externals) return fail(h, DEMI_ERR_INVALID, "mask_words too small");
-  for (uint32_t i = 0; i < n_externals; i++)
-    if (externals[i].kind != DEMI_EXT_START && externals[i].kind != DEMI_EXT_SEND)
-      return fail(h, DEMI_ERR_INVALID, "demi_incremental_ddmin: external %u: DPOR accepts Start and Send only", i);
-  { int32_t vrc = demi_check_externals(h, "demi_incremental_ddmin", externals, n_externals); if (vrc != DEMI_OK) return vrc; }
+  { int32_t vrc = demi_check_dpor_program(h, "demi_incremental_ddmin", externals, n_externals); if (vrc != DEMI_OK) return vrc; }
   SeedHost sh;
   if (seed) { int32_t rc = build_seed(h, seed, sh); if (rc != DEMI_OK) return rc; }
   memset(out, 0, sizeof(*out));

@@ -43,10 +43,10 @@ NcclApi* nccl_api() {
 #undef BIND
   return &api;
 }
-struct FrComm { ncclComm_t comm = nullptr; int rank = 0, world = 1; };
 #define NCCL_TRY(h, expr) do { ncclResult_t r_ = (expr); if (r_ != ncclSuccess) \
   return fail((h), DEMI_ERR_CUDA, "%s: %s", #expr, nccl_api()->GetErrorString(r_)); } while (0)
 }  // namespace
+struct FrComm { ncclComm_t comm = nullptr; int rank = 0, world = 1; };
 
 extern "C" int32_t demi_comm_unique_id(uint8_t id[DEMI_COMM_ID_BYTES]) {
   NcclApi* a = nccl_api();
@@ -75,13 +75,13 @@ extern "C" int32_t demi_comm_init(demi_handle* h, const uint8_t id[DEMI_COMM_ID_
 }
 extern "C" int32_t demi_comm_rank(const demi_handle* h, int32_t* rank, int32_t* world) {
   if (!h) return DEMI_ERR_INVALID;
-  const FrComm* c = (const FrComm*)h->comm;
+  const FrComm* c = h->comm;
   if (rank) *rank = c ? c->rank : 0;
   if (world) *world = c ? c->world : 1;
   return DEMI_OK;
 }
 void demi_comm_free(demi_handle* h) {
-  FrComm* c = (FrComm*)h->comm;
+  FrComm* c = h->comm;
   if (!c) return;
   if (c->comm) nccl_api()->CommDestroy(c->comm);
   delete c;
@@ -122,24 +122,21 @@ constexpr int SCAN_WPB = 4;
 
 struct FrRun { std::vector<unsigned long long> lo, hi; };      // per branch: the not yet dequeued part of the run, [lo, hi) in the queue array
 
-struct FrGeom;
 struct FrState {
   demi_handle* h = nullptr; FrComm* comm = nullptr; const FrVariant* v = nullptr;
-  demi_frontier_params F{}; uint32_t T1 = 0, W = 0, cap_pend = 0, rcap = 0, win_cap = 0, s_slots = 0, rec_u4 = 0;
+  demi_frontier_params F{}; uint32_t W = 0, win_cap = 0, segs_cap = 0;
+  size_t scan_smem = 0, cnt_smem = 0;             // dynamic shared memory of the scan kernel; of the count and scatter kernels
   cudaStream_t s = nullptr;
   std::vector<DevBuf> allocs;
-  // device
-  uint4* tr = nullptr; uint32_t* tr_meta = nullptr; unsigned long long* E = nullptr; ulonglong2* pool = nullptr;
-  ulonglong2* sel = nullptr; unsigned long long* out_hash = nullptr; uint32_t* out_viol = nullptr;
-  uint4* pendA = nullptr; uint32_t* pendP1 = nullptr; uint32_t* pendNX = nullptr;
-  uint32_t* races = nullptr; uint32_t* n_races = nullptr; uint32_t* counts = nullptr; uint32_t* tot = nullptr; uint32_t* tile_tot = nullptr;
-  unsigned long long* base = nullptr; unsigned long long* ctr = nullptr; FrInfo* info = nullptr;
-  ulonglong2* win = nullptr; uint8_t* flag = nullptr; unsigned long long* skey = nullptr; uint32_t* sidx = nullptr;
-  uint32_t* blockcnt = nullptr; FrSeg* segs_dev = nullptr; uint32_t segs_cap = 0;
-  uint4* sendbuf = nullptr; uint4* recvbuf = nullptr; uint32_t* hist = nullptr; unsigned long long* gather_dev = nullptr;
-  unsigned long long* log_keys = nullptr; unsigned int* log_n = nullptr; unsigned int log_cap = 0;     // explored pairs to share
+  // the device buffers, each in the argument struct of the kernels that use it (fr_setup binds them once): A for the
+  // executor and the enqueue, S for the select kernels (per window: the segments, the quota and where winners go),
+  // X for the steal round's pack and unpack (per batch: the records and where they go)
+  FrArgs A{};
+  FrSelArgs S{};
+  FrXArgs X{};
+  // NCCL buffers
+  uint4* sendbuf = nullptr; uint4* recvbuf = nullptr; unsigned long long* gather_dev = nullptr;
   unsigned long long* log_all = nullptr; unsigned long long* log_counts = nullptr;
-  uint4* ext_dev = nullptr;
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   // host: the queue directory
   std::vector<FrRun> runs;
@@ -147,16 +144,14 @@ struct FrState {
   std::vector<unsigned long long> branch_live;
   unsigned long long pool_top = 0, pool_live = 0, n_exec = 0;
   uint32_t n_slots = 0;
-  unsigned long long cap_exec = 0;
   unsigned long long explored_sel = 0;            // explored pairs after the last getNext (history on)
   bool round_failed = false;                      // a round ended in a capacity status: R.explored_pairs is final
   demi_frontier_result R{};
-  FrArgs A{};
 
-  template <class T> int32_t dalloc(T** p, size_t n) {
+  template <class T> int32_t dalloc(T*& p, size_t n) {
     allocs.emplace_back();
     const int32_t rc = allocs.back().grow(h, std::max<size_t>(n * sizeof(T), 256));
-    *p = allocs.back().get<T>();
+    p = allocs.back().get<T>();
     return rc;
   }
   ~FrState() { for (auto& e : ev) if (e) cudaEventDestroy(e); }
@@ -175,107 +170,101 @@ bool fr_same_geom(const FrGeom& a, const FrGeom& b, uint32_t n_ext) {
 int32_t fr_setup(FrState& st, const demi_ext_event* ext, uint32_t n_ext, bool reuse) {
   demi_handle* h = st.h;
   const demi_frontier_params& F = st.F;
-  st.T1 = (uint32_t)F.max_messages + 2;
-  st.W = F.width;
+  FrArgs& A = st.A; FrSelArgs& S = st.S; FrXArgs& X = st.X;
+  const uint32_t T1 = (uint32_t)F.max_messages + 2;
   uint32_t n_sends = 0;
   for (uint32_t i = 0; i < n_ext; i++) if (ext[i].kind == DEMI_EXT_SEND) n_sends++;
-  st.cap_pend = demi_fr_pool_entries(demi_model_key(h), F.max_messages, n_sends);
-  if (st.cap_pend >= 0xFFFFu) return fail(h, DEMI_ERR_CAPACITY, "demi_dpor_frontier: %u pending entries per interleaving exceed the 16-bit links", st.cap_pend);
-  st.rcap = st.T1 * (st.T1 - 1) / 2;
-  st.win_cap = std::min<uint32_t>(std::max<uint32_t>(4 * st.W, 4096), 1u << 22);
-  st.s_slots = 1; while (st.s_slots < 2 * st.win_cap) st.s_slots <<= 1;
-  st.rec_u4 = st.T1 + 2;
+  A.cap_pend = demi_fr_pool_entries(demi_model_key(h), F.max_messages, n_sends);
+  if (A.cap_pend >= 0xFFFFu) return fail(h, DEMI_ERR_CAPACITY, "demi_dpor_frontier: %u pending entries per interleaving exceed the 16-bit links", A.cap_pend);
   st.s = h->stream;
-  const int world = st.comm ? st.comm->world : 1;
-  st.cap_exec = F.max_interleavings + st.W + 1;
-  int32_t rc;
   if (!reuse) {
-#define DA(p, n) if ((rc = st.dalloc(&st.p, (size_t)(n))) != DEMI_OK) return rc;
-  DA(tr, (size_t)F.trace_cap * st.T1) DA(tr_meta, F.trace_cap) DA(E, F.explored_slots) DA(pool, F.pool_cap)
-  DA(sel, std::max<uint32_t>(st.W, F.steal_max)) DA(out_hash, st.cap_exec) DA(out_viol, st.cap_exec)
-  const size_t warps = (st.W + 31) / 32;
-  DA(pendA, warps * st.cap_pend * 32) DA(pendP1, warps * st.cap_pend * 32) DA(pendNX, warps * st.cap_pend * 32)
-  DA(races, (size_t)st.W * st.rcap) DA(n_races, st.W) DA(counts, (size_t)st.T1 * st.W) DA(tot, st.T1) DA(base, st.T1) DA(tile_tot, (size_t)st.T1 * ((st.W + FR_TILE - 1) / FR_TILE + 1))
-  DA(ctr, FRC_N) DA(info, 1)
-  DA(win, st.win_cap) DA(flag, st.win_cap) DA(skey, st.s_slots) DA(sidx, st.s_slots) DA(blockcnt, (st.win_cap + 255) / 256 + 1)
-  st.segs_cap = 1 << 16; DA(segs_dev, st.segs_cap)
-  if (world > 1) {
-    DA(sendbuf, (size_t)F.steal_max * (world - 1) * st.rec_u4) DA(recvbuf, (size_t)F.steal_max * (world - 1) * st.rec_u4)
-    DA(gather_dev, (size_t)world * std::max(world, 8))
-    if (!(F.flags & DEMI_FR_NO_HISTORY)) {
-      st.log_cap = (unsigned int)std::min<unsigned long long>(F.explored_slots / 2, 1ull << 22);
-      DA(log_keys, st.log_cap) DA(log_n, 4) DA(log_all, (size_t)world * st.log_cap) DA(log_counts, world)
+    const int world = st.comm ? st.comm->world : 1;
+    st.W = F.width;
+    st.win_cap = std::min<uint32_t>(std::max<uint32_t>(4 * st.W, 4096), 1u << 22);
+    st.segs_cap = 1 << 16;
+    st.scan_smem = (size_t)SCAN_WPB * fr_scan_words(T1) * 4; st.cnt_smem = (size_t)SCAN_WPB * fr_cnt_words(T1) * 4;
+    A.T1 = T1; A.rcap = T1 * (T1 - 1) / 2; A.e_slots = F.explored_slots; A.no_history = (F.flags & DEMI_FR_NO_HISTORY) ? 1u : 0u;
+    S.s_slots = 1; while (S.s_slots < 2 * st.win_cap) S.s_slots <<= 1;
+    X.rec_u4 = T1 + 2;
+    const unsigned long long cap_exec = F.max_interleavings + st.W + 1;
+    const size_t warps = (st.W + 31) / 32;
+    int32_t rc = DEMI_OK;
+    auto da = [&](auto*& p, size_t n) { if (rc == DEMI_OK) rc = st.dalloc(p, n); };
+    da(A.tr, (size_t)F.trace_cap * T1); da(A.tr_meta, F.trace_cap); da(A.E, F.explored_slots); da(A.pool, F.pool_cap);
+    da(S.sel, std::max<uint32_t>(st.W, F.steal_max)); da(A.out_hash, cap_exec); da(A.out_viol, cap_exec);
+    da(A.pendA, warps * A.cap_pend * 32); da(A.pendP1, warps * A.cap_pend * 32); da(A.pendNX, warps * A.cap_pend * 32);
+    da(A.races, (size_t)st.W * A.rcap); da(A.n_races, st.W); da(A.counts, (size_t)T1 * st.W); da(A.tot, T1); da(A.base, T1);
+    da(A.tile_tot, (size_t)T1 * ((st.W + FR_TILE - 1) / FR_TILE + 1));
+    da(A.ctr, FRC_N); da(A.info, 1);
+    da(S.win, st.win_cap); da(S.flag, st.win_cap); da(S.skey, S.s_slots); da(S.sidx, S.s_slots); da(S.blockcnt, (st.win_cap + 255) / 256 + 1);
+    da(S.segs, st.segs_cap);
+    if (world > 1) {
+      da(st.sendbuf, (size_t)F.steal_max * (world - 1) * X.rec_u4); da(st.recvbuf, (size_t)F.steal_max * (world - 1) * X.rec_u4);
+      da(st.gather_dev, (size_t)world * std::max(world, 8));
+      if (!A.no_history) {                                       // explored pairs to share
+        A.log.cap = (unsigned int)std::min<unsigned long long>(F.explored_slots / 2, 1ull << 22);
+        da(A.log.keys, A.log.cap); da(A.log.n, 4); da(st.log_all, (size_t)world * A.log.cap); da(st.log_counts, world);
+      }
     }
+    da(X.hist, T1);
+    da(A.ext, std::max<uint32_t>(n_ext, 64));
+    if (rc != DEMI_OK) return rc;
+    for (auto& e : st.ev) CUDA_TRY(h, cudaEventCreate(&e));
+    A.sel = S.sel;
+    S.pool = A.pool; S.E = A.E; S.e_slots = A.e_slots; S.info = A.info; S.ctr = A.ctr; S.no_history = A.no_history; S.log = A.log;
+    X.sel = S.sel; X.tr = A.tr; X.tr_meta = A.tr_meta; X.T1 = T1; X.pool = A.pool;
   }
-  DA(hist, st.T1)
-  DA(ext_dev, std::max<uint32_t>(n_ext, 64))
-#undef DA
-  for (auto& e : st.ev) CUDA_TRY(h, cudaEventCreate(&e));
-  }
+  A.model_flags = h->cfg.model_flags; A.blocked_mask = h->cfg.blocked_mask;
+  A.max_messages = F.max_messages; A.looking_for = F.looking_for; A.n_ext = n_ext;
   st.runs.clear(); st.pool_top = st.pool_live = st.n_exec = 0; st.n_slots = 0;
   st.explored_sel = 0; st.round_failed = false;
   memset(&st.R, 0, sizeof(st.R));
-  if (!(F.flags & DEMI_FR_NO_HISTORY)) CUDA_TRY(h, cudaMemsetAsync(st.E, 0, F.explored_slots * 8, st.s));
-  CUDA_TRY(h, cudaMemsetAsync(st.ctr, 0, FRC_N * 8, st.s));
-  if (st.log_n) CUDA_TRY(h, cudaMemsetAsync(st.log_n, 0, 16, st.s));
-  CUDA_TRY(h, cudaMemsetAsync(st.info, 0, sizeof(FrInfo), st.s));
-  if (n_ext) CUDA_TRY(h, cudaMemcpyAsync(st.ext_dev, ext, n_ext * sizeof(demi_ext_event), cudaMemcpyHostToDevice, st.s));
+  if (!A.no_history) CUDA_TRY(h, cudaMemsetAsync(A.E, 0, F.explored_slots * 8, st.s));
+  CUDA_TRY(h, cudaMemsetAsync(A.ctr, 0, FRC_N * 8, st.s));
+  if (A.log.n) CUDA_TRY(h, cudaMemsetAsync(A.log.n, 0, 16, st.s));
+  CUDA_TRY(h, cudaMemsetAsync(A.info, 0, sizeof(FrInfo), st.s));
+  if (n_ext) CUDA_TRY(h, cudaMemcpyAsync(const_cast<uint4*>(A.ext), ext, n_ext * sizeof(demi_ext_event), cudaMemcpyHostToDevice, st.s));
   CUDA_TRY(h, cudaFuncSetAttribute(st.v->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)st.v->smem));
-  const size_t scan_smem = (size_t)SCAN_WPB * fr_scan_words(st.T1) * 4, cnt_smem = (size_t)SCAN_WPB * fr_cnt_words(st.T1) * 4;
-  CUDA_TRY(h, cudaFuncSetAttribute(fr_scan_kernel<SCAN_WPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scan_smem));
-  CUDA_TRY(h, cudaFuncSetAttribute(fr_count_kernel<SCAN_WPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cnt_smem));
-  CUDA_TRY(h, cudaFuncSetAttribute(fr_scatter_kernel<SCAN_WPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cnt_smem));
-  st.brq.assign(st.T1, {}); st.branch_live.assign(st.T1, 0);
-  FrArgs& A = st.A;
-  A.model_flags = h->cfg.model_flags; A.blocked_mask = h->cfg.blocked_mask;
-  A.max_messages = F.max_messages; A.looking_for = F.looking_for; A.no_history = (F.flags & DEMI_FR_NO_HISTORY) ? 1u : 0u;
-  A.ext = st.ext_dev; A.n_ext = n_ext; A.T1 = st.T1;
-  A.tr = st.tr; A.tr_meta = st.tr_meta; A.E = st.E; A.e_slots = F.explored_slots;
-  A.sel = st.sel; A.out_hash = st.out_hash; A.out_viol = st.out_viol;
-  A.pendA = st.pendA; A.pendP1 = st.pendP1; A.pendNX = st.pendNX; A.cap_pend = st.cap_pend;
-  A.ctr = st.ctr; A.races = st.races; A.rcap = st.rcap; A.n_races = st.n_races;
-  A.counts = st.counts; A.tot = st.tot; A.base = st.base; A.tile_tot = st.tile_tot;
-  A.log = FrLog{st.log_keys, st.log_n, st.log_cap}; A.pool = st.pool; A.info = st.info;
+  CUDA_TRY(h, cudaFuncSetAttribute(fr_scan_kernel<SCAN_WPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)st.scan_smem));
+  CUDA_TRY(h, cudaFuncSetAttribute(fr_count_kernel<SCAN_WPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)st.cnt_smem));
+  CUDA_TRY(h, cudaFuncSetAttribute(fr_scatter_kernel<SCAN_WPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)st.cnt_smem));
+  st.brq.assign(T1, {}); st.branch_live.assign(T1, 0);
   return DEMI_OK;
 }
 
 // a new sorted run of `tot[b]` points per branch, laid out deeper-branch-first from `start`
 void fr_add_run(FrState& st, unsigned long long start, const uint32_t* tot) {
-  FrRun run; run.lo.assign(st.T1, 0); run.hi.assign(st.T1, 0);
+  FrRun run; run.lo.assign(st.A.T1, 0); run.hi.assign(st.A.T1, 0);
   unsigned long long off = start;
   const uint32_t idx = (uint32_t)st.runs.size();
   bool any = false;
-  for (uint32_t b = st.T1; b-- > 0;) {
+  for (uint32_t b = st.A.T1; b-- > 0;) {
     run.lo[b] = off; off += tot[b]; run.hi[b] = off;
     if (tot[b]) { st.brq[b].push_back(idx); st.branch_live[b] += tot[b]; st.pool_live += tot[b]; any = true; }
   }
   if (any) st.runs.push_back(std::move(run));
 }
 
-// the select kernels over one window given as ascending segments; `quota` winners at most are taken
-int32_t fr_select_window(FrState& st, const std::vector<FrSeg>& segs, uint32_t win_n, uint32_t quota, ulonglong2* dst, uint32_t dst_base,
+// the select kernels over one window given as ascending segments; `quota` winners at most are taken, written to
+// the selection from index `sel_base`
+int32_t fr_select_window(FrState& st, const std::vector<FrSeg>& segs, uint32_t win_n, uint32_t quota, uint32_t sel_base,
                          uint32_t* taken, uint32_t* cut) {
   demi_handle* h = st.h;
+  FrSelArgs& S = st.S;
   if (segs.size() > st.segs_cap) return fail(h, DEMI_ERR_CAPACITY, "demi_dpor_frontier: %zu queue segments in one window", segs.size());
-  CUDA_TRY(h, cudaMemcpyAsync(st.segs_dev, segs.data(), segs.size() * sizeof(FrSeg), cudaMemcpyHostToDevice, st.s));
-  CUDA_TRY(h, cudaMemsetAsync(st.skey, 0, (size_t)st.s_slots * 8, st.s));
-  CUDA_TRY(h, cudaMemsetAsync(st.sidx, 0xFF, (size_t)st.s_slots * 4, st.s));
-  FrSelArgs S{};
-  S.pool = st.pool; S.segs = st.segs_dev; S.n_segs = (uint32_t)segs.size(); S.win_n = win_n;
-  S.E = st.E; S.e_slots = st.F.explored_slots; S.win = st.win; S.flag = st.flag;
-  S.skey = st.skey; S.sidx = st.sidx; S.s_slots = st.s_slots;
-  S.blockcnt = st.blockcnt; S.n_blocks = (win_n + 255) / 256;
-  S.sel = dst; S.sel_base = dst_base; S.quota = quota; S.info = st.info; S.ctr = st.ctr;
-  S.no_history = (st.F.flags & DEMI_FR_NO_HISTORY) ? 1u : 0u;
-  S.log = FrLog{st.log_keys, st.log_n, st.log_cap};
+  CUDA_TRY(h, cudaMemcpyAsync(const_cast<FrSeg*>(S.segs), segs.data(), segs.size() * sizeof(FrSeg), cudaMemcpyHostToDevice, st.s));
+  CUDA_TRY(h, cudaMemsetAsync(S.skey, 0, (size_t)S.s_slots * 8, st.s));
+  CUDA_TRY(h, cudaMemsetAsync(S.sidx, 0xFF, (size_t)S.s_slots * 4, st.s));
+  S.n_segs = (uint32_t)segs.size(); S.win_n = win_n; S.n_blocks = (win_n + 255) / 256;
+  S.sel_base = sel_base; S.quota = quota;
   fr_sel_probe_kernel<<<S.n_blocks, 256, 0, st.s>>>(S);
   fr_sel_winner_kernel<<<S.n_blocks, 256, 0, st.s>>>(S);
   fr_sel_blockscan_kernel<<<1, 1024, 0, st.s>>>(S);
   fr_sel_assign_kernel<<<S.n_blocks, 256, 0, st.s>>>(S);
   CUDA_TRY(h, cudaGetLastError());
   FrInfo info;
-  CUDA_TRY(h, cudaMemcpyAsync(&info, st.info, sizeof(info), cudaMemcpyDeviceToHost, st.s));
-  if (!S.no_history) CUDA_TRY(h, cudaMemcpyAsync(&st.explored_sel, st.ctr + FRC_EXPLORED, 8, cudaMemcpyDeviceToHost, st.s));
+  CUDA_TRY(h, cudaMemcpyAsync(&info, S.info, sizeof(info), cudaMemcpyDeviceToHost, st.s));
+  if (!S.no_history) CUDA_TRY(h, cudaMemcpyAsync(&st.explored_sel, S.ctr + FRC_EXPLORED, 8, cudaMemcpyDeviceToHost, st.s));
   CUDA_TRY(h, cudaStreamSynchronize(st.s));
   *taken = info.taken; *cut = info.cut;
   h->perf.kernel_launches += 4;
@@ -290,7 +279,7 @@ int32_t fr_select_front(FrState& st, uint32_t quota, uint32_t* n_sel) {
   while (*n_sel < quota && st.pool_live > 0) {
     segs.clear(); src.clear();
     uint32_t win_n = 0;
-    for (uint32_t b = st.T1; b-- > 0 && win_n < st.win_cap;) {
+    for (uint32_t b = st.A.T1; b-- > 0 && win_n < st.win_cap;) {
       if (!st.branch_live[b]) continue;
       for (uint32_t r : st.brq[b]) {
         const FrRun& run = st.runs[r];
@@ -303,7 +292,7 @@ int32_t fr_select_front(FrState& st, uint32_t quota, uint32_t* n_sel) {
       }
     }
     uint32_t taken = 0, cut = 0;
-    int32_t rc = fr_select_window(st, segs, win_n, quota - *n_sel, st.sel, *n_sel, &taken, &cut);
+    int32_t rc = fr_select_window(st, segs, win_n, quota - *n_sel, *n_sel, &taken, &cut);
     if (rc != DEMI_OK) return rc;
     uint32_t left = cut;                                    // dequeue the first `cut` points of the window
     for (size_t i = 0; i < segs.size() && left; i++) {
@@ -321,12 +310,12 @@ int32_t fr_select_front(FrState& st, uint32_t quota, uint32_t* n_sel) {
   return DEMI_OK;
 }
 
-// the LAST m points of the queue (shallowest branch), filtered and marked like a dequeue; survivors -> st.sel[0..n)
+// the LAST m points of the queue (shallowest branch), filtered and marked like a dequeue; survivors -> the selection [0, n)
 int32_t fr_select_tail(FrState& st, unsigned long long m, uint32_t* n_out) {
   *n_out = 0;
   std::vector<FrSeg> segs;
   unsigned long long need = m;
-  for (uint32_t b = 0; b < st.T1 && need; b++) {
+  for (uint32_t b = 0; b < st.A.T1 && need; b++) {
     if (!st.branch_live[b]) continue;
     auto& q = st.brq[b];
     for (auto it = q.rbegin(); it != q.rend() && need; ++it) {
@@ -352,7 +341,7 @@ int32_t fr_select_tail(FrState& st, unsigned long long m, uint32_t* n_out) {
       if (off_in_seg == segs[i].count) { i++; off_in_seg = 0; }
     }
     uint32_t taken = 0, cut = 0;
-    int32_t rc = fr_select_window(st, w, win_n, win_n, st.sel, *n_out, &taken, &cut);
+    int32_t rc = fr_select_window(st, w, win_n, win_n, *n_out, &taken, &cut);
     if (rc != DEMI_OK) return rc;
     st.R.keys_dropped += win_n - taken;
     *n_out += taken;
@@ -380,20 +369,19 @@ int32_t fr_execute_and_scan(FrState& st, uint32_t n_sel, bool root) {
   st.v->fn<<<(n_sel + st.v->bd - 1) / st.v->bd, st.v->bd, st.v->smem, st.s>>>(A);
   CUDA_TRY(h, cudaEventRecord(st.ev[1], st.s));
   const uint32_t wb = (n_sel + SCAN_WPB - 1) / SCAN_WPB;
-  const size_t scan_smem = (size_t)SCAN_WPB * fr_scan_words(st.T1) * 4, cnt_smem = (size_t)SCAN_WPB * fr_cnt_words(st.T1) * 4;
-  fr_scan_kernel<SCAN_WPB><<<wb, SCAN_WPB * 32, scan_smem, st.s>>>(A);       // every race of the round is marked explored ...
-  fr_count_kernel<SCAN_WPB><<<wb, SCAN_WPB * 32, cnt_smem, st.s>>>(A);        // ... before any of its points is enqueued
+  fr_scan_kernel<SCAN_WPB><<<wb, SCAN_WPB * 32, st.scan_smem, st.s>>>(A);    // every race of the round is marked explored ...
+  fr_count_kernel<SCAN_WPB><<<wb, SCAN_WPB * 32, st.cnt_smem, st.s>>>(A);     // ... before any of its points is enqueued
   const uint32_t n_tiles = (n_sel + FR_TILE - 1) / FR_TILE;
-  fr_rowscan_kernel<<<dim3(st.T1, n_tiles), 256, 0, st.s>>>(A);
+  fr_rowscan_kernel<<<dim3(A.T1, n_tiles), 256, 0, st.s>>>(A);
   fr_base_kernel<<<1, 1024, 0, st.s>>>(A, n_tiles);
-  fr_scatter_kernel<SCAN_WPB><<<wb, SCAN_WPB * 32, cnt_smem, st.s>>>(A, st.F.pool_cap);
+  fr_scatter_kernel<SCAN_WPB><<<wb, SCAN_WPB * 32, st.cnt_smem, st.s>>>(A, st.F.pool_cap);
   CUDA_TRY(h, cudaGetLastError());
   CUDA_TRY(h, cudaEventRecord(st.ev[2], st.s));
   h->perf.kernel_launches += 6;
-  std::vector<uint32_t> tot(st.T1);
+  std::vector<uint32_t> tot(A.T1);
   unsigned long long ctr[FRC_N];
-  CUDA_TRY(h, cudaMemcpyAsync(tot.data(), st.tot, st.T1 * 4, cudaMemcpyDeviceToHost, st.s));
-  CUDA_TRY(h, cudaMemcpyAsync(ctr, st.ctr, sizeof(ctr), cudaMemcpyDeviceToHost, st.s));
+  CUDA_TRY(h, cudaMemcpyAsync(tot.data(), A.tot, A.T1 * 4, cudaMemcpyDeviceToHost, st.s));
+  CUDA_TRY(h, cudaMemcpyAsync(ctr, A.ctr, sizeof(ctr), cudaMemcpyDeviceToHost, st.s));
   CUDA_TRY(h, cudaStreamSynchronize(st.s));
   float ms = 0;
   cudaEventElapsedTime(&ms, st.ev[0], st.ev[1]); st.R.exec_ms += ms;
@@ -401,7 +389,7 @@ int32_t fr_execute_and_scan(FrState& st, uint32_t n_sel, bool root) {
   if (ctr[FRC_STATUS]) return fr_round_fail(st, (uint32_t)ctr[FRC_STATUS]);
   if (ctr[FRC_EXPLORED] * 2 >= st.F.explored_slots) return fr_round_fail(st, DEMI_DS_EXPLORED_OVF);   // after the round's scan
   unsigned long long added = 0;
-  for (uint32_t b = 0; b < st.T1; b++) added += tot[b];
+  for (uint32_t b = 0; b < A.T1; b++) added += tot[b];
   if (st.pool_top + added > st.F.pool_cap) return fr_round_fail(st, DEMI_DS_HEAP_OVF);   // pool_cap bounds the arena: every point enqueued or received
   fr_add_run(st, st.pool_top, tot.data());
   st.pool_top += added;
@@ -417,18 +405,19 @@ int32_t fr_execute_and_scan(FrState& st, uint32_t n_sel, bool root) {
 // order in which they were logged does not matter): the rank-local explored sets stop diverging
 int32_t fr_share_explored(FrState& st, const std::vector<unsigned long long>& n_new) {
   demi_handle* h = st.h; NcclApi* nc = nccl_api(); FrComm* cm = st.comm;
+  const FrLog& log = st.A.log;
   const int G = cm->world, me = cm->rank;
   unsigned long long maxn = 0;
   for (int q = 0; q < G; q++) maxn = std::max(maxn, n_new[q]);
   if (!maxn) return DEMI_OK;
-  if (maxn > st.log_cap) { st.R.status = DEMI_DS_EXPLORED_OVF; return DEMI_OK; }
+  if (maxn > log.cap) { st.R.status = DEMI_DS_EXPLORED_OVF; return DEMI_OK; }
   // equal-size all-gather: every rank contributes `maxn` slots of its log (the tail beyond its own count is ignored)
   CUDA_TRY(h, cudaMemcpyAsync(st.log_counts, n_new.data(), (size_t)G * 8, cudaMemcpyHostToDevice, st.s));
-  NCCL_TRY(h, nc->AllGather(st.log_keys, st.log_all, (size_t)maxn, ncclUint64, cm->comm, st.s));
+  NCCL_TRY(h, nc->AllGather(log.keys, st.log_all, (size_t)maxn, ncclUint64, cm->comm, st.s));
   fr_merge_keys_kernel<<<dim3((unsigned)((maxn + 255) / 256), (unsigned)G), 256, 0, st.s>>>(st.log_all, (unsigned int)maxn, st.log_counts, (unsigned)G, (unsigned)me,
-                                                                                          st.E, st.F.explored_slots, st.ctr);
+                                                                                          st.A.E, st.F.explored_slots, st.A.ctr);
   CUDA_TRY(h, cudaGetLastError());
-  CUDA_TRY(h, cudaMemsetAsync(st.log_n, 0, 4, st.s));
+  CUDA_TRY(h, cudaMemsetAsync(log.n, 0, 4, st.s));
   h->perf.kernel_launches++;
   st.R.bytes_sent += n_new[me] * 8ull * (unsigned long long)(G - 1);
   return DEMI_OK;
@@ -439,6 +428,7 @@ int32_t fr_exchange(FrState& st, const std::vector<unsigned long long>& have_in,
                     std::vector<unsigned long long>& have_after) {
   demi_handle* h = st.h; NcclApi* nc = nccl_api(); FrComm* cm = st.comm;
   const int G = cm->world, me = cm->rank;
+  const uint32_t rec_u4 = st.X.rec_u4, T1 = st.A.T1;
   const unsigned long long S = st.F.rounds_per_exchange ? st.F.rounds_per_exchange : 1;
   const unsigned long long need = S * st.F.width;
   const unsigned long long share = (total_pool + G - 1) / G;
@@ -470,13 +460,13 @@ int32_t fr_exchange(FrState& st, const std::vector<unsigned long long>& have_in,
     if (rc != DEMI_OK) return rc;
     send_off[rcv] = off;
     if (n) {
-      FrXArgs X{}; X.sel = st.sel; X.n = n; X.buf = st.sendbuf + off * st.rec_u4; X.rec_u4 = st.rec_u4; X.tr = st.tr; X.tr_meta = st.tr_meta; X.T1 = st.T1;
+      FrXArgs X = st.X; X.n = n; X.buf = st.sendbuf + off * rec_u4;
       fr_pack_kernel<<<n, 128, 0, st.s>>>(X);
       CUDA_TRY(h, cudaGetLastError());
       h->perf.kernel_launches++;
     }
     my_row[rcv] = n; off += n;
-    st.R.records_sent += n; st.R.bytes_sent += (unsigned long long)n * st.rec_u4 * 16;
+    st.R.records_sent += n; st.R.bytes_sent += (unsigned long long)n * rec_u4 * 16;
   }
   // every rank learns how many records really travel (points found explored on the donor are dropped there)
   std::vector<unsigned long long> row64(G), mat((size_t)G * G);
@@ -497,9 +487,9 @@ int32_t fr_exchange(FrState& st, const std::vector<unsigned long long>& have_in,
   for (int don = 0; don < G; don++) { recv_off[don] = roff; roff += (size_t)mat[(size_t)don * G + me]; }
   NCCL_TRY(h, nc->GroupStart());
   for (int rcv = 0; rcv < G; rcv++) if (my_row[rcv])
-    NCCL_TRY(h, nc->Send(st.sendbuf + send_off[rcv] * st.rec_u4, (size_t)my_row[rcv] * st.rec_u4 * 16, ncclUint8, rcv, cm->comm, st.s));
+    NCCL_TRY(h, nc->Send(st.sendbuf + send_off[rcv] * rec_u4, (size_t)my_row[rcv] * rec_u4 * 16, ncclUint8, rcv, cm->comm, st.s));
   for (int don = 0; don < G; don++) if (mat[(size_t)don * G + me])
-    NCCL_TRY(h, nc->Recv(st.recvbuf + recv_off[don] * st.rec_u4, (size_t)mat[(size_t)don * G + me] * st.rec_u4 * 16, ncclUint8, don, cm->comm, st.s));
+    NCCL_TRY(h, nc->Recv(st.recvbuf + recv_off[don] * rec_u4, (size_t)mat[(size_t)don * G + me] * rec_u4 * 16, ncclUint8, don, cm->comm, st.s));
   NCCL_TRY(h, nc->GroupEnd());
   // receiver side: every donor's batch becomes trace slots + one sorted run
   for (int don = 0; don < G; don++) {
@@ -507,16 +497,15 @@ int32_t fr_exchange(FrState& st, const std::vector<unsigned long long>& have_in,
     if (!n) continue;
     if ((unsigned long long)st.n_slots + n > st.F.trace_cap) { st.R.status = DEMI_DS_TRACE_OVF; break; }
     if (st.pool_top + n > st.F.pool_cap) { st.R.status = DEMI_DS_HEAP_OVF; break; }
-    CUDA_TRY(h, cudaMemsetAsync(st.hist, 0, st.T1 * 4, st.s));
-    FrXArgs X{}; X.n = n; X.buf = st.recvbuf + recv_off[don] * st.rec_u4; X.rec_u4 = st.rec_u4; X.tr = st.tr; X.tr_meta = st.tr_meta; X.T1 = st.T1;
-    X.first_slot = st.n_slots; X.pool = st.pool; X.pool_top = st.pool_top; X.hist = st.hist;
+    CUDA_TRY(h, cudaMemsetAsync(st.X.hist, 0, T1 * 4, st.s));
+    FrXArgs X = st.X; X.n = n; X.buf = st.recvbuf + recv_off[don] * rec_u4; X.first_slot = st.n_slots; X.pool_top = st.pool_top;
     // the batch arrives in the donor's queue order (branch desc, then its slot order), which the new slots preserve;
     // the run lays branches out deepest first, so the records of one branch must be contiguous: they are.
     fr_unpack_kernel<<<n, 128, 0, st.s>>>(X);
     CUDA_TRY(h, cudaGetLastError());
     h->perf.kernel_launches++;
-    std::vector<uint32_t> tot(st.T1);
-    CUDA_TRY(h, cudaMemcpyAsync(tot.data(), st.hist, st.T1 * 4, cudaMemcpyDeviceToHost, st.s));
+    std::vector<uint32_t> tot(T1);
+    CUDA_TRY(h, cudaMemcpyAsync(tot.data(), X.hist, T1 * 4, cudaMemcpyDeviceToHost, st.s));
     CUDA_TRY(h, cudaStreamSynchronize(st.s));
     fr_add_run(st, st.pool_top, tot.data());
     st.pool_top += n; st.n_slots += n; st.R.records_received += n;
@@ -524,8 +513,6 @@ int32_t fr_exchange(FrState& st, const std::vector<unsigned long long>& have_in,
   CUDA_TRY(h, cudaStreamSynchronize(st.s));
   return DEMI_OK;
 }
-
-struct FrCache { FrGeom geom; FrState st; };
 
 int32_t fr_run(FrState& st, demi_dpor_violation* viol, uint32_t cap_viol, uint64_t* hashes, uint64_t cap_hashes) {
   demi_handle* h = st.h;
@@ -543,9 +530,9 @@ int32_t fr_run(FrState& st, demi_dpor_violation* viol, uint32_t cap_viol, uint64
     if (G > 1) {
       const auto t0 = std::chrono::steady_clock::now();
       NcclApi* nc = nccl_api();
-      if (st.log_n) {                                                         // how many pair keys this rank has to share
+      if (st.A.log.n) {                                                       // how many pair keys this rank has to share
         unsigned int nn = 0;
-        CUDA_TRY(h, cudaMemcpyAsync(&nn, st.log_n, 4, cudaMemcpyDeviceToHost, st.s));
+        CUDA_TRY(h, cudaMemcpyAsync(&nn, st.A.log.n, 4, cudaMemcpyDeviceToHost, st.s));
         CUDA_TRY(h, cudaStreamSynchronize(st.s));
         mine[4] = nn;
       }
@@ -565,7 +552,7 @@ int32_t fr_run(FrState& st, demi_dpor_violation* viol, uint32_t cap_viol, uint64
     std::vector<unsigned long long> have_after = have;
     if (G > 1) {
       const auto t0 = std::chrono::steady_clock::now();
-      if (st.log_n && (rc = fr_share_explored(st, n_new)) != DEMI_OK) return rc;
+      if (st.A.log.n && (rc = fr_share_explored(st, n_new)) != DEMI_OK) return rc;
       if (st.R.status) continue;
       if ((rc = fr_exchange(st, have, total_pool, have_after)) != DEMI_OK) return rc;
       st.R.exchange_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
@@ -594,7 +581,7 @@ int32_t fr_run(FrState& st, demi_dpor_violation* viol, uint32_t cap_viol, uint64
   // results
   if (!st.round_failed) {
     unsigned long long ctr[FRC_N];                          // a steal round marks the points it hands over
-    CUDA_TRY(h, cudaMemcpy(ctr, st.ctr, sizeof(ctr), cudaMemcpyDeviceToHost));
+    CUDA_TRY(h, cudaMemcpy(ctr, st.A.ctr, sizeof(ctr), cudaMemcpyDeviceToHost));
     st.R.explored_pairs = ctr[FRC_EXPLORED];
   }
   st.R.pool_left = st.pool_live; st.R.trace_slots = st.n_slots;
@@ -602,14 +589,14 @@ int32_t fr_run(FrState& st, demi_dpor_violation* viol, uint32_t cap_viol, uint64
   if (st.n_exec) {
     // only what the caller asked for crosses PCIe: the schedule hashes if wanted, and the violating records (compacted
     // on the device, then put back in execution order)
-    if (hashes) CUDA_TRY(h, cudaMemcpy(hashes, st.out_hash, std::min<unsigned long long>(st.n_exec, cap_hashes) * 8, cudaMemcpyDeviceToHost));
+    if (hashes) CUDA_TRY(h, cudaMemcpy(hashes, st.A.out_hash, std::min<unsigned long long>(st.n_exec, cap_hashes) * 8, cudaMemcpyDeviceToHost));
     if (viol && cap_viol) {
       DevBuf buf;
       if ((rc = buf.grow(h, (size_t)cap_viol * sizeof(demi_dpor_violation) + 16)) != DEMI_OK) return rc;
       demi_dpor_violation* vd = buf.get<demi_dpor_violation>();
       unsigned int* cnt = (unsigned int*)(vd + cap_viol);
       CUDA_TRY(h, cudaMemsetAsync(cnt, 0, 4, st.s));
-      fr_collect_viol_kernel<<<(unsigned)((st.n_exec + 255) / 256), 256, 0, st.s>>>(st.out_hash, st.out_viol, st.n_exec, vd, cap_viol, cnt);
+      fr_collect_viol_kernel<<<(unsigned)((st.n_exec + 255) / 256), 256, 0, st.s>>>(st.A.out_hash, st.A.out_viol, st.n_exec, vd, cap_viol, cnt);
       CUDA_TRY(h, cudaGetLastError());
       unsigned int nv = 0;
       CUDA_TRY(h, cudaMemcpyAsync(&nv, cnt, 4, cudaMemcpyDeviceToHost, st.s));
@@ -624,10 +611,12 @@ int32_t fr_run(FrState& st, demi_dpor_violation* viol, uint32_t cap_viol, uint64
 }
 }  // namespace
 
+struct FrCache { FrGeom geom; FrState st; };
+
 void demi_frontier_free(demi_handle* h) {
   if (!h->frontier) return;
   cudaSetDevice(h->cfg.device);
-  delete (FrCache*)h->frontier;
+  delete h->frontier;
   h->frontier = nullptr;
 }
 
@@ -642,19 +631,14 @@ extern "C" int32_t demi_dpor_frontier(demi_handle* h, const demi_ext_event* ext,
   if (F.explored_slots < 1024 || (F.explored_slots & (F.explored_slots - 1))) return fail(h, DEMI_ERR_INVALID, "demi_dpor_frontier: explored_slots must be a power of two >= 1024");
   if (!F.pool_cap || !F.trace_cap || F.trace_cap >= (1u << 28)) return fail(h, DEMI_ERR_INVALID, "demi_dpor_frontier: pool_cap / trace_cap (below 2^28) must be positive");
   { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
-  const int n_actors = demi_model_actors(h);
-  for (uint32_t i = 0; i < n_ext; i++) {
-    if (ext[i].kind != DEMI_EXT_START && ext[i].kind != DEMI_EXT_SEND)       // "unsuported external event" (:710)
-      return fail(h, DEMI_ERR_INVALID, "demi_dpor_frontier: external %u is neither Start nor Send", i);
-    if (ext[i].a >= n_actors) return fail(h, DEMI_ERR_INVALID, "demi_dpor_frontier: external %u names an unknown actor", i);
-  }
-  FrComm* cm = (FrComm*)h->comm;
+  { int32_t vrc = demi_check_dpor_program(h, "demi_dpor_frontier", ext, n_ext); if (vrc != DEMI_OK) return vrc; }
+  FrComm* cm = h->comm;
   if (cm && cm->world > 1 && !F.steal_max) return fail(h, DEMI_ERR_INVALID, "demi_dpor_frontier: steal_max must be positive on %d ranks", cm->world);
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   uint32_t n_sends = 0;
   for (uint32_t i = 0; i < n_ext; i++) if (ext[i].kind == DEMI_EXT_SEND) n_sends++;
   FrGeom g{h->cfg.model, (cm && cm->world > 1) ? cm->world : 1, F, n_sends, std::max<uint32_t>(n_ext, 64)};
-  FrCache* cache = (FrCache*)h->frontier;
+  FrCache* cache = h->frontier;
   bool reuse = cache && fr_same_geom(cache->geom, g, n_ext);
   if (!reuse) { delete cache; cache = new FrCache(); cache->geom = g; h->frontier = cache; }
   FrState& st = cache->st;

@@ -19,6 +19,8 @@
 extern thread_local std::string g_create_error;
 
 struct demi_handle;
+struct FrComm;                                     // the communicator (capi_frontier.cu)
+struct FrCache;                                    // K3F's buffers and queue directory, kept between calls (capi_frontier.cu)
 // A device allocation with one owner, which frees it: moved, never copied.  Every device buffer of the library is one.
 class DevBuf {
  public:
@@ -76,7 +78,7 @@ struct demi_handle {
   demi::LaneTreeKey lane_tree_key{};
   int32_t lane_tree_depth = -1;                    // the depth the last fuzz launch walked (-1: not the steady one)
   DevBuf prov_scratch;
-  DevBuf dpor_buf[24];                             // K3 per-search structures (capi_dpor.cu)
+  std::vector<DevBuf> dpor_buf;                    // K3 per-search structures, one per entry of dpor_run's table (capi_dpor.cu)
   cudaStream_t stream = nullptr, copy_stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   demi_perf perf{};
@@ -100,8 +102,8 @@ struct demi_handle {
     DevBuf views;                                    // view, on the device
   } set;
   // ---- communicator (capi_frontier.cu): NCCL inside the library
-  void* comm = nullptr;
-  void* frontier = nullptr;      // cached K3F buffers
+  FrComm* comm = nullptr;
+  FrCache* frontier = nullptr;
   // ---- a model loaded with demi_load_model (model == DEMI_MODEL_IR)
   bool ir_loaded = false;
   DevBuf ir_blob_dev;                              // the blob's header and programs (ir_dev points into it)
@@ -200,6 +202,16 @@ inline int32_t demi_check_externals(demi_handle* h, const char* who, const demi_
   for (uint32_t i = 0; i < n; i++) {
     const int32_t rc = demi_check_external(h, who, "", ev, i, false, false);
     if (rc != DEMI_OK) return rc;
+  }
+  return DEMI_OK;
+}
+// a program for DPOR: Start and Send only ("unsuported external event", DPORwHeuristics.scala:710), actors of the model
+inline int32_t demi_check_dpor_program(demi_handle* h, const char* who, const demi_ext_event* ev, uint32_t n) {
+  const uint32_t na = (uint32_t)demi_model_actors(h);
+  for (uint32_t i = 0; i < n; i++) {
+    if (ev[i].kind != DEMI_EXT_START && ev[i].kind != DEMI_EXT_SEND)
+      return fail(h, DEMI_ERR_INVALID, "%s: external %u: DPOR accepts Start and Send only", who, i);
+    if (ev[i].a >= na) return fail(h, DEMI_ERR_INVALID, "%s: external %u names an unknown actor", who, i);
   }
   return DEMI_OK;
 }

@@ -410,20 +410,26 @@ class Engine(object):
     def dpor_batch(self, programs, max_messages, max_interleavings, looking_for=0, stop_if_found=False, depth_bound=-1,
                    node_cap=4096, explored_slots=1 << 16, heap_cap=1 << 15, cap_viol=64, want_hashes=False):
         """`programs`: list of external-event programs (Start/Send only), one independent search each."""
-        packed = [p if isinstance(p, np.ndarray) else pack_externals(p) for p in programs]
-        offs = np.zeros(len(packed) + 1, dtype=np.uint32)
-        offs[1:] = np.cumsum([len(p) for p in packed])
-        ext = np.ascontiguousarray(np.concatenate(packed), dtype=N.EXT_DTYPE)
+        ext, offs = self._pack_programs(programs)
+        n = len(offs) - 1
         P = N.DporParams(max_messages, depth_bound, max_interleavings, looking_for or 0, 1 if stop_if_found else 0,
                          node_cap, explored_slots, heap_cap)
-        res = np.zeros(len(packed), dtype=N.DPOR_RESULT_DTYPE)
-        viol = np.zeros((len(packed), cap_viol), dtype=N.DPOR_VIOL_DTYPE)
+        res = np.zeros(n, dtype=N.DPOR_RESULT_DTYPE)
+        viol = np.zeros((n, cap_viol), dtype=N.DPOR_VIOL_DTYPE)
         cap_h = max_interleavings + 1 if want_hashes else 0
-        hashes = np.zeros((len(packed), max(cap_h, 1)), dtype=np.uint64)
-        self._check(N.lib().demi_dpor_batch(self._h, ext.ctypes.data, offs.ctypes.data, len(packed), C.byref(P),
+        hashes = np.zeros((n, max(cap_h, 1)), dtype=np.uint64)
+        self._check(N.lib().demi_dpor_batch(self._h, ext.ctypes.data, offs.ctypes.data, n, C.byref(P),
                                             res.ctypes.data, viol.ctypes.data, cap_viol,
                                             hashes.ctypes.data if want_hashes else None, cap_h))
         return res, viol, hashes
+
+    @staticmethod
+    def _pack_programs(programs):
+        """DPOR programs -> (externals one program after the other, offsets[i] = where program i starts)."""
+        packed = [p if isinstance(p, np.ndarray) else pack_externals(p) for p in programs]
+        offs = np.zeros(len(packed) + 1, dtype=np.uint32)
+        offs[1:] = np.cumsum([len(p) for p in packed])
+        return np.ascontiguousarray(np.concatenate(packed), dtype=N.EXT_DTYPE), offs
 
     @staticmethod
     def _seed(seed):
@@ -437,10 +443,8 @@ class Engine(object):
         """DPOR instances in RunnerUtils.editDistanceDporDDMin's configuration.  `seed` = (events, dep_parent) of the
         recorded execution; `caps[i]` = the setMaxDistance values instance i is tested with, in order (None: one
         uncapped test)."""
-        packed = [p if isinstance(p, np.ndarray) else pack_externals(p) for p in programs]
-        offs = np.zeros(len(packed) + 1, dtype=np.uint32)
-        offs[1:] = np.cumsum([len(p) for p in packed])
-        ext = np.ascontiguousarray(np.concatenate(packed), dtype=N.EXT_DTYPE)
+        ext, offs = self._pack_programs(programs)
+        n = len(offs) - 1
         P = N.DporParams(max_messages, -1, max_interleavings, looking_for or 0, 1 if stop_if_found else 0,
                          node_cap, explored_slots, heap_cap)
         ex = N.DporEx(flags, None, None, None)
@@ -450,15 +454,15 @@ class Engine(object):
             keep += [sd, alive]
             ex.seed = C.pointer(sd)
         if caps is not None:
-            coff = np.zeros(len(packed) + 1, dtype=np.uint32)
+            coff = np.zeros(n + 1, dtype=np.uint32)
             coff[1:] = np.cumsum([len(c) for c in caps])
             cflat = np.ascontiguousarray(np.concatenate([np.asarray(c, dtype=np.int32) for c in caps]), dtype=np.int32)
             keep += [coff, cflat]
             ex.caps, ex.cap_offsets = cflat.ctypes.data, coff.ctypes.data
-        res = np.zeros(len(packed), dtype=N.DPOR_RESULT_DTYPE)
+        res = np.zeros(n, dtype=N.DPOR_RESULT_DTYPE)
         cap_h = max_interleavings + 1 if want_hashes else 0
-        hashes = np.zeros((len(packed), max(cap_h, 1)), dtype=np.uint64)
-        self._check(N.lib().demi_dpor_batch_ex(self._h, ext.ctypes.data, offs.ctypes.data, len(packed), C.byref(P),
+        hashes = np.zeros((n, max(cap_h, 1)), dtype=np.uint64)
+        self._check(N.lib().demi_dpor_batch_ex(self._h, ext.ctypes.data, offs.ctypes.data, n, C.byref(P),
                                                C.byref(ex), res.ctypes.data, None, 0,
                                                hashes.ctypes.data if want_hashes else None, cap_h))
         return res, hashes

@@ -268,21 +268,22 @@ def test_capacity_edges(oracle):
 
 
 def test_errors(oracle):
-    """No model loaded: DEMI_ERR_STATE from every K3 entry point; an external naming an actor at or above the loaded
-    count: DEMI_ERR_INVALID."""
+    """No model loaded: DEMI_ERR_STATE from every K3 and K3F entry point; an external naming an actor at or above the
+    loaded count, or of a kind other than Start and Send: DEMI_ERR_INVALID."""
     m = election_model()
     prog = election_program(wait=False)
     ev, par, steps, _ = election_recorded(oracle, SHRINKING_SEED)
     calls = (lambda e, p: e.dpor_batch([p], 10, 10),
              lambda e, p: e.dpor_batch_ex([p], 10, 10, seed=(ev, par), flags=N.DF_ARVIND_ORDERING),
-             lambda e, p: e.incremental_ddmin(p, steps, 10, (ev, par), looking_for=TWO_LEADERS))
+             lambda e, p: e.incremental_ddmin(p, steps, 10, (ev, par), looking_for=TWO_LEADERS),
+             lambda e, p: e.dpor_frontier(p, e.frontier_params(10, 10, 16)))
     bare = D.Engine(D.SchedulerConfig(N.MODEL_IR, model_flags=m.flags))
     for call in calls:
         with pytest.raises(D.DemiError) as e:
             call(bare, prog)
         assert e.value.code == N.ERR_STATE
     eng = ir_engine(m.blob, m.flags)
-    for bad in (prog + [D.Start(3)], prog + [D.Send(3, KICK, 0)], [D.Start(15)]):
+    for bad in (prog + [D.Start(3)], prog + [D.Send(3, KICK, 0)], [D.Start(15)], prog + [D.WaitQuiescence()]):
         for call in calls:
             with pytest.raises(D.DemiError) as e:
                 call(eng, bad)
