@@ -65,6 +65,10 @@ class IntMinOut(C.Structure):
                 ("replays_executed", C.c_uint32), ("batches", C.c_uint32)]
 
 
+INTMIN_OUT_DTYPE = np.dtype([(n, "<u4") for n, _ in IntMinOut._fields_])
+assert INTMIN_OUT_DTYPE.itemsize == C.sizeof(IntMinOut)
+
+
 class DporParams(C.Structure):
     _fields_ = [("max_messages", C.c_int32), ("depth_bound", C.c_int32), ("max_interleavings", C.c_uint32),
                 ("looking_for", C.c_uint32), ("stop_if_found", C.c_uint32), ("node_cap", C.c_uint32),
@@ -129,6 +133,7 @@ EXPORTS = [
     "demi_set_fuzzer", "demi_fuzz_campaign", "demi_fuzz_campaign_dev",
     "demi_random_test_batch", "demi_random_ddmin", "demi_random_test_trace",
     "demi_fuzz_traces", "demi_set_traces", "demi_replay_batch_many", "demi_ddmin_many",
+    "demi_replay_traces_many", "demi_internal_minimize_many",
 ]
 FILTER_RULE_DTYPE = np.dtype([("src_mask", "<u4"), ("dst_mask", "<u4"), ("type_mask", "<u4"), ("flags", "<u4")])
 FRULE_DEADLETTERS = 1
@@ -324,6 +329,10 @@ def lib():
     L.demi_replay_batch_many.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp]
     L.demi_ddmin_many.restype = C.c_int32
     L.demi_ddmin_many.argtypes = [vp, vp, C.c_uint32, C.c_int32, vp, C.c_uint32, vp, C.c_uint32, vp, vp]
+    L.demi_replay_traces_many.restype = C.c_int32
+    L.demi_replay_traces_many.argtypes = [vp, vp, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, vp]
+    L.demi_internal_minimize_many.restype = C.c_int32
+    L.demi_internal_minimize_many.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, vp]
     L.demi_stats.restype = C.c_int32
     L.demi_stats.argtypes = [vp, C.POINTER(Perf)]
     L.demi_lane_kernel.restype = C.c_int32

@@ -2,87 +2,12 @@
 // (minification/internal_minimization/ScheduleCheckers.scala:19-107) with the
 // LeftToRightOneAtATime (OneAtATimeRemoval.scala:17-137) or SrcDstFIFORemoval (:139-251) removal strategy.
 //
-// The reference tries ONE delivery at a time: drop it from the last failing trace,
-// ask STSSched whether the violation still shows, and on success continue from the
-// trace STSSched recorded.  While removals keep failing, the candidates all refer to
-// the same base trace, so they are independent: here the whole remaining left-to-right
-// candidate list of the current base trace is evaluated in one K2 launch
-// (demi_replay_batch_ex with skip_events) and then committed in the reference's order
-// up to the first success; the successful one is re-run in recording mode to obtain
-// the new base trace.  Decisions, counters and the final trace are the sequential ones.
-#include <map>
-#include <tuple>
+// IntMinDriver (intmin_driver.hpp) makes the decisions; here they are served on the handle's single trace: the
+// whole remaining candidate list of the current base trace is evaluated in one K2 launch (demi_replay_batch_ex with
+// skip_events), the first success is re-run in recording mode (demi_replay_trace), and the recorded trace becomes
+// the handle's trace.  Decisions, counters and the final trace are the sequential ones.
 #include "engine.hpp"
-
-namespace {
-typedef std::tuple<uint32_t, uint32_t, uint32_t, uint32_t, uint32_t> Key;   // (snd, rcv, type, p0, p1) == (snd, rcv, fingerprint)
-typedef std::map<Key, uint32_t> MultiSet;
-Key key_of(const demi_event& e) { return Key(e.src, e.dst, e.type, e.p0, e.p1); }
-uint32_t count_of(const MultiSet& m, const Key& k) { auto it = m.find(k); return it == m.end() ? 0u : it->second; }
-
-// RemovalStrategy state.  Copyable: the candidates the strategy would produce if every test failed are obtained
-// from a copy, the real object then replays the same calls as results are committed.
-struct Strategy {
-  typedef std::tuple<uint32_t, uint32_t, uint32_t> Fp;               // (type, p0, p1)
-  bool fifo = false;
-  MultiSet tried;                                                    // triedIgnoring (:20)
-  std::map<std::pair<uint32_t, uint32_t>, std::vector<Fp>> src_dst;  // srcDstToMessages (:150)
-  std::map<std::pair<uint32_t, uint32_t>, int> cur_idx;              // srcDstToCurrentIdx (:168)
-  bool have_prev = false; std::pair<uint32_t, uint32_t> prev;        // previouslyChosenSrcDst (:162)
-  const std::vector<demi_event>* verified = nullptr;
-
-  void init_fifo(const std::vector<demi_event>& v) {                 // :152-159
-    fifo = true; verified = &v;
-    for (const demi_event& e : v)
-      if (e.kind == DEMI_EV_MSG_EVENT && e.src < DEMI_MAX_ACTORS) src_dst[{e.src, e.dst}].push_back(Fp(e.type, e.p0, e.p1));
-  }
-  bool choice(const demi_event& e) {                                 // choiceFilter :178-203 (LeftToRight: true, :131-137)
-    if (!fifo) return true;
-    if (e.src < DEMI_MAX_ACTORS) {
-      auto it = src_dst.find({e.src, e.dst});
-      if (it != src_dst.end()) {
-        int idx = ++cur_idx[{e.src, e.dst}];
-        if (idx == (int)it->second.size() - 1) {
-          it->second.pop_back();
-          if (it->second.empty()) src_dst.erase(it);
-          have_prev = true; prev = {e.src, e.dst};
-          return true;
-        }
-      }
-    }
-    have_prev = false;
-    return e.src >= DEMI_MAX_ACTORS;                                 // "deadLetters": a timer
-  }
-  // getNextTrace (:57-124; SrcDstFIFORemoval's prologue :209-249): index of the delivery to drop, or -1
-  int next(const std::vector<demi_event>& trace, const MultiSet& pruned, bool triggered) {
-    if (fifo) {
-      if (!triggered && have_prev) src_dst.erase(prev);              // "this src,dst is done"
-      if (triggered) {
-        src_dst.clear();
-        MultiSet copy = pruned;
-        for (size_t i = verified->size(); i-- > 0;) {
-          const demi_event& e = (*verified)[i];
-          if (e.kind != DEMI_EV_MSG_EVENT || e.src >= DEMI_MAX_ACTORS) continue;
-          auto it = copy.find(key_of(e));
-          if (it != copy.end() && it->second) { it->second--; continue; }
-          auto& vec = src_dst[{e.src, e.dst}];
-          vec.insert(vec.begin(), Fp(e.type, e.p0, e.p1));
-        }
-      }
-      cur_idx.clear();
-      for (auto& kv : src_dst) cur_idx[kv.first] = -1;
-    }
-    MultiSet keys = pruned;                                          // keysThisIteration ++= alreadyRemoved
-    for (uint32_t i = 0; i < trace.size(); i++) {
-      if (trace[i].kind != DEMI_EV_MSG_EVENT) continue;
-      const Key k = key_of(trace[i]);
-      const uint32_t c = ++keys[k];
-      if (c > count_of(tried, k) && choice(trace[i])) { tried[k]++; return (int)i; }
-    }
-    return -1;
-  }
-};
-}
+#include "intmin_driver.hpp"
 
 extern "C" int32_t demi_internal_minimize(demi_handle* h, uint32_t looking_for, uint32_t flags,
                                           demi_event* out_trace, uint32_t cap_events,
@@ -90,82 +15,30 @@ extern "C" int32_t demi_internal_minimize(demi_handle* h, uint32_t looking_for, 
   if (!h) return DEMI_ERR_INVALID;
   if (!out) return fail(h, DEMI_ERR_INVALID, "demi_internal_minimize: null output");
   if (h->trace_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_trace has not been called");
-  memset(out, 0, sizeof(*out));
-  const uint32_t ext_mask = demi_ext_type_mask(h);
   const bool use_fifo = (flags & DEMI_IM_SRC_DST_FIFO) != 0;
   flags &= ~DEMI_IM_SRC_DST_FIFO;
-  const std::vector<demi_event> verified = h->trace_host;
-  std::vector<demi_event> cur = h->trace_host;
   const std::vector<demi_ext_event> ext = h->trace_ext_host;
   const uint32_t mw = std::max<uint32_t>(1, ((uint32_t)ext.size() + 63) / 64);
-  MultiSet pruned;
-  Strategy strat;
-  if (use_fifo) strat.init_fifo(verified);
-  // OneAtATimeStrategy.init (:27-48): external deliveries are never ignored
-  for (const demi_event& e : cur)
-    if (e.kind == DEMI_EV_MSG_EVENT && demi_type_is_external(ext_mask, e.type)) strat.tried[key_of(e)]++;
-  for (auto& kv : strat.tried) out->unignorable += kv.second;
-  bool triggered = false;                                             // violationTriggered (ScheduleCheckers.scala:48)
-  uint32_t last_size = 0;
-  for (const demi_event& e : cur) last_size += e.kind == DEMI_EV_MSG_EVENT;
-  out->deliveries_before = last_size;
-  std::vector<uint32_t> sizes;
+  demi::IntMinDriver d;
+  d.init(h->trace_host.data(), (uint32_t)h->trace_host.size(), demi_ext_type_mask(h), use_fifo, out);
   std::vector<demi_event> rec(65536);
-
   for (;;) {
-    // The candidate list getNextTrace would produce on this base trace if every test failed (:57-124)
-    std::vector<uint32_t> cand;
-    {
-      Strategy spec = strat;
-      bool t = triggered;
-      for (;;) {
-        const int found = spec.next(cur, pruned, t);
-        if (found < 0) break;
-        cand.push_back((uint32_t)found);
-        t = false;
-      }
-    }
+    const std::vector<uint32_t>& cand = d.candidates();
     if (cand.empty()) break;
     std::vector<demi_replay_result> res(cand.size());
     int32_t rc = demi_replay_batch_ex(h, nullptr, cand.data(), (uint32_t)cand.size(), mw, looking_for, flags, res.data());
     if (rc != DEMI_OK) return rc;
-    out->replays_executed += (uint32_t)cand.size();
-    out->batches++;
-    bool advanced = false;
-    for (size_t c = 0; c < cand.size(); c++) {
-      if (res[c].status) return fail(h, DEMI_ERR_CAPACITY, "demi_internal_minimize: a replay reported status %u", (unsigned)res[c].status);
-      out->total_replays++;                                           // stats.increment_replays
-      const int chosen = strat.next(cur, pruned, triggered);          // the real strategy takes the same step
-      if (chosen != (int)cand[c]) return fail(h, DEMI_ERR_STATE, "demi_internal_minimize: speculation diverged from the strategy");
-      triggered = res[c].violation != 0;
-      if (!res[c].violation) { sizes.push_back(last_size); continue; }   // "Ignoring didn't work."
-      // success: the trace STSSched recorded becomes lastFailingTrace (:57-91)
-      uint32_t n_rec = 0; demi_replay_result r1;
-      rc = demi_replay_trace(h, nullptr, mw, cand[c], looking_for, flags, rec.data(), (uint32_t)rec.size(), &n_rec, &r1);
-      if (rc != DEMI_OK) return rc;
-      if (r1.status || !r1.violation) return fail(h, DEMI_ERR_STATE, "demi_internal_minimize: recorded re-run disagrees with the batch");
-      MultiSet prior, fresh;
-      for (const demi_event& e : cur) if (e.kind == DEMI_EV_MSG_EVENT) prior[key_of(e)]++;
-      uint32_t new_size = 0;
-      for (uint32_t i = 0; i < n_rec; i++) if (rec[i].kind == DEMI_EV_MSG_EVENT) { fresh[key_of(rec[i])]++; new_size++; }
-      for (auto& kv : prior) {                                        // MultiSet.setDifference (schedulers/Util.scala:93-106)
-        uint32_t c2 = count_of(fresh, kv.first);
-        if (kv.second > c2) pruned[kv.first] += kv.second - c2;
-      }
-      cur.assign(rec.begin(), rec.begin() + n_rec);
-      last_size = new_size;
-      sizes.push_back(last_size);
-      rc = demi_set_trace(h, cur.data(), (uint32_t)cur.size(), ext.data(), (uint32_t)ext.size());
-      if (rc != DEMI_OK) return rc;
-      advanced = true;
-      break;
-    }
-    if (!advanced) break;          // every remaining candidate was tried and failed
+    uint32_t skip = 0;
+    const demi::IntMinDriver::Step step = d.commit(res.data(), &skip);
+    if (step == demi::IntMinDriver::FAILED) return fail(h, d.error, "%s", d.msg.c_str());
+    if (step == demi::IntMinDriver::DONE) break;
+    uint32_t n_rec = 0; demi_replay_result r1;
+    rc = demi_replay_trace(h, nullptr, mw, skip, looking_for, flags, rec.data(), (uint32_t)rec.size(), &n_rec, &r1);
+    if (rc != DEMI_OK) return rc;
+    if (!d.advance(r1, rec.data(), n_rec)) return fail(h, d.error, "%s", d.msg.c_str());
+    rc = demi_set_trace(h, d.cur.data(), (uint32_t)d.cur.size(), ext.data(), (uint32_t)ext.size());
+    if (rc != DEMI_OK) return rc;
   }
-  out->n_events = (uint32_t)cur.size();
-  out->deliveries_after = last_size;
-  out->n_internal_sizes = (uint32_t)sizes.size();
-  if (out_trace) std::copy(cur.begin(), cur.begin() + std::min<size_t>(cur.size(), cap_events), out_trace);
-  if (internal_sizes) for (uint32_t i = 0; i < cap_sizes && i < sizes.size(); i++) internal_sizes[i] = sizes[i];
+  d.finish(out_trace, cap_events, internal_sizes, cap_sizes);
   return DEMI_OK;
 }

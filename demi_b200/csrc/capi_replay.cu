@@ -19,10 +19,10 @@ using namespace demi;
 namespace {
 typedef void (*replay_fn)(const ReplayArgs);
 typedef void (*replay_many_fn)(const ReplayArgs, const ReplayTraceView*, const uint4*, uint32_t, ReplayArgs*);
-// K2 per model: the four instantiations of replay_lane_kernel, fn[WILD][REC], and replay_many_kernel, at the model's
-// block size and shared memory.  Every K2 instantiation is in this unit, so that its copy of model_ir.cuh's loaded model
-// is the one K2 reads.
-struct ReplayVariant { int model; int bd; replay_fn fn[2][2]; replay_many_fn many; size_t smem; int n_actors; };
+// K2 per model: the four instantiations of replay_lane_kernel, fn[WILD][REC], and replay_many_kernel, many[REC], at the
+// model's block size and shared memory.  Every K2 instantiation is in this unit, so that its copy of model_ir.cuh's
+// loaded model is the one K2 reads.
+struct ReplayVariant { int model; int bd; replay_fn fn[2][2]; replay_many_fn many[2]; size_t smem; int n_actors; };
 template <class MODEL>
 ReplayVariant make_rv() {
   constexpr int BD = replay_block<MODEL>;
@@ -30,7 +30,8 @@ ReplayVariant make_rv() {
   return ReplayVariant{MODEL::ID, BD,
                        {{replay_lane_kernel<MODEL, BD, false, false>, replay_lane_kernel<MODEL, BD, true, false>},
                         {replay_lane_kernel<MODEL, BD, false, true>, replay_lane_kernel<MODEL, BD, true, true>}},
-                       replay_many_kernel<MODEL, BD>, (size_t)M::WORDS * BD * sizeof(uint32_t), MODEL::N_ACTORS};
+                       {replay_many_kernel<MODEL, BD, false>, replay_many_kernel<MODEL, BD, true>},
+                       (size_t)M::WORDS * BD * sizeof(uint32_t), MODEL::N_ACTORS};
 }
 const ReplayVariant* pick_rv(int model) {
   static const std::vector<ReplayVariant> v = {make_rv<PingPong3>(), make_rv<Raft5>(), make_rv<Bcast32>(), make_rv<IrModel>()};
@@ -155,7 +156,8 @@ cudaError_t replay_ir_bind(const demi_handle* h, cudaStream_t s) {
 // its first generation and its counters, all in a.  Generation stamps: each launch gets a fresh range [gen_base,
 // gen_base + tests per thread]; the table is cleared only when it was (re)allocated, its geometry changed, or the
 // 16-bit range is exhausted.  A list leaves its entries behind, so the launch after it clears the table
-// (rp_gen_next = 0); a recording clears it first too, a wildcard list needs no clearing of its own.
+// (rp_gen_next = 0); a single recording clears it first too.  A wildcard list and the recordings of a multi-trace
+// launch need no clearing of their own: a test reads only the entries it wrote.
 int32_t replay_scratch(demi_handle* h, ReplayArgs& a, uint64_t warps, int n_actors, uint32_t per_thread, TableUse use,
                        cudaStream_t s) {
   int32_t rc;
@@ -192,7 +194,7 @@ int32_t replay_launch(demi_handle* h, ReplayArgs& a, bool wild, bool record, con
   if (!rv) return fail(h, DEMI_ERR_INVALID, "no replay kernel for model %d", h->cfg.model);
   int32_t rc;
   int bps = 0;
-  const void* fn = many ? (const void*)rv->many : (const void*)rv->fn[wild][record];
+  const void* fn = many ? (const void*)rv->many[record] : (const void*)rv->fn[wild][record];
   if ((rc = demi_occupancy(h, fn, rv->bd, rv->smem, &bps)) != DEMI_OK) return rc;
   if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
   // a block takes a test per thread of the single-trace kernel, a tile per warp of the multi-trace one; a recording
@@ -205,12 +207,12 @@ int32_t replay_launch(demi_handle* h, ReplayArgs& a, bool wild, bool record, con
   const int grid = (int)std::max<uint64_t>(1, blocks);
   const uint64_t warps = (uint64_t)grid * wpb;
   const uint32_t per_thread = (uint32_t)((items + (uint64_t)grid * per_block - 1) / ((uint64_t)grid * per_block)) + 1;
-  const TableUse use = wild ? TableUse::LIST : record ? TableUse::RECORD : TableUse::GENERATIONS;
+  const TableUse use = wild || (record && many) ? TableUse::LIST : record ? TableUse::RECORD : TableUse::GENERATIONS;
   if ((rc = replay_scratch(h, a, warps, rv->n_actors, per_thread, use, s)) != DEMI_OK) return rc;
   if (many && (rc = h->rp_bound.grow(h, warps * sizeof(ReplayArgs))) != DEMI_OK) return rc;
   CUDA_TRY(h, replay_ir_bind(h, s));
   if (timed) CUDA_TRY(h, cudaEventRecord(h->ev0, s));
-  if (many) rv->many<<<grid, rv->bd, rv->smem, s>>>(a, many->views, many->tiles, many->n_tiles, h->rp_bound.get<ReplayArgs>());
+  if (many) rv->many[record]<<<grid, rv->bd, rv->smem, s>>>(a, many->views, many->tiles, many->n_tiles, h->rp_bound.get<ReplayArgs>());
   else rv->fn[wild][record]<<<grid, rv->bd, rv->smem, s>>>(a);
   CUDA_TRY(h, cudaGetLastError());
   if (timed) CUDA_TRY(h, cudaEventRecord(h->ev1, s));

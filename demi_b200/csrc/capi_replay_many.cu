@@ -6,8 +6,12 @@
 // with a rendezvous: every driver in flight runs until it asks for an evaluation or finishes, then one launch evaluates
 // the union of their requests and each gets its own slice back.  A driver sees exactly the answers it would get alone,
 // so its decisions, MCS and counters do not depend on which other drivers share its launches.
+//
+// Internal minimization over a set runs the same way without threads: its driver (intmin_driver.hpp) is not recursive,
+// so every trace's driver steps in lock-step rounds of one exact launch and one recording launch.
 #include <atomic>
 #include <condition_variable>
+#include <functional>
 #include <mutex>
 #include <new>
 #include <system_error>
@@ -15,6 +19,7 @@
 #include "replay_kernel.cuh"
 #include "engine.hpp"
 #include "ddmin_driver.hpp"
+#include "intmin_driver.hpp"
 
 using namespace demi;
 
@@ -22,23 +27,40 @@ namespace {
 
 // tests per launch: larger unions are evaluated in several launches
 constexpr uint32_t MANY_MAX_TESTS = 1u << 20;
+// a recording launch's rows (tests x cap_events events) stay under this many bytes
+constexpr uint64_t MANY_MAX_REC_BYTES = 1ull << 30;
 // host threads demi_ddmin_many may run at once
 constexpr uint32_t MANY_MAX_WINDOW = 4096;
 
 struct LaunchCounts { uint32_t launches = 0; uint64_t tests = 0, violations = 0, deliveries = 0; double ms = 0; };
 
-// One K2 launch over tests [0, n) of the set: test i replays mask i on trace trace_of_test[i] (validated by the
-// caller).  Tests are grouped by trace into warp tiles, longest trace first; results come back in input order.
-int32_t launch_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks, uint32_t n, uint32_t mw,
-                    const uint32_t* looking_for, uint32_t flags, demi_replay_result* out, LaunchCounts& lc) {
-  const auto& S = h->set;
+// The traces a multi-trace launch reads: the set's, or the working traces of demi_internal_minimize_many
+struct Views {
+  const std::vector<ReplayTraceView>* host; const ReplayTraceView* dev;
+  static Views of(const demi_handle::TraceSet& S) { return Views{&S.view, S.views.get<const ReplayTraceView>()}; }
+};
+// A recording launch (the REC kernel): each test's EventTrace, at most `cap` events, is handed to take(test, events,
+// count) in input order once the launch is done
+struct Recording {
+  uint32_t cap;
+  std::function<void(uint32_t, const demi_event*, uint32_t)> take;
+};
+
+// One K2 launch over tests [0, n): test i replays mask i (every external when masks is null) on trace trace_of_test[i]
+// (validated by the caller), leaving out trace event skips[i] (none when skips is null or it is 0xFFFFFFFF).  Tests
+// are grouped by trace into warp tiles, longest trace first; results come back in input order.
+int32_t launch_many(demi_handle* h, const Views& V, const uint32_t* trace_of_test, const uint64_t* masks,
+                    const uint32_t* skips, uint32_t n, uint32_t mw, const uint32_t* looking_for, uint32_t flags,
+                    demi_replay_result* out, LaunchCounts& lc, const Recording* rec) {
+  const std::vector<ReplayTraceView>& view = *V.host;
+  const uint32_t n_traces = (uint32_t)view.size();
   // counting sort of the tests by the rank of their trace (longer traces first, then by index)
-  std::vector<uint32_t> count(S.n + 1, 0);
+  std::vector<uint32_t> count(n_traces + 1, 0);
   for (uint32_t i = 0; i < n; i++) count[trace_of_test[i]]++;
   std::vector<uint32_t> order_t;
-  for (uint32_t t = 0; t < S.n; t++) if (count[t]) order_t.push_back(t);
-  std::stable_sort(order_t.begin(), order_t.end(), [&](uint32_t a, uint32_t b) { return S.view[a].n_events > S.view[b].n_events; });
-  std::vector<uint32_t> first(S.n, 0);
+  for (uint32_t t = 0; t < n_traces; t++) if (count[t]) order_t.push_back(t);
+  std::stable_sort(order_t.begin(), order_t.end(), [&](uint32_t a, uint32_t b) { return view[a].n_events > view[b].n_events; });
+  std::vector<uint32_t> first(n_traces, 0);
   std::vector<uint4> tiles;
   ReplayTraceView geometry{};                       // the scratch's: the largest of the launch's traces
   uint32_t pos = 0;
@@ -46,40 +68,62 @@ int32_t launch_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_
     first[t] = pos;
     for (uint32_t k = 0; k < count[t]; k += 32) tiles.push_back(make_uint4(t, pos + k, std::min(32u, count[t] - k), looking_for[t]));
     pos += count[t];
-    const ReplayTraceView& v = S.view[t];
+    const ReplayTraceView& v = view[t];
     geometry.table_slots = std::max(geometry.table_slots, v.table_slots);
     geometry.tosend_cap = std::max(geometry.tosend_cap, v.tosend_cap);
     geometry.n_uniq_words = std::max(geometry.n_uniq_words, v.n_uniq_words);
     geometry.pending_cap = std::max(geometry.pending_cap, v.pending_cap);
   }
   std::vector<uint32_t> slot(n);                    // test i runs at position slot[i] of the grouped order
-  std::vector<uint64_t> grouped((size_t)n * mw);
+  std::vector<uint64_t> grouped(masks ? (size_t)n * mw : 0);
+  std::vector<uint32_t> grouped_skips(skips ? n : 0);
   for (uint32_t i = 0; i < n; i++) {
     slot[i] = first[trace_of_test[i]]++;
-    std::copy(masks + (size_t)i * mw, masks + (size_t)(i + 1) * mw, grouped.begin() + (size_t)slot[i] * mw);
+    if (masks) std::copy(masks + (size_t)i * mw, masks + (size_t)(i + 1) * mw, grouped.begin() + (size_t)slot[i] * mw);
+    if (skips) grouped_skips[slot[i]] = skips[i];
   }
   cudaStream_t s = h->stream;
   int32_t rc;
   const size_t mbytes = grouped.size() * sizeof(uint64_t), tbytes = tiles.size() * sizeof(uint4);
+  const size_t sbytes = grouped_skips.size() * sizeof(uint32_t);
   const size_t rbytes = (size_t)n * sizeof(demi_replay_result);
-  if ((rc = h->rp_masks.grow(h, mbytes + tbytes)) != DEMI_OK) return rc;
+  if ((rc = h->rp_masks.grow(h, tbytes + mbytes + sbytes)) != DEMI_OK) return rc;
   if ((rc = h->rp_results.grow(h, rbytes)) != DEMI_OK) return rc;
   char* base = h->rp_masks.get<char>();
   CUDA_TRY(h, cudaMemcpyAsync(base, tiles.data(), tbytes, cudaMemcpyHostToDevice, s));
-  CUDA_TRY(h, cudaMemcpyAsync(base + tbytes, grouped.data(), mbytes, cudaMemcpyHostToDevice, s));
+  if (masks) CUDA_TRY(h, cudaMemcpyAsync(base + tbytes, grouped.data(), mbytes, cudaMemcpyHostToDevice, s));
+  if (skips) CUDA_TRY(h, cudaMemcpyAsync(base + tbytes + mbytes, grouped_skips.data(), sbytes, cudaMemcpyHostToDevice, s));
   ReplayArgs a = replay_args(h, geometry, 0, flags);
-  a.masks = (const uint64_t*)(base + tbytes); a.n_masks = n; a.mask_words = mw;
+  a.masks = masks ? (const uint64_t*)(base + tbytes) : nullptr; a.n_masks = n; a.mask_words = mw;
+  a.skips = skips ? (const uint32_t*)(base + tbytes + mbytes) : nullptr;
   a.results = h->rp_results.get<demi_replay_result>();
-  const ReplayTiles many{S.views.get<ReplayTraceView>(), (const uint4*)base, (uint32_t)tiles.size()};
-  if ((rc = replay_launch(h, a, false, false, &many, true, s)) != DEMI_OK) return rc;
+  const size_t row_bytes = rec ? (size_t)rec->cap * sizeof(demi_event) : 0;
+  if (rec) {                                        // rows, then one count per test
+    if ((rc = h->rp_rec.grow(h, n * row_bytes + (size_t)n * sizeof(uint32_t))) != DEMI_OK) return rc;
+    a.rec_events = h->rp_rec.get<demi_event>(); a.rec_cap = rec->cap;
+    a.rec_count = (uint32_t*)(h->rp_rec.get<char>() + n * row_bytes);
+  }
+  const ReplayTiles many{V.dev, (const uint4*)base, (uint32_t)tiles.size()};
+  if ((rc = replay_launch(h, a, false, rec != nullptr, &many, true, s)) != DEMI_OK) return rc;
   std::vector<demi_replay_result> res(n);
+  std::vector<uint32_t> rec_count(rec ? n : 0);
   unsigned long long c[2] = {0, 0};
   CUDA_TRY(h, cudaMemcpyAsync(res.data(), a.results, rbytes, cudaMemcpyDeviceToHost, s));
   CUDA_TRY(h, cudaMemcpyAsync(c, a.counters, sizeof(c), cudaMemcpyDeviceToHost, s));
+  if (rec) CUDA_TRY(h, cudaMemcpyAsync(rec_count.data(), a.rec_count, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   CUDA_TRY(h, cudaStreamSynchronize(s));
   float ms = 0;
   CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
   for (uint32_t i = 0; i < n; i++) out[i] = res[slot[i]];
+  if (rec) {
+    // the rows as far as the longest recording of the launch reaches, in one strided copy
+    const uint32_t width = std::min(rec->cap, *std::max_element(rec_count.begin(), rec_count.end()));
+    std::vector<demi_event> rows((size_t)n * width);
+    if (width)
+      CUDA_TRY(h, cudaMemcpy2D(rows.data(), width * sizeof(demi_event), a.rec_events, row_bytes, width * sizeof(demi_event), n,
+                               cudaMemcpyDeviceToHost));
+    for (uint32_t i = 0; i < n; i++) rec->take(i, rows.data() + (size_t)slot[i] * width, rec_count[slot[i]]);
+  }
   lc.launches++; lc.tests += n; lc.ms += ms; lc.violations += c[0]; lc.deliveries += c[1];
   return DEMI_OK;
 }
@@ -89,12 +133,18 @@ void set_perf(demi_handle* h, const LaunchCounts& lc) {
   h->perf.violations = lc.violations; h->perf.deliveries = lc.deliveries;
 }
 
-// n tests in launches of at most MANY_MAX_TESTS
-int32_t replay_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks, uint32_t n, uint32_t mw,
-                    const uint32_t* looking_for, uint32_t flags, demi_replay_result* out, LaunchCounts& lc) {
-  for (uint32_t off = 0; off < n; off += MANY_MAX_TESTS) {
-    const uint32_t m = std::min(MANY_MAX_TESTS, n - off);
-    const int32_t rc = launch_many(h, trace_of_test + off, masks + (size_t)off * mw, m, mw, looking_for, flags, out + off, lc);
+// n tests in launches of at most MANY_MAX_TESTS (and, recording, of at most MANY_MAX_REC_BYTES of rows)
+int32_t replay_many(demi_handle* h, const Views& V, const uint32_t* trace_of_test, const uint64_t* masks,
+                    const uint32_t* skips, uint32_t n, uint32_t mw, const uint32_t* looking_for, uint32_t flags,
+                    demi_replay_result* out, LaunchCounts& lc, const Recording* rec = nullptr) {
+  uint32_t per_launch = MANY_MAX_TESTS;
+  if (rec) per_launch = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(per_launch, MANY_MAX_REC_BYTES / ((uint64_t)rec->cap * sizeof(demi_event))));
+  for (uint32_t off = 0; off < n; off += per_launch) {
+    const uint32_t m = std::min(per_launch, n - off);
+    Recording part;
+    if (rec) part = Recording{rec->cap, [&](uint32_t i, const demi_event* ev, uint32_t k) { rec->take(off + i, ev, k); }};
+    const int32_t rc = launch_many(h, V, trace_of_test + off, masks ? masks + (size_t)off * mw : nullptr,
+                                   skips ? skips + off : nullptr, m, mw, looking_for, flags, out + off, lc, rec ? &part : nullptr);
     if (rc != DEMI_OK) return rc;
   }
   return DEMI_OK;
@@ -204,7 +254,7 @@ extern "C" int32_t demi_replay_batch_many(demi_handle* h, const uint32_t* trace_
   if (n_tests == 0) return DEMI_OK;
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   LaunchCounts lc;
-  const int32_t rc = replay_many(h, trace_of_test, masks, n_tests, mask_words, looking_for, flags, out, lc);
+  const int32_t rc = replay_many(h, Views::of(h->set), trace_of_test, masks, nullptr, n_tests, mask_words, looking_for, flags, out, lc);
   set_perf(h, lc);
   return rc;
 }
@@ -292,7 +342,8 @@ extern "C" int32_t demi_ddmin_many(demi_handle* h, const uint32_t* looking_for, 
       }
       int32_t rc = call_rc;
       if (rc == DEMI_OK) {
-        rc = replay_many(h, tr.data(), flat.data(), (uint32_t)total, mask_words, looking_for, flags, res.data(), lc);
+        rc = replay_many(h, Views::of(h->set), tr.data(), flat.data(), nullptr, (uint32_t)total, mask_words, looking_for, flags,
+                         res.data(), lc);
         if (rc != DEMI_OK) { call_rc = rc; call_msg = h->err; }
       }
       k = 0;
@@ -310,6 +361,158 @@ extern "C" int32_t demi_ddmin_many(demi_handle* h, const uint32_t* looking_for, 
   for (std::thread& th : threads) th.join();
   set_perf(h, lc);
   if (call_rc != DEMI_OK) { h->err = call_msg; return call_rc; }
+  for (uint32_t t = 0; t < n; t++)
+    if (status[t] != DEMI_OK) { h->err = msg[t]; break; }
+  return DEMI_OK;
+}
+
+extern "C" int32_t demi_replay_traces_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks,
+                                           const uint32_t* skip_events, uint32_t n_tests, uint32_t mask_words,
+                                           const uint32_t* looking_for, uint32_t flags,
+                                           demi_event* events, uint32_t cap_events, uint32_t* n_events,
+                                           demi_replay_result* results) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!trace_of_test || !looking_for || !events || !cap_events || !n_events || !results)
+    return fail(h, DEMI_ERR_INVALID, "demi_replay_traces_many: null buffer");
+  if (!h->set.n) return fail(h, DEMI_ERR_STATE, "demi_set_traces has not been called");
+  for (uint32_t i = 0; i < n_tests; i++) {
+    const uint32_t t = trace_of_test[i];
+    if (t >= h->set.n) return fail(h, DEMI_ERR_INVALID, "demi_replay_traces_many: test %u names trace %u of %u", i, t, h->set.n);
+    if (masks && (uint64_t)mask_words * 64 < h->set.ext[t].size())
+      return fail(h, DEMI_ERR_INVALID, "mask_words %u too small for the %zu externals of trace %u", mask_words, h->set.ext[t].size(), t);
+  }
+  if (n_tests == 0) return DEMI_OK;
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  LaunchCounts lc;
+  const Recording rec{cap_events, [&](uint32_t i, const demi_event* ev, uint32_t k) {
+    n_events[i] = k;
+    std::copy(ev, ev + k, events + (size_t)i * cap_events);
+  }};
+  const int32_t rc = replay_many(h, Views::of(h->set), trace_of_test, masks, skip_events, n_tests, mask_words, looking_for,
+                                 flags, results, lc, &rec);
+  set_perf(h, lc);
+  return rc;
+}
+
+extern "C" int32_t demi_internal_minimize_many(demi_handle* h, const uint32_t* looking_for, uint32_t flags,
+                                               demi_event* out_traces, uint32_t cap_events,
+                                               uint32_t* internal_sizes, uint32_t cap_sizes,
+                                               demi_intmin_out* out, int32_t* status) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!looking_for || !out_traces || !cap_events || !out || !status)
+    return fail(h, DEMI_ERR_INVALID, "demi_internal_minimize_many: null buffer");
+  const demi_handle::TraceSet& S = h->set;
+  const uint32_t n = S.n;
+  if (!n) return fail(h, DEMI_ERR_STATE, "demi_set_traces has not been called");
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  const bool use_fifo = (flags & DEMI_IM_SRC_DST_FIFO) != 0;
+  flags &= ~DEMI_IM_SRC_DST_FIFO;
+  // the set's traces, read back once; the set itself is left as it is
+  std::vector<demi_event> all(S.events.bytes() / sizeof(demi_event));
+  if (!all.empty()) CUDA_TRY(h, cudaMemcpy(all.data(), S.events.get(), all.size() * sizeof(demi_event), cudaMemcpyDeviceToHost));
+  std::vector<demi::IntMinDriver> d(n);
+  for (uint32_t t = 0; t < n; t++) {
+    const demi_event* ev = all.data() + (S.view[t].events - S.events.get<const uint4>());
+    d[t].init(ev, S.view[t].n_events, demi_ext_type_mask(h), use_fifo, out + t);
+    status[t] = DEMI_OK;
+  }
+  // The working traces: a view table of their own.  A trace that advances gets its recorded trace and ordinals in the
+  // round's upload; its externals and their Send index stay the set's.
+  std::vector<ReplayTraceView> work = S.view;
+  DevBuf work_dev;
+  std::vector<DevBuf> rounds;                        // every round's new traces (a view may point into any of them)
+  std::vector<std::string> msg(n);
+  std::vector<uint8_t> live(n, 1);
+  auto fail_trace = [&](uint32_t t, int32_t code, const std::string& m) { status[t] = code; msg[t] = m; live[t] = 0; };
+  LaunchCounts lc;
+  int32_t rc;
+  for (;;) {
+    // 1. every unfinished driver's candidates
+    std::vector<uint32_t> tr, skip, first(n, 0);
+    for (uint32_t t = 0; t < n; t++) {
+      if (!live[t]) continue;
+      const std::vector<uint32_t>& cand = d[t].candidates();
+      if (cand.empty()) { live[t] = 0; continue; }
+      first[t] = (uint32_t)tr.size();
+      tr.insert(tr.end(), cand.size(), t);
+      skip.insert(skip.end(), cand.begin(), cand.end());
+    }
+    if (tr.empty()) break;
+    // 2. their union in one exact launch; 3. each driver commits
+    std::vector<demi_replay_result> res(tr.size());
+    const Views V{&work, work_dev.bytes() ? work_dev.get<const ReplayTraceView>() : S.views.get<const ReplayTraceView>()};
+    if ((rc = replay_many(h, V, tr.data(), nullptr, skip.data(), (uint32_t)tr.size(), 1, looking_for, flags, res.data(), lc)) != DEMI_OK)
+      break;
+    std::vector<uint32_t> rec_tr, rec_skip;
+    for (uint32_t t = 0; t < n; t++) {
+      if (!live[t]) continue;
+      uint32_t s = 0;
+      const demi::IntMinDriver::Step step = d[t].commit(res.data() + first[t], &s);
+      if (step == demi::IntMinDriver::FAILED) fail_trace(t, d[t].error, d[t].msg);
+      else if (step == demi::IntMinDriver::DONE) live[t] = 0;
+      else { rec_tr.push_back(t); rec_skip.push_back(s); }
+    }
+    if (rec_tr.empty()) continue;
+    // 4. every success re-run in one recording launch; the recorded trace advances its driver
+    std::vector<demi_replay_result> rres(rec_tr.size());
+    std::vector<uint32_t> advanced;
+    const Recording rec{cap_events, [&](uint32_t i, const demi_event* ev, uint32_t k) {
+      const uint32_t t = rec_tr[i];
+      if (rres[i].status == DEMI_PS_EVENT_OVF)
+        return fail_trace(t, DEMI_ERR_CAPACITY, "demi_internal_minimize_many: trace " + std::to_string(t) +
+                                                " needs a recording longer than cap_events " + std::to_string(cap_events));
+      if (!d[t].advance(rres[i], ev, k)) return fail_trace(t, d[t].error, d[t].msg);
+      advanced.push_back(t);
+    }};
+    if ((rc = replay_many(h, V, rec_tr.data(), nullptr, rec_skip.data(), (uint32_t)rec_tr.size(), 1, looking_for, flags,
+                          rres.data(), lc, &rec)) != DEMI_OK)
+      break;
+    // 5. the advanced traces' side tables on the host, their records in one upload, the view table in another
+    std::vector<demi_event> ev_all; std::vector<uint16_t> ord_all;
+    std::vector<size_t> off;
+    TraceTables tt;
+    char who[80];
+    for (uint32_t t : advanced) {
+      const std::vector<demi_event>& cur = d[t].cur;
+      snprintf(who, sizeof(who), "demi_internal_minimize_many: trace %u", t);
+      if ((rc = trace_tables(h, who, cur.data(), (uint32_t)cur.size(), S.ext[t].data(), (uint32_t)S.ext[t].size(), tt)) != DEMI_OK) {
+        fail_trace(t, rc, h->err);
+        off.push_back(SIZE_MAX);
+        continue;
+      }
+      off.push_back(ev_all.size());
+      ev_all.insert(ev_all.end(), cur.begin(), cur.end());
+      ord_all.insert(ord_all.end(), tt.ordinal.begin(), tt.ordinal.end());
+      const ReplayTraceView v = trace_view(tt, (uint32_t)cur.size(), (uint32_t)S.ext[t].size());
+      ReplayTraceView& w = work[t];
+      w.n_events = v.n_events; w.n_uniq_words = v.n_uniq_words;
+      w.pending_cap = v.pending_cap; w.tosend_cap = v.tosend_cap; w.table_slots = v.table_slots;
+    }
+    rc = DEMI_OK;
+    if (ev_all.empty()) continue;
+    const size_t ev_bytes = ev_all.size() * sizeof(demi_event);
+    rounds.emplace_back();
+    DevBuf& b = rounds.back();
+    if ((rc = b.grow(h, ev_bytes + ord_all.size() * sizeof(uint16_t))) != DEMI_OK) break;
+    CUDA_TRY(h, cudaMemcpyAsync(b.get(), ev_all.data(), ev_bytes, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(b.get<char>() + ev_bytes, ord_all.data(), ord_all.size() * sizeof(uint16_t),
+                                cudaMemcpyHostToDevice, h->stream));
+    for (size_t k = 0; k < advanced.size(); k++) {
+      if (off[k] == SIZE_MAX) continue;
+      ReplayTraceView& w = work[advanced[k]];
+      w.events = b.get<const uint4>() + off[k];
+      w.ev_ordinal = (const uint16_t*)(b.get<char>() + ev_bytes) + off[k];
+    }
+    if ((rc = work_dev.grow(h, work.size() * sizeof(ReplayTraceView))) != DEMI_OK) break;
+    CUDA_TRY(h, cudaMemcpyAsync(work_dev.get(), work.data(), work.size() * sizeof(ReplayTraceView), cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));    // the host vectors go out of scope
+  }
+  set_perf(h, lc);
+  if (rc != DEMI_OK) return rc;
+  for (uint32_t t = 0; t < n; t++)
+    if (status[t] == DEMI_OK)
+      d[t].finish(out_traces + (size_t)t * cap_events, cap_events, internal_sizes ? internal_sizes + (size_t)t * cap_sizes : nullptr,
+                  cap_sizes);
   for (uint32_t t = 0; t < n; t++)
     if (status[t] != DEMI_OK) { h->err = msg[t]; break; }
   return DEMI_OK;

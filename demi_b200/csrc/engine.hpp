@@ -93,6 +93,7 @@ struct demi_handle {
   DevBuf rp_tosend, rp_pruned, rp_masks, rp_results;
   DevBuf rp_counters;                              // unsigned long long[2]
   DevBuf rp_bound;                                 // demi::ReplayArgs per warp of a multi-trace K2 launch
+  DevBuf rp_rec;                                   // a multi-trace recording launch's rows (demi_event), then counts
   // ---- the trace set (demi_set_traces, capi_replay_many.cu): independent of the single trace above
   struct TraceSet {
     uint32_t n = 0;
@@ -133,8 +134,8 @@ namespace demi { struct ReplayArgs; }
 demi::ReplayArgs replay_args(const demi_handle* h, const demi::ReplayTraceView& trace, uint32_t looking_for, uint32_t flags);
 // the multi-trace kernel's own arguments: the set's views and the launch's tiles (capi_replay_many.cu)
 struct ReplayTiles { const demi::ReplayTraceView* views; const uint4* tiles; uint32_t n_tiles; };
-// Every K2 launch: the WILD or exact, REC or batch single-trace kernel, or with `many` the multi-trace kernel, on a's
-// tests; the grid, the per-warp scratch, the generation range and the counters, the loaded model's binding.  `timed`
+// Every K2 launch: the WILD or exact, REC or batch single-trace kernel, or with `many` the exact or REC multi-trace
+// kernel, on a's tests; the grid, the per-warp scratch, the generation range and the counters, the loaded model's binding.  `timed`
 // records h->ev0 and h->ev1 around the kernel alone.
 int32_t replay_launch(demi_handle* h, demi::ReplayArgs& a, bool wild, bool record, const ReplayTiles* many, bool timed,
                       cudaStream_t s);

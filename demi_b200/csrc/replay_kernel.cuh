@@ -72,8 +72,13 @@ template <class MODEL> constexpr int replay_block = MODEL::N_ACTORS <= 8 ? 256 :
 
 // WILD: ClockClusterizer's wildcarded trace (capi_wildcard.cu).  The pending set is the insertion-ordered list of
 // the REC variant (Uniq order = list order), compacted in place when taken entries dominate it.
-template <class MODEL, int BD, bool REC = false, bool WILD = false>
-struct ReplayMachine : TimerTable<MODEL> {
+// ROWS (with REC): many recordings in one launch; test idx records into row idx of rec_events (rec_cap events each)
+// and its count into rec_count[idx].  The row pointer is a member of the machines that record rows only, so the
+// other instantiations keep their layout (a loaded model's machine lives in the stack frame).
+template <bool ROWS> struct RecRow { uint4* rec_row; };
+template <> struct RecRow<false> {};
+template <class MODEL, int BD, bool REC = false, bool WILD = false, bool ROWS = false>
+struct ReplayMachine : TimerTable<MODEL>, RecRow<ROWS> {
   using Model = MODEL;
   static constexpr int BLOCK = BD;
   static constexpr bool LIST = REC || WILD;
@@ -118,7 +123,9 @@ struct ReplayMachine : TimerTable<MODEL> {
                                            uint32_t p0, uint32_t p1, uint32_t uniq) {
     if (!REC) return;
     if (n_rec >= A->rec_cap) { status = DEMI_PS_EVENT_OVF; return; }
-    reinterpret_cast<uint4*>(A->rec_events)[n_rec++] = make_uint4(kind | (src << 8) | (dst << 16) | (type << 24), p0, p1, uniq);
+    uint4* row;                      // ROWS: this test's row (A is the warp's, the row the lane's own)
+    if constexpr (ROWS) row = this->rec_row; else row = reinterpret_cast<uint4*>(A->rec_events);
+    row[n_rec++] = make_uint4(kind | (src << 8) | (dst << 16) | (type << 24), p0, p1, uniq);
   }
 
   // ---- pending multiset
@@ -314,7 +321,8 @@ struct ReplayMachine : TimerTable<MODEL> {
     mask = A->masks ? A->masks + (size_t)test_idx * A->mask_words : nullptr;
     mword_idx = 0xFFFFFFFFu; mword = 0;
     const uint32_t skip = A->skips ? A->skips[test_idx] : 0xFFFFFFFFu;
-    n_rec = n_uniq = n_list = 0;
+    n_rec = n_uniq = n_list = 0;       // the list is rebuilt from its first entry: nothing of a previous test is read
+    if constexpr (ROWS) this->rec_row = reinterpret_cast<uint4*>(A->rec_events) + (size_t)test_idx * A->rec_cap;
     if constexpr (WILD) { wc_inc = A->wc_include + (size_t)test_idx * A->wc_words; list_lo = 0; n_ign = 0; }
     gen = generation;
     actor_init(*this);
@@ -434,7 +442,7 @@ struct ReplayMachine : TimerTable<MODEL> {
 #undef PF_ROW
     if (!status && !diverged) flush();                               // :682 before trace_finished
     out.violation = 0; out.delivered = 0; out.ignored = 0; out.state_hash = 0;
-    if (REC && A->rec_count) *A->rec_count = n_rec;
+    if (REC && A->rec_count) A->rec_count[ROWS ? test_idx : 0] = n_rec;
     if (WILD && REC && A->wc_ignored_count) *A->wc_ignored_count = n_ign;
     if (status) { out.status = (uint16_t)status; return; }
     if (diverged) { out.status = DEMI_RS_DIVERGED; out.delivered = (uint16_t)delivered; return; }
@@ -520,11 +528,13 @@ replay_lane_kernel(const __grid_constant__ ReplayArgs args) {
 // traces; each tile binds its trace's view into the warp's copy of it, bound[warp] in global memory.  The copy is in
 // neither registers (they would come out of the per-event loop's) nor shared memory (a block's copies would cost raft5
 // one of its four resident blocks per SM); its fields are read through L1.
-template <class MODEL, int BD>
+// REC: every test records the EventTrace STSScheduler.test returns into its own row (ROWS above): the row is a
+// member of the lane's machine, set from its test index, so the warp's copy of the arguments stays shared.
+template <class MODEL, int BD, bool REC = false>
 __global__ void __launch_bounds__(BD, (model_replay_direct<MODEL>::value && MODEL::N_ACTORS <= 8) ? 1024 / BD : 1)
 replay_many_kernel(const __grid_constant__ ReplayArgs args, const ReplayTraceView* __restrict__ views,
                    const uint4* __restrict__ tiles, uint32_t n_tiles, ReplayArgs* bound) {
-  using M = ReplayMachine<MODEL, BD>;
+  using M = ReplayMachine<MODEL, BD, REC, false, REC>;
   extern __shared__ __align__(16) uint32_t lane_smem[];
   const uint32_t tid = threadIdx.x;
   const uint64_t gwarp = ((uint64_t)blockIdx.x * BD + tid) >> 5;

@@ -348,6 +348,37 @@ class Engine(object):
                                             mw, iters.ctypes.data, cap_iterations, out.ctypes.data, status.ctypes.data))
         return mcs, iters, out, status
 
+    def replay_traces_many(self, trace_of_test, masks=None, skip_events=None, looking_for=(), flags=0, cap_events=4096,
+                           mask_words=None):
+        """demi_replay_traces_many: test i replays masks[i] (None: full externals) on trace trace_of_test[i], leaving
+        out trace event skip_events[i] (None: none), recording its EventTrace.  (events [n, cap_events], n_events [n],
+        REPLAY_DTYPE [n]); row i is valid up to n_events[i]."""
+        tr = np.ascontiguousarray(trace_of_test, dtype=np.uint32)
+        mw = mask_words or self.set_mask_words()
+        m = None if masks is None else np.ascontiguousarray(masks, dtype=np.uint64).reshape(-1, mw)
+        sk = None if skip_events is None else np.ascontiguousarray(skip_events, dtype=np.uint32)
+        lf = np.ascontiguousarray(looking_for, dtype=np.uint32)
+        ev = np.zeros((len(tr), cap_events), dtype=N.EVENT_DTYPE)
+        ne = np.zeros(len(tr), dtype=np.uint32)
+        res = np.zeros(len(tr), dtype=N.REPLAY_DTYPE)
+        self._check(N.lib().demi_replay_traces_many(self._h, tr.ctypes.data, None if m is None else m.ctypes.data,
+                                                    None if sk is None else sk.ctypes.data, len(tr), mw, lf.ctypes.data,
+                                                    flags, ev.ctypes.data, cap_events, ne.ctypes.data, res.ctypes.data))
+        return ev, ne, res
+
+    def internal_minimize_many(self, looking_for, flags=0, cap_events=4096, cap_sizes=1024):
+        """demi_internal_minimize_many over the set: (traces [n, cap_events], sizes [n, cap_sizes], INTMIN_OUT_DTYPE [n],
+        status [n]).  Trace t is traces[t, :out[t]['n_events']]; a trace whose status is not OK has no outputs."""
+        n = len(self._set_ext)
+        lf = np.ascontiguousarray(looking_for, dtype=np.uint32)
+        ev = np.zeros((n, cap_events), dtype=N.EVENT_DTYPE)
+        sizes = np.zeros((n, cap_sizes), dtype=np.uint32)
+        out = np.zeros(n, dtype=N.INTMIN_OUT_DTYPE)
+        status = np.zeros(n, dtype=np.int32)
+        self._check(N.lib().demi_internal_minimize_many(self._h, lf.ctypes.data, flags, ev.ctypes.data, cap_events,
+                                                        sizes.ctypes.data, cap_sizes, out.ctypes.data, status.ctypes.data))
+        return ev, sizes, out, status
+
     def last_error(self):
         return N.lib().demi_last_error(self._h).decode()
 

@@ -405,6 +405,33 @@ int32_t demi_replay_batch_many(demi_handle* h, const uint32_t* trace_of_test, co
 int32_t demi_ddmin_many(demi_handle* h, const uint32_t* looking_for, uint32_t flags, int32_t check_unmodified,
                         uint64_t* mcs_masks, uint32_t mask_words, uint32_t* iteration_sizes, uint32_t cap_iterations,
                         demi_ddmin_out* out, int32_t* status);
+/* n_tests STSScheduler.test calls over the set in recording mode, in one launch: test i replays mask i (mask_words
+ * words; masks NULL: the trace's full externals) on trace trace_of_test[i], leaving out trace event skip_events[i]
+ * (skip_events NULL or 0xFFFFFFFF: none), looking for looking_for[trace_of_test[i]].  Its EventTrace goes to
+ * events + i*cap_events, its count to n_events[i] and its result to results[i]: each record equals what
+ * demi_set_trace(trace t) then demi_replay_trace(mask i, skip i, looking_for[t], flags, cap_events) returns, a status of
+ * DEMI_PS_EVENT_OVF when the row is too short included.  Past n_events[i], row i is left as it was.  This is
+ * verify_mcs's recording (RunnerUtils.scala:689-701) and STSSchedMinimizer's re-run of a successful removal for many
+ * traces at once.  demi_perf counts the launches, the tests and their kernel time. */
+int32_t demi_replay_traces_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks,
+                                const uint32_t* skip_events, uint32_t n_tests, uint32_t mask_words,
+                                const uint32_t* looking_for, uint32_t flags,
+                                demi_event* events, uint32_t cap_events, uint32_t* n_events,
+                                demi_replay_result* results);
+/* demi_internal_minimize (RunnerUtils.minimizeInternals with STSSchedMinimizer) on every trace t of the set, each a
+ * verified MCS trace whose externals are its MCS, looking for looking_for[t]; flags as demi_internal_minimize's.  The
+ * minimizations step in lock-step rounds: one launch evaluates every trace's candidate removals, one launch records
+ * every trace's successful removal.  status[t] is what demi_set_trace(trace t) then demi_internal_minimize(h,
+ * looking_for[t], flags, ...) would return, and when it is DEMI_OK, out_traces[t*cap_events ..], internal_sizes
+ * [t*cap_sizes ..] (may be NULL) and out[t] equal that call's outputs, replays_executed and batches included.
+ * cap_events is also the capacity of each recording: a trace that needs a longer one fails alone with
+ * DEMI_ERR_CAPACITY.  The results do not depend on which other traces are in the set.  The set is left as it was.  The
+ * call fails only on invalid arguments, without a set (DEMI_ERR_STATE) or on a CUDA error; when some traces fail, it
+ * returns DEMI_OK and demi_last_error holds the message of the lowest-indexed one. */
+int32_t demi_internal_minimize_many(demi_handle* h, const uint32_t* looking_for, uint32_t flags,
+                                    demi_event* out_traces, uint32_t cap_events,
+                                    uint32_t* internal_sizes, uint32_t cap_sizes,
+                                    demi_intmin_out* out, int32_t* status);
 
 /* DDMin with a RandomScheduler as the TestOracle (RunnerUtils.randomDDMin, RunnerUtils.scala:601-623).  The dag is the
  * handle's program (demi_set_externals) with every event in it, WaitQuiescence included: DDMin.minimize wraps the

@@ -250,6 +250,48 @@ class Engine {
     }
     return r;
   }
+  // demi_replay_traces_many: the EventTrace of test i (trace trace_of_test[i], masks[i] of set_mask_words() words or the
+  // full externals when masks is empty, trace event skip_events[i] left out or none when skip_events is empty)
+  struct RecordedReplay { EventTrace trace; demi_replay_result result; };
+  std::vector<RecordedReplay> replay_traces_many(const std::vector<uint32_t>& trace_of_test, const std::vector<uint64_t>& masks,
+                                                 const std::vector<uint32_t>& skip_events,
+                                                 const std::vector<ViolationFingerprint>& looking_for, uint32_t flags = 0,
+                                                 uint32_t cap_events = 4096) {
+    const size_t n = trace_of_test.size();
+    std::vector<demi_event> ev(n * (size_t)cap_events);
+    std::vector<uint32_t> ne(n);
+    std::vector<demi_replay_result> res(n);
+    check(demi_replay_traces_many(h, trace_of_test.data(), masks.empty() ? nullptr : masks.data(),
+                                  skip_events.empty() ? nullptr : skip_events.data(), (uint32_t)n, set_mask_words(),
+                                  looking_for.data(), flags, ev.data(), cap_events, ne.data(), res.data()));
+    std::vector<RecordedReplay> r(n);
+    for (size_t i = 0; i < n; i++) {
+      r[i].result = res[i];
+      r[i].trace.assign(ev.begin() + i * cap_events, ev.begin() + i * cap_events + std::min(ne[i], cap_events));
+    }
+    return r;
+  }
+  // demi_internal_minimize_many: per trace of the set (a verified MCS trace), its minimized trace and record, or the
+  // error code
+  struct IntMinManyResult { EventTrace trace; std::vector<uint32_t> internal_sizes; demi_intmin_out out; int32_t status; };
+  std::vector<IntMinManyResult> internal_minimize_many(const std::vector<ViolationFingerprint>& looking_for, uint32_t flags = 0,
+                                                       uint32_t cap_events = 4096, uint32_t cap_sizes = 1024) {
+    const size_t n = set_ext.size();
+    std::vector<demi_event> ev(n * (size_t)cap_events);
+    std::vector<uint32_t> sizes(n * (size_t)cap_sizes);
+    std::vector<demi_intmin_out> out(n);
+    std::vector<int32_t> status(n);
+    check(demi_internal_minimize_many(h, looking_for.data(), flags, ev.data(), cap_events, sizes.data(), cap_sizes, out.data(),
+                                      status.data()));
+    std::vector<IntMinManyResult> r(n);
+    for (size_t t = 0; t < n; t++) {
+      r[t].out = out[t]; r[t].status = status[t];
+      if (status[t] != DEMI_OK) continue;
+      r[t].trace.assign(ev.begin() + t * cap_events, ev.begin() + t * cap_events + std::min(out[t].n_events, cap_events));
+      r[t].internal_sizes.assign(sizes.begin() + t * cap_sizes, sizes.begin() + t * cap_sizes + std::min(out[t].n_internal_sizes, cap_sizes));
+    }
+    return r;
+  }
   const SchedulerConfig cfg;
  private:
   demi_handle* h = nullptr;

@@ -231,6 +231,22 @@ JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_ddminMany(JNIE
                          (uint32_t)maskWords, iterationSizes ? (uint32_t*)BUF(env, iterationSizes) : 0, (uint32_t)capIterations,
                          (demi_ddmin_out*)BUF(env, out), (int32_t*)BUF(env, status));
 }
+/* demi_replay_traces_many / demi_internal_minimize_many: the verified MCS traces of the set recorded, and their internal
+ * events minimized, with their tests in shared launches */
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_replayTracesMany(JNIEnv* env, jclass c, jlong h, jobject traceOfTest,
+    jobject masks, jobject skipEvents, jint nTests, jint maskWords, jobject lookingFor, jint flags, jobject events, jint capEvents,
+    jobject nEvents, jobject results) {
+  return demi_replay_traces_many(H(h), (const uint32_t*)BUF(env, traceOfTest), masks ? (const uint64_t*)BUF(env, masks) : 0,
+                                 skipEvents ? (const uint32_t*)BUF(env, skipEvents) : 0, (uint32_t)nTests, (uint32_t)maskWords,
+                                 (const uint32_t*)BUF(env, lookingFor), (uint32_t)flags, (demi_event*)BUF(env, events),
+                                 (uint32_t)capEvents, (uint32_t*)BUF(env, nEvents), (demi_replay_result*)BUF(env, results));
+}
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_internalMinimizeMany(JNIEnv* env, jclass c, jlong h,
+    jobject lookingFor, jint flags, jobject traces, jint capEvents, jobject sizes, jint capSizes, jobject out, jobject status) {
+  return demi_internal_minimize_many(H(h), (const uint32_t*)BUF(env, lookingFor), (uint32_t)flags, (demi_event*)BUF(env, traces),
+                                     (uint32_t)capEvents, sizes ? (uint32_t*)BUF(env, sizes) : 0, (uint32_t)capSizes,
+                                     (demi_intmin_out*)BUF(env, out), (int32_t*)BUF(env, status));
+}
 /* `exp` = a direct buffer laid out as demi_experiment whose pointer fields the Scala side fills with
  * GetDirectBufferAddress-style addresses (DemiNative.addressOf) */
 JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_experimentSave(JNIEnv* env, jclass c, jstring dir, jobject exp) {

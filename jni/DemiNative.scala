@@ -87,6 +87,15 @@ object DemiNative {
   /** demi_ddmin_many: RunnerUtils.stsSchedDDMin on every trace of the set; status(t) is that trace's return code */
   @native def ddminMany(h: Long, lookingFor: ByteBuffer, flags: Int, checkUnmodified: Int, mcsMasks: ByteBuffer, maskWords: Int,
                         iterationSizes: ByteBuffer, capIterations: Int, out: ByteBuffer, status: ByteBuffer): Int
+  /** demi_replay_traces_many: test i replays mask i (null: full externals) on trace traceOfTest(i), leaving out trace event
+   *  skipEvents(i) (null: none), and records its EventTrace at events + i*capEvents (verify_mcs's recording) */
+  @native def replayTracesMany(h: Long, traceOfTest: ByteBuffer, masks: ByteBuffer, skipEvents: ByteBuffer, nTests: Int,
+                               maskWords: Int, lookingFor: ByteBuffer, flags: Int, events: ByteBuffer, capEvents: Int,
+                               nEvents: ByteBuffer, results: ByteBuffer): Int
+  /** demi_internal_minimize_many: RunnerUtils.minimizeInternals on every trace of the set (verified MCS traces); trace t
+   *  at traces + t*capEvents, status(t) its return code */
+  @native def internalMinimizeMany(h: Long, lookingFor: ByteBuffer, flags: Int, traces: ByteBuffer, capEvents: Int,
+                                   sizes: ByteBuffer, capSizes: Int, out: ByteBuffer, status: ByteBuffer): Int
   /** The flat experiment directory that replaces ExperimentSerializer's *.bin object streams (Serialization.scala:57-74). */
   @native def experimentSave(dir: String, exp: ByteBuffer): Int
   @native def experimentLoad(dir: String, exp: ByteBuffer): Int
