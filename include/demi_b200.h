@@ -270,7 +270,9 @@ int32_t demi_set_trace(demi_handle* h, const demi_event* events, uint32_t n_even
                        const demi_ext_event* externals, uint32_t n_externals);
 /* n_masks independent STSScheduler.test(subseq, fingerprint) calls.  Mask i is
  * `mask_words` uint64 words; bit j selects external event j of the trace's
- * original_externals.  looking_for = the ViolationFingerprint code (0 = any). */
+ * original_externals.  looking_for = the ViolationFingerprint code (0 = any).
+ * Mask padding, here and in every call over a set: bits at or past a trace's n_externals, up to the call's
+ * mask_words, are ignored on input, and an output mask (demi_ddmin, demi_ddmin_many's mcs_masks) has them zero. */
 int32_t demi_replay_batch(demi_handle* h, const uint64_t* masks, uint32_t n_masks, uint32_t mask_words,
                           uint32_t looking_for, uint32_t flags, demi_replay_result* out_host);
 int32_t demi_replay_batch_dev(demi_handle* h, const void* masks_dev, uint32_t n_masks, uint32_t mask_words,
@@ -389,14 +391,15 @@ int32_t demi_set_traces(demi_handle* h, uint32_t n_traces,
                         const demi_ext_event* externals, const uint32_t* ext_offsets, const uint32_t* n_externals);
 /* n_tests STSScheduler.test calls over the set: test i replays mask i (mask_words words) on trace trace_of_test[i],
  * looking for looking_for[trace_of_test[i]].  Record i equals demi_replay_batch's record for that mask with that trace
- * alone, for every flag.  demi_perf counts the launches, the tests and their kernel time. */
+ * alone, for every flag; bits of mask i at or past that trace's n_externals are ignored.  demi_perf counts the launches, the tests and their kernel time. */
 int32_t demi_replay_batch_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks, uint32_t n_tests,
                                uint32_t mask_words, const uint32_t* looking_for, uint32_t flags,
                                demi_replay_result* out);
 /* demi_ddmin on every trace t of the set, looking for looking_for[t]: status[t] is what demi_set_trace(trace t) then
  * demi_ddmin(h, looking_for[t], flags, check_unmodified, ...) would return, and when it is DEMI_OK, mcs_masks[t*mask_words
  * ..], iteration_sizes[t*cap_iterations ..] (may be NULL) and out[t] equal that call's outputs, replays_executed and
- * batches included (they count that trace's own speculative batches); out[t].reserved holds host microseconds.  The
+ * batches included (they count that trace's own speculative batches); out[t].reserved holds host microseconds.  Trace
+ * t's MCS mask has every bit at or past its n_externals zero, the words past its own width included.  The
  * minimisations of many traces run side by side and their tests share launches; the results do not depend on how the
  * traces are grouped.  The call fails only on invalid arguments, without a set (DEMI_ERR_STATE) or on a CUDA error; when
  * some traces fail, it returns DEMI_OK and demi_last_error holds the message of the lowest-indexed one.
@@ -407,7 +410,8 @@ int32_t demi_ddmin_many(demi_handle* h, const uint32_t* looking_for, uint32_t fl
                         demi_ddmin_out* out, int32_t* status);
 /* n_tests STSScheduler.test calls over the set in recording mode, in one launch: test i replays mask i (mask_words
  * words; masks NULL: the trace's full externals) on trace trace_of_test[i], leaving out trace event skip_events[i]
- * (skip_events NULL or 0xFFFFFFFF: none), looking for looking_for[trace_of_test[i]].  Its EventTrace goes to
+ * (skip_events NULL or 0xFFFFFFFF: none), looking for looking_for[trace_of_test[i]]; bits of mask i at or past that
+ * trace's n_externals are ignored.  Its EventTrace goes to
  * events + i*cap_events, its count to n_events[i] and its result to results[i]: each record equals what
  * demi_set_trace(trace t) then demi_replay_trace(mask i, skip i, looking_for[t], flags, cap_events) returns, a status of
  * DEMI_PS_EVENT_OVF when the row is too short included.  Past n_events[i], row i is left as it was.  This is
