@@ -133,7 +133,8 @@ EXPORTS = [
     "demi_set_fuzzer", "demi_fuzz_campaign", "demi_fuzz_campaign_dev",
     "demi_random_test_batch", "demi_random_ddmin", "demi_random_test_trace",
     "demi_fuzz_traces", "demi_set_traces", "demi_replay_batch_many", "demi_ddmin_many",
-    "demi_replay_traces_many", "demi_internal_minimize_many",
+    "demi_replay_traces_many", "demi_internal_minimize_many", "demi_wildcard_replay_batch_many",
+    "demi_wildcard_minimize_many",
 ]
 FILTER_RULE_DTYPE = np.dtype([("src_mask", "<u4"), ("dst_mask", "<u4"), ("type_mask", "<u4"), ("flags", "<u4")])
 FRULE_DEADLETTERS = 1
@@ -333,6 +334,10 @@ def lib():
     L.demi_replay_traces_many.argtypes = [vp, vp, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, vp]
     L.demi_internal_minimize_many.restype = C.c_int32
     L.demi_internal_minimize_many.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, vp]
+    L.demi_wildcard_replay_batch_many.restype = C.c_int32
+    L.demi_wildcard_replay_batch_many.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp]
+    L.demi_wildcard_minimize_many.restype = C.c_int32
+    L.demi_wildcard_minimize_many.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, vp]
     L.demi_stats.restype = C.c_int32
     L.demi_stats.argtypes = [vp, C.POINTER(Perf)]
     L.demi_lane_kernel.restype = C.c_int32

@@ -18,11 +18,12 @@ using namespace demi;
 
 namespace {
 typedef void (*replay_fn)(const ReplayArgs);
-typedef void (*replay_many_fn)(const ReplayArgs, const ReplayTraceView*, const uint4*, uint32_t, ReplayArgs*);
-// K2 per model: the four instantiations of replay_lane_kernel, fn[WILD][REC], and replay_many_kernel, many[REC], at the
+typedef void (*replay_many_fn)(const ReplayArgs, const ReplayTraceView*, const uint4*, uint32_t, ReplayArgs*,
+                               const uint32_t* const*);
+// K2 per model: the four instantiations of replay_lane_kernel, fn[WILD][REC], and of replay_many_kernel, many[WILD][REC], at the
 // model's block size and shared memory.  Every K2 instantiation is in this unit, so that its copy of model_ir.cuh's
 // loaded model is the one K2 reads.
-struct ReplayVariant { int model; int bd; replay_fn fn[2][2]; replay_many_fn many[2]; size_t smem; int n_actors; };
+struct ReplayVariant { int model; int bd; replay_fn fn[2][2]; replay_many_fn many[2][2]; size_t smem; int n_actors; };
 template <class MODEL>
 ReplayVariant make_rv() {
   constexpr int BD = replay_block<MODEL>;
@@ -30,7 +31,8 @@ ReplayVariant make_rv() {
   return ReplayVariant{MODEL::ID, BD,
                        {{replay_lane_kernel<MODEL, BD, false, false>, replay_lane_kernel<MODEL, BD, true, false>},
                         {replay_lane_kernel<MODEL, BD, false, true>, replay_lane_kernel<MODEL, BD, true, true>}},
-                       {replay_many_kernel<MODEL, BD, false>, replay_many_kernel<MODEL, BD, true>},
+                       {{replay_many_kernel<MODEL, BD, false, false>, replay_many_kernel<MODEL, BD, true, false>},
+                        {replay_many_kernel<MODEL, BD, false, true>, replay_many_kernel<MODEL, BD, true, true>}},
                        (size_t)M::WORDS * BD * sizeof(uint32_t), MODEL::N_ACTORS};
 }
 const ReplayVariant* pick_rv(int model) {
@@ -194,7 +196,7 @@ int32_t replay_launch(demi_handle* h, ReplayArgs& a, bool wild, bool record, con
   if (!rv) return fail(h, DEMI_ERR_INVALID, "no replay kernel for model %d", h->cfg.model);
   int32_t rc;
   int bps = 0;
-  const void* fn = many ? (const void*)rv->many[record] : (const void*)rv->fn[wild][record];
+  const void* fn = many ? (const void*)rv->many[wild][record] : (const void*)rv->fn[wild][record];
   if ((rc = demi_occupancy(h, fn, rv->bd, rv->smem, &bps)) != DEMI_OK) return rc;
   if (bps < 1) return fail(h, DEMI_ERR_CAPACITY, "replay kernel does not fit on an SM");
   // a block takes a test per thread of the single-trace kernel, a tile per warp of the multi-trace one; a recording
@@ -212,7 +214,9 @@ int32_t replay_launch(demi_handle* h, ReplayArgs& a, bool wild, bool record, con
   if (many && (rc = h->rp_bound.grow(h, warps * sizeof(ReplayArgs))) != DEMI_OK) return rc;
   CUDA_TRY(h, replay_ir_bind(h, s));
   if (timed) CUDA_TRY(h, cudaEventRecord(h->ev0, s));
-  if (many) rv->many[record]<<<grid, rv->bd, rv->smem, s>>>(a, many->views, many->tiles, many->n_tiles, h->rp_bound.get<ReplayArgs>());
+  if (many)
+    rv->many[wild][record]<<<grid, rv->bd, rv->smem, s>>>(a, many->views, many->tiles, many->n_tiles, h->rp_bound.get<ReplayArgs>(),
+                                                          many->modes);
   else rv->fn[wild][record]<<<grid, rv->bd, rv->smem, s>>>(a);
   CUDA_TRY(h, cudaGetLastError());
   if (timed) CUDA_TRY(h, cudaEventRecord(h->ev1, s));

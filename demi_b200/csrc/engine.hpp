@@ -132,9 +132,10 @@ struct demi_handle {
 // the rest are zero
 namespace demi { struct ReplayArgs; }
 demi::ReplayArgs replay_args(const demi_handle* h, const demi::ReplayTraceView& trace, uint32_t looking_for, uint32_t flags);
-// the multi-trace kernel's own arguments: the set's views and the launch's tiles (capi_replay_many.cu)
-struct ReplayTiles { const demi::ReplayTraceView* views; const uint4* tiles; uint32_t n_tiles; };
-// Every K2 launch: the WILD or exact, REC or batch single-trace kernel, or with `many` the exact or REC multi-trace
+// the multi-trace kernel's own arguments: the set's views, the launch's tiles and, for WILD, each trace's mode table
+// (capi_replay_many.cu)
+struct ReplayTiles { const demi::ReplayTraceView* views; const uint4* tiles; uint32_t n_tiles; const uint32_t* const* modes; };
+// Every K2 launch: the WILD or exact, REC or batch single-trace kernel, or with `many` the same four of the multi-trace
 // kernel, on a's tests; the grid, the per-warp scratch, the generation range and the counters, the loaded model's binding.  `timed`
 // records h->ev0 and h->ev1 around the kernel alone.
 int32_t replay_launch(demi_handle* h, demi::ReplayArgs& a, bool wild, bool record, const ReplayTiles* many, bool timed,
@@ -149,6 +150,8 @@ int32_t trace_tables(demi_handle* h, const char* who, const demi_event* events, 
                      const demi_ext_event* externals, uint32_t n_externals, TraceTables& t);
 // the counts and capacities of a trace's view (its buffers are the caller's)
 demi::ReplayTraceView trace_view(const TraceTables& t, uint32_t n_events, uint32_t n_externals);
+// the flags a wildcard replay accepts (capi_wildcard.cu): DEMI_RF_FILTER_KNOWN_ABSENTS and DEMI_WC_LAST_ONLY
+int32_t wc_check_flags(demi_handle* h, const char* who, uint32_t flags);
 // DDMin's verdicts on n replays: out[i] = "replay i reproduced the violation"; a replay that reported a status fails
 int32_t replay_verdicts(demi_handle* h, const demi_replay_result* res, size_t n, signed char* out);
 // demi_ddmin's walk over a driver whose oracle, trace and flags are set: check_unmodified, ddmin2, verify_mcs, outputs

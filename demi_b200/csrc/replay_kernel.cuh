@@ -51,12 +51,11 @@ struct ReplayArgs {
   unsigned long long* counters;   // [0] reproduced, [1] delivered
   // wildcard replay (WILD instantiations only; the others ignore these): per trace event, for MsgEvents,
   // mode << 16 | delivery ordinal; include masks over deliveries; the causesClockIncrement type set; the
-  // trace positions of ignored deliveries (single-test REC launches)
+  // trace positions of ignored deliveries (REC launches: one list, or with ROWS a row of wc_ignored_cap per test)
   const uint32_t* wc_ev; const uint64_t* wc_include; uint32_t wc_words;
   uint32_t wc_incr[8];
   uint32_t* wc_ignored; uint32_t wc_ignored_cap; uint32_t* wc_ignored_count;
 };
-enum : uint32_t { WC_EXACT = 0, WC_CLASS = 1, WC_CLOCK = 2 };   // match mode of one delivery of the base trace
 
 // a's trace: the host binds the single trace (demi_set_trace), replay_many_kernel each tile's trace of a set
 __host__ __device__ __forceinline__ void bind_trace(ReplayArgs& a, const ReplayTraceView& v) {
@@ -73,12 +72,15 @@ template <class MODEL> constexpr int replay_block = MODEL::N_ACTORS <= 8 ? 256 :
 // WILD: ClockClusterizer's wildcarded trace (capi_wildcard.cu).  The pending set is the insertion-ordered list of
 // the REC variant (Uniq order = list order), compacted in place when taken entries dominate it.
 // ROWS (with REC): many recordings in one launch; test idx records into row idx of rec_events (rec_cap events each)
-// and its count into rec_count[idx].  The row pointer is a member of the machines that record rows only, so the
-// other instantiations keep their layout (a loaded model's machine lives in the stack frame).
-template <bool ROWS> struct RecRow { uint4* rec_row; };
-template <> struct RecRow<false> {};
+// and its count into rec_count[idx]; with WILD also the trace positions of its ignored deliveries into row idx of
+// wc_ignored (wc_ignored_cap each) and their count into wc_ignored_count[idx].  The row pointers are members of the
+// machines that record rows only, so the other instantiations keep their layout (a loaded model's machine lives in the
+// stack frame).
+template <bool ROWS, bool WILD> struct RecRow { uint4* rec_row; };
+template <> struct RecRow<true, true> { uint4* rec_row; uint32_t* ign_row; };
+template <bool WILD> struct RecRow<false, WILD> {};
 template <class MODEL, int BD, bool REC = false, bool WILD = false, bool ROWS = false>
-struct ReplayMachine : TimerTable<MODEL>, RecRow<ROWS> {
+struct ReplayMachine : TimerTable<MODEL>, RecRow<ROWS, WILD> {
   using Model = MODEL;
   static constexpr int BLOCK = BD;
   static constexpr bool LIST = REC || WILD;
@@ -313,7 +315,8 @@ struct ReplayMachine : TimerTable<MODEL>, RecRow<ROWS> {
   const uint64_t* wc_inc; uint32_t n_ign;
   __device__ __forceinline__ void note_ignored(uint32_t i) {
     if (!(WILD && REC)) return;
-    if (A->wc_ignored && n_ign < A->wc_ignored_cap) A->wc_ignored[n_ign] = i;
+    if constexpr (ROWS && WILD) { if (n_ign < A->wc_ignored_cap) this->ign_row[n_ign] = i; }
+    else if (A->wc_ignored && n_ign < A->wc_ignored_cap) A->wc_ignored[n_ign] = i;
     n_ign++;
   }
 
@@ -323,6 +326,7 @@ struct ReplayMachine : TimerTable<MODEL>, RecRow<ROWS> {
     const uint32_t skip = A->skips ? A->skips[test_idx] : 0xFFFFFFFFu;
     n_rec = n_uniq = n_list = 0;       // the list is rebuilt from its first entry: nothing of a previous test is read
     if constexpr (ROWS) this->rec_row = reinterpret_cast<uint4*>(A->rec_events) + (size_t)test_idx * A->rec_cap;
+    if constexpr (ROWS && WILD) this->ign_row = A->wc_ignored + (size_t)test_idx * A->wc_ignored_cap;
     if constexpr (WILD) { wc_inc = A->wc_include + (size_t)test_idx * A->wc_words; list_lo = 0; n_ign = 0; }
     gen = generation;
     actor_init(*this);
@@ -443,7 +447,7 @@ struct ReplayMachine : TimerTable<MODEL>, RecRow<ROWS> {
     if (!status && !diverged) flush();                               // :682 before trace_finished
     out.violation = 0; out.delivered = 0; out.ignored = 0; out.state_hash = 0;
     if (REC && A->rec_count) A->rec_count[ROWS ? test_idx : 0] = n_rec;
-    if (WILD && REC && A->wc_ignored_count) *A->wc_ignored_count = n_ign;
+    if (WILD && REC && A->wc_ignored_count) A->wc_ignored_count[ROWS ? test_idx : 0] = n_ign;
     if (status) { out.status = (uint16_t)status; return; }
     if (diverged) { out.status = DEMI_RS_DIVERGED; out.delivered = (uint16_t)delivered; return; }
     uint32_t v = MODEL::invariant(LaneAll<SW>{smw, BD}, A->model_flags);      // :283-289
@@ -530,11 +534,15 @@ replay_lane_kernel(const __grid_constant__ ReplayArgs args) {
 // one of its four resident blocks per SM); its fields are read through L1.
 // REC: every test records the EventTrace STSScheduler.test returns into its own row (ROWS above): the row is a
 // member of the lane's machine, set from its test index, so the warp's copy of the arguments stays shared.
-template <class MODEL, int BD, bool REC = false>
+// WILD: ClockClusterizer's tests over each tile's trace.  A tile also binds its trace's mode table, modes[trace]; test
+// idx reads its include mask at wc_include + idx * wc_words, the launch's stride.  With REC each test also writes its
+// ignored deliveries into its own row.
+template <class MODEL, int BD, bool REC = false, bool WILD = false>
 __global__ void __launch_bounds__(BD, (model_replay_direct<MODEL>::value && MODEL::N_ACTORS <= 8) ? 1024 / BD : 1)
 replay_many_kernel(const __grid_constant__ ReplayArgs args, const ReplayTraceView* __restrict__ views,
-                   const uint4* __restrict__ tiles, uint32_t n_tiles, ReplayArgs* bound) {
-  using M = ReplayMachine<MODEL, BD, REC, false, REC>;
+                   const uint4* __restrict__ tiles, uint32_t n_tiles, ReplayArgs* bound,
+                   const uint32_t* const* __restrict__ modes) {
+  using M = ReplayMachine<MODEL, BD, REC, WILD, REC>;
   extern __shared__ __align__(16) uint32_t lane_smem[];
   const uint32_t tid = threadIdx.x;
   const uint64_t gwarp = ((uint64_t)blockIdx.x * BD + tid) >> 5;
@@ -551,7 +559,10 @@ replay_many_kernel(const __grid_constant__ ReplayArgs args, const ReplayTraceVie
   for (uint64_t t = gwarp; t < n_tiles; t += total_warps) {
     const uint4 tile = tiles[t];
     __syncwarp();                                  // every lane is done with the previous tile's trace
-    if (lane == 0) { bind_trace(la, views[tile.x]); la.looking_for = tile.w; }
+    if (lane == 0) {
+      bind_trace(la, views[tile.x]); la.looking_for = tile.w;
+      if constexpr (WILD) la.wc_ev = modes[tile.x];
+    }
     __syncwarp();
     if (lane >= tile.z) continue;
     m.next_generation(generation, args);

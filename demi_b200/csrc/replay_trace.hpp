@@ -13,4 +13,7 @@ struct ReplayTraceView {
   uint32_t pending_cap, tosend_cap, table_slots, pad;
 };
 
+// Match mode of one delivery of a wildcard test's base trace (ClockClusterizer, wildcard_driver.hpp)
+enum : uint32_t { WC_EXACT = 0, WC_CLASS = 1, WC_CLOCK = 2 };
+
 }  // namespace demi

@@ -379,6 +379,32 @@ class Engine(object):
                                                         sizes.ctypes.data, cap_sizes, out.ctypes.data, status.ctypes.data))
         return ev, sizes, out, status
 
+    def wildcard_replay_batch_many(self, trace_of_test, include_masks, looking_for, flags=0, mask_words=None):
+        """demi_wildcard_replay_batch_many: test i is include_masks[i] (bits over the deliveries of trace
+        trace_of_test[i], in trace order) on that trace; looking_for[t] per trace.  REPLAY_DTYPE [n]."""
+        tr = np.ascontiguousarray(trace_of_test, dtype=np.uint32)
+        m = np.ascontiguousarray(include_masks, dtype=np.uint64)
+        mw = mask_words or (m.shape[1] if m.ndim == 2 else 1)
+        m = m.reshape(-1, mw)
+        lf = np.ascontiguousarray(looking_for, dtype=np.uint32)
+        out = np.empty(len(tr), dtype=N.REPLAY_DTYPE)
+        self._check(N.lib().demi_wildcard_replay_batch_many(self._h, tr.ctypes.data, m.ctypes.data, len(tr), mw,
+                                                            lf.ctypes.data, flags, out.ctypes.data))
+        return out
+
+    def wildcard_minimize_many(self, looking_for, flags=0, cap_events=4096, cap_sizes=1024):
+        """demi_wildcard_minimize_many over the set: (traces [n, cap_events], sizes [n, cap_sizes], INTMIN_OUT_DTYPE [n],
+        status [n]).  Trace t is traces[t, :out[t]['n_events']]; a trace whose status is not OK has no outputs."""
+        n = len(self._set_ext)
+        lf = np.ascontiguousarray(looking_for, dtype=np.uint32)
+        ev = np.zeros((n, cap_events), dtype=N.EVENT_DTYPE)
+        sizes = np.zeros((n, cap_sizes), dtype=np.uint32)
+        out = np.zeros(n, dtype=N.INTMIN_OUT_DTYPE)
+        status = np.zeros(n, dtype=np.int32)
+        self._check(N.lib().demi_wildcard_minimize_many(self._h, lf.ctypes.data, flags, ev.ctypes.data, cap_events,
+                                                        sizes.ctypes.data, cap_sizes, out.ctypes.data, status.ctypes.data))
+        return ev, sizes, out, status
+
     def last_error(self):
         return N.lib().demi_last_error(self._h).decode()
 

@@ -436,6 +436,33 @@ int32_t demi_internal_minimize_many(demi_handle* h, const uint32_t* looking_for,
                                     demi_event* out_traces, uint32_t cap_events,
                                     uint32_t* internal_sizes, uint32_t cap_sizes,
                                     demi_intmin_out* out, int32_t* status);
+/* n_tests wildcard STSScheduler.test calls over the set in one launch: test i is include mask i (mask_words words, over
+ * the deliveries of trace trace_of_test[i] in trace order) on that trace, looking for looking_for[trace_of_test[i]].
+ * Record i equals what demi_set_trace(trace t) then demi_wildcard_replay_batch(mask i, looking_for[t], flags) returns,
+ * under the handle's clock rules.  Bits of mask i at or past trace t's deliveries are ignored; mask_words must cover
+ * every named trace's deliveries (ceil(n / 64), at least 1), and every named trace's Uniq ids must be distinct, else
+ * DEMI_ERR_INVALID.  Tests past 2^20 go to further launches.  demi_perf counts the launches, the tests and their
+ * kernel time. */
+int32_t demi_wildcard_replay_batch_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* include_masks,
+                                        uint32_t n_tests, uint32_t mask_words, const uint32_t* looking_for,
+                                        uint32_t flags, demi_replay_result* out);
+/* demi_wildcard_minimize on every trace t of the set (a verified MCS trace whose externals are its MCS), looking for
+ * looking_for[t]; flags as demi_wildcard_minimize's, under the handle's clock rules.  The minimizations step in
+ * lock-step rounds: one launch evaluates the candidate tests of the round's traces, one launch records every success of
+ * the round.  A round admits unfinished traces in index order while their include masks fit 256 MiB of host memory
+ * (at least one trace); the others wait for a later round, which changes no result.  status[t] is what
+ * demi_set_trace(trace t) then demi_wildcard_minimize(h, looking_for[t], flags, ...) would return, and when it is
+ * DEMI_OK, out_traces[t*cap_events ..], internal_sizes[t*cap_sizes ..] (may be NULL) and out[t] equal that call's
+ * outputs, replays_executed and batches included.  cap_events is also the capacity of each recording: a trace that needs
+ * a longer one fails alone with DEMI_ERR_CAPACITY, as does one whose replay reports a status; a trace whose Uniq ids
+ * repeat fails alone with DEMI_ERR_INVALID.  The results do not depend on which other traces are in the set.  Neither
+ * the set nor the handle's trace changes.  The call fails only on invalid arguments or flags (DEMI_RF_STRICT, unknown
+ * bits), without a set (DEMI_ERR_STATE) or on a CUDA error; when some traces fail, it returns DEMI_OK and
+ * demi_last_error holds the message of the lowest-indexed one, which names it. */
+int32_t demi_wildcard_minimize_many(demi_handle* h, const uint32_t* looking_for, uint32_t flags,
+                                    demi_event* out_traces, uint32_t cap_events,
+                                    uint32_t* internal_sizes, uint32_t cap_sizes,
+                                    demi_intmin_out* out, int32_t* status);
 
 /* DDMin with a RandomScheduler as the TestOracle (RunnerUtils.randomDDMin, RunnerUtils.scala:601-623).  The dag is the
  * handle's program (demi_set_externals) with every event in it, WaitQuiescence included: DDMin.minimize wraps the

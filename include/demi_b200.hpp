@@ -292,6 +292,26 @@ class Engine {
     }
     return r;
   }
+  // demi_wildcard_minimize_many: per trace of the set (a verified MCS trace), its wildcard-minimized trace and record
+  // under the handle's clock rules, or the error code
+  std::vector<IntMinManyResult> wildcard_minimize_many(const std::vector<ViolationFingerprint>& looking_for, uint32_t flags = 0,
+                                                       uint32_t cap_events = 4096, uint32_t cap_sizes = 1024) {
+    const size_t n = set_ext.size();
+    std::vector<demi_event> ev(n * (size_t)cap_events);
+    std::vector<uint32_t> sizes(n * (size_t)cap_sizes);
+    std::vector<demi_intmin_out> out(n);
+    std::vector<int32_t> status(n);
+    check(demi_wildcard_minimize_many(h, looking_for.data(), flags, ev.data(), cap_events, sizes.data(), cap_sizes, out.data(),
+                                      status.data()));
+    std::vector<IntMinManyResult> r(n);
+    for (size_t t = 0; t < n; t++) {
+      r[t].out = out[t]; r[t].status = status[t];
+      if (status[t] != DEMI_OK) continue;
+      r[t].trace.assign(ev.begin() + t * cap_events, ev.begin() + t * cap_events + std::min(out[t].n_events, cap_events));
+      r[t].internal_sizes.assign(sizes.begin() + t * cap_sizes, sizes.begin() + t * cap_sizes + std::min(out[t].n_internal_sizes, cap_sizes));
+    }
+    return r;
+  }
   const SchedulerConfig cfg;
  private:
   demi_handle* h = nullptr;

@@ -247,6 +247,18 @@ JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_internalMinimi
                                      (uint32_t)capEvents, sizes ? (uint32_t*)BUF(env, sizes) : 0, (uint32_t)capSizes,
                                      (demi_intmin_out*)BUF(env, out), (int32_t*)BUF(env, status));
 }
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_wildcardReplayBatchMany(JNIEnv* env, jclass c, jlong h,
+    jobject traceOfTest, jobject includeMasks, jint nTests, jint maskWords, jobject lookingFor, jint flags, jobject out) {
+  return demi_wildcard_replay_batch_many(H(h), (const uint32_t*)BUF(env, traceOfTest), (const uint64_t*)BUF(env, includeMasks),
+                                         (uint32_t)nTests, (uint32_t)maskWords, (const uint32_t*)BUF(env, lookingFor),
+                                         (uint32_t)flags, (demi_replay_result*)BUF(env, out));
+}
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_wildcardMinimizeMany(JNIEnv* env, jclass c, jlong h,
+    jobject lookingFor, jint flags, jobject traces, jint capEvents, jobject sizes, jint capSizes, jobject out, jobject status) {
+  return demi_wildcard_minimize_many(H(h), (const uint32_t*)BUF(env, lookingFor), (uint32_t)flags, (demi_event*)BUF(env, traces),
+                                     (uint32_t)capEvents, sizes ? (uint32_t*)BUF(env, sizes) : 0, (uint32_t)capSizes,
+                                     (demi_intmin_out*)BUF(env, out), (int32_t*)BUF(env, status));
+}
 /* `exp` = a direct buffer laid out as demi_experiment whose pointer fields the Scala side fills with
  * GetDirectBufferAddress-style addresses (DemiNative.addressOf) */
 JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_experimentSave(JNIEnv* env, jclass c, jstring dir, jobject exp) {

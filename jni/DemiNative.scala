@@ -96,6 +96,14 @@ object DemiNative {
    *  at traces + t*capEvents, status(t) its return code */
   @native def internalMinimizeMany(h: Long, lookingFor: ByteBuffer, flags: Int, traces: ByteBuffer, capEvents: Int,
                                    sizes: ByteBuffer, capSizes: Int, out: ByteBuffer, status: ByteBuffer): Int
+  /** demi_wildcard_replay_batch_many: ClockClusterizer test i (an include mask over the deliveries of trace
+   *  traceOfTest(i)) on that trace of the set */
+  @native def wildcardReplayBatchMany(h: Long, traceOfTest: ByteBuffer, includeMasks: ByteBuffer, nTests: Int, maskWords: Int,
+                                      lookingFor: ByteBuffer, flags: Int, out: ByteBuffer): Int
+  /** demi_wildcard_minimize_many: WildcardMinimizer (STSSched, ClockClusterizer) on every trace of the set; trace t at
+   *  traces + t*capEvents, status(t) its return code */
+  @native def wildcardMinimizeMany(h: Long, lookingFor: ByteBuffer, flags: Int, traces: ByteBuffer, capEvents: Int,
+                                   sizes: ByteBuffer, capSizes: Int, out: ByteBuffer, status: ByteBuffer): Int
   /** The flat experiment directory that replaces ExperimentSerializer's *.bin object streams (Serialization.scala:57-74). */
   @native def experimentSave(dir: String, exp: ByteBuffer): Int
   @native def experimentLoad(dir: String, exp: ByteBuffer): Int
