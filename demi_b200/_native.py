@@ -88,6 +88,11 @@ class IncDDMinOut(C.Structure):
                 ("tests_executed", C.c_uint32), ("batches", C.c_uint32), ("interleavings_executed", C.c_uint64)]
 
 
+# demi_incddmin_out as a record array (demi_incremental_ddmin_many)
+INCDDMIN_OUT_DTYPE = np.dtype([("mcs_size", "<u4"), ("total_replays", "<u4"), ("rounds", "<u4"), ("instances", "<u4"),
+                               ("tests_executed", "<u4"), ("batches", "<u4"), ("interleavings_executed", "<u8")])
+
+
 DF_ARVIND_ORDERING, DF_PRIORITIZE_PENDING = 1, 2
 IM_SRC_DST_FIFO = 0x100
 WC_LAST_ONLY = 0x200
@@ -134,7 +139,7 @@ EXPORTS = [
     "demi_random_test_batch", "demi_random_ddmin", "demi_random_test_trace",
     "demi_fuzz_traces", "demi_set_traces", "demi_replay_batch_many", "demi_ddmin_many",
     "demi_replay_traces_many", "demi_internal_minimize_many", "demi_wildcard_replay_batch_many",
-    "demi_wildcard_minimize_many",
+    "demi_wildcard_minimize_many", "demi_incremental_ddmin_many", "demi_fuzz_traces_tree",
 ]
 FILTER_RULE_DTYPE = np.dtype([("src_mask", "<u4"), ("dst_mask", "<u4"), ("type_mask", "<u4"), ("flags", "<u4")])
 FRULE_DEADLETTERS = 1
@@ -338,6 +343,11 @@ def lib():
     L.demi_wildcard_replay_batch_many.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp]
     L.demi_wildcard_minimize_many.restype = C.c_int32
     L.demi_wildcard_minimize_many.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, vp]
+    L.demi_incremental_ddmin_many.restype = C.c_int32
+    L.demi_incremental_ddmin_many.argtypes = [vp, C.c_uint32, vp, vp, vp, vp, vp, vp, C.POINTER(DporParams), C.c_uint32,
+                                              C.c_int32, C.c_uint32, vp, C.c_uint32, vp, vp]
+    L.demi_fuzz_traces_tree.restype = C.c_int32
+    L.demi_fuzz_traces_tree.argtypes = [vp, C.POINTER(FuzzParams), vp, C.c_uint32, vp, C.c_uint32, vp, vp, C.c_uint32, vp, vp]
     L.demi_stats.restype = C.c_int32
     L.demi_stats.argtypes = [vp, C.POINTER(Perf)]
     L.demi_lane_kernel.restype = C.c_int32

@@ -805,17 +805,16 @@ extern "C" int32_t demi_fuzz_provenance(demi_handle* h, const demi_fuzz_params* 
 }
 
 // The EventTraces of executions seed_base + prefix_index[i], recorded as demi_fuzz_provenance records them (the lane
-// engine first, the slots it defers on the general engine) without the dep tree: the events of execution i go to
-// events + i*cap_events, its count to n_events[i] and its record to results[i] (may be NULL).
-extern "C" int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, const uint32_t* prefix_index, uint32_t n,
-                                    demi_event* events, uint32_t cap_events, uint32_t* n_events, demi_fuzz_result* results) {
-  if (!h) return DEMI_ERR_INVALID;
-  if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
-  if (!n) return DEMI_OK;
-  if (!prefix_index || !events || !cap_events || !n_events)
-    return fail(h, DEMI_ERR_INVALID, "demi_fuzz_traces: prefix_index, events, cap_events and n_events are required");
+// engine first, the slots it defers on the general engine): the events of execution i go to events + i*cap_events, its
+// count to n_events[i] and its record to results[i] (may be NULL).  With dep_parent, its DepTracker tree goes to
+// dep_parent + i*cap_nodes and its node count to n_nodes[i]; without, one parent entry per slot is staged and the tree
+// is not returned.
+static int32_t fuzz_traces(demi_handle* h, const char* who, const demi_fuzz_params* p, const uint32_t* prefix_index, uint32_t n,
+                           demi_event* events, uint32_t cap_events, uint32_t* n_events, uint16_t* dep_parent, uint32_t cap_nodes,
+                           uint32_t* n_nodes, demi_fuzz_result* results) {
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  const uint32_t chunk = record_chunk(cap_events, 1, 0);
+  const uint32_t par_cap = dep_parent ? cap_nodes : 1;
+  const uint32_t chunk = record_chunk(cap_events, par_cap, 0);
   cudaStream_t s = h->stream;
   DevBuf buf;
   int32_t rc;
@@ -832,9 +831,8 @@ extern "C" int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, c
     LaunchPlan plan;
     if ((rc = plan_launch(h, &q, LM_RECORD, h->ext_info, h->ext_dev.get<demi_ext_event>(), (uint32_t)h->ext_host.size(), &plan)) != DEMI_OK)
       return rc;
-    // one parent entry per slot: the tree is not returned
     Records rec;
-    if ((rc = stage_records(h, &plan, m, prefix_index + off, cap_events, 1, 0, buf, &rec, s)) != DEMI_OK) return rc;
+    if ((rc = stage_records(h, &plan, m, prefix_index + off, cap_events, par_cap, 0, buf, &rec, s)) != DEMI_OK) return rc;
     CUDA_TRY(h, cudaEventRecord(h->ev0, s));
     if ((rc = launch_plan(h, plan, m, s)) != DEMI_OK) return rc;
     CUDA_TRY(h, cudaEventRecord(h->ev1, s));
@@ -845,33 +843,63 @@ extern "C" int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, c
     float ms = 0.f;
     CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
     ms_all += ms;
-    // the events travel as rows as wide as the longest successful recording; a failing execution's partial recording
-    // is zeroed first, so that it returns no events
-    uint32_t width = 0;
+    // the events (and parents) travel as rows as wide as the longest successful recording; a failing execution's
+    // partial recording is zeroed first, so that it returns no events
+    uint32_t width = 0, pwidth = 0;
     for (uint32_t i = 0; i < m; i++) {
       n_events[off + i] = cnt[(size_t)i * 4];
+      if (n_nodes) n_nodes[off + i] = cnt[(size_t)i * 4 + 1];
       if (results) results[off + i] = res[i];
       if (res[i].status) {
         if (bad < 0) { bad = off + i; bad_status = res[i].status; }
         CUDA_TRY(h, cudaMemsetAsync(rec.events + (size_t)i * cap_events, 0, (size_t)cap_events * sizeof(demi_event), s));
+        if (dep_parent) CUDA_TRY(h, cudaMemsetAsync(rec.parents + (size_t)i * par_cap, 0, (size_t)par_cap * sizeof(uint16_t), s));
       } else {
         width = std::max(width, std::min(cnt[(size_t)i * 4], cap_events));
+        pwidth = std::max(pwidth, std::min(cnt[(size_t)i * 4 + 1], par_cap));
       }
     }
     if (width) {
       const size_t pitch = (size_t)cap_events * sizeof(demi_event);
       CUDA_TRY(h, cudaMemcpy2DAsync(events + (size_t)off * cap_events, pitch, rec.events, pitch, (size_t)width * sizeof(demi_event), m,
                                     cudaMemcpyDeviceToHost, s));
-      CUDA_TRY(h, cudaStreamSynchronize(s));
     }
+    if (dep_parent && pwidth) {
+      const size_t pitch = (size_t)par_cap * sizeof(uint16_t);
+      CUDA_TRY(h, cudaMemcpy2DAsync(dep_parent + (size_t)off * par_cap, pitch, rec.parents, pitch, (size_t)pwidth * sizeof(uint16_t), m,
+                                    cudaMemcpyDeviceToHost, s));
+    }
+    if (width || (dep_parent && pwidth)) CUDA_TRY(h, cudaStreamSynchronize(s));
   }
   h->perf.prefixes = n;
   h->perf.kernel_ms = ms_all;
   // as demi_fuzz_trace fails for that seed; every record is filled all the same
   if (bad >= 0)
-    return fail(h, DEMI_ERR_CAPACITY, "demi_fuzz_traces: execution %lld (prefix %u) status %u", (long long)bad,
-                prefix_index[bad], bad_status);
+    return fail(h, DEMI_ERR_CAPACITY, "%s: execution %lld (prefix %u) status %u", who, (long long)bad, prefix_index[bad], bad_status);
   return DEMI_OK;
+}
+
+extern "C" int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, const uint32_t* prefix_index, uint32_t n,
+                                    demi_event* events, uint32_t cap_events, uint32_t* n_events, demi_fuzz_result* results) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
+  if (!n) return DEMI_OK;
+  if (!prefix_index || !events || !cap_events || !n_events)
+    return fail(h, DEMI_ERR_INVALID, "demi_fuzz_traces: prefix_index, events, cap_events and n_events are required");
+  return fuzz_traces(h, "demi_fuzz_traces", p, prefix_index, n, events, cap_events, n_events, nullptr, 0, nullptr, results);
+}
+
+extern "C" int32_t demi_fuzz_traces_tree(demi_handle* h, const demi_fuzz_params* p, const uint32_t* prefix_index, uint32_t n,
+                                         demi_event* events, uint32_t cap_events, uint32_t* n_events,
+                                         uint16_t* dep_parent, uint32_t cap_nodes, uint32_t* n_nodes, demi_fuzz_result* results) {
+  if (!h) return DEMI_ERR_INVALID;
+  if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
+  if (!n) return DEMI_OK;
+  if (!prefix_index || !events || !cap_events || !n_events || !dep_parent || !cap_nodes || !n_nodes)
+    return fail(h, DEMI_ERR_INVALID,
+                "demi_fuzz_traces_tree: prefix_index, events, cap_events, n_events, dep_parent, cap_nodes and n_nodes are required");
+  return fuzz_traces(h, "demi_fuzz_traces_tree", p, prefix_index, n, events, cap_events, n_events, dep_parent, cap_nodes, n_nodes,
+                     results);
 }
 
 // ---------------------------------------------------------------------------------------------------------

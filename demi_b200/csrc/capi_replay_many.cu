@@ -3,25 +3,18 @@
 //
 // A minimisation of a small trace asks for tens to a few hundred tests at a time, a small fraction of one wave of the
 // replay kernel, and waits for each launch.  Here the drivers of many traces run side by side, each on a host thread
-// with a rendezvous: every driver in flight runs until it asks for an evaluation or finishes, then one launch evaluates
-// the union of their requests and each gets its own slice back.  A driver sees exactly the answers it would get alone,
-// so its decisions, MCS and counters do not depend on which other drivers share its launches.
+// with a rendezvous (many_rendezvous.hpp): one launch evaluates the union of the requests of every driver in flight.
 //
 // Internal minimization over a set runs the same way without threads: its driver (intmin_driver.hpp) is not recursive,
 // so every trace's driver steps in lock-step rounds of one exact launch and one recording launch.  Wildcard
 // minimization (wildcard_driver.hpp) steps the same way, with the WILD kernel for both launches.
-#include <atomic>
-#include <condition_variable>
 #include <functional>
-#include <mutex>
-#include <new>
-#include <system_error>
-#include <thread>
 #include "replay_kernel.cuh"
 #include "engine.hpp"
 #include "ddmin_driver.hpp"
 #include "intmin_driver.hpp"
 #include "wildcard_driver.hpp"
+#include "many_rendezvous.hpp"
 
 using namespace demi;
 
@@ -34,8 +27,6 @@ constexpr uint64_t MANY_MAX_REC_BYTES = 1ull << 30;
 // a round of demi_wildcard_minimize_many admits traces while their include masks stay under this many host bytes
 // (DEMI_TEST_WC_ROUND_BYTES overrides it, for tests)
 constexpr uint64_t WC_MANY_ROUND_BYTES = 256ull << 20;
-// host threads demi_ddmin_many may run at once
-constexpr uint32_t MANY_MAX_WINDOW = 4096;
 
 struct LaunchCounts { uint32_t launches = 0; uint64_t tests = 0, violations = 0, deliveries = 0; double ms = 0; };
 
@@ -186,32 +177,14 @@ int32_t replay_many(demi_handle* h, const Views& V, const uint32_t* trace_of_tes
 }
 
 // ---------------------------------------------------------------------- rounds of DDMin drivers
-// A driver's request for an evaluation: its masks (a slice of its arena, which stays put while it waits) and, once
-// served, their results or the launch's error.
-struct Request {
-  uint32_t trace; const uint64_t* masks; size_t n;
-  std::vector<demi_replay_result> res;
-  int32_t rc = DEMI_OK; bool done = false;
-};
-struct Rendezvous {
-  std::mutex mu;
-  std::condition_variable coord, work;
-  uint32_t running = 0;            // workers executing driver code; the others wait on a request or have left
-  std::vector<Request*> queue;
-};
+typedef ManyRequest<demi_replay_result> Request;
 
 // STSSched as DDMin's TestOracle on trace `trace` of the set, as StsDDMinDriver (capi_replay.cu) on the single trace
 struct SetDDMinDriver : DDMinDriver {
-  Rendezvous* R; uint32_t trace;
+  Rendezvous<demi_replay_result>* R; uint32_t trace;
   int32_t evaluate(const uint64_t* masks, size_t n, signed char* out) override {
     Request q; q.trace = trace; q.masks = masks; q.n = n;
-    {
-      std::unique_lock<std::mutex> lk(R->mu);
-      R->queue.push_back(&q);
-      R->running--;
-      R->coord.notify_one();
-      R->work.wait(lk, [&] { return q.done; });
-    }
+    R->submit(q);
     return q.rc != DEMI_OK ? q.rc : replay_verdicts(h, q.res.data(), n, out);
   }
 };
@@ -304,101 +277,45 @@ extern "C" int32_t demi_ddmin_many(demi_handle* h, const uint32_t* looking_for, 
   for (uint32_t t = 0; t < n; t++)
     if ((uint64_t)mask_words * 64 < h->set.ext[t].size())
       return fail(h, DEMI_ERR_INVALID, "mask_words %u too small for the %zu externals of trace %u", mask_words, h->set.ext[t].size(), t);
-  // drivers in flight: DEMI_DDMIN_MANY_WINDOW, 1..MANY_MAX_WINDOW (default 512); a thread that finishes a driver takes
-  // the next trace
-  uint32_t window = 512;
-  if (const char* w = getenv("DEMI_DDMIN_MANY_WINDOW")) {
-    char* end = nullptr;
-    const long v = strtol(w, &end, 10);
-    if (end == w || *end || v < 1 || v > (long)MANY_MAX_WINDOW)
-      return fail(h, DEMI_ERR_INVALID, "DEMI_DDMIN_MANY_WINDOW=%s: expected 1..%u", w, MANY_MAX_WINDOW);
-    window = (uint32_t)v;
-  }
-  window = std::min(window, n);
+  // drivers in flight: DEMI_DDMIN_MANY_WINDOW (many_window)
+  uint32_t window;
+  { int32_t wrc = many_window(h, n, window); if (wrc != DEMI_OK) return wrc; }
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   memset(out, 0, (size_t)n * sizeof(demi_ddmin_out));
-  Rendezvous R;
-  std::atomic<uint32_t> next{0};
-  std::vector<std::string> msg(n);
-  auto worker = [&]() {
-    // fail() records a message on the handle it is given: each worker's drivers get a handle of their own for that,
-    // so that the message of each failing trace is kept
-    demi_handle eh;
-    for (uint32_t t; (t = next.fetch_add(1)) < n;) {
-      try {
-        SetDDMinDriver d;
-        d.R = &R; d.trace = t;
-        d.h = &eh; d.looking_for = looking_for[t]; d.flags = flags; d.mw = mask_words;
-        d.n_ext = (uint32_t)h->set.ext[t].size(); d.ext = h->set.ext[t].data();
-        status[t] = ddmin_sts(d, check_unmodified, mcs_masks + (size_t)t * mask_words,
-                              iteration_sizes ? iteration_sizes + (size_t)t * cap_iterations : nullptr, cap_iterations, out + t);
-        if (status[t] != DEMI_OK) msg[t] = eh.err;
-      } catch (const std::bad_alloc&) {                // a driver out of host memory fails its trace alone
-        status[t] = DEMI_ERR_CAPACITY;
-        msg[t] = "demi_ddmin_many: out of host memory";
-      }
-    }
-    std::lock_guard<std::mutex> lk(R.mu);
-    R.running--;
-    R.coord.notify_one();
+  auto drive = [&](uint32_t t, Rendezvous<demi_replay_result>& R, demi_handle* eh) -> int32_t {
+    SetDDMinDriver d;
+    d.R = &R; d.trace = t;
+    d.h = eh; d.looking_for = looking_for[t]; d.flags = flags; d.mw = mask_words;
+    d.n_ext = (uint32_t)h->set.ext[t].size(); d.ext = h->set.ext[t].data();
+    return ddmin_sts(d, check_unmodified, mcs_masks + (size_t)t * mask_words,
+                     iteration_sizes ? iteration_sizes + (size_t)t * cap_iterations : nullptr, cap_iterations, out + t);
   };
   LaunchCounts lc;
-  int32_t call_rc = DEMI_OK;
-  std::string call_msg;
-  std::vector<std::thread> threads;
-  {
-    std::unique_lock<std::mutex> lk(R.mu);
-    // the workers are counted before any of them can take the lock; when the system refuses a thread, the ones already
-    // started carry the window (the results do not depend on it)
-    try {
-      threads.reserve(window);
-      for (uint32_t i = 0; i < window; i++) threads.emplace_back(worker);
-    } catch (const std::system_error&) {
-    } catch (const std::bad_alloc&) {
+  auto serve = [&](std::vector<Request*>& batch) -> int32_t {
+    size_t total = 0;
+    for (const Request* q : batch) total += q->n;
+    std::vector<uint32_t> tr(total);
+    std::vector<uint64_t> flat(total * mask_words);
+    std::vector<demi_replay_result> res(total);
+    size_t k = 0;
+    for (const Request* q : batch) {
+      std::fill(tr.begin() + k, tr.begin() + k + q->n, q->trace);
+      std::copy(q->masks, q->masks + q->n * mask_words, flat.begin() + k * mask_words);
+      k += q->n;
     }
-    R.running = (uint32_t)threads.size();
-    if (threads.empty()) return fail(h, DEMI_ERR_CAPACITY, "demi_ddmin_many: could not start a worker thread");
-    for (;;) {
-      R.coord.wait(lk, [&] { return R.running == 0; });
-      if (R.queue.empty()) break;                  // no driver waits and none runs: every trace is done
-      std::vector<Request*> batch;
-      batch.swap(R.queue);
-      lk.unlock();
-      size_t total = 0;
-      for (const Request* q : batch) total += q->n;
-      std::vector<uint32_t> tr(total);
-      std::vector<uint64_t> flat(total * mask_words);
-      std::vector<demi_replay_result> res(total);
-      size_t k = 0;
-      for (const Request* q : batch) {
-        std::fill(tr.begin() + k, tr.begin() + k + q->n, q->trace);
-        std::copy(q->masks, q->masks + q->n * mask_words, flat.begin() + k * mask_words);
-        k += q->n;
-      }
-      int32_t rc = call_rc;
-      if (rc == DEMI_OK) {
-        rc = replay_many(h, Views::of(h->set), tr.data(), flat.data(), nullptr, (uint32_t)total, mask_words, looking_for, flags,
-                         res.data(), lc);
-        if (rc != DEMI_OK) { call_rc = rc; call_msg = h->err; }
-      }
-      k = 0;
-      for (Request* q : batch) {
-        q->rc = rc;
-        if (rc == DEMI_OK) q->res.assign(res.begin() + k, res.begin() + k + q->n);
-        k += q->n;
-      }
-      lk.lock();
-      for (Request* q : batch) q->done = true;
-      R.running += (uint32_t)batch.size();
-      R.work.notify_all();
+    const int32_t rc = replay_many(h, Views::of(h->set), tr.data(), flat.data(), nullptr, (uint32_t)total, mask_words, looking_for,
+                                   flags, res.data(), lc);
+    if (rc != DEMI_OK) return rc;
+    k = 0;
+    for (Request* q : batch) {
+      q->res.assign(res.begin() + k, res.begin() + k + q->n);
+      k += q->n;
     }
-  }
-  for (std::thread& th : threads) th.join();
+    return DEMI_OK;
+  };
+  const int32_t rc = run_many<demi_replay_result>(h, "demi_ddmin_many", n, window, drive, serve, status);
   set_perf(h, lc);
-  if (call_rc != DEMI_OK) { h->err = call_msg; return call_rc; }
-  for (uint32_t t = 0; t < n; t++)
-    if (status[t] != DEMI_OK) { h->err = msg[t]; break; }
-  return DEMI_OK;
+  return rc;
 }
 
 extern "C" int32_t demi_replay_traces_many(demi_handle* h, const uint32_t* trace_of_test, const uint64_t* masks,

@@ -35,6 +35,14 @@ __host__ __device__ __forceinline__ uint32_t dpor_key_trace(DporKey q) { return 
 __host__ __device__ __forceinline__ uint32_t dpor_key_later(DporKey q) { return 0xFFFu - (uint32_t)((q >> 12) & 0xFFFu); }
 __host__ __device__ __forceinline__ uint32_t dpor_key_earlier(DporKey q) { return 0xFFFu - (uint32_t)(q & 0xFFFu); }
 
+// One trace's seed in a multi-trace launch (demi_incremental_ddmin_many): its init nodes and original indices are
+// init_nodes / orig_index [node_off, node_off + n_nodes), its init trace init_trace [trace_off, trace_off + n_trace),
+// and its own setMaxMessagesToSchedule and ViolationFingerprint.  32 bytes.
+struct DporSeedView {
+  uint32_t node_off, n_nodes, trace_off, n_trace;
+  int32_t max_messages; uint32_t looking_for; uint32_t pad[2];
+};
+
 struct DporArgs {
   uint32_t model_flags, blocked_mask;
   demi_dpor_params P;
@@ -64,10 +72,18 @@ struct DporArgs {
   // An instance's state is a function of the caps it was tested with, so a launch that replays that history is
   // side-effect free — which is what lets DDMin's tests be evaluated speculatively.  caps == null: one test, no cap.
   const int32_t* caps; const uint32_t* cap_offsets;
+  // multi-trace launches only (dpor_kernel<..., true>): search s reads seeds[trace_of_search[s]] instead of the seed
+  // fields above and P.max_messages / P.looking_for; the strides above use T1 = the launch's largest max_messages + 2
+  const DporSeedView* seeds; const uint32_t* trace_of_search;
 };
 
-template <class MODEL, int BD>
-struct DporMachine : TimerTable<MODEL> {
+// Where a search reads its seed, its max_messages and its looking_for: the launch's arguments (one seed per launch),
+// or, in a multi-trace launch, the view of its own trace, read once when the search starts
+template <bool MULTI> struct DporSeedSel {};
+template <> struct DporSeedSel<true> { DporSeedView sv; };
+
+template <class MODEL, int BD, bool MULTI = false>
+struct DporMachine : TimerTable<MODEL>, DporSeedSel<MULTI> {
   using Model = MODEL;
   static constexpr int BLOCK = BD;
   static constexpr int N = MODEL::N_ACTORS;
@@ -93,6 +109,19 @@ struct DporMachine : TimerTable<MODEL> {
   uint32_t status;
 
   __device__ __forceinline__ LaneState actor(uint32_t a) { return LaneState{smw + a * SW * BD, BD}; }
+  __device__ __forceinline__ uint32_t n_init_nodes() const { if constexpr (MULTI) return this->sv.n_nodes; else return A->n_init_nodes; }
+  __device__ __forceinline__ uint32_t n_init_trace() const { if constexpr (MULTI) return this->sv.n_trace; else return A->n_init_trace; }
+  __device__ __forceinline__ const uint4* init_nodes() const {
+    if constexpr (MULTI) return A->init_nodes + this->sv.node_off; else return A->init_nodes;
+  }
+  __device__ __forceinline__ const int32_t* orig_index() const {
+    if constexpr (MULTI) return A->orig_index + this->sv.node_off; else return A->orig_index;
+  }
+  __device__ __forceinline__ const uint32_t* init_trace() const {
+    if constexpr (MULTI) return A->init_trace + this->sv.trace_off; else return A->init_trace;
+  }
+  __device__ __forceinline__ int32_t max_messages() const { if constexpr (MULTI) return this->sv.max_messages; else return A->P.max_messages; }
+  __device__ __forceinline__ uint32_t looking_for() const { if constexpr (MULTI) return this->sv.looking_for; else return A->P.looking_for; }
   __device__ __forceinline__ uint32_t node_parent(uint32_t i) const { return nodes[i].w & 0xFFFFFu; }
   __device__ __forceinline__ uint32_t node_depth(uint32_t i) const { return nodes[i].w >> 20; }
   __device__ __forceinline__ uint32_t qindex(uint32_t src, uint32_t dst) const {
@@ -241,7 +270,7 @@ struct DporMachine : TimerTable<MODEL> {
     for (;;) {
       if (status) return 0;
       nsched++;
-      if (A->P.max_messages >= 0 && nsched > A->P.max_messages) return 0;       // :583-586
+      if (max_messages() >= 0 && nsched > max_messages()) return 0;             // :583-586
       uint32_t pick = 0;
       do {                                                                       // getNextMatchingMessage :542-555
         while (next_pos < next_len && next_rd[next_pos] == 0) next_pos++;     // getNextTraceMessage :363-372
@@ -299,7 +328,7 @@ struct DporMachine : TimerTable<MODEL> {
     }
     if (status) return 0;
     uint32_t v = MODEL::invariant(LaneAll<SW>{smw, BD}, A->model_flags);          // checkInvariant :394-418
-    if (A->P.looking_for) v = (v == A->P.looking_for) ? v : 0u;
+    if (looking_for()) v = (v == looking_for()) ? v : 0u;
     return v;
   }
 
@@ -319,8 +348,8 @@ struct DporMachine : TimerTable<MODEL> {
   // (getCommonPrefix(e1, e1)) ++ replayThis ++ [e1, e2]; +1 per event absent from the original trace, +1 per
   // earlier path element the original trace orders after it.  `path` holds original indices (-1 = absent).
   __device__ uint32_t arvind_distance(uint32_t branch, const uint32_t* kt, uint32_t li, uint32_t e1, uint32_t e2) {
-    const uint32_t n0 = A->n_init_nodes;
-    auto oi_of = [&](uint32_t v) -> int32_t { return v < n0 ? __ldg(A->orig_index + v) : -1; };
+    const uint32_t n0 = n_init_nodes();
+    auto oi_of = [&](uint32_t v) -> int32_t { return v < n0 ? __ldg(orig_index() + v) : -1; };
     const uint32_t depth = node_depth(e1);
     uint32_t v = e1;
     for (uint32_t i = depth + 1; i-- > 0; v = node_parent(v)) path[i] = oi_of(v);
@@ -445,6 +474,7 @@ struct DporMachine : TimerTable<MODEL> {
 
   // The DPORwHeuristics.test calls (:1193-1242) of one instance.
   __device__ void search(uint32_t sid) {
+    if constexpr (MULTI) this->sv = A->seeds[A->trace_of_search[sid]];
     const uint32_t ext_lo = A->ext_offsets[sid], ext_hi = A->ext_offsets[sid + 1];
     demi_dpor_result R; memset(&R, 0, sizeof(R));
     uint32_t n_viol = 0;
@@ -452,17 +482,17 @@ struct DporMachine : TimerTable<MODEL> {
     n_explored = n_heap = n_traces = 0; status = 0; found = 0; cur_len = 0;
     if (bk_head) bq_reset();
     // setInitialDepGraph (:214-217): start from the recorded execution's graph
-    if (A->n_init_nodes) {
-      if (A->n_init_nodes > A->P.node_cap) status = DEMI_DS_NODE_OVF;
-      for (uint32_t i = 1; i < A->n_init_nodes && !status; i++) {
-        const uint4 nd = __ldg(A->init_nodes + i);
+    if (n_init_nodes()) {
+      if (n_init_nodes() > A->P.node_cap) status = DEMI_DS_NODE_OVF;
+      for (uint32_t i = 1; i < n_init_nodes() && !status; i++) {
+        const uint4 nd = __ldg(init_nodes() + i);
         nodes[i] = nd;
         uint32_t s = demi_fmix32((nd.x * 0x9E3779B1u) ^ (nd.y * 0x85EBCA77u) ^ (nd.z * 0xC2B2AE3Du) ^ ((nd.w & 0xFFFFFu) * 0x27D4EB2Fu)) &
                      (A->child_slots - 1);
         while (child_hash[s]) s = (s + 1) & (A->child_slots - 1);
         child_hash[s] = i;
       }
-      if (!status) n_nodes = A->n_init_nodes;
+      if (!status) n_nodes = n_init_nodes();
     }
     for (uint32_t i = ext_lo; i < ext_hi; i++) {
       uint32_t kind = __ldg(A->ext + i).x & 0xFF;
@@ -479,8 +509,8 @@ struct DporMachine : TimerTable<MODEL> {
       if (started && n_heap) {
         if (!analyse(n_traces - 1, R)) next_len = 0;                              // None: run() clears nextTrace :757-759
         R.exhausted = 0;
-      } else if (A->n_init_trace) {
-        next_rd = A->init_trace; next_len = A->n_init_trace;                     // followed whole, however long
+      } else if (n_init_trace()) {
+        next_rd = init_trace(); next_len = n_init_trace();                       // followed whole, however long
       }
       started = true;
       while (!status) {
@@ -515,10 +545,11 @@ struct DporMachine : TimerTable<MODEL> {
   }
 };
 
-template <class MODEL, int BD>
+// MULTI: a multi-trace launch, each search bound to the seed of its own trace (DporSeedSel)
+template <class MODEL, int BD, bool MULTI = false>
 __global__ void __launch_bounds__(BD)
 dpor_kernel(const __grid_constant__ DporArgs args) {
-  using M = DporMachine<MODEL, BD>;
+  using M = DporMachine<MODEL, BD, MULTI>;
   extern __shared__ __align__(16) uint32_t lane_smem[];
   const uint32_t sid = blockIdx.x * BD + threadIdx.x;
   if (sid >= args.n_searches) return;

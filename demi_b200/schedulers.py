@@ -154,6 +154,23 @@ class Engine(object):
                                              ne.ctypes.data, res.ctypes.data))
         return ev, ne, res
 
+    def fuzz_traces_tree(self, seed_base, prefix_index, max_messages, interval, looking_for=0, cap_events=1024,
+                         cap_nodes=1024):
+        """demi_fuzz_traces_tree: fuzz_traces plus each execution's DepTracker tree.  Returns (events [n, cap_events],
+        n_events [n], dep_parent [n, cap_nodes], n_nodes [n], results [n]); row i of dep_parent holds n_nodes[i]
+        entries, what fuzz_trace returns as dep_parent for that seed."""
+        idx = np.ascontiguousarray(prefix_index, dtype=np.uint32)
+        p = N.FuzzParams(seed_base, len(idx), max_messages, interval, looking_for or 0, 0)
+        ev = np.zeros((len(idx), cap_events), dtype=N.EVENT_DTYPE)
+        ne = np.zeros(len(idx), dtype=np.uint32)
+        par = np.zeros((len(idx), cap_nodes), dtype=np.uint16)
+        nn = np.zeros(len(idx), dtype=np.uint32)
+        res = np.zeros(len(idx), dtype=N.RESULT_DTYPE)
+        self._check(N.lib().demi_fuzz_traces_tree(self._h, C.byref(p), idx.ctypes.data, len(idx), ev.ctypes.data,
+                                                  cap_events, ne.ctypes.data, par.ctypes.data, cap_nodes, nn.ctypes.data,
+                                                  res.ctypes.data))
+        return ev, ne, par, nn, res
+
     # ---- provenance pruning (ProvenanceTracker, schedulers/Util.scala:267-376)
     def provenance(self, events, dep_parent, affected_mask, mask_words=None):
         """pruneConcurrentEvents on one recorded execution: (keep mask over initialTrace positions, out record)."""
@@ -538,6 +555,43 @@ class Engine(object):
                                                    max_max_distance, stop_at_size, mcs.ctypes.data, mw, C.byref(out)))
         del alive
         return mcs, out
+
+    def incremental_ddmin_many(self, programs, max_messages, max_interleavings, seeds, looking_for=0, max_max_distance=8,
+                               stop_at_size=6, flags=N.DF_ARVIND_ORDERING | N.DF_PRIORITIZE_PENDING, node_cap=4096,
+                               explored_slots=1 << 16, heap_cap=1 << 15, mask_words=None):
+        """demi_incremental_ddmin_many: incremental_ddmin on every trace t, over programs[t] (or one program for all)
+        from seeds[t] = (events, dep_parent) (seeds None: no trace has a seed), with max_messages[t] and looking_for[t]
+        (a scalar applies to every trace).  Returns (MCS masks [n, mw], INCDDMIN_OUT_DTYPE [n], status [n]); a trace
+        whose status is not OK has no outputs, and the call raises only for call-level errors."""
+        multi = isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind")
+        n = len(programs) if multi else len(seeds)
+        progs = list(programs) if multi else [programs] * n
+        progs = [np.ascontiguousarray(p if isinstance(p, np.ndarray) else pack_externals(p), dtype=N.EXT_DTYPE)
+                 for p in progs]
+        n_ext = np.array([len(p) for p in progs], dtype=np.uint32)
+        ext = np.concatenate(progs + [np.zeros(1, dtype=N.EXT_DTYPE)])
+        eoff = np.zeros(n, dtype=np.uint32)
+        eoff[1:] = np.cumsum(n_ext)[:-1]
+        mm = np.ascontiguousarray(np.broadcast_to(np.asarray(max_messages, dtype=np.int32), (n,)))
+        lf = np.ascontiguousarray(np.broadcast_to(np.asarray(looking_for or 0, dtype=np.uint32), (n,)))
+        P = N.DporParams(0, -1, max_interleavings, 0, 1, node_cap, explored_slots, heap_cap)
+        alive, sd = [], None
+        if seeds is not None:
+            sd = (N.DporSeed * n)()
+            for t, s in enumerate(seeds):
+                sd[t], keep = self._seed(s)
+                alive.append(keep)
+        mw = mask_words or max(1, (int(n_ext.max()) + 63) // 64)
+        mcs = np.zeros((n, mw), dtype=np.uint64)
+        out = np.zeros(n, dtype=N.INCDDMIN_OUT_DTYPE)
+        status = np.zeros(n, dtype=np.int32)
+        self._check(N.lib().demi_incremental_ddmin_many(self._h, n, ext.ctypes.data, eoff.ctypes.data, n_ext.ctypes.data,
+                                                        C.cast(sd, C.c_void_p) if sd is not None else None,
+                                                        mm.ctypes.data, lf.ctypes.data, C.byref(P), flags,
+                                                        max_max_distance, stop_at_size, mcs.ctypes.data, mw,
+                                                        out.ctypes.data, status.ctypes.data))
+        del alive
+        return mcs, out, status
 
     # ---- frontier ("wide") DPOR: one DPORwHeuristics.test explored as a frontier of backtrack points
     @staticmethod
@@ -1012,6 +1066,29 @@ class IncrementalDDMin(object):
         self.last = out
         self._stats.increment_replays(out.total_replays)
         return [e for i, e in enumerate(prog) if (int(mcs[i >> 6]) >> (i & 63)) & 1]
+
+    def minimize_many(self, executions, violation_fingerprint):
+        """minimize() on many violating executions in one call (demi_incremental_ddmin_many).  executions[t] is
+        (program, events, dep_parent, max_messages): the externals to minimise, the recorded execution (events and
+        DepTracker tree) that seeds its DPOR instances, and its setMaxMessagesToSchedule; the oracle's engine,
+        max_interleavings and flags apply to every one.  Returns one
+        MCS per execution, None for one that failed; `last` holds the INCDDMIN_OUT_DTYPE records and `status` the
+        per-execution status."""
+        o = self.oracle
+        progs = [[e for e in x[0] if e.kind in (N.EXT_START, N.EXT_SEND)] for x in executions]
+        mcs, out, status = o.engine.incremental_ddmin_many(
+            progs, [x[3] for x in executions], o.max_interleavings, [(x[1], x[2]) for x in executions],
+            looking_for=violation_fingerprint, max_max_distance=self.maxMaxDistance, stop_at_size=self.stopAtSize,
+            flags=o.flags)
+        self.last, self.status = out, status
+        result = []
+        for t, prog in enumerate(progs):
+            if status[t]:
+                result.append(None)
+                continue
+            self._stats.increment_replays(int(out[t]["total_replays"]))
+            result.append([e for i, e in enumerate(prog) if (int(mcs[t, i >> 6]) >> (i & 63)) & 1])
+        return result
 
     def verify_mcs(self, mcs, violation_fingerprint):
         return self.oracle.test(mcs, violation_fingerprint)

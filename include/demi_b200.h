@@ -380,6 +380,13 @@ int32_t demi_ddmin(demi_handle* h, uint32_t looking_for, uint32_t flags, int32_t
  * as far as the longest successful recording of the call reaches; past n_events[i], row i's content is unspecified. */
 int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, const uint32_t* prefix_index, uint32_t n,
                          demi_event* events, uint32_t cap_events, uint32_t* n_events, demi_fuzz_result* results);
+/* demi_fuzz_traces that also returns each execution's DepTracker tree, the seed demi_incremental_ddmin_many needs:
+ * row i of dep_parent (cap_nodes entries) receives what demi_fuzz_trace returns in dep_parent for that seed, and
+ * n_nodes[i] its node count.  Records, failures and the row contract are demi_fuzz_traces's; a failing execution's
+ * parent row is zero. */
+int32_t demi_fuzz_traces_tree(demi_handle* h, const demi_fuzz_params* p, const uint32_t* prefix_index, uint32_t n,
+                              demi_event* events, uint32_t cap_events, uint32_t* n_events,
+                              uint16_t* dep_parent, uint32_t cap_nodes, uint32_t* n_nodes, demi_fuzz_result* results);
 /* A set of n_traces recorded executions to minimise, separate from the single trace of demi_set_trace (which it leaves
  * as it is).  Trace t is events[event_offsets[t] ..] (n_events[t] records) with the externals
  * externals[ext_offsets[t] ..] (n_externals[t] records); offsets are in elements, so the strided output of
@@ -615,6 +622,27 @@ int32_t demi_incremental_ddmin(demi_handle* h, const demi_ext_event* externals, 
                                const demi_dpor_params* params, uint32_t flags, const demi_dpor_seed* seed,
                                int32_t max_max_distance, uint32_t stop_at_size,
                                uint64_t* mcs_mask, uint32_t mask_words, demi_incddmin_out* out);
+/* demi_incremental_ddmin on each of n_traces violating executions, their DPOR tests in shared launches.  Trace t
+ * minimises externals[ext_offsets[t] ..] (n_externals[t] records; offsets in elements, so one program shared by every
+ * trace, all ext_offsets 0, is taken as it is) from seeds[t] (seeds NULL: no trace has a seed) with its own
+ * setMaxMessagesToSchedule max_messages[t] and ViolationFingerprint looking_for[t]; `params` supplies the other fields
+ * (its max_messages and looking_for are ignored) and is checked as demi_dpor_batch checks it.  status[t] is what
+ * demi_incremental_ddmin(h, trace t's externals, params with max_messages[t] and looking_for[t], flags, &seeds[t],
+ * max_max_distance, stop_at_size, ...) returns, and when it is DEMI_OK, mcs_masks[t*mask_words ..] and out[t] equal that
+ * call's outputs in every field, tests_executed, batches and interleavings_executed included: a trace's speculation
+ * depends on its own memo alone, so the results do not depend on which traces share a launch.  A trace fails alone:
+ * DEMI_ERR_INVALID for an external other than Start / Send or a bad seed, DEMI_ERR_CAPACITY for a DPOR instance status
+ * or a seed larger than node_cap; the call then returns DEMI_OK and demi_last_error names the lowest failing trace.  The
+ * call fails only on invalid arguments or a CUDA error.  The handle's trace and trace set are untouched.
+ * DEMI_DDMIN_MANY_WINDOW bounds the minimisations in flight as it does for demi_ddmin_many.  A round's searches are
+ * split into launches whose per-search buffers fit min(32 GiB, half the device memory free when the call starts), at
+ * least one search each; demi_perf counts every launch. */
+int32_t demi_incremental_ddmin_many(demi_handle* h, uint32_t n_traces,
+                                    const demi_ext_event* externals, const uint32_t* ext_offsets, const uint32_t* n_externals,
+                                    const demi_dpor_seed* seeds, const int32_t* max_messages, const uint32_t* looking_for,
+                                    const demi_dpor_params* params, uint32_t flags, int32_t max_max_distance,
+                                    uint32_t stop_at_size, uint64_t* mcs_masks, uint32_t mask_words,
+                                    demi_incddmin_out* out, int32_t* status);
 
 /* ---------------------------------------------------- frontier ("wide") DPOR */
 /* ONE DPORwHeuristics.test (DPORwHeuristics.scala:1193-1242, dpor() :1020-1185) explored as a frontier of

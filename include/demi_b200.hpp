@@ -200,6 +200,24 @@ class Engine {
     for (size_t i = 0; i < n.size(); i++) out[i].assign(ev.begin() + i * cap_events, ev.begin() + i * cap_events + n[i]);
     return out;
   }
+  // demi_fuzz_traces_tree: fuzz_traces plus each execution's DepTracker tree (fuzz_trace's dep_parent for that seed)
+  std::vector<std::pair<EventTrace, std::vector<uint16_t>>> fuzz_traces_tree(int64_t seed_base, const std::vector<uint32_t>& prefix_index,
+                                                                            int32_t max_messages, int32_t interval, uint32_t looking_for = 0,
+                                                                            uint32_t cap_events = 4096, uint32_t cap_nodes = 4096) {
+    demi_fuzz_params p{seed_base, prefix_index.size(), max_messages, interval, looking_for, 0};
+    const size_t n = prefix_index.size();
+    std::vector<demi_event> ev(n * (size_t)cap_events);
+    std::vector<uint16_t> par(n * (size_t)cap_nodes);
+    std::vector<uint32_t> ne(n), nn(n);
+    check(demi_fuzz_traces_tree(h, &p, prefix_index.data(), (uint32_t)n, ev.data(), cap_events, ne.data(), par.data(), cap_nodes,
+                                nn.data(), nullptr));
+    std::vector<std::pair<EventTrace, std::vector<uint16_t>>> out(n);
+    for (size_t i = 0; i < n; i++) {
+      out[i].first.assign(ev.begin() + i * cap_events, ev.begin() + i * cap_events + ne[i]);
+      out[i].second.assign(par.begin() + i * cap_nodes, par.begin() + i * cap_nodes + std::min(nn[i], cap_nodes));
+    }
+    return out;
+  }
   // demi_set_traces: trace i with externals[i] (or one program shared by all when externals has one entry)
   void set_traces(const std::vector<EventTrace>& traces, const std::vector<ExternalEvents>& externals) {
     const bool shared = externals.size() == 1;
@@ -807,6 +825,43 @@ class IncrementalDDMin {
                                                 &sd, maxMaxDistance, stopAtSize, mcs.data(), (uint32_t)mcs.size(), &last));
     if (stats) stats->increment_replays(last.total_replays);
     return events_of(prog, mcs);
+  }
+  // minimize() on many violating executions in one call (demi_incremental_ddmin_many): execution t is programs[t] recorded
+  // as traces[t] with DepTracker tree trees[t] and setMaxMessagesToSchedule max_messages[t]; the oracle's engine, budget
+  // and flags apply to every one.  status[t] is its return code (a failed execution's MCS is empty), outs[t] its counters.
+  std::vector<ExternalEvents> minimize_many(const std::vector<ExternalEvents>& programs, const std::vector<EventTrace>& traces,
+                                            const std::vector<std::vector<uint16_t>>& trees, const std::vector<int32_t>& max_messages,
+                                            ViolationFingerprint fp, std::vector<int32_t>* status = nullptr,
+                                            std::vector<demi_incddmin_out>* outs = nullptr) {
+    const size_t n = programs.size();
+    ExternalEvents flat; std::vector<uint32_t> off, cnt, lf(n, fp);
+    std::vector<demi_dpor_seed> seeds(n);
+    size_t words = 1;
+    for (size_t t = 0; t < n; t++) {
+      off.push_back((uint32_t)flat.size());
+      uint32_t k = 0;
+      for (const demi_ext_event& e : programs[t]) if (e.kind == DEMI_EXT_START || e.kind == DEMI_EXT_SEND) { flat.push_back(e); k++; }
+      cnt.push_back(k);
+      words = std::max<size_t>(words, (k + 63) / 64);
+      seeds[t] = demi_dpor_seed{traces[t].data(), (uint32_t)traces[t].size(), trees[t].data(), (uint32_t)trees[t].size()};
+    }
+    const demi_dpor_params P = oracle.params(fp);
+    std::vector<uint64_t> mcs(n * words, 0);
+    std::vector<demi_incddmin_out> out(n);
+    std::vector<int32_t> st(n);
+    oracle.engine->check(demi_incremental_ddmin_many(oracle.engine->handle(), (uint32_t)n, flat.data(), off.data(), cnt.data(),
+                                                     seeds.data(), max_messages.data(), lf.data(), &P, oracle.flags_value(),
+                                                     maxMaxDistance, stopAtSize, mcs.data(), (uint32_t)words, out.data(), st.data()));
+    std::vector<ExternalEvents> res(n);
+    for (size_t t = 0; t < n; t++) {
+      if (st[t] != DEMI_OK) continue;
+      if (stats) stats->increment_replays(out[t].total_replays);
+      ExternalEvents prog(flat.begin() + off[t], flat.begin() + off[t] + cnt[t]);
+      res[t] = events_of(prog, std::vector<uint64_t>(mcs.begin() + t * words, mcs.begin() + (t + 1) * words));
+    }
+    if (status) *status = st;
+    if (outs) *outs = out;
+    return res;
   }
   bool verify_mcs(const ExternalEvents& mcs, ViolationFingerprint fp) { return oracle.test(mcs, fp); }
   demi_incddmin_out last{};

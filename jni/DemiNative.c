@@ -7,6 +7,7 @@
  * are made on the Java side; handles travel as jlong.
  * Scala side: jni/DemiNative.scala.
  */
+#include <stdlib.h>
 #include <jni.h>
 #include <stdint.h>
 #include "demi_b200.h"
@@ -113,6 +114,34 @@ JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_incrementalDdm
                                 (uint32_t)stopAtSize, (uint64_t*)BUF(env, mcsMask), (uint32_t)maskWords,
                                 (demi_incddmin_out*)BUF(env, out));
 }
+/* demi_incremental_ddmin_many: seed t's events are seedEvents[seedEventOffsets[t] ..] (nSeedEvents[t] records) and its
+ * DepTracker tree seedParents[seedParentOffsets[t] ..] (nSeedNodes[t] entries); seedEvents null: no trace has a seed */
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_incrementalDdminMany(JNIEnv* env, jclass c, jlong h, jint nTraces,
+    jobject externals, jobject extOffsets, jobject nExternals, jobject seedEvents, jobject seedEventOffsets, jobject nSeedEvents,
+    jobject seedParents, jobject seedParentOffsets, jobject nSeedNodes, jobject maxMessages, jobject lookingFor, jobject params,
+    jint flags, jint maxMaxDistance, jint stopAtSize, jobject mcsMasks, jint maskWords, jobject out, jobject status) {
+  demi_dpor_seed* seeds = 0;
+  if (seedEvents && nTraces > 0) {
+    const demi_event* ev = (const demi_event*)BUF(env, seedEvents);
+    const uint16_t* par = (const uint16_t*)BUF(env, seedParents);
+    const uint32_t* eo = (const uint32_t*)BUF(env, seedEventOffsets); const uint32_t* ne = (const uint32_t*)BUF(env, nSeedEvents);
+    const uint32_t* po = (const uint32_t*)BUF(env, seedParentOffsets); const uint32_t* nn = (const uint32_t*)BUF(env, nSeedNodes);
+    seeds = (demi_dpor_seed*)malloc((size_t)nTraces * sizeof(demi_dpor_seed));
+    if (!seeds) return DEMI_ERR_CAPACITY;
+    for (jint t = 0; t < nTraces; t++) {
+      seeds[t].events = ev + eo[t]; seeds[t].n_events = ne[t];
+      seeds[t].dep_parent = par + po[t]; seeds[t].n_nodes = nn[t];
+    }
+  }
+  const int32_t rc = demi_incremental_ddmin_many(H(h), (uint32_t)nTraces, (const demi_ext_event*)BUF(env, externals),
+                                                 (const uint32_t*)BUF(env, extOffsets), (const uint32_t*)BUF(env, nExternals), seeds,
+                                                 (const int32_t*)BUF(env, maxMessages), (const uint32_t*)BUF(env, lookingFor),
+                                                 (const demi_dpor_params*)BUF(env, params), (uint32_t)flags, maxMaxDistance,
+                                                 (uint32_t)stopAtSize, (uint64_t*)BUF(env, mcsMasks), (uint32_t)maskWords,
+                                                 (demi_incddmin_out*)BUF(env, out), (int32_t*)BUF(env, status));
+  free(seeds);
+  return rc;
+}
 JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_provenance(JNIEnv* env, jclass c, jlong h, jobject events, jint nEvents,
     jobject depParent, jint nNodes, jint affectedMask, jobject keepMask, jint maskWords, jobject out) {
   return demi_provenance(H(h), (const demi_event*)BUF(env, events), (uint32_t)nEvents, (const uint16_t*)BUF(env, depParent),
@@ -211,6 +240,14 @@ JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_fuzzTraces(JNI
   return demi_fuzz_traces(H(h), (const demi_fuzz_params*)BUF(env, params), (const uint32_t*)BUF(env, prefixIndex), (uint32_t)n,
                           (demi_event*)BUF(env, events), (uint32_t)capEvents, (uint32_t*)BUF(env, nEvents),
                           results ? (demi_fuzz_result*)BUF(env, results) : 0);
+}
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_fuzzTracesTree(JNIEnv* env, jclass c, jlong h, jobject params,
+    jobject prefixIndex, jint n, jobject events, jint capEvents, jobject nEvents, jobject depParent, jint capNodes, jobject nNodes,
+    jobject results) {
+  return demi_fuzz_traces_tree(H(h), (const demi_fuzz_params*)BUF(env, params), (const uint32_t*)BUF(env, prefixIndex), (uint32_t)n,
+                               (demi_event*)BUF(env, events), (uint32_t)capEvents, (uint32_t*)BUF(env, nEvents),
+                               (uint16_t*)BUF(env, depParent), (uint32_t)capNodes, (uint32_t*)BUF(env, nNodes),
+                               results ? (demi_fuzz_result*)BUF(env, results) : 0);
 }
 JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_setTraces(JNIEnv* env, jclass c, jlong h, jint nTraces,
     jobject events, jobject eventOffsets, jobject nEvents, jobject externals, jobject extOffsets, jobject nExternals) {

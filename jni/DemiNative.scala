@@ -78,6 +78,17 @@ object DemiNative {
   /** demi_fuzz_traces: the EventTraces of executions seed_base + prefixIndex(i), execution i at events + i*capEvents */
   @native def fuzzTraces(h: Long, params: ByteBuffer, prefixIndex: ByteBuffer, n: Int, events: ByteBuffer, capEvents: Int,
                          nEvents: ByteBuffer, results: ByteBuffer): Int
+  /** demi_fuzz_traces_tree: fuzzTraces plus each execution's DepTracker tree, execution i's at depParent + i*capNodes */
+  @native def fuzzTracesTree(h: Long, params: ByteBuffer, prefixIndex: ByteBuffer, n: Int, events: ByteBuffer, capEvents: Int,
+                             nEvents: ByteBuffer, depParent: ByteBuffer, capNodes: Int, nNodes: ByteBuffer, results: ByteBuffer): Int
+  /** demi_incremental_ddmin_many: RunnerUtils.editDistanceDporDDMin's minimisation of every trace t (offsets in elements;
+    * seed t = seedEvents/seedParents at its offsets, seedEvents null: no seeds); status(t) is that trace's return code */
+  @native def incrementalDdminMany(h: Long, nTraces: Int, externals: ByteBuffer, extOffsets: ByteBuffer, nExternals: ByteBuffer,
+                                   seedEvents: ByteBuffer, seedEventOffsets: ByteBuffer, nSeedEvents: ByteBuffer,
+                                   seedParents: ByteBuffer, seedParentOffsets: ByteBuffer, nSeedNodes: ByteBuffer,
+                                   maxMessages: ByteBuffer, lookingFor: ByteBuffer, params: ByteBuffer, flags: Int,
+                                   maxMaxDistance: Int, stopAtSize: Int, mcsMasks: ByteBuffer, maskWords: Int, out: ByteBuffer,
+                                   status: ByteBuffer): Int
   /** demi_set_traces: a set of traces to minimise (offsets in elements), separate from setTrace's single trace */
   @native def setTraces(h: Long, nTraces: Int, events: ByteBuffer, eventOffsets: ByteBuffer, nEvents: ByteBuffer,
                         externals: ByteBuffer, extOffsets: ByteBuffer, nExternals: ByteBuffer): Int
