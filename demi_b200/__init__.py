@@ -8,4 +8,5 @@ from .schedulers import (DemiError, SchedulerConfig, Engine, RandomScheduler, ST
                          ProvenanceTracker, ResumableDPOR, IncrementalDDMin, ArvindDistanceOrdering,
                          DefaultBacktrackOrdering, mask_of, events_of,
                          WildcardMinimizer, BackTrackStrategy, LastOnlyStrategy, TestScheduler, ClusteringStrategy,
-                         raft5_clock_rules, fuzz, FuzzFound, PROGRAM_SEED_OFFSET, randomDDMin)
+                         raft5_clock_rules, fuzz, FuzzFound, PROGRAM_SEED_OFFSET, randomDDMin,
+                         randomDDMin_many)

@@ -140,6 +140,7 @@ EXPORTS = [
     "demi_fuzz_traces", "demi_set_traces", "demi_replay_batch_many", "demi_ddmin_many",
     "demi_replay_traces_many", "demi_internal_minimize_many", "demi_wildcard_replay_batch_many",
     "demi_wildcard_minimize_many", "demi_incremental_ddmin_many", "demi_fuzz_traces_tree",
+    "demi_random_test_batch_many", "demi_random_ddmin_many",
 ]
 FILTER_RULE_DTYPE = np.dtype([("src_mask", "<u4"), ("dst_mask", "<u4"), ("type_mask", "<u4"), ("flags", "<u4")])
 FRULE_DEADLETTERS = 1
@@ -165,7 +166,9 @@ class RandomDDMinOut(C.Structure):
                 ("batches", C.c_uint32), ("mcs_first_hit", C.c_int32), ("reserved", C.c_uint32)]
 
 
-assert RANDOM_TEST_DTYPE.itemsize == 16 and C.sizeof(RandomDDMinOut) == 48
+# RandomDDMinOut as an array element (demi_random_ddmin_many)
+RANDOM_DDMIN_OUT_DTYPE = np.dtype([(f, {C.c_uint32: "<u4", C.c_uint64: "<u8", C.c_int32: "<i4"}[t]) for f, t in RandomDDMinOut._fields_])
+assert RANDOM_TEST_DTYPE.itemsize == 16 and C.sizeof(RandomDDMinOut) == 48 and RANDOM_DDMIN_OUT_DTYPE.itemsize == 48
 
 
 def fuzzer_generate(cfg, seed, prefix, postfix=None):
@@ -324,6 +327,12 @@ def lib():
     L.demi_random_ddmin.restype = C.c_int32
     L.demi_random_ddmin.argtypes = [vp, C.POINTER(FuzzParams), C.c_int32, vp, C.c_uint32, vp, vp, C.c_uint32,
                                     C.POINTER(RandomDDMinOut)]
+    L.demi_random_test_batch_many.restype = C.c_int32
+    L.demi_random_test_batch_many.argtypes = [vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, C.c_uint32,
+                                              C.POINTER(FuzzParams), vp]
+    L.demi_random_ddmin_many.restype = C.c_int32
+    L.demi_random_ddmin_many.argtypes = [vp, C.c_uint32, vp, vp, vp, vp, vp, vp, C.POINTER(FuzzParams), C.c_int32, vp,
+                                         C.c_uint32, vp, vp, C.c_uint32, vp, vp]
     L.demi_random_test_trace.restype = C.c_int32
     L.demi_random_test_trace.argtypes = [vp, vp, C.c_uint32, C.POINTER(FuzzParams), C.c_int64, vp, C.c_uint32,
                                          C.POINTER(C.c_uint32), vp]

@@ -27,9 +27,10 @@ thread_local std::string g_create_error;
 constexpr int WARPS = 4;
 typedef void (*kernel_fn)(const KernelArgs);
 // What a fuzz launch runs: a batch of prefixes over the handle's program, the recording of chosen prefixes
-// (provenance, traces), a campaign's generated programs (PROG), or random-oracle tests over subsequences (PROG + TESTS).
-// Both engines have one instantiation per mode.
-enum LaunchMode { LM_BATCH, LM_RECORD, LM_PROGRAM, LM_TESTS, LM_COUNT };
+// (provenance, traces), a campaign's generated programs (PROG), random-oracle tests over subsequences (PROG + TESTS),
+// or random-oracle tests of many traces, each with its own parameters (PROG + TESTS + PARAMS).  Both engines have one
+// instantiation per mode.
+enum LaunchMode { LM_BATCH, LM_RECORD, LM_PROGRAM, LM_TESTS, LM_TEST_PARAMS, LM_COUNT };
 struct Variant {
   int model; uint32_t pcap, tcap; bool pend_global;
   size_t smem_per_warp;
@@ -41,7 +42,8 @@ static Variant make_variant() {
   Variant v{MODEL::ID, (uint32_t)PCAP, (uint32_t)TCAP, PG, sizeof(typename M::Smem),
             {fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS>, nullptr,
              REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC>,
-             REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC, !REC>}};
+             REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC, !REC>,
+             REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC, !REC, !REC>}};
   if (REC) std::swap(v.fn[LM_BATCH], v.fn[LM_RECORD]);
   return v;
 }
@@ -86,7 +88,8 @@ static LaneVariant make_lane_variant() {
   using S = LaneMachine<MODEL, BD, LPCAP, false, true>;
   return LaneVariant{MODEL::ID, BD, (uint32_t)LPCAP, (size_t)M::WORDS * BD * sizeof(uint32_t),
                      {fuzz_lane_kernel<MODEL, BD, LPCAP>, fuzz_lane_kernel<MODEL, BD, LPCAP, true>,
-                      fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>, fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true>},
+                      fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>, fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true>,
+                      fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true, false, true>},
                      fuzz_lane_kernel<MODEL, BD, LPCAP, false, false, false, true>, (size_t)S::WORDS * BD * sizeof(uint32_t),
                      lane_snapshot_kernel<MODEL>, lane_tree_kernel<MODEL, LPCAP>, S::NODE_WORDS * 4u, (uint32_t)MODEL::LANE_OUTBOX};
 }
@@ -325,15 +328,18 @@ static const LaneVariant* pick_lane_variant(const demi_handle* h, const ProgramI
 struct LaunchPlan { const Variant* v; LaunchMode mode; const ProgramInfo* prog; int grid; size_t smem; KernelArgs args; };
 
 // A launch of `mode` over the program (ext, n_ext) that `prog` describes.  A campaign has no one program: `prog` is
-// its Fuzzer's, sized for the largest program, and each execution binds its own events.
+// its Fuzzer's, sized for the largest program, and each execution binds its own events.  Nor has a launch of many
+// traces' tests: `prog` joins its base programs, and `pcap_at_least` is the largest of their pending capacities,
+// each under its own max_messages.
 static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, LaunchMode mode, const ProgramInfo& prog,
-                           const demi_ext_event* ext, uint32_t n_ext, LaunchPlan* plan) {
+                           const demi_ext_event* ext, uint32_t n_ext, LaunchPlan* plan, uint32_t pcap_at_least = 0) {
   if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
   if (mode == LM_PROGRAM && !h->has_fuzzer) return fail(h, DEMI_ERR_STATE, "demi_set_fuzzer has not been called");
-  if (mode != LM_PROGRAM && h->ext_host.empty()) return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
+  if (mode != LM_PROGRAM && mode != LM_TEST_PARAMS && h->ext_host.empty())
+    return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
   if (p->n_prefixes > 0xFFFFFFFFull) return fail(h, DEMI_ERR_INVALID, "n_prefixes > 2^32-1 per call");
   { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
-  const uint32_t pcap = demi_pending_cap(demi_model_key(h), p->max_messages, prog.sends);
+  const uint32_t pcap = std::max(pcap_at_least, demi_pending_cap(demi_model_key(h), p->max_messages, prog.sends));
   const uint32_t tcap = demi_tosend_cap(prog.sends);
   const bool fifo = h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;          // SrcDstFIFO lives in the HBM-pending variants
   // so does every program with a HardKill: Machine::hard_kill needs room for n_pending + matches <= 2 * pcap entries,
@@ -466,7 +472,8 @@ static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, c
     CUDA_TRY(h, cudaMemsetAsync(h->ovf_count.get(), 0, sizeof(uint32_t), s));
     KernelArgs la = a;
     la.lane_pend = h->lane_pend.get<uint4>();
-    la.ext_sends = plan.mode == LM_PROGRAM ? nullptr : h->ext_sends_dev.get<uint4>();     // a campaign binds each program's table
+    // a campaign and a launch of many traces' tests bind each program's table
+    la.ext_sends = plan.mode == LM_PROGRAM || plan.mode == LM_TEST_PARAMS ? nullptr : h->ext_sends_dev.get<uint4>();
     la.has_partitions = plan.prog->partitions ? 1u : 0u;
     la.prog_lane_pcap = h->lane_pending_cap;
     la.ovf_list = h->ovf_list.get<uint32_t>(); la.ovf_count = h->ovf_count.get<uint32_t>();
@@ -1102,13 +1109,8 @@ extern "C" int32_t demi_fuzz_campaign(demi_handle* h, const demi_fuzz_params* p,
 // One warp per test: the subsequence of the base program that the test's mask keeps, compacted (ballot + prefix sum)
 // into the arena layout of the campaigns: events[t * stride ..), hdr[t] = {length, Sends}, the lane-form Sends at
 // sends[t * send_stride ..).
-__global__ void __launch_bounds__(128)
-random_subseq_kernel(const demi_ext_event* base, uint32_t n_ext, const uint64_t* masks, uint32_t mask_words, uint32_t n_tests,
-                     demi_ext_event* events, uint32_t stride, uint2* hdr, uint4* sends, uint32_t send_stride) {
-  const uint32_t lane = threadIdx.x & 31;
-  const uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (t >= n_tests) return;
-  const uint64_t* mask = masks + t * mask_words;
+__device__ __forceinline__ void subseq_warp(const demi_ext_event* base, uint32_t n_ext, const uint64_t* mask, uint64_t t, uint32_t lane,
+                                            demi_ext_event* events, uint32_t stride, uint2* hdr, uint4* sends, uint32_t send_stride) {
   const uint32_t below = (1u << lane) - 1u;
   uint32_t len = 0, ns = 0;
   for (uint32_t b = 0; b < n_ext; b += 32) {
@@ -1124,11 +1126,33 @@ random_subseq_kernel(const demi_ext_event* base, uint32_t n_ext, const uint64_t*
   }
   if (lane == 0) hdr[t] = make_uint2(len, ns);
 }
+__global__ void __launch_bounds__(128)
+random_subseq_kernel(const demi_ext_event* base, uint32_t n_ext, const uint64_t* masks, uint32_t mask_words, uint32_t n_tests,
+                     demi_ext_event* events, uint32_t stride, uint2* hdr, uint4* sends, uint32_t send_stride) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (t >= n_tests) return;
+  subseq_warp(base, n_ext, masks + t * mask_words, t, lane, events, stride, hdr, sends, send_stride);
+}
+// The same over many base programs: test t keeps bits of program trace_of_test[t], which is
+// progs[prog_tab[trace].x ..), prog_tab[trace].y events long.
+__global__ void __launch_bounds__(128)
+random_subseq_many_kernel(const demi_ext_event* progs, const uint2* prog_tab, const uint32_t* trace_of_test, const uint64_t* masks,
+                          uint32_t mask_words, uint32_t n_tests, demi_ext_event* events, uint32_t stride, uint2* hdr, uint4* sends,
+                          uint32_t send_stride) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (t >= n_tests) return;
+  const uint2 pt = prog_tab[trace_of_test[t]];
+  subseq_warp(progs + pt.x, pt.y, masks + t * mask_words, t, lane, events, stride, hdr, sends, send_stride);
+}
 
-// One warp per test over its N execution records: the test record, and the executions that ran (not skipped).
+// One warp per test over its N execution records: the test record, and the executions that ran (not skipped), summed
+// into *executed and, with PER_TEST, also written per test to ran[t].
+template <bool PER_TEST>
 __global__ void __launch_bounds__(128)
 random_test_reduce_kernel(const demi_fuzz_result* res, uint32_t n_tests, uint32_t n_execs, demi_random_test_result* out,
-                          unsigned long long* executed) {
+                          unsigned long long* executed, uint32_t* ran_of_test) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (t >= n_tests) return;
@@ -1153,6 +1177,7 @@ random_test_reduce_kernel(const demi_fuzz_result* res, uint32_t n_tests, uint32_
   if (lane == 0) {
     out[t] = demi_random_test_result{first, first >= 0 ? (uint32_t)first + 1 : n_execs, violation, (uint16_t)status, 0};
     atomicAdd(executed, (unsigned long long)ran);
+    if constexpr (PER_TEST) ran_of_test[t] = ran;
   }
 }
 
@@ -1215,7 +1240,7 @@ static int32_t random_tests(demi_handle* h, const uint64_t* masks, uint32_t n_te
     a.prog_execs = N;
     a.prog_first_hit = first_hit;
     if ((rc = launch_plan(h, plan, q.n_prefixes, s)) != DEMI_OK) return rc;
-    random_test_reduce_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(results, m, N, odev, cnt);
+    random_test_reduce_kernel<false><<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(results, m, N, odev, cnt, nullptr);
     CUDA_TRY(h, cudaGetLastError());
     h->perf.kernel_launches++;
     CUDA_TRY(h, cudaMemcpyAsync(out + off, odev, (size_t)m * sizeof(demi_random_test_result), cudaMemcpyDeviceToHost, s));
@@ -1272,32 +1297,15 @@ extern "C" int32_t demi_random_test_trace(demi_handle* h, const uint64_t* mask, 
   return fuzz_trace(h, p, seed, events, cap_events, n_events, nullptr, 0, nullptr, result, dev.get<demi_ext_event>(), (uint32_t)sub.size(), info);
 }
 
-#include "ddmin_driver.hpp"
+#include "random_ddmin_driver.hpp"
+#include "many_rendezvous.hpp"
 namespace {
 
-// RandomScheduler as DDMin's TestOracle: a speculative batch of masks = one demi_random_test_batch
-struct RandomDDMinDriver : DDMinDriver {
+// the handle's program: a speculative batch of masks = one demi_random_test_batch
+struct HandleRandomDriver : RandomDDMinDriver {
   demi_fuzz_params p{};
-  std::map<Mask, demi_random_test_result> records;
-  std::vector<uint32_t> consumed_runs;      // executions_run of each test the sequential walk consumed, in order
-  uint64_t executions_executed = 0;
-  int32_t evaluate(const uint64_t* masks, size_t n, signed char* out) override {
-    std::vector<demi_random_test_result> res(n);
-    uint64_t executed = 0;
-    int32_t rc = random_tests(h, masks, (uint32_t)n, mw, &p, res.data(), &executed);
-    if (rc != DEMI_OK) return rc;
-    executions_executed += executed;
-    for (size_t i = 0; i < n; i++) {
-      records[Mask(masks + i * mw, masks + (i + 1) * mw)] = res[i];
-      out[i] = res[i].status == 0 && res[i].first_hit >= 0;
-    }
-    return DEMI_OK;
-  }
-  // a test's status fails the call only here, where the sequential walk uses its result
-  void consumed(const Mask& m) override {
-    const demi_random_test_result& r = records.at(m);
-    if (r.status) { error = fail(h, DEMI_ERR_CAPACITY, "demi_random_ddmin: a test execution reported status %u", (unsigned)r.status); return; }
-    consumed_runs.push_back(r.executions_run);
+  int32_t run_tests(const uint64_t* masks, size_t n, demi_random_test_result* res, uint64_t* executed) override {
+    return random_tests(h, masks, (uint32_t)n, mw, &p, res, executed);
   }
 };
 
@@ -1311,65 +1319,308 @@ extern "C" int32_t demi_random_ddmin(demi_handle* h, const demi_fuzz_params* p, 
   int32_t rc = check_random(h, "demi_random_ddmin", mask_words, p);
   if (rc != DEMI_OK) return rc;
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
-  memset(out, 0, sizeof(*out));
-  const uint32_t n_ext = (uint32_t)h->ext_host.size();
-  RandomDDMinDriver d;
-  d.h = h; d.p = *p; d.looking_for = p->looking_for; d.mw = mask_words; d.n_ext = n_ext;
+  HandleRandomDriver d;
+  d.h = h; d.p = *p; d.looking_for = p->looking_for; d.mw = mask_words; d.n_ext = (uint32_t)h->ext_host.size();
   d.ext = h->ext_host.data();
-  // tests per speculative batch, sized by executions per launch: about 2^20 executions (a few milliseconds of the lane
-  // engine on raft5-sized programs, so the launch latency is amortised), and never more than the 6000 tests of the
-  // replay path (beyond that the host's batch building costs more than the launch)
-  d.wide_cap = std::max<size_t>(16, std::min<size_t>(6000, ((size_t)1 << 20) / p->n_prefixes));
-  if (getenv("DEMI_DDMIN_WIDE")) d.wide_cap = (size_t)atol(getenv("DEMI_DDMIN_WIDE"));
-  // DDMin.minimize's dag is the whole program, WaitQuiescence included (UnmodifiedEventDag, Minimizer.scala:15-20)
-  Mask dag(mask_words, 0), zero(mask_words, 0);
-  for (uint32_t i = 0; i < n_ext; i++) DDMinDriver::setbit(dag, i);
-  if (check_unmodified) {                                                 // DeltaDebugging.scala:41-47
-    bool v = d.test(dag, dag, zero);
-    if (d.error != DEMI_OK) return d.error;
-    if (!v) return fail(h, DEMI_ERR_INVALID, "Unmodified trace does not trigger violation");
-    d.consumed_runs.clear();                                              // _stats.reset() (:48)
-  }
-  d.original_num_events = n_ext;
-  Mask mcs = d.ddmin2(dag, zero);
-  if (d.error != DEMI_OK) return d.error;
-  d.iteration_sizes.push_back(d.original_num_events - d.total_inputs_pruned);     // fencepost :60
-  if (d.original_num_events - d.total_inputs_pruned != DDMinDriver::popcount(mcs))
-    return fail(h, DEMI_ERR_STATE, "demi_random_ddmin: bookkeeping assertion failed (DeltaDebugging.scala:58)");
-  const uint32_t tests = (uint32_t)d.consumed_runs.size();
-  std::vector<uint64_t> keys;
-  uint64_t total = 0;
-  for (uint32_t r : d.consumed_runs) { total += r; keys.push_back(total); }
-  keys.push_back(total);                                                  // the fencepost's key
-  out->mcs_size = DDMinDriver::popcount(mcs);
-  bool verified = true;                                                   // nothing pruned: the original trace stands
-  out->mcs_first_hit = -1;
-  if (out->mcs_size < n_ext) {                                            // verify_mcs (RunnerUtils.scala:612-620)
-    // the MCS's own test alone: taken from the tests already run, else evaluated by itself (no speculation below it)
-    auto it = d.records.find(mcs);
-    if (it == d.records.end()) {
-      signed char v;
-      if ((rc = d.evaluate(mcs.data(), 1, &v)) != DEMI_OK) return rc;
-      d.replays_executed++;
-      it = d.records.find(mcs);
+  d.set_width(p->n_prefixes);
+  return d.minimize(check_unmodified != 0, mcs_mask, iteration_sizes, iteration_keys, cap, out);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Random-oracle tests and randomDDMin over many traces: each trace has its own program, seed base, max_messages and
+// looking_for; the tests of every trace share launches of the PROG + TESTS + PARAMS engines.
+namespace {
+
+// A call's traces: their programs (the caller's externals, uploaded once), what each program's launches need, and what
+// a trace fails with before any launch.
+struct RandomSet {
+  const demi_handle* h = nullptr;              // the call's handle: the configuration every trace runs under
+  uint32_t n = 0, mask_words = 0;
+  const uint32_t* n_externals = nullptr;
+  const int64_t* seed_base = nullptr; const int32_t* max_messages = nullptr; const uint32_t* looking_for = nullptr;
+  demi_fuzz_params p{};                        // N, interval and flags
+  std::vector<ProgramInfo> info;
+  std::vector<int32_t> pre; std::vector<std::string> pre_msg;
+  DevBuf dev;                                  // the externals, then uint2 {offset, length} per trace
+  const demi_ext_event* progs = nullptr; const uint2* tab = nullptr;
+};
+
+// The checks demi_set_externals and demi_random_test_batch make of trace t's program before a launch; the call-wide
+// ones (N, mask_words) are the caller's.  The programs and their table are uploaded once.
+int32_t random_set(demi_handle* h, uint32_t n, const demi_ext_event* externals, const uint32_t* ext_offsets, const uint32_t* n_externals,
+                   const int64_t* seed_base, const int32_t* max_messages, const uint32_t* looking_for, const demi_fuzz_params* p,
+                   RandomSet& rs) {
+  rs.h = h; rs.n = n; rs.n_externals = n_externals; rs.seed_base = seed_base; rs.max_messages = max_messages; rs.looking_for = looking_for;
+  rs.p = *p;
+  rs.info.assign(n, ProgramInfo{}); rs.pre.assign(n, DEMI_OK); rs.pre_msg.assign(n, std::string());
+  uint64_t span = 0;
+  std::vector<uint2> tab(n);
+  demi_handle eh;
+  for (uint32_t t = 0; t < n; t++) {
+    const demi_ext_event* ev = externals + ext_offsets[t];
+    std::vector<uint4> sv;
+    int32_t rc = DEMI_OK;
+    eh.err.clear();
+    eh.cfg = h->cfg; eh.ir_n_actors = h->ir_n_actors;            // demi_model_actors reads these
+    for (uint32_t i = 0; i < n_externals[t] && rc == DEMI_OK; i++) {
+      rc = demi_check_external(&eh, "demi_set_externals", "", ev, i, true, true);
+      if (rc == DEMI_OK) describe_event(&rs.info[t], &sv, ev[i]);
     }
-    const demi_random_test_result& r = it->second;
-    if (r.status) return fail(h, DEMI_ERR_CAPACITY, "demi_random_ddmin: the MCS's test reported status %u", (unsigned)r.status);
-    verified = r.first_hit >= 0;
-    out->mcs_first_hit = r.first_hit;
+    if (rc == DEMI_OK && !n_externals[t]) rc = fail(&eh, DEMI_ERR_STATE, "demi_set_externals has not been called");
+    if (rc != DEMI_OK) { rs.pre[t] = rc; rs.pre_msg[t] = eh.err; continue; }
+    tab[t] = make_uint2(ext_offsets[t], n_externals[t]);
+    span = std::max<uint64_t>(span, (uint64_t)ext_offsets[t] + n_externals[t]);
   }
-  std::copy(mcs.begin(), mcs.end(), mcs_mask);
-  out->tests = tests;
-  out->total_replays = total;
-  out->n_iterations = (uint32_t)d.iteration_sizes.size();
-  out->executions_executed = d.executions_executed;
-  out->tests_evaluated = d.replays_executed;
-  out->batches = d.batches;
-  out->verified = verified ? 1u : 0u;
-  for (uint32_t i = 0; i < cap && i < out->n_iterations; i++) {
-    if (iteration_sizes) iteration_sizes[i] = d.iteration_sizes[i];
-    if (iteration_keys) iteration_keys[i] = keys[i];
+  const size_t b_ev = ((size_t)span * sizeof(demi_ext_event) + 15) & ~(size_t)15;
+  int32_t rc = rs.dev.grow(h, b_ev + (size_t)n * sizeof(uint2));
+  if (rc != DEMI_OK) return rc;
+  if (span) CUDA_TRY(h, cudaMemcpy(rs.dev.get(), externals, (size_t)span * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
+  CUDA_TRY(h, cudaMemcpy(rs.dev.get<char>() + b_ev, tab.data(), (size_t)n * sizeof(uint2), cudaMemcpyHostToDevice));
+  rs.progs = rs.dev.get<demi_ext_event>(); rs.tab = (const uint2*)(rs.dev.get<char>() + b_ev);
+  return DEMI_OK;
+}
+
+// trace t's pending capacity under its own max_messages (demi_random_test_batch's, from its base program)
+uint32_t random_pcap(const RandomSet& rs, uint32_t t) {
+  return demi_pending_cap(demi_model_key(rs.h), rs.max_messages[t], rs.info[t].sends);
+}
+
+// What plan_launch refuses of a launch over trace t's program alone, in its order; the message goes to `h` (a driver's
+// own handle, or the call's).
+int32_t random_trace_launchable(demi_handle* h, const RandomSet& rs, uint32_t t) {
+  const bool fifo = rs.h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;
+  const uint32_t pcap = random_pcap(rs, t), tcap = demi_tosend_cap(rs.info[t].sends);
+  if (!pick_variant(rs.h->cfg.model, LM_TEST_PARAMS, pcap, tcap, fifo || rs.info[t].hard_kill))
+    return fail(h, DEMI_ERR_CAPACITY, "no kernel variant for pending_cap=%u tosend_cap=%u", pcap, tcap);
+  if (fifo && (rs.info[t].hard_kill || !rs.h->filter.empty()))
+    return fail(h, DEMI_ERR_INVALID, "HardKill and userDefinedFilter are offered for FullyRandom only");
+  return DEMI_OK;
+}
+
+// A test's record and the executions of it that ran
+struct RandomRec { demi_random_test_result rec; uint32_t ran; };
+
+// n tests: test i is masks[i * mask_words ..) over the program of trace tr[i], which random_trace_launchable accepts.
+// The tests go out in at most two groups, the programs the lane engine takes and the others (so that one HardKill
+// program does not send every test to the warp engine), each cut into launches of at most RANDOM_EXECS_PER_LAUNCH
+// executions and a 512 MB arena whose stride is the launch's largest program.
+int32_t random_tests_many(demi_handle* h, const RandomSet& rs, const uint32_t* tr, const uint64_t* masks, size_t n, RandomRec* out) {
+  const uint32_t N = (uint32_t)rs.p.n_prefixes, mw = rs.mask_words;
+  std::vector<size_t> group[2];
+  for (size_t i = 0; i < n; i++) group[pick_lane_variant(h, rs.info[tr[i]]) ? 0 : 1].push_back(i);
+  cudaStream_t s = h->stream;
+  std::vector<uint64_t> hm;
+  std::vector<uint4> hp;
+  std::vector<uint32_t> ht, hran;
+  std::vector<demi_random_test_result> hrec;
+  for (const std::vector<size_t>& g : group) {
+    for (size_t lo = 0; lo < g.size();) {
+      uint32_t stride = 1, send_stride = 1, pcap = 0;
+      ProgramInfo li;
+      size_t hi = lo;
+      for (; hi < g.size(); hi++) {
+        const uint32_t t = tr[g[hi]];
+        const uint32_t st = std::max(stride, rs.n_externals[t]), ss = std::max(send_stride, rs.info[t].sends);
+        const uint64_t per_test = (uint64_t)st * sizeof(demi_ext_event) + sizeof(uint2) + (uint64_t)ss * sizeof(uint4) +
+                                  (uint64_t)mw * 8 + sizeof(demi_random_test_result) + 4 + 4 + sizeof(uint4) + 4;
+        const uint64_t m = hi - lo + 1;
+        if (hi > lo && (m * N > RANDOM_EXECS_PER_LAUNCH || m * per_test > ((uint64_t)512 << 20))) break;
+        stride = st; send_stride = ss;
+        pcap = std::max(pcap, random_pcap(rs, t));
+        li.sends = std::max(li.sends, rs.info[t].sends);
+        li.hard_kill |= rs.info[t].hard_kill; li.partitions |= rs.info[t].partitions;
+        li.sends_distinct &= rs.info[t].sends_distinct;
+      }
+      const uint32_t m = (uint32_t)(hi - lo);
+      // arena: the programs | masks | first_hit | test records | executions that ran | parameters | traces | counter
+      auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
+      const size_t b_mask = al((size_t)m * mw * 8), b_fh = al((size_t)m * 4), b_out = al((size_t)m * sizeof(demi_random_test_result)),
+                   b_ran = al((size_t)m * 4), b_par = al((size_t)m * sizeof(uint4)), b_tr = al((size_t)m * 4);
+      ProgramArena pa;
+      unsigned char* rest;
+      int32_t rc = carve_programs(h, m, stride, send_stride, b_mask + b_fh + b_out + b_ran + b_par + b_tr + 16, &pa, &rest);
+      if (rc != DEMI_OK) return rc;
+      if ((rc = h->results_dev.grow(h, std::max<size_t>((size_t)m * N * sizeof(demi_fuzz_result), 32))) != DEMI_OK) return rc;
+      uint64_t* mdev = (uint64_t*)rest;
+      uint32_t* first_hit = (uint32_t*)(rest + b_mask);
+      demi_random_test_result* odev = (demi_random_test_result*)(rest + b_mask + b_fh);
+      uint32_t* rdev = (uint32_t*)(rest + b_mask + b_fh + b_out);
+      uint4* pdev = (uint4*)(rest + b_mask + b_fh + b_out + b_ran);
+      uint32_t* tdev = (uint32_t*)(rest + b_mask + b_fh + b_out + b_ran + b_par);
+      unsigned long long* cnt = (unsigned long long*)(rest + b_mask + b_fh + b_out + b_ran + b_par + b_tr);
+      hm.resize((size_t)m * mw); hp.resize(m); ht.resize(m);
+      for (uint32_t k = 0; k < m; k++) {
+        const size_t i = g[lo + k];
+        const uint32_t t = tr[i];
+        std::copy(masks + i * mw, masks + (i + 1) * mw, hm.begin() + (size_t)k * mw);
+        const uint64_t sb = (uint64_t)rs.seed_base[t];
+        hp[k] = make_uint4((uint32_t)sb, (uint32_t)(sb >> 32), (uint32_t)rs.max_messages[t], rs.looking_for[t]);
+        ht[k] = t;
+      }
+      CUDA_TRY(h, cudaMemcpyAsync(mdev, hm.data(), hm.size() * 8, cudaMemcpyHostToDevice, s));
+      CUDA_TRY(h, cudaMemcpyAsync(pdev, hp.data(), hp.size() * sizeof(uint4), cudaMemcpyHostToDevice, s));
+      CUDA_TRY(h, cudaMemcpyAsync(tdev, ht.data(), ht.size() * 4, cudaMemcpyHostToDevice, s));
+      CUDA_TRY(h, cudaMemsetAsync(first_hit, 0xFF, (size_t)m * 4, s));
+      CUDA_TRY(h, cudaMemsetAsync(cnt, 0, sizeof(unsigned long long), s));
+      demi_fuzz_params q = rs.p;
+      q.n_prefixes = (uint64_t)m * N;
+      q.max_messages = -1;                 // each test binds its own (prog_test_bind); pcap covers them all
+      q.looking_for = 0; q.seed_base = 0;
+      LaunchPlan plan;
+      if ((rc = plan_launch(h, &q, LM_TEST_PARAMS, li, nullptr, 0, &plan, pcap)) != DEMI_OK) return rc;
+      random_subseq_many_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(rs.progs, rs.tab, tdev, mdev, mw, m, pa.ev,
+                                                                                          stride, pa.hdr, pa.sends, send_stride);
+      CUDA_TRY(h, cudaGetLastError());
+      h->perf.kernel_launches++;
+      KernelArgs& a = plan.args;
+      a.results = h->results_dev.get<demi_fuzz_result>();
+      bind_programs(h, a, pa, -1);
+      a.prog_execs = N;
+      a.prog_first_hit = first_hit;
+      a.prog_params = pdev;
+      if ((rc = launch_plan(h, plan, q.n_prefixes, s)) != DEMI_OK) return rc;
+      random_test_reduce_kernel<true><<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(a.results, m, N, odev, cnt, rdev);
+      CUDA_TRY(h, cudaGetLastError());
+      h->perf.kernel_launches++;
+      hrec.resize(m); hran.resize(m);
+      CUDA_TRY(h, cudaMemcpyAsync(hrec.data(), odev, (size_t)m * sizeof(demi_random_test_result), cudaMemcpyDeviceToHost, s));
+      CUDA_TRY(h, cudaMemcpyAsync(hran.data(), rdev, (size_t)m * 4, cudaMemcpyDeviceToHost, s));
+      CUDA_TRY(h, cudaStreamSynchronize(s));
+      for (uint32_t k = 0; k < m; k++) {
+        out[g[lo + k]] = RandomRec{hrec[k], hran[k]};
+        h->perf.prefixes += hran[k];
+      }
+      lo = hi;
+    }
   }
+  return DEMI_OK;
+}
+
+// The call-wide checks of both entry points: what demi_random_test_batch / demi_random_ddmin refuse whatever the program
+int32_t check_random_many(demi_handle* h, const char* who, uint32_t n, const demi_ext_event* externals, const uint32_t* ext_offsets,
+                          const uint32_t* n_externals, const int64_t* seed_base, const int32_t* max_messages,
+                          const uint32_t* looking_for, const demi_fuzz_params* p, uint32_t mask_words) {
+  if (!externals || !ext_offsets || !n_externals || !seed_base || !max_messages || !looking_for || !p)
+    return fail(h, DEMI_ERR_INVALID, "%s: null argument", who);
+  { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
+  if (p->n_prefixes == 0 || p->n_prefixes > RANDOM_EXECS_PER_LAUNCH)
+    return fail(h, DEMI_ERR_INVALID, "%s: N = n_prefixes must be in 1..%llu", who, (unsigned long long)RANDOM_EXECS_PER_LAUNCH);
+  for (uint32_t t = 0; t < n; t++)
+    if ((uint64_t)mask_words * 64 < n_externals[t])
+      return fail(h, DEMI_ERR_INVALID, "%s: mask_words %u too small for the %u externals of trace %u", who, mask_words, n_externals[t], t);
+  return DEMI_OK;
+}
+
+typedef ManyRequest<RandomRec> RandomRequest;
+
+// randomDDMin on trace `trace` of a demi_random_ddmin_many call: its batches join the rendezvous
+struct ManyRandomDriver : RandomDDMinDriver {
+  Rendezvous<RandomRec>* R; uint32_t trace; const RandomSet* rs;
+  int32_t run_tests(const uint64_t* masks, size_t n, demi_random_test_result* res, uint64_t* executed) override {
+    int32_t rc = random_trace_launchable(h, *rs, trace);       // what plan_launch refuses of this trace's launch alone
+    if (rc != DEMI_OK) return rc;
+    RandomRequest q;
+    q.trace = trace; q.masks = masks; q.n = n;
+    R->submit(q);
+    if (q.rc != DEMI_OK) return q.rc;
+    *executed = 0;
+    for (size_t k = 0; k < n; k++) { res[k] = q.res[k].rec; *executed += q.res[k].ran; }
+    return DEMI_OK;
+  }
+};
+
+}  // namespace
+
+extern "C" int32_t demi_random_test_batch_many(demi_handle* h, uint32_t n_traces, const demi_ext_event* externals,
+                                               const uint32_t* ext_offsets, const uint32_t* n_externals, const int64_t* seed_base,
+                                               const int32_t* max_messages, const uint32_t* looking_for,
+                                               const uint32_t* trace_of_test, const uint64_t* masks, uint32_t n_tests,
+                                               uint32_t mask_words, const demi_fuzz_params* p, demi_random_test_result* out) {
+  if (!h) return DEMI_ERR_INVALID;
+  static const char* who = "demi_random_test_batch_many";
+  int32_t rc = check_random_many(h, who, n_traces, externals, ext_offsets, n_externals, seed_base, max_messages, looking_for, p,
+                                 mask_words);
+  if (rc != DEMI_OK) return rc;
+  if (n_tests && (!trace_of_test || !masks || !out)) return fail(h, DEMI_ERR_INVALID, "%s: null tests or output", who);
+  for (uint32_t i = 0; i < n_tests; i++)
+    if (trace_of_test[i] >= n_traces) return fail(h, DEMI_ERR_INVALID, "%s: test %u names trace %u of %u", who, i, trace_of_test[i], n_traces);
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  h->perf.kernel_launches = 0; h->perf.prefixes = 0;
+  if (!n_tests) return DEMI_OK;
+  RandomSet rs;
+  rs.mask_words = mask_words;
+  if ((rc = random_set(h, n_traces, externals, ext_offsets, n_externals, seed_base, max_messages, looking_for, p, rs)) != DEMI_OK) return rc;
+  // a test fails the call with what its program alone would give
+  for (uint32_t i = 0; i < n_tests; i++) {
+    const uint32_t t = trace_of_test[i];
+    if (rs.pre[t] != DEMI_OK) { h->err = std::string(who) + ": trace " + std::to_string(t) + ": " + rs.pre_msg[t]; return rs.pre[t]; }
+    if ((rc = random_trace_launchable(h, rs, t)) != DEMI_OK) { h->err = std::string(who) + ": trace " + std::to_string(t) + ": " + h->err; return rc; }
+  }
+  std::vector<RandomRec> res(n_tests);
+  if ((rc = random_tests_many(h, rs, trace_of_test, masks, n_tests, res.data())) != DEMI_OK) return rc;
+  for (uint32_t i = 0; i < n_tests; i++) out[i] = res[i].rec;
+  return DEMI_OK;
+}
+
+extern "C" int32_t demi_random_ddmin_many(demi_handle* h, uint32_t n_traces, const demi_ext_event* externals,
+                                          const uint32_t* ext_offsets, const uint32_t* n_externals, const int64_t* seed_base,
+                                          const int32_t* max_messages, const uint32_t* looking_for, const demi_fuzz_params* p,
+                                          int32_t check_unmodified, uint64_t* mcs_masks, uint32_t mask_words, uint32_t* iteration_sizes,
+                                          uint64_t* iteration_keys, uint32_t cap_iterations, demi_random_ddmin_out* out,
+                                          int32_t* status) {
+  if (!h) return DEMI_ERR_INVALID;
+  static const char* who = "demi_random_ddmin_many";
+  if (!n_traces) return DEMI_OK;
+  int32_t rc = check_random_many(h, who, n_traces, externals, ext_offsets, n_externals, seed_base, max_messages, looking_for, p,
+                                 mask_words);
+  if (rc != DEMI_OK) return rc;
+  if (!mcs_masks || !out || !status) return fail(h, DEMI_ERR_INVALID, "%s: null output", who);
+  const uint32_t n = n_traces;
+  uint32_t window;
+  if ((rc = many_window(h, n, window)) != DEMI_OK) return rc;
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  memset(out, 0, (size_t)n * sizeof(demi_random_ddmin_out));
+  h->perf.kernel_launches = 0; h->perf.prefixes = 0;
+  RandomSet rs;
+  rs.mask_words = mask_words;
+  if ((rc = random_set(h, n, externals, ext_offsets, n_externals, seed_base, max_messages, looking_for, p, rs)) != DEMI_OK) return rc;
+  demi_perf perf{};
+  // the union of a round's requests, in request order
+  auto serve = [&](std::vector<RandomRequest*>& batch) -> int32_t {
+    std::vector<uint32_t> tos;
+    std::vector<uint64_t> flat;
+    for (const RandomRequest* q : batch) {
+      tos.insert(tos.end(), q->n, q->trace);
+      flat.insert(flat.end(), q->masks, q->masks + q->n * mask_words);
+    }
+    std::vector<RandomRec> res(tos.size());
+    const int32_t src = random_tests_many(h, rs, tos.data(), flat.data(), tos.size(), res.data());
+    perf.kernel_launches += h->perf.kernel_launches; perf.prefixes += h->perf.prefixes;
+    h->perf.kernel_launches = 0; h->perf.prefixes = 0;
+    if (src != DEMI_OK) return src;
+    size_t k = 0;
+    for (RandomRequest* q : batch) {
+      q->res.assign(res.begin() + k, res.begin() + k + q->n);
+      k += q->n;
+    }
+    return DEMI_OK;
+  };
+  auto drive = [&](uint32_t t, Rendezvous<RandomRec>& R, demi_handle* eh) -> int32_t {
+    if (rs.pre[t] != DEMI_OK) { eh->err = rs.pre_msg[t]; return rs.pre[t]; }
+    ManyRandomDriver d;
+    d.R = &R; d.trace = t; d.rs = &rs;
+    d.h = eh; d.looking_for = looking_for[t]; d.mw = mask_words; d.n_ext = n_externals[t];
+    d.ext = externals + ext_offsets[t];
+    d.set_width(p->n_prefixes);
+    return d.minimize(check_unmodified != 0, mcs_masks + (size_t)t * mask_words,
+                      iteration_sizes ? iteration_sizes + (size_t)t * cap_iterations : nullptr,
+                      iteration_keys ? iteration_keys + (size_t)t * cap_iterations : nullptr, cap_iterations, out + t);
+  };
+  rc = run_many<RandomRec>(h, who, n, window, drive, serve, status);
+  h->perf.kernel_launches = perf.kernel_launches; h->perf.prefixes = perf.prefixes;
+  if (rc != DEMI_OK) return rc;
+  for (uint32_t t = 0; t < n; t++)
+    if (status[t] != DEMI_OK) { h->err = std::string(who) + ": trace " + std::to_string(t) + ": " + h->err; break; }
   return DEMI_OK;
 }
 

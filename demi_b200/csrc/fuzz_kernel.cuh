@@ -6,17 +6,21 @@
 // PROG + TESTS (random-oracle tests, demi_random_test_batch): prefix idx is execution idx % prog_execs of program
 // idx / prog_execs (prog_test_bind), skipped above its program's first hit.  A separate instantiation, so that the
 // campaign kernels stay as they were.
+// PROG + TESTS + PARAMS (demi_random_test_batch_many): the same, with each program's seed base, max_messages and
+// looking_for taken from `args.prog_params` (the programs of one launch belong to different traces).
 #pragma once
 #include "machine.cuh"
 #include "models/models.cuh"
 
 namespace demi {
 
-template <class MODEL, int PCAP, int TCAP, bool PEND_GLOBAL, bool RECORD, int WARPS, bool PROG = false, bool TESTS = false>
+template <class MODEL, int PCAP, int TCAP, bool PEND_GLOBAL, bool RECORD, int WARPS, bool PROG = false, bool TESTS = false,
+          bool PARAMS = false>
 __global__ void __launch_bounds__(WARPS * 32)
 fuzz_kernel(const __grid_constant__ KernelArgs args) {
   static_assert(!(PROG && RECORD), "a campaign execution is recorded through demi_fuzz_trace on its program");
   static_assert(PROG || !TESTS, "random-oracle tests bind their programs as campaigns do");
+  static_assert(TESTS || !PARAMS, "per-program parameters are those of random-oracle tests");
   using M = Machine<MODEL, PCAP, TCAP, PEND_GLOBAL, RECORD>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const uint32_t warp = threadIdx.x >> 5;
@@ -49,7 +53,7 @@ fuzz_kernel(const __grid_constant__ KernelArgs args) {
     if (RECORD) m.rec_ev = args.rec_events + it * (uint64_t)args.rec_cap;
     if constexpr (TESTS) {
       uint64_t prog; int64_t seed;
-      if (prog_test_bind(la, args, idx, false, prog, seed)) {
+      if (prog_test_bind<PARAMS>(la, args, idx, false, prog, seed)) {
         m.run(seed, r);
         if (lane == 0) prog_note_hit(args, idx, prog, r);
       } else {

@@ -870,12 +870,14 @@ lane_tree_kernel(const __grid_constant__ KernelArgs args, uint32_t* tree, const 
 // PROG (campaigns; with TESTS random-oracle tests, see fuzz_kernel): prefix idx runs its program of the arena in `args.prog_*`; the 0x80 | k entries
 // of messagesToSend resolve through that program's Send table.  A deferred prefix keeps its index, so the PROG
 // instantiation of the warp engine re-runs it on the same program.
-template <class MODEL, int BD, int LPCAP, bool REC = false, bool PROG = false, bool TESTS = false, bool STEADY = false>
+template <class MODEL, int BD, int LPCAP, bool REC = false, bool PROG = false, bool TESTS = false, bool STEADY = false,
+          bool PARAMS = false>
 __global__ void __launch_bounds__(BD, DEMI_K1_MIN_BLOCKS)
 fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
   static_assert(!(PROG && REC), "a campaign execution is recorded through demi_fuzz_trace on its program");
   static_assert(PROG || !TESTS, "random-oracle tests bind their programs as campaigns do");
   static_assert(!STEADY || !(REC || PROG), "a steady launch runs one fixed program, unrecorded");
+  static_assert(TESTS || !PARAMS, "per-program parameters are those of random-oracle tests");
   using M = LaneMachine<MODEL, BD, LPCAP, REC, STEADY>;
   extern __shared__ __align__(16) uint32_t lane_smem[];
   const uint32_t tid = threadIdx.x;
@@ -904,7 +906,7 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
     demi_fuzz_result r;
     if constexpr (TESTS) {
       uint64_t prog; int64_t seed;
-      if (prog_test_bind(la, args, idx, true, prog, seed)) {
+      if (prog_test_bind<PARAMS>(la, args, idx, true, prog, seed)) {
         m.run(seed, r);
         prog_note_hit(args, idx, prog, r);
       } else {

@@ -160,7 +160,13 @@ struct KernelArgs {
   uint4*    pend_scratch;     // [total_warps][pending_cap] when the pending set lives in HBM
   // recording launches: slot `it` (the position in the launch's work list) owns rec_events[it*rec_cap ..),
   // rec_counts[it*4 ..) = {n_events, n_nodes, affectedNodes, violation} and rec_parent[it*rec_parent_cap ..)
-  demi_event* rec_events; uint32_t rec_cap; uint32_t* rec_counts; uint16_t* rec_parent; uint32_t rec_parent_cap;
+  union {
+    demi_event* rec_events;
+    // the PARAMS kernels (demi_random_test_batch_many), which never record: test p's {seed_base lo, hi, max_messages
+    // as the caller gave it, looking_for}.  In the recording slot, so that the struct stays as it was.
+    const uint4* prog_params;
+  };
+  uint32_t rec_cap; uint32_t* rec_counts; uint16_t* rec_parent; uint32_t rec_parent_cap;
   // summary counters
   unsigned long long* sum_steps; unsigned long long* n_violations;
   // lane engine (lane_kernel.cuh)
@@ -193,28 +199,43 @@ struct KernelArgs {
 // the record status of an execution skipped because its program already has a hit at a lower index (never leaves
 // the device: the per-test reduction reads it)
 constexpr uint16_t PS_SKIPPED = 0xFFFEu;
-// The program view of a campaign execution: `la` is the executing thread's copy of the launch arguments.
-__device__ __forceinline__ void prog_bind(KernelArgs& la, const KernelArgs& args, uint64_t idx, bool lane) {
+// The program view of a campaign execution: `la` is the executing thread's copy of the launch arguments, and
+// `max_messages` the program's, unmapped.
+__device__ __forceinline__ void prog_bind(KernelArgs& la, const KernelArgs& args, uint64_t idx, bool lane, int32_t max_messages) {
   const uint2 h = args.prog_hdr[idx];
   la.ext = args.prog_ext + idx * (uint64_t)args.prog_stride;
   la.n_ext = h.x;
-  la.pending_cap = demi_pending_cap(args.prog_model_key, args.prog_max_messages, h.y);
+  la.pending_cap = demi_pending_cap(args.prog_model_key, max_messages, h.y);
   if (lane && args.prog_lane_pcap && args.prog_lane_pcap < la.pending_cap) la.pending_cap = args.prog_lane_pcap;
   la.tosend_cap = demi_tosend_cap(h.y);
-  la.node_cap = demi_node_cap(demi_pending_cap(args.prog_model_key, args.prog_max_messages, h.y));
+  la.node_cap = demi_node_cap(demi_pending_cap(args.prog_model_key, max_messages, h.y));
   la.ext_sends = args.prog_sends + idx * (uint64_t)args.prog_send_stride;
+}
+__device__ __forceinline__ void prog_bind(KernelArgs& la, const KernelArgs& args, uint64_t idx, bool lane) {
+  prog_bind(la, args, idx, lane, args.prog_max_messages);
 }
 // A random-oracle test execution (the TESTS kernels): execution idx is execution j = idx % prog_execs of program
 // prog = idx / prog_execs, under seed_base + j.  Binds the program on every path (so that the copy stays in
 // registers) and returns false if the execution is skipped.  `lane`: one thread per execution (else a warp, kept
-// uniform).
+// uniform).  PARAMS: the program's seed base, max_messages and looking_for come from prog_params[prog].
+template <bool PARAMS = false>
 __device__ __forceinline__ bool prog_test_bind(KernelArgs& la, const KernelArgs& args, uint64_t idx, bool lane, uint64_t& prog,
                                                int64_t& seed) {
   const uint32_t p = (uint32_t)idx / args.prog_execs, j = (uint32_t)idx - p * args.prog_execs;
-  prog = p; seed = seed_at(args.seed_base, j);
+  prog = p;
+  int32_t max_messages = args.prog_max_messages;
+  if constexpr (PARAMS) {
+    const uint4 q = args.prog_params[p];
+    seed = seed_at((int64_t)(((uint64_t)q.y << 32) | q.x), j);
+    max_messages = (int32_t)q.z;
+    la.max_messages = max_messages < 0 ? 0x7FFFFFFF : max_messages;   // as plan_launch maps it
+    la.looking_for = q.w;
+  } else {
+    seed = seed_at(args.seed_base, j);
+  }
   uint32_t fh = *(volatile const uint32_t*)(args.prog_first_hit + p);
   if (!lane) fh = __shfl_sync(FULL_MASK, fh, 0);
-  prog_bind(la, args, p, lane);
+  prog_bind(la, args, p, lane, max_messages);
   return j <= fh;
 }
 // after a TESTS execution: a hit lowers its program's first_hit (the caller writes from one thread per execution)

@@ -453,6 +453,68 @@ class Engine(object):
         n = min(out.n_iterations, cap_iterations)
         return mcs, sizes[:n].copy(), keys[:n].copy(), out
 
+    @staticmethod
+    def _programs(programs, n):
+        """Flattened programs for the _many calls: (externals, offsets, lengths); one program is shared by n traces."""
+        multi = isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind")
+        progs = list(programs) if multi else [programs] * n
+        progs = [np.ascontiguousarray(p if isinstance(p, np.ndarray) else pack_externals(p), dtype=N.EXT_DTYPE)
+                 for p in progs]
+        n_ext = np.array([len(p) for p in progs], dtype=np.uint32)
+        ext = np.concatenate(progs + [np.zeros(1, dtype=N.EXT_DTYPE)])
+        eoff = np.zeros(len(progs), dtype=np.uint32)
+        eoff[1:] = np.cumsum(n_ext)[:-1]
+        return ext, eoff, n_ext
+
+    @staticmethod
+    def _per_trace(seed_base, max_messages, looking_for, n):
+        sb = np.ascontiguousarray(np.broadcast_to(np.asarray(seed_base, dtype=np.int64), (n,)))
+        mm = np.ascontiguousarray(np.broadcast_to(np.asarray(max_messages, dtype=np.int32), (n,)))
+        lf = np.ascontiguousarray(np.broadcast_to(np.asarray(looking_for or 0, dtype=np.uint32), (n,)))
+        return sb, mm, lf
+
+    def random_test_batch_many(self, programs, trace_of_test, masks, n_execs, seed_base, max_messages, interval=0,
+                               looking_for=0, mask_words=None):
+        """demi_random_test_batch_many: test i is masks[i] over programs[trace_of_test[i]], with that trace's
+        seed_base, max_messages and looking_for (a scalar applies to every trace).  One RANDOM_TEST_DTYPE record per
+        test; the handle's program is not used."""
+        tr = np.ascontiguousarray(trace_of_test, dtype=np.uint32)
+        n = len(programs) if isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind") \
+            else int(tr.max()) + 1 if len(tr) else 1
+        ext, eoff, n_ext = self._programs(programs, n)
+        sb, mm, lf = self._per_trace(seed_base, max_messages, looking_for, n)
+        mw = mask_words or max(1, (int(n_ext.max()) + 63) // 64)
+        m = np.ascontiguousarray(masks, dtype=np.uint64).reshape(-1, mw)
+        out = np.zeros(len(m), dtype=N.RANDOM_TEST_DTYPE)
+        p = N.FuzzParams(0, n_execs, -1, interval, 0, 0)
+        self._check(N.lib().demi_random_test_batch_many(self._h, n, ext.ctypes.data, eoff.ctypes.data, n_ext.ctypes.data,
+                                                        sb.ctypes.data, mm.ctypes.data, lf.ctypes.data, tr.ctypes.data,
+                                                        m.ctypes.data, len(m), mw, C.byref(p), out.ctypes.data))
+        return out
+
+    def random_ddmin_many(self, programs, n_execs, seed_base, max_messages, looking_for, interval=0, check_unmodified=False,
+                          cap_iterations=1024, mask_words=None, n=None):
+        """demi_random_ddmin_many: random_ddmin on every program (or on one program n times) with per-trace seed_base,
+        max_messages and looking_for (a scalar applies to every trace).  Returns (MCS masks [n, mw], iteration sizes
+        [n, cap], their keys [n, cap], RANDOM_DDMIN_OUT_DTYPE [n], status [n]); trace t's iterations are the first
+        out[t]['n_iterations'] entries, and a trace whose status is not OK has no outputs."""
+        multi = isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind")
+        n = len(programs) if multi else n
+        ext, eoff, n_ext = self._programs(programs, n)
+        sb, mm, lf = self._per_trace(seed_base, max_messages, looking_for, n)
+        mw = mask_words or max(1, (int(n_ext.max()) + 63) // 64)
+        mcs = np.zeros((n, mw), dtype=np.uint64)
+        sizes = np.zeros((n, cap_iterations), dtype=np.uint32)
+        keys = np.zeros((n, cap_iterations), dtype=np.uint64)
+        out = np.zeros(n, dtype=N.RANDOM_DDMIN_OUT_DTYPE)
+        status = np.zeros(n, dtype=np.int32)
+        p = N.FuzzParams(0, n_execs, -1, interval, 0, 0)
+        self._check(N.lib().demi_random_ddmin_many(self._h, n, ext.ctypes.data, eoff.ctypes.data, n_ext.ctypes.data,
+                                                   sb.ctypes.data, mm.ctypes.data, lf.ctypes.data, C.byref(p),
+                                                   1 if check_unmodified else 0, mcs.ctypes.data, mw, sizes.ctypes.data,
+                                                   keys.ctypes.data, cap_iterations, out.ctypes.data, status.ctypes.data))
+        return mcs, sizes, keys, out, status
+
     def random_test_trace(self, mask, seed, max_messages, interval=0, looking_for=0, cap_events=65536):
         """The EventTrace of execution `seed` of the mask's subsequence of the program (demi_random_test_trace): what
         RandomScheduler.test returns for it.  Accepts adjacent WaitQuiescence.  (result, EventTrace)."""
@@ -927,6 +989,41 @@ def randomDDMin(schedulerConfig, trace, externals, violation, stats=None, max_ex
         m = mask_of(externals, mcs)
         _, verified = sched.engine.random_test_trace(m, seed + out.mcs_first_hit, len(trace), 0, violation)
     return mcs, ddmin._stats, verified, violation
+
+
+def randomDDMin_many(schedulerConfig, executions, max_executions=1, seeds=0, engine=None):
+    """randomDDMin on many recorded experiments in one call (demi_random_ddmin_many).  executions[t] is (trace,
+    externals, violation) as randomDDMin takes them, and seeds[t] its seed (a scalar applies to every one); each
+    experiment keeps its own setMaxMessages(trace.size).  Returns (results, status): results[t] is what randomDDMin
+    returns for experiment t, or None when status[t] is not OK.  The verified traces are recorded one experiment at a
+    time (demi_random_test_trace), which leaves the engine's program set to the last one recorded."""
+    eng = engine or Engine(schedulerConfig)
+    n = len(executions)
+    progs = [list(x[1]) for x in executions]
+    seeds = [int(s) for s in np.broadcast_to(np.asarray(seeds, dtype=np.int64), (n,))]
+    mcs, sizes, keys, out, status = eng.random_ddmin_many(progs, max_executions, seeds, [len(x[0]) for x in executions],
+                                                          [x[2] for x in executions])
+    results = []
+    for t, (trace, externals, violation) in enumerate(executions):
+        if status[t]:
+            results.append(None)
+            continue
+        stats = MinimizationStats()
+        stats.updateStrategy("DDMin", "RandomScheduler")
+        for size, key in zip(sizes[t, :out[t]["n_iterations"]], keys[t, :out[t]["n_iterations"]]):
+            stats.total_replays = int(key)
+            stats.record_iteration_size(size)
+        stats.total_replays = int(out[t]["total_replays"])
+        m = mcs[t]
+        mcs_events = [e for i, e in enumerate(progs[t]) if (int(m[i >> 6]) >> (i & 63)) & 1]
+        verified = trace
+        if len(mcs_events) < len(progs[t]):
+            verified = None
+            if out[t]["verified"]:
+                eng.set_externals(progs[t])
+                _, verified = eng.random_test_trace(m, seeds[t] + int(out[t]["mcs_first_hit"]), len(trace), 0, violation)
+        results.append((mcs_events, stats, verified, violation))
+    return results, status
 
 
 class ProvenanceTracker:

@@ -524,6 +524,43 @@ typedef struct {
 int32_t demi_random_ddmin(demi_handle* h, const demi_fuzz_params* p, int32_t check_unmodified, uint64_t* mcs_mask,
                           uint32_t mask_words, uint32_t* iteration_sizes, uint64_t* iteration_keys, uint32_t cap,
                           demi_random_ddmin_out* out);
+/* Random-oracle tests over many programs.  Program t is externals[ext_offsets[t] ..], n_externals[t] records (offsets
+ * in elements, so one program shared by every trace, all ext_offsets 0, is taken as it is), with its own seed base
+ * seed_base[t], max_messages[t] and looking_for[t]; `p` supplies N (n_prefixes), invariant_check_interval and flags, and
+ * its seed_base, max_messages and looking_for are ignored.  Neither call reads or changes the handle's program, trace or
+ * trace set, and neither needs demi_set_externals first.
+ *
+ * demi_random_test_batch_many: test i is masks[i*mask_words ..] over program trace_of_test[i]; out[i] equals the record
+ * demi_set_externals(h, program t) + demi_random_test_batch(h, mask i, p with program t's three values) gives.  A test
+ * whose program demi_set_externals would reject, or that no kernel variant fits, fails the call with that code (an empty
+ * program with DEMI_ERR_STATE); DEMI_ERR_INVALID for a trace_of_test entry >= n_traces, N = 0 or above 2^22,
+ * mask_words too small for a program, or null arguments.  demi_perf.prefixes is the number of executions that ran. */
+int32_t demi_random_test_batch_many(demi_handle* h, uint32_t n_traces, const demi_ext_event* externals, const uint32_t* ext_offsets,
+                                    const uint32_t* n_externals, const int64_t* seed_base, const int32_t* max_messages,
+                                    const uint32_t* looking_for, const uint32_t* trace_of_test, const uint64_t* masks,
+                                    uint32_t n_tests, uint32_t mask_words, const demi_fuzz_params* p, demi_random_test_result* out);
+/* demi_random_ddmin on each of n_traces programs, every trace's speculative tests in shared launches.  status[t] is what
+ * demi_set_externals(h, program t) followed by demi_random_ddmin(h, p with seed_base[t], max_messages[t] and
+ * looking_for[t], check_unmodified, ...) returns; when it is DEMI_OK, mcs_masks[t*mask_words ..], iteration_sizes and
+ * iteration_keys at t*cap_iterations (either may be NULL) and out[t] equal that call's outputs in every field but
+ * executions_executed, tests, tests_evaluated, batches, total_replays, verified and mcs_first_hit included: a trace's
+ * speculation width is the single call's (DEMI_DDMIN_WIDE included) and depends on its own memo alone, so its results
+ * do not depend on which traces share its launches.  executions_executed is the trace's own count of executions that
+ * ran, between the sum of executions_run over its evaluated tests and tests_evaluated x N (the single call's, too, is
+ * not fixed: executions above a test's first hit may or may not be skipped).  A trace fails alone, with the code and
+ * message of the single sequence: a program demi_set_externals rejects (DEMI_ERR_STATE for an empty one), no kernel
+ * variant for its capacities, "Unmodified trace does not trigger violation", a consumed test's or the MCS test's status
+ * (DEMI_ERR_CAPACITY), the bookkeeping assertion, or host memory exhaustion (DEMI_ERR_CAPACITY); the call then returns
+ * DEMI_OK and demi_last_error names the lowest failing trace.  The call fails only on invalid arguments (as
+ * demi_random_test_batch_many's) or a CUDA error.  DEMI_DDMIN_MANY_WINDOW bounds the minimisations in flight as it does
+ * for demi_ddmin_many.  A round's tests go out in at most two groups, the programs the lane engine takes and the
+ * others, each cut into launches of at most 2^22 executions and a 512 MB program arena; demi_perf counts every launch
+ * and demi_perf.prefixes the executions that ran. */
+int32_t demi_random_ddmin_many(demi_handle* h, uint32_t n_traces, const demi_ext_event* externals, const uint32_t* ext_offsets,
+                               const uint32_t* n_externals, const int64_t* seed_base, const int32_t* max_messages,
+                               const uint32_t* looking_for, const demi_fuzz_params* p, int32_t check_unmodified,
+                               uint64_t* mcs_masks, uint32_t mask_words, uint32_t* iteration_sizes, uint64_t* iteration_keys,
+                               uint32_t cap_iterations, demi_random_ddmin_out* out, int32_t* status);
 /* The EventTrace RandomScheduler.test returns for a subsequence: execution `seed` of the mask's subsequence of the
  * handle's program, recorded as demi_fuzz_trace records it (p->max_messages, p->looking_for and
  * p->invariant_check_interval as there; p->seed_base and p->n_prefixes are not read).  Unlike demi_set_externals +

@@ -330,6 +330,45 @@ class Engine {
     }
     return r;
   }
+  // demi_random_ddmin_many: randomDDMin on every program t (RandomScheduler.test with N = max_executions), with its own
+  // seed, setMaxMessages and violation; per trace its MCS mask, keyed iteration sizes and record, or the error code
+  struct RandomDDMinManyResult {
+    std::vector<uint64_t> mcs_mask; std::vector<uint32_t> iteration_sizes; std::vector<uint64_t> iteration_keys;
+    demi_random_ddmin_out out{}; int32_t status = DEMI_OK;
+  };
+  std::vector<RandomDDMinManyResult> random_ddmin_many(const std::vector<ExternalEvents>& programs, const std::vector<int64_t>& seeds,
+                                                       const std::vector<int32_t>& max_messages,
+                                                       const std::vector<ViolationFingerprint>& looking_for, uint32_t max_executions,
+                                                       int32_t interval = 0, bool check_unmodified = false,
+                                                       uint32_t cap_iterations = 1024) {
+    const size_t n = programs.size();
+    ExternalEvents flat; std::vector<uint32_t> off, cnt;
+    size_t words = 1;
+    for (const ExternalEvents& p : programs) {
+      off.push_back((uint32_t)flat.size()); cnt.push_back((uint32_t)p.size());
+      flat.insert(flat.end(), p.begin(), p.end());
+      words = std::max<size_t>(words, (p.size() + 63) / 64);
+    }
+    if (flat.empty()) flat.resize(1);
+    const demi_fuzz_params p{0, max_executions, -1, interval, 0, 0};
+    std::vector<uint64_t> mcs(n * words), keys(n * (size_t)cap_iterations);
+    std::vector<uint32_t> sizes(n * (size_t)cap_iterations);
+    std::vector<demi_random_ddmin_out> out(n);
+    std::vector<int32_t> status(n);
+    check(demi_random_ddmin_many(h, (uint32_t)n, flat.data(), off.data(), cnt.data(), seeds.data(), max_messages.data(),
+                                 looking_for.data(), &p, check_unmodified ? 1 : 0, mcs.data(), (uint32_t)words, sizes.data(),
+                                 keys.data(), cap_iterations, out.data(), status.data()));
+    std::vector<RandomDDMinManyResult> r(n);
+    for (size_t t = 0; t < n; t++) {
+      r[t].out = out[t]; r[t].status = status[t];
+      if (status[t] != DEMI_OK) continue;
+      const size_t k = std::min(out[t].n_iterations, cap_iterations);
+      r[t].mcs_mask.assign(mcs.begin() + t * words, mcs.begin() + (t + 1) * words);
+      r[t].iteration_sizes.assign(sizes.begin() + t * cap_iterations, sizes.begin() + t * cap_iterations + k);
+      r[t].iteration_keys.assign(keys.begin() + t * cap_iterations, keys.begin() + t * cap_iterations + k);
+    }
+    return r;
+  }
   const SchedulerConfig cfg;
  private:
   demi_handle* h = nullptr;

@@ -233,6 +233,31 @@ JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_randomTestTrac
                                 (int64_t)seed, (demi_event*)BUF(env, events), (uint32_t)capEvents, (uint32_t*)BUF(env, count),
                                 (demi_fuzz_result*)BUF(env, result));
 }
+/* demi_random_test_batch_many / demi_random_ddmin_many: the same over many programs (offsets in elements), each with its
+ * own seed base, max_messages and looking_for; status[t] is trace t's return code */
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_randomTestBatchMany(JNIEnv* env, jclass c, jlong h, jint nTraces,
+    jobject externals, jobject extOffsets, jobject nExternals, jobject seedBase, jobject maxMessages, jobject lookingFor,
+    jobject traceOfTest, jobject masks, jint nTests, jint maskWords, jobject params, jobject out) {
+  return demi_random_test_batch_many(H(h), (uint32_t)nTraces, (const demi_ext_event*)BUF(env, externals),
+                                     (const uint32_t*)BUF(env, extOffsets), (const uint32_t*)BUF(env, nExternals),
+                                     (const int64_t*)BUF(env, seedBase), (const int32_t*)BUF(env, maxMessages),
+                                     (const uint32_t*)BUF(env, lookingFor), (const uint32_t*)BUF(env, traceOfTest),
+                                     (const uint64_t*)BUF(env, masks), (uint32_t)nTests, (uint32_t)maskWords,
+                                     (const demi_fuzz_params*)BUF(env, params), (demi_random_test_result*)BUF(env, out));
+}
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_randomDDMinMany(JNIEnv* env, jclass c, jlong h, jint nTraces,
+    jobject externals, jobject extOffsets, jobject nExternals, jobject seedBase, jobject maxMessages, jobject lookingFor,
+    jobject params, jint checkUnmodified, jobject mcsMasks, jint maskWords, jobject iterationSizes, jobject iterationKeys,
+    jint capIterations, jobject out, jobject status) {
+  return demi_random_ddmin_many(H(h), (uint32_t)nTraces, (const demi_ext_event*)BUF(env, externals),
+                                (const uint32_t*)BUF(env, extOffsets), (const uint32_t*)BUF(env, nExternals),
+                                (const int64_t*)BUF(env, seedBase), (const int32_t*)BUF(env, maxMessages),
+                                (const uint32_t*)BUF(env, lookingFor), (const demi_fuzz_params*)BUF(env, params), checkUnmodified,
+                                (uint64_t*)BUF(env, mcsMasks), (uint32_t)maskWords,
+                                iterationSizes ? (uint32_t*)BUF(env, iterationSizes) : 0,
+                                iterationKeys ? (uint64_t*)BUF(env, iterationKeys) : 0, (uint32_t)capIterations,
+                                (demi_random_ddmin_out*)BUF(env, out), (int32_t*)BUF(env, status));
+}
 /* demi_fuzz_traces / demi_set_traces / demi_replay_batch_many / demi_ddmin_many: many violating executions recorded,
  * replayed and minimized with their tests in shared launches */
 JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_fuzzTraces(JNIEnv* env, jclass c, jlong h, jobject params,

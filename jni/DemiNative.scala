@@ -75,6 +75,17 @@ object DemiNative {
   /** demi_random_test_trace: the EventTrace RandomScheduler.test returns for a subsequence (the verified MCS trace) */
   @native def randomTestTrace(h: Long, mask: ByteBuffer, maskWords: Int, params: ByteBuffer, seed: Long, events: ByteBuffer,
                               capEvents: Int, count: ByteBuffer, result: ByteBuffer): Int
+  /** demi_random_test_batch_many: test i is mask i over program traceOfTest(i) (offsets in elements), with that trace's
+    * seedBase, maxMessages and lookingFor; the handle's program is not used */
+  @native def randomTestBatchMany(h: Long, nTraces: Int, externals: ByteBuffer, extOffsets: ByteBuffer, nExternals: ByteBuffer,
+                                  seedBase: ByteBuffer, maxMessages: ByteBuffer, lookingFor: ByteBuffer, traceOfTest: ByteBuffer,
+                                  masks: ByteBuffer, nTests: Int, maskWords: Int, params: ByteBuffer, out: ByteBuffer): Int
+  /** demi_random_ddmin_many: randomDDMin on every program t (its own seed, maxMessages = its trace's size, lookingFor),
+    * every trace's tests in shared launches; status(t) is that trace's return code */
+  @native def randomDDMinMany(h: Long, nTraces: Int, externals: ByteBuffer, extOffsets: ByteBuffer, nExternals: ByteBuffer,
+                              seedBase: ByteBuffer, maxMessages: ByteBuffer, lookingFor: ByteBuffer, params: ByteBuffer,
+                              checkUnmodified: Int, mcsMasks: ByteBuffer, maskWords: Int, iterationSizes: ByteBuffer,
+                              iterationKeys: ByteBuffer, capIterations: Int, out: ByteBuffer, status: ByteBuffer): Int
   /** demi_fuzz_traces: the EventTraces of executions seed_base + prefixIndex(i), execution i at events + i*capEvents */
   @native def fuzzTraces(h: Long, params: ByteBuffer, prefixIndex: ByteBuffer, n: Int, events: ByteBuffer, capEvents: Int,
                          nEvents: ByteBuffer, results: ByteBuffer): Int
