@@ -140,7 +140,7 @@ EXPORTS = [
     "demi_fuzz_traces", "demi_set_traces", "demi_replay_batch_many", "demi_ddmin_many",
     "demi_replay_traces_many", "demi_internal_minimize_many", "demi_wildcard_replay_batch_many",
     "demi_wildcard_minimize_many", "demi_incremental_ddmin_many", "demi_fuzz_traces_tree",
-    "demi_random_test_batch_many", "demi_random_ddmin_many",
+    "demi_random_test_batch_many", "demi_random_ddmin_many", "demi_fuzz_traces_many",
 ]
 FILTER_RULE_DTYPE = np.dtype([("src_mask", "<u4"), ("dst_mask", "<u4"), ("type_mask", "<u4"), ("flags", "<u4")])
 FRULE_DEADLETTERS = 1
@@ -357,6 +357,9 @@ def lib():
                                               C.c_int32, C.c_uint32, vp, C.c_uint32, vp, vp]
     L.demi_fuzz_traces_tree.restype = C.c_int32
     L.demi_fuzz_traces_tree.argtypes = [vp, C.POINTER(FuzzParams), vp, C.c_uint32, vp, C.c_uint32, vp, vp, C.c_uint32, vp, vp]
+    L.demi_fuzz_traces_many.restype = C.c_int32
+    L.demi_fuzz_traces_many.argtypes = [vp, C.c_uint32, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, C.POINTER(FuzzParams), vp,
+                                        C.c_uint32, vp, vp, C.c_uint32, vp, vp, vp]
     L.demi_stats.restype = C.c_int32
     L.demi_stats.argtypes = [vp, C.POINTER(Perf)]
     L.demi_lane_kernel.restype = C.c_int32

@@ -29,12 +29,13 @@ typedef void (*kernel_fn)(const KernelArgs);
 // What a fuzz launch runs: a batch of prefixes over the handle's program, the recording of chosen prefixes
 // (provenance, traces), a campaign's generated programs (PROG), random-oracle tests over subsequences (PROG + TESTS),
 // or random-oracle tests of many traces, each with its own parameters (PROG + TESTS + PARAMS).  Both engines have one
-// instantiation per mode.
-enum LaunchMode { LM_BATCH, LM_RECORD, LM_PROGRAM, LM_TESTS, LM_TEST_PARAMS, LM_COUNT };
+// instantiation per mode, except the recording of many programs' executions, each with its own parameters
+// (PROG + RECORD + PARAMS), which the warp engine alone runs.
+enum LaunchMode { LM_BATCH, LM_RECORD, LM_PROGRAM, LM_TESTS, LM_TEST_PARAMS, LM_RECORD_PARAMS, LM_COUNT };
 struct Variant {
   int model; uint32_t pcap, tcap; bool pend_global;
   size_t smem_per_warp;
-  kernel_fn fn[LM_COUNT];        // a recording variant has LM_RECORD alone, the others every mode but it
+  kernel_fn fn[LM_COUNT];        // a recording variant has LM_RECORD and LM_RECORD_PARAMS, the others every other mode
 };
 template <class MODEL, int PCAP, int TCAP, bool PG, bool REC>
 static Variant make_variant() {
@@ -43,7 +44,8 @@ static Variant make_variant() {
             {fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS>, nullptr,
              REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC>,
              REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC, !REC>,
-             REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC, !REC, !REC>}};
+             REC ? nullptr : fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, !REC, !REC, !REC>,
+             REC ? fuzz_kernel<MODEL, PCAP, TCAP, PG, REC, WARPS, REC, false, REC> : nullptr}};
   if (REC) std::swap(v.fn[LM_BATCH], v.fn[LM_RECORD]);
   return v;
 }
@@ -335,7 +337,7 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, LaunchMode
                            const demi_ext_event* ext, uint32_t n_ext, LaunchPlan* plan, uint32_t pcap_at_least = 0) {
   if (!p) return fail(h, DEMI_ERR_INVALID, "null params");
   if (mode == LM_PROGRAM && !h->has_fuzzer) return fail(h, DEMI_ERR_STATE, "demi_set_fuzzer has not been called");
-  if (mode != LM_PROGRAM && mode != LM_TEST_PARAMS && h->ext_host.empty())
+  if (mode != LM_PROGRAM && mode != LM_TEST_PARAMS && mode != LM_RECORD_PARAMS && h->ext_host.empty())
     return fail(h, DEMI_ERR_STATE, "demi_set_externals has not been called");
   if (p->n_prefixes > 0xFFFFFFFFull) return fail(h, DEMI_ERR_INVALID, "n_prefixes > 2^32-1 per call");
   { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
@@ -1621,6 +1623,212 @@ extern "C" int32_t demi_random_ddmin_many(demi_handle* h, uint32_t n_traces, con
   if (rc != DEMI_OK) return rc;
   for (uint32_t t = 0; t < n; t++)
     if (status[t] != DEMI_OK) { h->err = std::string(who) + ": trace " + std::to_string(t) + ": " + h->err; break; }
+  return DEMI_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Recording many programs' executions: execution t is the subsequence that mask t keeps of program t, run under its own
+// seed, max_messages and looking_for and recorded by the warp engine as demi_fuzz_trace records it.
+
+// Slots per recording launch: record_chunk's, or fewer when DEMI_TEST_FUZZ_MANY_SLOTS is set (tests force several
+// launches with it).
+static uint32_t fuzz_many_chunk(uint32_t cap_events, uint32_t par_cap) {
+  uint32_t c = record_chunk(cap_events, par_cap, 0);
+  if (const char* e = getenv("DEMI_TEST_FUZZ_MANY_SLOTS"))
+    if (*e) c = std::max(1u, std::min(c, (uint32_t)strtoul(e, nullptr, 10)));
+  return c;
+}
+
+extern "C" int32_t demi_fuzz_traces_many(demi_handle* h, uint32_t n_traces, const demi_ext_event* externals,
+                                         const uint32_t* ext_offsets, const uint32_t* n_externals, const uint64_t* masks,
+                                         uint32_t mask_words, const int64_t* seeds, const int32_t* max_messages,
+                                         const uint32_t* looking_for, const demi_fuzz_params* p, demi_event* events,
+                                         uint32_t cap_events, uint32_t* n_events, uint16_t* dep_parent, uint32_t cap_nodes,
+                                         uint32_t* n_nodes, demi_fuzz_result* results, int32_t* status) {
+  if (!h) return DEMI_ERR_INVALID;
+  static const char* who = "demi_fuzz_traces_many";
+  if (!n_traces) return DEMI_OK;
+  if (!externals || !ext_offsets || !n_externals || !seeds || !max_messages || !looking_for || !p || !events || !cap_events ||
+      !n_events || !status)
+    return fail(h, DEMI_ERR_INVALID, "%s: null argument", who);
+  if (dep_parent && (!n_nodes || !cap_nodes || cap_nodes > 65536))
+    return fail(h, DEMI_ERR_INVALID, "%s: a tree needs n_nodes and cap_nodes in 1..65536", who);
+  if (masks)
+    for (uint32_t t = 0; t < n_traces; t++)
+      if ((uint64_t)mask_words * 64 < n_externals[t])
+        return fail(h, DEMI_ERR_INVALID, "%s: mask_words %u too small for the %u externals of trace %u", who, mask_words, n_externals[t], t);
+  { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
+  CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+  const uint32_t n = n_traces;
+  h->perf.kernel_launches = 0; h->perf.prefixes = 0; h->perf.kernel_ms = 0;
+  memset(n_events, 0, (size_t)n * sizeof(uint32_t));
+  if (n_nodes) memset(n_nodes, 0, (size_t)n * sizeof(uint32_t));
+  if (results) memset(results, 0, (size_t)n * sizeof(demi_fuzz_result));
+  // demi_set_externals's checks of each program; the programs are uploaded once
+  RandomSet rs;
+  int32_t rc = random_set(h, n, externals, ext_offsets, n_externals, seeds, max_messages, looking_for, p, rs);
+  if (rc != DEMI_OK) return rc;
+  // Then demi_random_test_trace's and plan_launch's of each subsequence.  Every execution runs on the variant its single
+  // call picks: the traces are grouped by it, so that a HardKill or SrcDstFIFO program moves no other program.
+  uint32_t mw = masks ? mask_words : 1;                // without masks every trace keeps all: one row of ones serves all
+  if (!masks) for (uint32_t t = 0; t < n; t++) mw = std::max(mw, (n_externals[t] + 63) / 64);
+  const std::vector<uint64_t> ones(mw, ~0ull);
+  const bool fifo = h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;
+  std::vector<uint32_t> kept(n, 0), sends(n, 0), pcap(n, 0);
+  std::vector<bool> hard_kill(n, false);
+  std::vector<const Variant*> var(n, nullptr);
+  std::vector<std::string> msg(n);
+  char buf[160];
+  for (uint32_t t = 0; t < n; t++) {
+    status[t] = rs.pre[t];
+    if (rs.pre[t] != DEMI_OK) { msg[t] = rs.pre_msg[t]; continue; }
+    const demi_ext_event* ev = externals + ext_offsets[t];
+    const uint64_t* mk = masks ? masks + (size_t)t * mask_words : ones.data();
+    for (uint32_t i = 0; i < n_externals[t]; i++)
+      if ((mk[i >> 6] >> (i & 63)) & 1ull) {
+        kept[t]++;
+        if (ev[i].kind == DEMI_EXT_SEND) sends[t]++;
+        if (ev[i].kind == DEMI_EXT_HARD_KILL) hard_kill[t] = true;
+      }
+    if (!kept[t]) { status[t] = DEMI_ERR_INVALID; msg[t] = "demi_random_test_trace: the mask keeps no event"; continue; }
+    pcap[t] = demi_pending_cap(demi_model_key(h), max_messages[t], sends[t]);
+    const uint32_t tcap = demi_tosend_cap(sends[t]);
+    var[t] = pick_variant(h->cfg.model, LM_RECORD_PARAMS, pcap[t], tcap, fifo || hard_kill[t]);
+    if (!var[t]) {
+      snprintf(buf, sizeof(buf), "no kernel variant for pending_cap=%u tosend_cap=%u", pcap[t], tcap);
+      status[t] = DEMI_ERR_CAPACITY; msg[t] = buf;
+    } else if (fifo && (hard_kill[t] || !h->filter.empty())) {
+      status[t] = DEMI_ERR_INVALID; msg[t] = "HardKill and userDefinedFilter are offered for FullyRandom only";
+      var[t] = nullptr;
+    }
+  }
+  const uint32_t par_cap = dep_parent ? cap_nodes : 0;
+  const uint32_t chunk = fuzz_many_chunk(cap_events, par_cap);
+  cudaStream_t s = h->stream;
+  DevBuf rbuf;
+  std::vector<uint64_t> hm;
+  std::vector<uint4> hp;
+  std::vector<uint32_t> ht, cnt;
+  std::vector<demi_fuzz_result> res;
+  std::vector<demi_event> hev;
+  std::vector<uint16_t> hpar;
+  double ms_all = 0;
+  for (const Variant& v : variants()) {
+    std::vector<uint32_t> g;
+    for (uint32_t t = 0; t < n; t++) if (var[t] == &v) g.push_back(t);
+    // launches of at most `chunk` slots and a 512 MB program arena whose stride is the launch's longest subsequence
+    for (size_t lo = 0; lo < g.size();) {
+      uint32_t stride = 1, send_stride = 1, pc = 0;
+      ProgramInfo li;
+      size_t hi = lo;
+      for (; hi < g.size() && hi - lo < chunk; hi++) {
+        const uint32_t t = g[hi];
+        const uint32_t st = std::max(stride, kept[t]), ss = std::max(send_stride, sends[t]);
+        const uint64_t per = (uint64_t)st * sizeof(demi_ext_event) + sizeof(uint2) + (uint64_t)ss * sizeof(uint4) + (uint64_t)mw * 8 +
+                             sizeof(uint4) + 4;
+        if (hi > lo && (hi - lo + 1) * per > ((uint64_t)512 << 20)) break;
+        stride = st; send_stride = ss;
+        pc = std::max(pc, pcap[t]);
+        li.sends = std::max(li.sends, sends[t]);
+        li.hard_kill = li.hard_kill || hard_kill[t];
+      }
+      const uint32_t m = (uint32_t)(hi - lo);
+      // arena: the programs | masks | parameters | traces
+      auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
+      const size_t b_mask = al((size_t)m * mw * 8), b_par = al((size_t)m * sizeof(uint4)), b_tr = al((size_t)m * 4);
+      ProgramArena pa;
+      unsigned char* rest;
+      if ((rc = carve_programs(h, m, stride, send_stride, b_mask + b_par + b_tr, &pa, &rest)) != DEMI_OK) return rc;
+      uint64_t* mdev = (uint64_t*)rest;
+      uint4* pdev = (uint4*)(rest + b_mask);
+      uint32_t* tdev = (uint32_t*)(rest + b_mask + b_par);
+      hm.resize((size_t)m * mw); hp.resize(m); ht.resize(m);
+      for (uint32_t k = 0; k < m; k++) {
+        const uint32_t t = g[lo + k];
+        const uint64_t* mk = masks ? masks + (size_t)t * mask_words : ones.data();
+        std::copy(mk, mk + mw, hm.begin() + (size_t)k * mw);
+        const uint64_t sb = (uint64_t)seeds[t];
+        hp[k] = make_uint4((uint32_t)sb, (uint32_t)(sb >> 32), (uint32_t)max_messages[t], looking_for[t]);
+        ht[k] = t;
+      }
+      CUDA_TRY(h, cudaMemcpyAsync(mdev, hm.data(), hm.size() * 8, cudaMemcpyHostToDevice, s));
+      CUDA_TRY(h, cudaMemcpyAsync(pdev, hp.data(), hp.size() * sizeof(uint4), cudaMemcpyHostToDevice, s));
+      CUDA_TRY(h, cudaMemcpyAsync(tdev, ht.data(), ht.size() * 4, cudaMemcpyHostToDevice, s));
+      demi_fuzz_params q{};
+      q.n_prefixes = m;
+      q.max_messages = -1;                 // each execution binds its own (prog_params_bind); pc covers them all
+      q.invariant_check_interval = p->invariant_check_interval;
+      q.flags = p->flags;
+      LaunchPlan plan;
+      if ((rc = plan_launch(h, &q, LM_RECORD_PARAMS, li, nullptr, 0, &plan, pc)) != DEMI_OK) return rc;
+      Records rec;
+      if ((rc = stage_records(h, &plan, m, nullptr, cap_events, par_cap, 0, rbuf, &rec, s)) != DEMI_OK) return rc;
+      KernelArgs& a = plan.args;
+      a.sum_steps = nullptr; a.n_violations = nullptr;      // the handle's counters stay as they were
+      bind_programs(h, a, pa, -1);
+      a.rec_params = pdev;
+      CUDA_TRY(h, cudaEventRecord(h->ev0, s));
+      random_subseq_many_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(rs.progs, rs.tab, tdev, mdev, mw, m, pa.ev,
+                                                                                          stride, pa.hdr, pa.sends, send_stride);
+      CUDA_TRY(h, cudaGetLastError());
+      if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
+      plan.v->fn[LM_RECORD_PARAMS]<<<plan.grid, WARPS * 32, plan.smem, s>>>(a);
+      CUDA_TRY(h, cudaGetLastError());
+      CUDA_TRY(h, cudaEventRecord(h->ev1, s));
+      h->perf.kernel_launches += 2;
+      h->perf.prefixes += m;
+      res.resize(m); cnt.resize((size_t)m * 4);
+      CUDA_TRY(h, cudaMemcpyAsync(cnt.data(), rec.counts, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+      CUDA_TRY(h, cudaMemcpyAsync(res.data(), rec.results, res.size() * sizeof(demi_fuzz_result), cudaMemcpyDeviceToHost, s));
+      CUDA_TRY(h, cudaStreamSynchronize(s));
+      float ms = 0.f;
+      CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+      ms_all += ms;
+      // the rows travel as wide as the launch's longest successful recording, then go to their traces' rows
+      uint32_t width = 0, pwidth = 0;
+      for (uint32_t k = 0; k < m; k++) {
+        const uint32_t t = g[lo + k];
+        n_events[t] = cnt[(size_t)k * 4];
+        if (n_nodes) n_nodes[t] = cnt[(size_t)k * 4 + 1];
+        if (results) results[t] = res[k];
+        if (res[k].status) {
+          snprintf(buf, sizeof(buf), "demi_fuzz_trace: prefix status %u", (unsigned)res[k].status);
+          status[t] = DEMI_ERR_CAPACITY; msg[t] = buf;
+        } else {
+          width = std::max(width, std::min(cnt[(size_t)k * 4], cap_events));
+          pwidth = std::max(pwidth, std::min(cnt[(size_t)k * 4 + 1], par_cap));
+        }
+      }
+      if (width) {
+        hev.resize((size_t)m * width);
+        CUDA_TRY(h, cudaMemcpy2DAsync(hev.data(), (size_t)width * sizeof(demi_event), rec.events, (size_t)cap_events * sizeof(demi_event),
+                                      (size_t)width * sizeof(demi_event), m, cudaMemcpyDeviceToHost, s));
+      }
+      if (pwidth) {
+        hpar.resize((size_t)m * pwidth);
+        CUDA_TRY(h, cudaMemcpy2DAsync(hpar.data(), (size_t)pwidth * sizeof(uint16_t), rec.parents, (size_t)par_cap * sizeof(uint16_t),
+                                      (size_t)pwidth * sizeof(uint16_t), m, cudaMemcpyDeviceToHost, s));
+      }
+      if (width || pwidth) CUDA_TRY(h, cudaStreamSynchronize(s));
+      for (uint32_t k = 0; k < m; k++) {
+        const uint32_t t = g[lo + k];
+        if (status[t] != DEMI_OK) continue;
+        std::copy_n(hev.data() + (size_t)k * width, std::min(n_events[t], cap_events), events + (size_t)t * cap_events);
+        if (dep_parent) std::copy_n(hpar.data() + (size_t)k * pwidth, std::min(n_nodes[t], par_cap), dep_parent + (size_t)t * par_cap);
+      }
+      lo = hi;
+    }
+  }
+  h->perf.kernel_ms = ms_all;
+  // a failing trace has no events and no tree: zeros where they would be
+  int64_t bad = -1;
+  for (uint32_t t = 0; t < n; t++) {
+    if (status[t] == DEMI_OK) continue;
+    if (bad < 0) bad = t;
+    memset(events + (size_t)t * cap_events, 0, (size_t)cap_events * sizeof(demi_event));
+    if (dep_parent) memset(dep_parent + (size_t)t * par_cap, 0, (size_t)par_cap * sizeof(uint16_t));
+  }
+  if (bad >= 0) h->err = std::string(who) + ": trace " + std::to_string(bad) + ": " + msg[bad];
   return DEMI_OK;
 }
 

@@ -8,6 +8,8 @@
 // campaign kernels stay as they were.
 // PROG + TESTS + PARAMS (demi_random_test_batch_many): the same, with each program's seed base, max_messages and
 // looking_for taken from `args.prog_params` (the programs of one launch belong to different traces).
+// PROG + RECORD + PARAMS (demi_fuzz_traces_many): work-list slot idx records one execution of program idx under its own
+// seed, max_messages and looking_for (`args.rec_params`) and that program's capacities.  The only recording PROG kernel.
 #pragma once
 #include "machine.cuh"
 #include "models/models.cuh"
@@ -18,9 +20,10 @@ template <class MODEL, int PCAP, int TCAP, bool PEND_GLOBAL, bool RECORD, int WA
           bool PARAMS = false>
 __global__ void __launch_bounds__(WARPS * 32)
 fuzz_kernel(const __grid_constant__ KernelArgs args) {
-  static_assert(!(PROG && RECORD), "a campaign execution is recorded through demi_fuzz_trace on its program");
+  static_assert(!(PROG && RECORD) || (PARAMS && !TESTS),
+                "a campaign execution is recorded through demi_fuzz_trace on its program, or with its own parameters");
   static_assert(PROG || !TESTS, "random-oracle tests bind their programs as campaigns do");
-  static_assert(TESTS || !PARAMS, "per-program parameters are those of random-oracle tests");
+  static_assert(TESTS || !PARAMS || RECORD, "per-program parameters are those of random-oracle tests or recordings");
   using M = Machine<MODEL, PCAP, TCAP, PEND_GLOBAL, RECORD>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const uint32_t warp = threadIdx.x >> 5;
@@ -60,6 +63,10 @@ fuzz_kernel(const __grid_constant__ KernelArgs args) {
         r = demi_fuzz_result{};
         r.status = PS_SKIPPED;
       }
+    } else if constexpr (PROG && RECORD) {
+      int64_t seed;
+      prog_bind(la, args, idx, false, prog_params_bind(la, args.rec_params[idx], 0, seed));
+      m.run(seed, r);
     } else {
       if constexpr (PROG) prog_bind(la, args, idx, false);
       m.run(seed_at(args.seed_base, idx), r);

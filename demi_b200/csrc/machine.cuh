@@ -162,7 +162,7 @@ struct KernelArgs {
   // rec_counts[it*4 ..) = {n_events, n_nodes, affectedNodes, violation} and rec_parent[it*rec_parent_cap ..)
   union {
     demi_event* rec_events;
-    // the PARAMS kernels (demi_random_test_batch_many), which never record: test p's {seed_base lo, hi, max_messages
+    // the TESTS + PARAMS kernels (demi_random_test_batch_many), which never record: test p's {seed_base lo, hi, max_messages
     // as the caller gave it, looking_for}.  In the recording slot, so that the struct stays as it was.
     const uint4* prog_params;
   };
@@ -170,7 +170,13 @@ struct KernelArgs {
   // summary counters
   unsigned long long* sum_steps; unsigned long long* n_violations;
   // lane engine (lane_kernel.cuh)
-  uint4*    lane_pend;        // [total_warps][LPCAP][32] pending entries
+  union {
+    uint4*  lane_pend;        // [total_warps][LPCAP][32] pending entries
+    // the many-program recording kernels (demi_fuzz_traces_many), warp engine only: execution idx's {seed lo, hi,
+    // max_messages as the caller gave it, looking_for}, as `prog_params`.  In the lane engine's slot, which a warp-engine
+    // launch never reads, so that the struct stays as it was.
+    const uint4* rec_params;
+  };
   union {
     const uint4* ext_sends;   // the program's Send events as {hdr|EXTERNAL, p0, p1, 0}, in order
     // STEADY launches inject nothing and have no Send table: they read the program's pre-delivery snapshot
@@ -214,6 +220,16 @@ __device__ __forceinline__ void prog_bind(KernelArgs& la, const KernelArgs& args
 __device__ __forceinline__ void prog_bind(KernelArgs& la, const KernelArgs& args, uint64_t idx, bool lane) {
   prog_bind(la, args, idx, lane, args.prog_max_messages);
 }
+// A program's own parameters q = {seed base lo, hi, max_messages as the caller gave it, looking_for}: execution j of it
+// runs under seed base + j; binds max_messages (mapped as plan_launch maps it) and looking_for, and returns max_messages
+// unmapped, which the capacity rules read.
+__device__ __forceinline__ int32_t prog_params_bind(KernelArgs& la, const uint4 q, uint32_t j, int64_t& seed) {
+  seed = seed_at((int64_t)(((uint64_t)q.y << 32) | q.x), j);
+  const int32_t max_messages = (int32_t)q.z;
+  la.max_messages = max_messages < 0 ? 0x7FFFFFFF : max_messages;
+  la.looking_for = q.w;
+  return max_messages;
+}
 // A random-oracle test execution (the TESTS kernels): execution idx is execution j = idx % prog_execs of program
 // prog = idx / prog_execs, under seed_base + j.  Binds the program on every path (so that the copy stays in
 // registers) and returns false if the execution is skipped.  `lane`: one thread per execution (else a warp, kept
@@ -225,11 +241,7 @@ __device__ __forceinline__ bool prog_test_bind(KernelArgs& la, const KernelArgs&
   prog = p;
   int32_t max_messages = args.prog_max_messages;
   if constexpr (PARAMS) {
-    const uint4 q = args.prog_params[p];
-    seed = seed_at((int64_t)(((uint64_t)q.y << 32) | q.x), j);
-    max_messages = (int32_t)q.z;
-    la.max_messages = max_messages < 0 ? 0x7FFFFFFF : max_messages;   // as plan_launch maps it
-    la.looking_for = q.w;
+    max_messages = prog_params_bind(la, args.prog_params[p], j, seed);
   } else {
     seed = seed_at(args.seed_base, j);
   }

@@ -515,6 +515,43 @@ class Engine(object):
                                                    keys.ctypes.data, cap_iterations, out.ctypes.data, status.ctypes.data))
         return mcs, sizes, keys, out, status
 
+    def fuzz_traces_many(self, programs, seeds, max_messages, looking_for, interval, masks=None, cap_events=1024,
+                         cap_nodes=None, mask_words=None):
+        """demi_fuzz_traces_many: trace t is execution seeds[t] of programs[t] (or of one program shared by every
+        trace, passed once), or of the subsequence masks[t] keeps of it, with its own max_messages and looking_for (a
+        scalar applies to every trace).  Returns (events [n, cap_events], n_events [n], dep_parent [n, cap_nodes] or
+        None, n_nodes [n] or None, results [n], status [n]); row t holds n_events[t] events, what random_test_trace
+        (fuzz_trace for a full program) returns for it, and a trace whose status is not OK has no events."""
+        sd = np.ascontiguousarray(seeds, dtype=np.int64).reshape(-1)
+        n = len(sd)
+        multi = isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind")
+        if multi:
+            ext, eoff, n_ext = self._programs(programs, n)
+        else:                                # one program: every trace reads it at offset 0
+            ext, _, n1 = self._programs(programs, 1)
+            eoff = np.zeros(n, dtype=np.uint32)
+            n_ext = np.full(n, n1[0], dtype=np.uint32)
+        _, mm, lf = self._per_trace(0, max_messages, looking_for, n)
+        mw, mp = 0, None
+        if masks is not None:
+            mw = mask_words or max(1, (int(n_ext.max()) + 63) // 64)
+            m = np.ascontiguousarray(masks, dtype=np.uint64).reshape(n, mw)
+            mp = m.ctypes.data
+        ev = np.zeros((n, cap_events), dtype=N.EVENT_DTYPE)
+        ne = np.zeros(n, dtype=np.uint32)
+        par = np.zeros((n, cap_nodes), dtype=np.uint16) if cap_nodes else None
+        nn = np.zeros(n, dtype=np.uint32) if cap_nodes else None
+        res = np.zeros(n, dtype=N.RESULT_DTYPE)
+        status = np.zeros(n, dtype=np.int32)
+        p = N.FuzzParams(0, 0, -1, interval, 0, 0)
+        self._check(N.lib().demi_fuzz_traces_many(self._h, n, ext.ctypes.data, eoff.ctypes.data, n_ext.ctypes.data, mp, mw,
+                                                  sd.ctypes.data, mm.ctypes.data, lf.ctypes.data, C.byref(p),
+                                                  ev.ctypes.data, cap_events, ne.ctypes.data,
+                                                  par.ctypes.data if cap_nodes else None, cap_nodes or 0,
+                                                  nn.ctypes.data if cap_nodes else None, res.ctypes.data,
+                                                  status.ctypes.data))
+        return ev, ne, par, nn, res, status
+
     def random_test_trace(self, mask, seed, max_messages, interval=0, looking_for=0, cap_events=65536):
         """The EventTrace of execution `seed` of the mask's subsequence of the program (demi_random_test_trace): what
         RandomScheduler.test returns for it.  Accepts adjacent WaitQuiescence.  (result, EventTrace)."""

@@ -387,6 +387,36 @@ int32_t demi_fuzz_traces(demi_handle* h, const demi_fuzz_params* p, const uint32
 int32_t demi_fuzz_traces_tree(demi_handle* h, const demi_fuzz_params* p, const uint32_t* prefix_index, uint32_t n,
                               demi_event* events, uint32_t cap_events, uint32_t* n_events,
                               uint16_t* dep_parent, uint32_t cap_nodes, uint32_t* n_nodes, demi_fuzz_result* results);
+/* The EventTraces of n_traces executions of as many programs, recorded in shared launches: a campaign's violations, or
+ * randomDDMin's verified traces.  Trace t is the program externals[ext_offsets[t] ..] (n_externals[t] records; offsets in
+ * elements, so one program shared by every trace is all ext_offsets 0), of which it keeps what mask t
+ * (masks[t*mask_words ..]) keeps, or every event when masks is NULL; it runs under FullyRandom(seeds[t]) with
+ * max_messages[t] and looking_for[t].  Of p only invariant_check_interval and flags are read.
+ * status[t] is what demi_set_externals(h, program t) followed by demi_random_test_trace(h, mask t or all ones, p with t's
+ * three values, seeds[t], cap_events, ...) returns; when it is DEMI_OK, row t of events (cap_events records), n_events[t]
+ * and results[t] (results may be NULL) equal that call's outputs.  With an all-ones mask that is demi_fuzz_trace on
+ * program t; subsequences demi_set_externals would refuse (adjacent WaitQuiescence) are accepted as demi_random_test_trace
+ * accepts them.  With dep_parent, row t (cap_nodes entries) and n_nodes[t] are the DepTracker tree of that recording, for
+ * a full program what demi_fuzz_trace returns in dep_parent for that seed.
+ * A trace fails alone, with the single sequence's code and message: a program demi_set_externals rejects
+ * (DEMI_ERR_STATE for an empty one), a mask that keeps no event, no kernel variant for its capacities, or a nonzero
+ * prefix status (DEMI_ERR_CAPACITY; DEMI_PS_EVENT_OVF when cap_events is short, with its count and result as
+ * demi_fuzz_trace gives them).  A failing row has no events and no tree: zeros where they would be.  The call then
+ * returns DEMI_OK and demi_last_error names the lowest failing trace.  It fails only on invalid arguments (null required
+ * pointers, mask_words * 64 below some n_externals[t] when masks are given, cap_nodes 0 or above 65 536 with dep_parent)
+ * or a CUDA error.  Past n_events[t], row t's content is unspecified.
+ * Each execution runs under its own program's capacities, on the kernel variant its single call would use, so no record
+ * depends on which traces share a launch or on how the call is split into launches (at most ~4 GB of records and a
+ * 512 MB program arena each).  The warp engine records every execution.  The call neither reads nor changes the handle's
+ * program, trace or trace set; demi_perf counts its launches, its executions and their kernel time. */
+int32_t demi_fuzz_traces_many(demi_handle* h, uint32_t n_traces,
+                              const demi_ext_event* externals, const uint32_t* ext_offsets, const uint32_t* n_externals,
+                              const uint64_t* masks, uint32_t mask_words,
+                              const int64_t* seeds, const int32_t* max_messages, const uint32_t* looking_for,
+                              const demi_fuzz_params* p,
+                              demi_event* events, uint32_t cap_events, uint32_t* n_events,
+                              uint16_t* dep_parent, uint32_t cap_nodes, uint32_t* n_nodes,
+                              demi_fuzz_result* results, int32_t* status);
 /* A set of n_traces recorded executions to minimise, separate from the single trace of demi_set_trace (which it leaves
  * as it is).  Trace t is events[event_offsets[t] ..] (n_events[t] records) with the externals
  * externals[ext_offsets[t] ..] (n_externals[t] records); offsets are in elements, so the strided output of

@@ -369,6 +369,49 @@ class Engine {
     }
     return r;
   }
+  // demi_fuzz_traces_many: execution seeds[t] of programs[t] (of the subsequence masks[t] keeps of it, when masks is
+  // not empty), with its own setMaxMessages and violation; per trace its EventTrace, DepTracker tree (with_trees),
+  // record, or the error code
+  struct RecordedExecution { EventTrace trace; std::vector<uint16_t> depGraph; demi_fuzz_result result{}; int32_t status = DEMI_OK; };
+  std::vector<RecordedExecution> fuzz_traces_many(const std::vector<ExternalEvents>& programs, const std::vector<int64_t>& seeds,
+                                                  const std::vector<int32_t>& max_messages,
+                                                  const std::vector<ViolationFingerprint>& looking_for, int32_t interval,
+                                                  const std::vector<std::vector<uint64_t>>& masks = {}, bool with_trees = false,
+                                                  uint32_t cap_events = 4096, uint32_t cap_nodes = 4096) {
+    const size_t n = programs.size();
+    ExternalEvents flat; std::vector<uint32_t> off, cnt;
+    size_t words = 1;
+    for (const ExternalEvents& p : programs) {
+      off.push_back((uint32_t)flat.size()); cnt.push_back((uint32_t)p.size());
+      flat.insert(flat.end(), p.begin(), p.end());
+      words = std::max<size_t>(words, (p.size() + 63) / 64);
+    }
+    if (flat.empty()) flat.resize(1);
+    std::vector<uint64_t> mk;
+    if (!masks.empty())
+      for (size_t t = 0; t < n; t++) {
+        std::vector<uint64_t> row = masks.at(t);
+        row.resize(words, 0);
+        mk.insert(mk.end(), row.begin(), row.end());
+      }
+    const demi_fuzz_params p{0, 0, -1, interval, 0, 0};
+    std::vector<demi_event> ev(n * (size_t)cap_events);
+    std::vector<uint16_t> par(with_trees ? n * (size_t)cap_nodes : 0);
+    std::vector<uint32_t> ne(n), nn(n);
+    std::vector<demi_fuzz_result> res(n);
+    std::vector<int32_t> status(n);
+    check(demi_fuzz_traces_many(h, (uint32_t)n, flat.data(), off.data(), cnt.data(), mk.empty() ? nullptr : mk.data(), (uint32_t)words,
+                                seeds.data(), max_messages.data(), looking_for.data(), &p, ev.data(), cap_events, ne.data(),
+                                with_trees ? par.data() : nullptr, cap_nodes, nn.data(), res.data(), status.data()));
+    std::vector<RecordedExecution> r(n);
+    for (size_t t = 0; t < n; t++) {
+      r[t].result = res[t]; r[t].status = status[t];
+      if (status[t] != DEMI_OK) continue;
+      r[t].trace.assign(ev.begin() + t * cap_events, ev.begin() + t * cap_events + std::min(ne[t], cap_events));
+      if (with_trees) r[t].depGraph.assign(par.begin() + t * cap_nodes, par.begin() + t * cap_nodes + std::min(nn[t], cap_nodes));
+    }
+    return r;
+  }
   const SchedulerConfig cfg;
  private:
   demi_handle* h = nullptr;

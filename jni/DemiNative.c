@@ -274,6 +274,21 @@ JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_fuzzTracesTree
                                (uint16_t*)BUF(env, depParent), (uint32_t)capNodes, (uint32_t*)BUF(env, nNodes),
                                results ? (demi_fuzz_result*)BUF(env, results) : 0);
 }
+/* demi_fuzz_traces_many: execution seeds[t] of program t (offsets in elements), or of the subsequence mask t keeps (masks
+ * null: every event), each with its own maxMessages and lookingFor; status[t] is trace t's return code */
+JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_fuzzTracesMany(JNIEnv* env, jclass c, jlong h, jint nTraces,
+    jobject externals, jobject extOffsets, jobject nExternals, jobject masks, jint maskWords, jobject seeds, jobject maxMessages,
+    jobject lookingFor, jobject params, jobject events, jint capEvents, jobject nEvents, jobject depParent, jint capNodes,
+    jobject nNodes, jobject results, jobject status) {
+  return demi_fuzz_traces_many(H(h), (uint32_t)nTraces, (const demi_ext_event*)BUF(env, externals),
+                               (const uint32_t*)BUF(env, extOffsets), (const uint32_t*)BUF(env, nExternals),
+                               masks ? (const uint64_t*)BUF(env, masks) : 0, (uint32_t)maskWords, (const int64_t*)BUF(env, seeds),
+                               (const int32_t*)BUF(env, maxMessages), (const uint32_t*)BUF(env, lookingFor),
+                               (const demi_fuzz_params*)BUF(env, params), (demi_event*)BUF(env, events), (uint32_t)capEvents,
+                               (uint32_t*)BUF(env, nEvents), depParent ? (uint16_t*)BUF(env, depParent) : 0, (uint32_t)capNodes,
+                               nNodes ? (uint32_t*)BUF(env, nNodes) : 0, results ? (demi_fuzz_result*)BUF(env, results) : 0,
+                               (int32_t*)BUF(env, status));
+}
 JNIEXPORT jint JNICALL Java_akka_dispatch_verification_DemiNative_setTraces(JNIEnv* env, jclass c, jlong h, jint nTraces,
     jobject events, jobject eventOffsets, jobject nEvents, jobject externals, jobject extOffsets, jobject nExternals) {
   return demi_set_traces(H(h), (uint32_t)nTraces, (const demi_event*)BUF(env, events), (const uint32_t*)BUF(env, eventOffsets),

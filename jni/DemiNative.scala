@@ -92,6 +92,13 @@ object DemiNative {
   /** demi_fuzz_traces_tree: fuzzTraces plus each execution's DepTracker tree, execution i's at depParent + i*capNodes */
   @native def fuzzTracesTree(h: Long, params: ByteBuffer, prefixIndex: ByteBuffer, n: Int, events: ByteBuffer, capEvents: Int,
                              nEvents: ByteBuffer, depParent: ByteBuffer, capNodes: Int, nNodes: ByteBuffer, results: ByteBuffer): Int
+  /** demi_fuzz_traces_many: execution seeds(t) of program t (offsets in elements), or of the subsequence mask t keeps
+    * (masks null: every event), with its own maxMessages and lookingFor, recorded in shared launches; depParent null: no
+    * trees; status(t) is that trace's return code */
+  @native def fuzzTracesMany(h: Long, nTraces: Int, externals: ByteBuffer, extOffsets: ByteBuffer, nExternals: ByteBuffer,
+                             masks: ByteBuffer, maskWords: Int, seeds: ByteBuffer, maxMessages: ByteBuffer, lookingFor: ByteBuffer,
+                             params: ByteBuffer, events: ByteBuffer, capEvents: Int, nEvents: ByteBuffer, depParent: ByteBuffer,
+                             capNodes: Int, nNodes: ByteBuffer, results: ByteBuffer, status: ByteBuffer): Int
   /** demi_incremental_ddmin_many: RunnerUtils.editDistanceDporDDMin's minimisation of every trace t (offsets in elements;
     * seed t = seedEvents/seedParents at its offsets, seedEvents null: no seeds); status(t) is that trace's return code */
   @native def incrementalDdminMany(h: Long, nTraces: Int, externals: ByteBuffer, extOffsets: ByteBuffer, nExternals: ByteBuffer,
