@@ -329,6 +329,22 @@ static const LaneVariant* pick_lane_variant(const demi_handle* h, const ProgramI
 // ------------------------------------------------------------------- launch
 struct LaunchPlan { const Variant* v; LaunchMode mode; const ProgramInfo* prog; int grid; size_t smem; KernelArgs args; };
 
+// The variant (in *v, when v is given) that a launch of `mode` over a program `prog` describes runs on under h's
+// configuration, at pending capacity pcap and tosend capacity tcap.  Its two refusals, in this order, go to `to` (h, or
+// a trace's own handle): no variant fits, or SrcDstFIFO with a HardKill or a user filter.
+static int32_t check_variant(const demi_handle* h, demi_handle* to, LaunchMode mode, const ProgramInfo& prog, uint32_t pcap,
+                             uint32_t tcap, const Variant** v) {
+  const bool fifo = h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;          // SrcDstFIFO lives in the HBM-pending variants
+  // so does every program with a HardKill: Machine::hard_kill needs room for n_pending + matches <= 2 * pcap entries,
+  // which only the HBM variants (PCAP = 16384 >= 2 * 8192) have.  A random-oracle test decides on the base program.
+  const Variant* pv = pick_variant(h->cfg.model, mode, pcap, tcap, fifo || prog.hard_kill);
+  if (!pv) return fail(to, DEMI_ERR_CAPACITY, "no kernel variant for pending_cap=%u tosend_cap=%u", pcap, tcap);
+  if (fifo && (prog.hard_kill || !h->filter.empty()))
+    return fail(to, DEMI_ERR_INVALID, "HardKill and userDefinedFilter are offered for FullyRandom only");
+  if (v) *v = pv;
+  return DEMI_OK;
+}
+
 // A launch of `mode` over the program (ext, n_ext) that `prog` describes.  A campaign has no one program: `prog` is
 // its Fuzzer's, sized for the largest program, and each execution binds its own events.  Nor has a launch of many
 // traces' tests: `prog` joins its base programs, and `pcap_at_least` is the largest of their pending capacities,
@@ -343,13 +359,10 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, LaunchMode
   { int32_t mrc = demi_need_model(h); if (mrc != DEMI_OK) return mrc; }
   const uint32_t pcap = std::max(pcap_at_least, demi_pending_cap(demi_model_key(h), p->max_messages, prog.sends));
   const uint32_t tcap = demi_tosend_cap(prog.sends);
-  const bool fifo = h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;          // SrcDstFIFO lives in the HBM-pending variants
-  // so does every program with a HardKill: Machine::hard_kill needs room for n_pending + matches <= 2 * pcap entries,
-  // which only the HBM variants (PCAP = 16384 >= 2 * 8192) have.  A random-oracle test decides on the base program.
-  const Variant* v = pick_variant(h->cfg.model, mode, pcap, tcap, fifo || prog.hard_kill);
-  if (!v) return fail(h, DEMI_ERR_CAPACITY, "no kernel variant for pending_cap=%u tosend_cap=%u", pcap, tcap);
-  const size_t smem = v->smem_per_warp * WARPS;
+  const Variant* v;
   int32_t rc;
+  if ((rc = check_variant(h, h, mode, prog, pcap, tcap, &v)) != DEMI_OK) return rc;
+  const size_t smem = v->smem_per_warp * WARPS;
   int blocks_per_sm = 0;
   if ((rc = demi_occupancy(h, (const void*)v->fn[mode], WARPS * 32, smem, &blocks_per_sm)) != DEMI_OK) return rc;
   if (blocks_per_sm < 1) return fail(h, DEMI_ERR_CAPACITY, "kernel variant does not fit on an SM (smem %zu)", smem);
@@ -374,12 +387,10 @@ static int32_t plan_launch(demi_handle* h, const demi_fuzz_params* p, LaunchMode
   a.n_prefixes = p->n_prefixes;
   a.fuzz_flags = p->flags;
   a.strategy = h->cfg.strategy;
-  if (fifo) {
+  if (h->cfg.strategy == DEMI_RS_SRC_DST_FIFO) {
     if ((rc = h->fifo_scratch.grow(h, total_warps * (uint64_t)(v->pcap / 2 + 3 * FIFO_PAIRS) * sizeof(uint16_t))) != DEMI_OK) return rc;
     a.fifo_scratch = h->fifo_scratch.get<uint16_t>();
   }
-  if (fifo && (prog.hard_kill || !h->filter.empty()))
-    return fail(h, DEMI_ERR_INVALID, "HardKill and userDefinedFilter are offered for FullyRandom only");
   a.n_filter = (uint32_t)h->filter.size();
   for (uint32_t i = 0; i < a.n_filter; i++) a.filter[i] = make_uint4(h->filter[i].src_mask, h->filter[i].dst_mask, h->filter[i].type_mask, h->filter[i].flags);
   a.ext = ext;
@@ -1329,19 +1340,23 @@ extern "C" int32_t demi_random_ddmin(demi_handle* h, const demi_fuzz_params* p, 
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Random-oracle tests and randomDDMin over many traces: each trace has its own program, seed base, max_messages and
-// looking_for; the tests of every trace share launches of the PROG + TESTS + PARAMS engines.
+// Many programs in one call: random-oracle tests, randomDDMin and recorded executions over many traces, each trace
+// with its own program, seed base, max_messages and looking_for.  The work of every trace shares launches of the
+// PROG + PARAMS instantiations, packed by launch_many.
 namespace {
+
+// What a launch reads of the program of a trace (or of the subsequences its items keep): at most `len` events, the
+// pending capacity under the trace's max_messages, and what describe_event finds in it
+struct ManyProgram { uint32_t len = 0, pcap = 0; ProgramInfo info; };
 
 // A call's traces: their programs (the caller's externals, uploaded once), what each program's launches need, and what
 // a trace fails with before any launch.
-struct RandomSet {
+struct ProgramSet {
   const demi_handle* h = nullptr;              // the call's handle: the configuration every trace runs under
-  uint32_t n = 0, mask_words = 0;
-  const uint32_t* n_externals = nullptr;
+  uint32_t mask_words = 0;
   const int64_t* seed_base = nullptr; const int32_t* max_messages = nullptr; const uint32_t* looking_for = nullptr;
   demi_fuzz_params p{};                        // N, interval and flags
-  std::vector<ProgramInfo> info;
+  std::vector<ManyProgram> prog;               // each trace's whole program
   std::vector<int32_t> pre; std::vector<std::string> pre_msg;
   DevBuf dev;                                  // the externals, then uint2 {offset, length} per trace
   const demi_ext_event* progs = nullptr; const uint2* tab = nullptr;
@@ -1349,153 +1364,166 @@ struct RandomSet {
 
 // The checks demi_set_externals and demi_random_test_batch make of trace t's program before a launch; the call-wide
 // ones (N, mask_words) are the caller's.  The programs and their table are uploaded once.
-int32_t random_set(demi_handle* h, uint32_t n, const demi_ext_event* externals, const uint32_t* ext_offsets, const uint32_t* n_externals,
-                   const int64_t* seed_base, const int32_t* max_messages, const uint32_t* looking_for, const demi_fuzz_params* p,
-                   RandomSet& rs) {
-  rs.h = h; rs.n = n; rs.n_externals = n_externals; rs.seed_base = seed_base; rs.max_messages = max_messages; rs.looking_for = looking_for;
-  rs.p = *p;
-  rs.info.assign(n, ProgramInfo{}); rs.pre.assign(n, DEMI_OK); rs.pre_msg.assign(n, std::string());
+int32_t program_set(demi_handle* h, uint32_t n, const demi_ext_event* externals, const uint32_t* ext_offsets, const uint32_t* n_externals,
+                    const int64_t* seed_base, const int32_t* max_messages, const uint32_t* looking_for, const demi_fuzz_params* p,
+                    ProgramSet& ps) {
+  ps.h = h; ps.seed_base = seed_base; ps.max_messages = max_messages; ps.looking_for = looking_for;
+  ps.p = *p;
+  ps.prog.assign(n, ManyProgram{}); ps.pre.assign(n, DEMI_OK); ps.pre_msg.assign(n, std::string());
   uint64_t span = 0;
   std::vector<uint2> tab(n);
   demi_handle eh;
   for (uint32_t t = 0; t < n; t++) {
     const demi_ext_event* ev = externals + ext_offsets[t];
+    ManyProgram& pg = ps.prog[t];
     std::vector<uint4> sv;
     int32_t rc = DEMI_OK;
     eh.err.clear();
     eh.cfg = h->cfg; eh.ir_n_actors = h->ir_n_actors;            // demi_model_actors reads these
     for (uint32_t i = 0; i < n_externals[t] && rc == DEMI_OK; i++) {
       rc = demi_check_external(&eh, "demi_set_externals", "", ev, i, true, true);
-      if (rc == DEMI_OK) describe_event(&rs.info[t], &sv, ev[i]);
+      if (rc == DEMI_OK) describe_event(&pg.info, &sv, ev[i]);
     }
     if (rc == DEMI_OK && !n_externals[t]) rc = fail(&eh, DEMI_ERR_STATE, "demi_set_externals has not been called");
-    if (rc != DEMI_OK) { rs.pre[t] = rc; rs.pre_msg[t] = eh.err; continue; }
+    if (rc != DEMI_OK) { ps.pre[t] = rc; ps.pre_msg[t] = eh.err; continue; }
+    pg.len = n_externals[t];
+    pg.pcap = demi_pending_cap(demi_model_key(h), max_messages[t], pg.info.sends);   // demi_random_test_batch's
     tab[t] = make_uint2(ext_offsets[t], n_externals[t]);
     span = std::max<uint64_t>(span, (uint64_t)ext_offsets[t] + n_externals[t]);
   }
   const size_t b_ev = ((size_t)span * sizeof(demi_ext_event) + 15) & ~(size_t)15;
-  int32_t rc = rs.dev.grow(h, b_ev + (size_t)n * sizeof(uint2));
+  int32_t rc = ps.dev.grow(h, b_ev + (size_t)n * sizeof(uint2));
   if (rc != DEMI_OK) return rc;
-  if (span) CUDA_TRY(h, cudaMemcpy(rs.dev.get(), externals, (size_t)span * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
-  CUDA_TRY(h, cudaMemcpy(rs.dev.get<char>() + b_ev, tab.data(), (size_t)n * sizeof(uint2), cudaMemcpyHostToDevice));
-  rs.progs = rs.dev.get<demi_ext_event>(); rs.tab = (const uint2*)(rs.dev.get<char>() + b_ev);
+  if (span) CUDA_TRY(h, cudaMemcpy(ps.dev.get(), externals, (size_t)span * sizeof(demi_ext_event), cudaMemcpyHostToDevice));
+  CUDA_TRY(h, cudaMemcpy(ps.dev.get<char>() + b_ev, tab.data(), (size_t)n * sizeof(uint2), cudaMemcpyHostToDevice));
+  ps.progs = ps.dev.get<demi_ext_event>(); ps.tab = (const uint2*)(ps.dev.get<char>() + b_ev);
   return DEMI_OK;
 }
 
-// trace t's pending capacity under its own max_messages (demi_random_test_batch's, from its base program)
-uint32_t random_pcap(const RandomSet& rs, uint32_t t) {
-  return demi_pending_cap(demi_model_key(rs.h), rs.max_messages[t], rs.info[t].sends);
-}
+// A unit of work of a many-program launch: a test or an execution over the subsequence of trace `trace`'s program that
+// `mask` keeps.  Only items of the same key share a launch.
+struct ManyItem { uint32_t trace, key; const uint64_t* mask; };
 
-// What plan_launch refuses of a launch over trace t's program alone, in its order; the message goes to `h` (a driver's
-// own handle, or the call's).
-int32_t random_trace_launchable(demi_handle* h, const RandomSet& rs, uint32_t t) {
-  const bool fifo = rs.h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;
-  const uint32_t pcap = random_pcap(rs, t), tcap = demi_tosend_cap(rs.info[t].sends);
-  if (!pick_variant(rs.h->cfg.model, LM_TEST_PARAMS, pcap, tcap, fifo || rs.info[t].hard_kill))
-    return fail(h, DEMI_ERR_CAPACITY, "no kernel variant for pending_cap=%u tosend_cap=%u", pcap, tcap);
-  if (fifo && (rs.info[t].hard_kill || !rs.h->filter.empty()))
-    return fail(h, DEMI_ERR_INVALID, "HardKill and userDefinedFilter are offered for FullyRandom only");
+// One launch of launch_many, for its caller to finish: the plan with the programs bound, the items' parameter table on
+// the device, the caller's bytes, and the launch's m items (indices into the call's list).
+struct ManyLaunch { LaunchPlan& plan; const uint4* params; unsigned char* extra; const uint32_t* item; uint32_t m; };
+
+// Launches `items` (masks of mw words) over the programs of `ps` in launches of `mode`, `execs` executions per item;
+// progs[t] describes what the items of trace t keep.  The items go out grouped by key, in increasing key order, each
+// group cut greedily into launches of at most `cap` items and an arena of at most 512 MB, whose program stride is the
+// launch's longest program and which counts `extra` bytes of the caller's per item.  Per launch: the arena, laid out
+// programs | masks | parameters {seed lo, seed hi, max_messages, looking_for} | trace ids | the caller's 16 + m * extra
+// bytes; a plan with the launch's merged ProgramInfo and largest pending capacity (each item binds its own
+// max_messages); random_subseq_many_kernel; then run(ManyLaunch&), which binds what its mode needs and launches.
+template <class Run>
+int32_t launch_many(demi_handle* h, const ProgramSet& ps, LaunchMode mode, uint32_t execs, const ManyProgram* progs,
+                    const std::vector<ManyItem>& items, uint32_t mw, uint64_t cap, size_t extra, Run run) {
+  std::vector<uint32_t> order(items.size());
+  for (uint32_t i = 0; i < order.size(); i++) order[i] = i;
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return items[a].key < items[b].key; });
+  cudaStream_t s = h->stream;
+  std::vector<uint64_t> hm;
+  std::vector<uint4> hp;
+  std::vector<uint32_t> ht;
+  for (size_t lo = 0; lo < order.size();) {
+    uint32_t stride = 1, send_stride = 1, pcap = 0;
+    ProgramInfo li;
+    size_t hi = lo;
+    for (; hi < order.size() && hi - lo < cap && items[order[hi]].key == items[order[lo]].key; hi++) {
+      const ManyProgram& pg = progs[items[order[hi]].trace];
+      const uint32_t st = std::max(stride, pg.len), ss = std::max(send_stride, pg.info.sends);
+      const uint64_t per = (uint64_t)st * sizeof(demi_ext_event) + sizeof(uint2) + (uint64_t)ss * sizeof(uint4) + (uint64_t)mw * 8 +
+                           sizeof(uint4) + 4 + extra;
+      if (hi > lo && (hi - lo + 1) * per > ((uint64_t)512 << 20)) break;
+      stride = st; send_stride = ss;
+      pcap = std::max(pcap, pg.pcap);
+      li.sends = std::max(li.sends, pg.info.sends);
+      li.hard_kill |= pg.info.hard_kill; li.partitions |= pg.info.partitions;
+      li.sends_distinct &= pg.info.sends_distinct;
+    }
+    const uint32_t m = (uint32_t)(hi - lo);
+    auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    const size_t b_mask = al((size_t)m * mw * 8), b_par = al((size_t)m * sizeof(uint4)), b_tr = al((size_t)m * 4);
+    ProgramArena pa;
+    unsigned char* rest;
+    int32_t rc = carve_programs(h, m, stride, send_stride, b_mask + b_par + b_tr + 16 + (size_t)m * extra, &pa, &rest);
+    if (rc != DEMI_OK) return rc;
+    uint64_t* mdev = (uint64_t*)rest;
+    uint4* pdev = (uint4*)(rest + b_mask);
+    uint32_t* tdev = (uint32_t*)(rest + b_mask + b_par);
+    hm.resize((size_t)m * mw); hp.resize(m); ht.resize(m);
+    for (uint32_t k = 0; k < m; k++) {
+      const ManyItem& it = items[order[lo + k]];
+      std::copy(it.mask, it.mask + mw, hm.begin() + (size_t)k * mw);
+      const uint64_t sb = (uint64_t)ps.seed_base[it.trace];
+      hp[k] = make_uint4((uint32_t)sb, (uint32_t)(sb >> 32), (uint32_t)ps.max_messages[it.trace], ps.looking_for[it.trace]);
+      ht[k] = it.trace;
+    }
+    CUDA_TRY(h, cudaMemcpyAsync(mdev, hm.data(), hm.size() * 8, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(h, cudaMemcpyAsync(pdev, hp.data(), hp.size() * sizeof(uint4), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(h, cudaMemcpyAsync(tdev, ht.data(), ht.size() * 4, cudaMemcpyHostToDevice, s));
+    demi_fuzz_params q = ps.p;
+    q.n_prefixes = (uint64_t)m * execs;
+    q.max_messages = -1;                   // each item binds its own (prog_params_bind); pcap covers them all
+    q.looking_for = 0; q.seed_base = 0;
+    LaunchPlan plan;
+    if ((rc = plan_launch(h, &q, mode, li, nullptr, 0, &plan, pcap)) != DEMI_OK) return rc;
+    bind_programs(h, plan.args, pa, -1);
+    random_subseq_many_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(ps.progs, ps.tab, tdev, mdev, mw, m, pa.ev,
+                                                                                        stride, pa.hdr, pa.sends, send_stride);
+    CUDA_TRY(h, cudaGetLastError());
+    h->perf.kernel_launches++;
+    ManyLaunch L{plan, pdev, rest + b_mask + b_par + b_tr, order.data() + lo, m};
+    if ((rc = run(L)) != DEMI_OK) return rc;
+    lo = hi;
+  }
   return DEMI_OK;
 }
 
 // A test's record and the executions of it that ran
 struct RandomRec { demi_random_test_result rec; uint32_t ran; };
 
-// n tests: test i is masks[i * mask_words ..) over the program of trace tr[i], which random_trace_launchable accepts.
-// The tests go out in at most two groups, the programs the lane engine takes and the others (so that one HardKill
-// program does not send every test to the warp engine), each cut into launches of at most RANDOM_EXECS_PER_LAUNCH
-// executions and a 512 MB arena whose stride is the launch's largest program.
-int32_t random_tests_many(demi_handle* h, const RandomSet& rs, const uint32_t* tr, const uint64_t* masks, size_t n, RandomRec* out) {
-  const uint32_t N = (uint32_t)rs.p.n_prefixes, mw = rs.mask_words;
-  std::vector<size_t> group[2];
-  for (size_t i = 0; i < n; i++) group[pick_lane_variant(h, rs.info[tr[i]]) ? 0 : 1].push_back(i);
+// n tests: test i is masks[i * mask_words ..) over the program of trace tr[i], which check_variant accepts.  The tests
+// go out in at most two groups, the programs the lane engine takes and the others (so that one HardKill program does
+// not send every test to the warp engine), in launches of at most RANDOM_EXECS_PER_LAUNCH executions.
+int32_t random_tests_many(demi_handle* h, const ProgramSet& ps, const uint32_t* tr, const uint64_t* masks, size_t n, RandomRec* out) {
+  const uint32_t N = (uint32_t)ps.p.n_prefixes, mw = ps.mask_words;
+  std::vector<ManyItem> items(n);
+  for (size_t i = 0; i < n; i++) items[i] = ManyItem{tr[i], pick_lane_variant(h, ps.prog[tr[i]].info) ? 0u : 1u, masks + i * mw};
   cudaStream_t s = h->stream;
-  std::vector<uint64_t> hm;
-  std::vector<uint4> hp;
-  std::vector<uint32_t> ht, hran;
+  std::vector<uint32_t> hran;
   std::vector<demi_random_test_result> hrec;
-  for (const std::vector<size_t>& g : group) {
-    for (size_t lo = 0; lo < g.size();) {
-      uint32_t stride = 1, send_stride = 1, pcap = 0;
-      ProgramInfo li;
-      size_t hi = lo;
-      for (; hi < g.size(); hi++) {
-        const uint32_t t = tr[g[hi]];
-        const uint32_t st = std::max(stride, rs.n_externals[t]), ss = std::max(send_stride, rs.info[t].sends);
-        const uint64_t per_test = (uint64_t)st * sizeof(demi_ext_event) + sizeof(uint2) + (uint64_t)ss * sizeof(uint4) +
-                                  (uint64_t)mw * 8 + sizeof(demi_random_test_result) + 4 + 4 + sizeof(uint4) + 4;
-        const uint64_t m = hi - lo + 1;
-        if (hi > lo && (m * N > RANDOM_EXECS_PER_LAUNCH || m * per_test > ((uint64_t)512 << 20))) break;
-        stride = st; send_stride = ss;
-        pcap = std::max(pcap, random_pcap(rs, t));
-        li.sends = std::max(li.sends, rs.info[t].sends);
-        li.hard_kill |= rs.info[t].hard_kill; li.partitions |= rs.info[t].partitions;
-        li.sends_distinct &= rs.info[t].sends_distinct;
-      }
-      const uint32_t m = (uint32_t)(hi - lo);
-      // arena: the programs | masks | first_hit | test records | executions that ran | parameters | traces | counter
-      auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
-      const size_t b_mask = al((size_t)m * mw * 8), b_fh = al((size_t)m * 4), b_out = al((size_t)m * sizeof(demi_random_test_result)),
-                   b_ran = al((size_t)m * 4), b_par = al((size_t)m * sizeof(uint4)), b_tr = al((size_t)m * 4);
-      ProgramArena pa;
-      unsigned char* rest;
-      int32_t rc = carve_programs(h, m, stride, send_stride, b_mask + b_fh + b_out + b_ran + b_par + b_tr + 16, &pa, &rest);
-      if (rc != DEMI_OK) return rc;
-      if ((rc = h->results_dev.grow(h, std::max<size_t>((size_t)m * N * sizeof(demi_fuzz_result), 32))) != DEMI_OK) return rc;
-      uint64_t* mdev = (uint64_t*)rest;
-      uint32_t* first_hit = (uint32_t*)(rest + b_mask);
-      demi_random_test_result* odev = (demi_random_test_result*)(rest + b_mask + b_fh);
-      uint32_t* rdev = (uint32_t*)(rest + b_mask + b_fh + b_out);
-      uint4* pdev = (uint4*)(rest + b_mask + b_fh + b_out + b_ran);
-      uint32_t* tdev = (uint32_t*)(rest + b_mask + b_fh + b_out + b_ran + b_par);
-      unsigned long long* cnt = (unsigned long long*)(rest + b_mask + b_fh + b_out + b_ran + b_par + b_tr);
-      hm.resize((size_t)m * mw); hp.resize(m); ht.resize(m);
-      for (uint32_t k = 0; k < m; k++) {
-        const size_t i = g[lo + k];
-        const uint32_t t = tr[i];
-        std::copy(masks + i * mw, masks + (i + 1) * mw, hm.begin() + (size_t)k * mw);
-        const uint64_t sb = (uint64_t)rs.seed_base[t];
-        hp[k] = make_uint4((uint32_t)sb, (uint32_t)(sb >> 32), (uint32_t)rs.max_messages[t], rs.looking_for[t]);
-        ht[k] = t;
-      }
-      CUDA_TRY(h, cudaMemcpyAsync(mdev, hm.data(), hm.size() * 8, cudaMemcpyHostToDevice, s));
-      CUDA_TRY(h, cudaMemcpyAsync(pdev, hp.data(), hp.size() * sizeof(uint4), cudaMemcpyHostToDevice, s));
-      CUDA_TRY(h, cudaMemcpyAsync(tdev, ht.data(), ht.size() * 4, cudaMemcpyHostToDevice, s));
-      CUDA_TRY(h, cudaMemsetAsync(first_hit, 0xFF, (size_t)m * 4, s));
-      CUDA_TRY(h, cudaMemsetAsync(cnt, 0, sizeof(unsigned long long), s));
-      demi_fuzz_params q = rs.p;
-      q.n_prefixes = (uint64_t)m * N;
-      q.max_messages = -1;                 // each test binds its own (prog_test_bind); pcap covers them all
-      q.looking_for = 0; q.seed_base = 0;
-      LaunchPlan plan;
-      if ((rc = plan_launch(h, &q, LM_TEST_PARAMS, li, nullptr, 0, &plan, pcap)) != DEMI_OK) return rc;
-      random_subseq_many_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(rs.progs, rs.tab, tdev, mdev, mw, m, pa.ev,
-                                                                                          stride, pa.hdr, pa.sends, send_stride);
-      CUDA_TRY(h, cudaGetLastError());
-      h->perf.kernel_launches++;
-      KernelArgs& a = plan.args;
-      a.results = h->results_dev.get<demi_fuzz_result>();
-      bind_programs(h, a, pa, -1);
-      a.prog_execs = N;
-      a.prog_first_hit = first_hit;
-      a.prog_params = pdev;
-      if ((rc = launch_plan(h, plan, q.n_prefixes, s)) != DEMI_OK) return rc;
-      random_test_reduce_kernel<true><<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(a.results, m, N, odev, cnt, rdev);
-      CUDA_TRY(h, cudaGetLastError());
-      h->perf.kernel_launches++;
-      hrec.resize(m); hran.resize(m);
-      CUDA_TRY(h, cudaMemcpyAsync(hrec.data(), odev, (size_t)m * sizeof(demi_random_test_result), cudaMemcpyDeviceToHost, s));
-      CUDA_TRY(h, cudaMemcpyAsync(hran.data(), rdev, (size_t)m * 4, cudaMemcpyDeviceToHost, s));
-      CUDA_TRY(h, cudaStreamSynchronize(s));
-      for (uint32_t k = 0; k < m; k++) {
-        out[g[lo + k]] = RandomRec{hrec[k], hran[k]};
-        h->perf.prefixes += hran[k];
-      }
-      lo = hi;
+  return launch_many(h, ps, LM_TEST_PARAMS, N, ps.prog.data(), items, mw, RANDOM_EXECS_PER_LAUNCH / N,
+                     sizeof(demi_random_test_result) + 4 + 4, [&](ManyLaunch& L) -> int32_t {
+    // the caller's bytes: counter | test records | first_hit | executions that ran
+    const uint32_t m = L.m;
+    unsigned long long* cnt = (unsigned long long*)L.extra;
+    demi_random_test_result* odev = (demi_random_test_result*)(L.extra + 16);
+    uint32_t* first_hit = (uint32_t*)(odev + m);
+    uint32_t* rdev = first_hit + m;
+    int32_t rc = h->results_dev.grow(h, std::max<size_t>((size_t)m * N * sizeof(demi_fuzz_result), 32));
+    if (rc != DEMI_OK) return rc;
+    CUDA_TRY(h, cudaMemsetAsync(first_hit, 0xFF, (size_t)m * 4, s));
+    CUDA_TRY(h, cudaMemsetAsync(cnt, 0, sizeof(unsigned long long), s));
+    KernelArgs& a = L.plan.args;
+    a.results = h->results_dev.get<demi_fuzz_result>();
+    a.prog_execs = N;
+    a.prog_first_hit = first_hit;
+    a.prog_params = L.params;
+    if ((rc = launch_plan(h, L.plan, (uint64_t)m * N, s)) != DEMI_OK) return rc;
+    random_test_reduce_kernel<true><<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(a.results, m, N, odev, cnt, rdev);
+    CUDA_TRY(h, cudaGetLastError());
+    h->perf.kernel_launches++;
+    hrec.resize(m); hran.resize(m);
+    CUDA_TRY(h, cudaMemcpyAsync(hrec.data(), odev, (size_t)m * sizeof(demi_random_test_result), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(h, cudaMemcpyAsync(hran.data(), rdev, (size_t)m * 4, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(h, cudaStreamSynchronize(s));
+    for (uint32_t k = 0; k < m; k++) {
+      out[L.item[k]] = RandomRec{hrec[k], hran[k]};
+      h->perf.prefixes += hran[k];
     }
-  }
-  return DEMI_OK;
+    return DEMI_OK;
+  });
 }
 
 // The call-wide checks of both entry points: what demi_random_test_batch / demi_random_ddmin refuse whatever the program
@@ -1517,9 +1545,10 @@ typedef ManyRequest<RandomRec> RandomRequest;
 
 // randomDDMin on trace `trace` of a demi_random_ddmin_many call: its batches join the rendezvous
 struct ManyRandomDriver : RandomDDMinDriver {
-  Rendezvous<RandomRec>* R; uint32_t trace; const RandomSet* rs;
+  Rendezvous<RandomRec>* R; uint32_t trace; const ProgramSet* ps;
   int32_t run_tests(const uint64_t* masks, size_t n, demi_random_test_result* res, uint64_t* executed) override {
-    int32_t rc = random_trace_launchable(h, *rs, trace);       // what plan_launch refuses of this trace's launch alone
+    const ManyProgram& pg = ps->prog[trace];             // what plan_launch refuses of this trace's launch alone
+    int32_t rc = check_variant(ps->h, h, LM_TEST_PARAMS, pg.info, pg.pcap, demi_tosend_cap(pg.info.sends), nullptr);
     if (rc != DEMI_OK) return rc;
     RandomRequest q;
     q.trace = trace; q.masks = masks; q.n = n;
@@ -1549,17 +1578,21 @@ extern "C" int32_t demi_random_test_batch_many(demi_handle* h, uint32_t n_traces
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   h->perf.kernel_launches = 0; h->perf.prefixes = 0;
   if (!n_tests) return DEMI_OK;
-  RandomSet rs;
-  rs.mask_words = mask_words;
-  if ((rc = random_set(h, n_traces, externals, ext_offsets, n_externals, seed_base, max_messages, looking_for, p, rs)) != DEMI_OK) return rc;
+  ProgramSet ps;
+  ps.mask_words = mask_words;
+  if ((rc = program_set(h, n_traces, externals, ext_offsets, n_externals, seed_base, max_messages, looking_for, p, ps)) != DEMI_OK) return rc;
   // a test fails the call with what its program alone would give
   for (uint32_t i = 0; i < n_tests; i++) {
     const uint32_t t = trace_of_test[i];
-    if (rs.pre[t] != DEMI_OK) { h->err = std::string(who) + ": trace " + std::to_string(t) + ": " + rs.pre_msg[t]; return rs.pre[t]; }
-    if ((rc = random_trace_launchable(h, rs, t)) != DEMI_OK) { h->err = std::string(who) + ": trace " + std::to_string(t) + ": " + h->err; return rc; }
+    const ManyProgram& pg = ps.prog[t];
+    if (ps.pre[t] != DEMI_OK) { h->err = trace_msg(who, t, ps.pre_msg[t]); return ps.pre[t]; }
+    if ((rc = check_variant(h, h, LM_TEST_PARAMS, pg.info, pg.pcap, demi_tosend_cap(pg.info.sends), nullptr)) != DEMI_OK) {
+      h->err = trace_msg(who, t, h->err);
+      return rc;
+    }
   }
   std::vector<RandomRec> res(n_tests);
-  if ((rc = random_tests_many(h, rs, trace_of_test, masks, n_tests, res.data())) != DEMI_OK) return rc;
+  if ((rc = random_tests_many(h, ps, trace_of_test, masks, n_tests, res.data())) != DEMI_OK) return rc;
   for (uint32_t i = 0; i < n_tests; i++) out[i] = res[i].rec;
   return DEMI_OK;
 }
@@ -1583,34 +1616,27 @@ extern "C" int32_t demi_random_ddmin_many(demi_handle* h, uint32_t n_traces, con
   CUDA_TRY(h, cudaSetDevice(h->cfg.device));
   memset(out, 0, (size_t)n * sizeof(demi_random_ddmin_out));
   h->perf.kernel_launches = 0; h->perf.prefixes = 0;
-  RandomSet rs;
-  rs.mask_words = mask_words;
-  if ((rc = random_set(h, n, externals, ext_offsets, n_externals, seed_base, max_messages, looking_for, p, rs)) != DEMI_OK) return rc;
+  ProgramSet ps;
+  ps.mask_words = mask_words;
+  if ((rc = program_set(h, n, externals, ext_offsets, n_externals, seed_base, max_messages, looking_for, p, ps)) != DEMI_OK) return rc;
   demi_perf perf{};
   // the union of a round's requests, in request order
   auto serve = [&](std::vector<RandomRequest*>& batch) -> int32_t {
     std::vector<uint32_t> tos;
     std::vector<uint64_t> flat;
-    for (const RandomRequest* q : batch) {
-      tos.insert(tos.end(), q->n, q->trace);
-      flat.insert(flat.end(), q->masks, q->masks + q->n * mask_words);
-    }
+    flatten_requests(batch, mask_words, tos, flat);
     std::vector<RandomRec> res(tos.size());
-    const int32_t src = random_tests_many(h, rs, tos.data(), flat.data(), tos.size(), res.data());
+    const int32_t src = random_tests_many(h, ps, tos.data(), flat.data(), tos.size(), res.data());
     perf.kernel_launches += h->perf.kernel_launches; perf.prefixes += h->perf.prefixes;
     h->perf.kernel_launches = 0; h->perf.prefixes = 0;
     if (src != DEMI_OK) return src;
-    size_t k = 0;
-    for (RandomRequest* q : batch) {
-      q->res.assign(res.begin() + k, res.begin() + k + q->n);
-      k += q->n;
-    }
+    scatter_results(batch, res);
     return DEMI_OK;
   };
   auto drive = [&](uint32_t t, Rendezvous<RandomRec>& R, demi_handle* eh) -> int32_t {
-    if (rs.pre[t] != DEMI_OK) { eh->err = rs.pre_msg[t]; return rs.pre[t]; }
+    if (ps.pre[t] != DEMI_OK) { eh->err = ps.pre_msg[t]; return ps.pre[t]; }
     ManyRandomDriver d;
-    d.R = &R; d.trace = t; d.rs = &rs;
+    d.R = &R; d.trace = t; d.ps = &ps;
     d.h = eh; d.looking_for = looking_for[t]; d.mw = mask_words; d.n_ext = n_externals[t];
     d.ext = externals + ext_offsets[t];
     d.set_width(p->n_prefixes);
@@ -1622,7 +1648,7 @@ extern "C" int32_t demi_random_ddmin_many(demi_handle* h, uint32_t n_traces, con
   h->perf.kernel_launches = perf.kernel_launches; h->perf.prefixes = perf.prefixes;
   if (rc != DEMI_OK) return rc;
   for (uint32_t t = 0; t < n; t++)
-    if (status[t] != DEMI_OK) { h->err = std::string(who) + ": trace " + std::to_string(t) + ": " + h->err; break; }
+    if (status[t] != DEMI_OK) { h->err = trace_msg(who, t, h->err); break; }
   return DEMI_OK;
 }
 
@@ -1665,160 +1691,101 @@ extern "C" int32_t demi_fuzz_traces_many(demi_handle* h, uint32_t n_traces, cons
   if (n_nodes) memset(n_nodes, 0, (size_t)n * sizeof(uint32_t));
   if (results) memset(results, 0, (size_t)n * sizeof(demi_fuzz_result));
   // demi_set_externals's checks of each program; the programs are uploaded once
-  RandomSet rs;
-  int32_t rc = random_set(h, n, externals, ext_offsets, n_externals, seeds, max_messages, looking_for, p, rs);
+  ProgramSet ps;
+  int32_t rc = program_set(h, n, externals, ext_offsets, n_externals, seeds, max_messages, looking_for, p, ps);
   if (rc != DEMI_OK) return rc;
   // Then demi_random_test_trace's and plan_launch's of each subsequence.  Every execution runs on the variant its single
   // call picks: the traces are grouped by it, so that a HardKill or SrcDstFIFO program moves no other program.
   uint32_t mw = masks ? mask_words : 1;                // without masks every trace keeps all: one row of ones serves all
   if (!masks) for (uint32_t t = 0; t < n; t++) mw = std::max(mw, (n_externals[t] + 63) / 64);
   const std::vector<uint64_t> ones(mw, ~0ull);
-  const bool fifo = h->cfg.strategy == DEMI_RS_SRC_DST_FIFO;
-  std::vector<uint32_t> kept(n, 0), sends(n, 0), pcap(n, 0);
-  std::vector<bool> hard_kill(n, false);
-  std::vector<const Variant*> var(n, nullptr);
+  std::vector<ManyProgram> sub(n);                     // what each trace's mask keeps
+  std::vector<ManyItem> items;
   std::vector<std::string> msg(n);
-  char buf[160];
+  demi_handle eh;                                      // a trace's refusal
   for (uint32_t t = 0; t < n; t++) {
-    status[t] = rs.pre[t];
-    if (rs.pre[t] != DEMI_OK) { msg[t] = rs.pre_msg[t]; continue; }
+    status[t] = ps.pre[t];
+    if (ps.pre[t] != DEMI_OK) { msg[t] = ps.pre_msg[t]; continue; }
     const demi_ext_event* ev = externals + ext_offsets[t];
     const uint64_t* mk = masks ? masks + (size_t)t * mask_words : ones.data();
+    ManyProgram& sp = sub[t];
     for (uint32_t i = 0; i < n_externals[t]; i++)
       if ((mk[i >> 6] >> (i & 63)) & 1ull) {
-        kept[t]++;
-        if (ev[i].kind == DEMI_EXT_SEND) sends[t]++;
-        if (ev[i].kind == DEMI_EXT_HARD_KILL) hard_kill[t] = true;
+        sp.len++;
+        if (ev[i].kind == DEMI_EXT_SEND) sp.info.sends++;
+        if (ev[i].kind == DEMI_EXT_HARD_KILL) sp.info.hard_kill = true;
       }
-    if (!kept[t]) { status[t] = DEMI_ERR_INVALID; msg[t] = "demi_random_test_trace: the mask keeps no event"; continue; }
-    pcap[t] = demi_pending_cap(demi_model_key(h), max_messages[t], sends[t]);
-    const uint32_t tcap = demi_tosend_cap(sends[t]);
-    var[t] = pick_variant(h->cfg.model, LM_RECORD_PARAMS, pcap[t], tcap, fifo || hard_kill[t]);
-    if (!var[t]) {
-      snprintf(buf, sizeof(buf), "no kernel variant for pending_cap=%u tosend_cap=%u", pcap[t], tcap);
-      status[t] = DEMI_ERR_CAPACITY; msg[t] = buf;
-    } else if (fifo && (hard_kill[t] || !h->filter.empty())) {
-      status[t] = DEMI_ERR_INVALID; msg[t] = "HardKill and userDefinedFilter are offered for FullyRandom only";
-      var[t] = nullptr;
-    }
+    if (!sp.len) { status[t] = DEMI_ERR_INVALID; msg[t] = "demi_random_test_trace: the mask keeps no event"; continue; }
+    sp.pcap = demi_pending_cap(demi_model_key(h), max_messages[t], sp.info.sends);
+    const Variant* v;
+    status[t] = check_variant(h, &eh, LM_RECORD_PARAMS, sp.info, sp.pcap, demi_tosend_cap(sp.info.sends), &v);
+    if (status[t] != DEMI_OK) { msg[t] = eh.err; continue; }
+    items.push_back(ManyItem{t, (uint32_t)(v - variants().data()), mk});
   }
   const uint32_t par_cap = dep_parent ? cap_nodes : 0;
-  const uint32_t chunk = fuzz_many_chunk(cap_events, par_cap);
   cudaStream_t s = h->stream;
   DevBuf rbuf;
-  std::vector<uint64_t> hm;
-  std::vector<uint4> hp;
-  std::vector<uint32_t> ht, cnt;
+  std::vector<uint32_t> cnt;
   std::vector<demi_fuzz_result> res;
   std::vector<demi_event> hev;
   std::vector<uint16_t> hpar;
   double ms_all = 0;
-  for (const Variant& v : variants()) {
-    std::vector<uint32_t> g;
-    for (uint32_t t = 0; t < n; t++) if (var[t] == &v) g.push_back(t);
-    // launches of at most `chunk` slots and a 512 MB program arena whose stride is the launch's longest subsequence
-    for (size_t lo = 0; lo < g.size();) {
-      uint32_t stride = 1, send_stride = 1, pc = 0;
-      ProgramInfo li;
-      size_t hi = lo;
-      for (; hi < g.size() && hi - lo < chunk; hi++) {
-        const uint32_t t = g[hi];
-        const uint32_t st = std::max(stride, kept[t]), ss = std::max(send_stride, sends[t]);
-        const uint64_t per = (uint64_t)st * sizeof(demi_ext_event) + sizeof(uint2) + (uint64_t)ss * sizeof(uint4) + (uint64_t)mw * 8 +
-                             sizeof(uint4) + 4;
-        if (hi > lo && (hi - lo + 1) * per > ((uint64_t)512 << 20)) break;
-        stride = st; send_stride = ss;
-        pc = std::max(pc, pcap[t]);
-        li.sends = std::max(li.sends, sends[t]);
-        li.hard_kill = li.hard_kill || hard_kill[t];
+  rc = launch_many(h, ps, LM_RECORD_PARAMS, 1, sub.data(), items, mw, fuzz_many_chunk(cap_events, par_cap), 0, [&](ManyLaunch& L) -> int32_t {
+    const uint32_t m = L.m;
+    Records rec;
+    int32_t rc = stage_records(h, &L.plan, m, nullptr, cap_events, par_cap, 0, rbuf, &rec, s);
+    if (rc != DEMI_OK) return rc;
+    KernelArgs& a = L.plan.args;
+    a.sum_steps = nullptr; a.n_violations = nullptr;      // the handle's counters stay as they were
+    a.rec_params = L.params;
+    CUDA_TRY(h, cudaEventRecord(h->ev0, s));
+    if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
+    L.plan.v->fn[LM_RECORD_PARAMS]<<<L.plan.grid, WARPS * 32, L.plan.smem, s>>>(a);
+    CUDA_TRY(h, cudaGetLastError());
+    CUDA_TRY(h, cudaEventRecord(h->ev1, s));
+    h->perf.kernel_launches++;
+    h->perf.prefixes += m;
+    res.resize(m); cnt.resize((size_t)m * 4);
+    CUDA_TRY(h, cudaMemcpyAsync(cnt.data(), rec.counts, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(h, cudaMemcpyAsync(res.data(), rec.results, res.size() * sizeof(demi_fuzz_result), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(h, cudaStreamSynchronize(s));
+    float ms = 0.f;
+    CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+    ms_all += ms;
+    // the rows travel as wide as the launch's longest successful recording, then go to their traces' rows
+    uint32_t width = 0, pwidth = 0;
+    for (uint32_t k = 0; k < m; k++) {
+      const uint32_t t = items[L.item[k]].trace;
+      n_events[t] = cnt[(size_t)k * 4];
+      if (n_nodes) n_nodes[t] = cnt[(size_t)k * 4 + 1];
+      if (results) results[t] = res[k];
+      if (res[k].status) {
+        status[t] = DEMI_ERR_CAPACITY; msg[t] = "demi_fuzz_trace: prefix status " + std::to_string(res[k].status);
+      } else {
+        width = std::max(width, std::min(cnt[(size_t)k * 4], cap_events));
+        pwidth = std::max(pwidth, std::min(cnt[(size_t)k * 4 + 1], par_cap));
       }
-      const uint32_t m = (uint32_t)(hi - lo);
-      // arena: the programs | masks | parameters | traces
-      auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
-      const size_t b_mask = al((size_t)m * mw * 8), b_par = al((size_t)m * sizeof(uint4)), b_tr = al((size_t)m * 4);
-      ProgramArena pa;
-      unsigned char* rest;
-      if ((rc = carve_programs(h, m, stride, send_stride, b_mask + b_par + b_tr, &pa, &rest)) != DEMI_OK) return rc;
-      uint64_t* mdev = (uint64_t*)rest;
-      uint4* pdev = (uint4*)(rest + b_mask);
-      uint32_t* tdev = (uint32_t*)(rest + b_mask + b_par);
-      hm.resize((size_t)m * mw); hp.resize(m); ht.resize(m);
-      for (uint32_t k = 0; k < m; k++) {
-        const uint32_t t = g[lo + k];
-        const uint64_t* mk = masks ? masks + (size_t)t * mask_words : ones.data();
-        std::copy(mk, mk + mw, hm.begin() + (size_t)k * mw);
-        const uint64_t sb = (uint64_t)seeds[t];
-        hp[k] = make_uint4((uint32_t)sb, (uint32_t)(sb >> 32), (uint32_t)max_messages[t], looking_for[t]);
-        ht[k] = t;
-      }
-      CUDA_TRY(h, cudaMemcpyAsync(mdev, hm.data(), hm.size() * 8, cudaMemcpyHostToDevice, s));
-      CUDA_TRY(h, cudaMemcpyAsync(pdev, hp.data(), hp.size() * sizeof(uint4), cudaMemcpyHostToDevice, s));
-      CUDA_TRY(h, cudaMemcpyAsync(tdev, ht.data(), ht.size() * 4, cudaMemcpyHostToDevice, s));
-      demi_fuzz_params q{};
-      q.n_prefixes = m;
-      q.max_messages = -1;                 // each execution binds its own (prog_params_bind); pc covers them all
-      q.invariant_check_interval = p->invariant_check_interval;
-      q.flags = p->flags;
-      LaunchPlan plan;
-      if ((rc = plan_launch(h, &q, LM_RECORD_PARAMS, li, nullptr, 0, &plan, pc)) != DEMI_OK) return rc;
-      Records rec;
-      if ((rc = stage_records(h, &plan, m, nullptr, cap_events, par_cap, 0, rbuf, &rec, s)) != DEMI_OK) return rc;
-      KernelArgs& a = plan.args;
-      a.sum_steps = nullptr; a.n_violations = nullptr;      // the handle's counters stay as they were
-      bind_programs(h, a, pa, -1);
-      a.rec_params = pdev;
-      CUDA_TRY(h, cudaEventRecord(h->ev0, s));
-      random_subseq_many_kernel<<<(unsigned)(((uint64_t)m * 32 + 127) / 128), 128, 0, s>>>(rs.progs, rs.tab, tdev, mdev, mw, m, pa.ev,
-                                                                                          stride, pa.hdr, pa.sends, send_stride);
-      CUDA_TRY(h, cudaGetLastError());
-      if (h->cfg.model == DEMI_MODEL_IR) CUDA_TRY(h, ir_bind(h->ir_dev, s));
-      plan.v->fn[LM_RECORD_PARAMS]<<<plan.grid, WARPS * 32, plan.smem, s>>>(a);
-      CUDA_TRY(h, cudaGetLastError());
-      CUDA_TRY(h, cudaEventRecord(h->ev1, s));
-      h->perf.kernel_launches += 2;
-      h->perf.prefixes += m;
-      res.resize(m); cnt.resize((size_t)m * 4);
-      CUDA_TRY(h, cudaMemcpyAsync(cnt.data(), rec.counts, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-      CUDA_TRY(h, cudaMemcpyAsync(res.data(), rec.results, res.size() * sizeof(demi_fuzz_result), cudaMemcpyDeviceToHost, s));
-      CUDA_TRY(h, cudaStreamSynchronize(s));
-      float ms = 0.f;
-      CUDA_TRY(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
-      ms_all += ms;
-      // the rows travel as wide as the launch's longest successful recording, then go to their traces' rows
-      uint32_t width = 0, pwidth = 0;
-      for (uint32_t k = 0; k < m; k++) {
-        const uint32_t t = g[lo + k];
-        n_events[t] = cnt[(size_t)k * 4];
-        if (n_nodes) n_nodes[t] = cnt[(size_t)k * 4 + 1];
-        if (results) results[t] = res[k];
-        if (res[k].status) {
-          snprintf(buf, sizeof(buf), "demi_fuzz_trace: prefix status %u", (unsigned)res[k].status);
-          status[t] = DEMI_ERR_CAPACITY; msg[t] = buf;
-        } else {
-          width = std::max(width, std::min(cnt[(size_t)k * 4], cap_events));
-          pwidth = std::max(pwidth, std::min(cnt[(size_t)k * 4 + 1], par_cap));
-        }
-      }
-      if (width) {
-        hev.resize((size_t)m * width);
-        CUDA_TRY(h, cudaMemcpy2DAsync(hev.data(), (size_t)width * sizeof(demi_event), rec.events, (size_t)cap_events * sizeof(demi_event),
-                                      (size_t)width * sizeof(demi_event), m, cudaMemcpyDeviceToHost, s));
-      }
-      if (pwidth) {
-        hpar.resize((size_t)m * pwidth);
-        CUDA_TRY(h, cudaMemcpy2DAsync(hpar.data(), (size_t)pwidth * sizeof(uint16_t), rec.parents, (size_t)par_cap * sizeof(uint16_t),
-                                      (size_t)pwidth * sizeof(uint16_t), m, cudaMemcpyDeviceToHost, s));
-      }
-      if (width || pwidth) CUDA_TRY(h, cudaStreamSynchronize(s));
-      for (uint32_t k = 0; k < m; k++) {
-        const uint32_t t = g[lo + k];
-        if (status[t] != DEMI_OK) continue;
-        std::copy_n(hev.data() + (size_t)k * width, std::min(n_events[t], cap_events), events + (size_t)t * cap_events);
-        if (dep_parent) std::copy_n(hpar.data() + (size_t)k * pwidth, std::min(n_nodes[t], par_cap), dep_parent + (size_t)t * par_cap);
-      }
-      lo = hi;
     }
-  }
+    if (width) {
+      hev.resize((size_t)m * width);
+      CUDA_TRY(h, cudaMemcpy2DAsync(hev.data(), (size_t)width * sizeof(demi_event), rec.events, (size_t)cap_events * sizeof(demi_event),
+                                    (size_t)width * sizeof(demi_event), m, cudaMemcpyDeviceToHost, s));
+    }
+    if (pwidth) {
+      hpar.resize((size_t)m * pwidth);
+      CUDA_TRY(h, cudaMemcpy2DAsync(hpar.data(), (size_t)pwidth * sizeof(uint16_t), rec.parents, (size_t)par_cap * sizeof(uint16_t),
+                                    (size_t)pwidth * sizeof(uint16_t), m, cudaMemcpyDeviceToHost, s));
+    }
+    if (width || pwidth) CUDA_TRY(h, cudaStreamSynchronize(s));
+    for (uint32_t k = 0; k < m; k++) {
+      const uint32_t t = items[L.item[k]].trace;
+      if (status[t] != DEMI_OK) continue;
+      std::copy_n(hev.data() + (size_t)k * width, std::min(n_events[t], cap_events), events + (size_t)t * cap_events);
+      if (dep_parent) std::copy_n(hpar.data() + (size_t)k * pwidth, std::min(n_nodes[t], par_cap), dep_parent + (size_t)t * par_cap);
+    }
+    return DEMI_OK;
+  });
+  if (rc != DEMI_OK) return rc;
   h->perf.kernel_ms = ms_all;
   // a failing trace has no events and no tree: zeros where they would be
   int64_t bad = -1;
@@ -1828,7 +1795,7 @@ extern "C" int32_t demi_fuzz_traces_many(demi_handle* h, uint32_t n_traces, cons
     memset(events + (size_t)t * cap_events, 0, (size_t)cap_events * sizeof(demi_event));
     if (dep_parent) memset(dep_parent + (size_t)t * par_cap, 0, (size_t)par_cap * sizeof(uint16_t));
   }
-  if (bad >= 0) h->err = std::string(who) + ": trace " + std::to_string(bad) + ": " + msg[bad];
+  if (bad >= 0) h->err = trace_msg(who, (uint32_t)bad, msg[bad]);
   return DEMI_OK;
 }
 

@@ -428,11 +428,7 @@ extern "C" int32_t demi_incremental_ddmin_many(demi_handle* h, uint32_t n_traces
       perf.deliveries += h->perf.deliveries; perf.violations += h->perf.violations;
       lo = hi;
     }
-    size_t k = 0;
-    for (DporRequest* q : batch) {
-      q->res.assign(res.begin() + k, res.begin() + k + q->n);
-      k += q->n;
-    }
+    scatter_results(batch, res);
     return DEMI_OK;
   };
   auto drive = [&](uint32_t t, Rendezvous<demi_dpor_result>& R, demi_handle* eh) -> int32_t {
@@ -450,6 +446,6 @@ extern "C" int32_t demi_incremental_ddmin_many(demi_handle* h, uint32_t n_traces
   for (DevBuf& d : h->dpor_buf) d.reset();             // a round's launches may hold far more than one trace's call needs
   if (rc != DEMI_OK) return rc;
   for (uint32_t t = 0; t < n; t++)
-    if (status[t] != DEMI_OK) { h->err = std::string(who) + ": trace " + std::to_string(t) + ": " + h->err; break; }
+    if (status[t] != DEMI_OK) { h->err = trace_msg(who, t, h->err); break; }
   return DEMI_OK;
 }

@@ -292,25 +292,14 @@ extern "C" int32_t demi_ddmin_many(demi_handle* h, const uint32_t* looking_for, 
   };
   LaunchCounts lc;
   auto serve = [&](std::vector<Request*>& batch) -> int32_t {
-    size_t total = 0;
-    for (const Request* q : batch) total += q->n;
-    std::vector<uint32_t> tr(total);
-    std::vector<uint64_t> flat(total * mask_words);
-    std::vector<demi_replay_result> res(total);
-    size_t k = 0;
-    for (const Request* q : batch) {
-      std::fill(tr.begin() + k, tr.begin() + k + q->n, q->trace);
-      std::copy(q->masks, q->masks + q->n * mask_words, flat.begin() + k * mask_words);
-      k += q->n;
-    }
-    const int32_t rc = replay_many(h, Views::of(h->set), tr.data(), flat.data(), nullptr, (uint32_t)total, mask_words, looking_for,
+    std::vector<uint32_t> tr;
+    std::vector<uint64_t> flat;
+    flatten_requests(batch, mask_words, tr, flat);
+    std::vector<demi_replay_result> res(tr.size());
+    const int32_t rc = replay_many(h, Views::of(h->set), tr.data(), flat.data(), nullptr, (uint32_t)tr.size(), mask_words, looking_for,
                                    flags, res.data(), lc);
     if (rc != DEMI_OK) return rc;
-    k = 0;
-    for (Request* q : batch) {
-      q->res.assign(res.begin() + k, res.begin() + k + q->n);
-      k += q->n;
-    }
+    scatter_results(batch, res);
     return DEMI_OK;
   };
   const int32_t rc = run_many<demi_replay_result>(h, "demi_ddmin_many", n, window, drive, serve, status);
@@ -585,7 +574,7 @@ extern "C" int32_t demi_wildcard_minimize_many(demi_handle* h, const uint32_t* l
   auto fail_trace = [&](uint32_t t, int32_t code, const std::string& m) { status[t] = code; msg[t] = m; live[t] = 0; };
   // each trace of the set is the base trace of its driver, which takes over the deliveries and modes wild_set built
   std::vector<WildcardDriver> d(n);
-  auto fail_driver = [&](uint32_t t) { fail_trace(t, d[t].error, std::string(who) + ": trace " + std::to_string(t) + ": " + d[t].msg); };
+  auto fail_driver = [&](uint32_t t) { fail_trace(t, d[t].error, trace_msg(who, t, d[t].msg)); };
   for (uint32_t t = 0; t < n; t++) {
     status[t] = DEMI_OK;
     if (bad[t]) { fail_trace(t, DEMI_ERR_INVALID, msg[t]); continue; }

@@ -52,6 +52,32 @@ struct Rendezvous {
   }
 };
 
+// A round's requests as one list of tests, in request order: the trace of each test, and its masks of mask_words words
+template <class Res>
+void flatten_requests(const std::vector<ManyRequest<Res>*>& batch, uint32_t mask_words, std::vector<uint32_t>& tr,
+                      std::vector<uint64_t>& masks) {
+  tr.clear(); masks.clear();
+  for (const ManyRequest<Res>* q : batch) {
+    tr.insert(tr.end(), q->n, q->trace);
+    masks.insert(masks.end(), q->masks, q->masks + q->n * mask_words);
+  }
+}
+
+// Hands each request its slice of `res`, the results of the round's tests in request order
+template <class Res>
+void scatter_results(const std::vector<ManyRequest<Res>*>& batch, const std::vector<Res>& res) {
+  size_t k = 0;
+  for (ManyRequest<Res>* q : batch) {
+    q->res.assign(res.begin() + k, res.begin() + k + q->n);
+    k += q->n;
+  }
+}
+
+// "<who>: trace <t>: <msg>", how a call over many traces reports trace t's failure
+inline std::string trace_msg(const char* who, uint32_t t, const std::string& msg) {
+  return std::string(who) + ": trace " + std::to_string(t) + ": " + msg;
+}
+
 // Drivers in flight: DEMI_DDMIN_MANY_WINDOW, 1..MANY_MAX_WINDOW (default 512), at most n.  It bounds both
 // demi_ddmin_many and demi_incremental_ddmin_many.
 inline int32_t many_window(demi_handle* h, uint32_t n, uint32_t& window) {

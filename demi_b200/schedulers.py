@@ -454,10 +454,14 @@ class Engine(object):
         return mcs, sizes[:n].copy(), keys[:n].copy(), out
 
     @staticmethod
+    def _is_program_list(programs):
+        """Whether a _many call was given a list of programs rather than one program (events or an array)."""
+        return bool(isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind"))
+
+    @staticmethod
     def _programs(programs, n):
         """Flattened programs for the _many calls: (externals, offsets, lengths); one program is shared by n traces."""
-        multi = isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind")
-        progs = list(programs) if multi else [programs] * n
+        progs = list(programs) if Engine._is_program_list(programs) else [programs] * n
         progs = [np.ascontiguousarray(p if isinstance(p, np.ndarray) else pack_externals(p), dtype=N.EXT_DTYPE)
                  for p in progs]
         n_ext = np.array([len(p) for p in progs], dtype=np.uint32)
@@ -479,8 +483,7 @@ class Engine(object):
         seed_base, max_messages and looking_for (a scalar applies to every trace).  One RANDOM_TEST_DTYPE record per
         test; the handle's program is not used."""
         tr = np.ascontiguousarray(trace_of_test, dtype=np.uint32)
-        n = len(programs) if isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind") \
-            else int(tr.max()) + 1 if len(tr) else 1
+        n = len(programs) if self._is_program_list(programs) else int(tr.max()) + 1 if len(tr) else 1
         ext, eoff, n_ext = self._programs(programs, n)
         sb, mm, lf = self._per_trace(seed_base, max_messages, looking_for, n)
         mw = mask_words or max(1, (int(n_ext.max()) + 63) // 64)
@@ -498,8 +501,7 @@ class Engine(object):
         max_messages and looking_for (a scalar applies to every trace).  Returns (MCS masks [n, mw], iteration sizes
         [n, cap], their keys [n, cap], RANDOM_DDMIN_OUT_DTYPE [n], status [n]); trace t's iterations are the first
         out[t]['n_iterations'] entries, and a trace whose status is not OK has no outputs."""
-        multi = isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind")
-        n = len(programs) if multi else n
+        n = len(programs) if self._is_program_list(programs) else n
         ext, eoff, n_ext = self._programs(programs, n)
         sb, mm, lf = self._per_trace(seed_base, max_messages, looking_for, n)
         mw = mask_words or max(1, (int(n_ext.max()) + 63) // 64)
@@ -524,8 +526,7 @@ class Engine(object):
         (fuzz_trace for a full program) returns for it, and a trace whose status is not OK has no events."""
         sd = np.ascontiguousarray(seeds, dtype=np.int64).reshape(-1)
         n = len(sd)
-        multi = isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind")
-        if multi:
+        if self._is_program_list(programs):
             ext, eoff, n_ext = self._programs(programs, n)
         else:                                # one program: every trace reads it at offset 0
             ext, _, n1 = self._programs(programs, 1)
@@ -662,17 +663,9 @@ class Engine(object):
         from seeds[t] = (events, dep_parent) (seeds None: no trace has a seed), with max_messages[t] and looking_for[t]
         (a scalar applies to every trace).  Returns (MCS masks [n, mw], INCDDMIN_OUT_DTYPE [n], status [n]); a trace
         whose status is not OK has no outputs, and the call raises only for call-level errors."""
-        multi = isinstance(programs, (list, tuple)) and len(programs) and not hasattr(programs[0], "kind")
-        n = len(programs) if multi else len(seeds)
-        progs = list(programs) if multi else [programs] * n
-        progs = [np.ascontiguousarray(p if isinstance(p, np.ndarray) else pack_externals(p), dtype=N.EXT_DTYPE)
-                 for p in progs]
-        n_ext = np.array([len(p) for p in progs], dtype=np.uint32)
-        ext = np.concatenate(progs + [np.zeros(1, dtype=N.EXT_DTYPE)])
-        eoff = np.zeros(n, dtype=np.uint32)
-        eoff[1:] = np.cumsum(n_ext)[:-1]
-        mm = np.ascontiguousarray(np.broadcast_to(np.asarray(max_messages, dtype=np.int32), (n,)))
-        lf = np.ascontiguousarray(np.broadcast_to(np.asarray(looking_for or 0, dtype=np.uint32), (n,)))
+        n = len(programs) if self._is_program_list(programs) else len(seeds)
+        ext, eoff, n_ext = self._programs(programs, n)
+        _, mm, lf = self._per_trace(0, max_messages, looking_for, n)
         P = N.DporParams(0, -1, max_interleavings, 0, 1, node_cap, explored_slots, heap_cap)
         alive, sd = [], None
         if seeds is not None:

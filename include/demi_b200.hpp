@@ -342,20 +342,14 @@ class Engine {
                                                        int32_t interval = 0, bool check_unmodified = false,
                                                        uint32_t cap_iterations = 1024) {
     const size_t n = programs.size();
-    ExternalEvents flat; std::vector<uint32_t> off, cnt;
-    size_t words = 1;
-    for (const ExternalEvents& p : programs) {
-      off.push_back((uint32_t)flat.size()); cnt.push_back((uint32_t)p.size());
-      flat.insert(flat.end(), p.begin(), p.end());
-      words = std::max<size_t>(words, (p.size() + 63) / 64);
-    }
-    if (flat.empty()) flat.resize(1);
+    const FlatPrograms fp = flatten(programs);
+    const size_t words = fp.words;
     const demi_fuzz_params p{0, max_executions, -1, interval, 0, 0};
     std::vector<uint64_t> mcs(n * words), keys(n * (size_t)cap_iterations);
     std::vector<uint32_t> sizes(n * (size_t)cap_iterations);
     std::vector<demi_random_ddmin_out> out(n);
     std::vector<int32_t> status(n);
-    check(demi_random_ddmin_many(h, (uint32_t)n, flat.data(), off.data(), cnt.data(), seeds.data(), max_messages.data(),
+    check(demi_random_ddmin_many(h, (uint32_t)n, fp.ev.data(), fp.off.data(), fp.cnt.data(), seeds.data(), max_messages.data(),
                                  looking_for.data(), &p, check_unmodified ? 1 : 0, mcs.data(), (uint32_t)words, sizes.data(),
                                  keys.data(), cap_iterations, out.data(), status.data()));
     std::vector<RandomDDMinManyResult> r(n);
@@ -379,14 +373,8 @@ class Engine {
                                                   const std::vector<std::vector<uint64_t>>& masks = {}, bool with_trees = false,
                                                   uint32_t cap_events = 4096, uint32_t cap_nodes = 4096) {
     const size_t n = programs.size();
-    ExternalEvents flat; std::vector<uint32_t> off, cnt;
-    size_t words = 1;
-    for (const ExternalEvents& p : programs) {
-      off.push_back((uint32_t)flat.size()); cnt.push_back((uint32_t)p.size());
-      flat.insert(flat.end(), p.begin(), p.end());
-      words = std::max<size_t>(words, (p.size() + 63) / 64);
-    }
-    if (flat.empty()) flat.resize(1);
+    const FlatPrograms fp = flatten(programs);
+    const size_t words = fp.words;
     std::vector<uint64_t> mk;
     if (!masks.empty())
       for (size_t t = 0; t < n; t++) {
@@ -400,9 +388,9 @@ class Engine {
     std::vector<uint32_t> ne(n), nn(n);
     std::vector<demi_fuzz_result> res(n);
     std::vector<int32_t> status(n);
-    check(demi_fuzz_traces_many(h, (uint32_t)n, flat.data(), off.data(), cnt.data(), mk.empty() ? nullptr : mk.data(), (uint32_t)words,
-                                seeds.data(), max_messages.data(), looking_for.data(), &p, ev.data(), cap_events, ne.data(),
-                                with_trees ? par.data() : nullptr, cap_nodes, nn.data(), res.data(), status.data()));
+    check(demi_fuzz_traces_many(h, (uint32_t)n, fp.ev.data(), fp.off.data(), fp.cnt.data(), mk.empty() ? nullptr : mk.data(),
+                                (uint32_t)words, seeds.data(), max_messages.data(), looking_for.data(), &p, ev.data(), cap_events,
+                                ne.data(), with_trees ? par.data() : nullptr, cap_nodes, nn.data(), res.data(), status.data()));
     std::vector<RecordedExecution> r(n);
     for (size_t t = 0; t < n; t++) {
       r[t].result = res[t]; r[t].status = status[t];
@@ -414,6 +402,19 @@ class Engine {
   }
   const SchedulerConfig cfg;
  private:
+  // programs one after the other (one empty event at least, so that the pointer is valid), where each starts, its
+  // length, and the mask words of the longest
+  struct FlatPrograms { ExternalEvents ev; std::vector<uint32_t> off, cnt; size_t words = 1; };
+  static FlatPrograms flatten(const std::vector<ExternalEvents>& programs) {
+    FlatPrograms f;
+    for (const ExternalEvents& p : programs) {
+      f.off.push_back((uint32_t)f.ev.size()); f.cnt.push_back((uint32_t)p.size());
+      f.ev.insert(f.ev.end(), p.begin(), p.end());
+      f.words = std::max<size_t>(f.words, (p.size() + 63) / 64);
+    }
+    if (f.ev.empty()) f.ev.resize(1);
+    return f;
+  }
   demi_handle* h = nullptr;
   std::vector<ExternalEvents> set_ext;         // the externals of each trace of the set (demi_set_traces)
   demi_fuzzer_config fz_cfg{};
