@@ -126,7 +126,7 @@ PV_OK, PV_CYCLE, PV_OVERFLOW, PV_PREFIX_FAILED = 0, 1, 2, 3
 EXPORTS = [
     "demi_version", "demi_last_error", "demi_device_count", "demi_create", "demi_destroy",
     "demi_set_externals", "demi_fuzz_batch", "demi_fuzz_batch_dev", "demi_fuzz_summary_dev",
-    "demi_fuzz_trace", "demi_stats", "demi_lane_kernel", "demi_lane_tree_depth",
+    "demi_fuzz_trace", "demi_stats", "demi_lane_kernel", "demi_lane_tree_depth", "demi_lane_row_bytes",
     "demi_set_trace", "demi_replay_batch", "demi_replay_batch_dev", "demi_ddmin", "demi_dpor_batch",
     "demi_dedup_compact_dev", "demi_dedup_compact",
     "demi_replay_batch_ex", "demi_replay_trace", "demi_internal_minimize",
@@ -366,5 +366,7 @@ def lib():
     L.demi_lane_kernel.argtypes = [vp]
     L.demi_lane_tree_depth.restype = C.c_int32
     L.demi_lane_tree_depth.argtypes = [vp]
+    L.demi_lane_row_bytes.restype = C.c_int32
+    L.demi_lane_row_bytes.argtypes = [vp]
     _lib = L
     return L

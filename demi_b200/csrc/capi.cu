@@ -77,14 +77,16 @@ static const Variant* pick_variant(int model, LaunchMode mode, uint32_t pcap, ui
 // lane-engine table
 // `steady`: the LM_BATCH instantiation that starts from the program's tree (`snapshot` takes its root, `tree` builds
 // one level, of records `node_bytes` long); `ops` is the model's operations per receive(), which the node-capacity
-// proof of lane_steady_eligible counts with.
+// proof of lane_steady_eligible counts with.  `row8`: the steady instantiation with 8-byte pending rows, for the model
+// whose rows lane_row8_eligible can prove fit them (raft5), else null.
 typedef void (*snapshot_fn)(const KernelArgs, LaneSnapshot*);
 typedef void (*tree_fn)(const KernelArgs, uint32_t*, const uint2*, uint32_t, uint32_t);
 struct LaneVariant {
   int model; int bd; uint32_t lpcap; size_t smem_per_block; kernel_fn fn[LM_COUNT];
   kernel_fn steady; size_t steady_smem; snapshot_fn snapshot; tree_fn tree; uint32_t node_bytes; uint32_t ops;
+  kernel_fn row8;
 };
-template <class MODEL, int BD, int LPCAP>
+template <class MODEL, int BD, int LPCAP, bool ROW8 = false>
 static LaneVariant make_lane_variant() {
   using M = LaneMachine<MODEL, BD, LPCAP>;
   using S = LaneMachine<MODEL, BD, LPCAP, false, true>;
@@ -93,14 +95,15 @@ static LaneVariant make_lane_variant() {
                       fuzz_lane_kernel<MODEL, BD, LPCAP, false, true>, fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true>,
                       fuzz_lane_kernel<MODEL, BD, LPCAP, false, true, true, false, true>},
                      fuzz_lane_kernel<MODEL, BD, LPCAP, false, false, false, true>, (size_t)S::WORDS * BD * sizeof(uint32_t),
-                     lane_snapshot_kernel<MODEL>, lane_tree_kernel<MODEL, LPCAP>, S::NODE_WORDS * 4u, (uint32_t)MODEL::LANE_OUTBOX};
+                     lane_snapshot_kernel<MODEL>, lane_tree_kernel<MODEL, LPCAP>, S::NODE_WORDS * 4u, (uint32_t)MODEL::LANE_OUTBOX,
+                     ROW8 ? fuzz_lane_kernel<MODEL, BD, LPCAP, false, false, false, true, false, ROW8> : nullptr};
 }
 #ifndef DEMI_K1_BD_RAFT5
 #define DEMI_K1_BD_RAFT5 256
 #endif
 static const LaneVariant* lane_variant_of(int model) {
   static const std::vector<LaneVariant> v = {
-    make_lane_variant<Raft5, DEMI_K1_BD_RAFT5, DEMI_K1_LPCAP_RAFT5>(),
+    make_lane_variant<Raft5, DEMI_K1_BD_RAFT5, DEMI_K1_LPCAP_RAFT5, true>(),
     make_lane_variant<PingPong3, 256, 128>(),
     make_lane_variant<Bcast32, 128, 8192>(),
   };
@@ -457,6 +460,7 @@ static int32_t lane_tree(demi_handle* h, const LaneVariant* lv, const KernelArgs
 static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, cudaStream_t s) {
   KernelArgs& a = plan.args;
   h->lane_kernel = DEMI_LANE_NONE;
+  h->lane_row_bytes = 0;
   h->lane_tree_depth = -1;
   if (const LaneVariant* lv = pick_lane_variant(h, *plan.prog)) {
     const uint32_t lane_pcap = std::min(h->lane_pending_cap ? std::min(a.pending_cap, h->lane_pending_cap) : a.pending_cap, lv->lpcap);
@@ -471,7 +475,9 @@ static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, c
       l.lane_tosend_cap = LANE_TOSEND_CAP; l.ops_per_delivery = lv->ops;
       steady = lane_steady_eligible(h->lane_snap, l);
     }
-    const kernel_fn lfn = steady ? lv->steady : lv->fn[plan.mode];
+    // ... and with 8-byte pending rows when the launch's rows provably fit them
+    const bool row8 = steady && lv->row8 && lane_row8_eligible(h->lane_snap, a.max_messages, lv->ops);
+    const kernel_fn lfn = row8 ? lv->row8 : steady ? lv->steady : lv->fn[plan.mode];
     const size_t lsmem = steady ? lv->steady_smem : lv->smem_per_block;
     int32_t rc;
     int bps = 0;
@@ -499,6 +505,7 @@ static int32_t launch_plan(demi_handle* h, LaunchPlan& plan, uint64_t n_items, c
     lfn<<<lgrid, lv->bd, lsmem, s>>>(la);
     CUDA_TRY(h, cudaGetLastError());
     h->lane_kernel = steady ? DEMI_LANE_STEADY : DEMI_LANE_GENERIC;
+    h->lane_row_bytes = row8 ? 8 : 16;
     h->lane_tree_depth = steady ? (int32_t)h->lane_snap.depth : -1;
     h->perf.kernel_launches++;
     // what the lane engine could not prove exact: a recording launch numbers its outputs by work-list position
@@ -1801,6 +1808,7 @@ extern "C" int32_t demi_fuzz_traces_many(demi_handle* h, uint32_t n_traces, cons
 
 extern "C" int32_t demi_lane_kernel(const demi_handle* h) { return h ? h->lane_kernel : DEMI_ERR_INVALID; }
 extern "C" int32_t demi_lane_tree_depth(const demi_handle* h) { return h ? h->lane_tree_depth : DEMI_ERR_INVALID; }
+extern "C" int32_t demi_lane_row_bytes(const demi_handle* h) { return h ? h->lane_row_bytes : DEMI_ERR_INVALID; }
 
 extern "C" int32_t demi_stats(const demi_handle* h, demi_perf* out) {
   if (!h || !out) return DEMI_ERR_INVALID;

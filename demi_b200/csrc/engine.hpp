@@ -77,6 +77,7 @@ struct demi_handle {
   bool lane_tree_built = false;
   demi::LaneTreeKey lane_tree_key{};
   int32_t lane_tree_depth = -1;                    // the depth the last fuzz launch walked (-1: not the steady one)
+  int32_t lane_row_bytes = 0;                      // bytes per pending row of its lane kernel (0: none ran)
   DevBuf prov_scratch;
   std::vector<DevBuf> dpor_buf;                    // K3 per-search structures, one per entry of dpor_run's table (capi_dpor.cu)
   cudaStream_t stream = nullptr, copy_stream = nullptr;

@@ -12,8 +12,9 @@
 //                  thread-interleaved (word w of thread t at [w*BD + t]: every
 //                  access is bank-conflict free whatever each lane indexes)
 //   HBM / L1 / L2  the pending-message array (RandomizedHashSet.arr), 16-byte
-//                  entries, LPCAP contiguous ones per thread (entry i of
-//                  thread t at [t*LPCAP + i])
+//                  entries (8-byte in the steady raft5 kernel's ROW8 flavour),
+//                  LPCAP contiguous ones per thread (entry i of thread t at
+//                  [t*LPCAP + i])
 //
 // Exactness: every structure here is a bounded, duplicate-free restatement.
 // Whenever an execution could leave that regime (a capacity would overflow, or
@@ -26,6 +27,7 @@
 #include "machine.cuh"
 #include "models/models.cuh"
 #include "lane_steady.hpp"
+#include <type_traits>
 
 namespace demi {
 
@@ -111,6 +113,23 @@ __device__ __forceinline__ void st_l2_hint(uint4* p, uint4 v, uint64_t pol) {
 #if DEMI_K1_PEND_HINT
   asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;"
                :: "l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "l"(pol));
+#else
+  (void)pol; *p = v;
+#endif
+}
+// 8-byte rows (the steady raft5 kernel's ROW8 flavour, lane_steady.hpp) under the same policy
+__device__ __forceinline__ uint2 ld_l2_hint(const uint2* p, uint64_t pol) {
+#if DEMI_K1_PEND_HINT
+  uint2 v;
+  asm volatile("ld.global.L2::cache_hint.v2.u32 {%0,%1}, [%2], %3;" : "=r"(v.x), "=r"(v.y) : "l"(p), "l"(pol));
+  return v;
+#else
+  (void)pol; return *p;
+#endif
+}
+__device__ __forceinline__ void st_l2_hint(uint2* p, uint2 v, uint64_t pol) {
+#if DEMI_K1_PEND_HINT
+  asm volatile("st.global.L2::cache_hint.v2.u32 [%0], {%1,%2}, %3;" :: "l"(p), "r"(v.x), "r"(v.y), "l"(pol));
 #else
   (void)pol; *p = v;
 #endif
@@ -229,9 +248,13 @@ __device__ __forceinline__ void receive_phase(LaneDirectOutbox<M>& o, uint32_t r
 // partitions, isolated or killed actors, ignoreTimers, a violation filter or the node capacity, and tests the
 // pending array against one bound (A->pending_cap, which the host has clamped to LPCAP).  Every rule is the generic
 // one with those cases compiled out.
-template <class MODEL, int BD, int LPCAP, bool REC = false, bool STEADY = false>
+// ROW8 (STEADY raft5 only): the pending rows are 8 bytes in the layout of lane_steady.hpp, which the host has proven
+// holds every row of the launch (lane_row8_eligible).  A row is packed where it is stored and unpacked where it is
+// read, so the rest of the machine and the model see the 16-byte form.
+template <class MODEL, int BD, int LPCAP, bool REC = false, bool STEADY = false, bool ROW8 = false>
 struct LaneMachine {
   static_assert(!(STEADY && REC), "recording launches run the generic instantiation");
+  static_assert(!ROW8 || (STEADY && MODEL::ID == DEMI_MODEL_RAFT5), "the 8-byte layout and its proof are the steady raft5 machine's");
   static constexpr int N = MODEL::N_ACTORS;
   static constexpr int SW = MODEL::STATE_WORDS;
   static constexpr int OB = MODEL::LANE_OUTBOX;
@@ -245,7 +268,8 @@ struct LaneMachine {
   static constexpr int WORDS = N * SW + OBW + PW + TW;     // states + outbox + partition rows + cancellable timer copies
 
   uint32_t* smw;             // &smem[tid]; word w at smw[w*BD]
-  uint4* pend;               // entry i at pend[i]
+  using Row = typename std::conditional<ROW8, uint2, uint4>::type;
+  Row* pend;                 // entry i at pend[i]
   uint4* rec_ev; uint16_t* rec_par;   // REC: this execution's EventTrace slot and parent array
   uint64_t pol;              // L2 cache policy of the pending array
   const KernelArgs* A;
@@ -311,12 +335,41 @@ struct LaneMachine {
 
   // RandomizedHashSet.insert (schedulers/Util.scala:126-136).  max_pending is brought up to date before each removal
   // and at the end of the execution, the only points where the set can be at a maximum.
+  __device__ __forceinline__ static Row row_pack(const uint4& e) {
+    if constexpr (ROW8) {
+      static_assert(MODEL::N_ACTORS == (int)LANE_ROW8_ACTORS && MODEL::LOG_CAP < 16, "lane_steady.hpp's proof is about this model");
+      const uint64_t r = lane_row8_pack(e.x, e.y, e.z, e.w & 0xFFFFu);
+      return make_uint2((uint32_t)r, (uint32_t)(r >> 32));
+    } else {
+      return e;
+    }
+  }
+  __device__ __forceinline__ static uint4 row_unpack(const Row& q) {
+    if constexpr (ROW8) {
+      const uint64_t r = q.x | (uint64_t)q.y << 32;
+      // no flags in the header: nothing reads them but row_cancellable, which reads the row
+      return make_uint4(lane_row8_sdt(r), lane_row8_p0(r), lane_row8_p1(r), lane_row8_node(r) * 0x10001u);
+    } else {
+      return q;
+    }
+  }
+  // whether a stored row is a copy of the cancellable timer (type CT), and its receiver
+  __device__ __forceinline__ static bool row_cancellable(const Row& q) {
+    if constexpr (ROW8) return lane_row8_timer_of(q.x | (uint64_t)q.y << 32, CT);
+    else return cancellable_timer(q.x);
+  }
+  __device__ __forceinline__ static uint32_t row_dst(const Row& q) {
+    if constexpr (ROW8) return lane_row8_dst(q.x | (uint64_t)q.y << 32);
+    else return hdr_dst(q.x);
+  }
+  __device__ __forceinline__ uint4 row_load(uint32_t i) { return row_unpack(ld_l2_hint(pend + i, pol)); }
+
   __device__ __forceinline__ bool pending_full(uint32_t k) const {
     if constexpr (STEADY) return n_pending + k > A->pending_cap;
     return n_pending + k > A->pending_cap || n_pending + k > LPCAP;
   }
   __device__ __forceinline__ void pending_push(uint4 e) {          // the caller has checked pending_full
-    st_l2_hint(pend + n_pending, e, pol);
+    st_l2_hint(pend + n_pending, row_pack(e), pol);
     n_pending++;
   }
   __device__ __forceinline__ void pending_insert(uint4 e) {
@@ -326,18 +379,19 @@ struct LaneMachine {
   // RandomizedHashSet.remove (schedulers/Util.scala:146-163)
   __device__ __forceinline__ uint4 pending_remove_at(uint32_t i) {
     if (n_pending > max_pending) max_pending = n_pending;
-    uint4 v = ld_l2_hint(pend + i, pol);
-    uint4 last = ld_l2_hint(pend + (n_pending - 1), pol);
+    const Row vr = ld_l2_hint(pend + i, pol);
+    const Row last = ld_l2_hint(pend + (n_pending - 1), pol);
     st_l2_hint(pend + i, last, pol);
     n_pending--;
+    const uint4 v = row_unpack(vr);
     if constexpr (CT != 0) {
       // in place on the actor's half of the word: the count is at least 1 here, and indices stay below LPCAP < 0xFF
-      if (cancellable_timer(v.x)) {                      // one copy fewer, its index no longer known
-        const uint32_t a = hdr_dst(v.x), sh = (a & 1u) * 16;
+      if (row_cancellable(vr)) {                         // one copy fewer, its index no longer known
+        const uint32_t a = row_dst(vr), sh = (a & 1u) * 16;
         tcopy_word(a) = (tcopy_word(a) - (1u << sh)) | (0xFF00u << sh);
       }
-      if (cancellable_timer(last.x)) {                   // moved from index n_pending to i
-        const uint32_t a = hdr_dst(last.x), sh = (a & 1u) * 16 + 8;
+      if (row_cancellable(last)) {                       // moved from index n_pending to i
+        const uint32_t a = row_dst(last), sh = (a & 1u) * 16 + 8;
         uint32_t& w = tcopy_word(a);
         if (((w >> sh) & 0xFFu) == n_pending) w ^= (n_pending ^ i) << sh;
       }
@@ -520,7 +574,7 @@ struct LaneMachine {
     for (uint32_t i = 0; i < n_pending; i += 4) {
       uint4 q[4];
 #pragma unroll
-      for (uint32_t k = 0; k < 4; k++) q[k] = (i + k < n_pending) ? ld_l2_hint(pend + (i + k), pol) : make_uint4(0, 0, 0, 0);
+      for (uint32_t k = 0; k < 4; k++) q[k] = (i + k < n_pending) ? row_load(i + k) : make_uint4(0, 0, 0, 0);
 #pragma unroll
       for (uint32_t k = 0; k < 4; k++)
         if ((q[k].x & 0x00FFFFFFu) == want && q[k].y == p0 && q[k].z == p1) { pending_remove_at(i + k); return; }
@@ -695,8 +749,8 @@ struct LaneMachine {
     r[LN_THASH_LO] = (uint32_t)thash; r[LN_THASH_HI] = (uint32_t)(thash >> 32);
     for (uint32_t i = 0; i < (uint32_t)(N * SW + TW); i++) r[LANE_NODE_HEAD + i] = machine_word(i);
     uint4* rows = reinterpret_cast<uint4*>(r + NODE_ROWS_AT);
-    if (rows != pend)
-      for (uint32_t i = 0; i < n_pending; i++) rows[i] = ld_l2_hint(pend + i, pol);
+    if ((void*)rows != (void*)pend)
+      for (uint32_t i = 0; i < n_pending; i++) rows[i] = row_load(i);
   }
   // The steady machine becomes the one stored in record r (status 0): every register and shared word the rest of an
   // execution reads.  tosend is empty at a stored pick point, or never read again when the execution stops there.
@@ -715,7 +769,7 @@ struct LaneMachine {
     for (uint32_t i = 0; i < (uint32_t)(N * SW + TW); i++) machine_word(i) = __ldg(r + LANE_NODE_HEAD + i);
     const uint4* rows = reinterpret_cast<const uint4*>(r + NODE_ROWS_AT);
 #pragma unroll 1
-    for (uint32_t i = 0; i < n_pending; i++) st_l2_hint(pend + i, __ldg(rows + i), pol);
+    for (uint32_t i = 0; i < n_pending; i++) st_l2_hint(pend + i, row_pack(__ldg(rows + i)), pol);
   }
   // STEADY: the machine after the execution's first picks.  Each level of the tree draws the index pick_next would
   // draw; the walk stops at a node without children, or before a child that is not stored, and leaves the generator
@@ -779,7 +833,7 @@ struct LaneMachine {
       if (A->fuzz_flags & DEMI_FF_HASH_PENDING)
 #pragma unroll 1
         for (uint32_t i = 0; i < n_pending; i++) {
-          uint4 q = ld_l2_hint(pend + i, pol);
+          const uint4 q = row_load(i);
           sh += demi_pending_term(q.x & 0x00FFFFFFu, q.y, q.z);
         }
       out.violation = violation; out.steps = (uint32_t)nsched;
@@ -871,14 +925,14 @@ lane_tree_kernel(const __grid_constant__ KernelArgs args, uint32_t* tree, const 
 // of messagesToSend resolve through that program's Send table.  A deferred prefix keeps its index, so the PROG
 // instantiation of the warp engine re-runs it on the same program.
 template <class MODEL, int BD, int LPCAP, bool REC = false, bool PROG = false, bool TESTS = false, bool STEADY = false,
-          bool PARAMS = false>
+          bool PARAMS = false, bool ROW8 = false>
 __global__ void __launch_bounds__(BD, DEMI_K1_MIN_BLOCKS)
 fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
   static_assert(!(PROG && REC), "a campaign execution is recorded through demi_fuzz_trace on its program");
   static_assert(PROG || !TESTS, "random-oracle tests bind their programs as campaigns do");
   static_assert(!STEADY || !(REC || PROG), "a steady launch runs one fixed program, unrecorded");
   static_assert(TESTS || !PARAMS, "per-program parameters are those of random-oracle tests");
-  using M = LaneMachine<MODEL, BD, LPCAP, REC, STEADY>;
+  using M = LaneMachine<MODEL, BD, LPCAP, REC, STEADY, ROW8>;
   extern __shared__ __align__(16) uint32_t lane_smem[];
   const uint32_t tid = threadIdx.x;
   const uint64_t gthread = (uint64_t)blockIdx.x * BD + tid;
@@ -886,7 +940,7 @@ fuzz_lane_kernel(const __grid_constant__ KernelArgs args) {
 
   M m;
   m.smw = lane_smem + tid;
-  m.pend = args.lane_pend + gthread * (uint64_t)LPCAP;
+  m.pend = reinterpret_cast<typename M::Row*>(args.lane_pend) + gthread * (uint64_t)LPCAP;     // LPCAP rows per thread
   KernelArgs la;
   if constexpr (PROG) { la = args; m.A = &la; } else m.A = &args;
   m.pol = l2_evict_last_policy();

@@ -118,4 +118,78 @@ inline bool lane_steady_eligible(const LaneSnapshot& s, const LaneSteadyLaunch& 
   return lane_steady_node_bound(s.n_nodes, (uint64_t)l.max_messages + 1u, l.ops_per_delivery) <= l.node_cap;
 }
 
+// ---------------------------------------------------------------------------------------------- 8-byte raft5 rows
+// The steady raft5 lane kernel's ROW8 flavour keeps each pending row (header, p0, p1, DepTracker node) in 64 bits
+// instead of 128, which halves the rows' L2 footprint.  raft5's payloads leave fixed bits of p0 and p1 zero, and the
+// header and the node go into those bits, so a row is packed with a few ORs and unpacked with two ANDs and a few bit
+// extracts, and no row is range-tested on the device: lane_row8_eligible proves on the host, once per launch, that
+// every row a steady execution can create has its payload zero there.  The two 32-bit words:
+//   lo = p0 (bits 12..15 and 28..31 zero)  | type << 12 | (node >> 8) << 28
+//   hi = p1 (bits 1..7 and 24..31 zero)    | src code << 1 | dst << 4 | (node & 0xFF) << 24
+// so p0's byte 1 and byte 3 and p1's byte 0 hold 4, 4 and 1 bits, p1's byte 3 none, and the node 12 bits.  The src code
+// is the actor (0..4), or 5 + flags for a message from deadLetters (flags 0, EXTERNAL or TIMER): an actor's sends
+// carry no flags.  Word 3 of a row is node | node << 16 (Uniq equals node in the lane engine), so one field holds both.
+//
+// Why raft5's payloads fit (Raft5::receive, models.cuh), given that the snapshot's rows do (checked below): every p0
+// byte 0, byte 2 and p1 byte 1 and 2 is a term, a log term, a log value or a log index, each one state byte.  p0 byte 1
+// is RequestVote's lastIndex (LOGLEN <= LOG_CAP), a grant or ok bit, or AppendEntries' prev, which is NEXT[j]: NEXT
+// is only set to LOGLEN, lowered by one, or raised to the matchIndex of an AppendReply from an actor (DESIGN §3 raft5
+// R2: never from deadLetters, so never from an external Send), which is at most LOG_CAP.  p0 byte 3 is AppendEntries'
+// commit index, at most LOG_CAP (COMMIT is the minimum of a leaderCommit and a matchIndex <= LOG_CAP, or the highest of
+// at most LOG_CAP log entries).  p1 byte 0 is AppendEntries' has-entry bit.  Every other byte a receive() sends is zero,
+// and timers have p0 = p1 = 0.
+#if defined(__CUDACC__)
+#define LANE_ROW8_HD __host__ __device__ __forceinline__
+#else
+#define LANE_ROW8_HD inline
+#endif
+constexpr uint32_t LANE_ROW8_ACTORS = 5;            // Raft5::N_ACTORS
+constexpr uint32_t LANE_ROW8_NODE_BITS = 12;
+constexpr uint32_t LANE_ROW8_P0 = 0x0FFF0FFFu, LANE_ROW8_P1 = 0x00FFFF01u;     // the payload bits of lo and hi
+
+// lo | hi << 32; the caller knows that p0 and p1 have no bit outside LANE_ROW8_P0 / LANE_ROW8_P1 and node < 2^12
+LANE_ROW8_HD uint64_t lane_row8_pack(uint32_t hdr, uint32_t p0, uint32_t p1, uint32_t node) {
+  const uint32_t src = hdr & 0xFFu, code = src < LANE_ROW8_ACTORS ? src : 5u + (hdr >> 24);
+  const uint32_t lo = p0 | ((hdr >> 16) & 0xFu) << 12 | (node >> 8) << 28;
+  const uint32_t hi = p1 | (code & 7u) << 1 | ((hdr >> 8) & 7u) << 4 | node << 24;
+  return (uint64_t)lo | (uint64_t)hi << 32;
+}
+// src, dst and type of a packed row, as make_hdr places them, without the flags: all the steady machine reads of a
+// header, except whether the row is a timer message of a given type, which lane_row8_timer_of reads from the row
+LANE_ROW8_HD uint32_t lane_row8_sdt(uint64_t r) {
+  const uint32_t lo = (uint32_t)r, hi = (uint32_t)(r >> 32), code = (hi >> 1) & 7u;
+  return (code < LANE_ROW8_ACTORS ? code : 0xFFu) | ((hi >> 4) & 7u) << 8 | ((lo >> 12) & 0xFu) << 16;
+}
+LANE_ROW8_HD uint32_t lane_row8_dst(uint64_t r) { return (uint32_t)(r >> 36) & 7u; }
+// a timer message (from deadLetters, flagged TIMER: src code 7) of `type`
+LANE_ROW8_HD bool lane_row8_timer_of(uint64_t r, uint32_t type) {
+  return (((uint32_t)(r >> 32) & 0xEu) | ((uint32_t)r & 0xF000u)) == (0xEu | type << 12);
+}
+// the whole header (src, dst, type and flags as make_hdr builds them)
+LANE_ROW8_HD uint32_t lane_row8_hdr(uint64_t r) {
+  const uint32_t code = (uint32_t)(r >> 33) & 7u;
+  return lane_row8_sdt(r) | (code < LANE_ROW8_ACTORS ? 0u : (code - 5u) << 24);
+}
+LANE_ROW8_HD uint32_t lane_row8_p0(uint64_t r) { return (uint32_t)r & LANE_ROW8_P0; }
+LANE_ROW8_HD uint32_t lane_row8_p1(uint64_t r) { return (uint32_t)(r >> 32) & LANE_ROW8_P1; }
+LANE_ROW8_HD uint32_t lane_row8_node(uint64_t r) { return (uint32_t)(r >> 56) | ((uint32_t)r >> 28) << 8; }
+
+// Whether the layout holds a row exactly.
+LANE_ROW8_HD bool lane_row8_fits(uint32_t hdr, uint32_t p0, uint32_t p1) {
+  if ((p0 & ~LANE_ROW8_P0) | (p1 & ~LANE_ROW8_P1)) return false;
+  const uint64_t r = lane_row8_pack(hdr, p0, p1, 0);
+  return lane_row8_hdr(r) == hdr;
+}
+
+// True when a steady raft5 launch (lane_steady_eligible holds) may run the ROW8 flavour: every row of the snapshot
+// fits the layout, and every DepTracker node the execution can create is below 2^12 (lane_steady_node_bound over
+// max_messages + 1 deliveries, as in lane_steady_eligible).  The snapshot's rows are the only ones not made by
+// Raft5::receive or a timer: they hold the program's external Sends, whose payloads are whatever the program gave them.
+inline bool lane_row8_eligible(const LaneSnapshot& s, int32_t max_messages, uint32_t ops_per_delivery) {
+  if (max_messages < 0 || s.n_pending > LANE_SNAP_CAP) return false;
+  for (uint32_t i = 0; i < s.n_pending; i++)
+    if (!lane_row8_fits(s.pend[i][0], s.pend[i][1], s.pend[i][2])) return false;
+  return lane_steady_node_bound(s.n_nodes, (uint64_t)max_messages + 1u, ops_per_delivery) <= (1ull << LANE_ROW8_NODE_BITS);
+}
+
 }  // namespace demi

@@ -732,6 +732,11 @@ class Engine(object):
         """The depth of the tree the last fuzz launch walked when it ran LANE_STEADY, else -1."""
         return N.lib().demi_lane_tree_depth(self._h)
 
+    def lane_row_bytes(self):
+        """Bytes per pending row of the lane kernel the last fuzz launch ran: 16, 8 (the steady raft5 kernel's ROW8
+        flavour), or 0 when none ran."""
+        return N.lib().demi_lane_row_bytes(self._h)
+
     def stats(self):
         s = N.Perf()
         self._check(N.lib().demi_stats(self._h, C.byref(s)))

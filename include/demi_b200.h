@@ -918,6 +918,10 @@ int32_t demi_lane_kernel(const demi_handle* h);
  * each execution skips up to that many of its first deliveries, whose machines the tree holds.  -1 for every other
  * launch. */
 int32_t demi_lane_tree_depth(const demi_handle* h);
+/* The size of a pending row in the lane kernel the handle's last fuzz launch ran: 16, or 8 when a steady raft5 launch
+ * could prove that every row it creates fits the 8-byte layout, which halves the rows' cache footprint.  0 when no lane
+ * kernel ran.  The records are the same either way. */
+int32_t demi_lane_row_bytes(const demi_handle* h);
 
 #ifdef __cplusplus
 }
